@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- occupancy Mpoints/s (+ recon frames/s @256^3) of the fused hot path on N B200s of one node.
+"""bench.py -- occupancy Mpoints/s (+ recon frames/s @256^3) of the fused hot path on N H100s of one node.
 
     python bench.py --gpus 1 --steps K --warmup W
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
@@ -12,7 +12,8 @@ resident in HBM; `e2e` = the same through the C-ABI host-buffer entry point (fea
 timed region; at N > 1 the all-gather too).  `recon` reports BASELINE configs[1..3] (coarse-to-fine recon frames/s, with the
 netC colour pass, and the image stream with the PyTorch encoder as CUDA-graph captured frame steps), `configs4_dense513`
 BASELINE configs[4].  At N > 1 the line also asserts that the gathered volume equals the single-GPU volume bit for bit.
-Prints ONE JSON line on rank 0.
+Prints ONE JSON line on rank 0.  --dump-outputs DIR writes what the timed path computed in its last step (a fixed, seeded
+sample of the occupancy volume with its node indices) as DIR/*.npy, so that two builds can be compared output for output.
 """
 import argparse
 import ctypes
@@ -29,9 +30,6 @@ if ROOT not in sys.path:
 
 R_GRID = 257
 FLOP_PER_POINT = 2363906          # 2*(257*1024+1281*512+769*256+513*128+385*1)  (BASELINE.md §4)
-# DRAM bytes of one query_tc3_kernel launch over the dense 257^3 grid, from an `ncu --set full` capture (not re-measured by a
-# bench run: profiling and timing never share a run).  Updated by hand from profiles/ when the kernel changes.
-TRAFFIC_NCU = {"bytes": 82.69e6, "source": "profiles/r02_final_ncu_tc_summary.txt: 44.79 MB read + 37.90 MB written (ncu --set full pass of tools/gpu_r02_final.sh)"}
 B_MIN, B_MAX = (-1.0, -1.0, -1.0), (1.0, 1.0, 1.0)
 
 
@@ -45,11 +43,12 @@ def parse():
     ap.add_argument("--res", type=int, default=R_GRID)
     ap.add_argument("--exchange", default=os.environ.get("MONOPORT_B200_EXCHANGE", "auto"), choices=["auto", "nccl", "fused"],
                     help="N>1, how the ranks' ranges become the volume on every rank: 'nccl' = one in-place all-gather, 'fused' = "
-                         "peer-memory stores from the kernel epilogue + a barrier; 'auto' = fused from 4 GPUs on (measured: 2 GPUs "
-                         "1101 vs 1086 Mpoints/s in favour of NCCL, 8 GPUs 4647 vs 4733 in favour of the fused exchange)")
+                         "peer-memory stores from the kernel epilogue + a barrier; 'auto' = fused from 4 GPUs on")
     ap.add_argument("--fused-gather", action="store_true", help="same as --exchange fused")
     ap.add_argument("--no-recon", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write a seeded sample of the last timed step's occupancy volume (and its node indices) as DIR/*.npy")
     return ap.parse_args()
 
 
@@ -59,11 +58,12 @@ def peaks():
         d = json.load(open(p))
         return dict(source="measured", tf_burst=d["bf16_tflops"], tf_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     hbm=d["hbm_gbs"])
-    return dict(source="fallback", tf_burst=1590.0, tf_sustained=1400.0, hbm=6650.0)
+    # NVIDIA's data sheet for the H100 SXM (dense fp16 / bf16 tensor rate, HBM3 bandwidth at up to 700 W)
+    return dict(source="H100 SXM data sheet", tf_burst=989.0, tf_sustained=989.0, hbm=3350.0)
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -254,12 +254,12 @@ def run_ours(args):
     net.precision = args.mode
     mode_used = "tc" if (args.mode in ("auto", "tc") and net.surface_classifier.tc_supported()) else "fp32"
     if args.mode == "tc" and mode_used != "tc":
-        raise SystemExit("tcgen05 kernel unavailable")
+        raise SystemExit("tensor-core kernel unavailable")
     cal_cpu = scene_calib()
     cal = cal_cpu.to(dev)
     feats = [f.to(dev) for f in feats_cpu]
     n_pts_total = R ** 3
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > the 50 MB L2
     # balanced ranges of the z-major node order (z slabs whose boundaries need not fall on planes), ONE in-place all-gather
     sv = ShardedVolume(R, rank, world, dev)
     lin0, my_pts = sv.bounds[rank]
@@ -324,6 +324,13 @@ def run_ours(args):
         dist.all_reduce(same, op=dist.ReduceOp.MIN)
     volume_ok = bool(same.item())
     checksum = float(vol.double().sum().item())
+    if args.dump_outputs and rank == 0:
+        # what the timed path returned in its last step: a fixed, seeded sample of 4 Mi nodes of the volume (16 MB of fp32)
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        gs = torch.Generator().manual_seed(1234)
+        idx = torch.randperm(R ** 3, generator=gs)[:min(R ** 3, 1 << 22)].sort().values
+        np.save(os.path.join(args.dump_outputs, "occupancy_sample.npy"), vol.reshape(-1)[idx.to(dev)].float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "occupancy_sample_index.npy"), idx.double().numpy())
     g = torch.Generator().manual_seed(17)
     lin = torch.randint(0, R ** 3, (16384,), generator=g)
     parity = None
@@ -445,11 +452,10 @@ def run_ours(args):
             "gpu_launches": launches_per_step * args.steps,
             "roofline": {"bound": "tensor", "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s",
                          "frac": achieved_tf / peak_tf,
-                         "traffic": (TRAFFIC_NCU["bytes"] if (mode_used == "tc" and world == 1 and R == R_GRID) else None),
-                         "traffic_unit": "bytes/launch, dram__bytes_read.sum + dram__bytes_write.sum of query_tc3_kernel (%s)" % TRAFFIC_NCU["source"],
-                         "kernel": ("query_tc3_kernel (+ g0_tc_kernel, the per-frame per-texel layer-0 GEMM, 25 us)" if mode_used == "tc"
+                         "traffic": None, "traffic_unit": "not measured",
+                         "kernel": ("query_wg_kernel (+ g0_wg_kernel, the per-frame per-texel layer-0 GEMM)" if mode_used == "tc"
                                     else "query_fp32_kernel"),
-                         "kernel_ms": 1e3 * k_avg_s, "peak_source": pk["source"] + " bf16 sustained (cuBLAS loop)",
+                         "kernel_ms": 1e3 * k_avg_s, "peak_source": pk["source"] + " fp16 dense",
                          "frac_of_burst": achieved_tf / pk["tf_burst"],
                          "algorithmic_flop_per_point": FLOP_PER_POINT},
             "clocks": clocks,

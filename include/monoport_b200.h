@@ -1,5 +1,5 @@
 /*
- * monoport_b200 -- C ABI of the B200-native occupancy-field hot path of MonoPort.
+ * monoport_b200 -- C ABI of the H100-native occupancy-field hot path of MonoPort.
  *
  * The reference (Project-Splinter/MonoPort) is pure Python: it has no FFI.  Its boundary for this path is
  * a Python call protocol (SURVEY.md §8b).  This header is the C-ABI a binding for that protocol
@@ -46,8 +46,8 @@ extern "C" {
 
 /* arithmetic of the fused sample+MLP kernel */
 #define MP_MODE_FP32 0   /* CUDA-core fp32 everywhere (|err| ~1e-6 vs the reference)                 */
-#define MP_MODE_TC 1     /* tcgen05 fp16 operands / fp32 TMEM accumulators, last layer fp32 (<=1e-4)   */
-#define MP_MODE_AUTO 2   /* TC when the head/feature shape is supported by the tcgen05 kernel, else FP32 */
+#define MP_MODE_TC 1     /* wgmma fp16 operands / fp32 register accumulators, last layer fp32 (<=1e-4)   */
+#define MP_MODE_AUTO 2   /* TC when the head/feature shape is supported by the wgmma kernel, else FP32 */
 /* 3 was MP_MODE_TC_V2 (the self-contained tensor-core program, removed in round 2: 335 vs 485 Mpoints/s); rejected now */
 #define MP_MODE_TC_V3 4  /* alias of MP_MODE_TC: the one tensor-core program (layer 0 hoisted to texels)                     */
 
@@ -62,7 +62,7 @@ int mp_device_info(int* sm_count, int* cc_major, int* cc_minor);
  * weights[l] is filters.l.weight as [Cout_l, Cin_l] row-major fp32 with Cin_l = channels[l] +
  * (l>0 && skip ? channels[0] : 0)  (:24-34), biases[l] is [Cout_l].  skip = !no_residual.
  * Pointers are host (on_device=0) or device (on_device=1) memory; they are only read during the call.
- * The handle owns repacked copies (fp32 K-major for the CUDA-core kernel, fp16 UMMA tiles for tcgen05).
+ * The handle owns repacked copies (fp32 K-major for the CUDA-core kernel, fp16 K-major SWIZZLE_128B tiles for the wgmma kernel).
  * ------------------------------------------------------------------------------------------- */
 typedef struct mp_mlp mp_mlp_t;
 int mp_mlp_create(int n_layers, const int* channels, const float* const* weights,

@@ -1,4 +1,4 @@
-"""monoport_b200 -- B200-native (sm_100a) occupancy-field hot path of MonoPort.
+"""monoport_b200 -- H100-native (sm_90a) occupancy-field hot path of MonoPort.
 
 Public surface (mirrors the reference's, see INTEGRATION.md):
     monoport_b200.modeling.MonoPortNet / PIFuNetG / PIFuNetC     (monoport/lib/modeling/MonoPortNet.py)

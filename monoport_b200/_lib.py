@@ -92,7 +92,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise MonoportLibraryError(
-            "%s not found: build it with `python -m monoport_b200.build` (nvcc, sm_100a). "
+            "%s not found: build it with `python -m monoport_b200.build` (nvcc, sm_90a). "
             "monoport_b200 has no CPU / PyTorch fallback." % LIB_PATH)
     try:
         lib = ctypes.CDLL(LIB_PATH)

@@ -1,4 +1,4 @@
-"""Build recipe for libmonoport_b200.so (sm_100a only, in-tree so the .so travels to the GPU box)."""
+"""Build recipe for libmonoport_b200.so (sm_90a only, in-tree so the .so travels to the GPU box)."""
 import os
 import shutil
 import subprocess
@@ -10,7 +10,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmonoport_b200.so")
 SOURCES = ["mp_api.cu", "query_fp32.cu", "query_tc.cu", "octree.cu", "mcubes.cu", "surface.cu"]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",
 ]
 
@@ -32,7 +32,7 @@ def _stale():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu for sm_100a into one shared library.  Returns the library path."""
+    """Compile every .cu for sm_90a into one shared library.  Returns the library path."""
     if not force and not _stale():
         return LIB_PATH
     os.makedirs(LIB_DIR, exist_ok=True)
@@ -60,7 +60,7 @@ def build(force=False, verbose=False):
     if verbose:
         print("\n".join(log))
     tmp = LIB_PATH + ".tmp"
-    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp] + objs + ["-lcudart_static", "-lcuda", "-ldl", "-lrt", "-lpthread",
+    subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", tmp] + objs + ["-lcudart_static", "-lcuda", "-ldl", "-lrt", "-lpthread",
                            "-L/usr/local/cuda/lib64/stubs"])
     os.replace(tmp, LIB_PATH)
     return LIB_PATH

@@ -119,7 +119,7 @@ extern "C" int mp_mlp_create(int n_layers, const int* channels, const float* con
     mp_mlp_destroy(h);
     return MP_E_CUDA;
   }
-  int rc = mp_tc_prepare(h);   // sets tc_ok (0 when the head shape is not handled by the tcgen05 kernel)
+  int rc = mp_tc_prepare(h);   // sets tc_ok (0 when the head shape is not handled by the tensor-core kernel)
   if (rc != MP_OK) {
     mp_mlp_destroy(h);
     return rc;
@@ -266,7 +266,7 @@ int mp_query_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const M
   if (mode == MP_MODE_AUTO) mode = tc_can ? MP_MODE_TC : MP_MODE_FP32;
   if (mode == MP_MODE_TC || mode == MP_MODE_TC_V3) {
     if (!mlp->tc_ok) {
-      mp_set_error("MP_MODE_TC requested but the tcgen05 kernel does not support this head/device");
+      mp_set_error("MP_MODE_TC requested but the tensor-core kernel does not support this head/device");
       return MP_E_UNSUPPORTED;
     }
     // Range guard: the tensor-core program is validated (<= 1e-4 on what query() returns) for frames whose largest

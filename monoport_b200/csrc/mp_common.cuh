@@ -1,4 +1,4 @@
-// Shared internals of libmonoport_b200 (sm_100a only).  Not part of the ABI.
+// Shared internals of libmonoport_b200 (sm_90a only).  Not part of the ABI.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -71,9 +71,9 @@ struct mp_mlp {
   // fp32 path: per layer W^T as [cin][cout] (k-major rows, cout contiguous) + bias
   float* wt[MP_MAX_LAYERS];
   float* bias[MP_MAX_LAYERS];
-  // original [cout][cin] fp32 (row-major) kept for the fp32 last layer of the tcgen05 path
+  // original [cout][cin] fp32 (row-major) kept for the fp32 last layer of the tensor-core path
   float* w[MP_MAX_LAYERS];
-  // tcgen05 path (query_tc.cu): packed fp16 weight tiles + fp32 side vectors; null when unsupported
+  // tensor-core path (query_tc.cu): packed fp16 weight tiles + fp32 side vectors; null when unsupported
   void* tc;
   int tc_ok;
   int device;
@@ -90,7 +90,7 @@ struct mp_feat {
   float* nhwc_own;
   float* staging;   // [C][H][W] device staging for host uploads
   int device;
-  // layer-0 pre-activation per texel, G0 = W0[:, :C] . F  ([H*W][g0_n] fp16), built lazily by the tcgen05 v3 path
+  // layer-0 pre-activation per texel, G0 = W0[:, :C] . F  ([H*W][g0_n] fp16), built lazily by the tensor-core path
   // (bilinear sampling is linear, so sampling G0 equals applying W0 to the sampled features); valid for
   // (g0_owner == generation id of the head handle, g0_version == version).  The owner is the head's generation id, not
   // its address: a head rebuilt after a weight change may be handed the freed handle's address again.
@@ -158,7 +158,7 @@ struct MpOutDst {
 };
 
 // ---------------------------------------------------------------------------------------------
-// device helpers shared by the fp32 and tcgen05 kernels
+// device helpers shared by the fp32 and tensor-core kernels
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mp_load_point(const MpPointSrc& s, long long i, float& x, float& y, float& z) {
   if (s.kind == MP_SRC_ROWS) {

@@ -2,7 +2,7 @@
 // on CUDA cores, fp32 end to end.  Replaces MonoPortNet.query (monoport/lib/modeling/MonoPortNet.py:48-91):
 //   orthogonal()/perspective() geometry.py:19-55, index() geometry.py:4-16, DepthNormalizer.py:32,
 //   SurfaceClassifier.forward heads/SurfaceClassifier.py:39-71.
-// This is the exact (|err| ~1e-6) path and the one every head shape can use; the tcgen05 kernel
+// This is the exact (|err| ~1e-6) path and the one every head shape can use; the tensor-core kernel
 // (query_tc.cu) is the fast path for the shipped heads.
 //
 // One CTA owns a tile of P points and walks all layers with the activations resident in shared memory:

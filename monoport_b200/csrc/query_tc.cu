@@ -1,81 +1,87 @@
-// F1 (tcgen05 flavour): the fused  project -> mask -> bilinear gather -> z-concat -> 5-layer skip-MLP -> sigmoid -> mask
-// kernel of MonoPortNet.query (monoport/lib/modeling/MonoPortNet.py:48-91; heads/SurfaceClassifier.py:39-71) on the
-// 5th-generation tensor cores.  Specialised for the shipped geometry head PIFuNetGMLP
-// (filter_channels [257,1024,512,256,128,R], skip-concat, heads/SurfaceClassifier.py:74-79) on a 256-channel map.
+// F1 (tensor-core flavour): the fused  project -> mask -> bilinear gather -> z-concat -> 5-layer skip-MLP -> last op -> mask
+// kernel of MonoPortNet.query (monoport/lib/modeling/MonoPortNet.py:48-91; heads/SurfaceClassifier.py:39-71) on the Hopper
+// warpgroup tensor cores (wgmma).  Specialised for the two shipped heads, which share one program:
+//   geometry  PIFuNetGMLP  filter_channels [257,1024,512,256,128,1], Sigmoid, on a 256-channel map;
+//   colour    PIFuNetCMLP  filter_channels [513,1024,512,256,128,3], Tanh,    on a 512-channel map.
 //
-// Arithmetic: layers 0-3 fp16 operands x fp16 weights -> fp32 accumulators in TMEM; the depth column (z_feat) and the
-// bias of every layer are applied in fp32 in the epilogue (so K is exactly 256-aligned, no padding); the last layer
-// (385 -> R) runs in fp32 on CUDA cores from the fp32 layer-3 accumulators and the fp32-sampled features.
+// Arithmetic: layers 1-3 fp16 operands x fp16 weights -> fp32 accumulators in registers; the depth column (z_feat) and the
+// bias of every layer are applied in fp32 in the epilogue (so K is exactly 64-aligned, no padding); the last layer
+// (128 + C + 1 -> R) runs in fp32 on CUDA cores from the fp32 layer-3 accumulators and the fp32-sampled features.
+// Layer 0 is hoisted from points to texels: bilinear sampling is linear, so  W0[:, :C] . sample(F)(u,v) ==
+// sample(W0[:, :C] . F)(u,v).  g0_wg_kernel builds G0 = W0f . F once per frame and head (fp16, [texel][1024]) and the
+// query kernel SAMPLES the 1024-channel layer-0 pre-activation: h0 = lrelu(lerp(G0) + b0 + w0z * z).
+// Colour head only: layer 3 multiplies by W3 as an fp16 PAIR (hi + lo, two MMAs per K-step on the same A operand): the
+// Tanh output is four times as sensitive to the logit as the geometry head's Sigmoid, and the rounding of W3 is the largest
+// single term of its error.
 //
-// One persistent CTA per SM, a tile = 128 points = the M dimension of every MMA (one TMEM lane per point).  Layer 0 is
-// hoisted from points to texels (g0_tc_kernel builds G0 = W0f . F per frame on the tensor cores and the main kernel SAMPLES
-// the 1024-channel layer-0 pre-activation, see "program v3" below); layer 1 owns all 512 TMEM columns and is drained in
-// place; H1, H2 feed the next layer as the A operand from TMEM; weights stream L2 -> smem through a 3-stage ring of 32 KB
-// tiles filled by cp.async.bulk (TMA engine), pre-packed on the host in exactly the order the MMA warp consumes them.
-//
-// Round 2 removed two variants that had been kept selectable: the self-contained program v2 (all five layers per point,
-// layer 0 recomputed for the second half of layer 1: 335 vs 485 Mpoints/s) and the cta_group::2 flavour (a CTA pair
-// sharing every weight tile).  tools/tc_rate.cu measures why the pair does not pay on this chip: a 128x256x16 fp16 MMA
-// issued back to back from shared-memory operands takes 246 cycles with one CTA and 247.6 cycles for the M = 256 pair
-// instruction -- the same per-SM rate -- and the pair loses 40 more cycles per MMA to cluster-scope waits once the
-// weights stream (profiles/r02_call2_tc_rate_probe.txt).
-//
-// Warp roles (384 threads): warp 0 weight producer, warp 1 MMA issuer (one lane), warps 2-3 samplers (X operand, one tile
-// ahead; warp 2 also owns the TMEM allocation), warps 4-11 workers: layer-0 chunk generators, then two epilogue warpgroups.
+// One persistent CTA per SM; a tile = 64 points = the M of every warpgroup MMA.  Warps 0-3 and 4-7 are two consumer
+// warpgroups that split the N dimension of every layer (layer 1: 256 columns each, 128 fp32 accumulators per thread;
+// layer 2: 128; layer 3: 64); both sample the operands (X, the layer-0 chunks) and run the epilogues.  Warp 8 streams the
+// weights L2 -> shared memory through a ring of 32 KB stages (cp.async.bulk on mbarriers), pre-packed on the host as
+// K-major SWIZZLE_128B tiles in exactly the order the consumers take them.  The program is written so that layer-0 chunk
+// c+1 is generated while the MMAs of chunk c are in flight, but at 168 registers per thread (9 warps per CTA) ptxas
+// inserts warpgroup.arrive around the accumulators and serializes the wgmma instructions (C7520): today every MMA
+// completes before the next instruction, so that overlap does not happen.
 #include "mp_common.cuh"
 #include "tc_ptx.cuh"
 #include <stdlib.h>
-#include <cuda.h>          // CUtensorMap (the encoder itself is fetched from the driver at run time)
 
 namespace {
 
-constexpr int kC = 256;                 // feature channels
-constexpr int kTile = 128;              // points per tile
-constexpr int kThreads = 384;
-
-// weight ring: 96 KB.  One CTA per tile (CG = 1): 3 stages of 32 KB = whole weight tiles.  CTA pair (CG = 2, see
-// query_tc3_kernel): every CTA holds HALF of the rows of each tile, 6 stages of 16 KB -- the ring covers twice as many MMAs.
-template <int CG> struct CfgT {
-  static constexpr int Stages = 3 * CG;
-  static constexpr int StageBytes = 32768 / CG;
-  static constexpr int Sub = StageBytes / 2;       // second K-block of a two-K-block (128-row tile) stage
-};
-using Cfg = CfgT<1>;
-constexpr int kStages = 6;                          // weight-ring barrier slots (max over the variants)
-constexpr int kRingBytes = 98304;
+constexpr int kTile = 64;                       // points per tile
+constexpr int kConsumers = 256;                 // two consumer warpgroups
+constexpr int kThreads = kConsumers + 32;       // + the weight producer warp
 constexpr int kL0 = 1024, kL1 = 512, kL2 = 256, kL3 = 128;
-constexpr int kMaxRes = 1;             // output channels handled by the fp32 tail (PIFuNetGMLP: 1)
-
-// per-tile weight stream (32 KB stages), in MMA consumption order
-constexpr int kStagesPerTile3 = 32 + 8 + 12 + 4;                  // L1 hidden (8 chunks x 2 K-blocks x 2 N-halves) + L1 skip + L2 + L3
-
+constexpr int kStageBytes = 32768;              // one ring stage: 256 weight rows x 64 K (or 2 x 128 rows x 64 K)
+constexpr int kKb = kTile * 128;                // one 64-channel K-block of a 64-row A operand
 constexpr int kSideFloats = kL0 + kL1 + kL2 + kL3;      // 1920 hidden output channels over layers 0..3
 __host__ __device__ constexpr int side_off(int l) { return l == 0 ? 0 : l == 1 ? kL0 : l == 2 ? kL0 + kL1 : kL0 + kL1 + kL2; }
 
+// C = feature channels of the head's map (256: geometry, 512: colour)
+template <int C> struct Prog {
+  static constexpr int XKB = C / 64;                          // K-blocks of the skip operand X
+  static constexpr int RES = C == 256 ? 1 : 3;                // last-layer outputs
+  static constexpr int L3Pass = C == 256 ? 1 : 2;             // colour: W3 as (hi, lo)
+  // weight stream of one tile, in consumption order:
+  //   L1: per K-block (16 of H0, then XKB of X) two stages = output halves [0,256), [256,512)
+  //   L2: per K-block (8 of H1, then XKB of X) one stage = all 256 outputs
+  //   L3: per pass, per two K-blocks (XKB of X, then 4 of H2) one stage = 2 x 128 outputs
+  static constexpr int StagesL1 = 2 * (16 + XKB);
+  static constexpr int StagesL2 = 8 + XKB;
+  static constexpr int StagesL3 = L3Pass * (XKB + 4) / 2;
+  static constexpr int StagesPerTile = StagesL1 + StagesL2 + StagesL3;
+  static constexpr int Ring = C == 256 ? 3 : 2;
+  // shared memory (offsets inside the 1024-aligned dynamic block)
+  static constexpr int X = 0;                                 // XKB x 8 KB
+  static constexpr int H0 = X + XKB * kKb;                    // 2 chunk buffers x 2 K-blocks; H2 (4 K-blocks) after layer 1
+  static constexpr int H1 = H0 + 4 * kKb;                     // 8 K-blocks; the last layer's partial sums after layer 2
+  static constexpr int Wr = H1 + 8 * kKb;                     // Ring x 32 KB
+  static constexpr int Small = Wr + Ring * kStageBytes;       // zf[64], inimg[64], s4[RES][64]
+  static constexpr int Bars = Small + (2 + RES) * kTile * 4;  // full[Ring], empty[Ring]
+  static constexpr int Total = Bars + 2 * Ring * 8;
+};
+static_assert(Prog<256>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
+static_assert(Prog<512>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
+static_assert(Prog<256>::XKB % 2 == 0 && Prog<512>::XKB % 2 == 0, "layer-3 stages hold two K-blocks");
+
 struct TcPack {
-  __half* w3stream;       // stage stream of a tile: kStagesPerTile3 (geometry) / kStagesPerTileC (colour) x 32 KB
-  __half* w3pair[2];      // CTA-pair variant: per cluster rank, kStagesPerTile3 x 16 KB (this rank's half of the rows of every tile)
-  CUtensorMap tmap_pair[2];   // 2-D tensor maps over w3pair[r]: [rows][64 fp16], box = one 16 KB stage (128 rows)
-  int pair_ok;
-  __half* d_bias0;        // fp16 device copies of the layer-0 bias / depth column for per-lane channel access (v3 H0 generation)
+  __half* wstream;        // stage stream of a tile: Prog<C>::StagesPerTile x 32 KB
+  __half* d_bias0;        // fp16 copies of the layer-0 bias / depth column for the H0 generation
   __half* d_wz0;
-  uint8_t* d_w0t;         // the same as fp16 SWIZZLE_128B tiles [n tile 4][K block 4][256 x 64] for g0_tc_kernel
-  float* bias[4];         // per hidden layer
-  float* wz[4];           // z column of every hidden layer
+  uint8_t* d_w0t;         // W0[:, :C] as fp16 SWIZZLE_128B tiles [n tile 4][K block C/64][256 x 64] for g0_wg_kernel
   float h_bias[kSideFloats];   // host copies (passed by value in the kernel parameters)
   float h_wz[kSideFloats];
   float* w4h;             // [R][128]  last layer, hidden part
-  float* w4s;             // [R][256]  last layer, feature part
+  float* w4s;             // [R][C]    last layer, feature part
   float* w4z;             // [R]
   float* b4;              // [R]
   int res;
-  int kind;               // 0 = geometry head (programs v2 / v3), 1 = colour head (query_tc3c_kernel)
+  int kind;               // 0 = geometry head, 1 = colour head
 };
 
 struct TcParams {
   const __half* wstream;
-  // per-channel bias and depth-column weight of layers 0..3, carried in the kernel parameter (constant) bank: the
-  // epilogue reads them with warp-uniform indices, so they cost no load instructions and no shared memory
+  // per-channel bias and depth-column weight of layers 0..3, carried in the kernel parameter (constant) bank
   alignas(16) float bias_all[kSideFloats];
   alignas(16) float wz_all[kSideFloats];
   const float* w4h;
@@ -85,60 +91,32 @@ struct TcParams {
   int res;
   int last_op;
   int H, W;
-  const float* feat32;    // NHWC fp32 (bilinear taps are read in fp32: the last layer's skip access to the input
-                          // makes the output sensitive to the precision of x -- see DESIGN.md, precision)
-  const __half* g0;       // v3: [H*W][1024] fp16 per-texel layer-0 product
-  const __half* feat16;   // v3: NHWC fp16 copy of the map (taps of the X operand)
-  const float* s4tex;     // v3: [H*W][kMaxRes] fp32 per-texel last-layer feature part
-  const __half* d_bias0;  // v3: layer-0 bias and depth-feature column, fp16 [1024]
+  const __half* g0;       // [H*W][1024] fp16 per-texel layer-0 product
+  const __half* feat16;   // NHWC fp16 copy of the map (taps of the X operand)
+  const float* s4tex;     // [H*W][RES] fp32 per-texel last-layer feature part
+  const __half* d_bias0;  // layer-0 bias and depth-feature column, fp16 [1024]
   const __half* d_wz0;
-  unsigned long long* prof;   // optional [gridDim.x][32] cycle counters (MONOPORT_B200_TC_PROF=1), else null
-  int exp;                    // timing experiments only (MONOPORT_B200_TC_EXP bitmask; results are WRONG when set):
-                              // 1 = weights not re-streamed, 2 = layer-0 gathers all hit texel 0, 4 = X taps all hit texel 0
-  unsigned long long* trace;  // optional [128] absolute clock64 stamps of CTA 0's tile kTraceTile (MONOPORT_B200_TC_TRACE=1)
-  const unsigned* amax;       // range guard (see mp_guard_skips): max |feature| of the frame, limit of this head, sense
+  const unsigned* amax;   // range guard (see mp_guard_skips): max |feature| of the frame, limit of this head, sense
   float amax_limit;
   int guard;
-  alignas(64) CUtensorMap tmap_pair[2];     // CTA-pair variant: the two ranks' halves of the weight stream
 };
-constexpr int kTraceTile = 8;
-// v3 event ids: MMA issuer 0..31, worker warp 4 at 32.., worker warp 8 at 64.., sampler warp 2 at 96..
-// (all of these compile to nothing unless the kernel is instantiated with PROF: `kProf` is a constant of its scope)
-#define TRACE(cond, id) do { if (kProf && prm.trace && (cond)) prm.trace[id] = (unsigned long long)clock64(); } while (0)
-enum Prof { P_TOTAL = 0, P_XREADY, P_ACC0FREE, P_WFULL, P_UNUSED4, P_H0READY, P_ACC1DRAINED, P_H1READY, P_H2READY,
-            P_W_SAMPLE = 16, P_W_ACC0FULL, P_W_H0FREE, P_W_ACC1FULL, P_W_ACC2FULL, P_W_ACC3FULL, P_W_DRAIN0, P_W_DRAIN1,
-            P_W_DRAIN2, P_W_DRAIN3, P_W_XFREE };
-#define PROF_T0() const long long _t0 = (kProf && prof) ? clock64() : 0
-#define PROF_ADD(slot) do { if (kProf && prof) prof[slot] += (unsigned long long)(clock64() - _t0); } while (0)
 
-struct Smem {
-  // offsets inside the 1024-aligned dynamic shared memory block
-  static constexpr int X = 0;                                   // 4 K-blocks x 16 KB
-  static constexpr int H0 = X + 65536;                          // 2 buffers x (2 K-blocks x 16 KB)
-  static constexpr int Wr = H0 + 65536;                         // kStages x 32 KB
-  static constexpr int Small = Wr + kRingBytes;                 // zf[128], inimg[128], s4[kMaxRes][128]
-  static constexpr int Bars = Small + (2 + kMaxRes) * kTile * 4;
-  static constexpr int NumBars = 2 * kStages + 15;
-  static constexpr int TmemPtr = Bars + NumBars * 8;
-  static constexpr int Total = TmemPtr + 16;
+// Direct rendering of the visible surface (RTL/main.py:212-249) fused into the colour query: point i is the vertex
+// (X[i], Y[i], R - Z[i]) of forward_vertices mapped to world space by mat_color (RTL/main.py:201-210: diag((b_max-b_min)/R),
+// translation b_min), and its colour pred * 0.5 + 0.5 (:244) is scattered to canvas[X[i], Y[i], :] (:247-248) -- no
+// intermediate point / prediction tensors.  X == nullptr: the ordinary point sources and the [R,N] output.
+struct MpSurfaceSrc {
+  const long long* X;
+  const long long* Y;
+  const float* Z;
+  float scale[3], bmin[3];      // (b_max - b_min) / R and b_min, fp32 like torch's
+  float R;
+  float* canvas;                // [R, R, 3]
+  int canvas_R;
 };
-enum Bar { B_WFULL = 0, B_WEMPTY = kStages, B_XREADY = 2 * kStages, B_ACC0_FULL0, B_ACC0_FULL1, B_H0_READY0, B_H0_READY1,
-           B_H0_FREE0, B_H0_FREE1, B_ACC1_FULL, B_H1_READY, B_ACC2_FULL, B_H2_READY, B_ACC3_FULL, B_TILE_DONE, B_XFREE, B_PART_READY };
-static_assert(B_PART_READY + 1 == Smem::NumBars, "barrier count");
-static_assert(Smem::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
-
-__device__ __forceinline__ void wait_bar(uint64_t* bars, int which, uint32_t& count) {
-  tc::mbar_wait(bars + which, count & 1u);
-  ++count;
-}
-// "free"-type barriers: the first use must pass without any arrival
-__device__ __forceinline__ void wait_free(uint64_t* bars, int which, uint32_t& count) {
-  tc::mbar_wait(bars + which, (count & 1u) ^ 1u);
-  ++count;
-}
 
 // --------------------------------------------------------------------------------------------------------------------
-// sampling helpers shared by both programs
+// sampling helpers
 // --------------------------------------------------------------------------------------------------------------------
 struct PointTaps {
   int off[4];       // texel indices of the four bilinear taps (0 when the point is invalid)
@@ -147,14 +125,22 @@ struct PointTaps {
   bool in_img;      // MonoPortNet.py:74
 };
 
-// projection (geometry.py:19-55) + mask + taps of point i (i >= n: masked-out padding point)
-__device__ __forceinline__ PointTaps point_taps(const MpPointSrc& src, const MpCalib& cal, int H, int W, long long i, long long n) {
+// projection (geometry.py:19-55) + mask + taps of point i (i >= n: masked-out padding point); surface vertices when surf.X
+__device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const MpPointSrc& src, const MpCalib& cal, int H, int W,
+                                                long long i, long long n) {
   PointTaps pt;
   float u = 0.f, v = 0.f, w = 0.f;
   const bool valid = i < n;
   if (valid) {
     float x, y, z;
-    mp_load_point(src, i, x, y, z);
+    if (surf.X) {
+      const float vx = (float)__ldg(surf.X + i), vy = (float)__ldg(surf.Y + i), vz = __fsub_rn(surf.R, __ldg(surf.Z + i));
+      x = __fadd_rn(__fmul_rn(vx, surf.scale[0]), surf.bmin[0]);
+      y = __fadd_rn(__fmul_rn(vy, surf.scale[1]), surf.bmin[1]);
+      z = __fadd_rn(__fmul_rn(vz, surf.scale[2]), surf.bmin[2]);
+    } else {
+      mp_load_point(src, i, x, y, z);
+    }
     mp_project(cal, x, y, z, u, v, w);
   }
   pt.in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);
@@ -166,944 +152,14 @@ __device__ __forceinline__ PointTaps point_taps(const MpPointSrc& src, const MpC
   return pt;
 }
 
-// Whole warp: sample the 16 points whose taps sit in lanes 0..15 (`pt`, duplicated in lanes 16..31) into rows
-// [pbase, pbase+16) of the fp16 X tile (K-major SWIZZLE_128B, 4 K-blocks of 64 channels; lane covers 8 channels) from the
-// fp16 copy of the map, four points per batch; the last layer's direct feature access is NOT derived from these samples but from S4 (fp32, per texel), which
-// the lane owning the point interpolates in fp32.
-__device__ __forceinline__ void sample_x_group16(const TcParams& prm, uint8_t* smem_x, float* s_zf, float* s_in, float* s_s4,
-                                                 PointTaps pt, int pbase, int lane) {
-  const int cbase = lane * 8;
-#pragma unroll 1
-  for (int q0 = 0; q0 < 16; q0 += 4) {
-    uint4 raw[4][4];                         // [point][tap] 8 fp16 channels
-    float wgt[4][4];
-#pragma unroll
-    for (int qq = 0; qq < 4; ++qq)
-#pragma unroll
-      for (int a = 0; a < 4; ++a) {
-        const int off = __shfl_sync(0xffffffffu, pt.off[a], q0 + qq);
-        wgt[qq][a] = __shfl_sync(0xffffffffu, pt.wgt[a], q0 + qq);
-        raw[qq][a] = __ldg(reinterpret_cast<const uint4*>(prm.feat16 + (size_t)off * kC + cbase));
-      }
-#pragma unroll
-    for (int qq = 0; qq < 4; ++qq) {
-      const int p = pbase + q0 + qq;
-      float2 acc[4];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) {                   // same accumulation order as grid_sample: nw, ne, sw, se
-        const float2 w2 = make_float2(wgt[qq][a], wgt[qq][a]);
-        const __half2* h2 = reinterpret_cast<const __half2*>(&raw[qq][a]);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[j] = (a == 0) ? __fmul2_rn(__half22float2(h2[j]), w2) : __ffma2_rn(__half22float2(h2[j]), w2, acc[j]);
-      }
-      uint4 packed;
-      packed.x = tc::pack_half2(acc[0].x, acc[0].y);
-      packed.y = tc::pack_half2(acc[1].x, acc[1].y);
-      packed.z = tc::pack_half2(acc[2].x, acc[2].y);
-      packed.w = tc::pack_half2(acc[3].x, acc[3].y);
-      *reinterpret_cast<uint4*>(smem_x + (lane >> 3) * 16384 + tc::sw128_offset(p, (lane & 7) * 8)) = packed;
-    }
-  }
-  if (lane < 16) {
-    if (prm.exp & 4) { pt.off[0] = pt.off[1] = pt.off[2] = pt.off[3] = 0; }
-#pragma unroll
-    for (int r = 0; r < kMaxRes; ++r) {
-      if (r < prm.res) {
-        float s = 0.f;
-#pragma unroll
-        for (int a = 0; a < 4; ++a) s = fmaf(pt.wgt[a], __ldg(prm.s4tex + (size_t)pt.off[a] * kMaxRes + r), s);
-        s_s4[r * kTile + pbase + lane] = s + __ldg(prm.w4z + r) * pt.zf + __ldg(prm.b4 + r);
-      }
-    }
-    s_zf[pbase + lane] = pt.zf;
-    s_in[pbase + lane] = pt.in_img ? 1.f : 0.f;
-  }
-}
-
-// --------------------------------------------------------------------------------------------------------------------
-// hand-off helper: one elected lane per warp arrives after __syncwarp(); every lane has already executed its own
-// proxy / tcgen05 fence.
-__device__ __forceinline__ void warp_arrive_local(uint64_t* bar, int lane) {
-  __syncwarp();
-  if (lane == 0) tc::mbar_arrive(bar);
-}
-// ====================================================================================================================
-// v3: layer 0 hoisted from points to texels.
-// Bilinear sampling is linear, so  W0[:, :256] . sample(F)(u,v) == sample(W0[:, :256] . F)(u,v).  G0 = W0f . F is built once
-// per frame per texel (g0_kernel below: 16384 x 1024 x 256 fp32 GEMM, 4.3 GFLOP instead of 17 M points x 0.5 MFLOP), and
-// the kernel *samples* the 1024-channel layer-0 pre-activation: h0 = lrelu(lerp(G0) + b0 + w0z * z).
-//   * no layer-0 MMAs, no layer-0 accumulator in TMEM  =>  layer 1 owns all 512 TMEM columns, no halves, no recompute;
-//   * 1.0 MB less weight traffic per tile (1.84 MB instead of 2.88 MB);
-//   * the layer-0 chunk no longer depends on the tensor pipe (MMA -> drain -> MMA chain gone): workers generate H0
-//     chunks ahead of the MMA issuer through the double-buffered smem ring.
-// TMEM map: acc1 [0,512)  --drain in place-->  H1lo [0,128) | acc2 [128,384) | H1hi [384,512)
-//           --drain-->  H2 [0,128) | (free) | acc3 [384,512)
-// roofline.achieved keeps counting the ALGORITHMIC 2 363 906 FLOP/point; the hoisted layer is not executed per point.
-// PEERS: also store channel 0 into the peer volumes of dst (fused slab exchange); the default instantiation carries no
-// trace of it.
-//
-// CG = 2 (opt-in, MONOPORT_B200_TC_CG=2; measured 2.4 % slower than CG = 1, see mp_launch_query_tc): a CTA PAIR (2-CTA cluster
-// on one TPC) works on two tiles at once with tcgen05.mma.cta_group::2 (M = 256 = the 128 points of each CTA).  Every weight tile is split between the two shared memories (each CTA streams half of its rows by
-// tensor-map TMA, both halves completing on the leader's barrier), so each SM ingests half of the weight bytes per point
-// and the 96 KB ring covers twice as many MMAs.  That matters since the MMAs are issued at the tensor pipe's rate: the
-// one-CTA kernel then waits 16.5 k of 69 k cycles per tile for weight stages (profiles/r02_call6_*), the L2 -> SM stream
-// being the bound.  Everything per tile -- operands in shared / tensor memory, samplers, workers, epilogue -- stays local
-// to its CTA; the leader (rank 0) issues all MMAs, operand hand-offs are remote mbarrier arrivals on the leader's
-// barriers, MMA completions are multicast to both CTAs by tcgen05.commit.
-//
-// WM (CG = 1 only; the default for launches of several waves, see mp_launch_query_tc; MONOPORT_B200_TC_WM=0 / 1): two
-// INDEPENDENT one-CTA programs launched as a 2-CTA cluster that share the weight stream: each CTA fetches half of every 32 KB
-// stage and multicasts it into both shared memories (cp.async.bulk ... .multicast::cluster), so the L2 serves each weight
-// byte once per pair.  Everything else is CTA-local (cta_group::1 MMAs); the only coupling is the ring: a slot is refilled
-// when BOTH issuers have released it (tcgen05.commit multicast onto both CTAs' "empty" barriers), so the two CTAs drift by at
-// most the ring's three stages.
-// PROF: the in-kernel cycle attribution / trace (MONOPORT_B200_TC_PROF, MONOPORT_B200_TC_TRACE) as its own instantiation: the
-// shipped kernels carry no trace of it (the issue loop is sensitive to every instruction, see the issuer below).
-template <bool PEERS = false, int CG = 1, bool WM = false, bool PROF = false>
-__global__ void __launch_bounds__(kThreads, 1)
-query_tc3_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, MpOutDst dst) {
-  constexpr bool kProf = PROF;
-  static_assert(!(WM && CG == 2), "weight multicast is a variant of the one-CTA program");
-  constexpr int TP = (CG == 2 || WM) ? 2 : 1;          // tiles (CTAs) per scheduling group
-  using C = CfgT<CG>;
-  MP_DYN_SMEM(uint8_t, smem_raw);
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Smem::Bars);
-  float* s_zf = reinterpret_cast<float*>(smem + Smem::Small);
-  float* s_in = s_zf + kTile;
-  float* s_s4 = s_in + kTile;
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + Smem::TmemPtr);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid: nothing is allocated yet)
-  unsigned long long* prof = (kProf && prm.prof) ? prm.prof + (size_t)blockIdx.x * 32 : nullptr;
-
-  long long n = src.n;
-  if (src.count_dev) {
-    const long long c = *src.count_dev;
-    n = c < n ? c : n;
-  }
-  long long win0, win1;
-  mp_shard_window(src, n, win0, win1);
-  n = win1;                                          // points >= n are padding; tile 0 starts at point win0
-  const long long n_tiles = (win1 - win0 + kTile - 1) / kTile;
-  // the unit of scheduling is a group of CG tiles (one per CTA of the pair); both CTAs run the same number of iterations, a
-  // CTA whose tile lies beyond n_tiles computes on masked-out points
-  const long long n_groups = (n_tiles + TP - 1) / TP;
-  const long long g0 = blockIdx.x / TP, gstep = gridDim.x / TP;
-  const uint32_t rank = (TP == 2) ? tc::cluster_ctarank() : 0u;
-  const bool leader = CG == 1 || rank == 0;            // (who issues the MMAs: every CTA unless the pair shares them)
-
-  constexpr uint32_t cAcc1 = 0, cH1lo = 0, cH1hi = 384, cAcc2 = 128, cH2 = 0, cAcc3 = 384;
-
-  if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      tc::mbar_init(bars + B_WFULL + s, 1);
-      tc::mbar_init(bars + B_WEMPTY + s, WM ? 2 : 1);      // WM: released by both issuers of the pair
-    }
-    // operand hand-offs to the MMA issuer count one arrival per producing warp of EVERY CTA of the pair (they all arrive on
-    // the leader's barriers); what the issuer hands back (tcgen05.commit) reaches both CTAs' own barriers
-    constexpr int kW = 8 * CG;
-    tc::mbar_init(bars + B_XREADY, 2 * CG);        // the two sampler warps
-    tc::mbar_init(bars + B_H0_READY0, kW);
-    tc::mbar_init(bars + B_H0_READY1, kW);
-    tc::mbar_init(bars + B_H0_FREE0, 1);
-    tc::mbar_init(bars + B_H0_FREE1, 1);
-    tc::mbar_init(bars + B_ACC1_FULL, 1);
-    tc::mbar_init(bars + B_H1_READY, kW);
-    tc::mbar_init(bars + B_ACC2_FULL, 1);
-    tc::mbar_init(bars + B_H2_READY, kW);
-    tc::mbar_init(bars + B_ACC3_FULL, 1);
-    tc::mbar_init(bars + B_TILE_DONE, 8 * CG);         // both warpgroups read acc3 (fp32 tail)
-    tc::mbar_init(bars + B_XFREE, 1);
-    tc::mbar_init(bars + B_PART_READY, 4);         // v3 fp32 tail: warpgroup 1's partial dot products are in smem (CTA-local)
-    tc::mbar_init(bars + B_ACC0_FULL0, 2);         // v3: "per-point scalars of this tile are in smem" (CTA-local)
-    tc::mbar_init(bars + B_ACC0_FULL1, 1);
-    tc::fence_barrier_init();
-    if constexpr (CG == 2) tc::tma_prefetch_desc(&prm.tmap_pair[rank]);
-  }
-  if (warp == 2) {
-    if constexpr (CG == 1) { tc::tmem_alloc(s_tmem, 512); tc::tmem_relinquish(); }
-    else { tc::tmem_alloc2(s_tmem, 512); tc::tmem_relinquish2(); }
-  }
-  tc::tcgen05_fence_before();
-  if constexpr (TP == 1) __syncthreads(); else tc::cluster_sync_all();
-  tc::tcgen05_fence_after();
-  const uint32_t tbase = *s_tmem;
-  // an operand hand-off of a producing warp to the MMA issuer (which lives in the leader CTA)
-  auto arrive_issuer = [&](int which) {
-    __syncwarp();
-    if (lane == 0) {
-      if constexpr (CG == 1) tc::mbar_arrive(bars + which);
-      else tc::mbar_arrive_remote(bars + which, 0);
-    }
-  };
-
-  if (warp == 0) {
-    // ============================== weight producer (every CTA streams its own part of every tile) ===============
-    if (lane == 0) {
-      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
-      uint32_t it = 0;
-      for (long long g = g0; g < n_groups; g += gstep) {
-        for (int s = 0; s < kStagesPerTile3; ++s, ++it) {
-          const int slot = it % C::Stages;
-          const uint32_t use = it / C::Stages;
-          if constexpr (WM) {
-            // my half of the stage, into both CTAs; my barrier expects the whole stage (the other half comes from the peer)
-            tc::mbar_wait_cluster(bars + B_WEMPTY + slot, (use & 1u) ^ 1u);
-            tc::mbar_arrive_expect_tx(bars + B_WFULL + slot, C::StageBytes);
-            tc::bulk_g2s_multicast(smem + Smem::Wr + slot * C::StageBytes + rank * (C::StageBytes / 2),
-                                   wsrc + (size_t)s * C::StageBytes + rank * (C::StageBytes / 2), C::StageBytes / 2,
-                                   bars + B_WFULL + slot, (uint16_t)3);
-            continue;
-          }
-          tc::mbar_wait(bars + B_WEMPTY + slot, (use & 1u) ^ 1u);
-          if constexpr (CG == 1) {
-            if ((prm.exp & 1) && it >= (uint32_t)C::Stages) { tc::mbar_arrive(bars + B_WFULL + slot); continue; }
-            tc::mbar_arrive_expect_tx(bars + B_WFULL + slot, C::StageBytes);
-            tc::bulk_g2s(smem + Smem::Wr + slot * C::StageBytes, wsrc + (size_t)s * C::StageBytes, C::StageBytes,
-                         bars + B_WFULL + slot);
-          } else {
-            // both halves of the stage complete on the LEADER's barrier (the leader arms it for 2 x 16 KB)
-            if (leader) tc::mbar_arrive_expect_tx(bars + B_WFULL + slot, 2 * C::StageBytes);
-            tc::tma_load_2d_cg2(smem + Smem::Wr + slot * C::StageBytes, &prm.tmap_pair[rank], 0, s * (C::StageBytes / 128),
-                                bars + B_WFULL + slot);
-          }
-        }
-      }
-    }
-  } else if (warp == 1 && !leader) {
-    // (the peer CTA's warp 1 has nothing to do: the leader issues the MMAs of both tiles)
-  } else if (warp == 1) {
-    // ============================== MMA issuer ==============================
-    // The WHOLE warp runs the control flow -- ring position, phase counters, descriptor bases: all warp-uniform, so the
-    // compiler keeps them in uniform registers -- and ONE elected lane executes, per sampled chunk / per phase, a single
-    // region with everything that has to happen in order: barrier waits, fences, the tcgen05.mma instructions and their
-    // commits.  How the issue loop is written decides the rate of the tensor pipe (tools/tc_rate.cu, cycles per 128x256x16
-    // MMA inside this pipeline, weights streaming + worker hand-offs):  issuing from inside `if (lane == 0)` 246 (the
-    // operands become per-thread values and reach the uniform registers through an elect / R2UR loop per instruction);
-    // warp-uniform loop with separate elected regions for every wait, the MMAs and the commit 187;  one elected region per
-    // weight stage 161;  one region per two stages 147;  the bare loop without hand-offs 128 = the pipe's floor
-    // (profiles/r02_call17_*, r02_call18_*).  Hence: one region per CHUNK (four stages, 16 MMAs) / per phase.
-    {
-      [[maybe_unused]] unsigned long long* const prof_el = prof;   // (PROF builds: the elected lane records the in-kernel timers)
-      const uint32_t idesc128 = tc::make_idesc_f16(128 * CG, 128);
-      const uint32_t idesc256 = tc::make_idesc_f16(128 * CG, 256);
-      // descriptor bases; inside the regions only compile-time multiples are added (address field = bytes >> 4)
-      const uint64_t dX = tc::make_sdesc_sw128(tc::smem_u32(smem + Smem::X), 1024);
-      const uint64_t dH0 = tc::make_sdesc_sw128(tc::smem_u32(smem + Smem::H0), 1024);
-      const uint64_t dW = tc::make_sdesc_sw128(tc::smem_u32(smem + Smem::Wr), 1024);
-      constexpr uint64_t kKb = 16384 >> 4;                 // one K-block of an A operand (128 rows x 64 channels)
-      constexpr uint64_t kStage = C::StageBytes >> 4;      // one ring slot
-      constexpr uint64_t kSub = C::Sub >> 4;               // second K-block of a two-K-block (128-row tile) stage
-      uint32_t slot = 0, wpar = 0;                         // ring slot of the next stage and the parity of its "full" phase
-      uint32_t c_xready = 0, n_chunks = 0, c_h1ready = 0, c_h2ready = 0, c_tiledone = 0;
-      const long long t_begin = (kProf && prof) ? clock64() : 0;
-      // ---- (all of these run inside an elected region: one lane)
-      auto wait_b = [&](int which, uint32_t par, [[maybe_unused]] int prof_slot) {
-        [[maybe_unused]] long long t0 = 0;
-        if constexpr (kProf) t0 = prof_el ? clock64() : 0;
-        if constexpr (CG == 1 && !WM) tc::mbar_wait(bars + which, par);
-        else tc::mbar_wait_cluster(bars + which, par);       // (arrivals / bytes partly come from the peer CTA)
-        if constexpr (kProf) { if (prof_el && prof_slot >= 0) prof_el[prof_slot] += (unsigned long long)(clock64() - t0); }
-      };
-      auto commit_b = [&](int which) {
-        if constexpr (CG == 1) tc::mma_commit(bars + which);
-        else tc::mma_commit2(bars + which);
-      };
-      auto release = [&](uint32_t sl) {                      // the stage's MMAs done -> its ring slot may be refilled
-        if constexpr (WM) tc::mma_commit_pair(bars + B_WEMPTY + sl);
-        else commit_b(B_WEMPTY + (int)sl);
-      };
-      // one K-block (64 channels = four K = 16 steps): descriptors advance by 32 B (+2 in the address field)
-      auto kblock_ss = [&](uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc0) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          if constexpr (CG == 1) tc::mma_ss(d, ad + 2 * kk, bd + 2 * kk, idesc, kk == 0 ? acc0 : 1u);
-          else tc::mma_ss2(d, ad + 2 * kk, bd + 2 * kk, idesc, kk == 0 ? acc0 : 1u);
-        }
-      };
-      auto kblock_ts = [&](uint32_t d, uint32_t a_tmem, uint64_t bd, uint32_t idesc, uint32_t acc0) {
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk) {
-          if constexpr (CG == 1) tc::mma_ts(d, a_tmem + kk * 8, bd + 2 * kk, idesc, kk == 0 ? acc0 : 1u);
-          else tc::mma_ts2(d, a_tmem + kk * 8, bd + 2 * kk, idesc, kk == 0 ? acc0 : 1u);
-        }
-      };
-      // ---- (uniform, all lanes) the ring positions of the next N stages
-      auto take = [&](uint32_t (&sl)[12], uint32_t (&pr)[12], int n_take) {
-#pragma unroll
-        for (int q = 0; q < 12; ++q)
-          if (q < n_take) {
-            sl[q] = slot; pr[q] = wpar;
-            if (++slot == (uint32_t)C::Stages) { slot = 0; wpar ^= 1u; }
-          }
-      };
-
-      for (long long g = g0; g < n_groups; g += gstep) {
-        // acc1 = [0,512) overlaps the previous tile's H2 (readers already issued, in order), acc2 (drained before
-        // B_H2_READY, waited) and acc3 (drained by the fp32 tail: B_TILE_DONE)
-        const bool later_tile = g != g0;
-        uint32_t sl[12], pr[12];
-        const long long t_ph0 = (kProf && prof) ? clock64() : 0;
-        // ---- layer 1, hidden part: 8 sampled layer-0 chunks x (2 K-blocks x 2 output halves = 4 stages)
-#pragma unroll 1
-        for (int c = 0; c < 8; ++c) {
-          const int b = c & 1;
-          const uint32_t p_h0 = (n_chunks >> 1) & 1u;          // the two chunk buffers alternate strictly: use (n_chunks / 2) of buffer b
-          ++n_chunks;
-          take(sl, pr, 4);
-          // [384,512) holds the previous tile's acc3 until its fp32 tail has drained it; the lower half of acc1 does not
-          // overlap it, so only the first MMA into [256,512) has to wait
-          const bool wait_td = later_tile && c == 0;
-          const uint32_t p_td = c_tiledone & 1u;
-          if (wait_td) ++c_tiledone;
-          const uint32_t acc_first = c == 0 ? 0u : 1u;
-          if (tc::elect_one()) {
-            wait_b(B_H0_READY0 + b, p_h0, P_H0READY);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int kb = q >> 1, nh = q & 1;
-              wait_b(B_WFULL + (int)sl[q], pr[q], P_WFULL);
-              if (q == 1 && wait_td) wait_b(B_TILE_DONE, p_td, P_ACC1DRAINED);
-              tc::tcgen05_fence_after();
-              kblock_ss(tbase + cAcc1 + nh * 256, dH0 + (uint64_t)(b * 2 + kb) * kKb, dW + sl[q] * kStage, idesc256,
-                        kb == 0 ? acc_first : 1u);
-              release(sl[q]);
-            }
-            commit_b(B_H0_FREE0 + b);
-          }
-        }
-        if constexpr (kProf) { if (prof && lane == 0) prof[9] += (unsigned long long)(clock64() - t_ph0); }
-        // ---- layer 1, skip part: A = X (4 K-blocks x 2 output halves)
-        {
-          const uint32_t p_x = c_xready & 1u;
-          ++c_xready;
-          take(sl, pr, 8);
-          const long long t_ph1 = (kProf && prof) ? clock64() : 0;
-          if (tc::elect_one()) {
-            wait_b(B_XREADY, p_x, P_XREADY);
-#pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const int kb = q >> 1, nh = q & 1;
-              wait_b(B_WFULL + (int)sl[q], pr[q], P_WFULL);
-              tc::tcgen05_fence_after();
-              kblock_ss(tbase + cAcc1 + nh * 256, dX + (uint64_t)kb * kKb, dW + sl[q] * kStage, idesc256, 1u);
-              release(sl[q]);
-            }
-            commit_b(B_ACC1_FULL);
-          }
-          if constexpr (kProf) { if (prof && lane == 0) prof[10] += (unsigned long long)(clock64() - t_ph1); }
-        }
-        // ---- layer 2: A = H1 from TMEM (8 K-blocks) + X (4 K-blocks) -> acc2 [128,384)
-        {
-          const uint32_t p_h1 = c_h1ready & 1u;
-          ++c_h1ready;
-          take(sl, pr, 12);
-          if (tc::elect_one()) {
-            wait_b(B_H1_READY, p_h1, P_H1READY);
-            [[maybe_unused]] long long t_ph2 = 0;
-            if constexpr (kProf) t_ph2 = prof_el ? clock64() : 0;
-#pragma unroll
-            for (int q = 0; q < 12; ++q) {
-              if constexpr (kProf) { if (prof_el && q == 4) prof_el[11] += (unsigned long long)(clock64() - t_ph2); }   // first 4 TS K-blocks
-              wait_b(B_WFULL + (int)sl[q], pr[q], P_WFULL);
-              tc::tcgen05_fence_after();
-              if (q < 8) kblock_ts(tbase + cAcc2, tbase + (q < 4 ? cH1lo + q * 32 : cH1hi + (q - 4) * 32), dW + sl[q] * kStage, idesc256,
-                                   q == 0 ? 0u : 1u);
-              else kblock_ss(tbase + cAcc2, dX + (uint64_t)(q - 8) * kKb, dW + sl[q] * kStage, idesc256, 1u);
-              release(sl[q]);
-            }
-            commit_b(B_ACC2_FULL);
-          }
-        }
-        // ---- layer 3 -> acc3 [384,512): skip part first (then X is dead), then H2 from TMEM; two K-blocks per stage
-        {
-          const uint32_t p_h2 = c_h2ready & 1u;
-          ++c_h2ready;
-          take(sl, pr, 4);
-          if (tc::elect_one()) {
-#pragma unroll
-            for (int q = 0; q < 2; ++q) {
-              wait_b(B_WFULL + (int)sl[q], pr[q], P_WFULL);
-              tc::tcgen05_fence_after();
-              kblock_ss(tbase + cAcc3, dX + (uint64_t)(2 * q) * kKb, dW + sl[q] * kStage, idesc128, q == 0 ? 0u : 1u);
-              kblock_ss(tbase + cAcc3, dX + (uint64_t)(2 * q + 1) * kKb, dW + sl[q] * kStage + kSub, idesc128, 1u);
-              release(sl[q]);
-            }
-            commit_b(B_XFREE);
-            wait_b(B_H2_READY, p_h2, P_H2READY);
-#pragma unroll
-            for (int q = 2; q < 4; ++q) {
-              wait_b(B_WFULL + (int)sl[q], pr[q], P_WFULL);
-              tc::tcgen05_fence_after();
-              kblock_ts(tbase + cAcc3, tbase + cH2 + (2 * (q - 2)) * 32, dW + sl[q] * kStage, idesc128, 1u);
-              kblock_ts(tbase + cAcc3, tbase + cH2 + (2 * (q - 2) + 1) * 32, dW + sl[q] * kStage + kSub, idesc128, 1u);
-              release(sl[q]);
-            }
-            commit_b(B_ACC3_FULL);
-          }
-        }
-      }
-      if constexpr (kProf) { if (prof && lane == 0) prof[P_TOTAL] = (unsigned long long)(clock64() - t_begin); }
-    }
-  } else if (warp == 2 || warp == 3) {
-    // ============================== samplers: X (skip operand) + per-point scalars ==============================
-    // Two warps, 64 points each, run one tile ahead of the epilogue: they only need X to be dead (B_XFREE).
-    const int sw = warp - 2;
-    const int res = prm.res;
-    uint32_t c_xfree = 0;
-    for (long long g = g0; g < n_groups; g += gstep) {
-      const long long tile = g * TP + rank;
-      const long long p0 = win0 + tile * kTile;
-      const bool tr = blockIdx.x == 0 && sw == 0 && lane == 0 && (g - g0) / gstep == kTraceTile;
-      TRACE(tr, 96);
-      if (g != g0) wait_bar(bars, B_XFREE, c_xfree);
-      TRACE(tr, 97);
-#pragma unroll 1
-      for (int grp = 0; grp < 4; ++grp) {
-        const int pbase = sw * 64 + grp * 16;
-        PointTaps pt = point_taps(src, cal, prm.H, prm.W, p0 + pbase + (lane & 15), n);
-        if (prm.exp & 4) { pt.off[0] = pt.off[1] = pt.off[2] = pt.off[3] = 0; }
-        sample_x_group16(prm, smem + Smem::X, s_zf, s_in, s_s4, pt, pbase, lane);
-      }
-      tc::fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(bars + B_ACC0_FULL0);        // scalars ready (CTA-local, release)
-      arrive_issuer(B_XREADY);
-      TRACE(tr, 98);
-    }
-  } else if (warp >= 4) {
-    // ============================== workers: layer-0 chunk generators + epilogue ==============================
-    const int wk = warp - 4;
-    const int wg = wk >> 2;
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    uint32_t c_sready = 0, c_h0free[2] = {0, 0}, c_acc1full = 0, c_acc2full = 0, c_acc3full = 0, c_part = 0;
-    const int res = prm.res;
-    if (!(warp == 4 && lane == 0)) prof = nullptr;
-    const int l16 = lane & 15;
-
-    auto act_pack = [&](float a, float b) -> uint32_t {
-      const __half2 h = __floats2half2_rn(a, b);
-      const __half2 r = __hmax2(h, __hmul2(h, __float2half2_rn(MP_LEAKY_SLOPE)));
-      return *reinterpret_cast<const uint32_t*>(&r);
-    };
-
-    // ---- projection + taps of this warp's 16 points of a tile.  A quarter-warp (8 lanes x 16 channels) covers one
-    //      point, so a lane works on four fixed points (q = 4*i + lane/8) for the whole tile and keeps their taps in
-    //      registers: texel indices packed two per register (H*W <= 65536), weights and depth feature as fp16.
-    const int l8 = lane & 7, qw = lane >> 3;
-    uint32_t t_off[4][2], t_wgt[4][2], t_z[4];
-    int gtr = -1;                              // trace slot base for the chunk being generated (-1: off)
-    auto compute_taps = [&](long long g) {
-      const PointTaps pt = point_taps(src, cal, prm.H, prm.W, win0 + (g * TP + rank) * kTile + wk * 16 + l16, n);
-      const uint32_t o01 = (uint32_t)pt.off[0] | ((uint32_t)pt.off[1] << 16), o23 = (uint32_t)pt.off[2] | ((uint32_t)pt.off[3] << 16);
-      const uint32_t w01 = tc::pack_half2(pt.wgt[0], pt.wgt[1]), w23 = tc::pack_half2(pt.wgt[2], pt.wgt[3]);
-      const uint32_t zz = tc::pack_half2(pt.zf, pt.zf);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int q = 4 * i + qw;
-        t_off[i][0] = __shfl_sync(0xffffffffu, o01, q);
-        t_off[i][1] = __shfl_sync(0xffffffffu, o23, q);
-        t_wgt[i][0] = __shfl_sync(0xffffffffu, w01, q);
-        t_wgt[i][1] = __shfl_sync(0xffffffffu, w23, q);
-        t_z[i] = __shfl_sync(0xffffffffu, zz, q);
-      }
-    };
-    {
-      // ---- one sampled layer-0 chunk: h0[:, c*128 .. +128) = lrelu(lerp(G0) + b0 + w0z z) -> H0 smem buffer c&1.
-      //      The interpolation runs on packed fp16 FMAs (HFMA2: the taps are fp16 already, so no conversions): a
-      //      lane loads 2 x 16 B per tap (channels 8*l8.. of both 64-channel K-blocks) and issues 8 HFMA2 per tap.
-      //      tools/precision_emulate.py: the extra fp16 roundings do not move the output error (2.76e-5 vs 2.75e-5).
-      auto gen_chunk = [&](int c) {
-        const int b = c & 1;
-        TRACE(gtr >= 0, gtr + 0);
-        { PROF_T0(); wait_free(bars, B_H0_FREE0 + b, c_h0free[b]); PROF_ADD(P_W_H0FREE); }
-        TRACE(gtr >= 0, gtr + 1);
-        PROF_T0();
-        const int ch = c * 128 + l8 * 8;
-        __half2 b8[8], z8[8];
-        {
-          const uint4 bA = __ldg(reinterpret_cast<const uint4*>(prm.d_bias0 + ch)), bB = __ldg(reinterpret_cast<const uint4*>(prm.d_bias0 + ch + 64));
-          const uint4 zA = __ldg(reinterpret_cast<const uint4*>(prm.d_wz0 + ch)), zB = __ldg(reinterpret_cast<const uint4*>(prm.d_wz0 + ch + 64));
-          *reinterpret_cast<uint4*>(&b8[0]) = bA; *reinterpret_cast<uint4*>(&b8[4]) = bB;
-          *reinterpret_cast<uint4*>(&z8[0]) = zA; *reinterpret_cast<uint4*>(&z8[4]) = zB;
-        }
-        uint8_t* dstp = smem + Smem::H0 + b * 32768;
-        const __half2 slope2 = __float2half2_rn(MP_LEAKY_SLOPE);
-#pragma unroll
-        for (int batch = 0; batch < 2; ++batch) {      // (unrolled: the tap registers are indexed statically)
-          uint4 raw[2][4][2];                  // [point][tap][K-block]
-#pragma unroll
-          for (int ps = 0; ps < 2; ++ps) {
-            const int i = batch * 2 + ps;
-#pragma unroll
-            for (int a = 0; a < 4; ++a) {
-              uint32_t off = (a & 1) ? (t_off[i][a >> 1] >> 16) : (t_off[i][a >> 1] & 0xFFFFu);
-              if (prm.exp & 2) off = 0;
-              const uint4* srcp = reinterpret_cast<const uint4*>(prm.g0 + (size_t)off * kL0 + ch);
-              raw[ps][a][0] = __ldg(srcp);
-              raw[ps][a][1] = __ldg(srcp + 8);      // + 64 channels
-            }
-          }
-          TRACE(gtr >= 0, gtr + 2 + 2 * batch);
-#pragma unroll
-          for (int ps = 0; ps < 2; ++ps) {
-            const int i = batch * 2 + ps;
-            const int p = wk * 16 + 4 * i + qw;
-            const __half2 zq2 = *reinterpret_cast<const __half2*>(&t_z[i]);
-            __half2 acc[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) acc[j] = __hfma2(z8[j], zq2, b8[j]);
-#pragma unroll
-            for (int a = 0; a < 4; ++a) {          // same tap order as grid_sample: nw, ne, sw, se
-              const __half2 wp = *reinterpret_cast<const __half2*>(&t_wgt[i][a >> 1]);
-              const __half2 w2 = (a & 1) ? __high2half2(wp) : __low2half2(wp);
-              const __half2* h0 = reinterpret_cast<const __half2*>(&raw[ps][a][0]);
-              const __half2* h1 = reinterpret_cast<const __half2*>(&raw[ps][a][1]);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                acc[j] = __hfma2(h0[j], w2, acc[j]);
-                acc[4 + j] = __hfma2(h1[j], w2, acc[4 + j]);
-              }
-            }
-            uint32_t o[8];
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const __half2 r = __hmax2(acc[j], __hmul2(acc[j], slope2));
-              o[j] = *reinterpret_cast<const uint32_t*>(&r);
-            }
-            *reinterpret_cast<uint4*>(dstp + tc::sw128_offset(p, l8 * 8)) = make_uint4(o[0], o[1], o[2], o[3]);
-            *reinterpret_cast<uint4*>(dstp + 16384 + tc::sw128_offset(p, l8 * 8)) = make_uint4(o[4], o[5], o[6], o[7]);
-          }
-          TRACE(gtr >= 0, gtr + 3 + 2 * batch);
-        }
-        tc::fence_proxy_async_smem();
-        arrive_issuer(B_H0_READY0 + b);
-        TRACE(gtr >= 0, gtr + 6);
-        PROF_ADD(P_W_DRAIN0);
-      };
-      // The worker loop is software-pipelined across tiles: the first two sampled layer-0 chunks of the NEXT tile are
-      // generated while this tile's layer-2 / layer-3 MMAs run (the workers would idle there), so the next tile's
-      // layer 1 can start the moment the tensor pipe is free.  A virtual first iteration (g = g0 - gstep) only performs
-      // that pre-generation.  Every routine has a single call site to keep the instruction footprint small.
-      float zf = 0.f, inimg = 0.f;
-      float s4[kMaxRes];
-#pragma unroll
-      for (int r = 0; r < kMaxRes; ++r) s4[r] = 0.f;
-      auto load_pre = [&](uint32_t col, int ch0, float (&o)[32]) {
-        uint32_t v[32];
-        tc::tmem_ld32(tbase + lane_base + col, v);
-        tc::tmem_ld_wait();
-        // 128-bit constant-bank loads (ch0 is a multiple of 32): 16 LDC.128 instead of 64 scalar constant loads
-        const float4* bz = reinterpret_cast<const float4*>(&prm.bias_all[ch0]);
-        const float4* wz = reinterpret_cast<const float4*>(&prm.wz_all[ch0]);
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-          const float4 b = bz[j4], z = wz[j4];
-          o[4 * j4 + 0] = __uint_as_float(v[4 * j4 + 0]) + fmaf(z.x, zf, b.x);
-          o[4 * j4 + 1] = __uint_as_float(v[4 * j4 + 1]) + fmaf(z.y, zf, b.y);
-          o[4 * j4 + 2] = __uint_as_float(v[4 * j4 + 2]) + fmaf(z.z, zf, b.z);
-          o[4 * j4 + 3] = __uint_as_float(v[4 * j4 + 3]) + fmaf(z.w, zf, b.w);
-        }
-      };
-      for (long long g = g0 - gstep; g < n_groups; g += gstep) {
-        const bool real = g >= g0;
-        const bool has_next = g + gstep < n_groups;
-        const long long p0 = win0 + (g * TP + rank) * kTile;
-        const bool tr = blockIdx.x == 0 && real && (wk & 3) == 0 && lane == 0 && (g - g0) / gstep == kTraceTile;
-        const int tb = 32 + wg * 32;
-#pragma unroll 1
-        for (int step = 0; step < 11; ++step) {
-          TRACE(tr, tb + step);
-          int gc = -1;
-          if (step < 6) { if (real) gc = step + 2; }
-          else if (step == 7) { if (has_next) { compute_taps(g + gstep); gc = 0; } }
-          else if (step == 10) { if (has_next) gc = 1; }    // after the fp32 tail: B_TILE_DONE gates the next tile
-          gtr = (tr && step == 2) ? tb + 18 : -1;       // trace the inside of one chunk (chunk 4)
-          if (gc >= 0) gen_chunk(gc);
-          if (!real) continue;
-          if (step == 6) {
-          { PROF_T0(); wait_bar(bars, B_ACC0_FULL0, c_sready); PROF_ADD(P_W_XFREE); }
-          zf = s_zf[row];
-          inimg = s_in[row];
-#pragma unroll
-          for (int r = 0; r < kMaxRes; ++r) s4[r] = (r < res) ? s_s4[r * kTile + row] : 0.f;
-      // ---- layer 1 (512 columns) -> H1, drained IN PLACE: warpgroup 0 walks [0,256) upwards into [0,128), warpgroup 1
-      //      walks [256,512) downwards into [384,512); the packed destination of a group never reaches columns that are
-      //      still unread, and [128,384) comes out free for acc2.
-      { PROF_T0(); wait_bar(bars, B_ACC1_FULL, c_acc1full); PROF_ADD(P_W_ACC1FULL); }
-      TRACE(tr, tb + 11);
-      tc::tcgen05_fence_after();
-      {
-        PROF_T0();
-#pragma unroll 1
-        for (int gi = 0; gi < 8; ++gi) {
-          const int gq = (wg == 0) ? gi : 7 - gi;
-          const int lc = wg * 256 + gq * 32;                 // accumulator column == layer-1 output channel
-          float o[32];
-          load_pre(cAcc1 + lc, side_off(1) + lc, o);
-          uint32_t pk[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) pk[j] = act_pack(o[2 * j], o[2 * j + 1]);
-          const uint32_t dcol = (wg == 0) ? (cH1lo + lc / 2) : (cH1hi + (lc - 256) / 2);
-          tc::tmem_st16(tbase + lane_base + dcol, pk);
-          tc::tmem_st_wait();
-        }
-        tc::tcgen05_fence_before();
-        arrive_issuer(B_H1_READY);
-        PROF_ADD(P_W_DRAIN1);
-        TRACE(tr, tb + 12);
-      }
-          } else if (step == 8) {
-      // ---- layer 2 -> H2 [0,128)
-      { PROF_T0(); wait_bar(bars, B_ACC2_FULL, c_acc2full); PROF_ADD(P_W_ACC2FULL); }
-      TRACE(tr, tb + 13);
-      tc::tcgen05_fence_after();
-      {
-        PROF_T0();
-#pragma unroll 1
-        for (int gq = 0; gq < 4; ++gq) {
-          float o[32];
-          const int lc = wg * 128 + gq * 32;
-          load_pre(cAcc2 + lc, side_off(2) + lc, o);
-          uint32_t pk[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) pk[j] = act_pack(o[2 * j], o[2 * j + 1]);
-          tc::tmem_st16(tbase + lane_base + cH2 + lc / 2, pk);
-        }
-        tc::tmem_st_wait();
-        tc::tcgen05_fence_before();
-        arrive_issuer(B_H2_READY);
-        PROF_ADD(P_W_DRAIN2);
-        TRACE(tr, tb + 14);
-      }
-          } else if (step == 9) {
-      // ---- layer 3 + layer 4 in fp32.  Each warpgroup takes HALF of acc3's 128 columns (its warp of a quarter owns the same 32
-      //      rows in both groups): the tail is on the issuer's critical path -- [384,512) is the next tile's layer-1 accumulator,
-      //      B_TILE_DONE -- and with one warpgroup it took 4.8 k cycles per tile.  TMEM is released as soon as a warp's last
-      //      column group is in registers; warpgroup 1 passes its partial dot product through the (idle) second chunk buffer.
-      {
-        { PROF_T0(); wait_bar(bars, B_ACC3_FULL, c_acc3full); PROF_ADD(P_W_ACC3FULL); }
-        TRACE(tr, tb + 15);
-        tc::tcgen05_fence_after();
-        PROF_T0();
-        float logit[kMaxRes];
-#pragma unroll
-        for (int r = 0; r < kMaxRes; ++r) logit[r] = wg == 0 ? s4[r] : 0.f;
-#pragma unroll 1
-        for (int h = 0; h < 2; ++h) {
-          const int gq = 2 * wg + h;
-          float o[32];
-          load_pre(cAcc3 + gq * 32, side_off(3) + gq * 32, o);
-          if (h == 1) {                               // this warp has read all it needs of acc3
-            tc::tcgen05_fence_before();
-            arrive_issuer(B_TILE_DONE);
-          }
-#pragma unroll
-          for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], o[j] * MP_LEAKY_SLOPE);
-#pragma unroll
-          for (int r = 0; r < kMaxRes; ++r) {
-            if (r < res) {
-              const float4* wv = reinterpret_cast<const float4*>(prm.w4h + r * kL3 + gq * 32);
-#pragma unroll
-              for (int j4 = 0; j4 < 8; ++j4) {
-                const float4 w4 = __ldg(wv + j4);
-                logit[r] = fmaf(w4.x, o[4 * j4 + 0], logit[r]);
-                logit[r] = fmaf(w4.y, o[4 * j4 + 1], logit[r]);
-                logit[r] = fmaf(w4.z, o[4 * j4 + 2], logit[r]);
-                logit[r] = fmaf(w4.w, o[4 * j4 + 3], logit[r]);
-              }
-            }
-          }
-        }
-        // the second chunk buffer is idle here (its last reader was this tile's layer 1; the next tile's chunk 1 is generated
-        // at step 10): rows [16 q, 16 q + 16) of it are what warpgroup 0's warp of quarter q overwrites next, and nobody else
-        // (hand-off: a CTA-local mbarrier, one arrival per warp of warpgroup 1)
-        float* s_part = reinterpret_cast<float*>(smem + Smem::H0 + 32768 + quarter * 16 * 128);
-        if (wg == 1) {
-#pragma unroll
-          for (int r = 0; r < kMaxRes; ++r) s_part[r * 32 + lane] = logit[r];
-        }
-        if (wg == 1) {
-          warp_arrive_local(bars + B_PART_READY, lane);
-        } else {
-          wait_bar(bars, B_PART_READY, c_part);
-#pragma unroll
-          for (int r = 0; r < kMaxRes; ++r) logit[r] += s_part[r * 32 + lane];
-          __syncwarp();        // every lane has its partial before any lane of this warp overwrites these rows (chunk 1, step 10)
-        }
-        PROF_ADD(P_W_DRAIN3);
-        TRACE(tr, tb + 16);
-        if (wg == 0) {
-        const long long i = p0 + row;
-        if (i < n) {
-#pragma unroll
-          for (int r = 0; r < kMaxRes; ++r) {
-            if (r < res) {
-              const float val = inimg * mp_last_op(logit[r], prm.last_op);
-              if (dst.out) dst.out[(long long)r * dst.ld + i] = val;
-              if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = val;
-              if constexpr (PEERS) {
-                if (r == 0) {
-#pragma unroll
-                  for (int p = 0; p < MP_MAX_PEERS; ++p)
-                    if (p < dst.n_peers) dst.peer[p][dst.peer_off + i] = val;      // 128 B per warp and peer over NVLink
-                }
-              }
-            }
-          }
-        }
-        }
-      }
-          }
-        }
-      }
-    }
-  }
-  __syncwarp();
-  tc::tcgen05_fence_before();
-  if constexpr (CG == 1) {
-    if constexpr (WM) tc::cluster_sync_all();      // (the peer's last stage releases arrive on this CTA's barriers)
-    else __syncthreads();
-    if (warp == 2) tc::tmem_dealloc(tbase, 512);
-  } else {
-    tc::cluster_sync_all();
-    if (warp == 2) tc::tmem_dealloc2(tbase, 512);
-  }
-}
-
-// G0[texel][n] = sum_k F[texel][k] * W0f[n][k] on the tensor cores: fp16 operands (F rounded once while staging, W0f
-// pre-packed on the host as SWIZZLE_128B tiles [n tile][K block][256 x 64]) and fp32 accumulation in TMEM.
-// One CTA = 128 texels x all 1024 outputs: the A operand (128 x 256) is staged ONCE by warps 0-7 (fp32 global -> fp16
-// swizzled smem, the latency-bound part), the 16 B tiles stream through a 4-stage bulk-copy ring (warp 8), warp 9 issues
-// the MMAs of the four 256-wide output tiles into two alternating TMEM accumulators, and warps 0-7 drain tile nt
-// (tcgen05.ld -> fp16 -> G rows) while tile nt+1 is being multiplied.  The staging pass also publishes what it has in
-// hand: the fp16 copy of the map (F16, taps of the X operand) and S4 = W4s . F per texel in fp32 (the last layer's
-// direct access to the features: sampling S4 in fp32 keeps that path out of the fp16 roundings -- bilinear sampling
-// commutes with the dot product).  4.3 GFLOP per frame, one wave of 128 CTAs.
-constexpr int kG0Threads = 320;
-constexpr int kG0TileN = 256;
-constexpr int kG0NT = kL0 / kG0TileN;                 // 4 output tiles
-constexpr int kG0Stages = 4;
-constexpr uint32_t kG0SmemA = 4 * 16384, kG0SmemB = kG0Stages * 32768;
-constexpr uint32_t kG0Smem = kG0SmemA + kG0SmemB + 1024 /*align*/ + 128 /*barriers + tmem slot*/;
-
-__global__ void __launch_bounds__(kG0Threads, 1)
-g0_tc_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half* __restrict__ G, int M,
-             __half* __restrict__ F16, float* __restrict__ S4, const float* __restrict__ w4s, int res, unsigned* __restrict__ amax) {
-  MP_DYN_SMEM(uint8_t, g0_smem_raw);
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(g0_smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint8_t* sA = base;
-  uint8_t* sB = base + kG0SmemA;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + kG0SmemA + kG0SmemB);
-  uint64_t* b_full = bars;                   // [4] B stage landed
-  uint64_t* b_empty = bars + 4;              // [4] B stage consumed (tcgen05.commit)
-  uint64_t* acc_full = bars + 8;             // [2] accumulator complete
-  uint64_t* acc_free = bars + 10;            // [2] accumulator drained by the 8 epilogue warps
-  uint64_t* a_ready = bars + 12;             // A staged (8 warps)
-  uint32_t* tslot = reinterpret_cast<uint32_t*>(bars + 13);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int m0 = blockIdx.x * 128;
-  if (tid == 0) {
-    for (int i = 0; i < 4; ++i) { tc::mbar_init(&b_full[i], 1); tc::mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&acc_full[i], 1); tc::mbar_init(&acc_free[i], 8); }
-    tc::mbar_init(a_ready, 8);
-    tc::fence_barrier_init();
-  }
-  if (warp == 8) {
-    tc::tmem_alloc(tslot, 512);
-    tc::tmem_relinquish();
-  }
-  tc::tcgen05_fence_before();
-  __syncthreads();
-  tc::tcgen05_fence_after();
-  const uint32_t tbase = *tslot;
-  constexpr uint32_t idesc = tc::make_idesc_f16(128, kG0TileN);
-
-  if (warp == 8) {
-    // ---- B producer: 16 tiles in (nt, kb) order through the ring
-    if (lane == 0) {
-      for (int s = 0; s < kG0NT * 4; ++s) {
-        const int slot = s % kG0Stages;
-        if (s >= kG0Stages) tc::mbar_wait(&b_empty[slot], ((s / kG0Stages) & 1) ^ 1);
-        tc::mbar_arrive_expect_tx(&b_full[slot], 32768);
-        tc::bulk_g2s(sB + slot * 32768, Wt + (size_t)s * 32768, 32768, &b_full[slot]);
-      }
-    }
-  } else if (warp == 9) {
-    // ---- MMA issuer: the whole warp runs the (uniform) control flow, one elected lane executes ONE region per output tile --
-    //      waits, fences, MMAs, commits (see the issuer of query_tc3_kernel)
-    {
-      const uint64_t dA = tc::make_sdesc_sw128(tc::smem_u32(sA), 1024), dB = tc::make_sdesc_sw128(tc::smem_u32(sB), 1024);
-#pragma unroll 1
-      for (int nt = 0; nt < kG0NT; ++nt) {
-        const int buf = nt & 1;
-        if (tc::elect_one()) {
-          if (nt == 0) tc::mbar_wait(a_ready, 0);
-          if (nt >= 2) tc::mbar_wait(&acc_free[buf], ((nt >> 1) & 1) ^ 1);
-#pragma unroll
-          for (int kb = 0; kb < 4; ++kb) {
-            const int s = nt * 4 + kb, slot = s % kG0Stages;
-            tc::mbar_wait(&b_full[slot], (s / kG0Stages) & 1);
-            tc::tcgen05_fence_after();
-#pragma unroll
-            for (int k16 = 0; k16 < 4; ++k16)
-              tc::mma_ss(tbase + buf * kG0TileN, dA + (uint64_t)kb * (16384 >> 4) + 2 * k16, dB + (uint64_t)slot * (32768 >> 4) + 2 * k16, idesc,
-                         (kb | k16) ? 1u : 0u);
-            tc::mma_commit(&b_empty[slot]);
-          }
-          tc::mma_commit(&acc_full[buf]);
-        }
-      }
-    }
-  } else {
-    // ---- warps 0-7: stage A (thread -> row = tid / 2, 32-column half of each 64-wide K-block), then drain
-    const int row = tid >> 1, half = tid & 1;
-    const bool live = (m0 + row) < M;
-    const float* frow = F + (size_t)(live ? m0 + row : 0) * kC + half * 32;
-    float s4acc[kMaxRes];
-    float fmax_abs = 0.f;             // range guard: the largest |feature| this thread stages
-#pragma unroll
-    for (int r = 0; r < kMaxRes; ++r) s4acc[r] = 0.f;
-#pragma unroll 1
-    for (int kb = 0; kb < 4; ++kb) {
-      float4 v[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) v[j] = live ? __ldg(reinterpret_cast<const float4*>(frow + kb * 64) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) fmax_abs = fmaxf(fmax_abs, fmaxf(fmaxf(fabsf(v[j].x), fabsf(v[j].y)), fmaxf(fabsf(v[j].z), fabsf(v[j].w))));
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint4 pk;
-        pk.x = tc::pack_half2(v[2 * j].x, v[2 * j].y);
-        pk.y = tc::pack_half2(v[2 * j].z, v[2 * j].w);
-        pk.z = tc::pack_half2(v[2 * j + 1].x, v[2 * j + 1].y);
-        pk.w = tc::pack_half2(v[2 * j + 1].z, v[2 * j + 1].w);
-        *reinterpret_cast<uint4*>(sA + kb * 16384 + tc::sw128_offset(row, half * 32 + j * 8)) = pk;
-        if (live) *reinterpret_cast<uint4*>(F16 + (size_t)(m0 + row) * kC + kb * 64 + half * 32 + j * 8) = pk;
-      }
-#pragma unroll
-      for (int r = 0; r < kMaxRes; ++r)
-        if (r < res) {
-          const float4* wv = reinterpret_cast<const float4*>(w4s + r * kC + kb * 64 + half * 32);
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 w = __ldg(wv + j);
-            s4acc[r] = fmaf(w.x, v[j].x, s4acc[r]); s4acc[r] = fmaf(w.y, v[j].y, s4acc[r]);
-            s4acc[r] = fmaf(w.z, v[j].z, s4acc[r]); s4acc[r] = fmaf(w.w, v[j].w, s4acc[r]);
-          }
-        }
-    }
-    tc::fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) tc::mbar_arrive(a_ready);
-    if (amax) {
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) fmax_abs = fmaxf(fmax_abs, __shfl_xor_sync(0xffffffffu, fmax_abs, o));
-      if (lane == 0) atomicMax(amax, __float_as_uint(fmax_abs));       // non-negative floats order like their bit patterns
-    }
-#pragma unroll
-    for (int r = 0; r < kMaxRes; ++r) {
-      const float tot = s4acc[r] + __shfl_xor_sync(0xffffffffu, s4acc[r], 1);
-      if (live && half == 0 && r < res) S4[(size_t)(m0 + row) * kMaxRes + r] = tot;
-    }
-    // epilogue: warp w reads lanes 32*(w%4).. (its TMEM sub-partition), columns 128*(w/4)..+127 of the 256-wide tile
-    const int sub = warp & 3, ch = warp >> 2;
-    const int m = m0 + sub * 32 + lane;
-#pragma unroll 1
-    for (int nt = 0; nt < kG0NT; ++nt) {
-      const int buf = nt & 1;
-      tc::mbar_wait(&acc_full[buf], (nt >> 1) & 1);
-      __syncwarp();
-      tc::tcgen05_fence_after();
-      __half* grow = G + (size_t)(m < M ? m : 0) * kL0 + nt * kG0TileN + ch * 128;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tc::tmem_ld32(tbase + ((uint32_t)(sub * 32) << 16) + buf * kG0TileN + ch * 128 + c * 32, r);
-        tc::tmem_ld_wait();
-        if (m < M) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 pk;
-            pk.x = tc::pack_half2(__uint_as_float(r[8 * q + 0]), __uint_as_float(r[8 * q + 1]));
-            pk.y = tc::pack_half2(__uint_as_float(r[8 * q + 2]), __uint_as_float(r[8 * q + 3]));
-            pk.z = tc::pack_half2(__uint_as_float(r[8 * q + 4]), __uint_as_float(r[8 * q + 5]));
-            pk.w = tc::pack_half2(__uint_as_float(r[8 * q + 6]), __uint_as_float(r[8 * q + 7]));
-            *reinterpret_cast<uint4*>(grow + c * 32 + q * 8) = pk;
-          }
-        }
-      }
-      tc::tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_free[buf]);
-    }
-  }
-  tc::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 8) tc::tmem_dealloc(tbase, 512);
-}
-
-// ====================================================================================================================
-// Colour head: PIFuNetCMLP (filter_channels [513,1024,512,256,128,3], Tanh, heads/SurfaceClassifier.py:82-87) on the
-// 512-channel map of MonoPortNet.filter(feat_prior=...) (MonoPortNet.py:41-45), queried at the visible vertices
-// (RTL/main.py:212-249).  EXPERIMENTAL (opt-in, MONOPORT_B200_TC_NETC=1) until validated on a B200; checked on the CPU model
-// of the tcgen05 layer (tests/emu).  Same structure as program v3 (layer 0 hoisted to texels, layer 1 on all 512 TMEM
-// columns, in-place drains, A operands from TMEM) with two differences:
-//   * the skip operand X has 512 channels = 128 KB, which does not fit next to the H0 ring and the weight ring.  X keeps
-//     its 64 KB buffer and is filled in PHASES of 256 channels (A = 0..255, B = 256..511); the skip parts of the layers
-//     are issued in the order  L1:A,B  L2:B,A  L3:A,B  so that four fills per tile suffice.  The tensor pipe waits for
-//     the samplers at three of them -- acceptable for a query of 10^4..10^5 points (the dense path is the geometry head);
-//   * the per-point scalars (depth feature, in-image flag, the fp32 last-layer feature part S4[3]) are computed by the
-//     epilogue thread that owns the point instead of being passed through shared memory (no room, and no barrier);
-//   * layer 3 multiplies by W3 as an fp16 PAIR (hi + lo, two MMAs per K-step on the same A operand): the Tanh output is four
-//     times as sensitive to the logit as the geometry head's Sigmoid, and tools/precision_budget.py shows the rounding of
-//     W3 to be the largest single term of the error (1.0e-4 -> 5.6e-5 on what query() returns; +6 % MMAs of this program).
-constexpr int kCc = 512;                                   // feature channels of the colour map
-constexpr int kResC = 3;
-constexpr int kStagesPerTileC = 32 + 16 + 8 + 8 + 8 + 4;   // L1 hidden, L1 skip (A,B), L2 hidden, L2 skip (B,A), L3 skip (A,B) x (hi,lo), L3 hidden x (hi,lo)
-
-// Direct rendering of the visible surface (RTL/main.py:212-249) fused into the colour query: point i is the vertex
-// (X[i], Y[i], R - Z[i]) of forward_vertices mapped to world space by mat_color (RTL/main.py:201-210: diag((b_max-b_min)/R),
-// translation b_min), and its colour pred * 0.5 + 0.5 (:244) is scattered to canvas[X[i], Y[i], :] (:247-248) -- no
-// intermediate point / prediction tensors.  X == nullptr: the ordinary point sources and the [3,N] output.
-struct MpSurfaceSrc {
-  const long long* X;
-  const long long* Y;
-  const float* Z;
-  float scale[3], bmin[3];      // (b_max - b_min) / R and b_min, fp32 like torch's
-  float R;
-  float* canvas;                // [R, R, 3]
-  int canvas_R;
-};
-
-__device__ __forceinline__ PointTaps colour_taps(const MpSurfaceSrc& surf, const MpPointSrc& src, const MpCalib& cal, int H, int W,
-                                                 long long i, long long n) {
-  if (!surf.X) return point_taps(src, cal, H, W, i, n);
-  PointTaps pt;
-  float u = 0.f, v = 0.f, w = 0.f;
-  const bool valid = i < n;
-  if (valid) {
-    const float vx = (float)__ldg(surf.X + i), vy = (float)__ldg(surf.Y + i), vz = __fsub_rn(surf.R, __ldg(surf.Z + i));
-    const float x = __fadd_rn(__fmul_rn(vx, surf.scale[0]), surf.bmin[0]);
-    const float y = __fadd_rn(__fmul_rn(vy, surf.scale[1]), surf.bmin[1]);
-    const float z = __fadd_rn(__fmul_rn(vz, surf.scale[2]), surf.bmin[2]);
-    mp_project(cal, x, y, z, u, v, w);
-  }
-  pt.in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);
-  const MpTaps t = mp_taps(valid ? u : 0.f, valid ? v : 0.f, H, W);
-  const bool dead = !valid || !(u == u) || !(v == v);
-#pragma unroll
-  for (int a = 0; a < 4; ++a) { pt.off[a] = dead ? 0 : t.off[a]; pt.wgt[a] = dead ? 0.f : t.wgt[a]; }
-  pt.zf = w * cal.z_scale;
-  return pt;
-}
-
-// 16 points of one phase (256 channels starting at phase*256) of the fp16 map -> rows [pbase, pbase+16) of X
-__device__ __forceinline__ void sample_x_phase(const TcParams& prm, uint8_t* smem_x, const PointTaps& pt, int pbase, int lane, int phase) {
+// Whole warp: the 16 points whose taps sit in lanes 0..15 (duplicated in lanes 16..31), channels [phase*256, +256) of the
+// fp16 copy of the map, into rows [pbase, pbase+16) of the fp16 X tile (K-major SWIZZLE_128B; a lane covers 8 channels).
+// The last layer's direct feature access is NOT derived from these samples but from S4 (fp32, per texel), which the lane
+// owning the point interpolates in fp32 (phase 0).
+template <int C>
+__device__ __forceinline__ void sample_x16(const TcParams& prm, uint8_t* smem_x, float* s_zf, float* s_in, float* s_s4,
+                                           const PointTaps& pt, int pbase, int lane, int phase) {
+  constexpr int RES = Prog<C>::RES;
   const int cbase = phase * 256 + lane * 8;
 #pragma unroll 1
   for (int q0 = 0; q0 < 16; q0 += 4) {
@@ -1115,7 +171,7 @@ __device__ __forceinline__ void sample_x_phase(const TcParams& prm, uint8_t* sme
       for (int a = 0; a < 4; ++a) {
         const int off = __shfl_sync(0xffffffffu, pt.off[a], q0 + qq);
         wgt[qq][a] = __shfl_sync(0xffffffffu, pt.wgt[a], q0 + qq);
-        raw[qq][a] = __ldg(reinterpret_cast<const uint4*>(prm.feat16 + (size_t)off * kCc + cbase));
+        raw[qq][a] = __ldg(reinterpret_cast<const uint4*>(prm.feat16 + (size_t)off * C + cbase));
       }
 #pragma unroll
     for (int qq = 0; qq < 4; ++qq) {
@@ -1126,277 +182,197 @@ __device__ __forceinline__ void sample_x_phase(const TcParams& prm, uint8_t* sme
         const float2 w2 = make_float2(wgt[qq][a], wgt[qq][a]);
         const __half2* h2 = reinterpret_cast<const __half2*>(&raw[qq][a]);
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc[j] = (a == 0) ? __fmul2_rn(__half22float2(h2[j]), w2) : __ffma2_rn(__half22float2(h2[j]), w2, acc[j]);
+        for (int j = 0; j < 4; ++j) {
+          const float2 f = __half22float2(h2[j]);
+          acc[j] = (a == 0) ? make_float2(__fmul_rn(f.x, w2.x), __fmul_rn(f.y, w2.y)) : make_float2(fmaf(f.x, w2.x, acc[j].x), fmaf(f.y, w2.y, acc[j].y));
+        }
       }
       uint4 packed;
       packed.x = tc::pack_half2(acc[0].x, acc[0].y);
       packed.y = tc::pack_half2(acc[1].x, acc[1].y);
       packed.z = tc::pack_half2(acc[2].x, acc[2].y);
       packed.w = tc::pack_half2(acc[3].x, acc[3].y);
-      *reinterpret_cast<uint4*>(smem_x + (lane >> 3) * 16384 + tc::sw128_offset(p, (lane & 7) * 8)) = packed;
+      *reinterpret_cast<uint4*>(smem_x + (phase * 4 + (lane >> 3)) * kKb + tc::sw128_offset(p, (lane & 7) * 8)) = packed;
     }
+  }
+  if (phase == 0 && lane < 16) {
+#pragma unroll
+    for (int r = 0; r < RES; ++r) {
+      float s = 0.f;
+#pragma unroll
+      for (int a = 0; a < 4; ++a) s = fmaf(pt.wgt[a], __ldg(prm.s4tex + (size_t)pt.off[a] * RES + r), s);
+      s_s4[r * kTile + pbase + lane] = s + __ldg(prm.w4z + r) * pt.zf + __ldg(prm.b4 + r);
+    }
+    s_zf[pbase + lane] = pt.zf;
+    s_in[pbase + lane] = pt.in_img ? 1.f : 0.f;
   }
 }
 
+__device__ __forceinline__ uint32_t act_pack(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  const __half2 r = __hmax2(h, __hmul2(h, __float2half2_rn(MP_LEAKY_SLOPE)));
+  return *reinterpret_cast<const uint32_t*>(&r);
+}
+
+// ====================================================================================================================
+// The fused query program.  Register fragment of a 64 x N accumulator (wgmma m64nNk16, f32): thread t of the warpgroup
+// (warp wl = t/32, lane l) holds d[4j + e] = D[16 wl + l/4 + 8 (e>>1)][8 j + 2 (l%4) + (e&1)].
+// Hand-offs: every consumer takes EVERY stage of the stream (waits for it), uses the ones that carry its rows and
+// releases a stage once the MMAs that read it have completed (one arrival per consumer warp); the operand buffers written
+// by the consumers themselves are published with fence.proxy.async + a named barrier over the 256 consumer threads.
+// PEERS: also store channel 0 into the peer volumes of dst (fused slab exchange).
+template <int C, bool PEERS>
 __global__ void __launch_bounds__(kThreads, 1)
-query_tc3c_kernel(TcParams prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpSurfaceSrc surf) {
-  using C = Cfg;
+query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpSurfaceSrc surf) {
+  using P = Prog<C>;
+  constexpr int RES = P::RES, Ring = P::Ring, XKB = P::XKB;
   MP_DYN_SMEM(uint8_t, smem_raw);
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Smem::Bars);
-  uint32_t* s_tmem = reinterpret_cast<uint32_t*>(smem + Smem::TmemPtr);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::Bars);
+  uint64_t* empty = full + Ring;
+  float* s_zf = reinterpret_cast<float*>(smem + P::Small);
+  float* s_in = s_zf + kTile;
+  float* s_s4 = s_in + kTile;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid: nothing is allocated yet)
+  if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid)
+
   long long n = src.n;
   if (src.count_dev) {
     const long long c = *src.count_dev;
     n = c < n ? c : n;
   }
-  const long long n_tiles = (n + kTile - 1) / kTile;
-  const long long g0 = blockIdx.x, gstep = gridDim.x;
-
-  constexpr uint32_t cAcc1 = 0, cH1lo = 0, cH1hi = 384, cAcc2 = 128, cH2 = 0, cAcc3 = 384;
+  long long win0, win1;
+  mp_shard_window(src, n, win0, win1);
+  n = win1;                                          // points >= n are padding; tile 0 starts at point win0
+  const long long n_tiles = (win1 - win0 + kTile - 1) / kTile;
 
   if (tid == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      tc::mbar_init(bars + B_WFULL + s, 1);
-      tc::mbar_init(bars + B_WEMPTY + s, 1);
+    for (int s = 0; s < Ring; ++s) {
+      tc::mbar_init(full + s, 1);
+      tc::mbar_init(empty + s, kConsumers / 32);
     }
-    constexpr int kW = 8;
-    tc::mbar_init(bars + B_XREADY, 2);             // the two sampler warps, once per phase fill
-    tc::mbar_init(bars + B_XFREE, 1);              // tcgen05.commit after the last MMA reading a fill
-    tc::mbar_init(bars + B_H0_READY0, kW);
-    tc::mbar_init(bars + B_H0_READY1, kW);
-    tc::mbar_init(bars + B_H0_FREE0, 1);
-    tc::mbar_init(bars + B_H0_FREE1, 1);
-    tc::mbar_init(bars + B_ACC1_FULL, 1);
-    tc::mbar_init(bars + B_H1_READY, kW);
-    tc::mbar_init(bars + B_ACC2_FULL, 1);
-    tc::mbar_init(bars + B_H2_READY, kW);
-    tc::mbar_init(bars + B_ACC3_FULL, 1);
-    tc::mbar_init(bars + B_TILE_DONE, 4);
     tc::fence_barrier_init();
   }
-  if (warp == 2) { tc::tmem_alloc(s_tmem, 512); tc::tmem_relinquish(); }
-  tc::tcgen05_fence_before();
   __syncthreads();
-  tc::tcgen05_fence_after();
-  const uint32_t tbase = *s_tmem;
 
-  if (warp == 0) {
+  if (warp == kConsumers / 32) {
     // ============================== weight producer ==============================
     if (lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
       uint32_t it = 0;
-      for (long long g = g0; g < n_tiles; g += gstep) {
-        for (int s = 0; s < kStagesPerTileC; ++s, ++it) {
-          const int slot = it % C::Stages;
-          const uint32_t use = it / C::Stages;
-          tc::mbar_wait(bars + B_WEMPTY + slot, (use & 1u) ^ 1u);
-          tc::mbar_arrive_expect_tx(bars + B_WFULL + slot, C::StageBytes);
-          tc::bulk_g2s(smem + Smem::Wr + slot * C::StageBytes, wsrc + (size_t)s * C::StageBytes, C::StageBytes, bars + B_WFULL + slot);
+      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        for (int s = 0; s < P::StagesPerTile; ++s, ++it) {
+          const uint32_t slot = it % Ring, use = it / Ring;
+          tc::mbar_wait(empty + slot, (use & 1u) ^ 1u);
+          tc::mbar_arrive_expect_tx(full + slot, kStageBytes);
+          tc::bulk_g2s(smem + P::Wr + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================== MMA issuer: one elected region per chunk / phase (see program v3) ==============================
+    return;
+  }
+
+  // ============================== consumers ==============================
+  const int wg = tid >> 7, wl = warp & 3;
+  const int r0 = 16 * wl + (lane >> 2), cq = 2 * (lane & 3);
+  const uint32_t smem_base = tc::smem_u32(smem);
+  auto desc = [&](int off) { return tc::make_wdesc_sw128(smem_base + (uint32_t)off, 1024); };
+  auto sync_consumers = [&]() { tc::bar_sync(1, kConsumers); };
+
+  // ---- the weight ring, consumer side (all 32-bit stage counters run across tiles)
+  uint32_t next_stage = 0, npend = 0;
+  uint32_t pend[4];                                  // own stages whose MMAs may still be in flight (oldest first)
+  auto release = [&](uint32_t s) {
+    __syncwarp();
+    tc::mbar_arrive_if(empty + s % Ring, lane == 0);
+  };
+  auto flush = [&]() {
+    tc::wgmma_wait<0>();
+    for (uint32_t k = 0; k < npend; ++k) release(pend[k]);
+    npend = 0;
+  };
+  // the next stage of the stream; an own stage still in flight in the same ring slot is completed and released first
+  auto take = [&]() -> uint32_t {
+    const uint32_t s = next_stage++;
+    if (npend && (npend == 4 || s - pend[0] >= (uint32_t)Ring)) flush();
+    tc::mbar_wait(full + s % Ring, (s / Ring) & 1u);
+    return s;
+  };
+  auto keep = [&](uint32_t s) { tc::wgmma_commit(); pend[npend++] = s; };
+  auto wslot = [&](uint32_t s) { return P::Wr + (int)(s % Ring) * kStageBytes; };
+
+  // ---- taps of this warp's 8 points for the layer-0 chunks: lane = (point 4 i + qw, channels 8 l8 .. and 64 + 8 l8 ..)
+  const int l8 = lane & 7, qw = lane >> 3;
+  uint32_t t_off[2][2], t_wgt[2][2], t_z[2];
+  auto gen_chunk = [&](int c) {
+    const int ch = c * 128 + l8 * 8;
+    __half2 b8[8], z8[8];
     {
-      const uint32_t idesc128 = tc::make_idesc_f16(128, 128);
-      const uint32_t idesc256 = tc::make_idesc_f16(128, 256);
-      const uint64_t dX = tc::make_sdesc_sw128(tc::smem_u32(smem + Smem::X), 1024);
-      const uint64_t dH0 = tc::make_sdesc_sw128(tc::smem_u32(smem + Smem::H0), 1024);
-      const uint64_t dW = tc::make_sdesc_sw128(tc::smem_u32(smem + Smem::Wr), 1024);
-      constexpr uint64_t kKb = 16384 >> 4, kStage = C::StageBytes >> 4, kSub = C::Sub >> 4;
-      uint32_t slot = 0, wpar = 0;                         // ring slot of the next stage and the parity of its "full" phase
-      uint32_t c_xready = 0, n_chunks = 0, c_h1ready = 0, c_h2ready = 0, c_tiledone = 0;
-      // ---- (inside an elected region: one lane)
-      auto wait_b = [&](int which, uint32_t par) { tc::mbar_wait(bars + which, par); };
-      auto kblock_ss = [&](uint32_t d, uint64_t ad, uint64_t bd, uint32_t idesc, uint32_t acc0) {
+      const uint4 bA = __ldg(reinterpret_cast<const uint4*>(prm.d_bias0 + ch)), bB = __ldg(reinterpret_cast<const uint4*>(prm.d_bias0 + ch + 64));
+      const uint4 zA = __ldg(reinterpret_cast<const uint4*>(prm.d_wz0 + ch)), zB = __ldg(reinterpret_cast<const uint4*>(prm.d_wz0 + ch + 64));
+      *reinterpret_cast<uint4*>(&b8[0]) = bA; *reinterpret_cast<uint4*>(&b8[4]) = bB;
+      *reinterpret_cast<uint4*>(&z8[0]) = zA; *reinterpret_cast<uint4*>(&z8[4]) = zB;
+    }
+    uint8_t* dstp = smem + P::H0 + (c & 1) * 2 * kKb;
+    const __half2 slope2 = __float2half2_rn(MP_LEAKY_SLOPE);
+    uint4 raw[2][4][2];                  // [point][tap][K-block]
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) tc::mma_ss(d, ad + 2 * kk, bd + 2 * kk, idesc, kk == 0 ? acc0 : 1u);
-      };
-      auto kblock_ts = [&](uint32_t d, uint32_t a_tmem, uint64_t bd, uint32_t idesc, uint32_t acc0) {
+    for (int i = 0; i < 2; ++i)
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) tc::mma_ts(d, a_tmem + kk * 8, bd + 2 * kk, idesc, kk == 0 ? acc0 : 1u);
-      };
-      // ---- (uniform, all lanes) the ring positions of the next N stages / the parity of the next X phase
-      auto take = [&](uint32_t (&sl)[8], uint32_t (&pr)[8], int n_take) {
+      for (int a = 0; a < 4; ++a) {
+        const uint32_t off = (a & 1) ? (t_off[i][a >> 1] >> 16) : (t_off[i][a >> 1] & 0xFFFFu);
+        const uint4* srcp = reinterpret_cast<const uint4*>(prm.g0 + (size_t)off * kL0 + ch);
+        raw[i][a][0] = __ldg(srcp);
+        raw[i][a][1] = __ldg(srcp + 8);      // + 64 channels
+      }
 #pragma unroll
-        for (int q = 0; q < 8; ++q)
-          if (q < n_take) {
-            sl[q] = slot; pr[q] = wpar;
-            if (++slot == (uint32_t)C::Stages) { slot = 0; wpar ^= 1u; }
-          }
-      };
-      auto next_x = [&]() -> uint32_t { const uint32_t p = c_xready & 1u; ++c_xready; return p; };
-
-      for (long long g = g0; g < n_tiles; g += gstep) {
-        const bool later_tile = g != g0;
-        uint32_t sl[8], pr[8];
-        // ---- layer 1, hidden part: 8 sampled layer-0 chunks x (2 K-blocks x 2 output halves = 4 stages)
-#pragma unroll 1
-        for (int c = 0; c < 8; ++c) {
-          const int b = c & 1;
-          const uint32_t p_h0 = (n_chunks >> 1) & 1u;
-          ++n_chunks;
-          take(sl, pr, 4);
-          // [384,512) holds the previous tile's acc3 until its fp32 tail has drained it
-          const bool wait_td = later_tile && c == 0;
-          const uint32_t p_td = c_tiledone & 1u;
-          if (wait_td) ++c_tiledone;
-          const uint32_t acc_first = c == 0 ? 0u : 1u;
-          if (tc::elect_one()) {
-            wait_b(B_H0_READY0 + b, p_h0);
+    for (int i = 0; i < 2; ++i) {
+      const int p = warp * 8 + 4 * i + qw;
+      const __half2 zq2 = *reinterpret_cast<const __half2*>(&t_z[i]);
+      __half2 acc[8];
 #pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              const int kb = q >> 1, nh = q & 1;
-              wait_b(B_WFULL + (int)sl[q], pr[q]);
-              if (q == 1 && wait_td) wait_b(B_TILE_DONE, p_td);
-              tc::tcgen05_fence_after();
-              kblock_ss(tbase + cAcc1 + nh * 256, dH0 + (uint64_t)(b * 2 + kb) * kKb, dW + sl[q] * kStage, idesc256,
-                        kb == 0 ? acc_first : 1u);
-              tc::mma_commit(bars + B_WEMPTY + sl[q]);
-            }
-            tc::mma_commit(bars + B_H0_FREE0 + b);
-          }
-        }
-        // ---- layer 1, skip part: phase A, then phase B (8 stages each)
-#pragma unroll 1
-        for (int ph = 0; ph < 2; ++ph) {
-          const uint32_t p_x = next_x();
-          take(sl, pr, 8);
-          if (tc::elect_one()) {
-            wait_b(B_XREADY, p_x);
+      for (int j = 0; j < 8; ++j) acc[j] = __hfma2(z8[j], zq2, b8[j]);
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              const int kb = q >> 1, nh = q & 1;
-              wait_b(B_WFULL + (int)sl[q], pr[q]);
-              tc::tcgen05_fence_after();
-              kblock_ss(tbase + cAcc1 + nh * 256, dX + (uint64_t)kb * kKb, dW + sl[q] * kStage, idesc256, 1u);
-              tc::mma_commit(bars + B_WEMPTY + sl[q]);
-            }
-            if (ph == 0) tc::mma_commit(bars + B_XFREE);       // phase A consumed; phase B stays for layer 2
-            else tc::mma_commit(bars + B_ACC1_FULL);
-          }
-        }
-        // ---- layer 2: A = H1 from TMEM (8 K-blocks), then X phase B (resident), then phase A -> acc2 [128,384)
-        {
-          const uint32_t p_h1 = c_h1ready & 1u;
-          ++c_h1ready;
-          take(sl, pr, 8);
-          if (tc::elect_one()) {
-            wait_b(B_H1_READY, p_h1);
+      for (int a = 0; a < 4; ++a) {          // same tap order as grid_sample: nw, ne, sw, se
+        const __half2 wp = *reinterpret_cast<const __half2*>(&t_wgt[i][a >> 1]);
+        const __half2 w2 = (a & 1) ? __high2half2(wp) : __low2half2(wp);
+        const __half2* h0 = reinterpret_cast<const __half2*>(&raw[i][a][0]);
+        const __half2* h1 = reinterpret_cast<const __half2*>(&raw[i][a][1]);
 #pragma unroll
-            for (int q = 0; q < 8; ++q) {
-              wait_b(B_WFULL + (int)sl[q], pr[q]);
-              tc::tcgen05_fence_after();
-              kblock_ts(tbase + cAcc2, tbase + (q < 4 ? cH1lo + q * 32 : cH1hi + (q - 4) * 32), dW + sl[q] * kStage, idesc256,
-                        q == 0 ? 0u : 1u);
-              tc::mma_commit(bars + B_WEMPTY + sl[q]);
-            }
-          }
-#pragma unroll 1
-          for (int ph = 0; ph < 2; ++ph) {
-            const uint32_t p_x = ph == 1 ? next_x() : 0u;      // phase A again
-            take(sl, pr, 4);
-            if (tc::elect_one()) {
-              if (ph == 1) wait_b(B_XREADY, p_x);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                wait_b(B_WFULL + (int)sl[q], pr[q]);
-                tc::tcgen05_fence_after();
-                kblock_ss(tbase + cAcc2, dX + (uint64_t)q * kKb, dW + sl[q] * kStage, idesc256, 1u);
-                tc::mma_commit(bars + B_WEMPTY + sl[q]);
-              }
-              if (ph == 0) tc::mma_commit(bars + B_XFREE);     // phase B consumed
-              else tc::mma_commit(bars + B_ACC2_FULL);
-            }
-          }
-        }
-        // ---- layer 3 -> acc3 [384,512): skip phase A (resident), skip phase B, hidden part; every part multiplies by W3 as an
-        //      fp16 pair: stages 0,1 = hi(W3) of K-blocks (0,1) (2,3), stages 2,3 = lo(W3), same A
-#pragma unroll 1
-        for (int ph = 0; ph < 2; ++ph) {
-          const uint32_t p_x = ph == 1 ? next_x() : 0u;        // phase B again
-          take(sl, pr, 4);
-          if (tc::elect_one()) {
-            if (ph == 1) wait_b(B_XREADY, p_x);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-              wait_b(B_WFULL + (int)sl[q], pr[q]);
-              tc::tcgen05_fence_after();
-              kblock_ss(tbase + cAcc3, dX + (uint64_t)(2 * (q & 1)) * kKb, dW + sl[q] * kStage, idesc128, (ph == 0 && q == 0) ? 0u : 1u);
-              kblock_ss(tbase + cAcc3, dX + (uint64_t)(2 * (q & 1) + 1) * kKb, dW + sl[q] * kStage + kSub, idesc128, 1u);
-              tc::mma_commit(bars + B_WEMPTY + sl[q]);
-            }
-            tc::mma_commit(bars + B_XFREE);                    // after phase B: X is dead, the next tile's phase A may be sampled
-          }
-        }
-        {
-          const uint32_t p_h2 = c_h2ready & 1u;
-          ++c_h2ready;
-          take(sl, pr, 4);
-          if (tc::elect_one()) {
-            wait_b(B_H2_READY, p_h2);
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {                      // hi(W3) stages, then lo(W3) stages
-              wait_b(B_WFULL + (int)sl[q], pr[q]);
-              tc::tcgen05_fence_after();
-              kblock_ts(tbase + cAcc3, tbase + cH2 + (2 * (q & 1)) * 32, dW + sl[q] * kStage, idesc128, 1u);
-              kblock_ts(tbase + cAcc3, tbase + cH2 + (2 * (q & 1) + 1) * 32, dW + sl[q] * kStage + kSub, idesc128, 1u);
-              tc::mma_commit(bars + B_WEMPTY + sl[q]);
-            }
-            tc::mma_commit(bars + B_ACC3_FULL);
-          }
+        for (int j = 0; j < 4; ++j) {
+          acc[j] = __hfma2(h0[j], w2, acc[j]);
+          acc[4 + j] = __hfma2(h1[j], w2, acc[4 + j]);
         }
       }
-    }
-  } else if (warp == 2 || warp == 3) {
-    // ============================== samplers: four phase fills of X per tile (A, B, A, B) ==============================
-    const int sw = warp - 2;
-    uint32_t c_xfree = 0;
-    bool first_fill = true;
-    for (long long g = g0; g < n_tiles; g += gstep) {
-      const long long p0 = g * kTile;
-      for (int f = 0; f < 4; ++f) {
-        if (!first_fill) wait_bar(bars, B_XFREE, c_xfree);
-        first_fill = false;
-#pragma unroll 1
-        for (int grp = 0; grp < 4; ++grp) {
-          const int pbase = sw * 64 + grp * 16;
-          const PointTaps pt = colour_taps(surf, src, cal, prm.H, prm.W, p0 + pbase + (lane & 15), n);
-          sample_x_phase(prm, smem + Smem::X, pt, pbase, lane, f & 1);
-        }
-        tc::fence_proxy_async_smem();
-        warp_arrive_local(bars + B_XREADY, lane);
+      uint32_t o[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const __half2 r = __hmax2(acc[j], __hmul2(acc[j], slope2));
+        o[j] = *reinterpret_cast<const uint32_t*>(&r);
       }
+      *reinterpret_cast<uint4*>(dstp + tc::sw128_offset(p, l8 * 8)) = make_uint4(o[0], o[1], o[2], o[3]);
+      *reinterpret_cast<uint4*>(dstp + kKb + tc::sw128_offset(p, l8 * 8)) = make_uint4(o[4], o[5], o[6], o[7]);
     }
-  } else if (warp >= 4) {
-    // ============================== workers: layer-0 chunk generators + epilogue ==============================
-    const int wk = warp - 4;
-    const int wg = wk >> 2;
-    const int quarter = warp & 3;
-    const int row = quarter * 32 + lane;
-    const uint32_t lane_base = (uint32_t)(quarter * 32) << 16;
-    uint32_t c_h0free[2] = {0, 0}, c_acc1full = 0, c_acc2full = 0, c_acc3full = 0;
-    const int l16 = lane & 15;
+    tc::fence_proxy_async_smem();
+  };
 
-    auto act_pack = [&](float a, float b) -> uint32_t {
-      const __half2 h = __floats2half2_rn(a, b);
-      const __half2 r = __hmax2(h, __hmul2(h, __float2half2_rn(MP_LEAKY_SLOPE)));
-      return *reinterpret_cast<const uint32_t*>(&r);
-    };
-    // taps of this warp's 16 points (a quarter-warp per point, four points per lane), as in program v3
-    const int l8 = lane & 7, qw = lane >> 3;
-    uint32_t t_off[4][2], t_wgt[4][2], t_z[4];
-    auto compute_taps = [&](long long g) {
-      const PointTaps pt = colour_taps(surf, src, cal, prm.H, prm.W, g * kTile + wk * 16 + l16, n);
+  for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    const long long p0 = win0 + t * kTile;
+    // ---- X (skip operand) + per-point scalars: 4 groups of 16 points x C/256 channel phases over the 8 warps
+#pragma unroll 1
+    for (int job = warp; job < 4 * (C / 256); job += 8) {
+      const int grp = job & 3, phase = job >> 2;
+      const PointTaps pt = point_taps(surf, src, cal, prm.H, prm.W, p0 + grp * 16 + (lane & 15), n);
+      sample_x16<C>(prm, smem + P::X, s_zf, s_in, s_s4, pt, grp * 16, lane, phase);
+    }
+    {
+      const PointTaps pt = point_taps(surf, src, cal, prm.H, prm.W, p0 + warp * 8 + l8, n);
       const uint32_t o01 = (uint32_t)pt.off[0] | ((uint32_t)pt.off[1] << 16), o23 = (uint32_t)pt.off[2] | ((uint32_t)pt.off[3] << 16);
       const uint32_t w01 = tc::pack_half2(pt.wgt[0], pt.wgt[1]), w23 = tc::pack_half2(pt.wgt[2], pt.wgt[3]);
       const uint32_t zz = tc::pack_half2(pt.zf, pt.zf);
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
+      for (int i = 0; i < 2; ++i) {
         const int q = 4 * i + qw;
         t_off[i][0] = __shfl_sync(0xffffffffu, o01, q);
         t_off[i][1] = __shfl_sync(0xffffffffu, o23, q);
@@ -1404,284 +380,240 @@ query_tc3c_kernel(TcParams prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpSur
         t_wgt[i][1] = __shfl_sync(0xffffffffu, w23, q);
         t_z[i] = __shfl_sync(0xffffffffu, zz, q);
       }
-    };
-    // one sampled layer-0 chunk: h0[:, c*128 .. +128) = lrelu(lerp(G0) + b0 + w0z z) -> H0 smem buffer c&1 (packed-fp16 FMAs)
-    auto gen_chunk = [&](int c) {
-      const int b = c & 1;
-      wait_free(bars, B_H0_FREE0 + b, c_h0free[b]);
-      const int ch = c * 128 + l8 * 8;
-      __half2 b8[8], z8[8];
-      {
-        const uint4 bA = __ldg(reinterpret_cast<const uint4*>(prm.d_bias0 + ch)), bB = __ldg(reinterpret_cast<const uint4*>(prm.d_bias0 + ch + 64));
-        const uint4 zA = __ldg(reinterpret_cast<const uint4*>(prm.d_wz0 + ch)), zB = __ldg(reinterpret_cast<const uint4*>(prm.d_wz0 + ch + 64));
-        *reinterpret_cast<uint4*>(&b8[0]) = bA; *reinterpret_cast<uint4*>(&b8[4]) = bB;
-        *reinterpret_cast<uint4*>(&z8[0]) = zA; *reinterpret_cast<uint4*>(&z8[4]) = zB;
+    }
+    tc::fence_proxy_async_smem();
+    gen_chunk(0);
+    sync_consumers();
+    const float zf0 = s_zf[r0], zf1 = s_zf[r0 + 8];
+
+    // ---- layer 1: 8 sampled layer-0 chunks (2 K-blocks each), then X; this warpgroup's 256 of the 512 outputs
+    {
+      float acc[128];
+#pragma unroll
+      for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+#pragma unroll 1
+      for (int c = 0; c < 8; ++c) {
+        tc::wgmma_fence();
+#pragma unroll
+        for (int kb = 0; kb < 2; ++kb) {
+          // the K-block's two stages carry output halves 0 and 1: this warpgroup multiplies by its own, releases the other
+          const uint32_t s0 = take(), s1 = take();
+          const uint32_t mine = wg ? s1 : s0;
+          release(wg ? s0 : s1);
+          const uint64_t da = desc(P::H0 + ((c & 1) * 2 + kb) * kKb), db = desc(wslot(mine));
+#pragma unroll
+          for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
+          keep(mine);
+        }
+        if (c < 7) {
+          // the other chunk buffer was read by chunk c-1: complete it here (chunk c stays in flight), then in both warpgroups
+          tc::wgmma_wait<2>();
+          while (npend > 2) {
+            release(pend[0]);
+            for (uint32_t k = 1; k < npend; ++k) pend[k - 1] = pend[k];
+            --npend;
+          }
+          sync_consumers();
+          gen_chunk(c + 1);
+          sync_consumers();
+        }
       }
-      uint8_t* dstp = smem + Smem::H0 + b * 32768;
-      const __half2 slope2 = __float2half2_rn(MP_LEAKY_SLOPE);
+      tc::wgmma_fence();
+#pragma unroll 1
+      for (int kb = 0; kb < XKB; ++kb) {
+        const uint32_t s0 = take(), s1 = take();
+        const uint32_t mine = wg ? s1 : s0;
+        release(wg ? s0 : s1);
+        const uint64_t da = desc(P::X + kb * kKb), db = desc(wslot(mine));
 #pragma unroll
-      for (int batch = 0; batch < 2; ++batch) {
-        uint4 raw[2][4][2];                  // [point][tap][K-block]
+        for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
+        keep(mine);
+      }
+      flush();
+      // epilogue -> H1 (fp16, K-major): + bias + w_z z, leaky ReLU
 #pragma unroll
-        for (int ps = 0; ps < 2; ++ps) {
-          const int i = batch * 2 + ps;
-#pragma unroll
-          for (int a = 0; a < 4; ++a) {
-            const uint32_t off = (a & 1) ? (t_off[i][a >> 1] >> 16) : (t_off[i][a >> 1] & 0xFFFFu);
-            const uint4* srcp = reinterpret_cast<const uint4*>(prm.g0 + (size_t)off * kL0 + ch);
-            raw[ps][a][0] = __ldg(srcp);
-            raw[ps][a][1] = __ldg(srcp + 8);      // + 64 channels
-          }
-        }
-#pragma unroll
-        for (int ps = 0; ps < 2; ++ps) {
-          const int i = batch * 2 + ps;
-          const int p = wk * 16 + 4 * i + qw;
-          const __half2 zq2 = *reinterpret_cast<const __half2*>(&t_z[i]);
-          __half2 acc[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) acc[j] = __hfma2(z8[j], zq2, b8[j]);
-#pragma unroll
-          for (int a = 0; a < 4; ++a) {          // same tap order as grid_sample: nw, ne, sw, se
-            const __half2 wp = *reinterpret_cast<const __half2*>(&t_wgt[i][a >> 1]);
-            const __half2 w2 = (a & 1) ? __high2half2(wp) : __low2half2(wp);
-            const __half2* h0 = reinterpret_cast<const __half2*>(&raw[ps][a][0]);
-            const __half2* h1 = reinterpret_cast<const __half2*>(&raw[ps][a][1]);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              acc[j] = __hfma2(h0[j], w2, acc[j]);
-              acc[4 + j] = __hfma2(h1[j], w2, acc[4 + j]);
-            }
-          }
-          uint32_t o[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const __half2 r = __hmax2(acc[j], __hmul2(acc[j], slope2));
-            o[j] = *reinterpret_cast<const uint32_t*>(&r);
-          }
-          *reinterpret_cast<uint4*>(dstp + tc::sw128_offset(p, l8 * 8)) = make_uint4(o[0], o[1], o[2], o[3]);
-          *reinterpret_cast<uint4*>(dstp + 16384 + tc::sw128_offset(p, l8 * 8)) = make_uint4(o[4], o[5], o[6], o[7]);
-        }
+      for (int j = 0; j < 32; ++j) {
+        const int col = wg * 256 + 8 * j + cq;
+        const float b0 = prm.bias_all[side_off(1) + col], b1 = prm.bias_all[side_off(1) + col + 1];
+        const float z0 = prm.wz_all[side_off(1) + col], z1 = prm.wz_all[side_off(1) + col + 1];
+        uint8_t* kbp = smem + P::H1 + (col >> 6) * kKb;
+        *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0, col & 63)) =
+            act_pack(acc[4 * j + 0] + fmaf(z0, zf0, b0), acc[4 * j + 1] + fmaf(z1, zf0, b1));
+        *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0 + 8, col & 63)) =
+            act_pack(acc[4 * j + 2] + fmaf(z0, zf1, b0), acc[4 * j + 3] + fmaf(z1, zf1, b1));
       }
       tc::fence_proxy_async_smem();
-      warp_arrive_local(bars + B_H0_READY0 + b, lane);
-    };
-    float zf = 0.f, inimg = 0.f;
-    float s4[kResC] = {0.f, 0.f, 0.f};
-    auto load_pre = [&](uint32_t col, int ch0, float (&o)[32]) {
-      uint32_t v[32];
-      tc::tmem_ld32(tbase + lane_base + col, v);
-      tc::tmem_ld_wait();
-      const float4* bz = reinterpret_cast<const float4*>(&prm.bias_all[ch0]);
-      const float4* wz = reinterpret_cast<const float4*>(&prm.wz_all[ch0]);
+      sync_consumers();
+    }
+    // ---- layer 2: H1 (8 K-blocks), then X; this warpgroup's 128 of the 256 outputs -> H2 (over the chunk buffers)
+    {
+      float acc[64];
 #pragma unroll
-      for (int j4 = 0; j4 < 8; ++j4) {
-        const float4 b = bz[j4], z = wz[j4];
-        o[4 * j4 + 0] = __uint_as_float(v[4 * j4 + 0]) + fmaf(z.x, zf, b.x);
-        o[4 * j4 + 1] = __uint_as_float(v[4 * j4 + 1]) + fmaf(z.y, zf, b.y);
-        o[4 * j4 + 2] = __uint_as_float(v[4 * j4 + 2]) + fmaf(z.z, zf, b.z);
-        o[4 * j4 + 3] = __uint_as_float(v[4 * j4 + 3]) + fmaf(z.w, zf, b.w);
+      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+      tc::wgmma_fence();
+#pragma unroll 1
+      for (int kb = 0; kb < 8 + XKB; ++kb) {
+        const uint32_t s = take();
+        const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(wslot(s) + wg * 16384);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tc::wgmma_m64n128(acc, da + 2 * k, db + 2 * k);
+        keep(s);
       }
-    };
-    // worker loop, software-pipelined across tiles exactly like program v3 (virtual first iteration = pre-generation only)
-    for (long long g = g0 - gstep; g < n_tiles; g += gstep) {
-      const bool real = g >= g0;
-      const bool has_next = g + gstep < n_tiles;
-      const long long p0 = g * kTile;
+      flush();
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = wg * 128 + 8 * j + cq;
+        const float b0 = prm.bias_all[side_off(2) + col], b1 = prm.bias_all[side_off(2) + col + 1];
+        const float z0 = prm.wz_all[side_off(2) + col], z1 = prm.wz_all[side_off(2) + col + 1];
+        uint8_t* kbp = smem + P::H0 + (col >> 6) * kKb;
+        *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0, col & 63)) =
+            act_pack(acc[4 * j + 0] + fmaf(z0, zf0, b0), acc[4 * j + 1] + fmaf(z1, zf0, b1));
+        *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0 + 8, col & 63)) =
+            act_pack(acc[4 * j + 2] + fmaf(z0, zf1, b0), acc[4 * j + 3] + fmaf(z1, zf1, b1));
+      }
+      tc::fence_proxy_async_smem();
+      sync_consumers();
+    }
+    // ---- layer 3: X, then H2 (two K-blocks per stage; colour: hi then lo pass); 64 of the 128 outputs; layer 4 in fp32
+    {
+      float acc[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+      tc::wgmma_fence();
 #pragma unroll 1
-      for (int step = 0; step < 11; ++step) {
-        int gc = -1;
-        if (step < 6) { if (real) gc = step + 2; }
-        else if (step == 7) { if (has_next) { compute_taps(g + gstep); gc = 0; } }
-        else if (step == 10) { if (has_next) gc = 1; }
-        if (gc >= 0) gen_chunk(gc);
-        if (!real) continue;
-        if (step == 6) {
-          // per-point scalars of the point this thread owns in the epilogue (TMEM lane `row`)
-          {
-            const PointTaps me = colour_taps(surf, src, cal, prm.H, prm.W, p0 + row, n);
-            zf = me.zf;
-            inimg = me.in_img ? 1.f : 0.f;
-            if (wg == 0) {
+      for (int q = 0; q < P::StagesL3; ++q) {
+        const uint32_t s = take();
 #pragma unroll
-              for (int r = 0; r < kResC; ++r) {
-                float s = 0.f;
+        for (int sub = 0; sub < 2; ++sub) {
+          const int kb = (2 * q + sub) % (XKB + 4);
+          const uint64_t da = desc(kb < XKB ? P::X + kb * kKb : P::H0 + (kb - XKB) * kKb);
+          const uint64_t db = desc(wslot(s) + sub * 16384 + wg * 8192);
 #pragma unroll
-                for (int a = 0; a < 4; ++a) s = fmaf(me.wgt[a], __ldg(prm.s4tex + (size_t)me.off[a] * kResC + r), s);
-                s4[r] = s + __ldg(prm.w4z + r) * zf + __ldg(prm.b4 + r);
-              }
+          for (int k = 0; k < 4; ++k) tc::wgmma_m64n64(acc, da + 2 * k, db + 2 * k);
+        }
+        keep(s);
+      }
+      flush();
+      float lg[2][RES];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < RES; ++r) lg[h][r] = 0.f;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int col = wg * 64 + 8 * j + cq + (e & 1);
+          float o = acc[4 * j + e] + fmaf(prm.wz_all[side_off(3) + col], (e >> 1) ? zf1 : zf0, prm.bias_all[side_off(3) + col]);
+          o = fmaxf(o, o * MP_LEAKY_SLOPE);
+#pragma unroll
+          for (int r = 0; r < RES; ++r) lg[e >> 1][r] = fmaf(__ldg(prm.w4h + r * kL3 + col), o, lg[e >> 1][r]);
+        }
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < RES; ++r) {
+          lg[h][r] += __shfl_xor_sync(0xffffffffu, lg[h][r], 1);
+          lg[h][r] += __shfl_xor_sync(0xffffffffu, lg[h][r], 2);
+        }
+      // warpgroup 1's partial sums -> warpgroup 0 through the (dead) H1 buffer
+      float* s_part = reinterpret_cast<float*>(smem + P::H1);
+      const int mine = lane & 3;                 // lane 0 of a quad: row r0, lane 1: row r0 + 8
+      const int row = r0 + 8 * (mine & 1);
+      if (wg == 1 && mine < 2) {
+#pragma unroll
+        for (int r = 0; r < RES; ++r) s_part[r * kTile + row] = lg[mine][r];
+      }
+      sync_consumers();
+      if (wg == 0 && mine < 2) {
+        const long long i = p0 + row;
+        if (i < n) {
+          const float inimg = s_in[row];
+#pragma unroll
+          for (int r = 0; r < RES; ++r) {
+            const float logit = s_s4[r * kTile + row] + (lg[mine][r] + s_part[r * kTile + row]);
+            const float val = inimg * mp_last_op(logit, prm.last_op);
+            if (surf.canvas) {
+              float* px = surf.canvas + ((size_t)__ldg(surf.X + i) * surf.canvas_R + (size_t)__ldg(surf.Y + i)) * 3;
+              px[r] = __fadd_rn(__fmul_rn(val, 0.5f), 0.5f);      // RTL/main.py:244
+              continue;
             }
-          }
-          // ---- layer 1 (512 columns) -> H1, drained in place (see program v3)
-          wait_bar(bars, B_ACC1_FULL, c_acc1full);
-          tc::tcgen05_fence_after();
-#pragma unroll 1
-          for (int gi = 0; gi < 8; ++gi) {
-            const int gq = (wg == 0) ? gi : 7 - gi;
-            const int lc = wg * 256 + gq * 32;
-            float o[32];
-            load_pre(cAcc1 + lc, side_off(1) + lc, o);
-            uint32_t pk[16];
+            if (dst.out) dst.out[(long long)r * dst.ld + i] = val;
+            if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = val;
+            if constexpr (PEERS) {
+              if (r == 0) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) pk[j] = act_pack(o[2 * j], o[2 * j + 1]);
-            const uint32_t dcol = (wg == 0) ? (cH1lo + lc / 2) : (cH1hi + (lc - 256) / 2);
-            tc::tmem_st16(tbase + lane_base + dcol, pk);
-            tc::tmem_st_wait();
-          }
-          tc::tcgen05_fence_before();
-          warp_arrive_local(bars + B_H1_READY, lane);
-        } else if (step == 8) {
-          // ---- layer 2 -> H2 [0,128)
-          wait_bar(bars, B_ACC2_FULL, c_acc2full);
-          tc::tcgen05_fence_after();
-#pragma unroll 1
-          for (int gq = 0; gq < 4; ++gq) {
-            float o[32];
-            const int lc = wg * 128 + gq * 32;
-            load_pre(cAcc2 + lc, side_off(2) + lc, o);
-            uint32_t pk[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) pk[j] = act_pack(o[2 * j], o[2 * j + 1]);
-            tc::tmem_st16(tbase + lane_base + cH2 + lc / 2, pk);
-          }
-          tc::tmem_st_wait();
-          tc::tcgen05_fence_before();
-          warp_arrive_local(bars + B_H2_READY, lane);
-        } else if (step == 9) {
-          // ---- layer 3 + layer 4 (641 -> 3) in fp32, warpgroup 0
-          if (wg == 0) {
-            wait_bar(bars, B_ACC3_FULL, c_acc3full);
-            tc::tcgen05_fence_after();
-            float logit[kResC];
-#pragma unroll
-            for (int r = 0; r < kResC; ++r) logit[r] = s4[r];
-#pragma unroll 1
-            for (int gq = 0; gq < 4; ++gq) {
-              float o[32];
-              load_pre(cAcc3 + gq * 32, side_off(3) + gq * 32, o);
-#pragma unroll
-              for (int j = 0; j < 32; ++j) o[j] = fmaxf(o[j], o[j] * MP_LEAKY_SLOPE);
-#pragma unroll
-              for (int r = 0; r < kResC; ++r) {
-                const float4* wv = reinterpret_cast<const float4*>(prm.w4h + r * kL3 + gq * 32);
-#pragma unroll
-                for (int j4 = 0; j4 < 8; ++j4) {
-                  const float4 w4 = __ldg(wv + j4);
-                  logit[r] = fmaf(w4.x, o[4 * j4 + 0], logit[r]);
-                  logit[r] = fmaf(w4.y, o[4 * j4 + 1], logit[r]);
-                  logit[r] = fmaf(w4.z, o[4 * j4 + 2], logit[r]);
-                  logit[r] = fmaf(w4.w, o[4 * j4 + 3], logit[r]);
-                }
-              }
-            }
-            tc::tcgen05_fence_before();
-            warp_arrive_local(bars + B_TILE_DONE, lane);
-            const long long i = p0 + row;
-            if (i < n) {
-              if (surf.canvas) {
-                float* px = surf.canvas + ((size_t)__ldg(surf.X + i) * surf.canvas_R + (size_t)__ldg(surf.Y + i)) * 3;
-#pragma unroll
-                for (int r = 0; r < kResC; ++r)
-                  px[r] = __fadd_rn(__fmul_rn(inimg * mp_last_op(logit[r], prm.last_op), 0.5f), 0.5f);      // RTL/main.py:244
-              } else if (dst.out) {
-#pragma unroll
-                for (int r = 0; r < kResC; ++r) dst.out[(long long)r * dst.ld + i] = inimg * mp_last_op(logit[r], prm.last_op);
+                for (int pp = 0; pp < MP_MAX_PEERS; ++pp)
+                  if (pp < dst.n_peers) dst.peer[pp][dst.peer_off + i] = val;
               }
             }
           }
         }
       }
+      sync_consumers();        // the per-point scalars and X are rewritten by the next tile
     }
   }
-  __syncwarp();
-  tc::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 2) tc::tmem_dealloc(tbase, 512);
 }
 
-// G0 / fp16 copy / S4 of the 512-channel colour map: as g0_tc_kernel with eight K-blocks (A staged once: 128 KB, so the B
-// ring has two 32 KB stages) and three last-layer outputs.
-constexpr int kG0cKB = kCc / 64;                       // 8 K-blocks
-constexpr int kG0cStages = 2;
-constexpr uint32_t kG0cSmemA = kG0cKB * 16384, kG0cSmemB = kG0cStages * 32768;
-constexpr uint32_t kG0cSmem = kG0cSmemA + kG0cSmemB + 1024 /*align*/ + 128 /*barriers + tmem slot*/;
+// G0[texel][n] = sum_k F[texel][k] * W0f[n][k] on the tensor cores: fp16 operands (F rounded once while staging, W0f
+// pre-packed on the host as SWIZZLE_128B tiles [n tile][K block][256 x 64]) and fp32 accumulation in registers.
+// One CTA = 128 texels x all 1024 outputs: the A operand (128 x C) is staged ONCE by the two consumer warpgroups (fp32
+// global -> fp16 swizzled smem), the B tiles stream through a 2-stage bulk-copy ring (warp 8), and each warpgroup multiplies
+// its 64 rows by the four 256-wide output tiles.  The staging pass also publishes what it has in hand: the fp16 copy of the
+// map (F16, taps of the X operand) and S4 = W4s . F per texel in fp32 (the last layer's direct access to the features:
+// sampling S4 in fp32 keeps that path out of the fp16 roundings -- bilinear sampling commutes with the dot product).
+constexpr int kG0TileN = 256;
+constexpr int kG0NT = kL0 / kG0TileN;                 // 4 output tiles
+constexpr int kG0Stages = 2;
+template <int C> struct G0Cfg {
+  static constexpr int KB = C / 64;
+  static constexpr uint32_t SmemA = KB * 16384, SmemB = kG0Stages * 32768;
+  static constexpr uint32_t Smem = SmemA + SmemB + 1024 /*align*/ + 64 /*barriers*/;
+};
 
-__global__ void __launch_bounds__(kG0Threads, 1)
-g0c_tc_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half* __restrict__ G, int M,
-              __half* __restrict__ F16, float* __restrict__ S4, const float* __restrict__ w4s, unsigned* __restrict__ amax) {
+template <int C>
+__global__ void __launch_bounds__(kThreads, 1)
+g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half* __restrict__ G, int M,
+             __half* __restrict__ F16, float* __restrict__ S4, const float* __restrict__ w4s, unsigned* __restrict__ amax) {
+  using Cfg = G0Cfg<C>;
+  constexpr int RES = Prog<C>::RES, KB = Cfg::KB;
   MP_DYN_SMEM(uint8_t, g0_smem_raw);
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(g0_smem_raw) + 1023) & ~(uintptr_t)1023);
   uint8_t* sA = base;
-  uint8_t* sB = base + kG0cSmemA;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(base + kG0cSmemA + kG0cSmemB);
-  uint64_t* b_full = bars;                   // [2] B stage landed
-  uint64_t* b_empty = bars + 4;              // [2] B stage consumed (tcgen05.commit)
-  uint64_t* acc_full = bars + 8;             // [2] accumulator complete
-  uint64_t* acc_free = bars + 10;            // [2] accumulator drained by the 8 epilogue warps
-  uint64_t* a_ready = bars + 12;             // A staged (8 warps)
-  uint32_t* tslot = reinterpret_cast<uint32_t*>(bars + 13);
+  uint8_t* sB = base + Cfg::SmemA;
+  uint64_t* b_full = reinterpret_cast<uint64_t*>(base + Cfg::SmemA + Cfg::SmemB);
+  uint64_t* b_empty = b_full + kG0Stages;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.x * 128;
   if (tid == 0) {
-    for (int i = 0; i < kG0cStages; ++i) { tc::mbar_init(&b_full[i], 1); tc::mbar_init(&b_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { tc::mbar_init(&acc_full[i], 1); tc::mbar_init(&acc_free[i], 8); }
-    tc::mbar_init(a_ready, 8);
+    for (int i = 0; i < kG0Stages; ++i) { tc::mbar_init(&b_full[i], 1); tc::mbar_init(&b_empty[i], kConsumers / 32); }
     tc::fence_barrier_init();
   }
-  if (warp == 8) {
-    tc::tmem_alloc(tslot, 512);
-    tc::tmem_relinquish();
-  }
-  tc::tcgen05_fence_before();
   __syncthreads();
-  tc::tcgen05_fence_after();
-  const uint32_t tbase = *tslot;
-  constexpr uint32_t idesc = tc::make_idesc_f16(128, kG0TileN);
-  constexpr int kTiles = kG0NT * kG0cKB;       // 32 B tiles in (nt, kb) order
 
-  if (warp == 8) {
+  if (warp == kConsumers / 32) {
+    // ---- B producer: kG0NT x KB tiles in (nt, kb) order through the ring
     if (lane == 0) {
-      for (int s = 0; s < kTiles; ++s) {
-        const int slot = s % kG0cStages;
-        if (s >= kG0cStages) tc::mbar_wait(&b_empty[slot], ((s / kG0cStages) & 1) ^ 1);
+      for (int s = 0; s < kG0NT * KB; ++s) {
+        const int slot = s % kG0Stages;
+        tc::mbar_wait(&b_empty[slot], ((s / kG0Stages) & 1) ^ 1);
         tc::mbar_arrive_expect_tx(&b_full[slot], 32768);
         tc::bulk_g2s(sB + slot * 32768, Wt + (size_t)s * 32768, 32768, &b_full[slot]);
       }
     }
-  } else if (warp == 9) {
-    // ---- MMA issuer: one elected region per output tile (see g0_tc_kernel)
-    {
-      const uint64_t dA = tc::make_sdesc_sw128(tc::smem_u32(sA), 1024), dB = tc::make_sdesc_sw128(tc::smem_u32(sB), 1024);
-#pragma unroll 1
-      for (int nt = 0; nt < kG0NT; ++nt) {
-        const int buf = nt & 1;
-        if (tc::elect_one()) {
-          if (nt == 0) tc::mbar_wait(a_ready, 0);
-          if (nt >= 2) tc::mbar_wait(&acc_free[buf], ((nt >> 1) & 1) ^ 1);
-#pragma unroll
-          for (int kb = 0; kb < kG0cKB; ++kb) {
-            const int s = nt * kG0cKB + kb, slot = s % kG0cStages;
-            tc::mbar_wait(&b_full[slot], (s / kG0cStages) & 1);
-            tc::tcgen05_fence_after();
-#pragma unroll
-            for (int k16 = 0; k16 < 4; ++k16)
-              tc::mma_ss(tbase + buf * kG0TileN, dA + (uint64_t)kb * (16384 >> 4) + 2 * k16, dB + (uint64_t)slot * (32768 >> 4) + 2 * k16, idesc,
-                         (kb | k16) ? 1u : 0u);
-            tc::mma_commit(&b_empty[slot]);
-          }
-          tc::mma_commit(&acc_full[buf]);
-        }
-      }
-    }
-  } else {
-    // ---- warps 0-7: stage A (thread -> row = tid / 2, 32-column half of each 64-wide K-block), then drain
+    return;
+  }
+  // ---- stage A (thread -> row = tid / 2, 32-column half of each 64-wide K-block)
+  {
     const int row = tid >> 1, half = tid & 1;
     const bool live = (m0 + row) < M;
-    const float* frow = F + (size_t)(live ? m0 + row : 0) * kCc + half * 32;
-    float s4acc[kResC] = {0.f, 0.f, 0.f};
+    const float* frow = F + (size_t)(live ? m0 + row : 0) * C + half * 32;
+    float s4acc[RES];
     float fmax_abs = 0.f;             // range guard: the largest |feature| this thread stages
+#pragma unroll
+    for (int r = 0; r < RES; ++r) s4acc[r] = 0.f;
 #pragma unroll 1
-    for (int kb = 0; kb < kG0cKB; ++kb) {
+    for (int kb = 0; kb < KB; ++kb) {
       float4 v[8];
 #pragma unroll
       for (int j = 0; j < 8; ++j) v[j] = live ? __ldg(reinterpret_cast<const float4*>(frow + kb * 64) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -1695,11 +627,11 @@ g0c_tc_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __hal
         pk.z = tc::pack_half2(v[2 * j + 1].x, v[2 * j + 1].y);
         pk.w = tc::pack_half2(v[2 * j + 1].z, v[2 * j + 1].w);
         *reinterpret_cast<uint4*>(sA + kb * 16384 + tc::sw128_offset(row, half * 32 + j * 8)) = pk;
-        if (live) *reinterpret_cast<uint4*>(F16 + (size_t)(m0 + row) * kCc + kb * 64 + half * 32 + j * 8) = pk;
+        if (live) *reinterpret_cast<uint4*>(F16 + (size_t)(m0 + row) * C + kb * 64 + half * 32 + j * 8) = pk;
       }
 #pragma unroll
-      for (int r = 0; r < kResC; ++r) {
-        const float4* wv = reinterpret_cast<const float4*>(w4s + r * kCc + kb * 64 + half * 32);
+      for (int r = 0; r < RES; ++r) {
+        const float4* wv = reinterpret_cast<const float4*>(w4s + r * C + kb * 64 + half * 32);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float4 w = __ldg(wv + j);
@@ -1709,52 +641,51 @@ g0c_tc_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __hal
       }
     }
     tc::fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) tc::mbar_arrive(a_ready);
     if (amax) {
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) fmax_abs = fmaxf(fmax_abs, __shfl_xor_sync(0xffffffffu, fmax_abs, o));
       if (lane == 0) atomicMax(amax, __float_as_uint(fmax_abs));       // non-negative floats order like their bit patterns
     }
 #pragma unroll
-    for (int r = 0; r < kResC; ++r) {
+    for (int r = 0; r < RES; ++r) {
       const float tot = s4acc[r] + __shfl_xor_sync(0xffffffffu, s4acc[r], 1);
-      if (live && half == 0) S4[(size_t)(m0 + row) * kResC + r] = tot;
-    }
-    const int sub = warp & 3, ch = warp >> 2;
-    const int m = m0 + sub * 32 + lane;
-#pragma unroll 1
-    for (int nt = 0; nt < kG0NT; ++nt) {
-      const int buf = nt & 1;
-      tc::mbar_wait(&acc_full[buf], (nt >> 1) & 1);
-      __syncwarp();
-      tc::tcgen05_fence_after();
-      __half* grow = G + (size_t)(m < M ? m : 0) * kL0 + nt * kG0TileN + ch * 128;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t r[32];
-        tc::tmem_ld32(tbase + ((uint32_t)(sub * 32) << 16) + buf * kG0TileN + ch * 128 + c * 32, r);
-        tc::tmem_ld_wait();
-        if (m < M) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 pk;
-            pk.x = tc::pack_half2(__uint_as_float(r[8 * q + 0]), __uint_as_float(r[8 * q + 1]));
-            pk.y = tc::pack_half2(__uint_as_float(r[8 * q + 2]), __uint_as_float(r[8 * q + 3]));
-            pk.z = tc::pack_half2(__uint_as_float(r[8 * q + 4]), __uint_as_float(r[8 * q + 5]));
-            pk.w = tc::pack_half2(__uint_as_float(r[8 * q + 6]), __uint_as_float(r[8 * q + 7]));
-            *reinterpret_cast<uint4*>(grow + c * 32 + q * 8) = pk;
-          }
-        }
-      }
-      tc::tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) tc::mbar_arrive(&acc_free[buf]);
+      if (live && half == 0) S4[(size_t)(m0 + row) * RES + r] = tot;
     }
   }
-  tc::tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 8) tc::tmem_dealloc(tbase, 512);
+  tc::bar_sync(1, kConsumers);
+  // ---- MMAs + epilogue: warpgroup wg owns rows [64 wg, 64 wg + 64) of the CTA's 128
+  const int wg = tid >> 7, wl = warp & 3;
+  const int r0 = 16 * wl + (lane >> 2), cq = 2 * (lane & 3);
+  const uint32_t a_base = tc::smem_u32(sA) + wg * 8192, b_base = tc::smem_u32(sB);
+#pragma unroll 1
+  for (int nt = 0; nt < kG0NT; ++nt) {
+    float acc[128];
+#pragma unroll
+    for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+    tc::wgmma_fence();
+#pragma unroll 1
+    for (int kb = 0; kb < KB; ++kb) {
+      const int s = nt * KB + kb, slot = s % kG0Stages;
+      tc::mbar_wait(&b_full[slot], (s / kG0Stages) & 1);
+      const uint64_t da = tc::make_wdesc_sw128(a_base + kb * 16384, 1024), db = tc::make_wdesc_sw128(b_base + slot * 32768, 1024);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
+      tc::wgmma_commit();
+      tc::wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) tc::mbar_arrive(&b_empty[slot]);
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = m0 + 64 * wg + r0 + 8 * h;
+      if (m < M) {
+        __half* grow = G + (size_t)m * kL0 + nt * kG0TileN + cq;
+#pragma unroll
+        for (int j = 0; j < 32; ++j)
+          *reinterpret_cast<uint32_t*>(grow + 8 * j) = tc::pack_half2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
+    }
+  }
 }
 
 // --------------------------------------------------------------------------------------------------------------------
@@ -1772,29 +703,44 @@ void pack_tile(uint8_t* dst, const float* W, int cin, int row0, int nrows, int c
     }
 }
 
-bool shape_supported(const mp_mlp* m) {
-  if (m->n_layers != 5 || !m->skip) return false;
-  const int want[5] = {257, 1024, 512, 256, 128};
+// the head's feature channels when one of the two shipped shapes, else 0
+int head_channels(const mp_mlp* m) {
+  if (m->n_layers != 5 || !m->skip) return 0;
+  const int C = m->channels[0] - 1;
+  if (C != 256 && C != 512) return 0;
+  const int want[5] = {C + 1, kL0, kL1, kL2, kL3};
   for (int l = 0; l < 5; ++l)
-    if (m->channels[l] != want[l]) return false;
-  return m->channels[5] >= 1 && m->channels[5] <= kMaxRes;
+    if (m->channels[l] != want[l]) return 0;
+  return m->channels[5] == (C == 256 ? Prog<256>::RES : Prog<512>::RES) ? C : 0;
 }
 
-bool colour_shape(const mp_mlp* m) {
-  if (m->n_layers != 5 || !m->skip) return false;
-  const int want[6] = {kCc + 1, 1024, 512, 256, 128, kResC};
-  for (int l = 0; l <= 5; ++l)
-    if (m->channels[l] != want[l]) return false;
-  return true;
+// weight stream of one tile in the order query_wg_kernel<C> takes it (see Prog)
+template <int C>
+std::vector<uint8_t> build_stream(const std::vector<std::vector<float>>& W, const mp_mlp* mlp) {
+  using P = Prog<C>;
+  std::vector<uint8_t> out((size_t)P::StagesPerTile * kStageBytes, 0);
+  size_t st = 0;
+  auto stage_ptr = [&]() { return out.data() + (st++) * kStageBytes; };
+  const int cin1 = mlp->cin[1], cin2 = mlp->cin[2], cin3 = mlp->cin[3];
+  for (int kb = 0; kb < 16 + P::XKB; ++kb)                  // L1: H0, then X (the z column is applied in the epilogue)
+    for (int nh = 0; nh < 2; ++nh) pack_tile(stage_ptr(), W[1].data(), cin1, nh * 256, 256, kb * 64);
+  for (int kb = 0; kb < 8 + P::XKB; ++kb) pack_tile(stage_ptr(), W[2].data(), cin2, 0, 256, kb * 64);     // L2: H1, then X
+  for (int pass = 0; pass < P::L3Pass; ++pass)              // L3: X, then H2; colour: hi(W3), then lo(W3)
+    for (int q = 0; q < (P::XKB + 4) / 2; ++q) {
+      uint8_t* p = stage_ptr();
+      for (int sub = 0; sub < 2; ++sub) {
+        const int kb = 2 * q + sub;
+        const int col0 = kb < P::XKB ? kL2 + kb * 64 : (kb - P::XKB) * 64;
+        pack_tile(p + sub * 16384, W[3].data(), cin3, 0, 128, col0, pass == 1);
+      }
+    }
+  if ((int)st != P::StagesPerTile) out.clear();
+  return out;
 }
 
-// weight stream / side vectors of the colour head, in the order query_tc3c_kernel consumes them
-int tc_prepare_colour(mp_mlp* mlp) {
-  int dev = 0, major = 0, max_smem = 0;
-  MP_CUDA(cudaGetDevice(&dev));
-  MP_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  MP_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  if (major != 10 || max_smem < Smem::Total + 1024) return MP_OK;
+template <int C>
+int tc_prepare(mp_mlp* mlp) {
+  using P = Prog<C>;
   std::vector<std::vector<float>> W(5), Bv(5);
   for (int l = 0; l < 5; ++l) {
     W[l].resize((size_t)mlp->cin[l] * mlp->cout[l]);
@@ -1802,58 +748,34 @@ int tc_prepare_colour(mp_mlp* mlp) {
     MP_CUDA(cudaMemcpy(W[l].data(), mlp->w[l], W[l].size() * sizeof(float), cudaMemcpyDeviceToHost));
     MP_CUDA(cudaMemcpy(Bv[l].data(), mlp->bias[l], Bv[l].size() * sizeof(float), cudaMemcpyDeviceToHost));
   }
-  const int cin1 = mlp->cin[1], cin2 = mlp->cin[2], cin3 = mlp->cin[3];
-  std::vector<uint8_t> stream((size_t)kStagesPerTileC * 32768, 0);
-  size_t st = 0;
-  auto stage_ptr = [&]() { return stream.data() + (st++) * 32768; };
-  for (int c = 0; c < 8; ++c)                                               // L1 hidden
-    for (int kb = 0; kb < 2; ++kb)
-      for (int nh = 0; nh < 2; ++nh) pack_tile(stage_ptr(), W[1].data(), cin1, nh * 256, 256, c * 128 + kb * 64);
-  for (int ph = 0; ph < 2; ++ph)                                            // L1 skip: phase A, phase B
-    for (int kb = 0; kb < 4; ++kb)
-      for (int nh = 0; nh < 2; ++nh) pack_tile(stage_ptr(), W[1].data(), cin1, nh * 256, 256, kL0 + ph * 256 + kb * 64);
-  for (int kb = 0; kb < 8; ++kb) pack_tile(stage_ptr(), W[2].data(), cin2, 0, 256, kb * 64);     // L2 hidden
-  for (int ph = 1; ph >= 0; --ph)                                           // L2 skip: phase B, phase A
-    for (int kb = 0; kb < 4; ++kb) pack_tile(stage_ptr(), W[2].data(), cin2, 0, 256, kL1 + ph * 256 + kb * 64);
-  for (int ph = 0; ph < 2; ++ph)                                            // L3 skip: phase A, phase B; each hi(W3), then lo(W3)
-    for (int part = 0; part < 2; ++part)
-      for (int s2 = 0; s2 < 2; ++s2) {
-        uint8_t* p = stage_ptr();
-        pack_tile(p, W[3].data(), cin3, 0, 128, kL2 + ph * 256 + (2 * s2) * 64, part == 1);
-        pack_tile(p + 16384, W[3].data(), cin3, 0, 128, kL2 + ph * 256 + (2 * s2 + 1) * 64, part == 1);
-      }
-  for (int part = 0; part < 2; ++part)                                      // L3 hidden: hi(W3), then lo(W3)
-    for (int s2 = 0; s2 < 2; ++s2) {
-      uint8_t* p = stage_ptr();
-      pack_tile(p, W[3].data(), cin3, 0, 128, (2 * s2) * 64, part == 1);
-      pack_tile(p + 16384, W[3].data(), cin3, 0, 128, (2 * s2 + 1) * 64, part == 1);
-    }
-  if ((int)st != kStagesPerTileC) {
-    mp_set_error("internal: colour weight stream stage count mismatch");
+  const std::vector<uint8_t> stream = build_stream<C>(W, mlp);
+  if (stream.empty()) {
+    mp_set_error("internal: weight stream stage count mismatch");
     return MP_E_INVALID;
   }
   TcPack* pk = new TcPack();
   memset(pk, 0, sizeof(*pk));
-  pk->res = kResC;
-  pk->kind = 1;
+  pk->res = P::RES;
+  pk->kind = C == 256 ? 0 : 1;
   mlp->tc = pk;
   auto upload = [&](const void* src, size_t bytes, void** dptr) -> cudaError_t {
     cudaError_t e = cudaMalloc(dptr, bytes);
     if (e != cudaSuccess) return e;
     return cudaMemcpy(*dptr, src, bytes, cudaMemcpyHostToDevice);
   };
-  cudaError_t e = upload(stream.data(), stream.size(), (void**)&pk->w3stream);
-  if (e == cudaSuccess) {   // feature part of layer 0 as fp16 SWIZZLE_128B tiles [n tile 4][K block 8][256 x 64]
-    std::vector<uint8_t> w0t((size_t)kG0NT * kG0cKB * 32768);
+  cudaError_t e = upload(stream.data(), stream.size(), (void**)&pk->wstream);
+  if (e == cudaSuccess) {   // feature part of layer 0 as fp16 SWIZZLE_128B tiles, operand of the per-texel G0 GEMM
+    constexpr int KB = G0Cfg<C>::KB;
+    std::vector<uint8_t> w0t((size_t)kG0NT * KB * 32768);
     for (int nt = 0; nt < kG0NT; ++nt)
-      for (int kb = 0; kb < kG0cKB; ++kb)
-        pack_tile(w0t.data() + ((size_t)nt * kG0cKB + kb) * 32768, W[0].data(), mlp->cin[0], nt * kG0TileN, kG0TileN, kb * 64);
+      for (int kb = 0; kb < KB; ++kb)
+        pack_tile(w0t.data() + ((size_t)nt * KB + kb) * 32768, W[0].data(), mlp->cin[0], nt * kG0TileN, kG0TileN, kb * 64);
     e = upload(w0t.data(), w0t.size(), (void**)&pk->d_w0t);
   }
   const int hid[4] = {0, kL0, kL1, kL2};
   for (int l = 0; l < 4 && e == cudaSuccess; ++l) {
     std::vector<float> wz(mlp->cout[l]);
-    const int zcol = hid[l] + kCc;
+    const int zcol = hid[l] + C;
     for (int co = 0; co < mlp->cout[l]; ++co) wz[co] = W[l][(size_t)co * mlp->cin[l] + zcol];
     memcpy(pk->h_bias + side_off(l), Bv[l].data(), Bv[l].size() * sizeof(float));
     memcpy(pk->h_wz + side_off(l), wz.data(), wz.size() * sizeof(float));
@@ -1865,22 +787,23 @@ int tc_prepare_colour(mp_mlp* mlp) {
     }
   }
   if (e == cudaSuccess) {
-    const int cin4 = mlp->cin[4];
-    std::vector<float> w4h((size_t)kResC * kL3), w4s((size_t)kResC * kCc), w4z(kResC);
-    for (int r = 0; r < kResC; ++r) {
+    const int R = P::RES, cin4 = mlp->cin[4];
+    std::vector<float> w4h((size_t)R * kL3), w4s((size_t)R * C), w4z(R);
+    for (int r = 0; r < R; ++r) {
       for (int j = 0; j < kL3; ++j) w4h[(size_t)r * kL3 + j] = W[4][(size_t)r * cin4 + j];
-      for (int j = 0; j < kCc; ++j) w4s[(size_t)r * kCc + j] = W[4][(size_t)r * cin4 + kL3 + j];
-      w4z[r] = W[4][(size_t)r * cin4 + kL3 + kCc];
+      for (int j = 0; j < C; ++j) w4s[(size_t)r * C + j] = W[4][(size_t)r * cin4 + kL3 + j];
+      w4z[r] = W[4][(size_t)r * cin4 + kL3 + C];
     }
     e = upload(w4h.data(), w4h.size() * sizeof(float), (void**)&pk->w4h);
     if (e == cudaSuccess) e = upload(w4s.data(), w4s.size() * sizeof(float), (void**)&pk->w4s);
     if (e == cudaSuccess) e = upload(w4z.data(), w4z.size() * sizeof(float), (void**)&pk->w4z);
     if (e == cudaSuccess) e = upload(Bv[4].data(), Bv[4].size() * sizeof(float), (void**)&pk->b4);
   }
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_tc3c_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem::Total + 1024);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(g0c_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kG0cSmem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(g0_wg_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G0Cfg<C>::Smem);
   if (e != cudaSuccess) {
-    mp_set_error("tc_prepare_colour: %s", cudaGetErrorString(e));
+    mp_set_error("mp_tc_prepare: %s", cudaGetErrorString(e));
     mp_tc_release(mlp);
     return MP_E_CUDA;
   }
@@ -1888,38 +811,33 @@ int tc_prepare_colour(mp_mlp* mlp) {
   return MP_OK;
 }
 
-int launch_colour(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
-                  cudaStream_t st, const MpSurfaceSrc* surf_in = nullptr, int guard = MP_GUARD_NONE) {
-  MpSurfaceSrc surf;
-  memset(&surf, 0, sizeof(surf));
-  if (surf_in) surf = *surf_in;
+// per-frame per-texel products of the head (G0, the fp16 copy of the map, S4), then the fused query
+template <int C>
+int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
+           cudaStream_t st, const MpSurfaceSrc& surf, int guard) {
+  using P = Prog<C>;
   const long long HW = (long long)feat->H * feat->W;
-  if (feat->C != kCc || HW > 65536) {
-    mp_set_error("colour head: needs a %d-channel map of at most 65536 texels (got %d channels, %lld texels)", kCc, feat->C, HW);
-    return MP_E_INVALID;
-  }
-  if (dst.scatter_vol || dst.n_peers > 0 || (!dst.out && !surf.canvas)) {
-    mp_set_error("colour head: [3,N] output or surface canvas only");
-    return MP_E_UNSUPPORTED;
-  }
-  if (!feat->g0) {
+  if (!feat->g0 || feat->g0_n != kL0) {     // (a map has one channel count, so it serves one of the two heads)
+    if (feat->g0) cudaFree(feat->g0);
+    feat->g0 = nullptr;
     MP_CUDA(cudaMalloc(&feat->g0, (size_t)HW * kL0 * sizeof(__half)));
-    if (!feat->f16) MP_CUDA(cudaMalloc(&feat->f16, (size_t)HW * kCc * sizeof(__half)));
-    if (!feat->s4tex) MP_CUDA(cudaMalloc(&feat->s4tex, (size_t)HW * kResC * sizeof(float)));
+    if (!feat->f16) MP_CUDA(cudaMalloc(&feat->f16, (size_t)HW * C * sizeof(__half)));
+    if (!feat->s4tex) MP_CUDA(cudaMalloc(&feat->s4tex, (size_t)HW * P::RES * sizeof(float)));
     feat->g0_n = kL0;
     feat->g0_owner = 0;
   }
   if (feat->g0_owner != mlp->gen || feat->g0_version != feat->version) {
 #ifndef MP_CUDA_EMU
-    g0c_tc_kernel<<<(unsigned)((HW + 127) / 128), kG0Threads, kG0cSmem, st>>>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, feat->amax);
+    g0_wg_kernel<C><<<(unsigned)((HW + 127) / 128), kThreads, G0Cfg<C>::Smem, st>>>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16,
+                                                                                   feat->s4tex, pk->w4s, feat->amax);
 #else
-    MP_EMU_LAUNCH((unsigned)((HW + 127) / 128), kG0Threads, g0c_tc_kernel(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, feat->amax));
+    MP_EMU_LAUNCH((unsigned)((HW + 127) / 128), kThreads, g0_wg_kernel<C>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, feat->amax));
 #endif
     MP_CUDA(cudaGetLastError());
     feat->g0_owner = mlp->gen;
     feat->g0_version = feat->version;
   }
-  if (surf_in && isfinite(mlp->tc_amax_limit)) {
+  if (surf.X && isfinite(mlp->tc_amax_limit)) {
     // the fused rendering has no exact-kernel twin: check the frame's feature range on the host (one 4-byte read-back per
     // frame) and let the caller take the unfused path when it is outside the validated range
     unsigned bits = 0;
@@ -1935,28 +853,29 @@ int launch_colour(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPo
   TcParams prm;
   memset(&prm, 0, sizeof(prm));
   prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
-  prm.wstream = pk->w3stream;
+  prm.wstream = pk->wstream;
   memcpy(prm.bias_all, pk->h_bias, sizeof(prm.bias_all));
   memcpy(prm.wz_all, pk->h_wz, sizeof(prm.wz_all));
   prm.w4h = pk->w4h; prm.w4s = pk->w4s; prm.w4z = pk->w4z; prm.b4 = pk->b4;
   prm.res = pk->res;
   prm.last_op = mlp->last_op;
   prm.H = feat->H; prm.W = feat->W;
-  prm.feat32 = feat->nhwc32;
   prm.g0 = feat->g0;
   prm.feat16 = feat->f16;
   prm.s4tex = feat->s4tex;
   prm.d_bias0 = pk->d_bias0;
   prm.d_wz0 = pk->d_wz0;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   MP_CUDA(cudaGetDevice(&dev));
   MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   const long long tiles = (src.n + kTile - 1) / kTile;
   const int grid = (int)(tiles < (long long)sms ? tiles : sms);
 #ifndef MP_CUDA_EMU
-  query_tc3c_kernel<<<grid, kThreads, Smem::Total + 1024, st>>>(prm, src, cal, dst, surf);
+  if (dst.n_peers > 0) query_wg_kernel<C, true><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf);      // fused slab exchange
+  else query_wg_kernel<C, false><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf);
 #else
-  MP_EMU_LAUNCH(grid, kThreads, query_tc3c_kernel(prm, src, cal, dst, surf));
+  if (dst.n_peers > 0) MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, true>(prm, src, cal, dst, surf)));
+  else MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, false>(prm, src, cal, dst, surf)));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -1967,167 +886,24 @@ int launch_colour(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPo
 int mp_tc_prepare(mp_mlp* mlp) {
   mlp->tc = nullptr;
   mlp->tc_ok = 0;
-  if (colour_shape(mlp)) return tc_prepare_colour(mlp);     // tcgen05 program of the colour head (validated on B200, round 2)
-  if (!shape_supported(mlp)) return MP_OK;
+  const int C = head_channels(mlp);
+  if (!C) return MP_OK;
   int dev = 0, major = 0, max_smem = 0;
   MP_CUDA(cudaGetDevice(&dev));
   MP_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   MP_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  if (major != 10 || max_smem < Smem::Total + 1024) return MP_OK;     // tcgen05 is sm_100-family only
-
-  // pull the fp32 weights back to the host and repack
-  std::vector<std::vector<float>> W(5), Bv(5);
-  for (int l = 0; l < 5; ++l) {
-    W[l].resize((size_t)mlp->cin[l] * mlp->cout[l]);
-    Bv[l].resize(mlp->cout[l]);
-    MP_CUDA(cudaMemcpy(W[l].data(), mlp->w[l], W[l].size() * sizeof(float), cudaMemcpyDeviceToHost));
-    MP_CUDA(cudaMemcpy(Bv[l].data(), mlp->bias[l], Bv[l].size() * sizeof(float), cudaMemcpyDeviceToHost));
-  }
-  // v3 program (layer 0 hoisted): layer 1 over all 512 outputs as two 256-row tiles per K-block, then layers 2, 3
-  // cg = 1: 32 KB stages holding whole tiles; cg = 2 (CTA pair): 16 KB stages holding rank r's half of the rows of every
-  // tile (tcgen05.mma.cta_group::2 reads B rows [r*N/2, (r+1)*N/2) from CTA r)
-  auto build_stream3 = [&](int cg, int r, std::vector<uint8_t>& out) -> bool {
-    const int stage_bytes = 32768 / cg, sub = stage_bytes / 2;
-    out.assign((size_t)kStagesPerTile3 * stage_bytes, 0);
-    size_t st = 0;
-    auto stage_ptr = [&]() { return out.data() + (st++) * stage_bytes; };
-    const int n128 = 128 / cg, n256 = 256 / cg;
-    const int cin1 = mlp->cin[1], cin2 = mlp->cin[2], cin3 = mlp->cin[3];
-    for (int c = 0; c < 8; ++c)
-      for (int kb = 0; kb < 2; ++kb)
-        for (int nh = 0; nh < 2; ++nh) pack_tile(stage_ptr(), W[1].data(), cin1, nh * 256 + r * n256, n256, c * 128 + kb * 64);
-    for (int kb = 0; kb < 4; ++kb)
-      for (int nh = 0; nh < 2; ++nh) pack_tile(stage_ptr(), W[1].data(), cin1, nh * 256 + r * n256, n256, kL0 + kb * 64);
-    for (int kb = 0; kb < 8; ++kb) pack_tile(stage_ptr(), W[2].data(), cin2, r * n256, n256, kb * 64);
-    for (int kb = 0; kb < 4; ++kb) pack_tile(stage_ptr(), W[2].data(), cin2, r * n256, n256, kL1 + kb * 64);
-    for (int s2 = 0; s2 < 2; ++s2) {
-      uint8_t* p = stage_ptr();
-      pack_tile(p, W[3].data(), cin3, r * n128, n128, kL2 + (2 * s2) * 64);
-      pack_tile(p + sub, W[3].data(), cin3, r * n128, n128, kL2 + (2 * s2 + 1) * 64);
-    }
-    for (int s2 = 0; s2 < 2; ++s2) {
-      uint8_t* p = stage_ptr();
-      pack_tile(p, W[3].data(), cin3, r * n128, n128, (2 * s2) * 64);
-      pack_tile(p + sub, W[3].data(), cin3, r * n128, n128, (2 * s2 + 1) * 64);
-    }
-    return (int)st == kStagesPerTile3;
-  };
-  std::vector<uint8_t> s3, s3p[2];
-  if (!build_stream3(1, 0, s3) || !build_stream3(2, 0, s3p[0]) || !build_stream3(2, 1, s3p[1])) {
-    mp_set_error("internal: v3 weight stream stage count mismatch");
-    return MP_E_INVALID;
-  }
-
-  TcPack* pk = new TcPack();
-  memset(pk, 0, sizeof(*pk));
-  pk->res = mlp->channels[5];
-  auto upload = [&](const void* src, size_t bytes, void** dptr) -> cudaError_t {
-    cudaError_t e = cudaMalloc(dptr, bytes);
-    if (e != cudaSuccess) return e;
-    return cudaMemcpy(*dptr, src, bytes, cudaMemcpyHostToDevice);
-  };
-  cudaError_t e = upload(s3.data(), s3.size(), (void**)&pk->w3stream);
-  for (int r = 0; r < 2 && e == cudaSuccess; ++r) e = upload(s3p[r].data(), s3p[r].size(), (void**)&pk->w3pair[r]);
-#ifdef MP_CUDA_EMU
-  // (the CPU model's "tensor map" is the base pointer of the [rows][64 fp16] array, see tests/emu/tc_ptx_emu.h)
-  if (e == cudaSuccess) {
-    pk->pair_ok = 1;
-    for (int r = 0; r < 2; ++r) memcpy(&pk->tmap_pair[r], &pk->w3pair[r], sizeof(void*));
-  }
-#else
-  if (e == cudaSuccess) {
-    // tensor maps over the two half streams: [rows][64 fp16] with 128-byte rows, box = one 16 KB stage (the tiles are
-    // stored pre-swizzled, so the copy itself is a plain 2-D box: no swizzle, no interleave)
-    typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-    EncodeFn encode = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", (void**)&encode, cudaEnableDefault, &qres) == cudaSuccess && encode) {
-      pk->pair_ok = 1;
-      for (int r = 0; r < 2; ++r) {
-        const cuuint64_t gdim[2] = {64, (cuuint64_t)kStagesPerTile3 * 128};
-        const cuuint64_t gstr[1] = {128};
-        const cuuint32_t box[2] = {64, 128};
-        const cuuint32_t estr[2] = {1, 1};
-        if (encode(&pk->tmap_pair[r], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, pk->w3pair[r], gdim, gstr, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-          pk->pair_ok = 0;
-      }
-    }
-  }
-#endif
-  {   // feature part of layer 0 as fp16 SWIZZLE_128B tiles, operand of the per-texel G0 GEMM
-    if (e == cudaSuccess) {
-      std::vector<uint8_t> w0t((size_t)(kL0 / kG0TileN) * 4 * 32768);
-      for (int nt = 0; nt < kL0 / kG0TileN; ++nt)
-        for (int kb = 0; kb < 4; ++kb) pack_tile(w0t.data() + ((size_t)nt * 4 + kb) * 32768, W[0].data(), mlp->cin[0], nt * kG0TileN, kG0TileN, kb * 64);
-      e = upload(w0t.data(), w0t.size(), (void**)&pk->d_w0t);
-    }
-  }
-  const int hid[4] = {0, kL0, kL1, kL2};
-  for (int l = 0; l < 4 && e == cudaSuccess; ++l) {
-    std::vector<float> wz(mlp->cout[l]);
-    const int zcol = hid[l] + kC;
-    for (int co = 0; co < mlp->cout[l]; ++co) wz[co] = W[l][(size_t)co * mlp->cin[l] + zcol];
-    memcpy(pk->h_bias + side_off(l), Bv[l].data(), Bv[l].size() * sizeof(float));
-    memcpy(pk->h_wz + side_off(l), wz.data(), wz.size() * sizeof(float));
-    if (l == 0) {
-      std::vector<__half> b0h(Bv[0].size()), wz0h(wz.size());
-      for (size_t i = 0; i < b0h.size(); ++i) { b0h[i] = __float2half_rn(Bv[0][i]); wz0h[i] = __float2half_rn(wz[i]); }
-      e = upload(b0h.data(), b0h.size() * sizeof(__half), (void**)&pk->d_bias0);
-      if (e == cudaSuccess) e = upload(wz0h.data(), wz0h.size() * sizeof(__half), (void**)&pk->d_wz0);
-    }
-  }
-  if (e == cudaSuccess) {
-    const int R = pk->res, cin4 = mlp->cin[4];
-    std::vector<float> w4h((size_t)R * kL3), w4s((size_t)R * kC), w4z(R);
-    for (int r = 0; r < R; ++r) {
-      for (int j = 0; j < kL3; ++j) w4h[(size_t)r * kL3 + j] = W[4][(size_t)r * cin4 + j];
-      for (int j = 0; j < kC; ++j) w4s[(size_t)r * kC + j] = W[4][(size_t)r * cin4 + kL3 + j];
-      w4z[r] = W[4][(size_t)r * cin4 + kL3 + kC];
-    }
-    e = upload(w4h.data(), w4h.size() * sizeof(float), (void**)&pk->w4h);
-    if (e == cudaSuccess) e = upload(w4s.data(), w4s.size() * sizeof(float), (void**)&pk->w4s);
-    if (e == cudaSuccess) e = upload(w4z.data(), w4z.size() * sizeof(float), (void**)&pk->w4z);
-    if (e == cudaSuccess) e = upload(Bv[4].data(), Bv[4].size() * sizeof(float), (void**)&pk->b4);
-  }
-  mlp->tc = pk;
-  if (e != cudaSuccess) {
-    mp_set_error("mp_tc_prepare: %s", cudaGetErrorString(e));
-    mp_tc_release(mlp);
-    return MP_E_CUDA;
-  }
-  e = cudaFuncSetAttribute(query_tc3_kernel<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem::Total + 1024);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_tc3_kernel<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem::Total + 1024);
-#ifndef MP_CUDA_EMU
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_tc3_kernel<false, 1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem::Total + 1024);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_tc3_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem::Total + 1024);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_tc3_kernel<false, 1, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, Smem::Total + 1024);
-#endif
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(g0_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kG0Smem);
-  if (e != cudaSuccess) {
-    mp_set_error("mp_tc_prepare: cannot opt in to %d bytes of shared memory: %s", Smem::Total + 1024, cudaGetErrorString(e));
-    mp_tc_release(mlp);
-    return MP_E_CUDA;
-  }
-  mlp->tc_ok = 1;
-  return MP_OK;
+  // wgmma is sm_90a only (the library is built for exactly that target)
+  if (major != 9 || max_smem < (C == 256 ? Prog<256>::Total : Prog<512>::Total) + 1024) return MP_OK;
+  return C == 256 ? tc_prepare<256>(mlp) : tc_prepare<512>(mlp);
 }
 
 void mp_tc_release(mp_mlp* mlp) {
   TcPack* pk = static_cast<TcPack*>(mlp->tc);
   if (!pk) return;
-  if (pk->w3stream) cudaFree(pk->w3stream);
-  for (int r = 0; r < 2; ++r) if (pk->w3pair[r]) cudaFree(pk->w3pair[r]);
+  if (pk->wstream) cudaFree(pk->wstream);
   if (pk->d_bias0) cudaFree(pk->d_bias0);
   if (pk->d_wz0) cudaFree(pk->d_wz0);
   if (pk->d_w0t) cudaFree(pk->d_w0t);
-  for (int l = 0; l < 4; ++l) {
-    if (pk->bias[l]) cudaFree(pk->bias[l]);
-    if (pk->wz[l]) cudaFree(pk->wz[l]);
-  }
   if (pk->w4h) cudaFree(pk->w4h);
   if (pk->w4s) cudaFree(pk->w4s);
   if (pk->w4z) cudaFree(pk->w4z);
@@ -2142,8 +918,12 @@ int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* 
   if (n <= 0) return MP_OK;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
   if (!pk || !mlp->tc_ok || pk->kind != 1) {
-    mp_set_error("fused surface colourisation needs the tensor-core program of the colour head (MONOPORT_B200_TC_NETC=1)");
+    mp_set_error("fused surface colourisation needs the tensor-core program of the colour head");
     return MP_E_UNSUPPORTED;
+  }
+  if (feat->C != 512 || (long long)feat->H * feat->W > 65536) {
+    mp_set_error("colour head: needs a 512-channel map of at most 65536 texels (got %d channels, %d x %d)", feat->C, feat->H, feat->W);
+    return MP_E_INVALID;
   }
   MpSurfaceSrc surf;
   memset(&surf, 0, sizeof(surf));
@@ -2161,7 +941,7 @@ int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* 
   src.n = n;
   MpOutDst dst;
   dst.out = nullptr; dst.ld = 0; dst.scatter_vol = nullptr;
-  return launch_colour(mlp, pk, feat, src, cal, dst, st, &surf);
+  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, MP_GUARD_NONE);
 }
 
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
@@ -2169,181 +949,27 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
   if (src.n <= 0) return MP_OK;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
   if (!pk || !mlp->tc_ok) {
-    mp_set_error("tcgen05 path not prepared for this head");
+    mp_set_error("tensor-core path not prepared for this head");
     return MP_E_UNSUPPORTED;
   }
-  if (pk->kind == 1) return launch_colour(mlp, pk, feat, src, cal, dst, st, nullptr, guard);
-  if (feat->C != kC) {
+  const int C = pk->kind == 1 ? 512 : 256;
+  if (feat->C != C) {
     mp_set_error("head expects %d input channels but the feature map has %d (+1 depth)", mlp->channels[0], feat->C);
     return MP_E_INVALID;
   }
-  const long long HW = (long long)feat->H * feat->W;
-  if (HW > 65536) {      // texel indices travel as 16-bit pairs in registers
+  if ((long long)feat->H * feat->W > 65536) {      // texel indices travel as 16-bit pairs in registers
     mp_set_error("the tensor-core program handles feature maps of at most 65536 texels (got %d x %d); use MP_MODE_FP32", feat->H, feat->W);
     return MP_E_UNSUPPORTED;
   }
-  TcParams prm;
-  memset(&prm, 0, sizeof(prm));
-  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
-  memcpy(prm.bias_all, pk->h_bias, sizeof(prm.bias_all));
-  memcpy(prm.wz_all, pk->h_wz, sizeof(prm.wz_all));
-  prm.w4h = pk->w4h; prm.w4s = pk->w4s; prm.w4z = pk->w4z; prm.b4 = pk->b4;
-  prm.res = pk->res;
-  prm.last_op = mlp->last_op;
-  prm.H = feat->H; prm.W = feat->W;
-  prm.feat32 = feat->nhwc32;
-  int dev = 0, sms = 148;
-  MP_CUDA(cudaGetDevice(&dev));
-  MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const long long tiles = (src.n + kTile - 1) / kTile;
-  static const int do_prof = [] { const char* v = getenv("MONOPORT_B200_TC_PROF"); return v ? atoi(v) : 0; }();
-  unsigned long long* d_prof = nullptr;
-  if (do_prof && (tiles >= 2 * sms || do_prof >= 2)) {        // (=2: also launches of a wave or less)
-    MP_CUDA(cudaMalloc(&d_prof, (size_t)sms * 32 * sizeof(unsigned long long)));
-    MP_CUDA(cudaMemset(d_prof, 0, (size_t)sms * 32 * sizeof(unsigned long long)));
-    prm.prof = d_prof;
-  }
-  static const int exp_mask = [] { const char* v = getenv("MONOPORT_B200_TC_EXP"); return v ? atoi(v) : 0; }();
-  prm.exp = exp_mask;
-  static const int do_trace = [] { const char* v = getenv("MONOPORT_B200_TC_TRACE"); return v ? atoi(v) : 0; }();
-  unsigned long long* d_trace = nullptr;
-  if (do_trace && !d_prof && tiles >= (long long)(kTraceTile + 2) * sms) {
-    MP_CUDA(cudaMalloc(&d_trace, 128 * sizeof(unsigned long long)));
-    MP_CUDA(cudaMemset(d_trace, 0, 128 * sizeof(unsigned long long)));
-    prm.trace = d_trace;
-  }
-  auto report = [&](int grid) {
-    if (d_trace) {
-      cudaStreamSynchronize(st);
-      unsigned long long h[128];
-      cudaMemcpy(h, d_trace, sizeof(h), cudaMemcpyDeviceToHost);
-      cudaFree(d_trace);
-      unsigned long long t0 = ~0ull;
-      for (int k = 0; k < 128; ++k) if (h[k] && h[k] < t0) t0 = h[k];
-      for (int k = 0; k < 128; ++k) if (h[k]) fprintf(stderr, "[tc trace] %3d %8llu\n", k, h[k] - t0);
-      return;
-    }
-    if (!d_prof) return;
-    cudaStreamSynchronize(st);
-    std::vector<unsigned long long> h((size_t)sms * 32);
-    cudaMemcpy(h.data(), d_prof, h.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
-    cudaFree(d_prof);
-    static const char* names[32] = {"total", "xready", 0, "wfull", 0, "h0ready", "acc1drained", "h1ready", "h2ready",
-                                    "ph_L1hid(32st)", "ph_L1skip(8st)", "ph_L2_TS(4st)", 0, 0, 0, 0, 0, 0, "w_h0free", "w_acc1full", "w_acc2full", "w_acc3full",
-                                    "w_drain0", "w_drain1", "w_drain2", "w_drain3", "w_xfree", 0, 0, 0, 0, 0};
-    const long long tiles_per_cta = (tiles + grid - 1) / grid;
-    fprintf(stderr, "[tc prof] grid=%d tiles/cta~%lld  (cycles per tile, CTA 0 | CTA 1)\n", grid, tiles_per_cta);
-    for (int k = 0; k < 32; ++k)
-      if (names[k]) fprintf(stderr, "[tc prof] %-12s %10.0f | %10.0f\n", names[k], (double)h[k] / tiles_per_cta, (double)h[32 + k] / tiles_per_cta);
-  };
-  // the per-frame per-texel products of this head: G0 (layer-0 pre-activation), the fp16 copy of the map, S4
-  if (!feat->g0 || feat->g0_n != kL0) {
-    if (feat->g0) cudaFree(feat->g0);
-    feat->g0 = nullptr;
-    MP_CUDA(cudaMalloc(&feat->g0, (size_t)HW * kL0 * sizeof(__half)));
-    if (!feat->f16) MP_CUDA(cudaMalloc(&feat->f16, (size_t)HW * kC * sizeof(__half)));
-    if (!feat->s4tex) MP_CUDA(cudaMalloc(&feat->s4tex, (size_t)HW * kMaxRes * sizeof(float)));
-    feat->g0_n = kL0;
-    feat->g0_owner = 0;
-  }
-  if (feat->g0_owner != mlp->gen || feat->g0_version != feat->version) {
-#ifndef MP_CUDA_EMU
-    g0_tc_kernel<<<(unsigned)((HW + 127) / 128), kG0Threads, kG0Smem, st>>>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, pk->res, feat->amax);
-#else
-    MP_EMU_LAUNCH((unsigned)((HW + 127) / 128), kG0Threads, g0_tc_kernel(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, pk->res, feat->amax));
-#endif
-    MP_CUDA(cudaGetLastError());
-    feat->g0_owner = mlp->gen;
-    feat->g0_version = feat->version;
-  }
-  prm.g0 = feat->g0;
-  prm.feat16 = feat->f16;
-  prm.s4tex = feat->s4tex;
-  prm.d_bias0 = pk->d_bias0;
-  prm.d_wz0 = pk->d_wz0;
-  prm.wstream = pk->w3stream;
   if (dst.n_peers > MP_MAX_PEERS) {
     mp_set_error("at most %d peer volumes", MP_MAX_PEERS);
     return MP_E_UNSUPPORTED;
   }
-  // One CTA per tile by default.  MONOPORT_B200_TC_CG=2 selects the CTA-pair kernel (validated: the whole GPU suite passes
-  // with it) -- same box, same run: 486 Mpoints/s against 498 (profiles/r02_call8_ab_issue_pattern_x_cta_group.txt).  The
-  // pair halves the weight bytes per SM, but a 2-CTA MMA runs at the same per-SM rate (tools/tc_rate.cu) and every operand
-  // hand-off and weight-stage release crosses the cluster, which costs more than the halved stream gains.
-  static const int forced_cg = [] { const char* v = getenv("MONOPORT_B200_TC_CG"); return v ? atoi(v) : 0; }();
-  if (pk->pair_ok && forced_cg == 2 && sms >= 2 && dst.n_peers == 0) {
-    prm.tmap_pair[0] = pk->tmap_pair[0];
-    prm.tmap_pair[1] = pk->tmap_pair[1];
-    const long long groups = (tiles + 1) / 2;
-    const long long max_pairs = sms / 2;
-    const int pairs = (int)(groups < max_pairs ? groups : max_pairs);
-#ifndef MP_CUDA_EMU
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(2 * pairs);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = Smem::Total + 1024;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    MP_CUDA(cudaLaunchKernelEx(&cfg, query_tc3_kernel<false, 2>, prm, src, cal, dst));
-#else
-    MP_EMU_LAUNCH_CLUSTER2(2 * pairs, kThreads, (query_tc3_kernel<false, 2>(prm, src, cal, dst)));
-#endif
-    report(2 * pairs);
-    return MP_OK;
+  if (C == 512 && (dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
+    mp_set_error("colour head: [3,N] output or surface canvas only");
+    return MP_E_UNSUPPORTED;
   }
-  // Weight multicast: the one-CTA program in 2-CTA clusters that share the weight stream (halves the L2 -> SM weight requests
-  // like the CTA pair above without touching the MMAs).  With the round-1..mid-round-2 issuer it lost 0.7 % (the coupled ring
-  // cost more cycles than the saved power bought back, profiles/r02_call14_wm_ab.txt); with the issuer at the pipe's rate the
-  // weight ring is what the issuer waits for, and the same box measures 569.5 / 565.5 against 556.7 / 559.0 Mpoints/s
-  // (CTA pair: 540.5 / 542.4; profiles/r02_call20_weight_halving_ab.txt).  Default for launches of several waves (a launch
-  // of a wave or less is bound by the latency of one tile, which the coupling can only lengthen);
-  // MONOPORT_B200_TC_WM=0 / 1 forces it off / on.
-  static const int forced_wm = [] { const char* v = getenv("MONOPORT_B200_TC_WM"); return v ? atoi(v) : -1; }();
-  // (node lists with a device-side count -- the coarse-to-fine levels -- are latency-bound whatever their capacity: plain launch,
-  // 259.1 vs 265.8 us of F1 per frame, profiles/r02_call27_*, r02_call22_*)
-  const bool use_wm = forced_wm == 1 || (forced_wm < 0 && tiles >= 4ll * sms && src.count_dev == nullptr);
-  if (use_wm && dst.n_peers == 0 && sms >= 2 && tiles >= 2 && !prm.prof && !prm.trace) {
-    const long long groups = (tiles + 1) / 2;
-    const long long max_pairs = sms / 2;
-    const int pairs = (int)(groups < max_pairs ? groups : max_pairs);
-#ifndef MP_CUDA_EMU
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3(2 * pairs);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = Smem::Total + 1024;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    MP_CUDA(cudaLaunchKernelEx(&cfg, query_tc3_kernel<false, 1, true>, prm, src, cal, dst));
-#else
-    MP_EMU_LAUNCH_CLUSTER2(2 * pairs, kThreads, (query_tc3_kernel<false, 1, true>(prm, src, cal, dst)));     // (the CPU model runs the two CTAs of a cluster side by side)
-#endif
-    report(2 * pairs);
-    return MP_OK;
-  }
-  const int grid = (int)(tiles < (long long)sms ? tiles : sms);
-#ifndef MP_CUDA_EMU
-  if (dst.n_peers > 0) query_tc3_kernel<true, 1><<<grid, kThreads, Smem::Total + 1024, st>>>(prm, src, cal, dst);      // fused slab exchange
-  else if (prm.prof || prm.trace) query_tc3_kernel<false, 1, false, true><<<grid, kThreads, Smem::Total + 1024, st>>>(prm, src, cal, dst);
-  else query_tc3_kernel<false, 1><<<grid, kThreads, Smem::Total + 1024, st>>>(prm, src, cal, dst);
-#else
-  if (dst.n_peers > 0) MP_EMU_LAUNCH(grid, kThreads, (query_tc3_kernel<true, 1>(prm, src, cal, dst)));
-  else MP_EMU_LAUNCH(grid, kThreads, (query_tc3_kernel<false, 1>(prm, src, cal, dst)));
-#endif
-  MP_CUDA(cudaGetLastError());
-  report(grid);
-  return MP_OK;
+  MpSurfaceSrc surf;
+  memset(&surf, 0, sizeof(surf));
+  return C == 256 ? launch<256>(mlp, pk, feat, src, cal, dst, st, surf, guard) : launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard);
 }

@@ -3,7 +3,7 @@
 result consumer RTL/recon.py:32-38).  PARITY UNPINNED against upstream (see DESIGN.md).
 
 All index/byte work (2x up-sampling, boundary+dilation, ordered compaction, scatter, conflict loop, top-k select)
-runs in the sm_100a kernels of csrc/octree.cu through the C-ABI.  Two drive modes, identical volumes:
+runs in the sm_90a kernels of csrc/octree.cu through the C-ABI.  Two drive modes, identical volumes:
   * generic : any Python `query_func(points=[1,N,3], **kwargs) -> [1,1,N]` is called back once per batch
               (stepping API: mp_octree_begin / next / commit / finish);
   * fused   : when `query_func` was built by `make_query_func(net)` (it then carries `__monoport_fused__`),

@@ -1,5 +1,5 @@
 """MonoPortNet with the reference's API (monoport/lib/modeling/MonoPortNet.py) whose eval-mode `query()` is ONE
-fused sm_100a kernel launch (project -> mask -> bilinear gather -> z-concat -> 5-layer skip MLP -> last_op -> mask)
+fused sm_90a kernel launch (project -> mask -> bilinear gather -> z-concat -> 5-layer skip MLP -> last_op -> mask)
 through the C-ABI of libmonoport_b200.  There is no PyTorch / CPU fallback for query(): CPU tensors or a missing
 library raise."""
 import ctypes
@@ -79,7 +79,7 @@ class MonoPortNet(nn.Module):
         self.surface_classifier = globals()[opt_net.head.IMF](opt_net.head)
         self.projection = globals()[opt_net.projection]
         self.normalizer = globals()[opt_net.normalizer.IMF](opt_net.normalizer)
-        # arithmetic of the fused kernel: "auto" (tcgen05 when supported), "tc" (= "tc_v3"), "fp32"
+        # arithmetic of the fused kernel: "auto" (tensor cores when supported), "tc" (= "tc_v3"), "fp32"
         self.precision = os.environ.get("MONOPORT_B200_MODE", "auto")
         # True: skip the per-call feature upload when the tensor's (address, version) are unchanged (see FeatureHandle.upload
         # for what that identity cannot see); default off -- every query()/query_grid()/engine call uploads its frame

@@ -1,7 +1,7 @@
 """Skip-MLP head: parameter container with the reference's state-dict layout
 (`filters.{l}.weight [Cout,Cin,1]`, `filters.{l}.bias`; heads/SurfaceClassifier.py:7-37) plus the binding to the
 packed-weight handle of the fused kernel.  In eval mode MonoPortNet.query never calls `forward`: the MLP runs
-inside the fused sm_100a kernel."""
+inside the fused sm_90a kernel."""
 import ctypes
 
 import torch

@@ -48,6 +48,29 @@ def make_feat(C, H, W, seed, scale=1.0):
     return (torch.randn(1, C, H, W, generator=g) * scale).contiguous()
 
 
+def fill_seeded(module, seed):
+    """Overwrite every floating-point parameter and buffer of `module` from a seeded generator, key by key in sorted
+    name order (fan-in scaled weights, near-1 norm scales, positive running variances): two modules with the same state
+    dict keys and shapes -- the reference's encoder and ours -- get identical weights whatever their init order."""
+    g = torch.Generator().manual_seed(int(seed))
+    sd = module.state_dict()
+    with torch.no_grad():
+        for k in sorted(sd):
+            v = sd[k]
+            if not v.is_floating_point():
+                continue
+            r = torch.randn(v.shape, generator=g)
+            if k.endswith("running_var"):
+                v.copy_(torch.rand(v.shape, generator=g) + 0.5)
+            elif k.endswith("running_mean") or k.endswith("bias"):
+                v.copy_(r * 0.1)
+            elif v.dim() == 1:
+                v.copy_(1.0 + 0.1 * r)
+            else:
+                v.copy_(r / math.sqrt(max(1, v[0].numel())))
+    return module
+
+
 def make_points(N, seed, lo=-1.1, hi=1.1):
     g = torch.Generator().manual_seed(int(seed))
     return (torch.rand(1, 3, N, generator=g) * (hi - lo) + lo).contiguous()

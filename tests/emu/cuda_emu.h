@@ -3,7 +3,7 @@
 // one OS thread per CUDA thread, CTAs executed one after the other, __syncthreads() = a pthread barrier over the CTA,
 // warp shuffles = an exchange buffer between two 32-thread barriers, `__shared__` = a static variable (valid because
 // only one CTA is alive at a time).  It checks index arithmetic, scan / queue logic and table use against the oracle
-// before a kernel is ever sent to a B200; it says nothing about performance or memory-model subtleties.
+// before a kernel is ever sent to an H100; it says nothing about performance or memory-model subtleties.
 // Nothing under monoport_b200/ includes this file.
 #pragma once
 #include <atomic>

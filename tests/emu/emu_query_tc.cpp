@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE ONLY: monoport_b200/csrc/query_tc.cu -- host-side weight packing, launch logic, the per-frame G0
-// GEMM kernel and the fused tcgen05 sample+MLP kernels -- compiled UNMODIFIED for the CPU against the execution-model
-// emulation (cuda_emu.h) and the functional model of the tcgen05 / mbarrier / bulk-copy layer (tc_ptx_emu.h).
+// GEMM kernel and the fused wgmma sample+MLP kernel -- compiled UNMODIFIED for the CPU against the execution-model
+// emulation (cuda_emu.h) and the functional model of the wgmma / mbarrier / bulk-copy layer (tc_ptx_emu.h).
 //   emu_query_tc in.bin out.f32 program sms
 // in.bin: int32 header {C, H, W, N, has_calib, perspective, res, last_op}, float z_scale, calib[12], then fp32 arrays:
 //   feature map NCHW [C*H*W], points [3*N], for each of the 5 layers W_l [cout*cin] and b_l [cout].
@@ -29,7 +29,7 @@ alignas(1024) static uint8_t g_dyn_smem[2][240 * 1024];
 void* mp_emu_dyn_smem() { return g_dyn_smem[cuda_emu::t_rank]; }
 
 // ---- a host-memory stand-in for the few CUDA runtime calls of the launcher ----------------------------------------------
-static int g_fake_sms = 148;
+static int g_fake_sms = 132;
 extern "C" {
 cudaError_t cudaMalloc(void** p, size_t n) { *p = aligned_alloc(256, (n + 255) / 256 * 256); return *p ? cudaSuccess : cudaErrorMemoryAllocation; }
 cudaError_t cudaFree(void* p) { free(p); return cudaSuccess; }
@@ -38,7 +38,7 @@ cudaError_t cudaMemset(void* d, int v, size_t n) { memset(d, v, n); return cudaS
 cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t) { memcpy(d, s, n); return cudaSuccess; }
 cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) {
-  if (a == cudaDevAttrComputeCapabilityMajor) *v = 10;
+  if (a == cudaDevAttrComputeCapabilityMajor) *v = 9;
   else if (a == cudaDevAttrMaxSharedMemoryPerBlockOptin) *v = 232448;
   else if (a == cudaDevAttrMultiProcessorCount) *v = g_fake_sms;
   else *v = 0;

@@ -1,17 +1,14 @@
 // TEST INFRASTRUCTURE ONLY -- functional CPU model of monoport_b200/csrc/tc_ptx.cuh (included by it under MP_CUDA_EMU):
-// mbarriers with transaction counts, bulk async copies, tensor memory, tcgen05.mma (.kind::f16, cta_group::1, operands
-// from SWIZZLE_128B K-major shared-memory descriptors or packed fp16 in tensor memory), tcgen05.commit, tcgen05.ld/st;
-// and, for launches of 2-CTA clusters (cuda_emu::launch(..., 2): each CTA has its own shared and tensor memory), the
-// cluster rank, cluster barriers, remote mbarrier arrivals, multicast bulk copies and multicast commits, and
-// tcgen05.mma.cta_group::2 (M = 256: rows [0,128) are the leader CTA's, [128,256) the peer's -- A operand and accumulator of
-// each half in that CTA's shared / tensor memory; the N rows of B are split between the two shared memories) with plain
-// 2-D tensor-map copies completing on the leader's barrier.
+// mbarriers with transaction counts, bulk async copies, named barriers, and the warpgroup MMA (wgmma.mma_async, fp16
+// operands from SWIZZLE_128B K-major shared-memory descriptors, fp32 accumulators in the registers of the 128 threads of
+// a warpgroup, commit / wait_group).
 //
-// Asynchrony is modelled adversarially: a bulk copy or an MMA is only QUEUED when it is issued; queued operations are
-// executed (copies first, then MMAs / commits in issue order) when some thread is blocked in an mbarrier wait.  So
-//   * reading an accumulator without waiting for the commit barrier sees stale tensor memory,
-//   * overwriting a shared-memory operand (or a weight stage) before the MMA that reads it has been waited for makes
-//     that MMA consume the new bytes,
+// Asynchrony is modelled adversarially: a bulk copy is only QUEUED when it is issued and executed when some thread is
+// blocked in an mbarrier wait; a thread's wgmma is only recorded when it is issued and executed -- reading shared memory
+// at that moment -- when the thread's wait_group retires its group.  So
+//   * reading an accumulator before wait_group sees the old registers,
+//   * overwriting a shared-memory operand (or a weight stage) before the wgmma that reads it has been waited for makes
+//     that wgmma consume the new bytes,
 // both of which show up as wrong results, and a broken hand-off protocol shows up as a reported deadlock (all threads
 // waiting, nothing queued) instead of a hang.  Timing, bank conflicts and memory-model subtleties are NOT modelled.
 #pragma once
@@ -22,33 +19,22 @@
 namespace tc {
 
 namespace emu {
-constexpr uint32_t kLanes = 128, kCols = 512;
-struct Op {
-  enum Kind { COPY, MMA_SS, MMA_TS, COMMIT } kind;
-  // COPY
+struct Op {                                  // a queued bulk copy
   uint8_t* dst; const uint8_t* src; uint32_t bytes; uint64_t* bar;
-  // MMA
-  uint32_t d_tmem, a_tmem, idesc, accumulate;
-  uint64_t a_desc, b_desc;
-  int rank;                                  // the issuing CTA: whose shared / tensor memory the operands live in
-  int cg;                                    // 1, or 2: one instruction over both CTAs of the pair (issued by rank 0)
 };
 inline std::mutex g_mu;
-inline std::deque<Op> g_copies, g_mmas;
-inline uint32_t g_tmem_r[2][kLanes][kCols];
-inline uint8_t* g_smem_r[2] = {nullptr, nullptr};   // base of the dynamic shared memory of each CTA of the cluster (1024-B aligned)
+inline std::deque<Op> g_copies;
+inline uint8_t* g_smem_r[2] = {nullptr, nullptr};   // base of the dynamic shared memory (1024-B aligned)
 inline uint32_t g_smem_bytes = 0;
-#define g_tmem g_tmem_r[cuda_emu::t_rank]
 #define g_smem g_smem_r[cuda_emu::t_rank]
 inline std::atomic<unsigned long long> g_events{0};   // bumped by every state change (deadlock watchdog)
 inline std::atomic<int> g_waiting{0};
-// work counters (EMU_TC_STATS=1 prints them at exit): what the program actually executes per launch, to set against the
-// ALGORITHMIC flops the roofline is quoted on
-struct Stats { unsigned long long mma_flop = 0, mma_ops = 0, copy_bytes = 0, copies = 0, tmem_ld = 0, tmem_st = 0; };
+// work counters (EMU_TC_STATS=1 prints them at exit)
+struct Stats { std::atomic<unsigned long long> mma_flop{0}, mma_ops{0}, copy_bytes{0}, copies{0}; };
 inline Stats g_stats;
 inline void print_stats() {
-  fprintf(stderr, "[tc emu stats] mma: %llu ops, %.3f GFLOP | bulk copies: %llu, %.3f MB | tcgen05.ld x32: %llu  tcgen05.st x16: %llu\n",
-          g_stats.mma_ops, g_stats.mma_flop * 1e-9, g_stats.copies, g_stats.copy_bytes * 1e-6, g_stats.tmem_ld, g_stats.tmem_st);
+  fprintf(stderr, "[tc emu stats] wgmma (per warpgroup): %llu ops, %.3f GFLOP | bulk copies: %llu, %.3f MB\n",
+          g_stats.mma_ops.load() / 128, g_stats.mma_flop.load() * 1e-9, g_stats.copies.load(), g_stats.copy_bytes.load() * 1e-6);
 }
 inline void stats_init() {
   static const bool on = [] { const bool e = getenv("EMU_TC_STATS") != nullptr; if (e) atexit(print_stats); return e; }();
@@ -56,7 +42,6 @@ inline void stats_init() {
 }
 inline bool eager() { static const bool e = getenv("EMU_TC_EAGER") != nullptr; return e; }   // debugging aid: no deferral
 
-// `base1`: the shared memory of the second CTA of a cluster (same size; may be null when no cluster launch follows)
 inline void set_smem(void* base, uint32_t bytes, void* base1 = nullptr) {
   stats_init();
   if (((uintptr_t)base | (uintptr_t)base1) & 1023) { fprintf(stderr, "tc emu: shared memory base must be 1024-byte aligned\n"); abort(); }
@@ -64,23 +49,9 @@ inline void set_smem(void* base, uint32_t bytes, void* base1 = nullptr) {
   g_smem_r[1] = (uint8_t*)base1;
   g_smem_bytes = bytes;
   g_copies.clear();
-  g_mmas.clear();
-  memset(g_tmem_r, 0xCD, sizeof(g_tmem_r));  // poison: uninitialised accumulators are visible
-}
-// which CTA of the cluster owns a shared-memory pointer (-1: none), and the same offset in CTA `rank`
-inline int smem_rank_of(const void* p) {
-  for (int r = 0; r < 2; ++r)
-    if (g_smem_r[r] && (uintptr_t)p >= (uintptr_t)g_smem_r[r] && (uintptr_t)p < (uintptr_t)g_smem_r[r] + g_smem_bytes) return r;
-  return -1;
-}
-template <class T> inline T* smem_in_cta(T* p, int rank) {
-  const int own = smem_rank_of(p);
-  if (own < 0 || rank < 0 || rank >= cuda_emu::g_cluster || !g_smem_r[rank]) { fprintf(stderr, "tc emu: bad cluster address translation\n"); abort(); }
-  return reinterpret_cast<T*>(g_smem_r[rank] + ((uintptr_t)p - (uintptr_t)g_smem_r[own]));
 }
 
-// ---- mbarrier word: [0,20) pending arrivals | [20,40) arrival count of a phase | [40,62) pending tx bytes (SIGNED: in a
-//      cluster the peer's multicast bytes may complete before this CTA's expect_tx of the same phase) | 63 phase
+// ---- mbarrier word: [0,20) pending arrivals | [20,40) arrival count of a phase | [40,62) pending tx bytes | 63 phase
 inline uint32_t mb_pending(uint64_t w) { return (uint32_t)(w & 0xFFFFF); }
 inline uint32_t mb_count(uint64_t w) { return (uint32_t)((w >> 20) & 0xFFFFF); }
 inline int32_t mb_tx(uint64_t w) { const uint32_t v = (uint32_t)((w >> 40) & 0x3FFFFF); return (v & 0x200000u) ? (int32_t)v - 0x400000 : (int32_t)v; }
@@ -103,125 +74,71 @@ inline void mb_arrive_locked(uint64_t* bar) {
 
 inline float h2f(uint16_t h) { __half x; memcpy(&x, &h, 2); return __half2float(x); }
 inline uint32_t swz(uint32_t a) { return a ^ (((a >> 7) & 7u) << 4); }       // SWIZZLE_128B on the shared-memory address
-inline uint16_t smem_half(uint32_t addr, int rank) {
+inline uint16_t smem_half(uint32_t addr) {
   const uint32_t p = swz(addr);
   if (p + 2 > g_smem_bytes) { fprintf(stderr, "tc emu: MMA operand address %u outside shared memory\n", p); abort(); }
   uint16_t h;
-  memcpy(&h, g_smem_r[rank] + p, 2);
+  memcpy(&h, g_smem + p, 2);
   return h;
 }
-
-// D[128 x N] (+)= A[128 x 16] * B[N x 16]^T, fp16 operands, fp32 accumulation.  cta_group::2: M = 256 -- for each CTA h of the
-// pair D_h[128 x N] (+)= A_h * B^T with A_h and D_h in CTA h's memories and B = rows [0, N/2) from CTA 0's shared memory followed
-// by rows [N/2, N) from CTA 1's (same descriptor in both).
-inline void exec_mma(const Op& op) {
-  const uint32_t M = ((op.idesc >> 24) & 0x1F) << 4, N = ((op.idesc >> 17) & 0x3F) << 3;
-  if (M != 128u * (uint32_t)op.cg || N == 0 || N > 256 || (N & 15)) { fprintf(stderr, "tc emu: unsupported MMA shape %ux%u (cta_group::%d)\n", M, N, op.cg); abort(); }
-  if (((op.idesc >> 4) & 3) != 1 || ((op.idesc >> 7) & 7) != 0 || ((op.idesc >> 10) & 7) != 0) { fprintf(stderr, "tc emu: idesc formats\n"); abort(); }
-  if (op.cg == 2 && (op.rank != 0 || cuda_emu::g_cluster != 2)) { fprintf(stderr, "tc emu: cta_group::2 MMAs are issued by the leader of a 2-CTA cluster\n"); abort(); }
-  g_stats.mma_ops++;
-  g_stats.mma_flop += 2ull * M * N * 16;
-  const uint32_t dcol = op.d_tmem & 0xFFFF;
-  if ((op.d_tmem >> 16) != 0 || dcol + N > kCols) { fprintf(stderr, "tc emu: bad accumulator address %08x (N=%u)\n", op.d_tmem, N); abort(); }
-  auto desc_fields = [](uint64_t d, uint32_t& start, uint32_t& sbo) {
-    start = (uint32_t)(d & 0x3FFF) << 4;
-    sbo = (uint32_t)((d >> 32) & 0x3FFF) << 4;
-    if (((d >> 61) & 7) != 2) { fprintf(stderr, "tc emu: only SWIZZLE_128B descriptors are modelled\n"); abort(); }
-  };
-  static thread_local float A[128][16], B[256][16];
-  {
-    uint32_t st, sbo;
-    desc_fields(op.b_desc, st, sbo);
-    if (op.cg == 1) {
-      for (uint32_t n = 0; n < N; ++n)
-        for (uint32_t k = 0; k < 16; ++k) B[n][k] = h2f(smem_half(st + (n >> 3) * sbo + (n & 7) * 128 + k * 2, op.rank));
-    } else {
-      for (uint32_t n = 0; n < N; ++n) {
-        const uint32_t nl = n % (N / 2);
-        for (uint32_t k = 0; k < 16; ++k) B[n][k] = h2f(smem_half(st + (nl >> 3) * sbo + (nl & 7) * 128 + k * 2, (int)(n / (N / 2))));
-      }
-    }
-  }
-  for (int h = 0; h < op.cg; ++h) {
-    const int cta = op.cg == 1 ? op.rank : h;
-    if (op.kind == Op::MMA_SS) {
-      uint32_t st, sbo;
-      desc_fields(op.a_desc, st, sbo);
-      for (uint32_t m = 0; m < 128; ++m)
-        for (uint32_t k = 0; k < 16; ++k) A[m][k] = h2f(smem_half(st + (m >> 3) * sbo + (m & 7) * 128 + k * 2, cta));
-    } else {
-      const uint32_t acol = op.a_tmem & 0xFFFF;
-      if ((op.a_tmem >> 16) != 0 || acol + 8 > kCols) { fprintf(stderr, "tc emu: bad A tensor-memory address\n"); abort(); }
-      for (uint32_t m = 0; m < 128; ++m)
-        for (uint32_t k = 0; k < 16; ++k) {
-          const uint32_t w = g_tmem_r[cta][m][acol + (k >> 1)];
-          A[m][k] = h2f((uint16_t)((k & 1) ? (w >> 16) : (w & 0xFFFF)));
-        }
-    }
-    if (h == 0) {
-      static const int trace_n = getenv("EMU_TC_TRACE_MMA") ? atoi(getenv("EMU_TC_TRACE_MMA")) : 0;
-      static int seen = 0;
-      if (seen < trace_n) {
-        float amin = 1e30f, amax = -1e30f;
-        for (uint32_t m = 0; m < 128; ++m) for (uint32_t k = 0; k < 16; ++k) { amin = fminf(amin, A[m][k]); amax = fmaxf(amax, A[m][k]); }
-        fprintf(stderr, "[mma %3d] %s dcol=%3u N=%3u acc=%u  A[0][0..3]=%g %g %g %g  A range [%g, %g]  B[0][0..1]=%g %g\n", seen,
-                op.kind == Op::MMA_SS ? "SS" : "TS", dcol, N, op.accumulate, A[0][0], A[0][1], A[0][2], A[0][3], amin, amax, B[0][0], B[0][1]);
-        ++seen;
-      }
-    }
-    for (uint32_t m = 0; m < 128; ++m)
-      for (uint32_t n = 0; n < N; ++n) {
-        float acc = 0.f;
-        for (uint32_t k = 0; k < 16; ++k) acc += A[m][k] * B[n][k];
-        float d = 0.f;
-        if (op.accumulate) memcpy(&d, &g_tmem_r[cta][m][dcol + n], 4);
-        d += acc;
-        memcpy(&g_tmem_r[cta][m][dcol + n], &d, 4);
-      }
-  }
+inline void desc_fields(uint64_t d, uint32_t& start, uint32_t& sbo) {
+  start = (uint32_t)(d & 0x3FFF) << 4;
+  sbo = (uint32_t)((d >> 32) & 0x3FFF) << 4;
+  if (((d >> 62) & 3) != 1 || ((d >> 49) & 7) != 0) { fprintf(stderr, "tc emu: only SWIZZLE_128B descriptors without base offset are modelled\n"); abort(); }
 }
 
-// executes ONE queued asynchronous operation; returns false when nothing is queued.  Caller holds g_mu.
-// EMU_TC_ORDER=copies (default: bulk copies before MMAs -- a weight stage overwritten too early reaches a late MMA),
-// =mmas (MMAs first), =random[:seed] (either engine; MMAs stay in issue order, copies complete in any order).
+// one thread's share of D[64 x N] += A[64 x 16] * B[N x 16]^T: the accumulator fragment of thread t of the warpgroup
+// (warp wl = t/32, lane l) is d[4j + e] = D[16 wl + l/4 + 8 (e>>1)][8 j + 2 (l%4) + (e&1)]
+inline void exec_wgmma(float* d, int N, uint64_t a_desc, uint64_t b_desc) {
+  const int t = cuda_emu::linear_tid() & 127, wl = t >> 5, l = t & 31;
+  uint32_t as, asbo, bs, bsbo;
+  desc_fields(a_desc, as, asbo);
+  desc_fields(b_desc, bs, bsbo);
+  float A[2][16];
+  for (int h = 0; h < 2; ++h) {
+    const uint32_t m = 16 * wl + l / 4 + 8 * h;
+    for (uint32_t k = 0; k < 16; ++k) A[h][k] = h2f(smem_half(as + (m >> 3) * asbo + (m & 7) * 128 + k * 2));
+  }
+  for (int j = 0; j < N / 8; ++j)
+    for (int e = 0; e < 2; ++e) {
+      const uint32_t n = 8 * j + 2 * (l % 4) + e;
+      float B[16];
+      for (uint32_t k = 0; k < 16; ++k) B[k] = h2f(smem_half(bs + (n >> 3) * bsbo + (n & 7) * 128 + k * 2));
+      for (int h = 0; h < 2; ++h) {
+        float acc = 0.f;
+        for (uint32_t k = 0; k < 16; ++k) acc += A[h][k] * B[k];
+        d[4 * j + 2 * h + e] += acc;
+      }
+    }
+  g_stats.mma_ops++;
+  g_stats.mma_flop += 2ull * 16 * N * 16 / 4;    // (this thread's quarter-warp share, summed over the warpgroup)
+}
+struct Wgmma { float* d; int N; uint64_t a, b; };
+inline thread_local std::vector<Wgmma> t_open;                    // issued, not yet committed
+inline thread_local std::deque<std::vector<Wgmma>> t_groups;      // committed groups, oldest first
+
+// executes ONE queued bulk copy; returns false when nothing is queued.  Caller holds g_mu.
+// EMU_TC_ORDER=copies (default: in issue order), =random[:seed] (any outstanding copy may complete next).
 inline bool progress_locked() {
   static const int order = [] {
     const char* v = getenv("EMU_TC_ORDER");
-    if (!v || !strncmp(v, "copies", 6)) return 0;
-    if (!strncmp(v, "mmas", 4)) return 1;
+    if (!v || strncmp(v, "random", 6)) return 0;
     const char* c = strchr(v, ':');
     srand(c ? (unsigned)atoi(c + 1) : 1u);
     return 2;
   }();
-  bool copy_first = order == 0 || (order == 2 && (rand() & 1));
-  if (copy_first && g_copies.empty()) copy_first = false;
-  if (!copy_first && g_mmas.empty() && !g_copies.empty()) copy_first = true;
-  if (copy_first && order == 2 && g_copies.size() > 1) {       // any outstanding copy may complete next
-    const size_t k = (size_t)rand() % g_copies.size();
-    std::swap(g_copies[0], g_copies[k]);
-  }
-  if (copy_first) {
-    const Op op = g_copies.front();
-    g_copies.pop_front();
-    memcpy(op.dst, op.src, op.bytes);
-    g_stats.copies++;
-    g_stats.copy_bytes += op.bytes;
-    const uint64_t w = *op.bar;
-    // (inside one CTA a complete_tx never precedes its expect_tx -- the copy is issued after it; across a cluster it may)
-    if (mb_tx(w) < (int32_t)op.bytes && cuda_emu::g_cluster == 1) { fprintf(stderr, "tc emu: complete_tx without a matching expect_tx\n"); abort(); }
-    *op.bar = mb_make(mb_pending(w), mb_count(w), mb_tx(w) - (int32_t)op.bytes, mb_phase(w));
-    mb_check_complete(op.bar);
-    return true;
-  }
-  if (!g_mmas.empty()) {
-    const Op op = g_mmas.front();
-    g_mmas.pop_front();
-    if (op.kind == Op::COMMIT) mb_arrive_locked(op.bar);
-    else exec_mma(op);
-    g_events++;
-    return true;
-  }
-  return false;
+  if (g_copies.empty()) return false;
+  if (order == 2 && g_copies.size() > 1) std::swap(g_copies[0], g_copies[(size_t)rand() % g_copies.size()]);
+  const Op op = g_copies.front();
+  g_copies.pop_front();
+  memcpy(op.dst, op.src, op.bytes);
+  g_stats.copies++;
+  g_stats.copy_bytes += op.bytes;
+  const uint64_t w = *op.bar;
+  if (mb_tx(w) < (int32_t)op.bytes) { fprintf(stderr, "tc emu: complete_tx without a matching expect_tx\n"); abort(); }
+  *op.bar = mb_make(mb_pending(w), mb_count(w), mb_tx(w) - (int32_t)op.bytes, mb_phase(w));
+  mb_check_complete(op.bar);
+  return true;
 }
 }  // namespace emu
 
@@ -236,17 +153,12 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 inline void mbar_init(uint64_t* bar, uint32_t count) { std::lock_guard<std::mutex> g(emu::g_mu); *bar = emu::mb_make(count, count, 0, 0); emu::g_events++; }
 inline void fence_barrier_init() {}
 inline void mbar_arrive(uint64_t* bar) { std::lock_guard<std::mutex> g(emu::g_mu); emu::mb_arrive_locked(bar); }
+inline void mbar_arrive_if(uint64_t* bar, bool pred) { if (pred) mbar_arrive(bar); }
 inline void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
   std::lock_guard<std::mutex> g(emu::g_mu);
   const uint64_t w = *bar;
   *bar = emu::mb_make(emu::mb_pending(w), emu::mb_count(w), emu::mb_tx(w) + (int32_t)bytes, emu::mb_phase(w));
   emu::mb_arrive_locked(bar);
-}
-inline bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  if (emu::mb_phase(*bar) != (parity & 1u)) return true;
-  emu::progress_locked();                    // a polling thread also lets the asynchronous engines advance
-  return false;
 }
 inline bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   {
@@ -281,96 +193,56 @@ inline void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint6
   (void)smem_u32(smem_dst);
   std::lock_guard<std::mutex> g(emu::g_mu);
   emu::Op op{};
-  op.kind = emu::Op::COPY; op.dst = (uint8_t*)smem_dst; op.src = (const uint8_t*)gmem_src; op.bytes = bytes; op.bar = bar;
+  op.dst = (uint8_t*)smem_dst; op.src = (const uint8_t*)gmem_src; op.bytes = bytes; op.bar = bar;
   emu::g_copies.push_back(op);
   if (emu::eager()) while (emu::progress_locked()) {}
 }
 
-inline void bar_sync_workers256() {
-  // warps 4..11 of the CTA: the eight per-warp barriers in sequence form a 256-thread barrier (two rounds)
-  static pthread_barrier_t b;
-  static std::once_flag once;
-  std::call_once(once, [] { pthread_barrier_init(&b, nullptr, 256); });
-  pthread_barrier_wait(&b);
+// named barrier over the first `threads` threads of the CTA (one CTA runs at a time)
+inline void bar_sync(int id, int threads) {
+  static pthread_barrier_t b[16];
+  static int n[16];
+  static std::mutex mu;
+  {
+    std::lock_guard<std::mutex> g(mu);
+    if (n[id] != threads) { pthread_barrier_init(&b[id], nullptr, (unsigned)threads); n[id] = threads; }
+  }
+  if (cuda_emu::linear_tid() >= threads) { fprintf(stderr, "tc emu: thread outside the named barrier\n"); abort(); }
+  pthread_barrier_wait(&b[id]);
 }
 
 // ---------------------------------------------------------------- fences
 inline void fence_proxy_async_smem() {}
-inline void tcgen05_fence_before() {}
-inline void tcgen05_fence_after() {}
 
-// ---------------------------------------------------------------- TMEM allocation
-inline void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {
-  if (ncols != 512) { fprintf(stderr, "tc emu: the model hands out all 512 columns\n"); abort(); }
-  if ((cuda_emu::linear_tid() & 31) == 0) *smem_result = 0;
+// ---------------------------------------------------------------- warpgroup MMA
+inline void wgmma_fence() {}
+inline void wgmma_commit() {
+  emu::t_groups.push_back(std::move(emu::t_open));
+  emu::t_open.clear();
 }
-inline void tmem_relinquish() {}
-inline void tmem_dealloc(uint32_t, uint32_t) {}
-
-// ---------------------------------------------------------------- descriptors (same bit layouts as tc_ptx.cuh)
-inline uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t sbo_bytes) {
+template <int N>
+inline void wgmma_wait() {
+  if (!emu::t_open.empty()) { fprintf(stderr, "tc emu: wgmma issued but not committed before wait_group\n"); abort(); }
+  while (emu::t_groups.size() > (size_t)N) {
+    for (const emu::Wgmma& w : emu::t_groups.front()) emu::exec_wgmma(w.d, w.N, w.a, w.b);
+    emu::t_groups.pop_front();
+  }
+}
+inline uint64_t make_wdesc_sw128(uint32_t smem_addr, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-constexpr uint32_t make_idesc_f16(int M, int N) { return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24); }
-
-// ---------------------------------------------------------------- MMA
-inline void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  emu::Op op{};
-  op.kind = emu::Op::MMA_SS; op.d_tmem = d_tmem; op.a_desc = a_desc; op.b_desc = b_desc; op.idesc = idesc; op.accumulate = accumulate;
-  op.rank = cuda_emu::t_rank; op.cg = 1;
-  emu::g_mmas.push_back(op);
-  if (emu::eager()) while (emu::progress_locked()) {}
+inline void wgmma_issue(float* d, int N, uint64_t a, uint64_t b) {
+  emu::t_open.push_back(emu::Wgmma{d, N, a, b});
+  if (emu::eager()) { wgmma_commit(); wgmma_wait<0>(); }
 }
-inline void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  emu::Op op{};
-  op.kind = emu::Op::MMA_TS; op.d_tmem = d_tmem; op.a_tmem = a_tmem; op.b_desc = b_desc; op.idesc = idesc; op.accumulate = accumulate;
-  op.rank = cuda_emu::t_rank; op.cg = 1;
-  emu::g_mmas.push_back(op);
-  if (emu::eager()) while (emu::progress_locked()) {}
-}
-inline void mma_commit(uint64_t* bar) {
-  (void)smem_u32(bar);
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  emu::Op op{};
-  op.kind = emu::Op::COMMIT; op.bar = bar;
-  emu::g_mmas.push_back(op);
-  if (emu::eager()) while (emu::progress_locked()) {}
-}
-
-// ---------------------------------------------------------------- TMEM <-> registers (warp w owns lanes 32*(w%4)..+31)
-inline uint32_t tmem_row_checked(uint32_t taddr) {
-  const int tid = cuda_emu::linear_tid(), warp = tid >> 5, lane = tid & 31;
-  const uint32_t lane_field = taddr >> 16;
-  if (lane_field != (uint32_t)(32 * (warp & 3))) {
-    fprintf(stderr, "tc emu: warp %d may only touch tensor-memory lanes %d..%d (address lane %u)\n", warp, 32 * (warp & 3), 32 * (warp & 3) + 31, lane_field);
-    abort();
-  }
-  return lane_field + lane;
-}
-inline void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  const uint32_t row = tmem_row_checked(taddr), col = taddr & 0xFFFF;
-  if (col + 32 > emu::kCols) { fprintf(stderr, "tc emu: tcgen05.ld beyond column 512\n"); abort(); }
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  if ((cuda_emu::linear_tid() & 31) == 0) emu::g_stats.tmem_ld++;
-  for (int j = 0; j < 32; ++j) r[j] = emu::g_tmem[row][col + j];
-}
-inline void tmem_ld_wait() {}
-inline void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  const uint32_t row = tmem_row_checked(taddr), col = taddr & 0xFFFF;
-  if (col + 16 > emu::kCols) { fprintf(stderr, "tc emu: tcgen05.st beyond column 512\n"); abort(); }
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  if ((cuda_emu::linear_tid() & 31) == 0) emu::g_stats.tmem_st++;
-  for (int j = 0; j < 16; ++j) emu::g_tmem[row][col + j] = r[j];
-}
-inline void tmem_st_wait() {}
+inline void wgmma_m64n256(float (&d)[128], uint64_t a, uint64_t b) { wgmma_issue(d, 256, a, b); }
+inline void wgmma_m64n128(float (&d)[64], uint64_t a, uint64_t b) { wgmma_issue(d, 128, a, b); }
+inline void wgmma_m64n64(float (&d)[32], uint64_t a, uint64_t b) { wgmma_issue(d, 64, a, b); }
 
 // ---------------------------------------------------------------- operand layout helpers (as in tc_ptx.cuh)
 inline uint32_t sw128_offset(uint32_t row, uint32_t k) {
@@ -383,83 +255,5 @@ inline uint32_t pack_half2(float lo, float hi) {
   memcpy(&u, &h, 4);
   return u;
 }
-
-// ---------------------------------------------------------------- 2-CTA clusters (cuda_emu::launch(..., 2))
-inline uint32_t cluster_ctarank() { return (uint32_t)cuda_emu::t_rank; }
-inline void cluster_sync_all() {
-  if (cuda_emu::g_cluster == 1) { __syncthreads(); return; }
-  pthread_barrier_wait(&cuda_emu::g_cluster_barrier);
-}
-// arrive on the barrier at the same offset in CTA `rank`
-inline void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  emu::mb_arrive_locked(emu::smem_in_cta(bar, (int)rank));
-}
-inline void mbar_wait_cluster(uint64_t* bar, uint32_t parity) { mbar_wait(bar, parity); }
-// one copy per CTA of `cta_mask`, to the same offsets (data and barrier) in each
-inline void bulk_g2s_multicast(void* smem_dst, const void* gmem_src, uint32_t bytes, uint64_t* bar, uint16_t cta_mask) {
-  if (bytes % 16 || ((uintptr_t)smem_dst & 15) || ((uintptr_t)gmem_src & 15)) { fprintf(stderr, "tc emu: bulk copy alignment\n"); abort(); }
-  (void)smem_u32(smem_dst);
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  for (int r = 0; r < 2; ++r) {
-    if (!((cta_mask >> r) & 1)) continue;
-    emu::Op op{};
-    op.kind = emu::Op::COPY; op.dst = emu::smem_in_cta((uint8_t*)smem_dst, r); op.src = (const uint8_t*)gmem_src; op.bytes = bytes;
-    op.bar = emu::smem_in_cta(bar, r);
-    emu::g_copies.push_back(op);
-  }
-  if (emu::eager()) while (emu::progress_locked()) {}
-}
-// completion of this CTA's MMAs so far, signalled on the barrier at the same offset in BOTH CTAs
-inline void mma_commit_pair(uint64_t* bar) {
-  (void)smem_u32(bar);
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  for (int r = 0; r < 2; ++r) {
-    emu::Op op{};
-    op.kind = emu::Op::COMMIT; op.bar = emu::smem_in_cta(bar, r);
-    emu::g_mmas.push_back(op);
-  }
-  if (emu::eager()) while (emu::progress_locked()) {}
-}
-// ---- cta_group::2: allocation, MMAs over the pair, commits to both CTAs, tensor-map copies completing on the leader's barrier
-inline void tmem_alloc2(uint32_t* smem_result, uint32_t ncols) { tmem_alloc(smem_result, ncols); }
-inline void tmem_relinquish2() {}
-inline void tmem_dealloc2(uint32_t, uint32_t) {}
-inline void mma_ss2(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  emu::Op op{};
-  op.kind = emu::Op::MMA_SS; op.d_tmem = d_tmem; op.a_desc = a_desc; op.b_desc = b_desc; op.idesc = idesc; op.accumulate = accumulate;
-  op.rank = cuda_emu::t_rank; op.cg = 2;
-  emu::g_mmas.push_back(op);
-  if (emu::eager()) while (emu::progress_locked()) {}
-}
-inline void mma_ts2(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  emu::Op op{};
-  op.kind = emu::Op::MMA_TS; op.d_tmem = d_tmem; op.a_tmem = a_tmem; op.b_desc = b_desc; op.idesc = idesc; op.accumulate = accumulate;
-  op.rank = cuda_emu::t_rank; op.cg = 2;
-  emu::g_mmas.push_back(op);
-  if (emu::eager()) while (emu::progress_locked()) {}
-}
-inline void mma_commit2(uint64_t* bar) { mma_commit_pair(bar); }
-// The model's "tensor map": the first 8 bytes of the 128-byte object hold the base of a [rows][64 fp16] array (what
-// mp_tc_prepare stores under MP_CUDA_EMU); a copy is one plain 2-D box of 128 rows x 128 bytes at row c1, landing in the
-// CALLING CTA's shared memory and completing on the LEADER's barrier (cta_group::2 form).
-inline void tma_load_2d_cg2(void* smem_dst, const void* tmap, int c0, int c1, uint64_t* bar) {
-  if (c0 != 0 || c1 < 0) { fprintf(stderr, "tc emu: tensor-map copy coordinates\n"); abort(); }
-  (void)smem_u32(smem_dst);
-  const uint8_t* base;
-  memcpy(&base, tmap, sizeof(base));
-  std::lock_guard<std::mutex> g(emu::g_mu);
-  emu::Op op{};
-  op.kind = emu::Op::COPY; op.dst = (uint8_t*)smem_dst; op.src = base + (size_t)c1 * 128; op.bytes = 128 * 128;
-  op.bar = emu::smem_in_cta(bar, 0);
-  emu::g_copies.push_back(op);
-  if (emu::eager()) while (emu::progress_locked()) {}
-}
-inline void tma_load_2d(void*, const void*, int, int, uint64_t*) { fprintf(stderr, "tc emu: cta_group::1 tensor-map copies are not modelled\n"); abort(); }
-inline void tma_prefetch_desc(const void*) {}
-// elect.sync: the same lane for the same (full) member mask
-inline bool elect_one() { return (cuda_emu::linear_tid() & 31) == 0; }
 
 }  // namespace tc

@@ -139,10 +139,74 @@ def gen_calib(ns):
                         calib=np.stack([r["calib"] for r in rows]))
 
 
+def obj_case():
+    """Seeded mesh of the OBJ-writer comparison (vertices, faces, colours)."""
+    rng = np.random.default_rng(0)
+    V = rng.normal(size=(57, 3)).astype(np.float32)
+    Fc = rng.integers(0, 57, size=(101, 3)).astype(np.int32)
+    C = rng.random((57, 3)).astype(np.float32)
+    return V, Fc, C
+
+
+ENCODER_SEEDS = {"G": (101, 102), "C": (111, 112)}     # (weights, image)
+ENCODER_SAMPLE = 4096
+
+
+def encoder_sample_index(n):
+    return torch.randperm(n, generator=torch.Generator().manual_seed(7))[:min(n, ENCODER_SAMPLE)]
+
+
+def gen_reference_checks(ns):
+    """reference_checks.npz: what the reference's encoders (seeded weights, seeded 64x64 image), its OBJ writers and its
+    query() of 3000 points produce -- the values tests/test_host_logic.py and tests/test_oracle_golden.py compare with."""
+    import importlib.util
+    import tempfile
+    from oracle.ref_loader import REF_ROOT
+    rec = {}
+    for key, mk in (("G", ns.PIFuNetG), ("C", ns.PIFuNetC)):
+        wseed, iseed = ENCODER_SEEDS[key]
+        net = spec.fill_seeded(mk().eval(), wseed)
+        sd = net.state_dict()
+        rec["enc%s_keys" % key] = np.array(["%s:%s" % (k, tuple(sd[k].shape)) for k in sorted(sd)])
+        img = torch.randn(1, 3, 64, 64, generator=torch.Generator().manual_seed(iseed))
+        with torch.no_grad():
+            outs = net.image_filter(img)
+        rec["enc%s_n" % key] = np.array(len(outs))
+        for i, x in enumerate(outs):
+            x = x[0]
+            idx = encoder_sample_index(x.numel())
+            rec["enc%s_%d_shape" % (key, i)] = np.array(x.shape)
+            rec["enc%s_%d_index" % (key, i)] = idx.numpy()
+            rec["enc%s_%d_values" % (key, i)] = x.reshape(-1)[idx].numpy()
+            rec["enc%s_%d_checksum" % (key, i)] = checksum(x)
+    mu_spec = importlib.util.spec_from_file_location("_ref_mesh_util", os.path.join(REF_ROOT, "monoport/lib/mesh_util.py"))
+    mu = importlib.util.module_from_spec(mu_spec)
+    mu_spec.loader.exec_module(mu)
+    V, Fc, C = obj_case()
+    with tempfile.TemporaryDirectory() as d:
+        a, b = os.path.join(d, "a.obj"), os.path.join(d, "b.obj")
+        mu.save_obj_mesh(a, V, Fc)
+        mu.save_obj_mesh_with_color(b, V, Fc, C)
+        rec["obj_plain"] = np.frombuffer(open(a, "rb").read(), dtype=np.uint8)
+        rec["obj_color"] = np.frombuffer(open(b, "rb").read(), dtype=np.uint8)
+    net = ns.PIFuNetG().eval()
+    Ws, bs = spec.make_weights(spec.G_CHANNELS, 5)
+    load_head(net, Ws, bs)
+    feat = spec.make_feat(256, 64, 64, 6)
+    pts = spec.make_points(3000, 7)
+    cal = spec.scene_calib(20, -70)
+    with torch.no_grad():
+        rec["query3000"] = net.query([[feat]], pts, calibs=cal)[0][0].numpy()
+    rec["query3000_w_checksum"] = np.stack([checksum(w) for w in Ws])
+    rec["query3000_f_checksum"] = checksum(feat)
+    np.savez_compressed(os.path.join(HERE, "reference_checks.npz"), **rec)
+
+
 if __name__ == "__main__":
     torch.set_num_threads(8)
     ns = load_reference()
     gen_query(ns)
     gen_forward_vertices(ns)
     gen_calib(ns)
+    gen_reference_checks(ns)
     print("done")

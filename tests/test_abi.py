@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports every symbol include/monoport_b200.h declares
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports every symbol include/monoport_b200.h declares
 (no compute calls -- there is no GPU here)."""
 import os
 import re
@@ -25,12 +25,12 @@ def test_library_builds_and_exports_every_declared_symbol():
     assert lib.mp_version() >= 100
 
 
-def test_built_for_sm100a_only():
+def test_built_for_sm90a_only():
     import subprocess
     from monoport_b200 import _lib
     out = subprocess.run(["cuobjdump", "--list-elf", _lib.LIB_PATH], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):

@@ -1,7 +1,7 @@
 """CPU-side checks of the integer / byte CUDA kernels: the kernel sources (monoport_b200/csrc/*_kernels.cuh, mp_scan.cuh)
 are compiled UNMODIFIED against tests/emu/cuda_emu.h (one OS thread per CUDA thread, barriers for __syncthreads and
 warp shuffles) and compared with the oracle.  The build container has no GPU; this catches indexing / scan / table
-mistakes before a kernel is sent to a B200.  The `-m gpu` tests remain the parity tests of the real library."""
+mistakes before a kernel is sent to an H100.  The `-m gpu` tests remain the parity tests of the real library."""
 import os
 import shutil
 import subprocess
@@ -188,9 +188,9 @@ def test_surface_kernels_match_reference_golden(emu_surface, tmp_path, golden_di
         np.testing.assert_allclose(N, g["N_" + d], rtol=0, atol=1e-6, equal_nan=True)
 
 
-# ---- the flagship kernels: query_tc.cu (weight packing, launch logic, G0 GEMM kernel, fused tcgen05 sample+MLP programs
-#      v2 and v3) on the functional model of the tcgen05 / TMEM / mbarrier / bulk-copy layer (tests/emu/tc_ptx_emu.h), with
-#      asynchronous operations deferred adversarially, against the goldens of the UNMODIFIED reference --------------------------
+# ---- the flagship kernels: query_tc.cu (weight packing, launch logic, G0 GEMM kernel, fused wgmma sample+MLP program) on
+#      the functional model of the wgmma / mbarrier / bulk-copy layer (tests/emu/tc_ptx_emu.h), with asynchronous operations
+#      deferred adversarially, against the goldens of the UNMODIFIED reference ---------------------------------------------
 CUDA_INC = "/usr/local/cuda/include"
 
 
@@ -220,7 +220,7 @@ def _run_query_tc(exe, tmp_path, case, n, program, sms, extra_env=None):
         for W, b in zip(case["Ws"], case["bs"]):
             f.write(W.numpy().tobytes())
             f.write(b.numpy().tobytes())
-    env = dict(os.environ, MONOPORT_B200_TC_NETC="1")       # the colour head's tensor-core program is opt-in
+    env = dict(os.environ)
     env.update(extra_env or {})
     r = subprocess.run([exe, fin, fout, str(program), str(sms)], capture_output=True, text=True, timeout=900, env=env)
     assert r.returncode == 0, r.stderr[-2000:]
@@ -228,10 +228,10 @@ def _run_query_tc(exe, tmp_path, case, n, program, sms, extra_env=None):
 
 
 @pytest.mark.parametrize("name,n,program,sms", [
-    ("g_smallmap", 300, 3, 1),      # one CTA walks three tiles: cross-tile software pipelining of the workers, ragged last tile
+    ("g_smallmap", 300, 3, 1),      # one CTA walks five tiles: the weight ring across tiles, ragged last tile
     ("g_smallmap", 300, 3, 2),      # two CTAs
     ("g_smallmap", 200, 103, 1),    # program v3 with the fused slab exchange (peer stores)
-    pytest.param("g_rot33", 130, 3, 148, marks=full_only),   # 128 x 128 map: 128 CTAs of the G0 GEMM, rotated calibration
+    pytest.param("g_rot33", 130, 3, 132, marks=full_only),   # 128 x 128 map: 128 CTAs of the G0 GEMM, rotated calibration
     ("g_persp", 100, 3, 1),         # perspective projection
     ("g_nocalib", 150, 3, 3),       # calibs=None
 ])
@@ -243,57 +243,31 @@ def test_tcgen05_kernels_match_reference_golden(emu_query_tc, tmp_path, name, n,
     assert err <= 1e-4, err          # the GPU parity bar for the tensor-core programs (measured on the model: ~2e-5)
 
 
-@pytest.mark.parametrize("n,sms", [(300, 2), (600, 4)])
-def test_tcgen05_weight_multicast_clusters_match_reference_golden(emu_query_tc, tmp_path, n, sms):
-    """The default launch of multi-wave grids: 2-CTA clusters whose CTAs each fetch half of every weight stage and multicast it
-    into both shared memories, ring slots released by both issuers (tcgen05.commit multicast).  The CPU model runs the two CTAs
-    of a cluster side by side, each with its own shared / tensor memory.  300 points = 3 tiles on one cluster (the second CTA's
-    last tile is padding); 600 points = 5 tiles on two clusters."""
+@pytest.mark.parametrize("name,n,program,sms", [
+    ("g_smallmap", 300, 3, 1),      # geometry head, one CTA walks all five tiles: the weight ring wraps across tiles
+    ("g_smallmap", 300, 3, 2),      # two CTAs
+    ("g_smallmap", 200, 103, 3),    # with the peer stores of the fused slab exchange
+    ("c_rot33", 200, 0, 1),         # colour head: two-stage ring, (hi, lo) pass of layer 3
+])
+@pytest.mark.parametrize("order", ["random:1", "random:2", "random:3"])
+def test_tcgen05_handoffs_survive_other_completion_orders(emu_query_tc, tmp_path, name, n, program, sms, order):
+    """The model completes queued bulk copies in issue order by default.  The hand-off protocol (weight ring, operand
+    buffers, wgmma groups) must not depend on that: random completion orders of the copies give the same bits, for both
+    heads and for one or several CTAs."""
     import torch
     from helpers import load_query_case
-    case = load_query_case("g_smallmap")
-    got = _run_query_tc(emu_query_tc, tmp_path, case, n, 3, sms, {"MONOPORT_B200_TC_WM": "1"})
-    want = _run_query_tc(emu_query_tc, tmp_path, case, n, 3, sms, {"MONOPORT_B200_TC_WM": "0"})
-    assert torch.equal(got, want), "the cluster launch must reproduce the plain launch bit for bit"
-    err = (got - case["expected"][:, :n]).abs().max().item()
-    assert err <= 1e-4, err
-
-
-@pytest.mark.parametrize("n,sms", [(300, 2), (600, 4)])
-def test_tcgen05_cta_pair_kernel_matches_reference_golden(emu_query_tc, tmp_path, n, sms):
-    """The opt-in CTA-pair flavour (MONOPORT_B200_TC_CG=2): tcgen05.mma.cta_group::2 with M = 256 over the two CTAs of a
-    cluster -- the leader issues for both tiles, every weight tile is split over the two shared memories (tensor-map copies
-    completing on the leader's barrier), operand hand-offs are remote arrivals, completions are multicast commits."""
-    import torch
-    from helpers import load_query_case
-    case = load_query_case("g_smallmap")
-    got = _run_query_tc(emu_query_tc, tmp_path, case, n, 3, sms, {"MONOPORT_B200_TC_CG": "2"})
-    want = _run_query_tc(emu_query_tc, tmp_path, case, n, 3, sms, {"MONOPORT_B200_TC_WM": "0"})
-    assert torch.equal(got, want), "the CTA-pair kernel must reproduce the one-CTA kernel bit for bit"
-    err = (got - case["expected"][:, :n]).abs().max().item()
-    assert err <= 1e-4, err
-
-
-@pytest.mark.parametrize("flavour", ["plain", "multicast", "pair"])
-@pytest.mark.parametrize("order", ["mmas", "random:1", "random:2"])
-def test_tcgen05_handoffs_survive_other_completion_orders(emu_query_tc, tmp_path, flavour, order):
-    """The model completes queued asynchronous operations in an adversarial but fixed order (bulk copies before MMAs).  The
-    hand-off protocols must not depend on that: MMAs first, and random interleavings (copies in any order), give the same bits
-    for the one-CTA launch, the weight-multicast clusters and the CTA-pair kernel."""
-    import torch
-    from helpers import load_query_case
-    case = load_query_case("g_smallmap")
-    env = {"plain": {"MONOPORT_B200_TC_WM": "0"}, "multicast": {"MONOPORT_B200_TC_WM": "1"}, "pair": {"MONOPORT_B200_TC_CG": "2"}}[flavour]
-    want = _run_query_tc(emu_query_tc, tmp_path, case, 300, 3, 2, {"MONOPORT_B200_TC_WM": "0"})
-    got = _run_query_tc(emu_query_tc, tmp_path, case, 300, 3, 2, dict(env, EMU_TC_ORDER=order))
+    case = load_query_case(name)
+    want = _run_query_tc(emu_query_tc, tmp_path, case, n, program, sms)
+    got = _run_query_tc(emu_query_tc, tmp_path, case, n, program, sms, dict(EMU_TC_ORDER=order))
     assert torch.equal(got, want)
+    assert (got - case["expected"][:, :n]).abs().max().item() <= 1e-4
 
 
 @pytest.mark.parametrize("order", ["copies", "random:3"])
 def test_tcgen05_colour_head_matches_reference_golden(emu_query_tc, tmp_path, order):
-    """PIFuNetCMLP (513 -> 3, Tanh, 512-channel map): the phase-filled skip operand (four fills of X per tile), eight-K-block
-    G0 GEMM, three fp32 last-layer outputs; one emulated SM walks both tiles (default completion order of the asynchronous
-    engines and a random one)."""
+    """PIFuNetCMLP (513 -> 3, Tanh, 512-channel map): the 512-channel skip operand, the (hi, lo) pass of layer 3, eight-K-block
+    G0 GEMM, three fp32 last-layer outputs; one emulated SM walks all four tiles (default completion order of the bulk
+    copies and a random one)."""
     from helpers import load_query_case
     case = load_query_case("c_rot33")
     n = 200
@@ -404,8 +378,7 @@ def test_tcgen05_colour_head_fused_surface_rendering(emu_query_tc, tmp_path):
         for W, b in zip(Ws, bs):
             f.write(W.numpy().tobytes())
             f.write(b.numpy().tobytes())
-    r = subprocess.run([emu_query_tc, fin, fout, "0", "2", "surface", str(R)], capture_output=True, text=True, timeout=900,
-                       env=dict(os.environ, MONOPORT_B200_TC_NETC="1"))
+    r = subprocess.run([emu_query_tc, fin, fout, "0", "2", "surface", str(R)], capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stderr[-2000:]
     got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(R, R, 3)
 

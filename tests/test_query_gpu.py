@@ -51,7 +51,7 @@ def test_query_matches_reference_golden(name):
 def test_tc_mode_is_available_for_shipped_heads():
     c = load_query_case("g_identity")
     net = build_net(c)
-    assert net.surface_classifier.tc_supported(), "tcgen05 kernel must support PIFuNetGMLP on sm_100a"
+    assert net.surface_classifier.tc_supported(), "the wgmma kernel must support PIFuNetGMLP on sm_90a"
 
 
 def test_point_layouts_and_ragged_sizes():

@@ -1,7 +1,6 @@
 """compute-sanitizer memcheck over one small invocation of every kernel family (tools/san_check.py).  Opt-in
 (MONOPORT_B200_RUN_SANITIZER=1): the instrumented run takes minutes, the plain GPU suite seconds.
-    MONOPORT_B200_RUN_SANITIZER=1 python -m pytest tests/test_sanitizer_gpu.py -m gpu -q
-The last log of such a run is kept under profiles/ (r02_sanitizer_memcheck.log)."""
+    MONOPORT_B200_RUN_SANITIZER=1 python -m pytest tests/test_sanitizer_gpu.py -m gpu -q"""
 import os
 import shutil
 import subprocess

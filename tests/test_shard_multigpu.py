@@ -1,4 +1,4 @@
-"""Multi-GPU (>= 2 B200s on the box; skipped otherwise): z-slab sharded volumes -- through the NCCL all-gather and through
+"""Multi-GPU (>= 2 GPUs on the box; skipped otherwise): z-slab sharded volumes -- through the NCCL all-gather and through
 the fused peer-memory epilogue (mp_query_grid_peers) -- are bit-identical to the single-GPU volume on every rank."""
 import os
 import subprocess

@@ -1,4 +1,4 @@
-"""GPU check of the tcgen05 G0 GEMM (layer 0 hoisted to texels): program v3 vs. the oracle at several sizes, and the cost
+"""GPU check of the G0 GEMM (layer 0 hoisted to texels) vs. the oracle at several sizes, and the cost
 of one per-frame refresh (query after a feature upload vs. query on an unchanged feature map)."""
 import sys, os
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))

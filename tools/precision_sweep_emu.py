@@ -1,4 +1,4 @@
-"""Precision sweep of the tensor-core programs on the CPU model of the tcgen05 layer (no GPU needed):
+"""Precision sweep of the tensor-core programs on the CPU model of the wgmma layer (no GPU needed):
 max / mean |kernel - oracle| of query() outputs over seeded heads x feature maps x calibrations.
 Usage: python tools/precision_sweep_emu.py [n_seeds] [n_points] [map_size]   (builds tests/emu/emu_query_tc.cpp into /tmp)"""
 import os, struct, subprocess, sys
@@ -30,8 +30,7 @@ for net, chans, last in (("G", spec.G_CHANNELS, spec.LAST_SIGMOID), ("C", spec.C
                 f.write(feat.numpy().tobytes()); f.write(pts[0].numpy().tobytes())
                 for W, b in zip(Ws, bs):
                     f.write(W.numpy().tobytes()); f.write(b.numpy().tobytes())
-            r = subprocess.run([exe, "/tmp/sweep_in.bin", "/tmp/sweep_out.f32", str(prog), "4"], capture_output=True, text=True,
-                               env=dict(os.environ, MONOPORT_B200_TC_NETC="1"))
+            r = subprocess.run([exe, "/tmp/sweep_in.bin", "/tmp/sweep_out.f32", str(prog), "4"], capture_output=True, text=True)
             assert r.returncode == 0, r.stderr
             got = torch.from_numpy(np.fromfile("/tmp/sweep_out.f32", dtype=np.float32)).reshape(chans[-1], N)
             e = (got - want).abs()

@@ -1,4 +1,4 @@
-"""Quick GPU check of the tcgen05 query kernel against the oracle (small sizes first so a hang shows early)."""
+"""Quick GPU check of the tensor-core query kernel against the oracle (small sizes first so a hang shows early)."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
