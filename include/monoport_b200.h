@@ -93,6 +93,15 @@ int mp_feat_upload(mp_feat_t* h, const float* nchw, int on_device, void* stream)
 int mp_feat_bind_nhwc(mp_feat_t* h, const float* nhwc_dev, void* stream);
 int mp_feat_upload_nhwc(mp_feat_t* h, const float* nhwc_dev, void* stream);
 int mp_feat_destroy(mp_feat_t* h);
+/* A handle that holds B maps of [C,H,W] -- the features of a batch [B,C,H,W] (MonoPortNet.py:48-91 takes any B).
+ * mp_feat_create(C,H,W) is the B = 1 case.  On such a handle the three calls above read B contiguous maps: mp_feat_upload a
+ * [B,C,H,W] NCHW block, mp_feat_upload_nhwc / mp_feat_bind_nhwc a [B,H,W,C] block (the memory of a torch.channels_last
+ * [B,C,H,W] tensor).  Only mp_query_points_batch evaluates a handle with B > 1; every other entry point that takes an
+ * mp_feat_t* returns MP_E_INVALID for it.
+ * Memory: besides the B fp32 maps (and a staging copy for host uploads) the tensor-core program keeps per-texel products for
+ * every map -- per 128 x 128 map, G0 = 33.5 MB and the fp16 copy of the map 8.4 MB (16.8 MB for the colour head's 512
+ * channels): a batch of 8 geometry maps holds about 0.34 GB of them. */
+int mp_feat_create_batch(int B, int C, int H, int W, mp_feat_t** out);
 
 /* calib: 12 host floats = rows 0..2 of the [4,4] / [3,4] calibration (R | t), or NULL for calibs=None
  * (MonoPortNet.py:66-67).  z_scale = DepthNormalizer scale (normalizers/DepthNormalizer.py:32,40). */
@@ -104,6 +113,15 @@ int mp_feat_destroy(mp_feat_t* h);
 int mp_query_points(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
                     int64_t point_stride, const float* calib12, int projection, float z_scale, float* out_dev,
                     int64_t ld_out, int mode, void* stream);
+/* MonoPortNet.query(feats[B,C,H,W], points[B,3,N], calibs[B,3|4,4]) -> [B,Res,N] in ONE launch (tiles of 64 points never
+ * straddle two images).  B must equal the handle's batch (mp_feat_create_batch).  Coordinate a of point i of image b lives
+ * at points_dev[b*batch_stride + a*row_stride + i*point_stride]; its channel c goes to out_dev[b*out_batch_stride +
+ * c*ld_out + i].  calibs_dev: [B][12] fp32 in DEVICE memory (rows 0..2 of every [R|t]) or NULL for calibs=None -- nothing is
+ * read back to the host, the call does not synchronise.  All modes; MP_MODE_TC / MP_MODE_AUTO take the range guard per
+ * image: the tiles of an image whose largest |feature| is above the head's limit are evaluated by the exact fp32 kernel. */
+int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n, int64_t batch_stride,
+                          int64_t row_stride, int64_t point_stride, const float* calibs_dev, int projection, float z_scale,
+                          float* out_dev, int64_t out_batch_stride, int64_t ld_out, int mode, void* stream);
 /* Same call with HOST buffers (points [3,N], out [Res,N], feature map NCHW fp32 or NULL to reuse the
  * uploaded one): copies in, runs, copies out, synchronises.  This is what bench.py's e2e leg times. */
 int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,

@@ -39,6 +39,9 @@ SIGNATURES = {
     "mp_feat_upload_nhwc": (c_int, [c_void_p, c_void_p, c_void_p]),
     "mp_feat_bind_nhwc": (c_int, [c_void_p, c_void_p, c_void_p]),
     "mp_feat_destroy": (c_int, [c_void_p]),
+    "mp_feat_create_batch": (c_int, [c_int, c_int, c_int, c_int, P(c_void_p)]),
+    "mp_query_points_batch": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int,
+                                      c_float, c_void_p, c_int64, c_int64, c_int, c_void_p]),
     "mp_query_points": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
                                 c_void_p, c_int64, c_int, c_void_p]),
     "mp_query_points_host": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, P(c_float), c_int, c_float,

@@ -169,20 +169,21 @@ extern "C" int mp_feat_destroy(mp_feat_t* h) {
   return MP_OK;
 }
 
-extern "C" int mp_feat_create(int C, int H, int W, mp_feat_t** out) {
+extern "C" int mp_feat_create_batch(int B, int C, int H, int W, mp_feat_t** out) {
   MP_REQUIRE(out != nullptr, "out is NULL");
   *out = nullptr;
   MP_REQUIRE(C >= 1 && H >= 1 && W >= 1 && (long long)C * H * W < (1ll << 31), "bad feature shape %dx%dx%d", C, H, W);
+  MP_REQUIRE(B >= 1 && (long long)B * C * H * W < (1ll << 40), "bad batch size %d for %dx%dx%d maps", B, C, H, W);
   mp_feat* h = new mp_feat();
   memset(h, 0, sizeof(*h));
-  h->C = C; h->H = H; h->W = W;
+  h->B = B; h->C = C; h->H = H; h->W = W;
   cudaGetDevice(&h->device);
-  const size_t n = (size_t)C * H * W;
+  const size_t n = (size_t)B * C * H * W;
   cudaError_t e = cudaMalloc(&h->nhwc_own, n * sizeof(float));
   h->nhwc32 = h->nhwc_own;
   if (e == cudaSuccess) e = cudaMalloc(&h->staging, n * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->amax, sizeof(unsigned));
-  if (e == cudaSuccess) e = cudaMemset(h->amax, 0, sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMalloc(&h->amax, B * sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMemset(h->amax, 0, B * sizeof(unsigned));
   if (e != cudaSuccess) {
     mp_set_error("mp_feat_create: %s", cudaGetErrorString(e));
     mp_feat_destroy(h);
@@ -192,22 +193,24 @@ extern "C" int mp_feat_create(int C, int H, int W, mp_feat_t** out) {
   return MP_OK;
 }
 
+extern "C" int mp_feat_create(int C, int H, int W, mp_feat_t** out) { return mp_feat_create_batch(1, C, H, W, out); }
+
 extern "C" int mp_feat_upload(mp_feat_t* h, const float* nchw, int on_device, void* stream) {
   MP_REQUIRE(h && nchw, "NULL handle or data");
   MpRange nvtx("monoport_b200: feature upload (channel-last repack)");
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t n = (size_t)h->C * h->H * h->W;
+  const size_t per_map = (size_t)h->C * h->H * h->W;
   const float* src = nchw;
   if (!on_device) {
-    MP_CUDA(cudaMemcpyAsync(h->staging, nchw, n * sizeof(float), cudaMemcpyHostToDevice, st));
+    MP_CUDA(cudaMemcpyAsync(h->staging, nchw, h->B * per_map * sizeof(float), cudaMemcpyHostToDevice, st));
     src = h->staging;
   }
   const int HW = h->H * h->W;
   dim3 grid((HW + 31) / 32, (h->C + 31) / 32), block(32, 8);
   h->nhwc32 = h->nhwc_own;
-  nchw_to_nhwc_kernel<<<grid, block, 0, st>>>(src, h->nhwc32, h->C, HW);
+  for (int b = 0; b < h->B; ++b) nchw_to_nhwc_kernel<<<grid, block, 0, st>>>(src + b * per_map, h->nhwc32 + b * per_map, h->C, HW);
   MP_CUDA(cudaGetLastError());
-  MP_CUDA(cudaMemsetAsync(h->amax, 0, sizeof(unsigned), st));
+  MP_CUDA(cudaMemsetAsync(h->amax, 0, h->B * sizeof(unsigned), st));
   h->version += 1;
   return MP_OK;
 }
@@ -216,10 +219,10 @@ extern "C" int mp_feat_upload(mp_feat_t* h, const float* nchw, int on_device, vo
 // SURVEY.md §8f-3): one device-to-device copy instead of the transposing kernel.
 extern "C" int mp_feat_upload_nhwc(mp_feat_t* h, const float* nhwc_dev, void* stream) {
   MP_REQUIRE(h && nhwc_dev, "NULL handle or data");
-  const size_t n = (size_t)h->C * h->H * h->W;
+  const size_t n = (size_t)h->B * h->C * h->H * h->W;
   h->nhwc32 = h->nhwc_own;
   MP_CUDA(cudaMemcpyAsync(h->nhwc32, nhwc_dev, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  MP_CUDA(cudaMemsetAsync(h->amax, 0, sizeof(unsigned), (cudaStream_t)stream));
+  MP_CUDA(cudaMemsetAsync(h->amax, 0, h->B * sizeof(unsigned), (cudaStream_t)stream));
   h->version += 1;
   return MP_OK;
 }
@@ -230,7 +233,7 @@ extern "C" int mp_feat_bind_nhwc(mp_feat_t* h, const float* nhwc_dev, void* stre
   MP_REQUIRE(h && nhwc_dev, "NULL handle or data");
   MP_REQUIRE((reinterpret_cast<uintptr_t>(nhwc_dev) & 15) == 0, "the channel-last map must be 16-byte aligned");
   h->nhwc32 = const_cast<float*>(nhwc_dev);
-  MP_CUDA(cudaMemsetAsync(h->amax, 0, sizeof(unsigned), (cudaStream_t)stream));
+  MP_CUDA(cudaMemsetAsync(h->amax, 0, h->B * sizeof(unsigned), (cudaStream_t)stream));
   h->version += 1;
   return MP_OK;
 }
@@ -259,8 +262,9 @@ void mp_fill_grid_geom(MpPointSrc& s, int res, int node_stride, int r_final, con
 }
 
 int mp_query_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
-                      int mode, cudaStream_t st) {
+                      int mode, cudaStream_t st, const MpBatch* bt) {
   MpRange nvtx("monoport_b200: F1 fused sample+MLP query");
+  // (bt: a batched launch; the guard below is then decided per tile, from the maximum of the tile's image)
   // the tensor-core program covers maps of at most 65536 texels (16-bit texel indices in registers)
   const bool tc_can = mlp->tc_ok && (long long)feat->H * feat->W <= 65536;
   if (mode == MP_MODE_AUTO) mode = tc_can ? MP_MODE_TC : MP_MODE_FP32;
@@ -274,23 +278,35 @@ int mp_query_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const M
     // maximum (no host synchronisation, graph-capturable): the tensor-core launch runs when the frame is in range, the
     // exact fp32 launch when it is not; the other one returns at once.
     const bool guarded = isfinite(mlp->tc_amax_limit);
-    int rc = mp_launch_query_tc(mlp, feat, src, cal, dst, st, guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE);
+    int rc = mp_launch_query_tc(mlp, feat, src, cal, dst, st, guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE, bt);
     if (rc != MP_OK || !guarded) return rc;
-    return mp_launch_query_fp32(mlp, feat, src, cal, dst, st, MP_GUARD_OUT_OF_RANGE);
+    return mp_launch_query_fp32(mlp, feat, src, cal, dst, st, MP_GUARD_OUT_OF_RANGE, bt);
   }
   if (mode != MP_MODE_FP32) {
     mp_set_error("bad mode %d (3 was the removed MP_MODE_TC_V2)", mode);
     return MP_E_INVALID;
   }
-  return mp_launch_query_fp32(mlp, feat, src, cal, dst, st);
+  return mp_launch_query_fp32(mlp, feat, src, cal, dst, st, MP_GUARD_NONE, bt);
 }
 
-extern "C" int mp_query_points(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
-                               int64_t point_stride, const float* calib12, int projection, float z_scale,
-                               float* out_dev, int64_t ld_out, int mode, void* stream) {
+// mp_query_points and mp_query_points_batch: B images of n points.  calibs_dev == nullptr: the single-map call, whose calib
+// (calib12, host memory, or none) travels in the kernel parameters; otherwise B calibs in device memory and a batched launch.
+static int query_points(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n, int64_t batch_stride,
+                        int64_t row_stride, int64_t point_stride, const float* calib12, const float* calibs_dev, int projection,
+                        float z_scale, float* out_dev, int64_t out_batch_stride, int64_t ld_out, int mode, void* stream,
+                        bool batched) {
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE(n >= 0 && row_stride >= 1 && point_stride >= 1 && ld_out >= n, "bad sizes n=%lld strides=%lld,%lld ld_out=%lld",
              (long long)n, (long long)row_stride, (long long)point_stride, (long long)ld_out);
+  if (batched) {
+    MP_REQUIRE(B == feat->B, "batch size %d does not match the feature handle's %d maps", B, feat->B);
+    MP_REQUIRE(B == 1 || (batch_stride >= 1 && out_batch_stride >= 1), "bad batch strides %lld, %lld", (long long)batch_stride,
+               (long long)out_batch_stride);
+    // (the kernels find a tile's image with a 32-bit division: at most 2^31 tiles of 8 points per launch)
+    MP_REQUIRE((long long)B * ((n + 7) / 8) < (1ll << 31), "batch too large: %d x %lld points", B, (long long)n);
+  } else {
+    MP_REQUIRE_SINGLE_MAP(feat, "mp_query_points");
+  }
   if (n == 0) return MP_OK;
   MP_REQUIRE(points_dev && out_dev, "NULL points/out");
   MpPointSrc src;
@@ -303,13 +319,37 @@ extern "C" int mp_query_points(mp_mlp_t* mlp, mp_feat_t* feat, const float* poin
   mp_fill_calib(cal, calib12, projection, z_scale);
   MpOutDst dst;
   dst.out = out_dev; dst.ld = ld_out; dst.scatter_vol = nullptr;
-  return mp_query_dispatch(mlp, feat, src, cal, dst, mode, (cudaStream_t)stream);
+  if (!batched) return mp_query_dispatch(mlp, feat, src, cal, dst, mode, (cudaStream_t)stream);
+  MpBatch bt;
+  bt.B = B;
+  bt.pt_stride = batch_stride;
+  bt.out_stride = out_batch_stride;
+  bt.calibs = calibs_dev;
+  cal.has = calibs_dev != nullptr;
+  cal.perspective = projection == MP_PROJ_PERSPECTIVE && cal.has;
+  return mp_query_dispatch(mlp, feat, src, cal, dst, mode, (cudaStream_t)stream, &bt);
+}
+
+extern "C" int mp_query_points(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                               int64_t point_stride, const float* calib12, int projection, float z_scale,
+                               float* out_dev, int64_t ld_out, int mode, void* stream) {
+  return query_points(mlp, feat, 1, points_dev, n, 0, row_stride, point_stride, calib12, nullptr, projection, z_scale, out_dev, 0,
+                      ld_out, mode, stream, false);
+}
+
+extern "C" int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
+                                     int64_t batch_stride, int64_t row_stride, int64_t point_stride, const float* calibs_dev,
+                                     int projection, float z_scale, float* out_dev, int64_t out_batch_stride, int64_t ld_out,
+                                     int mode, void* stream) {
+  return query_points(mlp, feat, B, points_dev, n, batch_stride, row_stride, point_stride, nullptr, calibs_dev, projection, z_scale,
+                      out_dev, out_batch_stride, ld_out, mode, stream, true);
 }
 
 extern "C" int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,
                                     int64_t n, const float* calib12, int projection, float z_scale, float* out_host,
                                     int mode, void* stream) {
   MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE_SINGLE_MAP(feat, "mp_query_points_host");
   MP_REQUIRE(n >= 0, "bad n");
   cudaStream_t st = (cudaStream_t)stream;
   if (feat_nchw_host) {
@@ -346,6 +386,7 @@ static int query_grid_range(mp_mlp_t* mlp, mp_feat_t* feat, int R, long long lin
                             const float* b_max3, const float* calib12, int projection, float z_scale, float* out_dev,
                             float* const* peer_vols, int n_peers, int mode, void* stream) {
   MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE_SINGLE_MAP(feat, "the grid query");
   MP_REQUIRE(R >= 1 && lin0 >= 0 && n >= 0 && lin0 + n <= (long long)R * R * R, "bad range R=%d lin0=%lld n=%lld", R, lin0, n);
   MP_REQUIRE(b_min3 && b_max3, "NULL bounds");
   MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "grid queries need a single-channel head");
@@ -410,6 +451,7 @@ extern "C" int mp_colorize_surface(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t
                                    int64_t n, int R, const float* b_min3, const float* b_max3, const float* calib12, int projection,
                                    float z_scale, float* canvas_dev, void* stream) {
   MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE_SINGLE_MAP(feat, "mp_colorize_surface");
   MP_REQUIRE(n >= 0 && R >= 1, "bad sizes n=%lld R=%d", (long long)n, R);
   if (n == 0) return MP_OK;
   MP_REQUIRE(x_dev && y_dev && z_dev && canvas_dev && b_min3 && b_max3, "NULL argument");
@@ -461,6 +503,7 @@ extern "C" int mp_query_grid_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* f
                                   const float* b_min3, const float* b_max3, const float* calib12, int projection,
                                   float z_scale, float* out_host, int mode, void* stream) {
   MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE_SINGLE_MAP(feat, "mp_query_grid_host");
   MP_REQUIRE(R >= 1 && z0 >= 0 && nz >= 0 && z0 + nz <= R, "bad slab R=%d z0=%d nz=%d", R, z0, nz);
   cudaStream_t st = (cudaStream_t)stream;
   if (feat_nchw_host) {

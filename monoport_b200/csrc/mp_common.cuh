@@ -58,6 +58,11 @@ void mp_ensure_pool();
     }                              \
   } while (0)
 
+// entry points that evaluate one map refuse a batch handle instead of silently evaluating its image 0
+#define MP_REQUIRE_SINGLE_MAP(feat, what)                                                                          \
+  MP_REQUIRE((feat)->B == 1, "%s takes a single-map feature handle, this one holds %d maps (batched queries: "      \
+             "mp_query_points_batch)", what, (feat)->B)
+
 // ---------------------------------------------------------------------------------------------
 // handles
 // ---------------------------------------------------------------------------------------------
@@ -85,6 +90,8 @@ struct mp_mlp {
 
 struct mp_feat {
   int C, H, W;
+  int B;            // maps held (mp_feat_create: 1; mp_feat_create_batch: B).  Every per-texel array below is B
+                    // consecutive per-image blocks, image b's at offset b * (its per-image size); amax has B entries.
   float* nhwc32;    // [H][W][C] fp32 (one bilinear tap = one contiguous C*4-byte vector): the CURRENT map -- the handle's own
                     // repacked copy (nhwc_own) or, after mp_feat_bind_nhwc, the caller's channel-last tensor itself
   float* nhwc_own;
@@ -143,6 +150,17 @@ struct MpCalib {
   float z_scale;
 };
 
+// A batched query (mp_query_points_batch): B images of n points each, evaluated by one launch whose tiles never straddle
+// two images (tile t belongs to image t / tiles_per_image).  Image b reads its points at px/py/pz + b * pt_stride, its
+// calibration (rows 0..2 of [R|t], when MpCalib::has) from calibs[12 b ..] in device memory, its map's per-texel arrays at
+// the per-image offsets of mp_feat, and writes its outputs at out + b * out_stride.
+struct MpBatch {
+  int B;
+  long long pt_stride;
+  long long out_stride;
+  const float* calibs;   // [B][12] device
+};
+
 // where results go
 #define MP_MAX_PEERS 8
 struct MpOutDst {
@@ -190,6 +208,32 @@ __device__ __forceinline__ void mp_load_point(const MpPointSrc& s, long long i, 
   x = __fadd_rn(__fmul_rn(__fadd_rn(__fdiv_rn(cx, R), s.half_inv_r), s.bext[0]), s.bmin[0]);
   y = __fadd_rn(__fmul_rn(__fadd_rn(__fdiv_rn(cy, R), s.half_inv_r), s.bext[1]), s.bmin[1]);
   z = __fadd_rn(__fmul_rn(__fadd_rn(__fdiv_rn(cz, R), s.half_inv_r), s.bext[2]), s.bmin[2]);
+}
+
+// image of tile t of a batched launch.  mp_query_points_batch keeps the launch under 2^31 tiles, so this is a 32-bit
+// division (a 64-bit one is a call, whose saved registers would spill in the tensor-core program)
+__device__ __forceinline__ int mp_tile_image(long long t, long long tiles_per_image) {
+  return (int)((unsigned)t / (unsigned)tiles_per_image);
+}
+
+// point i of image b of a batched launch (MP_SRC_ROWS)
+__device__ __forceinline__ void mp_load_image_point(const MpPointSrc& s, const MpBatch& bt, int b, long long i, float& x, float& y,
+                                                    float& z) {
+  const long long o = (long long)b * bt.pt_stride + i * s.pstride;
+  x = __ldg(s.px + o);
+  y = __ldg(s.py + o);
+  z = __ldg(s.pz + o);
+}
+
+// image b's calibration of a batched launch (the same projection and depth scale, its own [R|t] rows)
+__device__ __forceinline__ MpCalib mp_image_calib(const MpCalib& c, const MpBatch& bt, int b) {
+  MpCalib r;
+  r.has = c.has;
+  r.perspective = c.perspective;
+  r.z_scale = c.z_scale;
+#pragma unroll
+  for (int k = 0; k < 12; ++k) r.m[k] = c.has ? __ldg(bt.calibs + 12 * (long long)b + k) : 0.f;
+  return r;
 }
 
 // the window [i0, i1) of a query's n points that this launch evaluates (see MpPointSrc::shard_rank)
@@ -260,12 +304,15 @@ __device__ __forceinline__ float mp_lrelu(float v) { return v > 0.f ? v : v * MP
 // host-side launchers implemented in the kernel files
 // `guard`: the launch is conditional on the frame's feature range (feat->amax vs mlp->tc_amax_limit), evaluated on the device:
 //   MP_GUARD_NONE always run, MP_GUARD_IN_RANGE run when max|feature| <= limit, MP_GUARD_OUT_OF_RANGE run when it is above.
+// `bt` (batched launches only, nullptr otherwise): the launch covers bt->B images of src.n points; the guard is then
+// decided per tile from the maximum of the tile's own image (feat->amax[b]).
 enum { MP_GUARD_NONE = 0, MP_GUARD_IN_RANGE = 1, MP_GUARD_OUT_OF_RANGE = 2 };
 int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
-                         const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE);
+                         const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
-                       const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE);
-// device-side predicate shared by the kernels: true = this launch must do nothing
+                       const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
+// device-side predicate shared by the kernels: true = this launch (batched: this tile, amax = its image's entry) must do
+// nothing.  In the tensor-core program the weight producer and the consumers both take it, per tile, from the same word.
 __device__ __forceinline__ bool mp_guard_skips(const unsigned* amax, float limit, int guard) {
   if (guard == MP_GUARD_NONE || amax == nullptr) return false;
   const bool above = __uint_as_float(*amax) > limit;
@@ -279,6 +326,6 @@ void mp_tc_release(mp_mlp* mlp);
 
 // generic query dispatch (mode handling) used by the API and the octree engine
 int mp_query_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
-                      int mode, cudaStream_t st);
+                      int mode, cudaStream_t st, const MpBatch* bt = nullptr);
 void mp_fill_calib(MpCalib& c, const float* calib12, int projection, float z_scale);
 void mp_fill_grid_geom(MpPointSrc& s, int res, int node_stride, int r_final, const float* bmin, const float* bmax);

@@ -546,6 +546,7 @@ static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const 
 extern "C" int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib12, int projection,
                                          float z_scale, int mode, float* out_dev, void* stream) {
   MP_REQUIRE(h && mlp && feat && out_dev, "NULL argument");
+  MP_REQUIRE_SINGLE_MAP(feat, "the occupancy engine");
   MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "the occupancy engine needs a single-channel head");
   MP_REQUIRE(h->use_topk || h->faster, "the lossless engine's conflict loop reads counts on the host; use mp_octree_run_fused");
   MpRange nvtx("monoport_b200: F2 coarse-to-fine engine (enqueue)");
@@ -583,6 +584,7 @@ extern "C" int mp_octree_run_fused(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* fea
                                    float z_scale, int mode, float* out_dev, int* nonempty, int64_t* stats_host,
                                    void* stream) {
   MP_REQUIRE(h && mlp && feat && out_dev && nonempty, "NULL argument");
+  MP_REQUIRE_SINGLE_MAP(feat, "the occupancy engine");
   MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "the occupancy engine needs a single-channel head");
   MpRange nvtx("monoport_b200: F2 coarse-to-fine engine");
   cudaStream_t st = (cudaStream_t)stream;

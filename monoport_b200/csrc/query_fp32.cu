@@ -117,9 +117,11 @@ __device__ void dense_layer(const float* __restrict__ wt, const float* __restric
   }
 }
 
-template <int P>
+// BATCH: bt.B images of src.n points (MP_SRC_ROWS); tile t is tile t % n_tiles of image t / n_tiles, which samples its own
+// map and calibration and writes its own outputs; the range guard is decided per tile from that image's maximum.
+template <int P, bool BATCH = false>
 __global__ void __launch_bounds__(kThreads, 1)
-query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst) {
+query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpBatch bt) {
   MP_DYN_SMEM_ALIGNED(float, smem, 16);
   float* sX = smem;                                  // [c0][P]
   float* sA = sX + (size_t)prm.c0 * P;               // [h_ping][P]
@@ -127,7 +129,9 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst) {
   float* sMeta = sB + (size_t)prm.h_pong * P;        // [8][P]: in_img, u, v, z_feat, (4 spare)
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
-  if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid)
+  if constexpr (!BATCH) {
+    if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid)
+  }
 
   long long n = src.n;
   if (src.count_dev) {
@@ -137,9 +141,15 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst) {
   long long win0, win1;
   mp_shard_window(src, n, win0, win1);
   n = win1;                                          // points >= n are padding; the first evaluated one is win0
-  const long long n_tiles = (win1 - win0 + P - 1) / P;
+  const long long n_tiles = (win1 - win0 + P - 1) / P;          // (per image)
+  const long long all_tiles = BATCH ? n_tiles * bt.B : n_tiles;
 
-  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+  for (long long at = blockIdx.x; at < all_tiles; at += gridDim.x) {
+    const int b = BATCH ? mp_tile_image(at, n_tiles) : 0;
+    if (BATCH && mp_guard_skips(prm.amax + b, prm.amax_limit, prm.guard)) continue;      // (uniform over the CTA)
+    const long long tile = BATCH ? at - (long long)b * n_tiles : at;
+    const float* feat = BATCH ? prm.feat + (size_t)b * prm.H * prm.W * prm.C : prm.feat;
+    float* out = BATCH ? dst.out + b * bt.out_stride : dst.out;
     const long long p0 = win0 + tile * P;
     // ---- 1. projection, mask, taps ------------------------------------------------------------
     __shared__ int sOff[4][P];
@@ -150,8 +160,13 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst) {
       bool valid = i < n;
       if (valid) {
         float x, y, z;
-        mp_load_point(src, i, x, y, z);
-        mp_project(cal, x, y, z, u, v, w);
+        if constexpr (BATCH) {
+          mp_load_image_point(src, bt, b, i, x, y, z);
+          mp_project(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
+        } else {
+          mp_load_point(src, i, x, y, z);
+          mp_project(cal, x, y, z, u, v, w);
+        }
       }
       const bool in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);   // MonoPortNet.py:74
       MpTaps t = mp_taps(valid ? u : 0.f, valid ? v : 0.f, prm.H, prm.W);
@@ -168,10 +183,10 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst) {
     __syncthreads();
     // ---- 2. bilinear gather: warp per point, lanes over channels (NHWC => contiguous) ---------
     for (int p = warp; p < P; p += kThreads / 32) {
-      const float* f0 = prm.feat + (size_t)sOff[0][p] * prm.C;
-      const float* f1 = prm.feat + (size_t)sOff[1][p] * prm.C;
-      const float* f2 = prm.feat + (size_t)sOff[2][p] * prm.C;
-      const float* f3 = prm.feat + (size_t)sOff[3][p] * prm.C;
+      const float* f0 = feat + (size_t)sOff[0][p] * prm.C;
+      const float* f1 = feat + (size_t)sOff[1][p] * prm.C;
+      const float* f2 = feat + (size_t)sOff[2][p] * prm.C;
+      const float* f3 = feat + (size_t)sOff[3][p] * prm.C;
       const float w0 = sWgt[0][p], w1 = sWgt[1][p], w2 = sWgt[2][p], w3 = sWgt[3][p];
       for (int c = lane; c < prm.C; c += 32) {
         // same accumulation order as grid_sample: nw, ne, sw, se
@@ -222,7 +237,7 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst) {
           if (i < n) {
             float v = mp_last_op(acc + __ldg(prm.bias[l] + r), prm.last_op);
             v = sMeta[p] * v;                                                              // MonoPortNet.py:89
-            if (dst.out) dst.out[(long long)r * dst.ld + i] = v;
+            if (out) out[(long long)r * dst.ld + i] = v;
             if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = v;
             if (r == 0)
               for (int pp = 0; pp < dst.n_peers; ++pp) dst.peer[pp][dst.peer_off + i] = v;      // peer-memory stores (NVLink)
@@ -236,22 +251,34 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst) {
 
 template <int P>
 int launch(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst, cudaStream_t st,
-           int sm_count) {
+           int sm_count, int max_smem, const MpBatch* bt) {
   const size_t smem = Fp32Smem<P>::bytes(prm.c0, prm.h_ping, prm.h_pong);
-  // (the opt-in is sticky per device: raising it again for every launch costs a driver call per query)
-  static thread_local size_t opted[64] = {};
+  // The opt-in is a property of the kernel, shared by every thread, and heads of different widths launch the same
+  // instantiation with different sizes: it is always set to the same bound -- the device's maximum less the 2 KB the size
+  // selection below keeps free for the kernel's static shared memory -- so no thread lowers it under another thread's
+  // launch.  (Sticky per device: raising it again for every launch costs a driver call per query.)
+  const int opt_in = max_smem - 2048;
+  static thread_local bool opted[2][64] = {};
+  const int variant = bt ? 1 : 0;
   int dev_ = 0;
   MP_CUDA(cudaGetDevice(&dev_));
-  if (dev_ < 0 || dev_ >= 64 || opted[dev_] < smem) {
-    MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (dev_ >= 0 && dev_ < 64) opted[dev_] = smem;
+  if (dev_ < 0 || dev_ >= 64 || !opted[variant][dev_]) {
+    if (bt) MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
+    else MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
+    if (dev_ >= 0 && dev_ < 64) opted[variant][dev_] = true;
   }
-  long long tiles = (src.n + P - 1) / P;
+  long long tiles = (bt ? bt->B : 1) * ((src.n + P - 1) / P);
   int grid = (int)(tiles < (long long)sm_count ? (tiles > 0 ? tiles : 1) : sm_count);
+  MpBatch b1;
+  memset(&b1, 0, sizeof(b1));
+  const MpBatch& bb = bt ? *bt : b1;
 #ifndef MP_CUDA_EMU
-  query_fp32_kernel<P><<<grid, kThreads, smem, st>>>(prm, src, cal, dst);
+  if (bt) query_fp32_kernel<P, true><<<grid, kThreads, smem, st>>>(prm, src, cal, dst, bb);
+  else query_fp32_kernel<P><<<grid, kThreads, smem, st>>>(prm, src, cal, dst, bb);
 #else
-  MP_EMU_LAUNCH(grid, kThreads, query_fp32_kernel<P>(prm, src, cal, dst));      // tests/emu: CPU model of the execution model
+  // tests/emu: CPU model of the execution model
+  if (bt) MP_EMU_LAUNCH(grid, kThreads, (query_fp32_kernel<P, true>(prm, src, cal, dst, bb)));
+  else MP_EMU_LAUNCH(grid, kThreads, query_fp32_kernel<P>(prm, src, cal, dst, bb));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -260,7 +287,7 @@ int launch(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, con
 }  // namespace
 
 int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
-                         const MpOutDst& dst, cudaStream_t st, int guard) {
+                         const MpOutDst& dst, cudaStream_t st, int guard, const MpBatch* bt) {
   if (src.n <= 0) return MP_OK;
   Fp32Params prm;
   memset(&prm, 0, sizeof(prm));
@@ -303,9 +330,13 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
       if (dev >= 0 && dev < 64) { c_sms[dev] = sms; c_smem[dev] = max_smem; }
     }
   }
-  if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32>(prm, src, cal, dst, st, sms);
-  if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16>(prm, src, cal, dst, st, sms);
-  if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8>(prm, src, cal, dst, st, sms);
+  if (bt && (src.kind != MP_SRC_ROWS || dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
+    mp_set_error("batched launches take point rows and write [R,N] outputs");
+    return MP_E_UNSUPPORTED;
+  }
+  if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32>(prm, src, cal, dst, st, sms, max_smem, bt);
+  if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16>(prm, src, cal, dst, st, sms, max_smem, bt);
+  if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8>(prm, src, cal, dst, st, sms, max_smem, bt);
   mp_set_error("head too wide for the fp32 kernel's shared-memory tiling");
   return MP_E_UNSUPPORTED;
 }

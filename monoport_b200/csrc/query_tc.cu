@@ -14,7 +14,7 @@
 // Tanh output is four times as sensitive to the logit as the geometry head's Sigmoid, and the rounding of W3 is the largest
 // single term of its error.
 //
-// One persistent CTA per SM; a tile = 64 points = the M of every warpgroup MMA.  Warps 0-3 and 4-7 are two consumer
+// One persistent CTA per SM; a tile = 64 points = the M of every warpgroup MMA (a batched launch: of one image, see BATCH).  Warps 0-3 and 4-7 are two consumer
 // warpgroups that split the N dimension of every layer (layer 1: 256 columns each, 128 fp32 accumulators per thread;
 // layer 2: 128; layer 3: 64); both sample the operands (X, the layer-0 chunks) and run the epilogues.  Warp 8 streams the
 // weights L2 -> shared memory through a ring of 32 KB stages (cp.async.bulk on mbarriers), pre-packed on the host as
@@ -125,23 +125,30 @@ struct PointTaps {
   bool in_img;      // MonoPortNet.py:74
 };
 
-// projection (geometry.py:19-55) + mask + taps of point i (i >= n: masked-out padding point); surface vertices when surf.X
-__device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const MpPointSrc& src, const MpCalib& cal, int H, int W,
-                                                long long i, long long n) {
+// projection (geometry.py:19-55) + mask + taps of point i (i >= n: masked-out padding point); surface vertices when surf.X.
+// BATCH: point i of image b, projected with image b's calibration.
+template <bool BATCH>
+__device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
+                                                int b, int H, int W, long long i, long long n) {
   PointTaps pt;
   float u = 0.f, v = 0.f, w = 0.f;
   const bool valid = i < n;
   if (valid) {
     float x, y, z;
-    if (surf.X) {
-      const float vx = (float)__ldg(surf.X + i), vy = (float)__ldg(surf.Y + i), vz = __fsub_rn(surf.R, __ldg(surf.Z + i));
-      x = __fadd_rn(__fmul_rn(vx, surf.scale[0]), surf.bmin[0]);
-      y = __fadd_rn(__fmul_rn(vy, surf.scale[1]), surf.bmin[1]);
-      z = __fadd_rn(__fmul_rn(vz, surf.scale[2]), surf.bmin[2]);
+    if constexpr (BATCH) {
+      mp_load_image_point(src, bt, b, i, x, y, z);
+      mp_project(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
     } else {
-      mp_load_point(src, i, x, y, z);
+      if (surf.X) {
+        const float vx = (float)__ldg(surf.X + i), vy = (float)__ldg(surf.Y + i), vz = __fsub_rn(surf.R, __ldg(surf.Z + i));
+        x = __fadd_rn(__fmul_rn(vx, surf.scale[0]), surf.bmin[0]);
+        y = __fadd_rn(__fmul_rn(vy, surf.scale[1]), surf.bmin[1]);
+        z = __fadd_rn(__fmul_rn(vz, surf.scale[2]), surf.bmin[2]);
+      } else {
+        mp_load_point(src, i, x, y, z);
+      }
+      mp_project(cal, x, y, z, u, v, w);
     }
-    mp_project(cal, x, y, z, u, v, w);
   }
   pt.in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);
   const MpTaps t = mp_taps(valid ? u : 0.f, valid ? v : 0.f, H, W);
@@ -156,9 +163,10 @@ __device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const 
 // fp16 copy of the map, into rows [pbase, pbase+16) of the fp16 X tile (K-major SWIZZLE_128B; a lane covers 8 channels).
 // The last layer's direct feature access is NOT derived from these samples but from S4 (fp32, per texel), which the lane
 // owning the point interpolates in fp32 (phase 0).
+// (feat16 / s4tex: the fp16 map and the S4 products of the tile's image)
 template <int C>
-__device__ __forceinline__ void sample_x16(const TcParams& prm, uint8_t* smem_x, float* s_zf, float* s_in, float* s_s4,
-                                           const PointTaps& pt, int pbase, int lane, int phase) {
+__device__ __forceinline__ void sample_x16(const TcParams& prm, const __half* feat16, const float* s4tex, uint8_t* smem_x, float* s_zf,
+                                           float* s_in, float* s_s4, const PointTaps& pt, int pbase, int lane, int phase) {
   constexpr int RES = Prog<C>::RES;
   const int cbase = phase * 256 + lane * 8;
 #pragma unroll 1
@@ -171,7 +179,7 @@ __device__ __forceinline__ void sample_x16(const TcParams& prm, uint8_t* smem_x,
       for (int a = 0; a < 4; ++a) {
         const int off = __shfl_sync(0xffffffffu, pt.off[a], q0 + qq);
         wgt[qq][a] = __shfl_sync(0xffffffffu, pt.wgt[a], q0 + qq);
-        raw[qq][a] = __ldg(reinterpret_cast<const uint4*>(prm.feat16 + (size_t)off * C + cbase));
+        raw[qq][a] = __ldg(reinterpret_cast<const uint4*>(feat16 + (size_t)off * C + cbase));
       }
 #pragma unroll
     for (int qq = 0; qq < 4; ++qq) {
@@ -200,7 +208,7 @@ __device__ __forceinline__ void sample_x16(const TcParams& prm, uint8_t* smem_x,
     for (int r = 0; r < RES; ++r) {
       float s = 0.f;
 #pragma unroll
-      for (int a = 0; a < 4; ++a) s = fmaf(pt.wgt[a], __ldg(prm.s4tex + (size_t)pt.off[a] * RES + r), s);
+      for (int a = 0; a < 4; ++a) s = fmaf(pt.wgt[a], __ldg(s4tex + (size_t)pt.off[a] * RES + r), s);
       s_s4[r * kTile + pbase + lane] = s + __ldg(prm.w4z + r) * pt.zf + __ldg(prm.b4 + r);
     }
     s_zf[pbase + lane] = pt.zf;
@@ -221,11 +229,15 @@ __device__ __forceinline__ uint32_t act_pack(float a, float b) {
 // releases a stage once the MMAs that read it have completed (one arrival per consumer warp); the operand buffers written
 // by the consumers themselves are published with fence.proxy.async + a named barrier over the 256 consumer threads.
 // PEERS: also store channel 0 into the peer volumes of dst (fused slab exchange).
-template <int C, bool PEERS>
+// BATCH: bt.B images of src.n points (MP_SRC_ROWS, [R,N] outputs); tile t is tile t % n_tiles of image t / n_tiles, and the
+// range guard skips the tiles of the images outside the head's range -- the producer and the consumers skip exactly the
+// same tiles (same predicate on the same amax word), so the weight-ring stage counters stay in step.
+template <int C, bool PEERS, bool BATCH = false>
 __global__ void __launch_bounds__(kThreads, 1)
-query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpSurfaceSrc surf) {
+query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpSurfaceSrc surf, MpBatch bt) {
   using P = Prog<C>;
   constexpr int RES = P::RES, Ring = P::Ring, XKB = P::XKB;
+  static_assert(!(BATCH && PEERS), "batched launches have no peer stores");
   MP_DYN_SMEM(uint8_t, smem_raw);
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::Bars);
@@ -235,7 +247,9 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   float* s_s4 = s_in + kTile;
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid)
+  if constexpr (!BATCH) {
+    if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid)
+  }
 
   long long n = src.n;
   if (src.count_dev) {
@@ -245,7 +259,11 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   long long win0, win1;
   mp_shard_window(src, n, win0, win1);
   n = win1;                                          // points >= n are padding; tile 0 starts at point win0
-  const long long n_tiles = (win1 - win0 + kTile - 1) / kTile;
+  const long long n_tiles = (win1 - win0 + kTile - 1) / kTile;       // (per image)
+  const long long all_tiles = BATCH ? n_tiles * bt.B : n_tiles;
+  auto tile_skipped = [&](long long t) {
+    return BATCH && mp_guard_skips(prm.amax + mp_tile_image(t, n_tiles), prm.amax_limit, prm.guard);
+  };
 
   if (tid == 0) {
     for (int s = 0; s < Ring; ++s) {
@@ -261,7 +279,8 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
     if (lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
       uint32_t it = 0;
-      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+      for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
+        if (tile_skipped(t)) continue;
         for (int s = 0; s < P::StagesPerTile; ++s, ++it) {
           const uint32_t slot = it % Ring, use = it / Ring;
           tc::mbar_wait(empty + slot, (use & 1u) ^ 1u);
@@ -305,6 +324,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   // ---- taps of this warp's 8 points for the layer-0 chunks: lane = (point 4 i + qw, channels 8 l8 .. and 64 + 8 l8 ..)
   const int l8 = lane & 7, qw = lane >> 3;
   uint32_t t_off[2][2], t_wgt[2][2], t_z[2];
+  int img = 0;                       // BATCH: the tile's image (its per-texel arrays start at texel img * H * W)
   auto gen_chunk = [&](int c) {
     const int ch = c * 128 + l8 * 8;
     __half2 b8[8], z8[8];
@@ -322,7 +342,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
 #pragma unroll
       for (int a = 0; a < 4; ++a) {
         const uint32_t off = (a & 1) ? (t_off[i][a >> 1] >> 16) : (t_off[i][a >> 1] & 0xFFFFu);
-        const uint4* srcp = reinterpret_cast<const uint4*>(prm.g0 + (size_t)off * kL0 + ch);
+        const uint4* srcp = reinterpret_cast<const uint4*>(prm.g0 + ((BATCH ? (size_t)img * prm.H * prm.W : 0) + (size_t)off) * kL0 + ch);
         raw[i][a][0] = __ldg(srcp);
         raw[i][a][1] = __ldg(srcp + 8);      // + 64 channels
       }
@@ -357,17 +377,22 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
     tc::fence_proxy_async_smem();
   };
 
-  for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-    const long long p0 = win0 + t * kTile;
+  for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
+    if (tile_skipped(t)) continue;
+    const int b = BATCH ? mp_tile_image(t, n_tiles) : 0;
+    const long long p0 = win0 + (BATCH ? t - (long long)b * n_tiles : t) * kTile;
+    if constexpr (BATCH) img = b;
+    const size_t texel0 = (size_t)b * prm.H * prm.W;
     // ---- X (skip operand) + per-point scalars: 4 groups of 16 points x C/256 channel phases over the 8 warps
 #pragma unroll 1
     for (int job = warp; job < 4 * (C / 256); job += 8) {
       const int grp = job & 3, phase = job >> 2;
-      const PointTaps pt = point_taps(surf, src, cal, prm.H, prm.W, p0 + grp * 16 + (lane & 15), n);
-      sample_x16<C>(prm, smem + P::X, s_zf, s_in, s_s4, pt, grp * 16, lane, phase);
+      const PointTaps pt = point_taps<BATCH>(surf, src, cal, bt, b, prm.H, prm.W, p0 + grp * 16 + (lane & 15), n);
+      sample_x16<C>(prm, prm.feat16 + (BATCH ? texel0 * C : 0), prm.s4tex + (BATCH ? texel0 * RES : 0), smem + P::X, s_zf, s_in, s_s4,
+                    pt, grp * 16, lane, phase);
     }
     {
-      const PointTaps pt = point_taps(surf, src, cal, prm.H, prm.W, p0 + warp * 8 + l8, n);
+      const PointTaps pt = point_taps<BATCH>(surf, src, cal, bt, b, prm.H, prm.W, p0 + warp * 8 + l8, n);
       const uint32_t o01 = (uint32_t)pt.off[0] | ((uint32_t)pt.off[1] << 16), o23 = (uint32_t)pt.off[2] | ((uint32_t)pt.off[3] << 16);
       const uint32_t w01 = tc::pack_half2(pt.wgt[0], pt.wgt[1]), w23 = tc::pack_half2(pt.wgt[2], pt.wgt[3]);
       const uint32_t zz = tc::pack_half2(pt.zf, pt.zf);
@@ -538,6 +563,10 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
               px[r] = __fadd_rn(__fmul_rn(val, 0.5f), 0.5f);      // RTL/main.py:244
               continue;
             }
+            if constexpr (BATCH) {
+              dst.out[mp_tile_image(t, n_tiles) * bt.out_stride + (long long)r * dst.ld + i] = val;
+              continue;
+            }
             if (dst.out) dst.out[(long long)r * dst.ld + i] = val;
             if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = val;
             if constexpr (PEERS) {
@@ -557,7 +586,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
 
 // G0[texel][n] = sum_k F[texel][k] * W0f[n][k] on the tensor cores: fp16 operands (F rounded once while staging, W0f
 // pre-packed on the host as SWIZZLE_128B tiles [n tile][K block][256 x 64]) and fp32 accumulation in registers.
-// One CTA = 128 texels x all 1024 outputs: the A operand (128 x C) is staged ONCE by the two consumer warpgroups (fp32
+// One CTA = 128 texels of one map (grid: texel blocks x maps of the handle) x all 1024 outputs: the A operand (128 x C) is staged ONCE by the two consumer warpgroups (fp32
 // global -> fp16 swizzled smem), the B tiles stream through a 2-stage bulk-copy ring (warp 8), and each warpgroup multiplies
 // its 64 rows by the four 256-wide output tiles.  The staging pass also publishes what it has in hand: the fp16 copy of the
 // map (F16, taps of the X operand) and S4 = W4s . F per texel in fp32 (the last layer's direct access to the features:
@@ -585,6 +614,16 @@ g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half
   uint64_t* b_empty = b_full + kG0Stages;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.x * 128;
+  {
+    // blockIdx.y = the image of a batch handle: its own blocks of every per-texel array and its own amax entry (a CTA never
+    // straddles two images, whatever M % 128)
+    const size_t img = blockIdx.y;
+    F += img * M * C;
+    G += img * M * kL0;
+    F16 += img * M * C;
+    S4 += img * M * RES;
+    if (amax) amax += img;
+  }
   if (tid == 0) {
     for (int i = 0; i < kG0Stages; ++i) { tc::mbar_init(&b_full[i], 1); tc::mbar_init(&b_empty[i], kConsumers / 32); }
     tc::fence_barrier_init();
@@ -801,6 +840,7 @@ int tc_prepare(mp_mlp* mlp) {
   }
   if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(g0_wg_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G0Cfg<C>::Smem);
   if (e != cudaSuccess) {
     mp_set_error("mp_tc_prepare: %s", cudaGetErrorString(e));
@@ -811,27 +851,32 @@ int tc_prepare(mp_mlp* mlp) {
   return MP_OK;
 }
 
-// per-frame per-texel products of the head (G0, the fp16 copy of the map, S4), then the fused query
+// per-frame per-texel products of the head (G0, the fp16 copy of the map, S4) for every map of the handle, then the fused
+// query (bt: a batched launch over all of them)
 template <int C>
 int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
-           cudaStream_t st, const MpSurfaceSrc& surf, int guard) {
+           cudaStream_t st, const MpSurfaceSrc& surf, int guard, const MpBatch* bt) {
   using P = Prog<C>;
   const long long HW = (long long)feat->H * feat->W;
+  const int maps = feat->B > 1 ? feat->B : 1;
   if (!feat->g0 || feat->g0_n != kL0) {     // (a map has one channel count, so it serves one of the two heads)
     if (feat->g0) cudaFree(feat->g0);
     feat->g0 = nullptr;
-    MP_CUDA(cudaMalloc(&feat->g0, (size_t)HW * kL0 * sizeof(__half)));
-    if (!feat->f16) MP_CUDA(cudaMalloc(&feat->f16, (size_t)HW * C * sizeof(__half)));
-    if (!feat->s4tex) MP_CUDA(cudaMalloc(&feat->s4tex, (size_t)HW * P::RES * sizeof(float)));
+    MP_CUDA(cudaMalloc(&feat->g0, (size_t)maps * HW * kL0 * sizeof(__half)));
+    if (!feat->f16) MP_CUDA(cudaMalloc(&feat->f16, (size_t)maps * HW * C * sizeof(__half)));
+    if (!feat->s4tex) MP_CUDA(cudaMalloc(&feat->s4tex, (size_t)maps * HW * P::RES * sizeof(float)));
     feat->g0_n = kL0;
     feat->g0_owner = 0;
   }
   if (feat->g0_owner != mlp->gen || feat->g0_version != feat->version) {
+    const dim3 g0_grid((unsigned)((HW + 127) / 128), (unsigned)maps);
 #ifndef MP_CUDA_EMU
-    g0_wg_kernel<C><<<(unsigned)((HW + 127) / 128), kThreads, G0Cfg<C>::Smem, st>>>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16,
-                                                                                   feat->s4tex, pk->w4s, feat->amax);
+    g0_wg_kernel<C><<<g0_grid, kThreads, G0Cfg<C>::Smem, st>>>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s,
+                                                              feat->amax);
 #else
-    MP_EMU_LAUNCH((unsigned)((HW + 127) / 128), kThreads, g0_wg_kernel<C>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, feat->amax));
+    // (a 2-D grid: the CPU model's launcher of tests/emu takes the dim3 itself)
+    cuda_emu::launch(g0_grid, dim3((unsigned)kThreads),
+                     [&] { g0_wg_kernel<C>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, feat->amax); });
 #endif
     MP_CUDA(cudaGetLastError());
     feat->g0_owner = mlp->gen;
@@ -868,14 +913,19 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
   int dev = 0, sms = 132;
   MP_CUDA(cudaGetDevice(&dev));
   MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const long long tiles = (src.n + kTile - 1) / kTile;
+  const long long tiles = (bt ? bt->B : 1) * ((src.n + kTile - 1) / kTile);
   const int grid = (int)(tiles < (long long)sms ? tiles : sms);
+  MpBatch b1;
+  memset(&b1, 0, sizeof(b1));
+  const MpBatch& bb = bt ? *bt : b1;
 #ifndef MP_CUDA_EMU
-  if (dst.n_peers > 0) query_wg_kernel<C, true><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf);      // fused slab exchange
-  else query_wg_kernel<C, false><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf);
+  if (bt) query_wg_kernel<C, false, true><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bb);
+  else if (dst.n_peers > 0) query_wg_kernel<C, true><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bb);      // fused slab exchange
+  else query_wg_kernel<C, false><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bb);
 #else
-  if (dst.n_peers > 0) MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, true>(prm, src, cal, dst, surf)));
-  else MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, false>(prm, src, cal, dst, surf)));
+  if (bt) MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, false, true>(prm, src, cal, dst, surf, bb)));
+  else if (dst.n_peers > 0) MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, true>(prm, src, cal, dst, surf, bb)));
+  else MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, false>(prm, src, cal, dst, surf, bb)));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -941,11 +991,11 @@ int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* 
   src.n = n;
   MpOutDst dst;
   dst.out = nullptr; dst.ld = 0; dst.scatter_vol = nullptr;
-  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, MP_GUARD_NONE);
+  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, MP_GUARD_NONE, nullptr);
 }
 
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
-                       const MpOutDst& dst, cudaStream_t st, int guard) {
+                       const MpOutDst& dst, cudaStream_t st, int guard, const MpBatch* bt) {
   if (src.n <= 0) return MP_OK;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
   if (!pk || !mlp->tc_ok) {
@@ -957,7 +1007,7 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
     mp_set_error("head expects %d input channels but the feature map has %d (+1 depth)", mlp->channels[0], feat->C);
     return MP_E_INVALID;
   }
-  if ((long long)feat->H * feat->W > 65536) {      // texel indices travel as 16-bit pairs in registers
+  if ((long long)feat->H * feat->W > 65536) {      // texel indices travel as 16-bit pairs in registers (per map of a batch)
     mp_set_error("the tensor-core program handles feature maps of at most 65536 texels (got %d x %d); use MP_MODE_FP32", feat->H, feat->W);
     return MP_E_UNSUPPORTED;
   }
@@ -971,5 +1021,10 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
   }
   MpSurfaceSrc surf;
   memset(&surf, 0, sizeof(surf));
-  return C == 256 ? launch<256>(mlp, pk, feat, src, cal, dst, st, surf, guard) : launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard);
+  if (bt && (src.kind != MP_SRC_ROWS || dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
+    mp_set_error("batched launches take point rows and write [R,N] outputs");
+    return MP_E_UNSUPPORTED;
+  }
+  return C == 256 ? launch<256>(mlp, pk, feat, src, cal, dst, st, surf, guard, bt)
+                  : launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, bt);
 }

@@ -21,14 +21,18 @@ _MODES = {"fp32": _lib.MODE_FP32, "tc": _lib.MODE_TC, "auto": _lib.MODE_AUTO, "t
 
 
 class FeatureHandle:
-    """Device-side channel-last copy of one [1,C,H,W] feature map (mp_feat_t)."""
+    """Device-side channel-last copy of one [1,C,H,W] feature map, or of the B maps of a [B,C,H,W] batch (mp_feat_t)."""
 
-    def __init__(self, C, H, W, device):
+    def __init__(self, C, H, W, device, B=1):
         self.shape = (C, H, W)
+        self.batch = B
         self.device = device
         self.ptr = ctypes.c_void_p()
         with _lib.device_guard(device):
-            _lib.check(_lib.load().mp_feat_create(C, H, W, ctypes.byref(self.ptr)), "mp_feat_create")
+            if B == 1:
+                _lib.check(_lib.load().mp_feat_create(C, H, W, ctypes.byref(self.ptr)), "mp_feat_create")
+            else:
+                _lib.check(_lib.load().mp_feat_create_batch(B, C, H, W, ctypes.byref(self.ptr)), "mp_feat_create_batch")
         self.key = None
         self._src = None
         self._scope = 0
@@ -115,6 +119,17 @@ class MonoPortNet(nn.Module):
         h.upload(feat, trust_identity=self.feature_cache)
         return h
 
+    def batch_feature_handle(self, feat):
+        """The handle of a [B,C,H,W] batch (B > 1) for query(): B maps, evaluated together by mp_query_points_batch.  The
+        single-map entry points (feature_handle, the grid queries, the engines) do not take it."""
+        B, C, H, W = feat.shape
+        key = ("batch", B, C, H, W, feat.device.index, threading.get_ident())
+        h = self._feat_handles.get(key)
+        if h is None:
+            h = self._feat_handles[key] = FeatureHandle(C, H, W, feat.device, B=B)
+        h.upload(feat, trust_identity=self.feature_cache)
+        return h
+
     def invalidate_features(self):
         """Forget every uploaded frame (call after writing into a feature tensor behind PyTorch's back)."""
         for h in self._feat_handles.values():
@@ -128,8 +143,9 @@ class MonoPortNet(nn.Module):
 
     @torch.no_grad()
     def query(self, feats_stages, points, calibs=None, transforms=None):
-        """list(list([1,C,H,W])), points [1,3,N], calibs [1,4,4]|[1,3,4]|None -> [ [1,Res,N] ]
-        (MonoPortNet.py:48-91, eval mode: only the LAST stage is evaluated, :63-64)."""
+        """list(list([B,C,H,W])), points [B,3,N], calibs [B,4,4]|[B,3,4]|None -> [ [B,Res,N] ]
+        (MonoPortNet.py:48-91, eval mode: only the LAST stage is evaluated, :63-64).  B == 1 is the single-frame path of the
+        demo; B > 1 evaluates all images in one launch (mp_query_points_batch)."""
         if self.training:
             raise NotImplementedError("training-mode (multi-stage, autograd) query is outside the accelerated hot path; "
                                       "call .eval() (RTL/main.py:116)")
@@ -141,6 +157,8 @@ class MonoPortNet(nn.Module):
         feat = feats[0]
         if feat.device.type != "cuda":
             raise RuntimeError("monoport_b200.query: features must be CUDA tensors (there is no CPU path)")
+        if feat.dim() == 4 and feat.shape[0] > 1:
+            return self._query_batch(feat, points, calibs)
         if points.dim() != 3 or points.shape[0] != 1 or points.shape[1] != 3:
             raise ValueError("points must be [1,3,N]; got %s" % (tuple(points.shape),))
         if points.device != feat.device:
@@ -164,6 +182,40 @@ class MonoPortNet(nn.Module):
                 head.handle(), fh.ptr, ctypes.c_void_p(points.data_ptr()), n, s[1], s[2], _lib.calib12(calibs), proj,
                 ctypes.c_float(self.normalizer.scale), ctypes.c_void_p(out.data_ptr()), n, self._mode(),
                 _lib.stream_ptr(feat.device)), "mp_query_points")
+        return [out]
+
+    def _query_batch(self, feat, points, calibs):
+        """query() of B > 1 images: one launch; the calibs stay on the device (no read-back, no synchronisation)."""
+        B = feat.shape[0]
+        if points.dim() != 3 or points.shape[1] != 3 or points.shape[0] != B:
+            raise ValueError("points must be [B,3,N] with the features' B=%d; got %s" % (B, tuple(points.shape)))
+        if calibs is not None and (calibs.dim() != 3 or calibs.shape[0] != B or calibs.shape[1] not in (3, 4)
+                                   or calibs.shape[2] != 4):
+            raise ValueError("calibs must be [B,4,4] or [B,3,4] with the features' B=%d; got %s" % (B, tuple(calibs.shape)))
+        if points.device != feat.device:
+            raise ValueError("points and features live on different devices")
+        if points.dtype != torch.float32:
+            points = points.float()
+        n = points.shape[2]
+        s = points.stride()
+        if n > 0 and min(s) < 1:
+            points = points.contiguous()
+            s = points.stride()
+        res = self.surface_classifier.filter_channels[-1]
+        out = torch.empty((B, res, n), dtype=torch.float32, device=feat.device)
+        if n == 0:
+            return [out]
+        with _lib.device_guard(feat.device):
+            cal = None
+            if calibs is not None:
+                cal = calibs.detach()[:, :3, :4].to(device=feat.device, dtype=torch.float32).contiguous()
+            fh = self.batch_feature_handle(feat)
+            proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
+            _lib.check(_lib.load().mp_query_points_batch(
+                self.surface_classifier.handle(), fh.ptr, B, ctypes.c_void_p(points.data_ptr()), n, s[0], s[1], s[2],
+                None if cal is None else ctypes.c_void_p(cal.data_ptr()), proj, ctypes.c_float(self.normalizer.scale),
+                ctypes.c_void_p(out.data_ptr()), res * n, n, self._mode(), _lib.stream_ptr(feat.device)),
+                "mp_query_points_batch")
         return [out]
 
     def query_grid(self, feat, calibs, resolution, b_min, b_max, z0=0, nz=None, out=None, fh=None):

@@ -37,5 +37,15 @@ netC = build_net("C", cW, cb)
 featC = spec.make_feat(512, 128, 128, 6, 0.5).cuda()
 img = colorization(netC, [[featC]], X, Y, Z, cal, resolution=33)
 big = net.query([[feat.cuda() * 60.0]], pts, calibs=cal)[0]
+# batched queries (one launch over B images) in every mode; image 1 is outside the range guard's limit, so the guarded
+# modes split the launch per image between the tensor-core and the exact kernel
+fb = torch.cat([feat, feat * 60.0, spec.make_feat(256, 128, 128, 8, 0.5)], 0).cuda()
+pb = torch.cat([spec.make_points(100, 2), spec.make_points(100, 3), spec.make_points(100, 4)], 0).cuda()
+cb = torch.cat([spec.scene_calib(20, 33), spec.scene_calib(-10, 5), spec.scene_calib(30, 70)], 0).cuda()
+for mode in ("fp32", "tc", "auto"):
+    net.precision = mode
+    ob = net.query([[fb]], pb, calibs=cb)[0]
+    torch.cuda.synchronize()
+    print("batch", mode, float(ob.sum()))
 torch.cuda.synchronize()
 print("ok", X.numel(), v.shape, f.shape, float(img.sum()), float(big.sum()))
