@@ -16,12 +16,12 @@
 //
 // One persistent CTA per SM; a tile = 64 points = the M of every warpgroup MMA (a batched launch: of one image, see BATCH).  Warps 0-3 and 4-7 are two consumer
 // warpgroups that split the N dimension of every layer (layer 1: 256 columns each, 128 fp32 accumulators per thread;
-// layer 2: 128; layer 3: 64); both sample the operands (X, the layer-0 chunks) and run the epilogues.  Warp 8 streams the
-// weights L2 -> shared memory through a ring of 32 KB stages (cp.async.bulk on mbarriers), pre-packed on the host as
-// K-major SWIZZLE_128B tiles in exactly the order the consumers take them.  The program is written so that layer-0 chunk
-// c+1 is generated while the MMAs of chunk c are in flight, but at 168 registers per thread (9 warps per CTA) ptxas
-// inserts warpgroup.arrive around the accumulators and serializes the wgmma instructions (C7520): today every MMA
-// completes before the next instruction, so that overlap does not happen.
+// layer 2: 128; layer 3: 64); both sample the operands (X, the layer-0 chunks) and run the epilogues.  Warpgroup 2 is the
+// producer: one thread of it streams the weights L2 -> shared memory through a ring of 32 KB stages (cp.async.bulk on
+// mbarriers), pre-packed on the host as K-major SWIZZLE_128B tiles in exactly the order the consumers take them.  The
+// producer gives its registers to the consumers (setmaxnreg: 40 and 232 per thread).  The MMAs run asynchronously: the
+// role branches are warp-uniform by construction and the consumers wait for their MMAs at fixed points of a static
+// schedule (see the ring below), so layer-0 chunk c+1 is generated while the MMAs of chunk c are in flight.
 #include "mp_common.cuh"
 #include "tc_ptx.cuh"
 #include <stdlib.h>
@@ -30,7 +30,10 @@ namespace {
 
 constexpr int kTile = 64;                       // points per tile
 constexpr int kConsumers = 256;                 // two consumer warpgroups
-constexpr int kThreads = kConsumers + 32;       // + the weight producer warp
+constexpr int kThreads = kConsumers + 128;      // + the producer warpgroup (query_wg_kernel)
+constexpr int kProducerRegs = 40, kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + kConsumers * kConsumerRegs <= 65536, "register file of one SM");
+constexpr int kG0Threads = kConsumers + 32;     // g0_wg_kernel: two consumer warpgroups + one producer warp
 constexpr int kL0 = 1024, kL1 = 512, kL2 = 256, kL3 = 128;
 constexpr int kStageBytes = 32768;              // one ring stage: 256 weight rows x 64 K (or 2 x 128 rows x 64 K)
 constexpr int kKb = kTile * 128;                // one 64-channel K-block of a 64-row A operand
@@ -63,6 +66,7 @@ template <int C> struct Prog {
 static_assert(Prog<256>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
 static_assert(Prog<512>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
 static_assert(Prog<256>::XKB % 2 == 0 && Prog<512>::XKB % 2 == 0, "layer-3 stages hold two K-blocks");
+static_assert(Prog<256>::StagesL3 >= Prog<256>::Ring && Prog<512>::StagesL3 >= Prog<512>::Ring, "a layer ends by releasing its last Ring stages");
 
 struct TcPack {
   __half* wstream;        // stage stream of a tile: Prog<C>::StagesPerTile x 32 KB
@@ -239,21 +243,27 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   constexpr int RES = P::RES, Ring = P::Ring, XKB = P::XKB;
   static_assert(!(BATCH && PEERS), "batched launches have no peer stores");
   MP_DYN_SMEM(uint8_t, smem_raw);
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // aligned by an offset from the shared array itself (not through an integer cast), so the compiler keeps knowing that
+  // every pointer below is a shared-memory pointer: 32-bit addresses and st.shared instead of 64-bit generic ones
+  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::Bars);
   uint64_t* empty = full + Ring;
   float* s_zf = reinterpret_cast<float*>(smem + P::Small);
   float* s_in = s_zf + kTile;
   float* s_s4 = s_in + kTile;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // Every branch that decides a role or skips work is warp-uniform by construction: the warp index and every value read
+  // from memory that steers control flow come from lane 0 through a shuffle.  ptxas then knows that no wgmma sits on a
+  // divergent path; otherwise it wraps every wgmma in warpgroup.arrive / wait and the MMAs run one at a time (C7520).
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0), wg = warp >> 2;
   if constexpr (!BATCH) {
-    if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid)
+    if (__shfl_sync(0xffffffffu, (int)mp_guard_skips(prm.amax, prm.amax_limit, prm.guard), 0)) return;      // (uniform over the grid)
   }
 
   long long n = src.n;
   if (src.count_dev) {
-    const long long c = *src.count_dev;
+    const long long c = __shfl_sync(0xffffffffu, *src.count_dev, 0);
     n = c < n ? c : n;
   }
   long long win0, win1;
@@ -261,7 +271,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   n = win1;                                          // points >= n are padding; tile 0 starts at point win0
   const long long n_tiles = (win1 - win0 + kTile - 1) / kTile;       // (per image)
   const long long all_tiles = BATCH ? n_tiles * bt.B : n_tiles;
-  auto tile_skipped = [&](long long t) {
+  auto tile_skipped = [&](long long t) {       // (the consumer warps take lane 0's answer)
     return BATCH && mp_guard_skips(prm.amax + mp_tile_image(t, n_tiles), prm.amax_limit, prm.guard);
   };
 
@@ -274,9 +284,10 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   }
   __syncthreads();
 
-  if (warp == kConsumers / 32) {
+  if (wg == 2) {
     // ============================== weight producer ==============================
-    if (lane == 0) {
+    tc::setmaxnreg_dec<kProducerRegs>();
+    if (warp == 8 && lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
       uint32_t it = 0;
       for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
@@ -293,33 +304,72 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   }
 
   // ============================== consumers ==============================
-  const int wg = tid >> 7, wl = warp & 3;
+  tc::setmaxnreg_inc<kConsumerRegs>();
+  const int wl = warp & 3;
   const int r0 = 16 * wl + (lane >> 2), cq = 2 * (lane & 3);
   const uint32_t smem_base = tc::smem_u32(smem);
   auto desc = [&](int off) { return tc::make_wdesc_sw128(smem_base + (uint32_t)off, 1024); };
   auto sync_consumers = [&]() { tc::bar_sync(1, kConsumers); };
 
-  // ---- the weight ring, consumer side (all 32-bit stage counters run across tiles)
-  uint32_t next_stage = 0, npend = 0;
-  uint32_t pend[4];                                  // own stages whose MMAs may still be in flight (oldest first)
+  // ---- the weight ring, consumer side.  Every consumer takes every stage of a tile (56 for the geometry head, 76 for the
+  // colour head) in a fixed order, so which stages a warpgroup still has in flight at any point is known at compile time:
+  // each wait below is a fixed wgmma_wait<N> and each release names its stage by arithmetic on the tile's first stage id
+  // s_tile (32-bit counters running across tiles, in step with the producer's).  No stage is ever queued at run time.
+  // Deadlock freedom: the producer refills the slot of stage s - Ring with stage s once all 8 consumer warps have released
+  // s - Ring, so every consumer must have released s - Ring before it waits for s.  Where that release needs the stage's
+  // MMAs complete, the wait for them comes first:
+  //   layer 1 (two stages per K-block i: 2i carries output half 0 for warpgroup 0, 2i+1 half 1 for warpgroup 1; each
+  //     warpgroup releases the other's stage right after taking it and its own once the K-block's MMAs completed):
+  //     Ring 3: taking 2i+1 needs 2i-2 -- warpgroup 0's own stage of K-block i-1 -- so before it the warpgroup waits for
+  //             all its MMAs (wait<0>) and releases its own stage of K-block i-1; taking 2i needs 2i-3, released by
+  //             warpgroup 1 at that same point one K-block earlier;
+  //     Ring 2: taking 2i needs 2i-2 (warpgroup 0's own of K-block i-1), taking 2i+1 needs 2i-1 (warpgroup 1's), so the
+  //             wait<0> and the release come before both takes;
+  //   layers 2 and 3 (one stage per K-block step, read by both warpgroups): taking stage k needs k - Ring, so before it
+  //     the warpgroup lets at most Ring - 1 groups stay in flight (wait<Ring-1>) and releases k - Ring.
+  // Every layer ends with wait<0> and releases its own stages still held, so a layer starts with nothing in flight.
+  uint32_t s_tile = 0;
   auto release = [&](uint32_t s) {
     __syncwarp();
     tc::mbar_arrive_if(empty + s % Ring, lane == 0);
   };
-  auto flush = [&]() {
-    tc::wgmma_wait<0>();
-    for (uint32_t k = 0; k < npend; ++k) release(pend[k]);
-    npend = 0;
-  };
-  // the next stage of the stream; an own stage still in flight in the same ring slot is completed and released first
-  auto take = [&]() -> uint32_t {
-    const uint32_t s = next_stage++;
-    if (npend && (npend == 4 || s - pend[0] >= (uint32_t)Ring)) flush();
-    tc::mbar_wait(full + s % Ring, (s / Ring) & 1u);
-    return s;
-  };
-  auto keep = [&](uint32_t s) { tc::wgmma_commit(); pend[npend++] = s; };
+  auto take = [&](uint32_t s) { tc::mbar_wait(full + s % Ring, (s / Ring) & 1u); };
   auto wslot = [&](uint32_t s) { return P::Wr + (int)(s % Ring) * kStageBytes; };
+  // layer 1, K-block i (A operand at shared offset a_off): this warpgroup's 256 outputs times its stage 2i + wg
+  auto l1_kblock = [&](float (&acc)[128], int i, int a_off) {
+    const uint32_t s0 = s_tile + 2 * i, mine = s0 + wg, prev = mine - 2;
+    if constexpr (Ring < 3) {
+      tc::wgmma_wait<0>();
+      if (i > 0) release(prev);
+    }
+    take(s0);
+    if constexpr (Ring >= 3) {
+      tc::wgmma_wait<0>();
+      if (i > 0) release(prev);
+    }
+    take(s0 + 1);
+    release(s0 + 1 - wg);                            // the other warpgroup's half
+    const uint64_t da = desc(a_off), db = desc(wslot(mine));
+    tc::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
+    tc::wgmma_commit();
+  };
+  // layers 2 and 3, step k of a layer whose stages start at s_layer: frees the slot of stage k (see above) and takes it
+  auto step_take = [&](uint32_t s_layer, int k) {
+    if (k >= Ring) {
+      tc::wgmma_wait<Ring - 1>();
+      release(s_layer + k - Ring);
+    }
+    take(s_layer + k);
+    tc::wgmma_fence();
+  };
+  // end of a layer of n steps (n >= Ring): all MMAs complete, the last Ring stages released
+  auto layer_end = [&](uint32_t s_layer, int n) {
+    tc::wgmma_wait<0>();
+#pragma unroll
+    for (int j = Ring; j > 0; --j) release(s_layer + n - j);
+  };
 
   // ---- taps of this warp's 8 points for the layer-0 chunks: lane = (point 4 i + qw, channels 8 l8 .. and 64 + 8 l8 ..)
   const int l8 = lane & 7, qw = lane >> 3;
@@ -378,7 +428,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   };
 
   for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
-    if (tile_skipped(t)) continue;
+    if (__shfl_sync(0xffffffffu, (int)tile_skipped(t), 0)) continue;
     const int b = BATCH ? mp_tile_image(t, n_tiles) : 0;
     const long long p0 = win0 + (BATCH ? t - (long long)b * n_tiles : t) * kTile;
     if constexpr (BATCH) img = b;
@@ -418,43 +468,20 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
       for (int j = 0; j < 128; ++j) acc[j] = 0.f;
 #pragma unroll 1
       for (int c = 0; c < 8; ++c) {
-        tc::wgmma_fence();
 #pragma unroll
-        for (int kb = 0; kb < 2; ++kb) {
-          // the K-block's two stages carry output halves 0 and 1: this warpgroup multiplies by its own, releases the other
-          const uint32_t s0 = take(), s1 = take();
-          const uint32_t mine = wg ? s1 : s0;
-          release(wg ? s0 : s1);
-          const uint64_t da = desc(P::H0 + ((c & 1) * 2 + kb) * kKb), db = desc(wslot(mine));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
-          keep(mine);
-        }
+        for (int kb = 0; kb < 2; ++kb) l1_kblock(acc, 2 * c + kb, P::H0 + ((c & 1) * 2 + kb) * kKb);
         if (c < 7) {
-          // the other chunk buffer was read by chunk c-1: complete it here (chunk c stays in flight), then in both warpgroups
-          tc::wgmma_wait<2>();
-          while (npend > 2) {
-            release(pend[0]);
-            for (uint32_t k = 1; k < npend; ++k) pend[k - 1] = pend[k];
-            --npend;
-          }
+          // the other chunk buffer was last read by chunk c-1, whose MMAs completed before chunk c's second K-block was
+          // issued (in both warpgroups once they meet here); chunk c's second K-block stays in flight meanwhile
           sync_consumers();
           gen_chunk(c + 1);
           sync_consumers();
         }
       }
-      tc::wgmma_fence();
 #pragma unroll 1
-      for (int kb = 0; kb < XKB; ++kb) {
-        const uint32_t s0 = take(), s1 = take();
-        const uint32_t mine = wg ? s1 : s0;
-        release(wg ? s0 : s1);
-        const uint64_t da = desc(P::X + kb * kKb), db = desc(wslot(mine));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
-        keep(mine);
-      }
-      flush();
+      for (int kb = 0; kb < XKB; ++kb) l1_kblock(acc, 16 + kb, P::X + kb * kKb);
+      tc::wgmma_wait<0>();
+      release(s_tile + 2 * (16 + XKB - 1) + wg);
       // epilogue -> H1 (fp16, K-major): + bias + w_z z, leaky ReLU
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -475,16 +502,16 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
       float acc[64];
 #pragma unroll
       for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-      tc::wgmma_fence();
+      const uint32_t s_l2 = s_tile + P::StagesL1;
 #pragma unroll 1
-      for (int kb = 0; kb < 8 + XKB; ++kb) {
-        const uint32_t s = take();
-        const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(wslot(s) + wg * 16384);
+      for (int kb = 0; kb < P::StagesL2; ++kb) {
+        step_take(s_l2, kb);
+        const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(wslot(s_l2 + kb) + wg * 16384);
 #pragma unroll
         for (int k = 0; k < 4; ++k) tc::wgmma_m64n128(acc, da + 2 * k, db + 2 * k);
-        keep(s);
+        tc::wgmma_commit();
       }
-      flush();
+      layer_end(s_l2, P::StagesL2);
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int col = wg * 128 + 8 * j + cq;
@@ -504,21 +531,22 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
       float acc[32];
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-      tc::wgmma_fence();
+      const uint32_t s_l3 = s_tile + P::StagesL1 + P::StagesL2;
 #pragma unroll 1
       for (int q = 0; q < P::StagesL3; ++q) {
-        const uint32_t s = take();
+        step_take(s_l3, q);
 #pragma unroll
         for (int sub = 0; sub < 2; ++sub) {
           const int kb = (2 * q + sub) % (XKB + 4);
           const uint64_t da = desc(kb < XKB ? P::X + kb * kKb : P::H0 + (kb - XKB) * kKb);
-          const uint64_t db = desc(wslot(s) + sub * 16384 + wg * 8192);
+          const uint64_t db = desc(wslot(s_l3 + q) + sub * 16384 + wg * 8192);
 #pragma unroll
           for (int k = 0; k < 4; ++k) tc::wgmma_m64n64(acc, da + 2 * k, db + 2 * k);
         }
-        keep(s);
+        tc::wgmma_commit();
       }
-      flush();
+      layer_end(s_l3, P::StagesL3);
+      s_tile += P::StagesPerTile;
       float lg[2][RES];
 #pragma unroll
       for (int h = 0; h < 2; ++h)
@@ -545,9 +573,10 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
       float* s_part = reinterpret_cast<float*>(smem + P::H1);
       const int mine = lane & 3;                 // lane 0 of a quad: row r0, lane 1: row r0 + 8
       const int row = r0 + 8 * (mine & 1);
+      auto lg_mine = [&](int r) { return (mine & 1) ? lg[1][r] : lg[0][r]; };       // (a select: lg stays in registers)
       if (wg == 1 && mine < 2) {
 #pragma unroll
-        for (int r = 0; r < RES; ++r) s_part[r * kTile + row] = lg[mine][r];
+        for (int r = 0; r < RES; ++r) s_part[r * kTile + row] = lg_mine(r);
       }
       sync_consumers();
       if (wg == 0 && mine < 2) {
@@ -556,7 +585,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
           const float inimg = s_in[row];
 #pragma unroll
           for (int r = 0; r < RES; ++r) {
-            const float logit = s_s4[r * kTile + row] + (lg[mine][r] + s_part[r * kTile + row]);
+            const float logit = s_s4[r * kTile + row] + (lg_mine(r) + s_part[r * kTile + row]);
             const float val = inimg * mp_last_op(logit, prm.last_op);
             if (surf.canvas) {
               float* px = surf.canvas + ((size_t)__ldg(surf.X + i) * surf.canvas_R + (size_t)__ldg(surf.Y + i)) * 3;
@@ -601,7 +630,7 @@ template <int C> struct G0Cfg {
 };
 
 template <int C>
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kG0Threads, 1)
 g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half* __restrict__ G, int M,
              __half* __restrict__ F16, float* __restrict__ S4, const float* __restrict__ w4s, unsigned* __restrict__ amax) {
   using Cfg = G0Cfg<C>;
@@ -612,7 +641,8 @@ g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half
   uint8_t* sB = base + Cfg::SmemA;
   uint64_t* b_full = reinterpret_cast<uint64_t*>(base + Cfg::SmemA + Cfg::SmemB);
   uint64_t* b_empty = b_full + kG0Stages;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);       // provably warp-uniform (see query_wg_kernel)
   const int m0 = blockIdx.x * 128;
   {
     // blockIdx.y = the image of a batch handle: its own blocks of every per-texel array and its own amax entry (a CTA never
@@ -693,7 +723,7 @@ g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half
   }
   tc::bar_sync(1, kConsumers);
   // ---- MMAs + epilogue: warpgroup wg owns rows [64 wg, 64 wg + 64) of the CTA's 128
-  const int wg = tid >> 7, wl = warp & 3;
+  const int wg = warp >> 2, wl = warp & 3;
   const int r0 = 16 * wl + (lane >> 2), cq = 2 * (lane & 3);
   const uint32_t a_base = tc::smem_u32(sA) + wg * 8192, b_base = tc::smem_u32(sB);
 #pragma unroll 1
@@ -871,11 +901,11 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
   if (feat->g0_owner != mlp->gen || feat->g0_version != feat->version) {
     const dim3 g0_grid((unsigned)((HW + 127) / 128), (unsigned)maps);
 #ifndef MP_CUDA_EMU
-    g0_wg_kernel<C><<<g0_grid, kThreads, G0Cfg<C>::Smem, st>>>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s,
+    g0_wg_kernel<C><<<g0_grid, kG0Threads, G0Cfg<C>::Smem, st>>>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s,
                                                               feat->amax);
 #else
     // (a 2-D grid: the CPU model's launcher of tests/emu takes the dim3 itself)
-    cuda_emu::launch(g0_grid, dim3((unsigned)kThreads),
+    cuda_emu::launch(g0_grid, dim3((unsigned)kG0Threads),
                      [&] { g0_wg_kernel<C>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, feat->amax); });
 #endif
     MP_CUDA(cudaGetLastError());

@@ -61,7 +61,7 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gmem_src, u
                : "memory");
 }
 
-// named barrier `id` over the first `threads` threads of the CTA (the two consumer warpgroups; the producer warp stays out)
+// named barrier `id` over the first `threads` threads of the CTA (the two consumer warpgroups; the producer warps stay out)
 __device__ __forceinline__ void bar_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
 
 // ---------------------------------------------------------------- fences
@@ -133,3 +133,24 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
 }  // namespace tc
 
 #endif  // MP_CUDA_EMU
+
+namespace tc {
+
+// ---------------------------------------------------------------- per-warpgroup register budget
+// every warp of the warpgroup executes the same one; N is a multiple of 8 in [24, 256].  dec hands registers back to the
+// CTA's pool, inc takes them from it (and waits until the pool has them).  The functional CPU model has no register
+// file, so there they do nothing.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+#ifndef MP_CUDA_EMU
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+#endif
+}
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+#ifndef MP_CUDA_EMU
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+#endif
+}
+
+}  // namespace tc
