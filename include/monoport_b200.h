@@ -122,6 +122,16 @@ int mp_query_points(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int
 int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n, int64_t batch_stride,
                           int64_t row_stride, int64_t point_stride, const float* calibs_dev, int projection, float z_scale,
                           float* out_dev, int64_t out_batch_stride, int64_t ld_out, int mode, void* stream);
+/* Gradient of MonoPortNet.query (mp_query_points, MP_MODE_FP32) with respect to the points: exact fp32 on CUDA cores, one
+ * fused launch (forward pass + reverse pass through the projection, the bilinear taps, the depth column and the skip MLP).
+ * dpoints_dev: [3][ld_dpoints], coordinate a of point i at dpoints_dev[a*ld_dpoints + i] = d(sum_c grad_out[c,i] * out[c,i]) /
+ * d points[a,i].  grad_out_dev: [Res][ld_grad], or NULL for all ones (the geometry head then gives grad sigma).
+ * out_dev: [Res][ld_out], the value -- bit-identical to mp_query_points in MP_MODE_FP32 -- or NULL to skip it.  Points
+ * outside the image get value 0 and gradient exactly 0 (in_img multiplies the output, MonoPortNet.py:89); at a
+ * leaky-ReLU kink the derivative of the non-positive side is taken (torch's convention).  Single-map handles only. */
+int mp_query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                         int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
+                         int64_t ld_grad, float* out_dev, int64_t ld_out, float* dpoints_dev, int64_t ld_dpoints, void* stream);
 /* Same call with HOST buffers (points [3,N], out [Res,N], feature map NCHW fp32 or NULL to reuse the
  * uploaded one): copies in, runs, copies out, synchronises.  This is what bench.py's e2e leg times. */
 int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,

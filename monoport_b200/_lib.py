@@ -44,6 +44,8 @@ SIGNATURES = {
                                       c_float, c_void_p, c_int64, c_int64, c_int, c_void_p]),
     "mp_query_points": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
                                 c_void_p, c_int64, c_int, c_void_p]),
+    "mp_query_points_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
+                                     c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
     "mp_query_points_host": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, P(c_float), c_int, c_float,
                                      c_void_p, c_int, c_void_p]),
     "mp_query_grid": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, P(c_float), P(c_float), P(c_float), c_int,

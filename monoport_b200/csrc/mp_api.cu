@@ -345,6 +345,31 @@ extern "C" int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, cons
                       out_dev, out_batch_stride, ld_out, mode, stream, true);
 }
 
+extern "C" int mp_query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                                    int64_t point_stride, const float* calib12, int projection, float z_scale,
+                                    const float* grad_out_dev, int64_t ld_grad, float* out_dev, int64_t ld_out,
+                                    float* dpoints_dev, int64_t ld_dpoints, void* stream) {
+  MpRange nvtx("monoport_b200: F1'' query gradient");
+  MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE_SINGLE_MAP(feat, "mp_query_points_grad");
+  MP_REQUIRE(n >= 0 && row_stride >= 1 && point_stride >= 1 && ld_dpoints >= n && (!out_dev || ld_out >= n) &&
+                 (!grad_out_dev || ld_grad >= n),
+             "bad sizes n=%lld strides=%lld,%lld ld_grad=%lld ld_out=%lld ld_dpoints=%lld", (long long)n, (long long)row_stride,
+             (long long)point_stride, (long long)ld_grad, (long long)ld_out, (long long)ld_dpoints);
+  if (n == 0) return MP_OK;
+  MP_REQUIRE(points_dev && dpoints_dev, "NULL points/dpoints");
+  MpPointSrc src;
+  memset(&src, 0, sizeof(src));
+  src.kind = MP_SRC_ROWS;
+  src.px = points_dev; src.py = points_dev + row_stride; src.pz = points_dev + 2 * row_stride;
+  src.pstride = point_stride;
+  src.n = n;
+  MpCalib cal;
+  mp_fill_calib(cal, calib12, projection, z_scale);
+  return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints,
+                              (cudaStream_t)stream);
+}
+
 extern "C" int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,
                                     int64_t n, const float* calib12, int projection, float z_scale, float* out_host,
                                     int mode, void* stream) {

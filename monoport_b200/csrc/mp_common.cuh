@@ -311,6 +311,12 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
                          const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                        const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
+// gradient of the fp32 query with respect to the points (query_fp32.cu): value -> out[r*ld_out+i] (out may be null; written
+// by a query_fp32_kernel launch, so it is that kernel's value bit for bit),
+// d(sum_r grad_out[r*ld_grad+i] * value_r)/d point_i -> dpoints[a*ld_dp+i] (grad_out null = ones); MP_SRC_ROWS, one map
+int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
+                         const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
+                         long long ld_dp, cudaStream_t st);
 // device-side predicate shared by the kernels: true = this launch (batched: this tile, amax = its image's entry) must do
 // nothing.  In the tensor-core program the weight producer and the consumers both take it, per tile, from the same word.
 __device__ __forceinline__ bool mp_guard_skips(const unsigned* amax, float limit, int guard) {

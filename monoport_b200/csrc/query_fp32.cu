@@ -58,9 +58,10 @@ __device__ __forceinline__ void fma_rows(float (&acc)[NCO][P], const float* __re
 }
 
 // One hidden layer: out[co][p] = lrelu(b[co] + sum_k Wt[k][co] * in[k][p]),  in = [hidden rows ; skip rows]
-template <int P, int NCO>
+// MASK (the gradient kernel): also store the sign of every pre-activation, bit co % 32 of sMask[(co / 32) * P + p]
+template <int P, int NCO, bool MASK = false>
 __device__ void dense_layer(const float* __restrict__ wt, const float* __restrict__ bias, int cin_hidden, int cin_skip,
-                            int cout, const float* sHidden, const float* sSkip, float* sOut) {
+                            int cout, const float* sHidden, const float* sSkip, float* sOut, unsigned* sMask = nullptr) {
   const int tid = threadIdx.x;
   for (int base = 0; base < cout; base += kThreads * NCO) {
     int co[NCO];
@@ -100,6 +101,22 @@ __device__ void dense_layer(const float* __restrict__ wt, const float* __restric
         fma_rows<P, NCO>(acc, act + (size_t)k * P, w);
       }
     }
+    if constexpr (MASK) {
+      // lane l of a warp owns channel 32 w + l (kThreads is a multiple of 32), so one ballot per point is one mask word;
+      // lane p stores point p's word.  (Bits of clamped channels >= cout are never read.)
+      const int lane = tid & 31;
+#pragma unroll
+      for (int j = 0; j < NCO; ++j) {
+        const int word = (base + j * kThreads + (tid & ~31)) >> 5;
+        unsigned mine = 0u;
+#pragma unroll
+        for (int p = 0; p < P; ++p) {
+          const unsigned bits = __ballot_sync(0xffffffffu, acc[j][p] > 0.f);
+          if (lane == p) mine = bits;
+        }
+        if (lane < P && word * 32 < cout) sMask[(size_t)word * P + lane] = mine;
+      }
+    }
 #pragma unroll
     for (int j = 0; j < NCO; ++j) {
       if (!ok[j]) continue;
@@ -115,6 +132,107 @@ __device__ void dense_layer(const float* __restrict__ wt, const float* __restric
       }
     }
   }
+}
+
+// ---- the forward half of a tile for query_grad_kernel -----------------------------------------------------------------
+// The statements of query_fp32_kernel's steps 1-4 below (same helpers mp_project / mp_taps / dense_layer, same order of
+// every sum).  query_fp32_kernel keeps them inline: moved into shared functions they make ptxas contract the projection's
+// multiply-adds differently in its instantiations, which changes its results in the last bit.  So the value the gradient
+// call returns is computed by query_fp32_kernel itself; this copy feeds only the gradient.
+// 1. projection, mask, taps; 2. bilinear gather: sX = [sampled features ; z * z_scale], sMeta[p] = in_img
+template <int P, bool BATCH>
+__device__ __forceinline__ void tile_sample(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
+                                            int b, const float* feat, long long p0, long long n, float* sX, float* sMeta,
+                                            int (&sOff)[4][P], float (&sWgt)[4][P]) {
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  if (tid < P) {
+    const long long i = p0 + tid;
+    float u = 0.f, v = 0.f, w = 0.f;
+    bool valid = i < n;
+    if (valid) {
+      float x, y, z;
+      if constexpr (BATCH) {
+        mp_load_image_point(src, bt, b, i, x, y, z);
+        mp_project(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
+      } else {
+        mp_load_point(src, i, x, y, z);
+        mp_project(cal, x, y, z, u, v, w);
+      }
+    }
+    const bool in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);   // MonoPortNet.py:74
+    MpTaps t = mp_taps(valid ? u : 0.f, valid ? v : 0.f, prm.H, prm.W);
+    // NaN coordinates (perspective with w==0): in_img is false; keep taps finite
+    if (!(u == u) || !(v == v)) {
+#pragma unroll
+      for (int a = 0; a < 4; ++a) { t.off[a] = 0; t.wgt[a] = 0.f; }
+    }
+#pragma unroll
+    for (int a = 0; a < 4; ++a) { sOff[a][tid] = t.off[a]; sWgt[a][tid] = t.wgt[a]; }
+    sMeta[0 * P + tid] = in_img ? 1.f : 0.f;
+    sX[(size_t)prm.C * P + tid] = w * cal.z_scale;                                          // DepthNormalizer.py:32
+  }
+  __syncthreads();
+  // warp per point, lanes over channels (NHWC => contiguous)
+  for (int p = warp; p < P; p += kThreads / 32) {
+    const float* f0 = feat + (size_t)sOff[0][p] * prm.C;
+    const float* f1 = feat + (size_t)sOff[1][p] * prm.C;
+    const float* f2 = feat + (size_t)sOff[2][p] * prm.C;
+    const float* f3 = feat + (size_t)sOff[3][p] * prm.C;
+    const float w0 = sWgt[0][p], w1 = sWgt[1][p], w2 = sWgt[2][p], w3 = sWgt[3][p];
+    for (int c = lane; c < prm.C; c += 32) {
+      // same accumulation order as grid_sample: nw, ne, sw, se
+      float v = __ldg(f0 + c) * w0;
+      v += __ldg(f1 + c) * w1;
+      v += __ldg(f2 + c) * w2;
+      v += __ldg(f3 + c) * w3;
+      sX[(size_t)c * P + p] = v;
+    }
+  }
+  __syncthreads();
+}
+
+// 3. hidden layers, ping-ponging between sA and sB (layer l writes sA for even l, sB for odd l); returns the last hidden
+// layer's activations.  MASK: layer l also stores its pre-activation signs at sMask + mask_off[l].
+template <int P, bool MASK>
+__device__ __forceinline__ const float* tile_hidden(const Fp32Params& prm, const float* sX, float* sA, float* sB,
+                                                    unsigned* sMask = nullptr, const int* mask_off = nullptr) {
+  const float* sIn = sX;
+  float* sOut = sA;
+  for (int l = 0; l < prm.n_layers - 1; ++l) {
+    const int hid = prm.hid[l];
+    const int skipw = prm.cin[l] - hid;
+    unsigned* m = MASK ? sMask + mask_off[l] : nullptr;
+    if (l == 0) {
+      dense_layer<P, 2, MASK>(prm.wt[l], prm.bias[l], 0, prm.cin[l], prm.cout[l], sX, sX, sOut, m);
+    } else if (prm.cout[l] > kThreads) {
+      dense_layer<P, 2, MASK>(prm.wt[l], prm.bias[l], hid, skipw, prm.cout[l], sIn, sX, sOut, m);
+    } else {
+      dense_layer<P, 1, MASK>(prm.wt[l], prm.bias[l], hid, skipw, prm.cout[l], sIn, sX, sOut, m);
+    }
+    __syncthreads();
+    sIn = sOut;
+    sOut = (sOut == sA) ? sB : sA;
+  }
+  return sIn;
+}
+
+// 4. last layer, one warp per (point p, out channel r): the logit without its bias, on every lane
+template <int P>
+__device__ __forceinline__ float last_layer_dot(const Fp32Params& prm, const float* sX, const float* sIn, int p, int r, int lane) {
+  const int l = prm.n_layers - 1;
+  const int hid = prm.n_layers == 1 ? 0 : prm.hid[l];
+  const int cin = prm.cin[l];
+  const float* wrow = prm.w_last + (size_t)r * cin;
+  float acc = 0.f;
+  for (int k = lane; k < cin; k += 32) {
+    const float a = (prm.n_layers == 1) ? sX[(size_t)k * P + p]
+                    : (k < hid ? sIn[(size_t)k * P + p] : sX[(size_t)(k - hid) * P + p]);
+    acc = fmaf(__ldg(wrow + k), a, acc);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  return acc;
 }
 
 // BATCH: bt.B images of src.n points (MP_SRC_ROWS); tile t is tile t % n_tiles of image t / n_tiles, which samples its own
@@ -249,6 +367,227 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpB
   }
 }
 
+// ---- F1'': gradient of the query with respect to the points -----------------------------------------------------------
+// Forward half = the fp32 kernel's tile steps (tile_sample / tile_hidden / last_layer_dot above), which also record the sign
+// of every hidden pre-activation as bit masks (1920 bits per point for the shipped heads).  Reverse half, per tile:
+//   g      = grad_out * last_op'(value) * in_img                                    -> sG    [Res][P]
+//   δ_l    = (W_{l+1}[:, :hid]^T δ_{l+1}) * lrelu'(pre_l)   (δ_l in layer l's ping/pong block)
+//   dX     = W_0^T δ_0 + sum_{l>=1} W_l[:, hid:]^T δ_l         (accumulated in sX, which the forward half no longer needs)
+//   d(u,v) = sum_c dX_c * dX_c/d(u,v)   (grid_sample's backward: the tap differences), dw = z_scale * dX_C
+//   dp     = J^T d(u,v,w),  J = d(u,v,w)/dp of the projection
+// The transposed products read the row-major [cout][cin] weight copy: the thread that owns input channel k reads w[co][k].
+struct GradParams {
+  const float* w[MP_MAX_LAYERS];   // [cout][cin] row-major
+  int mask_off[MP_MAX_LAYERS];     // words (of P points) before hidden layer l's sign mask
+  int mask_words;
+  const float* grad_out;           // [Res][ld_grad] or null (= ones)
+  long long ld_grad;
+  float* dp;                       // [3][ld_dp]
+  long long ld_dp;
+};
+
+template <int P>
+struct GradSmem {
+  static __host__ __device__ size_t bytes(int c0, int h_ping, int h_pong, int mask_words, int res) {
+    return Fp32Smem<P>::bytes(c0, h_ping, h_pong) + (size_t)mask_words * P * sizeof(unsigned) + (size_t)res * P * sizeof(float);
+  }
+};
+
+// out[k][p] = sum_co W[co][k] * delta[co][p] for the cin input channels k of a layer; rows k < hid are the previous layer's
+// δ (times lrelu' from its mask), rows k >= hid go to dX[k - hid] (assigned when `first`, accumulated otherwise)
+template <int P, int NCO>
+__device__ void transposed_layer(const float* __restrict__ w, int cin, int cout, int hid, const float* sDelta, float* sHid,
+                                 const unsigned* sMask, float* sDX, bool first) {
+  const int tid = threadIdx.x;
+  for (int base = 0; base < cin; base += kThreads * NCO) {
+    int k[NCO];
+    bool ok[NCO];
+#pragma unroll
+    for (int j = 0; j < NCO; ++j) {
+      k[j] = base + j * kThreads + tid;
+      ok[j] = k[j] < cin;
+      if (!ok[j]) k[j] = cin - 1;
+    }
+    float acc[NCO][P];
+#pragma unroll
+    for (int j = 0; j < NCO; ++j)
+#pragma unroll
+      for (int p = 0; p < P; ++p) acc[j][p] = 0.f;
+    int co = 0;
+    for (; co + 4 <= cout; co += 4) {
+      float wv[4][NCO];
+#pragma unroll
+      for (int cc = 0; cc < 4; ++cc)
+#pragma unroll
+        for (int j = 0; j < NCO; ++j) wv[cc][j] = __ldg(w + (size_t)(co + cc) * cin + k[j]);
+#pragma unroll
+      for (int cc = 0; cc < 4; ++cc) fma_rows<P, NCO>(acc, sDelta + (size_t)(co + cc) * P, wv[cc]);
+    }
+    for (; co < cout; ++co) {
+      float wv[NCO];
+#pragma unroll
+      for (int j = 0; j < NCO; ++j) wv[j] = __ldg(w + (size_t)co * cin + k[j]);
+      fma_rows<P, NCO>(acc, sDelta + (size_t)co * P, wv);
+    }
+#pragma unroll
+    for (int j = 0; j < NCO; ++j) {
+      if (!ok[j]) continue;
+      if (k[j] < hid) {
+        const unsigned* m = sMask + (size_t)(k[j] >> 5) * P;
+        const unsigned bit = 1u << (k[j] & 31);
+        float* o = sHid + (size_t)k[j] * P;
+#pragma unroll
+        for (int p = 0; p < P; ++p) o[p] = (m[p] & bit) ? acc[j][p] : acc[j][p] * MP_LEAKY_SLOPE;   // torch: lrelu'(0) = slope
+      } else {
+        float* o = sDX + (size_t)(k[j] - hid) * P;
+#pragma unroll
+        for (int p = 0; p < P; ++p) o[p] = first ? acc[j][p] : o[p] + acc[j][p];
+      }
+    }
+  }
+}
+
+template <int P>
+__global__ void __launch_bounds__(kThreads, 1)
+query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
+  MP_DYN_SMEM_ALIGNED(float, smem, 16);
+  float* sX = smem;                                  // [c0][P]: sampled input, then dX
+  float* sA = sX + (size_t)prm.c0 * P;               // [h_ping][P]: activations of even layers, then their δ
+  float* sB = sA + (size_t)prm.h_ping * P;           // [h_pong][P]: odd layers
+  float* sMeta = sB + (size_t)prm.h_pong * P;        // [8][P]: in_img
+  unsigned* sMask = reinterpret_cast<unsigned*>(sMeta + 8 * P);          // [mask_words][P]
+  float* sG = reinterpret_cast<float*>(sMask + (size_t)gp.mask_words * P);   // [Res][P]
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int L = prm.n_layers;
+  const int res = prm.cout[L - 1];
+  const long long n = src.n;
+  const long long n_tiles = (n + P - 1) / P;
+  const MpBatch b1{};                                // (unused: single-map launches)
+
+  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const long long p0 = tile * P;
+    // ---- forward half: the fp32 kernel's code, plus the sign masks --------------------------------
+    __shared__ int sOff[4][P];
+    __shared__ float sWgt[4][P];
+    tile_sample<P, false>(prm, src, cal, b1, 0, prm.feat, p0, n, sX, sMeta, sOff, sWgt);
+    const float* sIn = tile_hidden<P, true>(prm, sX, sA, sB, sMask, gp.mask_off);
+    for (int job = warp; job < P * res; job += kThreads / 32) {
+      const int p = job % P, r = job / P;
+      const float acc = last_layer_dot<P>(prm, sX, sIn, p, r, lane);
+      if (lane == 0) {
+        const long long i = p0 + p;
+        float g = 0.f;
+        if (i < n) {
+          const float y = mp_last_op(acc + __ldg(prm.bias[L - 1] + r), prm.last_op);
+          const float d = prm.last_op == MP_LAST_SIGMOID ? y * (1.f - y) : (prm.last_op == MP_LAST_TANH ? 1.f - y * y : 1.f);
+          g = (gp.grad_out ? __ldg(gp.grad_out + (long long)r * gp.ld_grad + i) : 1.f) * d;
+          if (sMeta[p] == 0.f) g = 0.f;                  // in_img multiplies the output (and y may be NaN/inf there)
+        }
+        sG[r * P + p] = g;
+      }
+    }
+    __syncthreads();
+    // ---- reverse half: last layer down to layer 0 -------------------------------------------------
+    const float* sDelta = sG;
+    for (int l = L - 1; l >= 0; --l) {
+      const int hid = l == 0 ? 0 : prm.hid[l];
+      float* sHid = l == 0 ? nullptr : (((l - 1) & 1) ? sB : sA);
+      const unsigned* m = l == 0 ? nullptr : sMask + gp.mask_off[l - 1];
+      if (prm.cin[l] > kThreads)
+        transposed_layer<P, 2>(gp.w[l], prm.cin[l], prm.cout[l], hid, sDelta, sHid, m, sX, l == L - 1);
+      else
+        transposed_layer<P, 1>(gp.w[l], prm.cin[l], prm.cout[l], hid, sDelta, sHid, m, sX, l == L - 1);
+      __syncthreads();
+      sDelta = sHid;
+    }
+    // ---- input gradient -> d(u,v,w) -> dp: warp per point, lanes over channels ---------------------
+    for (int p = warp; p < P; p += kThreads / 32) {
+      const long long i = p0 + p;
+      if (i >= n) continue;
+      float* dp = gp.dp + i;
+      if (sMeta[p] == 0.f) {                             // outside the image: exactly 0
+        if (lane < 3) dp[lane * gp.ld_dp] = 0.f;
+        continue;
+      }
+      float x, y, z, u, v, w;
+      mp_load_point(src, i, x, y, z);
+      mp_project(cal, x, y, z, u, v, w);
+      // the tap cell of mp_taps; a tap outside the map is zero padding and contributes nothing
+      const float ix = ((u + 1.f) / 2.f) * (float)(prm.W - 1);
+      const float iy = ((v + 1.f) / 2.f) * (float)(prm.H - 1);
+      const float x0 = floorf(ix), y0 = floorf(iy);
+      const float fx = ix - x0, fy = iy - y0;
+      const float x1 = x0 + 1.f, y1 = y0 + 1.f;
+      const bool x0ok = (x0 >= 0.f) && (x0 <= (float)(prm.W - 1));
+      const bool x1ok = (x1 >= 0.f) && (x1 <= (float)(prm.W - 1));
+      const bool y0ok = (y0 >= 0.f) && (y0 <= (float)(prm.H - 1));
+      const bool y1ok = (y1 >= 0.f) && (y1 <= (float)(prm.H - 1));
+      const bool ok_nw = x0ok && y0ok, ok_ne = x1ok && y0ok, ok_sw = x0ok && y1ok, ok_se = x1ok && y1ok;
+      const float* f0 = prm.feat + (size_t)sOff[0][p] * prm.C;
+      const float* f1 = prm.feat + (size_t)sOff[1][p] * prm.C;
+      const float* f2 = prm.feat + (size_t)sOff[2][p] * prm.C;
+      const float* f3 = prm.feat + (size_t)sOff[3][p] * prm.C;
+      float du = 0.f, dv = 0.f;
+      for (int c = lane; c < prm.C; c += 32) {
+        const float fnw = ok_nw ? __ldg(f0 + c) : 0.f, fne = ok_ne ? __ldg(f1 + c) : 0.f;
+        const float fsw = ok_sw ? __ldg(f2 + c) : 0.f, fse = ok_se ? __ldg(f3 + c) : 0.f;
+        const float dx = sX[(size_t)c * P + p];
+        du = fmaf(dx, (1.f - fy) * (fne - fnw) + fy * (fse - fsw), du);
+        dv = fmaf(dx, (1.f - fx) * (fsw - fnw) + fx * (fse - fne), dv);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        du += __shfl_xor_sync(0xffffffffu, du, o);
+        dv += __shfl_xor_sync(0xffffffffu, dv, o);
+      }
+      if (lane == 0) {
+        du *= 0.5f * (float)(prm.W - 1);
+        dv *= 0.5f * (float)(prm.H - 1);
+        const float dw = cal.z_scale * sX[(size_t)prm.C * P + p];
+        float g[3];
+        if (!cal.has) {
+          g[0] = du; g[1] = dv; g[2] = dw;
+        } else if (!cal.perspective) {                   // J = R
+#pragma unroll
+          for (int a = 0; a < 3; ++a) g[a] = cal.m[a] * du + cal.m[4 + a] * dv + cal.m[8 + a] * dw;
+        } else {                                         // J rows: (R0 - u R2) / w, (R1 - v R2) / w, R2
+          const float su = du / w, sv = dv / w;
+          const float s2 = dw - su * u - sv * v;
+#pragma unroll
+          for (int a = 0; a < 3; ++a) g[a] = cal.m[a] * su + cal.m[4 + a] * sv + cal.m[8 + a] * s2;
+        }
+#pragma unroll
+        for (int a = 0; a < 3; ++a) dp[a * gp.ld_dp] = g[a];
+      }
+    }
+    __syncthreads();
+  }
+}
+
+template <int P>
+int launch_grad(const Fp32Params& prm, const GradParams& gp, const MpPointSrc& src, const MpCalib& cal, cudaStream_t st,
+                int sm_count, int max_smem) {
+  const size_t smem = GradSmem<P>::bytes(prm.c0, prm.h_ping, prm.h_pong, gp.mask_words, prm.cout[prm.n_layers - 1]);
+  const int opt_in = max_smem - 2048;             // one device-wide bound, as in launch() below
+  static thread_local bool opted[64] = {};
+  int dev_ = 0;
+  MP_CUDA(cudaGetDevice(&dev_));
+  if (dev_ < 0 || dev_ >= 64 || !opted[dev_]) {
+    MP_CUDA(cudaFuncSetAttribute(query_grad_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
+    if (dev_ >= 0 && dev_ < 64) opted[dev_] = true;
+  }
+  const long long tiles = (src.n + P - 1) / P;
+  const int grid = (int)(tiles < (long long)sm_count ? (tiles > 0 ? tiles : 1) : sm_count);
+#ifndef MP_CUDA_EMU
+  query_grad_kernel<P><<<grid, kThreads, smem, st>>>(prm, gp, src, cal);
+#else
+  MP_EMU_LAUNCH(grid, kThreads, query_grad_kernel<P>(prm, gp, src, cal));
+#endif
+  MP_CUDA(cudaGetLastError());
+  return MP_OK;
+}
+
 template <int P>
 int launch(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst, cudaStream_t st,
            int sm_count, int max_smem, const MpBatch* bt) {
@@ -286,10 +625,8 @@ int launch(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, con
 
 }  // namespace
 
-int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
-                         const MpOutDst& dst, cudaStream_t st, int guard, const MpBatch* bt) {
-  if (src.n <= 0) return MP_OK;
-  Fp32Params prm;
+// Fp32Params of a head and a map, and the device's SM count and shared-memory opt-in limit (both kernels)
+static int fill_params(const mp_mlp* mlp, const mp_feat* feat, Fp32Params& prm, int& sms, int& max_smem) {
   memset(&prm, 0, sizeof(prm));
   prm.n_layers = mlp->n_layers;
   prm.c0 = mlp->channels[0];
@@ -318,8 +655,8 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
   prm.last_op = mlp->last_op;
   prm.h_ping = ping; prm.h_pong = pong;
   prm.feat = feat->nhwc32;
-  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
-  int dev = 0, sms = 148, max_smem = 0;
+  int dev = 0;
+  sms = 148; max_smem = 0;
   MP_CUDA(cudaGetDevice(&dev));
   {
     static thread_local int c_sms[64] = {}, c_smem[64] = {};
@@ -330,6 +667,18 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
       if (dev >= 0 && dev < 64) { c_sms[dev] = sms; c_smem[dev] = max_smem; }
     }
   }
+  return MP_OK;
+}
+
+int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
+                         const MpOutDst& dst, cudaStream_t st, int guard, const MpBatch* bt) {
+  if (src.n <= 0) return MP_OK;
+  Fp32Params prm;
+  int sms = 0, max_smem = 0;
+  const int rc = fill_params(mlp, feat, prm, sms, max_smem);
+  if (rc != MP_OK) return rc;
+  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
+  const int ping = prm.h_ping, pong = prm.h_pong;
   if (bt && (src.kind != MP_SRC_ROWS || dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
     mp_set_error("batched launches take point rows and write [R,N] outputs");
     return MP_E_UNSUPPORTED;
@@ -338,5 +687,48 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
   if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16>(prm, src, cal, dst, st, sms, max_smem, bt);
   if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8>(prm, src, cal, dst, st, sms, max_smem, bt);
   mp_set_error("head too wide for the fp32 kernel's shared-memory tiling");
+  return MP_E_UNSUPPORTED;
+}
+
+int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
+                         const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
+                         long long ld_dp, cudaStream_t st) {
+  if (src.n <= 0) return MP_OK;
+  if (src.kind != MP_SRC_ROWS) {
+    mp_set_error("the gradient kernel takes point rows");
+    return MP_E_UNSUPPORTED;
+  }
+  Fp32Params prm;
+  int sms = 0, max_smem = 0;
+  const int rc = fill_params(mlp, feat, prm, sms, max_smem);
+  if (rc != MP_OK) return rc;
+  GradParams gp;
+  memset(&gp, 0, sizeof(gp));
+  int words = 0;
+  for (int l = 0; l < mlp->n_layers; ++l) {
+    gp.w[l] = mlp->w[l];
+    gp.mask_off[l] = words;                      // (mask words per point here; scaled to words of a P-point tile below)
+    if (l < mlp->n_layers - 1) words += (mlp->cout[l] + 31) / 32;
+  }
+  gp.mask_words = words;
+  gp.grad_out = grad_out; gp.ld_grad = ld_grad;
+  gp.dp = dpoints; gp.ld_dp = ld_dp;
+  if (out) {                                      // the value: query_fp32_kernel's own, bit for bit
+    MpOutDst dst;
+    dst.out = out; dst.ld = ld_out; dst.scatter_vol = nullptr;
+    const int rq = mp_launch_query_fp32(mlp, feat, src, cal, dst, st);
+    if (rq != MP_OK) return rq;
+  }
+  const int res = prm.cout[prm.n_layers - 1];
+  auto fits = [&](size_t bytes) { return bytes + 2048 <= (size_t)max_smem; };
+  auto scaled = [&](int P) {
+    GradParams g = gp;
+    for (int l = 0; l < mlp->n_layers; ++l) g.mask_off[l] = gp.mask_off[l] * P;
+    return g;
+  };
+  if (fits(GradSmem<32>::bytes(prm.c0, prm.h_ping, prm.h_pong, words, res))) return launch_grad<32>(prm, scaled(32), src, cal, st, sms, max_smem);
+  if (fits(GradSmem<16>::bytes(prm.c0, prm.h_ping, prm.h_pong, words, res))) return launch_grad<16>(prm, scaled(16), src, cal, st, sms, max_smem);
+  if (fits(GradSmem<8>::bytes(prm.c0, prm.h_ping, prm.h_pong, words, res))) return launch_grad<8>(prm, scaled(8), src, cal, st, sms, max_smem);
+  mp_set_error("head too wide for the gradient kernel's shared-memory tiling");
   return MP_E_UNSUPPORTED;
 }

@@ -184,6 +184,59 @@ class MonoPortNet(nn.Module):
                 _lib.stream_ptr(feat.device)), "mp_query_points")
         return [out]
 
+    @torch.no_grad()
+    def query_gradient(self, feats_stages, points, calibs=None, grad_output=None):
+        """query() and its gradient with respect to the points, in one launch of the exact fp32 kernel
+        (mp_query_points_grad).  feats/points/calibs as for query() with B == 1; grad_output [1,Res,N] or None (ones).
+        -> (preds [1,Res,N] -- bit-identical to query() with precision "fp32" --,
+            dpoints [1,3,N] = d sum(grad_output * preds) / d points; for the geometry head and grad_output=None, grad sigma).
+        Points outside the image get 0 for both.  Autograd is not involved: `points.requires_grad` is ignored."""
+        if self.training:
+            raise NotImplementedError("query_gradient is eval-mode only (the gradient of the last stage, like query()); "
+                                      "call .eval()")
+        feats = feats_stages[-1]
+        if len(feats) != 1:
+            raise NotImplementedError("multi-level feature lists (HRNet) are not supported")
+        feat = feats[0]
+        if feat.device.type != "cuda":
+            raise RuntimeError("monoport_b200.query_gradient: features must be CUDA tensors (there is no CPU path)")
+        if feat.dim() != 4 or feat.shape[0] != 1:
+            raise ValueError("query_gradient takes one feature map [1,C,H,W]; got %s" % (tuple(feat.shape),))
+        if points.dim() != 3 or points.shape[0] != 1 or points.shape[1] != 3:
+            raise ValueError("points must be [1,3,N]; got %s" % (tuple(points.shape),))
+        if points.device != feat.device:
+            raise ValueError("points and features live on different devices")
+        points = points.detach()
+        if points.dtype != torch.float32:
+            points = points.float()
+        n = points.shape[2]
+        s = points.stride()
+        if n > 0 and (s[1] < 1 or s[2] < 1):
+            points = points.contiguous()
+            s = points.stride()
+        head = self.surface_classifier
+        res = head.filter_channels[-1]
+        gout = None
+        if grad_output is not None:
+            if tuple(grad_output.shape) != (1, res, n):
+                raise ValueError("grad_output must be [1,%d,%d]; got %s" % (res, n, tuple(grad_output.shape)))
+            if grad_output.device != feat.device:
+                raise ValueError("grad_output and features live on different devices")
+            gout = grad_output.detach()[0].to(torch.float32).contiguous()
+        out = torch.empty((1, res, n), dtype=torch.float32, device=feat.device)
+        dp = torch.empty((1, 3, n), dtype=torch.float32, device=feat.device)
+        if n == 0:
+            return out, dp
+        with _lib.device_guard(feat.device):
+            fh = self.feature_handle(feat)
+            proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
+            _lib.check(_lib.load().mp_query_points_grad(
+                head.handle(), fh.ptr, ctypes.c_void_p(points.data_ptr()), n, s[1], s[2], _lib.calib12(calibs), proj,
+                ctypes.c_float(self.normalizer.scale), None if gout is None else ctypes.c_void_p(gout.data_ptr()), n,
+                ctypes.c_void_p(out.data_ptr()), n, ctypes.c_void_p(dp.data_ptr()), n, _lib.stream_ptr(feat.device)),
+                "mp_query_points_grad")
+        return out, dp
+
     def _query_batch(self, feat, points, calibs):
         """query() of B > 1 images: one launch; the calibs stay on the device (no read-back, no synchronisation)."""
         B = feat.shape[0]

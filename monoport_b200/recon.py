@@ -97,15 +97,25 @@ def marching_cubes(vol, iso=0.5):
     return verts, faces
 
 
+def _unit_or_zero(v):
+    """rows of v [N,3] scaled to unit length; a zero row stays zero"""
+    norm = v.norm(dim=1, keepdim=True)
+    return torch.where(norm > 0, v / norm.clamp_min(torch.finfo(v.dtype).tiny), torch.zeros_like(v))
+
+
 @torch.no_grad()
 def reconstruction(net, cuda, calib_tensor, resolution, b_min, b_max, use_octree=False, num_samples=10000,
-                   transform=None, feats=None, engine=None):
+                   transform=None, feats=None, engine=None, normals=False):
     """PIFu-shaped mesh reconstruction (upstream signature, SURVEY.md §8b): evaluate the occupancy field on a
     `resolution`^3 grid over [b_min,b_max] (dense through the fused kernel, or coarse-to-fine when `use_octree`),
     run marching cubes at 0.5, map vertices to world space.  `feats` = net.filter(image) output.
-    Returns (verts [V,3] world, faces [F,3], normals None, values None) or -1 when the volume is empty
+    Returns (verts [V,3] world, faces [F,3], normals, values None) or -1 when the volume is empty
     (upstream returns -1 on marching-cubes failure).  `num_samples` is accepted for signature compatibility
-    (the fused kernel needs no batching)."""
+    (the fused kernel needs no batching).
+    normals: False -> None.  True -> [V,3] outward unit normals -grad sigma / |grad sigma| at the returned vertices (sigma >
+    0.5 is inside), evaluated exactly by the fp32 gradient kernel (MonoPortNet.query_gradient); a vertex where the
+    gradient vanishes gets a zero vector.  With `transform` they are mapped like the vertices (inverse transpose of its 3x3
+    part, renormalised: a rotation rotates them)."""
     if feats is None:
         raise ValueError("pass feats=net.filter(image)")
     R = int(resolution)
@@ -136,10 +146,16 @@ def reconstruction(net, cuda, calib_tensor, resolution, b_min, b_max, use_octree
     # index space -> world:  (v + 0.5)/R * (b_max-b_min) + b_min  (node-centre convention of the engines)
     scale = ((b_max_t - b_min_t) / R).to(verts.device)
     verts = (verts + 0.5) * scale + b_min_t.to(verts.device)
+    nrm = None
+    if normals:
+        _, grad = net.query_gradient(feats, verts.t().unsqueeze(0), calib_tensor)
+        nrm = _unit_or_zero(-grad[0].t())
     if transform is not None:
         T = torch.as_tensor(transform, dtype=torch.float32, device=verts.device)
         verts = verts @ T[:3, :3].T + T[:3, 3]
-    return verts, faces, None, None
+        if nrm is not None:
+            nrm = _unit_or_zero(nrm @ torch.linalg.inv(T[:3, :3].cpu()).to(nrm.device))      # n' = T^-T n
+    return verts, faces, nrm, None
 
 
 @torch.no_grad()
@@ -170,7 +186,7 @@ def colorization(netC, feat_tensor_C, X, Y, Z, calib_tensor, norm=None, resoluti
     if norm is not None:
         image[X, Y, :] = ((norm + 1) / 2).clamp(0, 1)
         return image
-    from .modeling.geometry import orthogonal, perspective
+    from .modeling.geometry import perspective
     head = netC.surface_classifier
     feat = feat_tensor_C[-1][0]
     if (netC.precision in ("auto", "tc") and not netC.training and X.is_cuda and feat.is_cuda and feat.device == device
@@ -193,10 +209,36 @@ def colorization(netC, feat_tensor_C, X, Y, Z, calib_tensor, norm=None, resoluti
             return image
         # features outside the validated range of the tensor-core colour program: the generic route below (its query()
         # takes the exact fp32 kernel for such a frame)
-    verts = torch.stack([X.float(), Y.float(), resolution - Z.float()], dim=1)          # RTL/main.py:231-233
-    samples = verts.unsqueeze(0).permute(0, 2, 1).contiguous()                          # [1,3,N]
-    samples = orthogonal(samples, make_mat_color(resolution, b_min, b_max, device).unsqueeze(0))
+    samples = _visible_world_points(X, Y, Z, resolution, b_min, b_max, device)
     feats = [[f.to(device) for f in fs] for fs in feat_tensor_C]
     preds = netC.query(feats, points=samples, calibs=calib_tensor)[0]
     image[X, Y, :] = (preds[0] * 0.5 + 0.5).t()
     return image
+
+
+def _visible_world_points(X, Y, Z, resolution, b_min, b_max, device):
+    """forward_vertices("front") output -> the world points [1,3,N] the demo queries there: (X, Y, R - Z) through
+    mat_color (RTL/main.py:201-210, 231-233)"""
+    from .modeling.geometry import orthogonal
+    verts = torch.stack([X.float(), Y.float(), resolution - Z.float()], dim=1)          # RTL/main.py:231-233
+    samples = verts.unsqueeze(0).permute(0, 2, 1).contiguous()                          # [1,3,N]
+    return orthogonal(samples, make_mat_color(resolution, b_min, b_max, device).unsqueeze(0))
+
+
+@torch.no_grad()
+def surface_normals(net, feats, X, Y, Z, calib_tensor, resolution=257, b_min=(-1, -1, -1), b_max=(1, 1, 1)):
+    """Exact normals of the visible surface of forward_vertices(sdf, "front"), for colorization(..., norm=...): the
+    geometry net's gradient (MonoPortNet.query_gradient) at the points colorization() samples, (X, Y, R - Z) through
+    mat_color, returned [N,3] in forward_vertices' frame and sign.  Its normals are -(d/dX, d/dY, d/dZ) of the volume
+    in its (X, Y, Z) index axes (finite differences, RTL/recon.py:80-87); Z runs against the world z axis (R - Z above), so
+    the normal is -(g_x L_x, g_y L_y, -g_z L_z) / R normalised, with g the world gradient and L = b_max - b_min.  A vertex
+    where the gradient vanishes gets a zero vector.  None when there is no surface (X is None)."""
+    if X is None:
+        return None
+    device = calib_tensor.device
+    samples = _visible_world_points(X, Y, Z, resolution, b_min, b_max, device)
+    feats = [[f.to(device) for f in fs] for fs in feats]
+    _, grad = net.query_gradient(feats, samples, calib_tensor)
+    length = (torch.as_tensor(np.asarray(b_max, dtype=np.float32)) - torch.as_tensor(np.asarray(b_min, dtype=np.float32)))
+    axis = (length.view(3) / resolution * torch.tensor([1.0, 1.0, -1.0])).to(device)
+    return _unit_or_zero(-(grad[0].t() * axis))

@@ -1,0 +1,164 @@
+"""CPU checks of the point gradient of query() (mp_query_points_grad): the differentiable restatement against the reference's
+autograd goldens, and the gradient kernel -- compiled unmodified on the CPU model of tests/emu -- against those goldens, against
+the fp32 query kernel's values bit for bit, across simulated SM counts, and outside the image.  Also the ptxas report of the
+kernel's sm_90a instantiations."""
+import os
+import re
+import shutil
+import struct
+import subprocess
+
+import numpy as np
+import pytest
+import torch
+
+from oracle import spec
+from grad_cases import grad_cases, load_grad_case, query_grad_ref, within_bar
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+EMU = os.path.join(HERE, "emu")
+CUDA_INC = "/usr/local/cuda/include"
+
+
+def test_grad_goldens_cover_the_cases():
+    assert set(grad_cases()) >= {"g_rot", "g_persp", "g_nocalib", "g_bigfeat", "c_rot"}
+    assert load_grad_case("c_rot")["grad_output"] is not None
+
+
+@pytest.mark.parametrize("name", grad_cases())
+def test_restatement_matches_reference_grad_golden(name):
+    c = load_grad_case(name)
+    _, g64 = query_grad_ref(c["feat"], c["points"], c["calib"], c["Ws"], c["bs"], c["last_op"], c["proj"],
+                            grad_output=c["grad_output"], dtype=torch.float64)
+    assert (g64 - c["grad64"]).abs().max().item() <= 1e-9 * c["grad64"].abs().max().item()
+    val, g32 = query_grad_ref(c["feat"], c["points"], c["calib"], c["Ws"], c["bs"], c["last_op"], c["proj"],
+                            grad_output=c["grad_output"])
+    assert (val - c["value"]).abs().max().item() < 2e-6
+    ok, msg = within_bar(g32, c["grad32"])
+    assert ok, msg
+
+
+# ---- the kernel on the CPU model -------------------------------------------------------------------------------------------
+def _build(tmp, name):
+    if shutil.which("g++") is None:
+        pytest.skip("g++ not available")
+    if not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")):
+        pytest.skip("CUDA headers not found")
+    exe = os.path.join(tmp, name)
+    cmd = ["g++", "-std=c++17", "-O3", "-march=native", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas",
+           "-fno-strict-aliasing", "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU, "-o", exe, os.path.join(EMU, name + ".cpp")]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr[-3000:]
+    return exe
+
+
+@pytest.fixture(scope="module")
+def emu(tmp_path_factory):
+    """(gradient harness, fp32 query harness)"""
+    d = str(tmp_path_factory.mktemp("emu_grad"))
+    return _build(d, "emu_query_grad"), _build(d, "emu_query_fp32")
+
+
+def _write_input(path, c, n):
+    """in.bin of the emulation harnesses (the layout of emu_query_fp32)"""
+    C, H, W = c["feat"].shape[1:]
+    res = c["chans"][-1]
+    with open(path, "wb") as f:
+        f.write(struct.pack("8i", C, H, W, n, 1 if c["calib"] is not None else 0, 1 if c["proj"] == "perspective" else 0,
+                            res, c["last_op"]))
+        f.write(struct.pack("f", spec.Z_SCALE))
+        head = c["calib"][0, :3, :4].reshape(-1).tolist() if c["calib"] is not None else [0.0] * 12
+        f.write(struct.pack("12f", *head))
+        f.write(c["feat"].contiguous().numpy().tobytes())
+        f.write(c["points"][0, :, :n].contiguous().numpy().tobytes())
+        for Wl, bl in zip(c["Ws"], c["bs"]):
+            f.write(Wl.numpy().tobytes())
+            f.write(bl.numpy().tobytes())
+
+
+def _run_grad(emu, tmp_path, c, n, sms=3, tag="g"):
+    """-> (value [Res,n], dpoints [3,n]) of the gradient kernel"""
+    res = c["chans"][-1]
+    fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
+    _write_input(fin, c, n)
+    args = [emu[0], fin, fout, str(sms)]
+    if c["grad_output"] is not None:
+        fg = str(tmp_path / ("gout_%s.f32" % tag))
+        c["grad_output"][:, :n].contiguous().numpy().astype(np.float32).tofile(fg)
+        args.append(fg)
+    r = subprocess.run(args, capture_output=True, text=True, timeout=1800)
+    assert r.returncode == 0, r.stderr[-2000:]
+    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
+    assert out.numel() == (res + 3) * n
+    return out[:res * n].reshape(res, n), out[res * n:].reshape(3, n)
+
+
+def _run_fp32(emu, tmp_path, c, n):
+    fin, fout = str(tmp_path / "in_q.bin"), str(tmp_path / "out_q.f32")
+    _write_input(fin, c, n)
+    r = subprocess.run([emu[1], fin, fout], capture_output=True, text=True, timeout=1800)
+    assert r.returncode == 0, r.stderr[-2000:]
+    return torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(c["chans"][-1], n)
+
+
+# the first 8 points of every case are border_points(): on the image border / corners and far outside
+@pytest.mark.parametrize("name,n", [("g_rot", 40), ("g_persp", 37), ("g_nocalib", 35), ("g_bigfeat", 33), ("c_rot", 34)])
+def test_kernel_matches_reference_grad_golden(emu, tmp_path, name, n):
+    c = load_grad_case(name)
+    val, dp = _run_grad(emu, tmp_path, c, n)
+    assert (val - c["value"][:, :n]).abs().max().item() <= 2e-5
+    ok, msg = within_bar(dp, c["grad32"][:, :n])
+    assert ok, msg
+
+
+@pytest.mark.parametrize("name", ["g_rot", "c_rot"])
+def test_kernel_value_is_the_fp32_query_bit_for_bit(emu, tmp_path, name):
+    c = load_grad_case(name)
+    n = 35
+    val, _ = _run_grad(emu, tmp_path, c, n)
+    assert torch.equal(val, _run_fp32(emu, tmp_path, c, n))
+
+
+def test_kernel_is_identical_on_1_to_3_sms(emu, tmp_path):
+    c = load_grad_case("g_nocalib")
+    n = 50                    # 4 tiles of 16 points, the last one ragged
+    want = _run_grad(emu, tmp_path, c, n, sms=1, tag="s1")
+    for sms in (2, 3):
+        got = _run_grad(emu, tmp_path, c, n, sms=sms, tag="s%d" % sms)
+        assert torch.equal(got[0], want[0]) and torch.equal(got[1], want[1]), sms
+
+
+def test_kernel_gradient_is_exactly_zero_outside_the_image(emu, tmp_path):
+    c = load_grad_case("g_rot")
+    n = 48
+    _, dp = _run_grad(emu, tmp_path, c, n)
+    xyz = spec.project_ref(c["points"][0, :, :n], c["calib"][0])
+    outside = ~((xyz[0] >= -1) & (xyz[0] <= 1) & (xyz[1] >= -1) & (xyz[1] <= 1))
+    assert int(outside.sum()) >= 3
+    assert bool((dp[:, outside] == 0).all())
+    assert bool((dp[:, ~outside].abs().sum(0) > 0).all())
+
+
+# ---- ptxas report ----------------------------------------------------------------------------------------------------------
+def test_grad_kernel_has_no_spill_and_no_stack_frame(tmp_path):
+    from monoport_b200 import build as lib_build
+    try:
+        nvcc = lib_build._nvcc()
+    except RuntimeError:
+        pytest.skip("nvcc not available")
+    cmd = [nvcc] + lib_build.NVCC_FLAGS + ["-c", os.path.join(lib_build.CSRC, "query_fp32.cu"), "-o", str(tmp_path / "q.o")]
+    p = subprocess.run(cmd, capture_output=True, text=True)
+    assert p.returncode == 0, p.stdout + p.stderr
+    found, current = {}, None
+    for line in (p.stdout + p.stderr).splitlines():
+        m = re.search(r"Compiling entry function '([^']+)'", line)
+        if m:
+            current = m.group(1) if "query_grad_kernel" in m.group(1) else None
+            if current:
+                found[current] = ""
+        elif current and ("spill" in line or "stack" in line):
+            found[current] += line
+    assert len(found) == 3, list(found)               # P = 32, 16, 8
+    for name, stats in found.items():
+        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", stats)
+        assert m and m.groups() == ("0", "0", "0"), (name, stats)

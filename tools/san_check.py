@@ -1,5 +1,5 @@
-"""Tiny invocation of every kernel family for compute-sanitizer (memcheck): both tensor-core programs, the fp32 kernel,
-the octree engine, marching cubes and the visible-surface kernel."""
+"""Tiny invocation of every kernel family for compute-sanitizer (memcheck): both tensor-core programs, the fp32 kernel and
+its point-gradient kernel, the octree engine, marching cubes and the visible-surface kernel."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -47,5 +47,11 @@ for mode in ("fp32", "tc", "auto"):
     ob = net.query([[fb]], pb, calibs=cb)[0]
     torch.cuda.synchronize()
     print("batch", mode, float(ob.sum()))
+# the point-gradient kernel: geometry head (ragged last tile), colour head with a grad_output and [N,3]-strided points
+vg, dg = net.query_gradient([[feat.cuda()]], pts[:, :, :123], calibs=cal)
+pv = pts[0, :, :77].t().contiguous().t()[None]
+vc, dc = netC.query_gradient([[featC]], pv, calibs=cal, grad_output=torch.randn(1, 3, 77, device="cuda"))
+torch.cuda.synchronize()
+print("grad", float(dg.abs().sum()), float(dc.abs().sum()))
 torch.cuda.synchronize()
 print("ok", X.numel(), v.shape, f.shape, float(img.sum()), float(big.sum()))
