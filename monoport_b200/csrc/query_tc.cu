@@ -18,7 +18,8 @@
 // warpgroups that split the N dimension of every layer (layer 1: 256 columns each, 128 fp32 accumulators per thread;
 // layer 2: 128; layer 3: 64); both sample the operands (X, the layer-0 chunks) and run the epilogues.  Warpgroup 2 is the
 // producer: one thread of it streams the weights L2 -> shared memory through a ring of 32 KB stages (cp.async.bulk on
-// mbarriers), pre-packed on the host as K-major SWIZZLE_128B tiles in exactly the order the consumers take them.  The
+// mbarriers), pre-packed on the host as K-major SWIZZLE_128B tiles in exactly the order the consumers take them; in layer
+// 1 the ring also borrows the two halves of H1, the layer-2 operand, two more stages in flight where they matter.  The
 // producer gives its registers to the consumers (setmaxnreg: 40 and 232 per thread).  The MMAs run asynchronously: the
 // role branches are warp-uniform by construction and the consumers wait for their MMAs at fixed points of a static
 // schedule (see the ring below), so layer-0 chunk c+1 is generated while the MMAs of chunk c are in flight.
@@ -53,20 +54,26 @@ template <int C> struct Prog {
   static constexpr int StagesL2 = 8 + XKB;
   static constexpr int StagesL3 = L3Pass * (XKB + 4) / 2;
   static constexpr int StagesPerTile = StagesL1 + StagesL2 + StagesL3;
-  static constexpr int Ring = C == 256 ? 3 : 2;
+  static constexpr int Ring = C == 256 ? 3 : 2;               // slots of the weight ring proper (Wr)
+  // Layer 1 streams through Slots = Ring + 2: H1 is only written by layer 1's epilogue, so until then its two 32 KB
+  // halves are ring slots 0 and 1 and the ring slots proper are 2 .. Slots-1 (slot q at H1 + q x 32 KB)
+  static constexpr int Slots = Ring + 2;
   // shared memory (offsets inside the 1024-aligned dynamic block)
   static constexpr int X = 0;                                 // XKB x 8 KB
   static constexpr int H0 = X + XKB * kKb;                    // 2 chunk buffers x 2 K-blocks; H2 (4 K-blocks) after layer 1
-  static constexpr int H1 = H0 + 4 * kKb;                     // 8 K-blocks; the last layer's partial sums after layer 2
+  static constexpr int H1 = H0 + 4 * kKb;                     // 8 K-blocks (layer 1: ring slots 0, 1); the last layer's partial sums after layer 2
   static constexpr int Wr = H1 + 8 * kKb;                     // Ring x 32 KB
   static constexpr int Small = Wr + Ring * kStageBytes;       // zf[64], inimg[64], s4[RES][64]
-  static constexpr int Bars = Small + (2 + RES) * kTile * 4;  // full[Ring], empty[Ring]
-  static constexpr int Total = Bars + 2 * Ring * 8;
+  static constexpr int Bars = Small + (2 + RES) * kTile * 4;  // full[Slots], empty[Slots]
+  static constexpr int Total = Bars + 2 * Slots * 8;
 };
 static_assert(Prog<256>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
 static_assert(Prog<512>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
 static_assert(Prog<256>::XKB % 2 == 0 && Prog<512>::XKB % 2 == 0, "layer-3 stages hold two K-blocks");
 static_assert(Prog<256>::StagesL3 >= Prog<256>::Ring && Prog<512>::StagesL3 >= Prog<512>::Ring, "a layer ends by releasing its last Ring stages");
+static_assert(Prog<256>::H1 + 2 * kStageBytes == Prog<256>::Wr && Prog<512>::H1 + 2 * kStageBytes == Prog<512>::Wr, "H1 = ring slots 0, 1");
+static_assert(Prog<256>::StagesL1 % Prog<256>::Slots == 0 && Prog<512>::StagesL1 % Prog<512>::Slots == 0,
+              "layer 1's last stages in slots 0 and 1 are StagesL1 - Slots and the one after it");
 
 struct TcPack {
   __half* wstream;        // stage stream of a tile: Prog<C>::StagesPerTile x 32 KB
@@ -247,7 +254,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   // every pointer below is a shared-memory pointer: 32-bit addresses and st.shared instead of 64-bit generic ones
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::Bars);
-  uint64_t* empty = full + Ring;
+  uint64_t* empty = full + P::Slots;
   float* s_zf = reinterpret_cast<float*>(smem + P::Small);
   float* s_in = s_zf + kTile;
   float* s_s4 = s_in + kTile;
@@ -276,27 +283,31 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   };
 
   if (tid == 0) {
-    for (int s = 0; s < Ring; ++s) {
+    for (int s = 0; s < P::Slots; ++s) {
       tc::mbar_init(full + s, 1);
       tc::mbar_init(empty + s, kConsumers / 32);
     }
     tc::fence_barrier_init();
   }
   __syncthreads();
+  // slot of a tile's stage: layer 1 stage s -> s % Slots; step k of layers 2 and 3 (counted across both) -> 2 + k % Ring
+  auto l1_slot = [](uint32_t s) { return s % (uint32_t)P::Slots; };
+  auto l23_slot = [](uint32_t k) { return 2u + k % (uint32_t)Ring; };
 
   if (wg == 2) {
     // ============================== weight producer ==============================
     tc::setmaxnreg_dec<kProducerRegs>();
     if (warp == 8 && lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
-      uint32_t it = 0;
+      uint32_t phase = 0;                  // bit q: parity of slot q's next refill
       for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
         if (tile_skipped(t)) continue;
-        for (int s = 0; s < P::StagesPerTile; ++s, ++it) {
-          const uint32_t slot = it % Ring, use = it / Ring;
-          tc::mbar_wait(empty + slot, (use & 1u) ^ 1u);
+        for (int s = 0; s < P::StagesPerTile; ++s) {
+          const uint32_t slot = s < P::StagesL1 ? l1_slot(s) : l23_slot(s - P::StagesL1);
+          tc::mbar_wait(empty + slot, ((phase >> slot) & 1u) ^ 1u);
+          phase ^= 1u << slot;
           tc::mbar_arrive_expect_tx(full + slot, kStageBytes);
-          tc::bulk_g2s(smem + P::Wr + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
+          tc::bulk_g2s(smem + P::H1 + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
         }
       }
     }
@@ -313,62 +324,67 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
 
   // ---- the weight ring, consumer side.  Every consumer takes every stage of a tile (56 for the geometry head, 76 for the
   // colour head) in a fixed order, so which stages a warpgroup still has in flight at any point is known at compile time:
-  // each wait below is a fixed wgmma_wait<N> and each release names its stage by arithmetic on the tile's first stage id
-  // s_tile (32-bit counters running across tiles, in step with the producer's).  No stage is ever queued at run time.
-  // Deadlock freedom: the producer refills the slot of stage s - Ring with stage s once all 8 consumer warps have released
-  // s - Ring, so every consumer must have released s - Ring before it waits for s.  Where that release needs the stage's
-  // MMAs complete, the wait for them comes first:
+  // each wait below is a fixed wgmma_wait<N> and each release names its stage by arithmetic on its index in the tile.
+  // No stage is ever queued at run time; the parity of each slot's next fill is one bit per slot (fphase), flipped by
+  // every take, as the producer flips its own bit per refill.
+  // Layer 1 streams through Slots = Ring + 2 slots (H1's halves are slots 0 and 1), layers 2 and 3 through the Ring slots
+  // 2 .. Slots-1: the deeper ring lets the producer run one more K-block ahead in layer 1, where each warpgroup waits for
+  // its K-block's MMAs before it takes the next.  H1's slots are refilled with the next tile's stages 0 and 1 only once
+  // H1 is dead: their last layer-1 stages (Defer, Defer + 1) are released at the end of the tile, and the layer-1
+  // epilogue writes H1 only after both warpgroups retired every MMA that read those slots.
+  // Deadlock freedom: the producer refills a slot with stage s once all 8 consumer warps have released the stage that last
+  // used it, so every consumer must have released that stage before it waits for s.  Where that release needs the
+  // stage's MMAs complete, the wait for them comes first:
   //   layer 1 (two stages per K-block i: 2i carries output half 0 for warpgroup 0, 2i+1 half 1 for warpgroup 1; each
   //     warpgroup releases the other's stage right after taking it and its own once the K-block's MMAs completed):
-  //     Ring 3: taking 2i+1 needs 2i-2 -- warpgroup 0's own stage of K-block i-1 -- so before it the warpgroup waits for
-  //             all its MMAs (wait<0>) and releases its own stage of K-block i-1; taking 2i needs 2i-3, released by
-  //             warpgroup 1 at that same point one K-block earlier;
-  //     Ring 2: taking 2i needs 2i-2 (warpgroup 0's own of K-block i-1), taking 2i+1 needs 2i-1 (warpgroup 1's), so the
-  //             wait<0> and the release come before both takes;
-  //   layers 2 and 3 (one stage per K-block step, read by both warpgroups): taking stage k needs k - Ring, so before it
-  //     the warpgroup lets at most Ring - 1 groups stay in flight (wait<Ring-1>) and releases k - Ring.
+  //     taking 2i+1 needs 2i+1-Slots <= 2i-3, which both warpgroups released by the end of K-block i-1's takes (its
+  //     owner after its wait<0> there); taking 2i needs 2i-Slots, released a K-block earlier still.  The deferred stages
+  //     are last users of slots 0 and 1, whose next stages are the next tile's 0 and 1;
+  //   layers 2 and 3 (one stage per K-block step, read by both warpgroups): taking step k needs k - Ring (for k < Ring a
+  //     layer-1 stage of slot 2 + k, released in layer 1), so before it the warpgroup lets at most Ring - 1 groups stay
+  //     in flight (wait<Ring-1>) and releases k - Ring.
   // Every layer ends with wait<0> and releases its own stages still held, so a layer starts with nothing in flight.
-  uint32_t s_tile = 0;
-  auto release = [&](uint32_t s) {
+  constexpr uint32_t Defer = P::StagesL1 - P::Slots;
+  uint32_t fphase = 0;
+  auto release_if = [&](uint32_t slot, bool pred) {
     __syncwarp();
-    tc::mbar_arrive_if(empty + s % Ring, lane == 0);
+    tc::mbar_arrive_if(empty + slot, pred && lane == 0);
   };
-  auto take = [&](uint32_t s) { tc::mbar_wait(full + s % Ring, (s / Ring) & 1u); };
-  auto wslot = [&](uint32_t s) { return P::Wr + (int)(s % Ring) * kStageBytes; };
+  auto release = [&](uint32_t slot) { release_if(slot, true); };
+  auto l1_release = [&](uint32_t s) { release_if(l1_slot(s), s - Defer >= 2u); };
+  auto take = [&](uint32_t slot) {
+    tc::mbar_wait(full + slot, (fphase >> slot) & 1u);
+    fphase ^= 1u << slot;
+  };
+  auto slot_off = [&](uint32_t slot) { return P::H1 + (int)slot * kStageBytes; };
   // layer 1, K-block i (A operand at shared offset a_off): this warpgroup's 256 outputs times its stage 2i + wg
   auto l1_kblock = [&](float (&acc)[128], int i, int a_off) {
-    const uint32_t s0 = s_tile + 2 * i, mine = s0 + wg, prev = mine - 2;
-    if constexpr (Ring < 3) {
-      tc::wgmma_wait<0>();
-      if (i > 0) release(prev);
-    }
-    take(s0);
-    if constexpr (Ring >= 3) {
-      tc::wgmma_wait<0>();
-      if (i > 0) release(prev);
-    }
-    take(s0 + 1);
-    release(s0 + 1 - wg);                            // the other warpgroup's half
-    const uint64_t da = desc(a_off), db = desc(wslot(mine));
+    const uint32_t s0 = 2 * i, mine = s0 + wg, prev = mine - 2;
+    take(l1_slot(s0));
+    tc::wgmma_wait<0>();
+    if (i > 0) l1_release(prev);
+    take(l1_slot(s0 + 1));
+    l1_release(s0 + 1 - wg);                         // the other warpgroup's half
+    const uint64_t da = desc(a_off), db = desc(slot_off(l1_slot(mine)));
     tc::wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
     tc::wgmma_commit();
   };
-  // layers 2 and 3, step k of a layer whose stages start at s_layer: frees the slot of stage k (see above) and takes it
-  auto step_take = [&](uint32_t s_layer, int k) {
+  // layers 2 and 3, step k of a layer whose steps start at k_layer: frees the slot of step k (see above) and takes it
+  auto step_take = [&](uint32_t k_layer, int k) {
     if (k >= Ring) {
       tc::wgmma_wait<Ring - 1>();
-      release(s_layer + k - Ring);
+      release(l23_slot(k_layer + k - Ring));
     }
-    take(s_layer + k);
+    take(l23_slot(k_layer + k));
     tc::wgmma_fence();
   };
   // end of a layer of n steps (n >= Ring): all MMAs complete, the last Ring stages released
-  auto layer_end = [&](uint32_t s_layer, int n) {
+  auto layer_end = [&](uint32_t k_layer, int n) {
     tc::wgmma_wait<0>();
 #pragma unroll
-    for (int j = Ring; j > 0; --j) release(s_layer + n - j);
+    for (int j = Ring; j > 0; --j) release(l23_slot(k_layer + n - j));
   };
 
   // ---- taps of this warp's 8 points for the layer-0 chunks: lane = (point 4 i + qw, channels 8 l8 .. and 64 + 8 l8 ..)
@@ -481,7 +497,8 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
 #pragma unroll 1
       for (int kb = 0; kb < XKB; ++kb) l1_kblock(acc, 16 + kb, P::X + kb * kKb);
       tc::wgmma_wait<0>();
-      release(s_tile + 2 * (16 + XKB - 1) + wg);
+      l1_release(2 * (16 + XKB - 1) + wg);
+      sync_consumers();        // H1 was ring slots 0 and 1: every MMA that read them has retired in both warpgroups
       // epilogue -> H1 (fp16, K-major): + bias + w_z z, leaky ReLU
 #pragma unroll
       for (int j = 0; j < 32; ++j) {
@@ -502,16 +519,15 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
       float acc[64];
 #pragma unroll
       for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-      const uint32_t s_l2 = s_tile + P::StagesL1;
 #pragma unroll 1
       for (int kb = 0; kb < P::StagesL2; ++kb) {
-        step_take(s_l2, kb);
-        const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(wslot(s_l2 + kb) + wg * 16384);
+        step_take(0, kb);
+        const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(slot_off(l23_slot(kb)) + wg * 16384);
 #pragma unroll
         for (int k = 0; k < 4; ++k) tc::wgmma_m64n128(acc, da + 2 * k, db + 2 * k);
         tc::wgmma_commit();
       }
-      layer_end(s_l2, P::StagesL2);
+      layer_end(0, P::StagesL2);
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int col = wg * 128 + 8 * j + cq;
@@ -531,22 +547,20 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
       float acc[32];
 #pragma unroll
       for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-      const uint32_t s_l3 = s_tile + P::StagesL1 + P::StagesL2;
 #pragma unroll 1
       for (int q = 0; q < P::StagesL3; ++q) {
-        step_take(s_l3, q);
+        step_take(P::StagesL2, q);
 #pragma unroll
         for (int sub = 0; sub < 2; ++sub) {
           const int kb = (2 * q + sub) % (XKB + 4);
           const uint64_t da = desc(kb < XKB ? P::X + kb * kKb : P::H0 + (kb - XKB) * kKb);
-          const uint64_t db = desc(wslot(s_l3 + q) + sub * 16384 + wg * 8192);
+          const uint64_t db = desc(slot_off(l23_slot(P::StagesL2 + q)) + sub * 16384 + wg * 8192);
 #pragma unroll
           for (int k = 0; k < 4; ++k) tc::wgmma_m64n64(acc, da + 2 * k, db + 2 * k);
         }
         tc::wgmma_commit();
       }
-      layer_end(s_l3, P::StagesL3);
-      s_tile += P::StagesPerTile;
+      layer_end(P::StagesL2, P::StagesL3);
       float lg[2][RES];
 #pragma unroll
       for (int h = 0; h < 2; ++h)
@@ -609,6 +623,10 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
         }
       }
       sync_consumers();        // the per-point scalars and X are rewritten by the next tile
+      // H1 (the layer-2 operand, then the partial sums) is dead: its slots may take the next tile's first stages
+      tc::fence_proxy_async_smem();
+      release(l1_slot(Defer));
+      release(l1_slot(Defer + 1));
     }
   }
 }
