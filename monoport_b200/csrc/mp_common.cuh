@@ -150,15 +150,16 @@ struct MpCalib {
   float z_scale;
 };
 
-// A batched query (mp_query_points_batch): B images of n points each, evaluated by one launch whose tiles never straddle
-// two images (tile t belongs to image t / tiles_per_image).  Image b reads its points at px/py/pz + b * pt_stride, its
-// calibration (rows 0..2 of [R|t], when MpCalib::has) from calibs[12 b ..] in device memory, its map's per-texel arrays at
-// the per-image offsets of mp_feat, and writes its outputs at out + b * out_stride.
+// The images of a query launch: B images of n points each, evaluated by one launch whose tiles never straddle two images
+// (tile t belongs to image t / tiles_per_image).  Image b reads its points at px/py/pz + b * pt_stride, its calibration
+// (rows 0..2 of [R|t], when MpCalib::has) from calibs[12 b ..] in device memory (null: MpCalib::m), its map's per-texel
+// arrays at the per-image offsets of mp_feat, and writes its outputs at out + b * out_stride.  The default is a
+// single-map launch.
 struct MpBatch {
-  int B;
-  long long pt_stride;
-  long long out_stride;
-  const float* calibs;   // [B][12] device
+  int B = 1;
+  long long pt_stride = 0;
+  long long out_stride = 0;
+  const float* calibs = nullptr;   // [B][12] device
 };
 
 // where results go
@@ -178,11 +179,14 @@ struct MpOutDst {
 // ---------------------------------------------------------------------------------------------
 // device helpers shared by the fp32 and tensor-core kernels
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void mp_load_point(const MpPointSrc& s, long long i, float& x, float& y, float& z) {
+// point i of image b (batched launches: MP_SRC_ROWS only)
+__device__ __forceinline__ void mp_load_point(const MpPointSrc& s, const MpBatch& bt, int b, long long i, float& x, float& y,
+                                              float& z) {
   if (s.kind == MP_SRC_ROWS) {
-    x = __ldg(s.px + i * s.pstride);
-    y = __ldg(s.py + i * s.pstride);
-    z = __ldg(s.pz + i * s.pstride);
+    const long long o = (long long)b * bt.pt_stride + i * s.pstride;
+    x = __ldg(s.px + o);
+    y = __ldg(s.py + o);
+    z = __ldg(s.pz + o);
     return;
   }
   int ix, iy, iz;
@@ -210,29 +214,27 @@ __device__ __forceinline__ void mp_load_point(const MpPointSrc& s, long long i, 
   z = __fadd_rn(__fmul_rn(__fadd_rn(__fdiv_rn(cz, R), s.half_inv_r), s.bext[2]), s.bmin[2]);
 }
 
-// image of tile t of a batched launch.  mp_query_points_batch keeps the launch under 2^31 tiles, so this is a 32-bit
-// division (a 64-bit one is a call, whose saved registers would spill in the tensor-core program)
-__device__ __forceinline__ int mp_tile_image(long long t, long long tiles_per_image) {
-  return (int)((unsigned)t / (unsigned)tiles_per_image);
+// Image of tile t.  Divisions stay 32-bit (a 64-bit one is a call, whose saved registers would spill in the tensor-core
+// program): mp_query_points_batch keeps a batched launch under 2^31 tiles, and a single-map launch, which has no such
+// bound, maps every tile to image 0 without dividing.
+__device__ __forceinline__ int mp_tile_image(const MpBatch& bt, long long t, long long tiles_per_image) {
+  return bt.B == 1 ? 0 : (int)((unsigned)t / (unsigned)tiles_per_image);
 }
 
-// point i of image b of a batched launch (MP_SRC_ROWS)
-__device__ __forceinline__ void mp_load_image_point(const MpPointSrc& s, const MpBatch& bt, int b, long long i, float& x, float& y,
-                                                    float& z) {
-  const long long o = (long long)b * bt.pt_stride + i * s.pstride;
-  x = __ldg(s.px + o);
-  y = __ldg(s.py + o);
-  z = __ldg(s.pz + o);
+// Tile t of image b is skipped by the range guard, and so is the rest of image b: the tile from which the launch's
+// grid-stride loop goes on to this CTA's first tile of image b + 1 (for the last image, one from which it ends).
+__device__ __forceinline__ long long mp_skip_image(const MpBatch& bt, long long t, int b, long long tiles_per_image) {
+  const long long end = (long long)(b + 1) * tiles_per_image;
+  if (b == bt.B - 1) return end - 1;
+  return t + (long long)((unsigned)(end - 1 - t) / gridDim.x) * gridDim.x;
 }
 
-// image b's calibration of a batched launch (the same projection and depth scale, its own [R|t] rows)
+// image b's calibration (the same projection and depth scale, its own [R|t] rows)
 __device__ __forceinline__ MpCalib mp_image_calib(const MpCalib& c, const MpBatch& bt, int b) {
-  MpCalib r;
-  r.has = c.has;
-  r.perspective = c.perspective;
-  r.z_scale = c.z_scale;
+  if (!bt.calibs) return c;
+  MpCalib r = c;
 #pragma unroll
-  for (int k = 0; k < 12; ++k) r.m[k] = c.has ? __ldg(bt.calibs + 12 * (long long)b + k) : 0.f;
+  for (int k = 0; k < 12; ++k) r.m[k] = __ldg(bt.calibs + 12 * (long long)b + k);
   return r;
 }
 
@@ -249,15 +251,22 @@ __device__ __forceinline__ void mp_shard_window(const MpPointSrc& s, long long n
   }
 }
 
-// geometry.py:19-34 / :37-55
+// geometry.py:19-34 / :37-55.  The roundings of every row m0 x + m1 y + m2 z + m3 are written out, so the result does not
+// depend on which product the compiler would leave unfused: the fp32 kernels round m1 y first, the tensor-core program
+// (X_FIRST) m0 x -- the results each program has always given.
+template <bool X_FIRST = false>
 __device__ __forceinline__ void mp_project(const MpCalib& c, float x, float y, float z, float& u, float& v, float& w) {
   if (!c.has) {
     u = x; v = y; w = z;
     return;
   }
-  u = c.m[0] * x + c.m[1] * y + c.m[2] * z + c.m[3];
-  v = c.m[4] * x + c.m[5] * y + c.m[6] * z + c.m[7];
-  w = c.m[8] * x + c.m[9] * y + c.m[10] * z + c.m[11];
+  auto row = [&](const float* m) {
+    const float p = X_FIRST ? fmaf(m[1], y, __fmul_rn(m[0], x)) : fmaf(m[0], x, __fmul_rn(m[1], y));
+    return __fadd_rn(fmaf(m[2], z, p), m[3]);
+  };
+  u = row(c.m);
+  v = row(c.m + 4);
+  w = row(c.m + 8);
   if (c.perspective) {
     u = u / w;
     v = v / w;
@@ -304,8 +313,8 @@ __device__ __forceinline__ float mp_lrelu(float v) { return v > 0.f ? v : v * MP
 // host-side launchers implemented in the kernel files
 // `guard`: the launch is conditional on the frame's feature range (feat->amax vs mlp->tc_amax_limit), evaluated on the device:
 //   MP_GUARD_NONE always run, MP_GUARD_IN_RANGE run when max|feature| <= limit, MP_GUARD_OUT_OF_RANGE run when it is above.
-// `bt` (batched launches only, nullptr otherwise): the launch covers bt->B images of src.n points; the guard is then
-// decided per tile from the maximum of the tile's own image (feat->amax[b]).
+// `bt` (batched launches; nullptr = one map): the launch covers bt->B images of src.n points.  The guard is decided per tile
+// from the maximum of the tile's own image (feat->amax[b]).
 enum { MP_GUARD_NONE = 0, MP_GUARD_IN_RANGE = 1, MP_GUARD_OUT_OF_RANGE = 2 };
 int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
@@ -317,8 +326,8 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
 int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
                          long long ld_dp, cudaStream_t st);
-// device-side predicate shared by the kernels: true = this launch (batched: this tile, amax = its image's entry) must do
-// nothing.  In the tensor-core program the weight producer and the consumers both take it, per tile, from the same word.
+// device-side predicate shared by the kernels: true = the tiles of this image (amax = its entry) must do nothing.  In the
+// tensor-core program the weight producer and the consumers both take it, per tile, from the same word.
 __device__ __forceinline__ bool mp_guard_skips(const unsigned* amax, float limit, int guard) {
   if (guard == MP_GUARD_NONE || amax == nullptr) return false;
   const bool above = __uint_as_float(*amax) > limit;

@@ -25,7 +25,7 @@ __global__ void node_points_kernel(MpPointSrc src, float* __restrict__ pts) {
   if (src.count_dev) { const long long c = *src.count_dev; n = c < n ? c : n; }
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     float x, y, z;
-    mp_load_point(src, i, x, y, z);
+    mp_load_point(src, MpBatch(), 0, i, x, y, z);
     pts[3 * i + 0] = x; pts[3 * i + 1] = y; pts[3 * i + 2] = z;
   }
 }

@@ -134,13 +134,10 @@ __device__ void dense_layer(const float* __restrict__ wt, const float* __restric
   }
 }
 
-// ---- the forward half of a tile for query_grad_kernel -----------------------------------------------------------------
-// The statements of query_fp32_kernel's steps 1-4 below (same helpers mp_project / mp_taps / dense_layer, same order of
-// every sum).  query_fp32_kernel keeps them inline: moved into shared functions they make ptxas contract the projection's
-// multiply-adds differently in its instantiations, which changes its results in the last bit.  So the value the gradient
-// call returns is computed by query_fp32_kernel itself; this copy feeds only the gradient.
-// 1. projection, mask, taps; 2. bilinear gather: sX = [sampled features ; z * z_scale], sMeta[p] = in_img
-template <int P, bool BATCH>
+// ---- the steps of a tile, shared by query_fp32_kernel and the forward half of query_grad_kernel ------------------------
+// 1. projection, mask, taps of image b's points; 2. bilinear gather from its map `feat`: sX = [sampled features ;
+// z * z_scale], sMeta[p] = in_img
+template <int P>
 __device__ __forceinline__ void tile_sample(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
                                             int b, const float* feat, long long p0, long long n, float* sX, float* sMeta,
                                             int (&sOff)[4][P], float (&sWgt)[4][P]) {
@@ -152,13 +149,8 @@ __device__ __forceinline__ void tile_sample(const Fp32Params& prm, const MpPoint
     bool valid = i < n;
     if (valid) {
       float x, y, z;
-      if constexpr (BATCH) {
-        mp_load_image_point(src, bt, b, i, x, y, z);
-        mp_project(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
-      } else {
-        mp_load_point(src, i, x, y, z);
-        mp_project(cal, x, y, z, u, v, w);
-      }
+      mp_load_point(src, bt, b, i, x, y, z);
+      mp_project(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
     }
     const bool in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);   // MonoPortNet.py:74
     MpTaps t = mp_taps(valid ? u : 0.f, valid ? v : 0.f, prm.H, prm.W);
@@ -181,9 +173,8 @@ __device__ __forceinline__ void tile_sample(const Fp32Params& prm, const MpPoint
     const float* f3 = feat + (size_t)sOff[3][p] * prm.C;
     const float w0 = sWgt[0][p], w1 = sWgt[1][p], w2 = sWgt[2][p], w3 = sWgt[3][p];
     for (int c = lane; c < prm.C; c += 32) {
-      // same accumulation order as grid_sample: nw, ne, sw, se
-      float v = __ldg(f0 + c) * w0;
-      v += __ldg(f1 + c) * w1;
+      // same accumulation order as grid_sample: nw, ne, sw, se (the first sum rounded as written: ne's product first)
+      float v = fmaf(__ldg(f0 + c), w0, __fmul_rn(__ldg(f1 + c), w1));
       v += __ldg(f2 + c) * w2;
       v += __ldg(f3 + c) * w3;
       sX[(size_t)c * P + p] = v;
@@ -235,9 +226,9 @@ __device__ __forceinline__ float last_layer_dot(const Fp32Params& prm, const flo
   return acc;
 }
 
-// BATCH: bt.B images of src.n points (MP_SRC_ROWS); tile t is tile t % n_tiles of image t / n_tiles, which samples its own
-// map and calibration and writes its own outputs; the range guard is decided per tile from that image's maximum.
-template <int P, bool BATCH = false>
+// bt.B images of src.n points (more than one: MP_SRC_ROWS); tile t is tile t % n_tiles of image t / n_tiles, which samples
+// its own map and calibration and writes its own outputs; the range guard is decided per tile from that image's maximum.
+template <int P>
 __global__ void __launch_bounds__(kThreads, 1)
 query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpBatch bt) {
   MP_DYN_SMEM_ALIGNED(float, smem, 16);
@@ -247,9 +238,6 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpB
   float* sMeta = sB + (size_t)prm.h_pong * P;        // [8][P]: in_img, u, v, z_feat, (4 spare)
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
-  if constexpr (!BATCH) {
-    if (mp_guard_skips(prm.amax, prm.amax_limit, prm.guard)) return;      // (uniform over the grid)
-  }
 
   long long n = src.n;
   if (src.count_dev) {
@@ -260,106 +248,33 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpB
   mp_shard_window(src, n, win0, win1);
   n = win1;                                          // points >= n are padding; the first evaluated one is win0
   const long long n_tiles = (win1 - win0 + P - 1) / P;          // (per image)
-  const long long all_tiles = BATCH ? n_tiles * bt.B : n_tiles;
+  const long long all_tiles = n_tiles * bt.B;
 
   for (long long at = blockIdx.x; at < all_tiles; at += gridDim.x) {
-    const int b = BATCH ? mp_tile_image(at, n_tiles) : 0;
-    if (BATCH && mp_guard_skips(prm.amax + b, prm.amax_limit, prm.guard)) continue;      // (uniform over the CTA)
-    const long long tile = BATCH ? at - (long long)b * n_tiles : at;
-    const float* feat = BATCH ? prm.feat + (size_t)b * prm.H * prm.W * prm.C : prm.feat;
-    float* out = BATCH ? dst.out + b * bt.out_stride : dst.out;
-    const long long p0 = win0 + tile * P;
-    // ---- 1. projection, mask, taps ------------------------------------------------------------
+    const int b = mp_tile_image(bt, at, n_tiles);
+    if (mp_guard_skips(prm.amax + b, prm.amax_limit, prm.guard)) {      // (uniform over the CTA)
+      at = mp_skip_image(bt, at, b, n_tiles);
+      continue;
+    }
+    const long long p0 = win0 + (at - (long long)b * n_tiles) * P;
     __shared__ int sOff[4][P];
     __shared__ float sWgt[4][P];
-    if (tid < P) {
-      const long long i = p0 + tid;
-      float u = 0.f, v = 0.f, w = 0.f;
-      bool valid = i < n;
-      if (valid) {
-        float x, y, z;
-        if constexpr (BATCH) {
-          mp_load_image_point(src, bt, b, i, x, y, z);
-          mp_project(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
-        } else {
-          mp_load_point(src, i, x, y, z);
-          mp_project(cal, x, y, z, u, v, w);
-        }
-      }
-      const bool in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);   // MonoPortNet.py:74
-      MpTaps t = mp_taps(valid ? u : 0.f, valid ? v : 0.f, prm.H, prm.W);
-      // NaN coordinates (perspective with w==0): in_img is false; keep taps finite
-      if (!(u == u) || !(v == v)) {
-#pragma unroll
-        for (int a = 0; a < 4; ++a) { t.off[a] = 0; t.wgt[a] = 0.f; }
-      }
-#pragma unroll
-      for (int a = 0; a < 4; ++a) { sOff[a][tid] = t.off[a]; sWgt[a][tid] = t.wgt[a]; }
-      sMeta[0 * P + tid] = in_img ? 1.f : 0.f;
-      sX[(size_t)prm.C * P + tid] = w * cal.z_scale;                                          // DepthNormalizer.py:32
-    }
-    __syncthreads();
-    // ---- 2. bilinear gather: warp per point, lanes over channels (NHWC => contiguous) ---------
-    for (int p = warp; p < P; p += kThreads / 32) {
-      const float* f0 = feat + (size_t)sOff[0][p] * prm.C;
-      const float* f1 = feat + (size_t)sOff[1][p] * prm.C;
-      const float* f2 = feat + (size_t)sOff[2][p] * prm.C;
-      const float* f3 = feat + (size_t)sOff[3][p] * prm.C;
-      const float w0 = sWgt[0][p], w1 = sWgt[1][p], w2 = sWgt[2][p], w3 = sWgt[3][p];
-      for (int c = lane; c < prm.C; c += 32) {
-        // same accumulation order as grid_sample: nw, ne, sw, se
-        float v = __ldg(f0 + c) * w0;
-        v += __ldg(f1 + c) * w1;
-        v += __ldg(f2 + c) * w2;
-        v += __ldg(f3 + c) * w3;
-        sX[(size_t)c * P + p] = v;
-      }
-    }
-    __syncthreads();
-    // ---- 3. hidden layers ---------------------------------------------------------------------
-    const float* sIn = sX;
-    float* sOut = sA;
-    for (int l = 0; l < prm.n_layers - 1; ++l) {
-      const int hid = prm.hid[l];
-      const int skipw = prm.cin[l] - hid;
-      if (l == 0) {
-        dense_layer<P, 2>(prm.wt[l], prm.bias[l], 0, prm.cin[l], prm.cout[l], sX, sX, sOut);
-      } else if (prm.cout[l] > kThreads) {
-        dense_layer<P, 2>(prm.wt[l], prm.bias[l], hid, skipw, prm.cout[l], sIn, sX, sOut);
-      } else {
-        dense_layer<P, 1>(prm.wt[l], prm.bias[l], hid, skipw, prm.cout[l], sIn, sX, sOut);
-      }
-      __syncthreads();
-      sIn = sOut;
-      sOut = (sOut == sA) ? sB : sA;
-    }
-    // ---- 4. last layer: one warp per (point, out channel) dot product -------------------------
-    {
-      const int l = prm.n_layers - 1;
-      const int res = prm.cout[l];
-      const int hid = prm.n_layers == 1 ? 0 : prm.hid[l];
-      const int cin = prm.cin[l];
-      for (int job = warp; job < P * res; job += kThreads / 32) {
-        const int p = job % P, r = job / P;
-        const float* wrow = prm.w_last + (size_t)r * cin;
-        float acc = 0.f;
-        for (int k = lane; k < cin; k += 32) {
-          const float a = (prm.n_layers == 1) ? sX[(size_t)k * P + p]
-                          : (k < hid ? sIn[(size_t)k * P + p] : sX[(size_t)(k - hid) * P + p]);
-          acc = fmaf(__ldg(wrow + k), a, acc);
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-        if (lane == 0) {
-          const long long i = p0 + p;
-          if (i < n) {
-            float v = mp_last_op(acc + __ldg(prm.bias[l] + r), prm.last_op);
-            v = sMeta[p] * v;                                                              // MonoPortNet.py:89
-            if (out) out[(long long)r * dst.ld + i] = v;
-            if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = v;
-            if (r == 0)
-              for (int pp = 0; pp < dst.n_peers; ++pp) dst.peer[pp][dst.peer_off + i] = v;      // peer-memory stores (NVLink)
-          }
+    tile_sample<P>(prm, src, cal, bt, b, prm.feat + (size_t)b * prm.H * prm.W * prm.C, p0, n, sX, sMeta, sOff, sWgt);
+    const float* sIn = tile_hidden<P, false>(prm, sX, sA, sB);
+    const int l = prm.n_layers - 1;
+    float* out = dst.out + b * bt.out_stride;
+    for (int job = warp; job < P * prm.cout[l]; job += kThreads / 32) {
+      const int p = job % P, r = job / P;
+      const float acc = last_layer_dot<P>(prm, sX, sIn, p, r, lane);
+      if (lane == 0) {
+        const long long i = p0 + p;
+        if (i < n) {
+          float v = mp_last_op(acc + __ldg(prm.bias[l] + r), prm.last_op);
+          v = sMeta[p] * v;                                                              // MonoPortNet.py:89
+          if (out) out[(long long)r * dst.ld + i] = v;
+          if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = v;
+          if (r == 0)
+            for (int pp = 0; pp < dst.n_peers; ++pp) dst.peer[pp][dst.peer_off + i] = v;      // peer-memory stores (NVLink)
         }
       }
     }
@@ -463,14 +378,14 @@ query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
   const int res = prm.cout[L - 1];
   const long long n = src.n;
   const long long n_tiles = (n + P - 1) / P;
-  const MpBatch b1{};                                // (unused: single-map launches)
+  const MpBatch one;                                 // (a single map)
 
   for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const long long p0 = tile * P;
-    // ---- forward half: the fp32 kernel's code, plus the sign masks --------------------------------
+    // ---- forward half: the fp32 kernel's steps, plus the sign masks --------------------------------
     __shared__ int sOff[4][P];
     __shared__ float sWgt[4][P];
-    tile_sample<P, false>(prm, src, cal, b1, 0, prm.feat, p0, n, sX, sMeta, sOff, sWgt);
+    tile_sample<P>(prm, src, cal, one, 0, prm.feat, p0, n, sX, sMeta, sOff, sWgt);
     const float* sIn = tile_hidden<P, true>(prm, sX, sA, sB, sMask, gp.mask_off);
     for (int job = warp; job < P * res; job += kThreads / 32) {
       const int p = job % P, r = job / P;
@@ -511,7 +426,7 @@ query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
         continue;
       }
       float x, y, z, u, v, w;
-      mp_load_point(src, i, x, y, z);
+      mp_load_point(src, one, 0, i, x, y, z);
       mp_project(cal, x, y, z, u, v, w);
       // the tap cell of mp_taps; a tap outside the map is zero padding and contributes nothing
       const float ix = ((u + 1.f) / 2.f) * (float)(prm.W - 1);
@@ -590,34 +505,27 @@ int launch_grad(const Fp32Params& prm, const GradParams& gp, const MpPointSrc& s
 
 template <int P>
 int launch(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst, cudaStream_t st,
-           int sm_count, int max_smem, const MpBatch* bt) {
+           int sm_count, int max_smem, const MpBatch& bt) {
   const size_t smem = Fp32Smem<P>::bytes(prm.c0, prm.h_ping, prm.h_pong);
   // The opt-in is a property of the kernel, shared by every thread, and heads of different widths launch the same
   // instantiation with different sizes: it is always set to the same bound -- the device's maximum less the 2 KB the size
   // selection below keeps free for the kernel's static shared memory -- so no thread lowers it under another thread's
   // launch.  (Sticky per device: raising it again for every launch costs a driver call per query.)
   const int opt_in = max_smem - 2048;
-  static thread_local bool opted[2][64] = {};
-  const int variant = bt ? 1 : 0;
+  static thread_local bool opted[64] = {};
   int dev_ = 0;
   MP_CUDA(cudaGetDevice(&dev_));
-  if (dev_ < 0 || dev_ >= 64 || !opted[variant][dev_]) {
-    if (bt) MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
-    else MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
-    if (dev_ >= 0 && dev_ < 64) opted[variant][dev_] = true;
+  if (dev_ < 0 || dev_ >= 64 || !opted[dev_]) {
+    MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
+    if (dev_ >= 0 && dev_ < 64) opted[dev_] = true;
   }
-  long long tiles = (bt ? bt->B : 1) * ((src.n + P - 1) / P);
+  long long tiles = bt.B * ((src.n + P - 1) / P);
   int grid = (int)(tiles < (long long)sm_count ? (tiles > 0 ? tiles : 1) : sm_count);
-  MpBatch b1;
-  memset(&b1, 0, sizeof(b1));
-  const MpBatch& bb = bt ? *bt : b1;
 #ifndef MP_CUDA_EMU
-  if (bt) query_fp32_kernel<P, true><<<grid, kThreads, smem, st>>>(prm, src, cal, dst, bb);
-  else query_fp32_kernel<P><<<grid, kThreads, smem, st>>>(prm, src, cal, dst, bb);
+  query_fp32_kernel<P><<<grid, kThreads, smem, st>>>(prm, src, cal, dst, bt);
 #else
   // tests/emu: CPU model of the execution model
-  if (bt) MP_EMU_LAUNCH(grid, kThreads, (query_fp32_kernel<P, true>(prm, src, cal, dst, bb)));
-  else MP_EMU_LAUNCH(grid, kThreads, query_fp32_kernel<P>(prm, src, cal, dst, bb));
+  MP_EMU_LAUNCH(grid, kThreads, query_fp32_kernel<P>(prm, src, cal, dst, bt));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -683,9 +591,10 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
     mp_set_error("batched launches take point rows and write [R,N] outputs");
     return MP_E_UNSUPPORTED;
   }
-  if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32>(prm, src, cal, dst, st, sms, max_smem, bt);
-  if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16>(prm, src, cal, dst, st, sms, max_smem, bt);
-  if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8>(prm, src, cal, dst, st, sms, max_smem, bt);
+  const MpBatch& b = bt ? *bt : MpBatch();
+  if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32>(prm, src, cal, dst, st, sms, max_smem, b);
+  if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16>(prm, src, cal, dst, st, sms, max_smem, b);
+  if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8>(prm, src, cal, dst, st, sms, max_smem, b);
   mp_set_error("head too wide for the fp32 kernel's shared-memory tiling");
   return MP_E_UNSUPPORTED;
 }

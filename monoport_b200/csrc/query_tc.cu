@@ -14,7 +14,7 @@
 // Tanh output is four times as sensitive to the logit as the geometry head's Sigmoid, and the rounding of W3 is the largest
 // single term of its error.
 //
-// One persistent CTA per SM; a tile = 64 points = the M of every warpgroup MMA (a batched launch: of one image, see BATCH).  Warps 0-3 and 4-7 are two consumer
+// One persistent CTA per SM; a tile = 64 points (of one image) = the M of every warpgroup MMA.  Warps 0-3 and 4-7 are two consumer
 // warpgroups that split the N dimension of every layer (layer 1: 256 columns each, 128 fp32 accumulators per thread;
 // layer 2: 128; layer 3: 64); both sample the operands (X, the layer-0 chunks) and run the epilogues.  Warpgroup 2 is the
 // producer: one thread of it streams the weights L2 -> shared memory through a ring of 32 KB stages (cp.async.bulk on
@@ -136,9 +136,8 @@ struct PointTaps {
   bool in_img;      // MonoPortNet.py:74
 };
 
-// projection (geometry.py:19-55) + mask + taps of point i (i >= n: masked-out padding point); surface vertices when surf.X.
-// BATCH: point i of image b, projected with image b's calibration.
-template <bool BATCH>
+// projection (geometry.py:19-55) + mask + taps of point i of image b (i >= n: masked-out padding point), projected with
+// image b's calibration; surface vertices when surf.X.
 __device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
                                                 int b, int H, int W, long long i, long long n) {
   PointTaps pt;
@@ -146,20 +145,15 @@ __device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const 
   const bool valid = i < n;
   if (valid) {
     float x, y, z;
-    if constexpr (BATCH) {
-      mp_load_image_point(src, bt, b, i, x, y, z);
-      mp_project(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
+    if (surf.X) {
+      const float vx = (float)__ldg(surf.X + i), vy = (float)__ldg(surf.Y + i), vz = __fsub_rn(surf.R, __ldg(surf.Z + i));
+      x = __fadd_rn(__fmul_rn(vx, surf.scale[0]), surf.bmin[0]);
+      y = __fadd_rn(__fmul_rn(vy, surf.scale[1]), surf.bmin[1]);
+      z = __fadd_rn(__fmul_rn(vz, surf.scale[2]), surf.bmin[2]);
     } else {
-      if (surf.X) {
-        const float vx = (float)__ldg(surf.X + i), vy = (float)__ldg(surf.Y + i), vz = __fsub_rn(surf.R, __ldg(surf.Z + i));
-        x = __fadd_rn(__fmul_rn(vx, surf.scale[0]), surf.bmin[0]);
-        y = __fadd_rn(__fmul_rn(vy, surf.scale[1]), surf.bmin[1]);
-        z = __fadd_rn(__fmul_rn(vz, surf.scale[2]), surf.bmin[2]);
-      } else {
-        mp_load_point(src, i, x, y, z);
-      }
-      mp_project(cal, x, y, z, u, v, w);
+      mp_load_point(src, bt, b, i, x, y, z);
     }
+    mp_project<true>(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
   }
   pt.in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);
   const MpTaps t = mp_taps(valid ? u : 0.f, valid ? v : 0.f, H, W);
@@ -240,15 +234,14 @@ __device__ __forceinline__ uint32_t act_pack(float a, float b) {
 // releases a stage once the MMAs that read it have completed (one arrival per consumer warp); the operand buffers written
 // by the consumers themselves are published with fence.proxy.async + a named barrier over the 256 consumer threads.
 // PEERS: also store channel 0 into the peer volumes of dst (fused slab exchange).
-// BATCH: bt.B images of src.n points (MP_SRC_ROWS, [R,N] outputs); tile t is tile t % n_tiles of image t / n_tiles, and the
-// range guard skips the tiles of the images outside the head's range -- the producer and the consumers skip exactly the
-// same tiles (same predicate on the same amax word), so the weight-ring stage counters stay in step.
-template <int C, bool PEERS, bool BATCH = false>
+// bt.B images of src.n points (more than one: MP_SRC_ROWS, [R,N] outputs); tile t is tile t % n_tiles of image t / n_tiles,
+// and the range guard skips the tiles of the images outside the head's range -- the producer and the consumers skip
+// exactly the same tiles (same predicate on the same amax word), so the weight-ring stage counters stay in step.
+template <int C, bool PEERS>
 __global__ void __launch_bounds__(kThreads, 1)
 query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpSurfaceSrc surf, MpBatch bt) {
   using P = Prog<C>;
   constexpr int RES = P::RES, Ring = P::Ring, XKB = P::XKB;
-  static_assert(!(BATCH && PEERS), "batched launches have no peer stores");
   MP_DYN_SMEM(uint8_t, smem_raw);
   // aligned by an offset from the shared array itself (not through an integer cast), so the compiler keeps knowing that
   // every pointer below is a shared-memory pointer: 32-bit addresses and st.shared instead of 64-bit generic ones
@@ -264,9 +257,6 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   // divergent path; otherwise it wraps every wgmma in warpgroup.arrive / wait and the MMAs run one at a time (C7520).
   const int tid = threadIdx.x, lane = tid & 31;
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0), wg = warp >> 2;
-  if constexpr (!BATCH) {
-    if (__shfl_sync(0xffffffffu, (int)mp_guard_skips(prm.amax, prm.amax_limit, prm.guard), 0)) return;      // (uniform over the grid)
-  }
 
   long long n = src.n;
   if (src.count_dev) {
@@ -277,10 +267,10 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   mp_shard_window(src, n, win0, win1);
   n = win1;                                          // points >= n are padding; tile 0 starts at point win0
   const long long n_tiles = (win1 - win0 + kTile - 1) / kTile;       // (per image)
-  const long long all_tiles = BATCH ? n_tiles * bt.B : n_tiles;
-  auto tile_skipped = [&](long long t) {       // (the consumer warps take lane 0's answer)
-    return BATCH && mp_guard_skips(prm.amax + mp_tile_image(t, n_tiles), prm.amax_limit, prm.guard);
-  };
+  const long long all_tiles = n_tiles * bt.B;
+  // the range guard of image b, read once per image a CTA meets (consecutive tiles of an image need no second read; the
+  // consumer warps take lane 0's answer)
+  auto image_skipped = [&](int b) { return mp_guard_skips(prm.amax + b, prm.amax_limit, prm.guard); };
 
   if (tid == 0) {
     for (int s = 0; s < P::Slots; ++s) {
@@ -300,8 +290,18 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
     if (warp == 8 && lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
       uint32_t phase = 0;                  // bit q: parity of slot q's next refill
+      int guard_b = -1;
+      bool skip = false;
       for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
-        if (tile_skipped(t)) continue;
+        const int b = mp_tile_image(bt, t, n_tiles);
+        if (b != guard_b) {
+          skip = image_skipped(b);
+          guard_b = b;
+        }
+        if (skip) {
+          t = mp_skip_image(bt, t, b, n_tiles);
+          continue;
+        }
         for (int s = 0; s < P::StagesPerTile; ++s) {
           const uint32_t slot = s < P::StagesL1 ? l1_slot(s) : l23_slot(s - P::StagesL1);
           tc::mbar_wait(empty + slot, ((phase >> slot) & 1u) ^ 1u);
@@ -390,7 +390,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   // ---- taps of this warp's 8 points for the layer-0 chunks: lane = (point 4 i + qw, channels 8 l8 .. and 64 + 8 l8 ..)
   const int l8 = lane & 7, qw = lane >> 3;
   uint32_t t_off[2][2], t_wgt[2][2], t_z[2];
-  int img = 0;                       // BATCH: the tile's image (its per-texel arrays start at texel img * H * W)
+  const __half* g0 = prm.g0;         // the tile's image's block of G0
   auto gen_chunk = [&](int c) {
     const int ch = c * 128 + l8 * 8;
     __half2 b8[8], z8[8];
@@ -408,7 +408,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
 #pragma unroll
       for (int a = 0; a < 4; ++a) {
         const uint32_t off = (a & 1) ? (t_off[i][a >> 1] >> 16) : (t_off[i][a >> 1] & 0xFFFFu);
-        const uint4* srcp = reinterpret_cast<const uint4*>(prm.g0 + ((BATCH ? (size_t)img * prm.H * prm.W : 0) + (size_t)off) * kL0 + ch);
+        const uint4* srcp = reinterpret_cast<const uint4*>(g0 + (size_t)off * kL0 + ch);
         raw[i][a][0] = __ldg(srcp);
         raw[i][a][1] = __ldg(srcp + 8);      // + 64 channels
       }
@@ -443,22 +443,29 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
     tc::fence_proxy_async_smem();
   };
 
+  int guard_b = -1, skip = 0;
   for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
-    if (__shfl_sync(0xffffffffu, (int)tile_skipped(t), 0)) continue;
-    const int b = BATCH ? mp_tile_image(t, n_tiles) : 0;
-    const long long p0 = win0 + (BATCH ? t - (long long)b * n_tiles : t) * kTile;
-    if constexpr (BATCH) img = b;
+    const int b = mp_tile_image(bt, t, n_tiles);
+    if (b != guard_b) {
+      skip = __shfl_sync(0xffffffffu, (int)image_skipped(b), 0);
+      guard_b = b;
+    }
+    if (skip) {
+      t = mp_skip_image(bt, t, b, n_tiles);
+      continue;
+    }
+    const long long p0 = win0 + (t - (long long)b * n_tiles) * kTile;
     const size_t texel0 = (size_t)b * prm.H * prm.W;
+    g0 = prm.g0 + texel0 * kL0;
     // ---- X (skip operand) + per-point scalars: 4 groups of 16 points x C/256 channel phases over the 8 warps
 #pragma unroll 1
     for (int job = warp; job < 4 * (C / 256); job += 8) {
       const int grp = job & 3, phase = job >> 2;
-      const PointTaps pt = point_taps<BATCH>(surf, src, cal, bt, b, prm.H, prm.W, p0 + grp * 16 + (lane & 15), n);
-      sample_x16<C>(prm, prm.feat16 + (BATCH ? texel0 * C : 0), prm.s4tex + (BATCH ? texel0 * RES : 0), smem + P::X, s_zf, s_in, s_s4,
-                    pt, grp * 16, lane, phase);
+      const PointTaps pt = point_taps(surf, src, cal, bt, b, prm.H, prm.W, p0 + grp * 16 + (lane & 15), n);
+      sample_x16<C>(prm, prm.feat16 + texel0 * C, prm.s4tex + texel0 * RES, smem + P::X, s_zf, s_in, s_s4, pt, grp * 16, lane, phase);
     }
     {
-      const PointTaps pt = point_taps<BATCH>(surf, src, cal, bt, b, prm.H, prm.W, p0 + warp * 8 + l8, n);
+      const PointTaps pt = point_taps(surf, src, cal, bt, b, prm.H, prm.W, p0 + warp * 8 + l8, n);
       const uint32_t o01 = (uint32_t)pt.off[0] | ((uint32_t)pt.off[1] << 16), o23 = (uint32_t)pt.off[2] | ((uint32_t)pt.off[3] << 16);
       const uint32_t w01 = tc::pack_half2(pt.wgt[0], pt.wgt[1]), w23 = tc::pack_half2(pt.wgt[2], pt.wgt[3]);
       const uint32_t zz = tc::pack_half2(pt.zf, pt.zf);
@@ -606,11 +613,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
               px[r] = __fadd_rn(__fmul_rn(val, 0.5f), 0.5f);      // RTL/main.py:244
               continue;
             }
-            if constexpr (BATCH) {
-              dst.out[mp_tile_image(t, n_tiles) * bt.out_stride + (long long)r * dst.ld + i] = val;
-              continue;
-            }
-            if (dst.out) dst.out[(long long)r * dst.ld + i] = val;
+            if (dst.out) dst.out[mp_tile_image(bt, t, n_tiles) * bt.out_stride + (long long)r * dst.ld + i] = val;
             if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = val;
             if constexpr (PEERS) {
               if (r == 0) {
@@ -888,7 +891,6 @@ int tc_prepare(mp_mlp* mlp) {
   }
   if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(g0_wg_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G0Cfg<C>::Smem);
   if (e != cudaSuccess) {
     mp_set_error("mp_tc_prepare: %s", cudaGetErrorString(e));
@@ -900,10 +902,10 @@ int tc_prepare(mp_mlp* mlp) {
 }
 
 // per-frame per-texel products of the head (G0, the fp16 copy of the map, S4) for every map of the handle, then the fused
-// query (bt: a batched launch over all of them)
+// query over the images of bt
 template <int C>
 int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
-           cudaStream_t st, const MpSurfaceSrc& surf, int guard, const MpBatch* bt) {
+           cudaStream_t st, const MpSurfaceSrc& surf, int guard, const MpBatch& bt) {
   using P = Prog<C>;
   const long long HW = (long long)feat->H * feat->W;
   const int maps = feat->B > 1 ? feat->B : 1;
@@ -961,19 +963,14 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
   int dev = 0, sms = 132;
   MP_CUDA(cudaGetDevice(&dev));
   MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const long long tiles = (bt ? bt->B : 1) * ((src.n + kTile - 1) / kTile);
+  const long long tiles = bt.B * ((src.n + kTile - 1) / kTile);
   const int grid = (int)(tiles < (long long)sms ? tiles : sms);
-  MpBatch b1;
-  memset(&b1, 0, sizeof(b1));
-  const MpBatch& bb = bt ? *bt : b1;
 #ifndef MP_CUDA_EMU
-  if (bt) query_wg_kernel<C, false, true><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bb);
-  else if (dst.n_peers > 0) query_wg_kernel<C, true><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bb);      // fused slab exchange
-  else query_wg_kernel<C, false><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bb);
+  if (dst.n_peers > 0) query_wg_kernel<C, true><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bt);      // fused slab exchange
+  else query_wg_kernel<C, false><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bt);
 #else
-  if (bt) MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, false, true>(prm, src, cal, dst, surf, bb)));
-  else if (dst.n_peers > 0) MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, true>(prm, src, cal, dst, surf, bb)));
-  else MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, false>(prm, src, cal, dst, surf, bb)));
+  if (dst.n_peers > 0) MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, true>(prm, src, cal, dst, surf, bt)));
+  else MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, false>(prm, src, cal, dst, surf, bt)));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -1039,7 +1036,7 @@ int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* 
   src.n = n;
   MpOutDst dst;
   dst.out = nullptr; dst.ld = 0; dst.scatter_vol = nullptr;
-  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, MP_GUARD_NONE, nullptr);
+  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, MP_GUARD_NONE, MpBatch());
 }
 
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
@@ -1073,6 +1070,7 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
     mp_set_error("batched launches take point rows and write [R,N] outputs");
     return MP_E_UNSUPPORTED;
   }
-  return C == 256 ? launch<256>(mlp, pk, feat, src, cal, dst, st, surf, guard, bt)
-                  : launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, bt);
+  const MpBatch& b = bt ? *bt : MpBatch();
+  return C == 256 ? launch<256>(mlp, pk, feat, src, cal, dst, st, surf, guard, b)
+                  : launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, b);
 }

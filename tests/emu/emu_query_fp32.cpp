@@ -1,6 +1,7 @@
 // TEST INFRASTRUCTURE ONLY: monoport_b200/csrc/query_fp32.cu (the exact CUDA-core kernel: default path of the colour head
 // and of every head shape the tensor-core programs do not cover) compiled unmodified on the CPU emulation layer.
-//   emu_query_fp32 in.bin out.f32        (in.bin as for emu_query_tc)
+//   emu_query_fp32 in.bin out.f32 [batch B]        (in.bin and out.f32 as for emu_query_tc, batch B included: one launch over
+//   B images, what mp_query_points_batch sets up)
 #include <cuda_runtime.h>
 #include <stdarg.h>
 
@@ -33,7 +34,9 @@ void mp_set_error(const char* fmt, ...) {
 #include "../../monoport_b200/csrc/query_fp32.cu"
 
 int main(int argc, char** argv) {
-  if (argc != 3) { fprintf(stderr, "usage: emu_query_fp32 in.bin out.f32\n"); return 2; }
+  const bool batched = argc == 5 && !strcmp(argv[3], "batch");
+  if (argc != 3 && !batched) { fprintf(stderr, "usage: emu_query_fp32 in.bin out.f32 [batch B]\n"); return 2; }
+  const int B = batched ? atoi(argv[4]) : 1;
   FILE* f = fopen(argv[1], "rb");
   if (!f) { perror(argv[1]); return 2; }
   int32_t hd[8];
@@ -41,7 +44,9 @@ int main(int argc, char** argv) {
   if (fread(hd, 4, 8, f) != 8 || fread(&zs, 4, 1, f) != 1 || fread(calib, 4, 12, f) != 12) { fprintf(stderr, "short header\n"); return 2; }
   const int C = hd[0], H = hd[1], W = hd[2], N = hd[3], has_calib = hd[4], persp = hd[5], res = hd[6], last_op = hd[7];
   auto rd = [&](size_t n) { std::vector<float> v(n); if (fread(v.data(), 4, n, f) != n) { fprintf(stderr, "short file\n"); exit(2); } return v; };
-  std::vector<float> nchw = rd((size_t)C * H * W), pts = rd((size_t)3 * N);
+  const size_t per_map = (size_t)C * H * W;
+  std::vector<float> nchw = rd(B * per_map), pts = rd((size_t)B * 3 * N);
+  std::vector<float> calibs = batched && has_calib ? rd((size_t)B * 12) : std::vector<float>();
   const int chans[6] = {C + 1, 1024, 512, 256, 128, res};
   mp_mlp mlp;
   memset(&mlp, 0, sizeof(mlp));
@@ -59,12 +64,13 @@ int main(int argc, char** argv) {
     mlp.w[l] = Ws[l].data(); mlp.wt[l] = Wt[l].data(); mlp.bias[l] = Bs[l].data();
   }
   fclose(f);
-  std::vector<float> nhwc((size_t)C * H * W);
-  for (int c = 0; c < C; ++c)
-    for (int p = 0; p < H * W; ++p) nhwc[(size_t)p * C + c] = nchw[(size_t)c * H * W + p];
+  std::vector<float> nhwc(B * per_map);
+  for (int b = 0; b < B; ++b)
+    for (int c = 0; c < C; ++c)
+      for (int p = 0; p < H * W; ++p) nhwc[b * per_map + (size_t)p * C + c] = nchw[b * per_map + (size_t)c * H * W + p];
   mp_feat feat;
   memset(&feat, 0, sizeof(feat));
-  feat.C = C; feat.H = H; feat.W = W; feat.nhwc32 = nhwc.data();
+  feat.B = B; feat.C = C; feat.H = H; feat.W = W; feat.nhwc32 = nhwc.data();
   MpPointSrc src;
   memset(&src, 0, sizeof(src));
   src.kind = MP_SRC_ROWS;
@@ -77,14 +83,19 @@ int main(int argc, char** argv) {
   memcpy(cal.m, calib, sizeof(calib));
   cal.perspective = persp && has_calib;
   cal.z_scale = zs;
-  std::vector<float> out((size_t)res * N + 1, -4242.f);
+  MpBatch bt;                     // (batched: the [R|t] rows come from the device calibs)
+  bt.B = B;
+  bt.pt_stride = 3ll * N;
+  bt.out_stride = (long long)res * N;
+  bt.calibs = has_calib ? calibs.data() : nullptr;
+  std::vector<float> out((size_t)B * res * N + 1, -4242.f);
   MpOutDst dst;
   dst.out = out.data(); dst.ld = N; dst.scatter_vol = nullptr;
-  const int rc = mp_launch_query_fp32(&mlp, &feat, src, cal, dst, nullptr);
+  const int rc = mp_launch_query_fp32(&mlp, &feat, src, cal, dst, nullptr, MP_GUARD_NONE, batched ? &bt : nullptr);
   if (rc != MP_OK) { fprintf(stderr, "mp_launch_query_fp32: %s\n", g_err); return 3; }
-  if (out[(size_t)res * N] != -4242.f) { fprintf(stderr, "wrote past the output\n"); return 3; }
+  if (out[(size_t)B * res * N] != -4242.f) { fprintf(stderr, "wrote past the output\n"); return 3; }
   f = fopen(argv[2], "wb");
-  fwrite(out.data(), 4, (size_t)res * N, f);
+  fwrite(out.data(), 4, (size_t)B * res * N, f);
   fclose(f);
   return 0;
 }

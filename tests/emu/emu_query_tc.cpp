@@ -1,9 +1,13 @@
 // TEST INFRASTRUCTURE ONLY: monoport_b200/csrc/query_tc.cu -- host-side weight packing, launch logic, the per-frame G0
 // GEMM kernel and the fused wgmma sample+MLP kernel -- compiled UNMODIFIED for the CPU against the execution-model
 // emulation (cuda_emu.h) and the functional model of the wgmma / mbarrier / bulk-copy layer (tc_ptx_emu.h).
-//   emu_query_tc in.bin out.f32 program sms
+//   emu_query_tc in.bin out.f32 program sms [grid R z0 nz | nodes R res | surface R | batch B]
 // in.bin: int32 header {C, H, W, N, has_calib, perspective, res, last_op}, float z_scale, calib[12], then fp32 arrays:
 //   feature map NCHW [C*H*W], points [3*N], for each of the 5 layers W_l [cout*cin] and b_l [cout].
+// batch B: the batched launch (what mp_query_points_batch sets up: one launch over B images, the per-frame G0 kernel on a
+//   texel-blocks x B grid, the range guard decided per tile).  in.bin then holds B feature maps [B*C*H*W] and B point sets
+//   [B*3*N], and when has_calib B calibs [B*12] (rows 0..2 of [R|t]) after them instead of the header's calib;
+//   out.f32 is [B][res][N], pre-filled with -4242 (the tiles a guarded launch skips keep it).
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdarg.h>
@@ -64,7 +68,8 @@ template <class T> static cudaError_t cudaFuncSetAttribute(T*, cudaFuncAttribute
 
 #include "../../monoport_b200/csrc/query_tc.cu"
 
-int mp_launch_query_fp32(const mp_mlp*, const mp_feat*, const MpPointSrc&, const MpCalib&, const MpOutDst&, cudaStream_t, int) { return MP_E_UNSUPPORTED; }
+int mp_launch_query_fp32(const mp_mlp*, const mp_feat*, const MpPointSrc&, const MpCalib&, const MpOutDst&, cudaStream_t, int,
+                         const MpBatch*) { return MP_E_UNSUPPORTED; }
 
 // mp_api.cu's helper (that file holds <<<>>> launches and is not part of this build)
 static void fill_grid_geom(MpPointSrc& s, int res, int node_stride, int r_final) {
@@ -82,7 +87,9 @@ int main(int argc, char** argv) {
   //   nodes: every third node of the res^3 level of an R^3 pyramid, through an index list + a device-side count that
   //          is smaller than the list capacity, scattered into a res^3 volume (the octree engine's fused path)
   const char* src_kind = argc >= 6 ? argv[5] : "rows";
-  if (argc < 5) { fprintf(stderr, "usage: emu_query_tc in.bin out.f32 program sms [grid R z0 nz | nodes R res]\n"); return 2; }
+  if (argc < 5) { fprintf(stderr, "usage: emu_query_tc in.bin out.f32 program sms [grid R z0 nz | nodes R res | surface R | batch B]\n"); return 2; }
+  const bool batched = !strcmp(src_kind, "batch");
+  const int B = batched ? atoi(argv[6]) : 1;
   const int program = atoi(argv[3]);
   g_fake_sms = atoi(argv[4]);
   FILE* f = fopen(argv[1], "rb");
@@ -92,7 +99,9 @@ int main(int argc, char** argv) {
   if (fread(hd, 4, 8, f) != 8 || fread(&zs, 4, 1, f) != 1 || fread(calib, 4, 12, f) != 12) { fprintf(stderr, "short header\n"); return 2; }
   const int C = hd[0], H = hd[1], W = hd[2], N = hd[3], has_calib = hd[4], persp = hd[5], res = hd[6], last_op = hd[7];
   auto rd = [&](size_t n) { std::vector<float> v(n); if (fread(v.data(), 4, n, f) != n) { fprintf(stderr, "short file\n"); exit(2); } return v; };
-  std::vector<float> nchw = rd((size_t)C * H * W), pts = rd((size_t)3 * N);
+  const size_t per_map = (size_t)C * H * W;
+  std::vector<float> nchw = rd(B * per_map), pts = rd((size_t)B * 3 * N);
+  std::vector<float> calibs = batched && has_calib ? rd((size_t)B * 12) : std::vector<float>();
   const int chans[6] = {C + 1, 1024, 512, 256, 128, res};
   mp_mlp mlp;
   memset(&mlp, 0, sizeof(mlp));
@@ -118,15 +127,16 @@ int main(int argc, char** argv) {
     fprintf(stderr, "d_bias0[0..3] = %g %g %g %g   d_wz0[0..1] = %g %g  h_bias[0]=%g\n", __half2float(pk->d_bias0[0]), __half2float(pk->d_bias0[1]),
             __half2float(pk->d_bias0[2]), __half2float(pk->d_bias0[3]), __half2float(pk->d_wz0[0]), __half2float(pk->d_wz0[1]), pk->h_bias[0]);
   }
-  // feature handle: channel-last copy (what nchw_to_nhwc_kernel produces)
-  std::vector<float> nhwc((size_t)C * H * W);
-  for (int c = 0; c < C; ++c)
-    for (int p = 0; p < H * W; ++p) nhwc[(size_t)p * C + c] = nchw[(size_t)c * H * W + p];
+  // feature handle: B channel-last maps, one after the other (what nchw_to_nhwc_kernel produces), one amax word per map
+  std::vector<float> nhwc(B * per_map);
+  for (int b = 0; b < B; ++b)
+    for (int c = 0; c < C; ++c)
+      for (int p = 0; p < H * W; ++p) nhwc[b * per_map + (size_t)p * C + c] = nchw[b * per_map + (size_t)c * H * W + p];
   mp_feat feat;
   memset(&feat, 0, sizeof(feat));
-  feat.C = C; feat.H = H; feat.W = W; feat.nhwc32 = nhwc.data(); feat.version = 1;
-  unsigned amax_word = 0;
-  feat.amax = &amax_word;
+  feat.B = B; feat.C = C; feat.H = H; feat.W = W; feat.nhwc32 = nhwc.data(); feat.version = 1;
+  std::vector<unsigned> amax(B, 0u);
+  feat.amax = amax.data();
   MpPointSrc src;
   memset(&src, 0, sizeof(src));
   src.kind = MP_SRC_ROWS;
@@ -185,7 +195,12 @@ int main(int argc, char** argv) {
     mp_tc_release(&mlp);
     return 0;
   }
-  std::vector<float> out((size_t)res * n_out + 1, -4242.f);
+  MpBatch bt;                     // (batched: the [R|t] rows come from the device calibs)
+  bt.B = B;
+  bt.pt_stride = 3ll * N;
+  bt.out_stride = (long long)res * N;
+  bt.calibs = has_calib ? calibs.data() : nullptr;
+  std::vector<float> out((size_t)B * res * n_out + 1, -4242.f);
   MpOutDst dst;
   dst.out = out.data(); dst.ld = n_out; dst.scatter_vol = nullptr;
   if (!scatter.empty()) { dst.out = nullptr; dst.ld = 0; dst.scatter_vol = scatter.data(); }
@@ -203,11 +218,12 @@ int main(int argc, char** argv) {
   for (int r = 0; r < shard_world && rc == MP_OK; ++r) {
     src.shard_rank = r;
     src.shard_world = shard_world;
-    rc = mp_launch_query_tc(&mlp, &feat, src, cal, dst, nullptr, guard);
+    rc = mp_launch_query_tc(&mlp, &feat, src, cal, dst, nullptr, guard, batched ? &bt : nullptr);
   }
-  if (getenv("EMU_TC_AMAX")) { float a; memcpy(&a, &amax_word, 4); fprintf(stderr, "amax %.9g\n", a); }
+  if (getenv("EMU_TC_AMAX"))
+    for (int b = 0; b < B; ++b) { float a; memcpy(&a, &amax[b], 4); fprintf(stderr, "amax[%d] %.9g\n", b, a); }
   if (rc != MP_OK) { fprintf(stderr, "mp_launch_query_tc: %s\n", g_err); return 3; }
-  if (out[(size_t)res * n_out] != -4242.f) { fprintf(stderr, "wrote past the output\n"); return 3; }
+  if (out[(size_t)B * res * n_out] != -4242.f) { fprintf(stderr, "wrote past the output\n"); return 3; }
   if (!scatter.empty()) out.assign(scatter.begin(), scatter.end());       // report the scattered volume
   for (int p = 0; p < n_peers; ++p)
     for (long long i = 0; i < (long long)peer[p].size(); ++i) {
@@ -217,7 +233,7 @@ int main(int argc, char** argv) {
       if (memcmp(&peer[p][i], &want, 4) != 0) { fprintf(stderr, "peer volume %d differs at %lld\n", p, i); return 3; }
     }
   f = fopen(argv[2], "wb");
-  fwrite(out.data(), 4, (size_t)res * n_out, f);
+  fwrite(out.data(), 4, (size_t)B * res * n_out, f);
   fclose(f);
   if (const char* dump = getenv("EMU_TC_DUMP")) {       // per-texel products of the G0 kernel, for debugging the model
     if (feat.g0) {

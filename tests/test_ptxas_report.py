@@ -50,10 +50,10 @@ def _entries(log):
     return found
 
 
-def test_every_instantiation_is_reported(ptxas_log):
+def test_each_head_has_a_plain_and_a_peer_store_instantiation(ptxas_log):
     names = list(_entries(ptxas_log))
-    # query_wg_kernel: 2 heads x (plain, peer stores, batch); g0_wg_kernel: 2 heads
-    assert sum("query_wg_kernel" in n for n in names) == 6, names
+    # query_wg_kernel: 2 heads x (plain, peer stores); g0_wg_kernel: 2 heads
+    assert sum("query_wg_kernel" in n for n in names) == 4, names
     assert sum("g0_wg_kernel" in n for n in names) == 2, names
 
 

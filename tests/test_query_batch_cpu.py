@@ -51,15 +51,12 @@ def _build(tmp, name):
 
 @pytest.fixture(scope="module")
 def emu_tc(tmp_path_factory):
-    """(batched launches, single-image launches)"""
-    d = str(tmp_path_factory.mktemp("emu_batch_tc"))
-    return _build(d, "emu_query_tc_batch"), _build(d, "emu_query_tc")
+    return _build(str(tmp_path_factory.mktemp("emu_batch_tc")), "emu_query_tc")
 
 
 @pytest.fixture(scope="module")
 def emu_fp32(tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("emu_batch_fp32"))
-    return _build(d, "emu_query_fp32_batch"), _build(d, "emu_query_fp32")
+    return _build(str(tmp_path_factory.mktemp("emu_batch_fp32")), "emu_query_fp32")
 
 
 def _write_input(path, feat, points, calib, proj, res, last_op, Ws, bs, batched):
@@ -81,9 +78,8 @@ def _write_input(path, feat, points, calib, proj, res, last_op, Ws, bs, batched)
             f.write(bl.numpy().tobytes())
 
 
-def _run(exes, tmp_path, case, n, args, batched, env=None, feat=None, tag="x"):
-    """-> [B,Res,n] (batched harness) or [Res,n] (single-image harness)"""
-    exe = exes[0] if batched else exes[1]
+def _run(exe, tmp_path, case, n, args, batched, env=None, feat=None, tag="x"):
+    """-> [B,Res,n] (a batched launch: args end with "batch B") or [Res,n] (a single-image launch)"""
     feat = case["feat"] if feat is None else feat
     res = case["expected"].shape[1]
     fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
@@ -113,7 +109,7 @@ def _single(case, b):
 ])
 def test_tc_batch_matches_batched_reference_golden(emu_tc, tmp_path, name, n, sms):
     c = load_batch_case(name)
-    got = _run(emu_tc, tmp_path, c, n, [0 if c["net"] == "C" else 3, sms, c["B"]], True)
+    got = _run(emu_tc, tmp_path, c, n, [0 if c["net"] == "C" else 3, sms, "batch", c["B"]], True)
     want = c["expected"][:, :, :n]
     assert (got - want).abs().max().item() <= 1e-4
     assert torch.equal(got[want == 0], want[want == 0]), "out-of-image points must be exactly 0"
@@ -122,7 +118,7 @@ def test_tc_batch_matches_batched_reference_golden(emu_tc, tmp_path, name, n, sm
 @pytest.mark.parametrize("name,n", [("g_nocalib", 150), ("g_persp", 70), ("c_rot", 40), ("g_rot", 33)])
 def test_fp32_batch_matches_batched_reference_golden(emu_fp32, tmp_path, name, n):
     c = load_batch_case(name)
-    got = _run(emu_fp32, tmp_path, c, n, [c["B"]], True)
+    got = _run(emu_fp32, tmp_path, c, n, ["batch", c["B"]], True)
     want = c["expected"][:, :, :n]
     assert (got - want).abs().max().item() <= 2e-5
     assert torch.equal(got[want == 0], want[want == 0])
@@ -131,7 +127,7 @@ def test_fp32_batch_matches_batched_reference_golden(emu_fp32, tmp_path, name, n
 def test_fp32_batch_image_equals_single_run(emu_fp32, tmp_path):
     c = load_batch_case("g_nocalib")
     n = 77
-    got = _run(emu_fp32, tmp_path, c, n, [c["B"]], True)
+    got = _run(emu_fp32, tmp_path, c, n, ["batch", c["B"]], True)
     for b in range(c["B"]):
         one = _run(emu_fp32, tmp_path, _single(c, b), n, [], False, tag="one%d" % b)
         assert torch.equal(got[b], one), b
@@ -143,7 +139,7 @@ def test_tc_batch_image_equals_single_run_bit_for_bit(emu_tc, tmp_path, sms):
     on one CTA, the weight ring running across images)."""
     c = load_batch_case("g_nocalib")
     n = 130
-    got = _run(emu_tc, tmp_path, c, n, [3, sms, c["B"]], True)
+    got = _run(emu_tc, tmp_path, c, n, [3, sms, "batch", c["B"]], True)
     for b in range(c["B"]):
         one = _run(emu_tc, tmp_path, _single(c, b), n, [3, sms], False, tag="one%d" % b)
         assert torch.equal(got[b], one), (sms, b)
@@ -153,8 +149,8 @@ def test_tc_batch_image_equals_single_run_bit_for_bit(emu_tc, tmp_path, sms):
 def test_tc_batch_bit_identity_under_other_completion_orders(emu_tc, tmp_path, order):
     c = load_batch_case("g_nocalib")
     n = 100
-    want = _run(emu_tc, tmp_path, c, n, [3, 2, c["B"]], True)
-    got = _run(emu_tc, tmp_path, c, n, [3, 2, c["B"]], True, env={"EMU_TC_ORDER": order}, tag="ord")
+    want = _run(emu_tc, tmp_path, c, n, [3, 2, "batch", c["B"]], True)
+    got = _run(emu_tc, tmp_path, c, n, [3, 2, "batch", c["B"]], True, env={"EMU_TC_ORDER": order}, tag="ord")
     assert torch.equal(got, want)
     for b in range(c["B"]):
         one = _run(emu_tc, tmp_path, _single(c, b), n, [3, 2], False, env={"EMU_TC_ORDER": order}, tag="one%d" % b)
@@ -175,9 +171,9 @@ def test_tc_batch_range_guard_skips_exactly_the_out_of_range_image(emu_tc, tmp_p
     assert amax[1] > limit and amax[0] < limit and amax[2] < limit, amax
     n = 140
     env = {"EMU_TC_LIMIT": str(limit), "EMU_TC_GUARD": "1"}
-    got = _run(emu_tc, tmp_path, case, n, [3, sms, 3], True, env=env)
+    got = _run(emu_tc, tmp_path, case, n, [3, sms, "batch", 3], True, env=env)
     assert bool((got[1] == -4242.0).all()), "the out-of-range image's outputs must stay untouched"
-    free = _run(emu_tc, tmp_path, case, n, [3, sms, 3], True, tag="free")      # no guard
+    free = _run(emu_tc, tmp_path, case, n, [3, sms, "batch", 3], True, tag="free")      # no guard
     assert torch.equal(got[0], free[0]) and torch.equal(got[2], free[2])
     for b in (0, 2):
         one = _run(emu_tc, tmp_path, _single(case, b), n, [3, sms], False, tag="one%d" % b)

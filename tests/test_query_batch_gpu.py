@@ -16,17 +16,6 @@ TOL = {"fp32": 2e-5, "tc": 1e-4, "auto": 1e-4}
 TOL_COLOUR = {"fp32": 2e-5, "tc": 1e-4, "auto": 1e-4}
 
 
-def _same(mode, a, b):
-    """A batched image against the single query of that image.  The exact kernel gives the same bits.  The batch
-    instantiation of the tensor-core program is compiled separately, and its fp32 arithmetic outside the MMAs (projection,
-    depth feature, last layer) is not pinned by explicit roundings, so the compiler is free to fuse it differently: on the
-    GPU the two agree to rounding level, inside the parity bar.  The CPU model, built without contraction, is bit-identical
-    (tests/test_query_batch_cpu.py)."""
-    if mode == "fp32":
-        return torch.equal(a, b)
-    return (a - b).abs().max().item() <= 1e-4
-
-
 def _modes(net):
     return ["fp32", "tc", "auto"] if net.surface_classifier.tc_supported() else ["fp32"]
 
@@ -79,7 +68,7 @@ def test_batched_images_equal_single_queries(B):
                 b_ = net.query([[feat]], p.permute(0, 2, 1).contiguous().permute(0, 2, 1), calibs=calib)[0]
                 assert torch.equal(a, b_), (mode, n)
                 for b in range(B):
-                    assert _same(mode, a[b], singles[b]), (mode, n, b, (a[b] - singles[b]).abs().max().item())
+                    assert torch.equal(a[b], singles[b]), (mode, n, b, (a[b] - singles[b]).abs().max().item())
         e = net.query([[feat]], torch.zeros(B, 3, 0, device="cuda"), calibs=cal)[0]
         assert e.shape == (B, 1, 0)
 
@@ -93,12 +82,12 @@ def test_batched_colour_head_equals_single_queries():
         a = net.query([[feat]], pts, calibs=cal)[0]
         for b in range(c["B"]):
             one = _single(net, feat, pts, cal, b)
-            assert _same(mode, a[b], one), (mode, b, (a[b] - one).abs().max().item())
+            assert torch.equal(a[b], one), (mode, b, (a[b] - one).abs().max().item())
 
 
 def test_per_image_range_guard():
     """g_mixed: image 1 is above the geometry head's limit.  In "auto" mode it is evaluated by the exact kernel (equal to
-    its fp32-mode single query, bit for bit), the others on the tensor cores (their tc-mode single queries, see _same)."""
+    its fp32-mode single query, bit for bit), the others on the tensor cores (their tc-mode single queries, bit for bit)."""
     c = load_batch_case("g_mixed")
     net = build_net(c)
     if not net.surface_classifier.tc_supported():
@@ -111,7 +100,7 @@ def test_per_image_range_guard():
     net.precision = "tc"
     tc0, tc2 = _single(net, feat, pts, cal, 0), _single(net, feat, pts, cal, 2)
     assert torch.equal(got[1], exact1)
-    assert _same("tc", got[0], tc0) and _same("tc", got[2], tc2)
+    assert torch.equal(got[0], tc0) and torch.equal(got[2], tc2)
     net.precision = "fp32"
     assert not torch.equal(got[0], _single(net, feat, pts, cal, 0)), "image 0 is in range: the tensor cores evaluate it"
     assert (got.cpu() - c["expected"]).abs().max().item() <= TOL["auto"]
