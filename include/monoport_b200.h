@@ -267,6 +267,20 @@ int mp_forward_vertices_async(const float* vol_dev, int R, int direction, int64_
 int mp_colorize_surface(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev, const float* z_dev,
                         int64_t n, int R, const float* b_min3, const float* b_max3, const float* calib12, int projection,
                         float z_scale, float* canvas_dev, void* stream);
+/* The same render for CUDA-graph captured frame steps: enqueue-only (no host read, no allocation, no synchronisation).
+ * The vertex count is the int64 count_dev of mp_forward_vertices_async, read on the device and clamped to `capacity` (the
+ * length of the x/y/z buffers, at most R*R); vertices at or beyond it are neither evaluated nor drawn.  `mode` as for
+ * mp_query_points: MP_MODE_FP32 renders with the exact fp32 kernel; MP_MODE_TC / MP_MODE_AUTO with the tensor-core program
+ * when the frame's largest |feature| is inside the head's limit and with the exact kernel when it is not, decided on the
+ * device (MP_MODE_AUTO without a tensor-core program: the exact kernel).  Any head with 3 outputs; single-map handles. */
+int mp_colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev, const float* z_dev,
+                              const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
+                              const float* calib12, int projection, float z_scale, int mode, float* canvas_dev, void* stream);
+/* The normal image of the demo (RTL/main.py:212-228, colorization(norm=...)): canvas[X[i], Y[i], :] =
+ * clamp((norm[i] + 1) / 2, 0, 1) for the first min(*count_dev, capacity) vertices, bit for bit what torch gives (NaN
+ * normals stay NaN).  Enqueue-only like the call above; capacity <= R*R. */
+int mp_render_normals_async(const int64_t* x_dev, const int64_t* y_dev, const float* norm_dev, const int64_t* count_dev,
+                            int64_t capacity, int R, float* canvas_dev, void* stream);
 
 #ifdef __cplusplus
 }

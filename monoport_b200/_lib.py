@@ -80,7 +80,10 @@ SIGNATURES = {
     "mp_mcubes_emit": (c_int, [c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p]),
     "mp_colorize_surface": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, P(c_float), P(c_float),
                                     P(c_float), c_int, c_float, c_void_p, c_void_p]),
-    "mp_forward_vertices": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, P(c_int64),
+    "mp_colorize_surface_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, P(c_float),
+                                          P(c_float), P(c_float), c_int, c_float, c_int, c_void_p, c_void_p]),
+    "mp_render_normals_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
+    "mp_forward_vertices":(c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, P(c_int64),
                                     c_void_p]),
     "mp_forward_vertices_scratch_bytes": (c_int64, [c_int]),
     "mp_forward_vertices_async": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,

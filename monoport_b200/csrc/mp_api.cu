@@ -486,6 +486,42 @@ extern "C" int mp_colorize_surface(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t
                                   n, R, b_min3, b_max3, cal, canvas_dev, (cudaStream_t)stream);
 }
 
+// The same render, enqueue-only (graph-capturable): the vertex count stays on the device and the range guard is decided
+// there, exactly as mp_query_dispatch decides it for a query -- the tensor-core launch renders a frame inside the head's
+// range, its exact fp32 twin one outside it, and the other launch returns at once.
+extern "C" int mp_colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev,
+                                         const float* z_dev, const int64_t* count_dev, int64_t capacity, int R, const float* b_min3,
+                                         const float* b_max3, const float* calib12, int projection, float z_scale, int mode,
+                                         float* canvas_dev, void* stream) {
+  MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE_SINGLE_MAP(feat, "mp_colorize_surface_async");
+  MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 3, "surface colourisation needs a head with 3 outputs (got %d)",
+             mlp->cout[mlp->n_layers - 1]);
+  MP_REQUIRE(capacity >= 0 && R >= 1 && capacity <= (int64_t)R * R, "bad sizes capacity=%lld R=%d", (long long)capacity, R);
+  MP_REQUIRE(x_dev && y_dev && z_dev && count_dev && canvas_dev && b_min3 && b_max3, "NULL argument");
+  if (capacity == 0) return MP_OK;
+  MpRange nvtx("monoport_b200: F1 fused surface colourisation");
+  MpCalib cal;
+  mp_fill_calib(cal, calib12, projection, z_scale);
+  const MpSurfaceSrc surf = mp_surface_src(reinterpret_cast<const long long*>(x_dev), reinterpret_cast<const long long*>(y_dev), z_dev,
+                                           reinterpret_cast<const long long*>(count_dev), R, b_min3, b_max3, canvas_dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool tc_can = mlp->tc_ok && (long long)feat->H * feat->W <= 65536;
+  if (mode == MP_MODE_AUTO) mode = tc_can ? MP_MODE_TC : MP_MODE_FP32;
+  if (mode == MP_MODE_TC || mode == MP_MODE_TC_V3) {
+    if (!mlp->tc_ok) {
+      mp_set_error("MP_MODE_TC requested but the tensor-core kernel does not support this head/device");
+      return MP_E_UNSUPPORTED;
+    }
+    const bool guarded = isfinite(mlp->tc_amax_limit);
+    int rc = mp_launch_surface_tc(mlp, feat, surf, capacity, cal, st, guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE);
+    if (rc != MP_OK || !guarded) return rc;
+    return mp_launch_surface_fp32(mlp, feat, surf, capacity, cal, st, MP_GUARD_OUT_OF_RANGE);
+  }
+  MP_REQUIRE(mode == MP_MODE_FP32, "bad mode %d", mode);
+  return mp_launch_surface_fp32(mlp, feat, surf, capacity, cal, st, MP_GUARD_NONE);
+}
+
 // Volumes that other processes of the node write into: plain cudaMalloc blocks (exportable; the caching allocators of
 // frameworks hand out sub-blocks, which legacy IPC handles cannot describe) + their 64-byte IPC handle.
 extern "C" int mp_ipc_alloc(size_t bytes, void** dev_ptr, unsigned char* handle64) {

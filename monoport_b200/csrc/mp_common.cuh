@@ -162,6 +162,51 @@ struct MpBatch {
   const float* calibs = nullptr;   // [B][12] device
 };
 
+// Direct rendering of the visible surface (RTL/main.py:212-249), shared by both query programs: point i is the vertex
+// (X[i], Y[i], R - Z[i]) of forward_vertices mapped to world space by mat_color (RTL/main.py:201-210: diag((b_max-b_min)/R),
+// translation b_min), and its colour pred * 0.5 + 0.5 (:244) is scattered to canvas[X[i], Y[i], :] (:247-248) -- no
+// intermediate point / prediction tensors.  X == nullptr: the ordinary point sources and the [R,N] output.
+struct MpSurfaceSrc {
+  const long long* X;
+  const long long* Y;
+  const float* Z;
+  const long long* count;       // nullable: the vertex count on the device (mp_forward_vertices_async's count_dev); the
+                                // launch's n is then the capacity, and vertices at or beyond min(*count, n) are not touched
+  float scale[3], bmin[3];      // (b_max - b_min) / R and b_min, fp32 like torch's
+  float R;
+  float* canvas;                // [R, R, 3]
+  int canvas_R;
+};
+
+inline MpSurfaceSrc mp_surface_src(const long long* X, const long long* Y, const float* Z, const long long* count, int R,
+                                   const float* b_min3, const float* b_max3, float* canvas) {
+  MpSurfaceSrc s;
+  memset(&s, 0, sizeof(s));
+  s.X = X; s.Y = Y; s.Z = Z; s.count = count;
+  for (int a = 0; a < 3; ++a) {
+    s.scale[a] = (b_max3[a] - b_min3[a]) / (float)R;          // mat[a,a] = length / resolution  (RTL/main.py:207)
+    s.bmin[a] = b_min3[a];
+  }
+  s.R = (float)R;
+  s.canvas = canvas;
+  s.canvas_R = R;
+  return s;
+}
+
+// world position of vertex i: the two fp32 roundings of torch's `verts * scale + b_min` (RTL/main.py:231-237)
+__device__ __forceinline__ void mp_surface_point(const MpSurfaceSrc& s, long long i, float& x, float& y, float& z) {
+  const float vx = (float)__ldg(s.X + i), vy = (float)__ldg(s.Y + i), vz = __fsub_rn(s.R, __ldg(s.Z + i));
+  x = __fadd_rn(__fmul_rn(vx, s.scale[0]), s.bmin[0]);
+  y = __fadd_rn(__fmul_rn(vy, s.scale[1]), s.bmin[1]);
+  z = __fadd_rn(__fmul_rn(vz, s.scale[2]), s.bmin[2]);
+}
+
+// the canvas pixel of vertex i takes channel r of its value v as v * 0.5 + 0.5 (RTL/main.py:244-248)
+__device__ __forceinline__ void mp_surface_store(const MpSurfaceSrc& s, long long i, int r, float v) {
+  float* px = s.canvas + ((size_t)__ldg(s.X + i) * s.canvas_R + (size_t)__ldg(s.Y + i)) * 3;
+  px[r] = __fadd_rn(__fmul_rn(v, 0.5f), 0.5f);
+}
+
 // where results go
 #define MP_MAX_PEERS 8
 struct MpOutDst {
@@ -334,8 +379,16 @@ __device__ __forceinline__ bool mp_guard_skips(const unsigned* amax, float limit
   return guard == MP_GUARD_IN_RANGE ? above : !above;
 }
 // colour head only: vertices (X, Y, R - Z) of the visible surface -> world -> colour -> canvas[X, Y, :]   (query_tc.cu)
+// The eager entry point: the vertex count n on the host, the feature range checked on the host (MP_E_RANGE above the limit).
 int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* X, const long long* Y, const float* Z, long long n,
                              int R, const float* b_min3, const float* b_max3, const MpCalib& cal, float* canvas, cudaStream_t st);
+// The same render by either program, enqueue-only: n = the capacity (surf.count, when set, the count on the device) and the
+// range guard decided on the device (`guard` as above).  _tc: the colour head's tensor-core program (query_tc.cu); _fp32: the
+// exact kernel (query_fp32.cu), any head with 3 outputs.
+int mp_launch_surface_tc(const mp_mlp* mlp, mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
+                         cudaStream_t st, int guard);
+int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
+                           cudaStream_t st, int guard);
 int mp_tc_prepare(mp_mlp* mlp);     // builds mlp->tc; sets tc_ok
 void mp_tc_release(mp_mlp* mlp);
 

@@ -136,11 +136,11 @@ __device__ void dense_layer(const float* __restrict__ wt, const float* __restric
 
 // ---- the steps of a tile, shared by query_fp32_kernel and the forward half of query_grad_kernel ------------------------
 // 1. projection, mask, taps of image b's points; 2. bilinear gather from its map `feat`: sX = [sampled features ;
-// z * z_scale], sMeta[p] = in_img
-template <int P>
+// z * z_scale], sMeta[p] = in_img.  SURF: the points are the vertices of *surf (one map) instead of src's.
+template <int P, bool SURF = false>
 __device__ __forceinline__ void tile_sample(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
                                             int b, const float* feat, long long p0, long long n, float* sX, float* sMeta,
-                                            int (&sOff)[4][P], float (&sWgt)[4][P]) {
+                                            int (&sOff)[4][P], float (&sWgt)[4][P], const MpSurfaceSrc* surf = nullptr) {
   const int tid = threadIdx.x;
   const int warp = tid >> 5, lane = tid & 31;
   if (tid < P) {
@@ -149,7 +149,8 @@ __device__ __forceinline__ void tile_sample(const Fp32Params& prm, const MpPoint
     bool valid = i < n;
     if (valid) {
       float x, y, z;
-      mp_load_point(src, bt, b, i, x, y, z);
+      if constexpr (SURF) mp_surface_point(*surf, i, x, y, z);
+      else mp_load_point(src, bt, b, i, x, y, z);
       mp_project(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
     }
     const bool in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);   // MonoPortNet.py:74
@@ -228,9 +229,12 @@ __device__ __forceinline__ float last_layer_dot(const Fp32Params& prm, const flo
 
 // bt.B images of src.n points (more than one: MP_SRC_ROWS); tile t is tile t % n_tiles of image t / n_tiles, which samples
 // its own map and calibration and writes its own outputs; the range guard is decided per tile from that image's maximum.
-template <int P>
+// SURF (a separate instantiation, so the query instantiations keep their code): the exact twin of the tensor-core program's
+// surface render -- src.n vertices of surf (one map; surf.count, when set, the count on the device), their colours into
+// surf.canvas.
+template <int P, bool SURF>
 __global__ void __launch_bounds__(kThreads, 1)
-query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpBatch bt) {
+query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpBatch bt, MpSurfaceSrc surf) {
   MP_DYN_SMEM_ALIGNED(float, smem, 16);
   float* sX = smem;                                  // [c0][P]
   float* sA = sX + (size_t)prm.c0 * P;               // [h_ping][P]
@@ -243,6 +247,12 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpB
   if (src.count_dev) {
     const long long c = *src.count_dev;
     n = c < n ? c : n;
+  }
+  if constexpr (SURF) {
+    if (surf.count) {
+      const long long c = *surf.count;
+      n = c < n ? c : n;
+    }
   }
   long long win0, win1;
   mp_shard_window(src, n, win0, win1);
@@ -259,7 +269,7 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpB
     const long long p0 = win0 + (at - (long long)b * n_tiles) * P;
     __shared__ int sOff[4][P];
     __shared__ float sWgt[4][P];
-    tile_sample<P>(prm, src, cal, bt, b, prm.feat + (size_t)b * prm.H * prm.W * prm.C, p0, n, sX, sMeta, sOff, sWgt);
+    tile_sample<P, SURF>(prm, src, cal, bt, b, prm.feat + (size_t)b * prm.H * prm.W * prm.C, p0, n, sX, sMeta, sOff, sWgt, &surf);
     const float* sIn = tile_hidden<P, false>(prm, sX, sA, sB);
     const int l = prm.n_layers - 1;
     float* out = dst.out + b * bt.out_stride;
@@ -271,6 +281,10 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpB
         if (i < n) {
           float v = mp_last_op(acc + __ldg(prm.bias[l] + r), prm.last_op);
           v = sMeta[p] * v;                                                              // MonoPortNet.py:89
+          if constexpr (SURF) {
+            mp_surface_store(surf, i, r, v);                                             // RTL/main.py:244-248
+            continue;
+          }
           if (out) out[(long long)r * dst.ld + i] = v;
           if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = v;
           if (r == 0)
@@ -503,9 +517,9 @@ int launch_grad(const Fp32Params& prm, const GradParams& gp, const MpPointSrc& s
   return MP_OK;
 }
 
-template <int P>
+template <int P, bool SURF = false>
 int launch(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst, cudaStream_t st,
-           int sm_count, int max_smem, const MpBatch& bt) {
+           int sm_count, int max_smem, const MpBatch& bt, const MpSurfaceSrc& surf = MpSurfaceSrc()) {
   const size_t smem = Fp32Smem<P>::bytes(prm.c0, prm.h_ping, prm.h_pong);
   // The opt-in is a property of the kernel, shared by every thread, and heads of different widths launch the same
   // instantiation with different sizes: it is always set to the same bound -- the device's maximum less the 2 KB the size
@@ -516,16 +530,16 @@ int launch(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, con
   int dev_ = 0;
   MP_CUDA(cudaGetDevice(&dev_));
   if (dev_ < 0 || dev_ >= 64 || !opted[dev_]) {
-    MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
+    MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P, SURF>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
     if (dev_ >= 0 && dev_ < 64) opted[dev_] = true;
   }
   long long tiles = bt.B * ((src.n + P - 1) / P);
   int grid = (int)(tiles < (long long)sm_count ? (tiles > 0 ? tiles : 1) : sm_count);
 #ifndef MP_CUDA_EMU
-  query_fp32_kernel<P><<<grid, kThreads, smem, st>>>(prm, src, cal, dst, bt);
+  query_fp32_kernel<P, SURF><<<grid, kThreads, smem, st>>>(prm, src, cal, dst, bt, surf);
 #else
   // tests/emu: CPU model of the execution model
-  MP_EMU_LAUNCH(grid, kThreads, query_fp32_kernel<P>(prm, src, cal, dst, bt));
+  MP_EMU_LAUNCH(grid, kThreads, (query_fp32_kernel<P, SURF>(prm, src, cal, dst, bt, surf)));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -595,6 +609,33 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
   if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32>(prm, src, cal, dst, st, sms, max_smem, b);
   if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16>(prm, src, cal, dst, st, sms, max_smem, b);
   if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8>(prm, src, cal, dst, st, sms, max_smem, b);
+  mp_set_error("head too wide for the fp32 kernel's shared-memory tiling");
+  return MP_E_UNSUPPORTED;
+}
+
+int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
+                           cudaStream_t st, int guard) {
+  if (n <= 0) return MP_OK;
+  if (mlp->cout[mlp->n_layers - 1] != 3) {
+    mp_set_error("surface colourisation needs a head with 3 outputs (got %d)", mlp->cout[mlp->n_layers - 1]);
+    return MP_E_INVALID;
+  }
+  Fp32Params prm;
+  int sms = 0, max_smem = 0;
+  const int rc = fill_params(mlp, feat, prm, sms, max_smem);
+  if (rc != MP_OK) return rc;
+  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
+  MpPointSrc src;
+  memset(&src, 0, sizeof(src));
+  src.kind = MP_SRC_ROWS;
+  src.n = n;
+  MpOutDst dst;
+  dst.out = nullptr; dst.ld = 0; dst.scatter_vol = nullptr;
+  const MpBatch one;
+  const int ping = prm.h_ping, pong = prm.h_pong;
+  if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32, true>(prm, src, cal, dst, st, sms, max_smem, one, surf);
+  if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16, true>(prm, src, cal, dst, st, sms, max_smem, one, surf);
+  if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8, true>(prm, src, cal, dst, st, sms, max_smem, one, surf);
   mp_set_error("head too wide for the fp32 kernel's shared-memory tiling");
   return MP_E_UNSUPPORTED;
 }

@@ -112,19 +112,7 @@ struct TcParams {
   int guard;
 };
 
-// Direct rendering of the visible surface (RTL/main.py:212-249) fused into the colour query: point i is the vertex
-// (X[i], Y[i], R - Z[i]) of forward_vertices mapped to world space by mat_color (RTL/main.py:201-210: diag((b_max-b_min)/R),
-// translation b_min), and its colour pred * 0.5 + 0.5 (:244) is scattered to canvas[X[i], Y[i], :] (:247-248) -- no
-// intermediate point / prediction tensors.  X == nullptr: the ordinary point sources and the [R,N] output.
-struct MpSurfaceSrc {
-  const long long* X;
-  const long long* Y;
-  const float* Z;
-  float scale[3], bmin[3];      // (b_max - b_min) / R and b_min, fp32 like torch's
-  float R;
-  float* canvas;                // [R, R, 3]
-  int canvas_R;
-};
+// Direct rendering of the visible surface (RTL/main.py:212-249) is fused into the colour query: MpSurfaceSrc (mp_common.cuh).
 
 // --------------------------------------------------------------------------------------------------------------------
 // sampling helpers
@@ -146,10 +134,7 @@ __device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const 
   if (valid) {
     float x, y, z;
     if (surf.X) {
-      const float vx = (float)__ldg(surf.X + i), vy = (float)__ldg(surf.Y + i), vz = __fsub_rn(surf.R, __ldg(surf.Z + i));
-      x = __fadd_rn(__fmul_rn(vx, surf.scale[0]), surf.bmin[0]);
-      y = __fadd_rn(__fmul_rn(vy, surf.scale[1]), surf.bmin[1]);
-      z = __fadd_rn(__fmul_rn(vz, surf.scale[2]), surf.bmin[2]);
+      mp_surface_point(surf, i, x, y, z);
     } else {
       mp_load_point(src, bt, b, i, x, y, z);
     }
@@ -261,6 +246,10 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   long long n = src.n;
   if (src.count_dev) {
     const long long c = __shfl_sync(0xffffffffu, *src.count_dev, 0);
+    n = c < n ? c : n;
+  }
+  if (surf.count) {                                  // (the vertex count of a captured frame step, read the same way)
+    const long long c = __shfl_sync(0xffffffffu, *surf.count, 0);
     n = c < n ? c : n;
   }
   long long win0, win1;
@@ -609,8 +598,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
             const float logit = s_s4[r * kTile + row] + (lg_mine(r) + s_part[r * kTile + row]);
             const float val = inimg * mp_last_op(logit, prm.last_op);
             if (surf.canvas) {
-              float* px = surf.canvas + ((size_t)__ldg(surf.X + i) * surf.canvas_R + (size_t)__ldg(surf.Y + i)) * 3;
-              px[r] = __fadd_rn(__fmul_rn(val, 0.5f), 0.5f);      // RTL/main.py:244
+              mp_surface_store(surf, i, r, val);                   // RTL/main.py:244
               continue;
             }
             if (dst.out) dst.out[mp_tile_image(bt, t, n_tiles) * bt.out_stride + (long long)r * dst.ld + i] = val;
@@ -932,9 +920,10 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
     feat->g0_owner = mlp->gen;
     feat->g0_version = feat->version;
   }
-  if (surf.X && isfinite(mlp->tc_amax_limit)) {
-    // the fused rendering has no exact-kernel twin: check the frame's feature range on the host (one 4-byte read-back per
-    // frame) and let the caller take the unfused path when it is outside the validated range
+  if (surf.X && guard == MP_GUARD_NONE && isfinite(mlp->tc_amax_limit)) {
+    // the eager rendering (mp_colorize_surface): check the frame's feature range on the host (one 4-byte read-back per
+    // frame) and let the caller take the unfused path when it is outside the validated range.  (The enqueue-only render,
+    // mp_colorize_surface_async, passes MP_GUARD_IN_RANGE instead and launches the exact twin beside this one.)
     unsigned bits = 0;
     MP_CUDA(cudaMemcpyAsync(&bits, feat->amax, sizeof(bits), cudaMemcpyDeviceToHost, st));
     MP_CUDA(cudaStreamSynchronize(st));
@@ -1008,8 +997,8 @@ void mp_tc_release(mp_mlp* mlp) {
   mlp->tc_ok = 0;
 }
 
-int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* X, const long long* Y, const float* Z, long long n,
-                             int R, const float* b_min3, const float* b_max3, const MpCalib& cal, float* canvas, cudaStream_t st) {
+int mp_launch_surface_tc(const mp_mlp* mlp, mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
+                         cudaStream_t st, int guard) {
   if (n <= 0) return MP_OK;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
   if (!pk || !mlp->tc_ok || pk->kind != 1) {
@@ -1020,23 +1009,19 @@ int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* 
     mp_set_error("colour head: needs a 512-channel map of at most 65536 texels (got %d channels, %d x %d)", feat->C, feat->H, feat->W);
     return MP_E_INVALID;
   }
-  MpSurfaceSrc surf;
-  memset(&surf, 0, sizeof(surf));
-  surf.X = X; surf.Y = Y; surf.Z = Z;
-  for (int a = 0; a < 3; ++a) {
-    surf.scale[a] = (b_max3[a] - b_min3[a]) / (float)R;          // mat[a,a] = length / resolution  (RTL/main.py:207)
-    surf.bmin[a] = b_min3[a];
-  }
-  surf.R = (float)R;
-  surf.canvas = canvas;
-  surf.canvas_R = R;
   MpPointSrc src;
   memset(&src, 0, sizeof(src));
   src.kind = MP_SRC_ROWS;
   src.n = n;
   MpOutDst dst;
   dst.out = nullptr; dst.ld = 0; dst.scatter_vol = nullptr;
-  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, MP_GUARD_NONE, MpBatch());
+  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, MpBatch());
+}
+
+int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* X, const long long* Y, const float* Z, long long n,
+                             int R, const float* b_min3, const float* b_max3, const MpCalib& cal, float* canvas, cudaStream_t st) {
+  if (n <= 0) return MP_OK;
+  return mp_launch_surface_tc(mlp, feat, mp_surface_src(X, Y, Z, nullptr, R, b_min3, b_max3, canvas), n, cal, st, MP_GUARD_NONE);
 }
 
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,

@@ -43,6 +43,20 @@ extern "C" int mp_forward_vertices_async(const float* vol_dev, int R, int direct
   return MP_OK;
 }
 
+// The normal image of the demo, enqueue-only (graph-capturable): the count is read on the device.
+extern "C" int mp_render_normals_async(const int64_t* x_dev, const int64_t* y_dev, const float* norm_dev, const int64_t* count_dev,
+                                       int64_t capacity, int R, float* canvas_dev, void* stream) {
+  MP_REQUIRE(x_dev && y_dev && norm_dev && count_dev && canvas_dev, "NULL argument");
+  MP_REQUIRE(capacity >= 0 && R >= 1 && capacity <= (int64_t)R * R, "bad sizes capacity=%lld R=%d", (long long)capacity, R);
+  if (capacity == 0) return MP_OK;
+  const long long blocks = (capacity + kNormThreads - 1) / kNormThreads;
+  const int grid = (int)(blocks < 1024 ? blocks : 1024);
+  render_normals_kernel<<<grid, kNormThreads, 0, (cudaStream_t)stream>>>(
+      (const long long*)x_dev, (const long long*)y_dev, norm_dev, (const long long*)count_dev, capacity, R, canvas_dev);
+  MP_CUDA(cudaGetLastError());
+  return MP_OK;
+}
+
 extern "C" int mp_forward_vertices(const float* vol_dev, int R, int direction, int64_t* x_dev, int64_t* y_dev,
                                    float* z_dev, float* norm_dev, int64_t* n_out, void* stream) {
   MP_REQUIRE(vol_dev && x_dev && y_dev && z_dev && norm_dev && n_out, "NULL argument");

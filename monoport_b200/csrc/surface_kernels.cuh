@@ -96,4 +96,25 @@ struct HitEmit {
   }
 };
 
+// The normal image of the demo (RTL/main.py:212-228): canvas[X[i], Y[i], :] = clamp((norm[i] + 1) / 2, 0, 1) for the
+// min(*count, cap) vertices of forward_vertices.  The bits are torch's: one rounding for the sum, the halving is exact, and
+// the clamp lets NaN through (the normals of a column whose finite differences vanish are NaN) -- no fminf / fmaxf.
+constexpr int kNormThreads = 256;
+__global__ void __launch_bounds__(kNormThreads)
+render_normals_kernel(const long long* __restrict__ X, const long long* __restrict__ Y, const float* __restrict__ norm,
+                      const long long* __restrict__ count, long long cap, int R, float* __restrict__ canvas) {
+  long long n = *count;
+  if (n > cap) n = cap;
+  const long long step = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += step) {
+    float* px = canvas + ((size_t)X[i] * R + (size_t)Y[i]) * 3;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      float v = __fmul_rn(__fadd_rn(norm[3 * i + a], 1.f), 0.5f);
+      v = v < 0.f ? 0.f : (v > 1.f ? 1.f : v);
+      px[a] = v;
+    }
+  }
+}
+
 }  // namespace surface_k

@@ -60,9 +60,20 @@ class FrameGraph:
     counts on the host and cannot be captured).  calib: [1,4,4] tensor (read once, at construction).
     `feature_hook(feat) -> feat` (optional) runs inside the captured step on the encoder's last-stage map.
     launch(x) enqueues a frame (x = image [1,3,H,W] with an encoder, else the [1,C,h,w] feature map); result() waits for it
-    and returns (sdf or None, X, Y, Z, norm) exactly like engine(...) followed by forward_vertices(sdf, direction)."""
+    and returns (sdf or None, X, Y, Z, norm) exactly like engine(...) followed by forward_vertices(sdf, direction).
 
-    def __init__(self, net, engine, calib, direction="front", with_encoder=True, input_shape=None, feature_hook=None):
+    The demo's two images (RTL/main.py:417-441) can be rendered inside the same captured step:
+      netC: the colour net.  Its map is netC.filter(x_colour, feat_prior=<the geometry map the engine receives>) with the
+        encoder (MonoPortNet.py:41-45, RTL/main.py:373-379), else x_colour itself ([1,C,h,w]); netC is queried at the
+        visible vertices into an [R,R,3] canvas like colorization(netC, ...) -- mp_colorize_surface_async: the vertex count
+        stays on the device and the range guard of the tensor-core colour program is decided there (a frame outside it
+        is rendered by the exact fp32 kernel, like netC.query would evaluate it);
+      render_normals: the normal image, like colorization(norm=N) (mp_render_normals_async);
+      canvas: the background of both images ([R,R,3], default ones).
+    launch(x, x_colour) then takes the netC input too, and rendered() (after result()) returns (render_norm, render_tex)."""
+
+    def __init__(self, net, engine, calib, direction="front", with_encoder=True, input_shape=None, feature_hook=None,
+                 netC=None, render_normals=False, canvas=None):
         from .modeling.MonoPortNet import FeatureHandle
         from .modeling.geometry import perspective
         from .recon import _DIRS
@@ -80,10 +91,30 @@ class FrameGraph:
         self._cal12 = _lib.calib12(calib.detach().cpu())
         if input_shape is None:
             input_shape = (1, 3, 512, 512) if with_encoder else (1, net.surface_classifier.filter_channels[0] - 1, 128, 128)
+        self.netC = netC
+        self.render_normals = bool(render_normals)
         lib = self._lib = _lib.load()
         with torch.cuda.device(dev):
             self.stream = torch.cuda.Stream(dev)
             self.static_in = torch.zeros(input_shape, dtype=torch.float32, device=dev)
+            self.render_tex = self.render_norm = None
+            if netC is not None or self.render_normals:
+                bg = torch.ones((R, R, 3), dtype=torch.float32) if canvas is None else canvas.detach()
+                if tuple(bg.shape) != (R, R, 3):
+                    raise ValueError("canvas must be [%d,%d,3] (the engine's resolution); got %s" % (R, R, tuple(bg.shape)))
+                self._bg = bg.to(device=dev, dtype=torch.float32).contiguous()
+                self.render_norm = torch.empty_like(self._bg) if self.render_normals else None
+            if netC is not None:
+                if with_encoder:                    # the netC image, the same size as the geometry net's
+                    colour_shape = input_shape
+                else:                               # netC's own map, at the geometry map's size
+                    colour_shape = (1, netC.surface_classifier.filter_channels[0] - 1) + tuple(input_shape[2:])
+                self.static_in_c = torch.zeros(colour_shape, dtype=torch.float32, device=dev)
+                self.render_tex = torch.empty_like(self._bg)
+                self._fhc = None
+                self._headC = netC.surface_classifier.handle()
+                self._projC = _lib.PROJ_PERSPECTIVE if netC.projection is perspective else _lib.PROJ_ORTHOGONAL
+                self._bmin3, self._bmax3 = _lib.f3(engine.b_min), _lib.f3(engine.b_max)
             self.volume = torch.empty((1, 1, R, R, R), dtype=torch.float32, device=dev)
             cap = R * R
             self.X = torch.empty(cap, dtype=torch.int64, device=dev)
@@ -106,6 +137,7 @@ class FrameGraph:
             with torch.cuda.graph(self.graph, stream=self.stream), torch.no_grad():
                 self._step()
         self.last_stats = None
+        self._nonempty = None
 
     def _step(self):
         lib, dev = self._lib, self.device
@@ -128,13 +160,40 @@ class FrameGraph:
             ctypes.c_void_p(self.volume.data_ptr()), self.R, self._dir, ctypes.c_void_p(self.X.data_ptr()),
             ctypes.c_void_p(self.Y.data_ptr()), ctypes.c_void_p(self.Z.data_ptr()), ctypes.c_void_p(self.N.data_ptr()),
             ctypes.c_void_p(self.count.data_ptr()), ctypes.c_void_p(self._scratch.data_ptr()), st), "mp_forward_vertices_async")
+        cap = self.X.numel()
+        if self.render_normals:
+            self.render_norm.copy_(self._bg)
+            _lib.check(lib.mp_render_normals_async(
+                ctypes.c_void_p(self.X.data_ptr()), ctypes.c_void_p(self.Y.data_ptr()), ctypes.c_void_p(self.N.data_ptr()),
+                ctypes.c_void_p(self.count.data_ptr()), cap, self.R, ctypes.c_void_p(self.render_norm.data_ptr()), st),
+                "mp_render_normals_async")
+        if self.netC is not None:
+            # netC's map: its encoder with the geometry map the engine received as the prior, or the map as given
+            featc = self.netC.filter(self.static_in_c, feat_prior=feat)[-1][0] if self.with_encoder else self.static_in_c
+            if self._fhc is None:
+                _, C, H, W = featc.shape
+                self._fhc = self._FeatureHandle(C, H, W, dev)
+            self._fhc.key = None
+            self._fhc.upload(featc)
+            self.render_tex.copy_(self._bg)
+            _lib.check(lib.mp_colorize_surface_async(
+                self._headC, self._fhc.ptr, ctypes.c_void_p(self.X.data_ptr()), ctypes.c_void_p(self.Y.data_ptr()),
+                ctypes.c_void_p(self.Z.data_ptr()), ctypes.c_void_p(self.count.data_ptr()), cap, self.R, self._bmin3,
+                self._bmax3, self._cal12, self._projC, ctypes.c_float(self.netC.normalizer.scale), self.netC._mode(),
+                ctypes.c_void_p(self.render_tex.data_ptr()), st), "mp_colorize_surface_async")
 
-    def launch(self, x):
-        """Enqueue one frame (returns at once)."""
+    def launch(self, x, x_colour=None):
+        """Enqueue one frame (returns at once).  x_colour: netC's input (its image with the encoder, else its map), required
+        exactly when the graph was built with netC."""
+        if (x_colour is None) != (self.netC is None):
+            raise ValueError("x_colour is required exactly when the FrameGraph renders with netC")
         self.stream.wait_stream(torch.cuda.current_stream(self.device))     # x may still be produced on the caller's stream
         with torch.cuda.stream(self.stream):
             self.static_in.copy_(x, non_blocking=True)
+            if x_colour is not None:
+                self.static_in_c.copy_(x_colour, non_blocking=True)
             self.graph.replay()
+        self._nonempty = None
         return self
 
     def result(self):
@@ -146,10 +205,21 @@ class FrameGraph:
             _lib.check(self._lib.mp_octree_fetch(self._oct, ctypes.byref(nonempty), stats, _lib.stream_ptr(self.device)),
                        "mp_octree_fetch")                                    # (synchronises the graph's stream)
         self.last_stats = list(stats)
+        self._nonempty = bool(nonempty.value)
         if not nonempty.value:
             return None, None, None, None, None
         k = int(self.count.item())
         return self.volume, self.X[:k], self.Y[:k], self.Z[:k], self.N[:k]
+
+    def rendered(self):
+        """After result(): (render_norm, render_tex), the [R,R,3] images of the frame -- views of this graph's buffers, valid
+        until its next launch.  An image the graph was not built to render is None; both are None for an empty frame (like
+        colorization(X=None))."""
+        if self._nonempty is None:
+            raise RuntimeError("FrameGraph.rendered() needs the frame's result() first")
+        if not self._nonempty:
+            return None, None
+        return self.render_norm, self.render_tex
 
     def close(self):
         if self._oct is not None:
@@ -166,20 +236,28 @@ class FrameGraph:
 
 class FrameGraphRing:
     """`n_lanes` FrameGraphs used round-robin: up to n_lanes frames in flight, results in input order (the graph-captured
-    counterpart of FramePipeline for the stages of this library)."""
+    counterpart of FramePipeline for the stages of this library).  Lanes built with netC take (x, x_colour) items and yield
+    result() + rendered(): (sdf, X, Y, Z, norm, render_norm, render_tex)."""
 
     def __init__(self, make_graph, n_lanes=2):
         self.lanes = [make_graph() for _ in range(int(n_lanes))]
+
+    @staticmethod
+    def _out(lane):
+        out = lane.result()
+        if lane.netC is not None or lane.render_normals:
+            out = out + lane.rendered()
+        return out
 
     def run(self, iterable):
         inflight = deque()
         for i, x in enumerate(iterable):
             lane = self.lanes[i % len(self.lanes)]
             if len(inflight) >= len(self.lanes):
-                yield inflight.popleft().result()
-            inflight.append(lane.launch(x))
+                yield self._out(inflight.popleft())
+            inflight.append(lane.launch(*x) if lane.netC is not None else lane.launch(x))
         while inflight:
-            yield inflight.popleft().result()
+            yield self._out(inflight.popleft())
 
     def close(self):
         for lane in self.lanes:

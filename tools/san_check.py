@@ -1,5 +1,6 @@
 """Tiny invocation of every kernel family for compute-sanitizer (memcheck): both tensor-core programs, the fp32 kernel and
-its point-gradient kernel, the octree engine, marching cubes and the visible-surface kernel."""
+its point-gradient kernel, the octree engine, marching cubes, the visible-surface kernel and the enqueue-only renders of
+captured frames (mp_colorize_surface_async on both programs, mp_render_normals_async)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -36,6 +37,27 @@ cW, cb = spec.make_weights(spec.C_CHANNELS, 5)
 netC = build_net("C", cW, cb)
 featC = spec.make_feat(512, 128, 128, 6, 0.5).cuda()
 img = colorization(netC, [[featC]], X, Y, Z, cal, resolution=33)
+# the enqueue-only renders of captured frames: counts on the device (capacity R*R, the tail past the count unread), the
+# colour render in range (tensor cores) and out of range (the exact twin)
+import ctypes
+from monoport_b200 import _lib
+lib = _lib.load()
+k = X.numel()
+Xb, Yb = torch.zeros(33 * 33, dtype=torch.int64, device="cuda"), torch.zeros(33 * 33, dtype=torch.int64, device="cuda")
+Zb, Nb = torch.zeros(33 * 33, device="cuda"), torch.zeros(33 * 33, 3, device="cuda")
+Xb[:k], Yb[:k], Zb[:k], Nb[:k] = X, Y, Z, n
+cnt = torch.tensor([k], dtype=torch.int64, device="cuda")
+canv = torch.ones(33, 33, 3, device="cuda")
+P = lambda t: ctypes.c_void_p(t.data_ptr())
+_lib.check(lib.mp_render_normals_async(P(Xb), P(Yb), P(Nb), P(cnt), 33 * 33, 33, P(canv), _lib.stream_ptr()), "normals")
+for fc in (featC, featC * 60.0):
+    fh = netC.feature_handle(fc)
+    _lib.check(lib.mp_colorize_surface_async(netC.surface_classifier.handle(), fh.ptr, P(Xb), P(Yb), P(Zb), P(cnt), 33 * 33, 33,
+                                             _lib.f3([-1, -1, -1]), _lib.f3([1, 1, 1]), _lib.calib12(cal), 0,
+                                             ctypes.c_float(netC.normalizer.scale), _lib.MODE_AUTO, P(canv), _lib.stream_ptr()),
+               "colour async")
+    torch.cuda.synchronize()
+print("async renders", float(canv.sum()))
 big = net.query([[feat.cuda() * 60.0]], pts, calibs=cal)[0]
 # batched queries (one launch over B images) in every mode; image 1 is outside the range guard's limit, so the guarded
 # modes split the launch per image between the tensor-core and the exact kernel
