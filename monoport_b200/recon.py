@@ -189,8 +189,10 @@ def colorization(netC, feat_tensor_C, X, Y, Z, calib_tensor, norm=None, resoluti
     from .modeling.geometry import perspective
     head = netC.surface_classifier
     feat = feat_tensor_C[-1][0]
+    # the tensor-core program covers maps of at most 65536 texels: a larger map takes the generic route, whose query() runs
+    # the exact kernel in "auto" and refuses in "tc"
     if (netC.precision in ("auto", "tc") and not netC.training and X.is_cuda and feat.is_cuda and feat.device == device
-            and head.filter_channels[-1] == 3 and head.tc_supported()):
+            and head.filter_channels[-1] == 3 and head.tc_supported() and feat.shape[-2] * feat.shape[-1] <= 65536):
         # one launch: vertices -> world (mat_color) -> netC -> pred*0.5+0.5 -> canvas  (tensor-core program of the colour head)
         n = int(X.numel())
         rc = _lib.MP_OK
