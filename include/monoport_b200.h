@@ -132,6 +132,20 @@ int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* po
 int mp_query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
                          int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
                          int64_t ld_grad, float* out_dev, int64_t ld_out, float* dpoints_dev, int64_t ld_dpoints, void* stream);
+/* mp_query_points_grad with a precision mode and an optional point count on the device (count_dev: one int32, or NULL;
+ * n is then the capacity and the points at or beyond min(*count_dev, n) are not touched).  Enqueue-only: nothing is read
+ * back to the host, so the call can be captured in a CUDA graph.
+ *   MP_MODE_FP32: the exact kernel, bit for bit mp_query_points_grad.
+ *   MP_MODE_TC:   the tensor-core program's forward-mode derivative (three tangents per point carried as extra rows of the
+ *                 wgmma program); its value is mp_query_points' MP_MODE_TC value bit for bit.  A frame whose largest
+ *                 |feature| is above the head's limit is differentiated by the exact kernel instead, decided on the device
+ *                 (as mp_query_points decides it).  Maps above 65536 texels are refused.
+ *   MP_MODE_AUTO: MP_MODE_TC where the head and the map allow it, else MP_MODE_FP32.
+ * Single-map handles only. */
+int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                              int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
+                              int64_t ld_grad, float* out_dev, int64_t ld_out, float* dpoints_dev, int64_t ld_dpoints,
+                              const int32_t* count_dev, int mode, void* stream);
 /* Same call with HOST buffers (points [3,N], out [Res,N], feature map NCHW fp32 or NULL to reuse the
  * uploaded one): copies in, runs, copies out, synchronises.  This is what bench.py's e2e leg times. */
 int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,
@@ -281,6 +295,16 @@ int mp_colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_d
  * normals stay NaN).  Enqueue-only like the call above; capacity <= R*R. */
 int mp_render_normals_async(const int64_t* x_dev, const int64_t* y_dev, const float* norm_dev, const int64_t* count_dev,
                             int64_t capacity, int R, float* canvas_dev, void* stream);
+/* Analytic normals of the visible surface, enqueue-only (graph-capturable): for the first min(*count_dev, capacity) vertices
+ * (X, Y, Z) of mp_forward_vertices_async (int64 count on the device), the geometry head's gradient at the world point
+ * (X, Y, R - Z) through mat_color (the points mp_colorize_surface_async renders) -> norm_dev[i] = -(g_x L_x, g_y L_y,
+ * -g_z L_z) / R normalised (L = b_max - b_min), zero where the gradient vanishes: forward_vertices' frame and sign.
+ * mode: as mp_query_points_grad_mode.  scratch_dev: 6 * capacity + 1 floats of device memory.  Heads with one output,
+ * single-map handles; capacity <= R*R.  norm_dev can then be drawn with mp_render_normals_async. */
+int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev, const float* z_dev,
+                             const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
+                             const float* calib12, int projection, float z_scale, int mode, float* scratch_dev, float* norm_dev,
+                             void* stream);
 
 #ifdef __cplusplus
 }

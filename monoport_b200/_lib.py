@@ -46,6 +46,8 @@ SIGNATURES = {
                                 c_void_p, c_int64, c_int, c_void_p]),
     "mp_query_points_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
                                      c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
+    "mp_query_points_grad_mode": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
+                                          c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int, c_void_p]),
     "mp_query_points_host": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, P(c_float), c_int, c_float,
                                      c_void_p, c_int, c_void_p]),
     "mp_query_grid": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, P(c_float), P(c_float), P(c_float), c_int,
@@ -83,6 +85,8 @@ SIGNATURES = {
     "mp_colorize_surface_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, P(c_float),
                                           P(c_float), P(c_float), c_int, c_float, c_int, c_void_p, c_void_p]),
     "mp_render_normals_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
+    "mp_surface_normals_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, P(c_float),
+                                         P(c_float), P(c_float), c_int, c_float, c_int, c_void_p, c_void_p, c_void_p]),
     "mp_forward_vertices":(c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, P(c_int64),
                                     c_void_p]),
     "mp_forward_vertices_scratch_bytes": (c_int64, [c_int]),

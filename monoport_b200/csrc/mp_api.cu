@@ -345,13 +345,14 @@ extern "C" int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, cons
                       out_dev, out_batch_stride, ld_out, mode, stream, true);
 }
 
-extern "C" int mp_query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
-                                    int64_t point_stride, const float* calib12, int projection, float z_scale,
-                                    const float* grad_out_dev, int64_t ld_grad, float* out_dev, int64_t ld_out,
-                                    float* dpoints_dev, int64_t ld_dpoints, void* stream) {
+// mp_query_points_grad and mp_query_points_grad_mode
+static int query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                             int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
+                             int64_t ld_grad, float* out_dev, int64_t ld_out, float* dpoints_dev, int64_t ld_dpoints,
+                             const int32_t* count_dev, int mode, void* stream, const char* what) {
   MpRange nvtx("monoport_b200: F1'' query gradient");
   MP_REQUIRE(mlp && feat, "NULL handle");
-  MP_REQUIRE_SINGLE_MAP(feat, "mp_query_points_grad");
+  MP_REQUIRE_SINGLE_MAP(feat, what);
   MP_REQUIRE(n >= 0 && row_stride >= 1 && point_stride >= 1 && ld_dpoints >= n && (!out_dev || ld_out >= n) &&
                  (!grad_out_dev || ld_grad >= n),
              "bad sizes n=%lld strides=%lld,%lld ld_grad=%lld ld_out=%lld ld_dpoints=%lld", (long long)n, (long long)row_stride,
@@ -364,10 +365,108 @@ extern "C" int mp_query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float*
   src.px = points_dev; src.py = points_dev + row_stride; src.pz = points_dev + 2 * row_stride;
   src.pstride = point_stride;
   src.n = n;
+  src.count_dev = count_dev;
   MpCalib cal;
   mp_fill_calib(cal, calib12, projection, z_scale);
-  return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints,
-                              (cudaStream_t)stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  // the rule of mp_query_dispatch: the tensor-core program covers maps of at most 65536 texels, and a frame above the head's
+  // feature limit is taken by the exact kernel, decided on the device
+  const bool tc_can = mlp->tc_ok && (long long)feat->H * feat->W <= 65536;
+  if (mode == MP_MODE_AUTO) mode = tc_can ? MP_MODE_TC : MP_MODE_FP32;
+  if (mode == MP_MODE_TC || mode == MP_MODE_TC_V3) {
+    if (!mlp->tc_ok) {
+      mp_set_error("MP_MODE_TC requested but the tensor-core kernel does not support this head/device");
+      return MP_E_UNSUPPORTED;
+    }
+    const bool guarded = isfinite(mlp->tc_amax_limit);
+    int rc = mp_launch_query_jvp_tc(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st,
+                                    guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE);
+    if (rc != MP_OK || !guarded) return rc;
+    return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st,
+                                MP_GUARD_OUT_OF_RANGE);
+  }
+  MP_REQUIRE(mode == MP_MODE_FP32, "bad mode %d", mode);
+  return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st);
+}
+
+extern "C" int mp_query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                                    int64_t point_stride, const float* calib12, int projection, float z_scale,
+                                    const float* grad_out_dev, int64_t ld_grad, float* out_dev, int64_t ld_out,
+                                    float* dpoints_dev, int64_t ld_dpoints, void* stream) {
+  return query_points_grad(mlp, feat, points_dev, n, row_stride, point_stride, calib12, projection, z_scale, grad_out_dev, ld_grad,
+                           out_dev, ld_out, dpoints_dev, ld_dpoints, nullptr, MP_MODE_FP32, stream, "mp_query_points_grad");
+}
+
+extern "C" int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                                         int64_t point_stride, const float* calib12, int projection, float z_scale,
+                                         const float* grad_out_dev, int64_t ld_grad, float* out_dev, int64_t ld_out,
+                                         float* dpoints_dev, int64_t ld_dpoints, const int32_t* count_dev, int mode, void* stream) {
+  return query_points_grad(mlp, feat, points_dev, n, row_stride, point_stride, calib12, projection, z_scale, grad_out_dev, ld_grad,
+                           out_dev, ld_out, dpoints_dev, ld_dpoints, count_dev, mode, stream, "mp_query_points_grad_mode");
+}
+
+// ---------------------------------------------------------------------------------------------
+// analytic normals of the visible surface, enqueue-only (mp_surface_normals_async)
+// ---------------------------------------------------------------------------------------------
+// step 1: vertex i -> its world point (mp_surface_point's two roundings) in rows [3][cap]; the count, clamped to the
+// capacity, as the int32 point count of the gradient launches
+__global__ void normals_points_kernel(MpSurfaceSrc s, long long cap, float* __restrict__ pts, int32_t* __restrict__ count32) {
+  long long n = *s.count;
+  n = n < 0 ? 0 : (n > cap ? cap : n);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *count32 = (int32_t)n;
+  const long long step = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += step) {
+    float x, y, z;
+    mp_surface_point(s, i, x, y, z);
+    pts[i] = x;
+    pts[cap + i] = y;
+    pts[2 * cap + i] = z;
+  }
+}
+
+// step 3: the world gradient g [3][cap] -> -(g_x a_x, g_y a_y, g_z a_z) normalised into norm [cap][3], zero where g vanishes
+__global__ void normals_finish_kernel(const float* __restrict__ g, const long long* __restrict__ count, long long cap, float ax,
+                                      float ay, float az, float* __restrict__ norm) {
+  long long n = *count;
+  n = n < 0 ? 0 : (n > cap ? cap : n);
+  const long long step = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += step) {
+    const float v[3] = {-(g[i] * ax), -(g[cap + i] * ay), -(g[2 * cap + i] * az)};
+    const float len = sqrtf(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) norm[3 * i + a] = len > 0.f ? v[a] / len : 0.f;
+  }
+}
+
+extern "C" int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev,
+                                        const float* z_dev, const int64_t* count_dev, int64_t capacity, int R,
+                                        const float* b_min3, const float* b_max3, const float* calib12, int projection,
+                                        float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
+  MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE_SINGLE_MAP(feat, "mp_surface_normals_async");
+  MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "surface normals need a head with one output (got %d)", mlp->cout[mlp->n_layers - 1]);
+  MP_REQUIRE(capacity >= 0 && R >= 1 && capacity <= (int64_t)R * R, "bad sizes capacity=%lld R=%d", (long long)capacity, R);
+  MP_REQUIRE(x_dev && y_dev && z_dev && count_dev && b_min3 && b_max3 && scratch_dev && norm_dev, "NULL argument");
+  if (capacity == 0) return MP_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const MpSurfaceSrc surf = mp_surface_src(reinterpret_cast<const long long*>(x_dev), reinterpret_cast<const long long*>(y_dev), z_dev,
+                                           reinterpret_cast<const long long*>(count_dev), R, b_min3, b_max3, nullptr);
+  float* pts = scratch_dev;
+  float* grad = scratch_dev + 3 * capacity;
+  int32_t* count32 = reinterpret_cast<int32_t*>(scratch_dev + 6 * capacity);
+  const long long blocks = (capacity + 255) / 256;
+  const int grid = (int)(blocks < 1024 ? blocks : 1024);
+  normals_points_kernel<<<grid, 256, 0, st>>>(surf, capacity, pts, count32);
+  MP_CUDA(cudaGetLastError());
+  const int rc = query_points_grad(mlp, feat, pts, capacity, capacity, 1, calib12, projection, z_scale, nullptr, 0, nullptr, 0, grad,
+                                   capacity, count32, mode, stream, "mp_surface_normals_async");
+  if (rc != MP_OK) return rc;
+  // forward_vertices' frame: its (X, Y, Z) index axes are the world axes scaled by R / (b_max - b_min), Z reversed
+  float a[3];
+  for (int k = 0; k < 3; ++k) a[k] = (b_max3[k] - b_min3[k]) / (float)R;
+  normals_finish_kernel<<<grid, 256, 0, st>>>(grad, reinterpret_cast<const long long*>(count_dev), capacity, a[0], a[1], -a[2], norm_dev);
+  MP_CUDA(cudaGetLastError());
+  return MP_OK;
 }
 
 extern "C" int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,

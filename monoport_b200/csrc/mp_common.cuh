@@ -367,10 +367,16 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
                        const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
 // gradient of the fp32 query with respect to the points (query_fp32.cu): value -> out[r*ld_out+i] (out may be null; written
 // by a query_fp32_kernel launch, so it is that kernel's value bit for bit),
-// d(sum_r grad_out[r*ld_grad+i] * value_r)/d point_i -> dpoints[a*ld_dp+i] (grad_out null = ones); MP_SRC_ROWS, one map
+// d(sum_r grad_out[r*ld_grad+i] * value_r)/d point_i -> dpoints[a*ld_dp+i] (grad_out null = ones); MP_SRC_ROWS, one map.
+// src.count_dev (when set) is the point count on the device; `guard` as for the query launchers.
 int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
-                         long long ld_dp, cudaStream_t st);
+                         long long ld_dp, cudaStream_t st, int guard = MP_GUARD_NONE);
+// the same outputs from the tensor-core program's forward-mode derivative (query_tc.cu: query_jvp_kernel), whose value is
+// the tensor-core query's bit for bit; the shipped heads, MP_SRC_ROWS, one map of at most 65536 texels
+int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
+                           long long ld_grad, float* out, long long ld_out, float* dpoints, long long ld_dp, cudaStream_t st,
+                           int guard);
 // device-side predicate shared by the kernels: true = the tiles of this image (amax = its entry) must do nothing.  In the
 // tensor-core program the weight producer and the consumers both take it, per tile, from the same word.
 __device__ __forceinline__ bool mp_guard_skips(const unsigned* amax, float limit, int guard) {

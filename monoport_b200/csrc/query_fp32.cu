@@ -390,8 +390,13 @@ query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
   const int warp = tid >> 5, lane = tid & 31;
   const int L = prm.n_layers;
   const int res = prm.cout[L - 1];
-  const long long n = src.n;
-  const long long n_tiles = (n + P - 1) / P;
+  long long n = src.n;
+  if (src.count_dev) {                               // (the point count on the device: src.n is then the capacity)
+    const long long c = *src.count_dev;
+    n = c < n ? c : n;
+  }
+  // the range guard, decided per launch as query_fp32_kernel decides it (uniform over the grid)
+  const long long n_tiles = mp_guard_skips(prm.amax, prm.amax_limit, prm.guard) ? 0 : (n + P - 1) / P;
   const MpBatch one;                                 // (a single map)
 
   for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
@@ -642,7 +647,7 @@ int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfa
 
 int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
-                         long long ld_dp, cudaStream_t st) {
+                         long long ld_dp, cudaStream_t st, int guard) {
   if (src.n <= 0) return MP_OK;
   if (src.kind != MP_SRC_ROWS) {
     mp_set_error("the gradient kernel takes point rows");
@@ -652,6 +657,7 @@ int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
   int sms = 0, max_smem = 0;
   const int rc = fill_params(mlp, feat, prm, sms, max_smem);
   if (rc != MP_OK) return rc;
+  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
   GradParams gp;
   memset(&gp, 0, sizeof(gp));
   int words = 0;
@@ -666,7 +672,7 @@ int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
   if (out) {                                      // the value: query_fp32_kernel's own, bit for bit
     MpOutDst dst;
     dst.out = out; dst.ld = ld_out; dst.scatter_vol = nullptr;
-    const int rq = mp_launch_query_fp32(mlp, feat, src, cal, dst, st);
+    const int rq = mp_launch_query_fp32(mlp, feat, src, cal, dst, st, guard);
     if (rq != MP_OK) return rq;
   }
   const int res = prm.cout[prm.n_layers - 1];

@@ -622,6 +622,531 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   }
 }
 
+// ====================================================================================================================
+// F1‴: the gradient of the query program with respect to the points, forward mode (a JVP with three tangents).  The output
+// depends on a point only through its texel coordinates (ix, iy) and its depth feature zf, and a tangent goes through the
+// same weights as the value in the same order: so the tangents are three more rows of the A operand, and a tile of 64 rows
+// is 16 points x (value, d/dix, d/diy, d/dzf).  The weight stream, the ring, the wait schedule and every MMA are those of
+// query_wg_kernel; the value rows are its rows, bit for bit (same taps, same roundings, same layer-4 summation order).
+// Row map (jvp_row): point k (0..15) of the tile has its value on row 16 (k/4) + k%4, d/dix 8 rows below, d/diy 4 rows
+// below, d/dzf 12 rows below -- in the accumulator fragment, lanes 0-15 of warp k/4 hold (value, d/dix) and lanes 16-31
+// the same columns of (d/diy, d/dzf), so a value's leaky-ReLU branch reaches its tangents as packed sign bits through one
+// __shfl_xor_sync(.., 16) per 32 columns.
+//   X:        value = the fp16 map sampled as query_wg_kernel does; d/dix, d/diy = the bilinear derivative of the map
+//             (differences of the same taps), rounded once to fp16; d/dzf = 0 (the depth column is not part of X).
+//   layer 0:  value = query_wg_kernel's chunk; tangents = slope(value) * (derivative of the sampled G0, or w0z for zf).
+//   layers 1-3: bias and depth column on the value row, the depth column alone on the zf row, every tangent times the
+//             value's slope (1 above 0, else 0.01: torch's lrelu'(0) = slope, as in query_grad_kernel).
+//   layer 4:  the same fp32 hidden dot for every row, plus S4's value / x / y derivative, or w4z for the zf row.
+// Per point: g = grad_out * act'(y), d/d(ix, iy, zf) = sum_r g_r * y'_r, then d/du = d/dix (W-1)/2, d/dv = d/diy (H-1)/2,
+// d/dw = d/dzf z_scale and the projection's Jacobian as in query_grad_kernel.  Points outside the image get 0 for both.
+// One map; the range guard is decided per launch from amax[0] (producer and consumers take the same predicate).
+constexpr int kJvpPts = kTile / 4;      // points per tile
+constexpr int kJvpDwBytes = kJvpPts * 8 * 4;   // d wgt / d(ix, iy) of the tile's points, after Prog<C>::Total
+static_assert(Prog<256>::Total + kJvpDwBytes + 1024 <= 232448 && Prog<512>::Total + kJvpDwBytes + 1024 <= 232448,
+              "shared memory budget of query_jvp_kernel (227 KB per CTA)");
+
+struct JvpOut {
+  float* out;             // [Res][ld_out] value, or null
+  long long ld_out;
+  float* dp;              // [3][ld_dp]
+  long long ld_dp;
+  const float* grad_out;  // [Res][ld_grad], or null (ones)
+  long long ld_grad;
+};
+
+// A-operand row of tangent t (0 value, 1 d/dix, 2 d/diy, 3 d/dzf) of point k of a tile
+__device__ __forceinline__ int jvp_row(int k, int t) { return 16 * (k >> 2) + (k & 3) + (t == 1 ? 8 : t == 2 ? 4 : t == 3 ? 12 : 0); }
+
+struct JvpTaps {
+  PointTaps pt;           // the value's taps, as query_wg_kernel takes them
+  float dx[4], dy[4];     // d wgt / d ix and d wgt / d iy of the taps (0 for the taps that are zero padding, and outside the image)
+  float u, v, w;          // the projected point
+};
+
+__device__ __forceinline__ JvpTaps jvp_taps(const MpPointSrc& src, const MpCalib& cal, int H, int W, long long i, long long n) {
+  JvpTaps j;
+  MpSurfaceSrc nosurf;
+  memset(&nosurf, 0, sizeof(nosurf));
+  const MpBatch one;
+  j.pt = point_taps(nosurf, src, cal, one, 0, H, W, i, n);
+  float u = 0.f, v = 0.f, w = 0.f;
+  if (i < n) {
+    float x, y, z;
+    mp_load_point(src, one, 0, i, x, y, z);
+    mp_project<true>(cal, x, y, z, u, v, w);
+  }
+  j.u = u; j.v = v; j.w = w;
+  // the tap cell of mp_taps
+  const float ix = ((u + 1.f) / 2.f) * (float)(W - 1), iy = ((v + 1.f) / 2.f) * (float)(H - 1);
+  const float x0 = floorf(ix), y0 = floorf(iy), x1 = x0 + 1.f, y1 = y0 + 1.f;
+  const bool x0ok = (x0 >= 0.f) && (x0 <= (float)(W - 1)), x1ok = (x1 >= 0.f) && (x1 <= (float)(W - 1));
+  const bool y0ok = (y0 >= 0.f) && (y0 <= (float)(H - 1)), y1ok = (y1 >= 0.f) && (y1 <= (float)(H - 1));
+  const bool live = j.pt.in_img;
+  const bool ok[4] = {live && x0ok && y0ok, live && x1ok && y0ok, live && x0ok && y1ok, live && x1ok && y1ok};
+  const float ddx[4] = {-(y1 - iy), y1 - iy, -(iy - y0), iy - y0};       // nw, ne, sw, se
+  const float ddy[4] = {-(x1 - ix), -(ix - x0), x1 - ix, ix - x0};
+#pragma unroll
+  for (int a = 0; a < 4; ++a) {
+    j.dx[a] = ok[a] ? ddx[a] : 0.f;
+    j.dy[a] = ok[a] ? ddy[a] : 0.f;
+  }
+  return j;
+}
+
+// epilogue of hidden layer 1 or 2 (side = its side_off): this lane's NJ x 2 columns (from col0 + cq) of rows r0 and r0 + 8
+// -> the fp16 K-major operand at buf.  isv: the lane holds (value, d/dix) rows, else (d/diy, d/dzf).  Column pair by column
+// pair, so that each accumulator dies at its first use (the value's signs cross to lanes 16-31 as two bits per pair).
+// zt: the depth feature's tangent on row r0 + 8 (0: d/dix, 1: d/dzf), a multiplier rather than a select, so that no
+// per-lane product of the weights is hoisted out of the tile loop.
+template <int NJ>
+__device__ __forceinline__ void jvp_hidden_epilogue(const TcParams& prm, const float (&acc)[4 * NJ], int side, int col0, uint8_t* buf,
+                                                    int r0, int cq, float zf, bool isv, float zt) {
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = col0 + 8 * j + cq;
+    const float z0 = prm.wz_all[side + col], z1 = prm.wz_all[side + col + 1];
+    uint8_t* kbp = buf + (col >> 6) * kKb;
+    // the value row as query_wg_kernel writes it (lanes 0-15), and the signs of its fp16 pre-activations
+    const float a0 = acc[4 * j + 0] + fmaf(z0, zf, prm.bias_all[side + col]);
+    const float a1 = acc[4 * j + 1] + fmaf(z1, zf, prm.bias_all[side + col + 1]);
+    const float2 h = __half22float2(__floats2half2_rn(a0, a1));
+    uint32_t bits = (h.x > 0.f ? 1u : 0u) | (h.y > 0.f ? 2u : 0u);
+    const uint32_t other = __shfl_xor_sync(0xffffffffu, bits, 16);
+    bits = isv ? bits : other;
+    const float s0 = (bits & 1u) ? 1.f : MP_LEAKY_SLOPE, s1 = (bits & 2u) ? 1.f : MP_LEAKY_SLOPE;
+    *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0, col & 63)) =
+        isv ? act_pack(a0, a1) : tc::pack_half2(acc[4 * j + 0] * s0, acc[4 * j + 1] * s1);
+    *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0 + 8, col & 63)) =
+        tc::pack_half2(fmaf(z0, zt, acc[4 * j + 2]) * s0, fmaf(z1, zt, acc[4 * j + 3]) * s1);
+  }
+}
+
+template <int C>
+__global__ void __launch_bounds__(kThreads, 1)
+query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, JvpOut jo) {
+  using P = Prog<C>;
+  constexpr int RES = P::RES, Ring = P::Ring, XKB = P::XKB, NP = kJvpPts;
+  static_assert((5 + 3 * RES) * NP <= (2 + RES) * kTile, "per-point scalars of a JVP tile fit the Small block");
+  MP_DYN_SMEM(uint8_t, smem_raw);
+  uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::Bars);
+  uint64_t* empty = full + P::Slots;
+  float* s_zf = reinterpret_cast<float*>(smem + P::Small);   // [NP]
+  float* s_in = s_zf + NP;                                    // [NP]
+  float* s_uvw = s_in + NP;                                   // [3][NP]
+  float* s_s4 = s_uvw + 3 * NP;                               // [3][RES][NP]: S4 sampled, its d/dix, its d/diy
+  float* s_dw = reinterpret_cast<float*>(smem + P::Total);   // [NP][8]: d wgt / d ix of the four taps, then d wgt / d iy
+
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0), wg = warp >> 2;
+  long long n = src.n;
+  if (src.count_dev) {
+    const long long c = __shfl_sync(0xffffffffu, *src.count_dev, 0);
+    n = c < n ? c : n;
+  }
+  const int skip = __shfl_sync(0xffffffffu, (int)mp_guard_skips(prm.amax, prm.amax_limit, prm.guard), 0);
+  const long long n_tiles = skip ? 0 : (n + NP - 1) / NP;
+
+  if (tid == 0) {
+    for (int s = 0; s < P::Slots; ++s) {
+      tc::mbar_init(full + s, 1);
+      tc::mbar_init(empty + s, kConsumers / 32);
+    }
+    tc::fence_barrier_init();
+  }
+  __syncthreads();
+  auto l1_slot = [](uint32_t s) { return s % (uint32_t)P::Slots; };
+  auto l23_slot = [](uint32_t k) { return 2u + k % (uint32_t)Ring; };
+
+  if (wg == 2) {
+    // ============================== weight producer (query_wg_kernel's) ==============================
+    tc::setmaxnreg_dec<kProducerRegs>();
+    if (warp == 8 && lane == 0) {
+      const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
+      uint32_t phase = 0;
+      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+        for (int s = 0; s < P::StagesPerTile; ++s) {
+          const uint32_t slot = s < P::StagesL1 ? l1_slot(s) : l23_slot(s - P::StagesL1);
+          tc::mbar_wait(empty + slot, ((phase >> slot) & 1u) ^ 1u);
+          phase ^= 1u << slot;
+          tc::mbar_arrive_expect_tx(full + slot, kStageBytes);
+          tc::bulk_g2s(smem + P::H1 + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
+        }
+      }
+    }
+    return;
+  }
+
+  // ============================== consumers: query_wg_kernel's ring protocol ==============================
+  tc::setmaxnreg_inc<kConsumerRegs>();
+  const int wl = warp & 3;
+  const int r0 = 16 * wl + (lane >> 2), cq = 2 * (lane & 3);
+  const bool isv = lane < 16;                         // rows r0, r0 + 8 hold (value, d/dix), else (d/diy, d/dzf)
+  const int kpt = 4 * wl + ((lane >> 2) & 3);         // ... of point kpt
+  const float zt = (float)(lane >> 4);                // the depth feature's tangent on row r0 + 8
+  const uint32_t smem_base = tc::smem_u32(smem);
+  auto desc = [&](int off) { return tc::make_wdesc_sw128(smem_base + (uint32_t)off, 1024); };
+  auto sync_consumers = [&]() { tc::bar_sync(1, kConsumers); };
+  constexpr uint32_t Defer = P::StagesL1 - P::Slots;
+  uint32_t fphase = 0;
+  auto release_if = [&](uint32_t slot, bool pred) {
+    __syncwarp();
+    tc::mbar_arrive_if(empty + slot, pred && lane == 0);
+  };
+  auto release = [&](uint32_t slot) { release_if(slot, true); };
+  auto l1_release = [&](uint32_t s) { release_if(l1_slot(s), s - Defer >= 2u); };
+  auto take = [&](uint32_t slot) {
+    tc::mbar_wait(full + slot, (fphase >> slot) & 1u);
+    fphase ^= 1u << slot;
+  };
+  auto slot_off = [&](uint32_t slot) { return P::H1 + (int)slot * kStageBytes; };
+  auto l1_kblock = [&](float (&acc)[128], int i, int a_off) {
+    const uint32_t s0 = 2 * i, mine = s0 + wg, prev = mine - 2;
+    take(l1_slot(s0));
+    tc::wgmma_wait<0>();
+    if (i > 0) l1_release(prev);
+    take(l1_slot(s0 + 1));
+    l1_release(s0 + 1 - wg);
+    const uint64_t da = desc(a_off), db = desc(slot_off(l1_slot(mine)));
+    tc::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
+    tc::wgmma_commit();
+  };
+  auto step_take = [&](uint32_t k_layer, int k) {
+    if (k >= Ring) {
+      tc::wgmma_wait<Ring - 1>();
+      release(l23_slot(k_layer + k - Ring));
+    }
+    take(l23_slot(k_layer + k));
+    tc::wgmma_fence();
+  };
+  auto layer_end = [&](uint32_t k_layer, int n_steps) {
+    tc::wgmma_wait<0>();
+#pragma unroll
+    for (int j = Ring; j > 0; --j) release(l23_slot(k_layer + n_steps - j));
+  };
+
+  // ---- layer-0 chunks: lane = (point 2 warp + lane/16, K-block half (lane/8)%2, channels 8 (lane%8) ..), all four rows
+  const int l8 = lane & 7, kbh = (lane >> 3) & 1, gq = 2 * warp + (lane >> 4);
+  uint32_t t_off[2], t_wgt[2], t_z;
+  const __half* g0 = prm.g0;
+  auto gen_chunk = [&](int c) {
+    const int ch = c * 128 + kbh * 64 + l8 * 8;
+    __half2 b4[4], z4[4];
+    *reinterpret_cast<uint4*>(&b4[0]) = __ldg(reinterpret_cast<const uint4*>(prm.d_bias0 + ch));
+    *reinterpret_cast<uint4*>(&z4[0]) = __ldg(reinterpret_cast<const uint4*>(prm.d_wz0 + ch));
+    uint8_t* dstp = smem + P::H0 + ((c & 1) * 2 + kbh) * kKb;
+    const __half2 slope2 = __float2half2_rn(MP_LEAKY_SLOPE);
+    uint4 raw[4];
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      const uint32_t off = (a & 1) ? (t_off[a >> 1] >> 16) : (t_off[a >> 1] & 0xFFFFu);
+      raw[a] = __ldg(reinterpret_cast<const uint4*>(g0 + (size_t)off * kL0 + ch));
+    }
+    const __half2 zq2 = *reinterpret_cast<const __half2*>(&t_z);
+    const float4 dxa = *reinterpret_cast<const float4*>(s_dw + gq * 8), dya = *reinterpret_cast<const float4*>(s_dw + gq * 8 + 4);
+    const float t_dx[4] = {dxa.x, dxa.y, dxa.z, dxa.w}, t_dy[4] = {dya.x, dya.y, dya.z, dya.w};
+    __half2 acc[4];
+    float2 dx[4], dy[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[j] = __hfma2(z4[j], zq2, b4[j]);
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {            // same tap order as query_wg_kernel: nw, ne, sw, se
+      const __half2 wp = *reinterpret_cast<const __half2*>(&t_wgt[a >> 1]);
+      const __half2 w2 = (a & 1) ? __high2half2(wp) : __low2half2(wp);
+      const __half2* h = reinterpret_cast<const __half2*>(&raw[a]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        acc[j] = __hfma2(h[j], w2, acc[j]);
+        const float2 f = __half22float2(h[j]);
+        dx[j] = a == 0 ? make_float2(f.x * t_dx[0], f.y * t_dx[0]) : make_float2(fmaf(f.x, t_dx[a], dx[j].x), fmaf(f.y, t_dx[a], dx[j].y));
+        dy[j] = a == 0 ? make_float2(f.x * t_dy[0], f.y * t_dy[0]) : make_float2(fmaf(f.x, t_dy[a], dy[j].x), fmaf(f.y, t_dy[a], dy[j].y));
+      }
+    }
+    uint32_t o[4][4];                        // [row kind][channel pair]
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const __half2 r = __hmax2(acc[j], __hmul2(acc[j], slope2));
+      o[0][j] = *reinterpret_cast<const uint32_t*>(&r);
+      const float2 pre = __half22float2(acc[j]), wz = __half22float2(z4[j]);
+      const float s0 = pre.x > 0.f ? 1.f : MP_LEAKY_SLOPE, s1 = pre.y > 0.f ? 1.f : MP_LEAKY_SLOPE;
+      o[1][j] = tc::pack_half2(dx[j].x * s0, dx[j].y * s1);
+      o[2][j] = tc::pack_half2(dy[j].x * s0, dy[j].y * s1);
+      o[3][j] = tc::pack_half2(wz.x * s0, wz.y * s1);
+    }
+#pragma unroll
+    for (int t = 0; t < 4; ++t)
+      *reinterpret_cast<uint4*>(dstp + tc::sw128_offset(jvp_row(gq, t), l8 * 8)) = make_uint4(o[t][0], o[t][1], o[t][2], o[t][3]);
+    tc::fence_proxy_async_smem();
+  };
+
+  for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
+    const long long p0 = t * NP;
+    // ---- this lane's point (lane % 16) of the tile; X and the per-point scalars: warp w samples points 2w, 2w + 1
+    const JvpTaps jt = jvp_taps(src, cal, prm.H, prm.W, p0 + (lane & 15), n);
+#pragma unroll 1
+    for (int qq = 0; qq < 2; ++qq) {
+      const int q = 2 * warp + qq;
+      int off[4];
+      float wgt[4], wx[4], wy[4];
+#pragma unroll
+      for (int a = 0; a < 4; ++a) {
+        off[a] = __shfl_sync(0xffffffffu, jt.pt.off[a], q);
+        wgt[a] = __shfl_sync(0xffffffffu, jt.pt.wgt[a], q);
+        wx[a] = __shfl_sync(0xffffffffu, jt.dx[a], q);
+        wy[a] = __shfl_sync(0xffffffffu, jt.dy[a], q);
+      }
+#pragma unroll 1
+      for (int phase = 0; phase < C / 256; ++phase) {
+        const int cbase = phase * 256 + lane * 8;
+        uint4 raw[4];
+#pragma unroll
+        for (int a = 0; a < 4; ++a) raw[a] = __ldg(reinterpret_cast<const uint4*>(prm.feat16 + (size_t)off[a] * C + cbase));
+        float2 acc[4], ax[4], ay[4];
+#pragma unroll
+        for (int a = 0; a < 4; ++a) {        // the value as sample_x16 takes it: nw, ne, sw, se
+          const float2 w2 = make_float2(wgt[a], wgt[a]);
+          const __half2* h2 = reinterpret_cast<const __half2*>(&raw[a]);
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            const float2 f = __half22float2(h2[j]);
+            acc[j] = (a == 0) ? make_float2(__fmul_rn(f.x, w2.x), __fmul_rn(f.y, w2.y)) : make_float2(fmaf(f.x, w2.x, acc[j].x), fmaf(f.y, w2.y, acc[j].y));
+            ax[j] = (a == 0) ? make_float2(__fmul_rn(f.x, wx[0]), __fmul_rn(f.y, wx[0])) : make_float2(fmaf(f.x, wx[a], ax[j].x), fmaf(f.y, wx[a], ax[j].y));
+            ay[j] = (a == 0) ? make_float2(__fmul_rn(f.x, wy[0]), __fmul_rn(f.y, wy[0])) : make_float2(fmaf(f.x, wy[a], ay[j].x), fmaf(f.y, wy[a], ay[j].y));
+          }
+        }
+        uint8_t* xkb = smem + P::X + (phase * 4 + (lane >> 3)) * kKb;
+        const int k8 = (lane & 7) * 8;
+        *reinterpret_cast<uint4*>(xkb + tc::sw128_offset(jvp_row(q, 0), k8)) =
+            make_uint4(tc::pack_half2(acc[0].x, acc[0].y), tc::pack_half2(acc[1].x, acc[1].y), tc::pack_half2(acc[2].x, acc[2].y), tc::pack_half2(acc[3].x, acc[3].y));
+        *reinterpret_cast<uint4*>(xkb + tc::sw128_offset(jvp_row(q, 1), k8)) =
+            make_uint4(tc::pack_half2(ax[0].x, ax[0].y), tc::pack_half2(ax[1].x, ax[1].y), tc::pack_half2(ax[2].x, ax[2].y), tc::pack_half2(ax[3].x, ax[3].y));
+        *reinterpret_cast<uint4*>(xkb + tc::sw128_offset(jvp_row(q, 2), k8)) =
+            make_uint4(tc::pack_half2(ay[0].x, ay[0].y), tc::pack_half2(ay[1].x, ay[1].y), tc::pack_half2(ay[2].x, ay[2].y), tc::pack_half2(ay[3].x, ay[3].y));
+        *reinterpret_cast<uint4*>(xkb + tc::sw128_offset(jvp_row(q, 3), k8)) = make_uint4(0u, 0u, 0u, 0u);
+      }
+    }
+    if (lane < 16 && (lane >> 1) == warp) {          // point `lane`: its scalars (S4 as sample_x16 samples it)
+      const PointTaps& pt = jt.pt;
+#pragma unroll
+      for (int r = 0; r < RES; ++r) {
+        float s = 0.f, sx = 0.f, sy = 0.f;
+#pragma unroll
+        for (int a = 0; a < 4; ++a) {
+          const float s4 = __ldg(prm.s4tex + (size_t)pt.off[a] * RES + r);
+          s = fmaf(pt.wgt[a], s4, s);
+          sx = fmaf(jt.dx[a], s4, sx);
+          sy = fmaf(jt.dy[a], s4, sy);
+        }
+        s_s4[r * NP + lane] = s + __ldg(prm.w4z + r) * pt.zf + __ldg(prm.b4 + r);
+        s_s4[(RES + r) * NP + lane] = sx;
+        s_s4[(2 * RES + r) * NP + lane] = sy;
+      }
+      s_zf[lane] = pt.zf;
+      s_in[lane] = pt.in_img ? 1.f : 0.f;
+      s_uvw[lane] = jt.u;
+      s_uvw[NP + lane] = jt.v;
+      s_uvw[2 * NP + lane] = jt.w;
+#pragma unroll
+      for (int a = 0; a < 4; ++a) {
+        s_dw[lane * 8 + a] = jt.dx[a];
+        s_dw[lane * 8 + 4 + a] = jt.dy[a];
+      }
+    }
+    {
+      const PointTaps& pt = jt.pt;
+      const uint32_t o01 = (uint32_t)pt.off[0] | ((uint32_t)pt.off[1] << 16), o23 = (uint32_t)pt.off[2] | ((uint32_t)pt.off[3] << 16);
+      const uint32_t w01 = tc::pack_half2(pt.wgt[0], pt.wgt[1]), w23 = tc::pack_half2(pt.wgt[2], pt.wgt[3]);
+      const uint32_t zz = tc::pack_half2(pt.zf, pt.zf);
+      t_off[0] = __shfl_sync(0xffffffffu, o01, gq & 15);
+      t_off[1] = __shfl_sync(0xffffffffu, o23, gq & 15);
+      t_wgt[0] = __shfl_sync(0xffffffffu, w01, gq & 15);
+      t_wgt[1] = __shfl_sync(0xffffffffu, w23, gq & 15);
+      t_z = __shfl_sync(0xffffffffu, zz, gq & 15);
+    }
+    tc::fence_proxy_async_smem();
+    sync_consumers();                                // s_dw
+    gen_chunk(0);
+    sync_consumers();
+    const float zf = s_zf[kpt];
+    // the epilogues' row and column, re-derived per tile: otherwise their 2 x 48 swizzled store offsets are hoisted out of
+    // the tile loop, which leaves no registers for layer 1
+    int r0t = r0, cqt = cq;
+    asm volatile("" : "+r"(r0t), "+r"(cqt));
+
+    // ---- layer 1 (query_wg_kernel's schedule)
+    {
+      float acc[128];
+#pragma unroll
+      for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+#pragma unroll 1
+      for (int c = 0; c < 8; ++c) {
+#pragma unroll
+        for (int kb = 0; kb < 2; ++kb) l1_kblock(acc, 2 * c + kb, P::H0 + ((c & 1) * 2 + kb) * kKb);
+        if (c < 7) {
+          sync_consumers();
+          gen_chunk(c + 1);
+          sync_consumers();
+        }
+      }
+#pragma unroll 1
+      for (int kb = 0; kb < XKB; ++kb) l1_kblock(acc, 16 + kb, P::X + kb * kKb);
+      tc::wgmma_wait<0>();
+      l1_release(2 * (16 + XKB - 1) + wg);
+      sync_consumers();
+      jvp_hidden_epilogue<32>(prm, acc, side_off(1), wg * 256, smem + P::H1, r0t, cqt, zf, isv, zt);
+      tc::fence_proxy_async_smem();
+      sync_consumers();
+    }
+    // ---- layer 2
+    {
+      float acc[64];
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+#pragma unroll 1
+      for (int kb = 0; kb < P::StagesL2; ++kb) {
+        step_take(0, kb);
+        const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(slot_off(l23_slot(kb)) + wg * 16384);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tc::wgmma_m64n128(acc, da + 2 * k, db + 2 * k);
+        tc::wgmma_commit();
+      }
+      layer_end(0, P::StagesL2);
+      jvp_hidden_epilogue<16>(prm, acc, side_off(2), wg * 128, smem + P::H0, r0t, cqt, zf, isv, zt);
+      tc::fence_proxy_async_smem();
+      sync_consumers();
+    }
+    // ---- layer 3, then layer 4 in fp32
+    {
+      float acc[32];
+#pragma unroll
+      for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+#pragma unroll 1
+      for (int q = 0; q < P::StagesL3; ++q) {
+        step_take(P::StagesL2, q);
+#pragma unroll
+        for (int sub = 0; sub < 2; ++sub) {
+          const int kb = (2 * q + sub) % (XKB + 4);
+          const uint64_t da = desc(kb < XKB ? P::X + kb * kKb : P::H0 + (kb - XKB) * kKb);
+          const uint64_t db = desc(slot_off(l23_slot(P::StagesL2 + q)) + sub * 16384 + wg * 8192);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) tc::wgmma_m64n64(acc, da + 2 * k, db + 2 * k);
+        }
+        tc::wgmma_commit();
+      }
+      layer_end(P::StagesL2, P::StagesL3);
+      // row r0: the value's hidden dot exactly as query_wg_kernel sums it (lanes < 16), and the signs of its layer-3 outputs
+      float lg[2][RES], lt[RES];
+#pragma unroll
+      for (int r = 0; r < RES; ++r) lg[0][r] = lg[1][r] = lt[r] = 0.f;
+      uint32_t m = 0u;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = wg * 64 + 8 * j + cq + e;
+          float o = acc[4 * j + e] + fmaf(prm.wz_all[side_off(3) + col], zf, prm.bias_all[side_off(3) + col]);
+          m |= (o > 0.f ? 1u : 0u) << (2 * j + e);
+          o = fmaxf(o, o * MP_LEAKY_SLOPE);
+#pragma unroll
+          for (int r = 0; r < RES; ++r) lg[0][r] = fmaf(__ldg(prm.w4h + r * kL3 + col), o, lg[0][r]);
+        }
+      {
+        const uint32_t o = __shfl_xor_sync(0xffffffffu, m, 16);
+        m = isv ? m : o;
+      }
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int col = wg * 64 + 8 * j + cq + (e & 1);
+          const float s = ((m >> (2 * j + (e & 1))) & 1u) ? 1.f : MP_LEAKY_SLOPE;
+          if (e < 2) {                                  // d/diy (lanes >= 16)
+#pragma unroll
+            for (int r = 0; r < RES; ++r) lt[r] = fmaf(__ldg(prm.w4h + r * kL3 + col), acc[4 * j + e] * s, lt[r]);
+          } else {                                      // d/dix, d/dzf (+ the depth column)
+            const float t3 = fmaf(prm.wz_all[side_off(3) + col], zt, acc[4 * j + e]) * s;
+#pragma unroll
+            for (int r = 0; r < RES; ++r) lg[1][r] = fmaf(__ldg(prm.w4h + r * kL3 + col), t3, lg[1][r]);
+          }
+        }
+#pragma unroll
+      for (int r = 0; r < RES; ++r) lg[0][r] = isv ? lg[0][r] : lt[r];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < RES; ++r) {
+          lg[h][r] += __shfl_xor_sync(0xffffffffu, lg[h][r], 1);
+          lg[h][r] += __shfl_xor_sync(0xffffffffu, lg[h][r], 2);
+        }
+      float* s_part = reinterpret_cast<float*>(smem + P::H1);
+      const int mine = lane & 3;
+      const int row = r0 + 8 * (mine & 1);
+      auto lg_mine = [&](int r) { return (mine & 1) ? lg[1][r] : lg[0][r]; };
+      if (wg == 1 && mine < 2) {
+#pragma unroll
+        for (int r = 0; r < RES; ++r) s_part[r * kTile + row] = lg_mine(r);
+      }
+      sync_consumers();
+      if (wg == 0) {
+        // this lane's row: 0 value, 1 d/dix, 2 d/diy, 3 d/dzf (of point kpt; lanes with mine >= 2 duplicate)
+        const int kind = (isv ? 0 : 2) + (mine & 1);
+        float y[RES], yx[RES], yy[RES], yz[RES];
+#pragma unroll
+        for (int r = 0; r < RES; ++r) {
+          const float base = kind == 3 ? __ldg(prm.w4z + r) : s_s4[((kind == 0 ? 0 : kind == 1 ? RES : 2 * RES) + r) * NP + kpt];
+          y[r] = base + (lg_mine(r) + s_part[r * kTile + row]);
+        }
+        // the point's four rows meet in its value lane 4k: d/dix from lane 4k + 1, d/diy from 4k + 16, d/dzf from 4k + 17
+        const int lv = lane & 12;
+#pragma unroll
+        for (int r = 0; r < RES; ++r) {
+          yx[r] = __shfl_sync(0xffffffffu, y[r], lv + 1);
+          yy[r] = __shfl_sync(0xffffffffu, y[r], lv + 16);
+          yz[r] = __shfl_sync(0xffffffffu, y[r], lv + 17);
+        }
+        const long long i = p0 + kpt;
+        if (isv && mine == 0 && i < n) {
+          const float inimg = s_in[kpt];
+          float gx = 0.f, gy = 0.f, gz = 0.f;
+#pragma unroll
+          for (int r = 0; r < RES; ++r) {
+            const float act = mp_last_op(y[r], prm.last_op);
+            if (jo.out) jo.out[(long long)r * jo.ld_out + i] = inimg * act;
+            const float d = prm.last_op == MP_LAST_SIGMOID ? act * (1.f - act) : (prm.last_op == MP_LAST_TANH ? 1.f - act * act : 1.f);
+            const float g = (jo.grad_out ? __ldg(jo.grad_out + (long long)r * jo.ld_grad + i) : 1.f) * d;
+            gx = fmaf(g, yx[r], gx);
+            gy = fmaf(g, yy[r], gy);
+            gz = fmaf(g, yz[r], gz);
+          }
+          const float du = gx * (0.5f * (float)(prm.W - 1)), dv = gy * (0.5f * (float)(prm.H - 1)), dw = cal.z_scale * gz;
+          float gp[3];
+          if (!cal.has) {
+            gp[0] = du; gp[1] = dv; gp[2] = dw;
+          } else if (!cal.perspective) {                 // J = R
+#pragma unroll
+            for (int a = 0; a < 3; ++a) gp[a] = cal.m[a] * du + cal.m[4 + a] * dv + cal.m[8 + a] * dw;
+          } else {                                       // J rows: (R0 - u R2) / w, (R1 - v R2) / w, R2
+            const float u = s_uvw[kpt], v = s_uvw[NP + kpt], w = s_uvw[2 * NP + kpt];
+            const float su = du / w, sv = dv / w;
+            const float s2 = dw - su * u - sv * v;
+#pragma unroll
+            for (int a = 0; a < 3; ++a) gp[a] = cal.m[a] * su + cal.m[4 + a] * sv + cal.m[8 + a] * s2;
+          }
+#pragma unroll
+          for (int a = 0; a < 3; ++a) jo.dp[a * jo.ld_dp + i] = inimg != 0.f ? gp[a] : 0.f;     // outside the image: exactly 0
+        }
+      }
+      sync_consumers();
+      tc::fence_proxy_async_smem();
+      release(l1_slot(Defer));
+      release(l1_slot(Defer + 1));
+    }
+  }
+}
+
 // G0[texel][n] = sum_k F[texel][k] * W0f[n][k] on the tensor cores: fp16 operands (F rounded once while staging, W0f
 // pre-packed on the host as SWIZZLE_128B tiles [n tile][K block][256 x 64]) and fp32 accumulation in registers.
 // One CTA = 128 texels of one map (grid: texel blocks x maps of the handle) x all 1024 outputs: the A operand (128 x C) is staged ONCE by the two consumer warpgroups (fp32
@@ -880,6 +1405,7 @@ int tc_prepare(mp_mlp* mlp) {
   if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(query_wg_kernel<C, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + 1024);
   if (e == cudaSuccess) e = cudaFuncSetAttribute(g0_wg_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G0Cfg<C>::Smem);
+  if (e == cudaSuccess) e = cudaFuncSetAttribute(query_jvp_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize, P::Total + kJvpDwBytes + 1024);
   if (e != cudaSuccess) {
     mp_set_error("mp_tc_prepare: %s", cudaGetErrorString(e));
     mp_tc_release(mlp);
@@ -889,11 +1415,9 @@ int tc_prepare(mp_mlp* mlp) {
   return MP_OK;
 }
 
-// per-frame per-texel products of the head (G0, the fp16 copy of the map, S4) for every map of the handle, then the fused
-// query over the images of bt
+// per-frame per-texel products of the head (G0, the fp16 copy of the map, S4) for every map of the handle, when stale
 template <int C>
-int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
-           cudaStream_t st, const MpSurfaceSrc& surf, int guard, const MpBatch& bt) {
+int frame_products(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, cudaStream_t st) {
   using P = Prog<C>;
   const long long HW = (long long)feat->H * feat->W;
   const int maps = feat->B > 1 ? feat->B : 1;
@@ -920,20 +1444,11 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
     feat->g0_owner = mlp->gen;
     feat->g0_version = feat->version;
   }
-  if (surf.X && guard == MP_GUARD_NONE && isfinite(mlp->tc_amax_limit)) {
-    // the eager rendering (mp_colorize_surface): check the frame's feature range on the host (one 4-byte read-back per
-    // frame) and let the caller take the unfused path when it is outside the validated range.  (The enqueue-only render,
-    // mp_colorize_surface_async, passes MP_GUARD_IN_RANGE instead and launches the exact twin beside this one.)
-    unsigned bits = 0;
-    MP_CUDA(cudaMemcpyAsync(&bits, feat->amax, sizeof(bits), cudaMemcpyDeviceToHost, st));
-    MP_CUDA(cudaStreamSynchronize(st));
-    float a;
-    memcpy(&a, &bits, sizeof(a));
-    if (a > mlp->tc_amax_limit) {
-      mp_set_error("feature magnitude %.3g is outside the validated range of the tensor-core colour program (limit %.3g)", a, mlp->tc_amax_limit);
-      return MP_E_RANGE;
-    }
-  }
+  return MP_OK;
+}
+
+// the kernel parameters of the head's program on the current frame of feat
+TcParams tc_params(const mp_mlp* mlp, const TcPack* pk, const mp_feat* feat, int guard) {
   TcParams prm;
   memset(&prm, 0, sizeof(prm));
   prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
@@ -949,6 +1464,31 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
   prm.s4tex = feat->s4tex;
   prm.d_bias0 = pk->d_bias0;
   prm.d_wz0 = pk->d_wz0;
+  return prm;
+}
+
+// the per-frame products, then the fused query over the images of bt
+template <int C>
+int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
+           cudaStream_t st, const MpSurfaceSrc& surf, int guard, const MpBatch& bt) {
+  using P = Prog<C>;
+  const int rp = frame_products<C>(mlp, pk, feat, st);
+  if (rp != MP_OK) return rp;
+  if (surf.X && guard == MP_GUARD_NONE && isfinite(mlp->tc_amax_limit)) {
+    // the eager rendering (mp_colorize_surface): check the frame's feature range on the host (one 4-byte read-back per
+    // frame) and let the caller take the unfused path when it is outside the validated range.  (The enqueue-only render,
+    // mp_colorize_surface_async, passes MP_GUARD_IN_RANGE instead and launches the exact twin beside this one.)
+    unsigned bits = 0;
+    MP_CUDA(cudaMemcpyAsync(&bits, feat->amax, sizeof(bits), cudaMemcpyDeviceToHost, st));
+    MP_CUDA(cudaStreamSynchronize(st));
+    float a;
+    memcpy(&a, &bits, sizeof(a));
+    if (a > mlp->tc_amax_limit) {
+      mp_set_error("feature magnitude %.3g is outside the validated range of the tensor-core colour program (limit %.3g)", a, mlp->tc_amax_limit);
+      return MP_E_RANGE;
+    }
+  }
+  const TcParams prm = tc_params(mlp, pk, feat, guard);
   int dev = 0, sms = 132;
   MP_CUDA(cudaGetDevice(&dev));
   MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -960,6 +1500,28 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
 #else
   if (dst.n_peers > 0) MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, true>(prm, src, cal, dst, surf, bt)));
   else MP_EMU_LAUNCH(grid, kThreads, (query_wg_kernel<C, false>(prm, src, cal, dst, surf, bt)));
+#endif
+  MP_CUDA(cudaGetLastError());
+  return MP_OK;
+}
+
+// the per-frame products, then the JVP program over src.n points of the single map of feat (16 points per tile)
+template <int C>
+int launch_jvp(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const JvpOut& jo,
+               cudaStream_t st, int guard) {
+  using P = Prog<C>;
+  const int rp = frame_products<C>(mlp, pk, feat, st);
+  if (rp != MP_OK) return rp;
+  const TcParams prm = tc_params(mlp, pk, feat, guard);
+  int dev = 0, sms = 132;
+  MP_CUDA(cudaGetDevice(&dev));
+  MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const long long tiles = (src.n + kJvpPts - 1) / kJvpPts;
+  const int grid = (int)(tiles < (long long)sms ? tiles : sms);
+#ifndef MP_CUDA_EMU
+  query_jvp_kernel<C><<<grid, kThreads, P::Total + kJvpDwBytes + 1024, st>>>(prm, src, cal, jo);
+#else
+  MP_EMU_LAUNCH(grid, kThreads, (query_jvp_kernel<C>(prm, src, cal, jo)));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -1058,4 +1620,32 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
   const MpBatch& b = bt ? *bt : MpBatch();
   return C == 256 ? launch<256>(mlp, pk, feat, src, cal, dst, st, surf, guard, b)
                   : launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, b);
+}
+
+int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
+                           long long ld_grad, float* out, long long ld_out, float* dpoints, long long ld_dp, cudaStream_t st, int guard) {
+  if (src.n <= 0) return MP_OK;
+  const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
+  if (!pk || !mlp->tc_ok) {
+    mp_set_error("tensor-core path not prepared for this head");
+    return MP_E_UNSUPPORTED;
+  }
+  const int C = pk->kind == 1 ? 512 : 256;
+  if (feat->C != C) {
+    mp_set_error("head expects %d input channels but the feature map has %d (+1 depth)", mlp->channels[0], feat->C);
+    return MP_E_INVALID;
+  }
+  if ((long long)feat->H * feat->W > 65536) {      // (as mp_launch_query_tc)
+    mp_set_error("the tensor-core program handles feature maps of at most 65536 texels (got %d x %d); use MP_MODE_FP32", feat->H, feat->W);
+    return MP_E_UNSUPPORTED;
+  }
+  if (src.kind != MP_SRC_ROWS || feat->B != 1) {
+    mp_set_error("the gradient program takes point rows of one map");
+    return MP_E_UNSUPPORTED;
+  }
+  JvpOut jo;
+  jo.out = out; jo.ld_out = ld_out;
+  jo.dp = dpoints; jo.ld_dp = ld_dp;
+  jo.grad_out = grad_out; jo.ld_grad = ld_grad;
+  return C == 256 ? launch_jvp<256>(mlp, pk, feat, src, cal, jo, st, guard) : launch_jvp<512>(mlp, pk, feat, src, cal, jo, st, guard);
 }

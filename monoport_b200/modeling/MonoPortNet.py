@@ -185,12 +185,18 @@ class MonoPortNet(nn.Module):
         return [out]
 
     @torch.no_grad()
-    def query_gradient(self, feats_stages, points, calibs=None, grad_output=None):
-        """query() and its gradient with respect to the points, in one launch of the exact fp32 kernel
-        (mp_query_points_grad).  feats/points/calibs as for query() with B == 1; grad_output [1,Res,N] or None (ones).
-        -> (preds [1,Res,N] -- bit-identical to query() with precision "fp32" --,
-            dpoints [1,3,N] = d sum(grad_output * preds) / d points; for the geometry head and grad_output=None, grad sigma).
+    def query_gradient(self, feats_stages, points, calibs=None, grad_output=None, precision="fp32"):
+        """query() and its gradient with respect to the points (mp_query_points_grad_mode).  feats/points/calibs as for
+        query() with B == 1; grad_output [1,Res,N] or None (ones).
+        precision "fp32" (default): one launch of the exact fp32 kernel; preds bit-identical to query() with precision "fp32".
+        "tc": the tensor-core program's forward-mode derivative; preds bit-identical to query() with precision "tc", and a
+        frame above the head's feature limit is differentiated exactly (decided on the GPU).  Maps above 65536 texels are
+        refused.  "auto": "tc" where the head and the map allow it, else "fp32".
+        -> (preds [1,Res,N], dpoints [1,3,N] = d sum(grad_output * preds) / d points; for the geometry head and
+            grad_output=None, grad sigma).
         Points outside the image get 0 for both.  Autograd is not involved: `points.requires_grad` is ignored."""
+        if precision not in ("fp32", "tc", "auto"):
+            raise ValueError("precision must be one of 'fp32', 'tc', 'auto'; got %r" % (precision,))
         if self.training:
             raise NotImplementedError("query_gradient is eval-mode only (the gradient of the last stage, like query()); "
                                       "call .eval()")
@@ -230,11 +236,11 @@ class MonoPortNet(nn.Module):
         with _lib.device_guard(feat.device):
             fh = self.feature_handle(feat)
             proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
-            _lib.check(_lib.load().mp_query_points_grad(
+            _lib.check(_lib.load().mp_query_points_grad_mode(
                 head.handle(), fh.ptr, ctypes.c_void_p(points.data_ptr()), n, s[1], s[2], _lib.calib12(calibs), proj,
                 ctypes.c_float(self.normalizer.scale), None if gout is None else ctypes.c_void_p(gout.data_ptr()), n,
-                ctypes.c_void_p(out.data_ptr()), n, ctypes.c_void_p(dp.data_ptr()), n, _lib.stream_ptr(feat.device)),
-                "mp_query_points_grad")
+                ctypes.c_void_p(out.data_ptr()), n, ctypes.c_void_p(dp.data_ptr()), n, None, _MODES[precision],
+                _lib.stream_ptr(feat.device)), "mp_query_points_grad_mode")
         return out, dp
 
     def _query_batch(self, feat, points, calibs):

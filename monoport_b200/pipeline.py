@@ -68,7 +68,9 @@ class FrameGraph:
         visible vertices into an [R,R,3] canvas like colorization(netC, ...) -- mp_colorize_surface_async: the vertex count
         stays on the device and the range guard of the tensor-core colour program is decided there (a frame outside it
         is rendered by the exact fp32 kernel, like netC.query would evaluate it);
-      render_normals: the normal image, like colorization(norm=N) (mp_render_normals_async);
+      render_normals: the normal image, like colorization(norm=N) (mp_render_normals_async).  True: N = forward_vertices'
+        finite-difference normals (the norm result() returns); "gradient": N = the analytic normals of the geometry net,
+        surface_normals(..., precision="auto") computed inside the step (mp_surface_normals_async, the count on the device);
       canvas: the background of both images ([R,R,3], default ones).
     launch(x, x_colour) then takes the netC input too, and rendered() (after result()) returns (render_norm, render_tex)."""
 
@@ -92,7 +94,9 @@ class FrameGraph:
         if input_shape is None:
             input_shape = (1, 3, 512, 512) if with_encoder else (1, net.surface_classifier.filter_channels[0] - 1, 128, 128)
         self.netC = netC
-        self.render_normals = bool(render_normals)
+        if render_normals not in (False, True, "gradient"):
+            raise ValueError("render_normals must be False, True or 'gradient'; got %r" % (render_normals,))
+        self.render_normals = render_normals
         lib = self._lib = _lib.load()
         with torch.cuda.device(dev):
             self.stream = torch.cuda.Stream(dev)
@@ -114,7 +118,7 @@ class FrameGraph:
                 self._fhc = None
                 self._headC = netC.surface_classifier.handle()
                 self._projC = _lib.PROJ_PERSPECTIVE if netC.projection is perspective else _lib.PROJ_ORTHOGONAL
-                self._bmin3, self._bmax3 = _lib.f3(engine.b_min), _lib.f3(engine.b_max)
+            self._bmin3, self._bmax3 = _lib.f3(engine.b_min), _lib.f3(engine.b_max)
             self.volume = torch.empty((1, 1, R, R, R), dtype=torch.float32, device=dev)
             cap = R * R
             self.X = torch.empty(cap, dtype=torch.int64, device=dev)
@@ -122,6 +126,9 @@ class FrameGraph:
             self.Z = torch.empty(cap, dtype=torch.float32, device=dev)
             self.N = torch.empty((cap, 3), dtype=torch.float32, device=dev)
             self.count = torch.zeros(1, dtype=torch.int64, device=dev)
+            if render_normals == "gradient":
+                self.N_grad = torch.empty((cap, 3), dtype=torch.float32, device=dev)
+                self._nscratch = torch.empty(6 * cap + 1, dtype=torch.float32, device=dev)
             self._scratch = torch.empty(int(lib.mp_forward_vertices_scratch_bytes(R)), dtype=torch.uint8, device=dev)
             self._oct = engine._new_handle(dev)            # private workspace: graphs of different lanes overlap
             self._fh = None
@@ -162,9 +169,17 @@ class FrameGraph:
             ctypes.c_void_p(self.count.data_ptr()), ctypes.c_void_p(self._scratch.data_ptr()), st), "mp_forward_vertices_async")
         cap = self.X.numel()
         if self.render_normals:
+            norm = self.N
+            if self.render_normals == "gradient":
+                norm = self.N_grad
+                _lib.check(lib.mp_surface_normals_async(
+                    self._head, self._fh.ptr, ctypes.c_void_p(self.X.data_ptr()), ctypes.c_void_p(self.Y.data_ptr()),
+                    ctypes.c_void_p(self.Z.data_ptr()), ctypes.c_void_p(self.count.data_ptr()), cap, self.R, self._bmin3,
+                    self._bmax3, self._cal12, self._proj, ctypes.c_float(self.net.normalizer.scale), _lib.MODE_AUTO,
+                    ctypes.c_void_p(self._nscratch.data_ptr()), ctypes.c_void_p(norm.data_ptr()), st), "mp_surface_normals_async")
             self.render_norm.copy_(self._bg)
             _lib.check(lib.mp_render_normals_async(
-                ctypes.c_void_p(self.X.data_ptr()), ctypes.c_void_p(self.Y.data_ptr()), ctypes.c_void_p(self.N.data_ptr()),
+                ctypes.c_void_p(self.X.data_ptr()), ctypes.c_void_p(self.Y.data_ptr()), ctypes.c_void_p(norm.data_ptr()),
                 ctypes.c_void_p(self.count.data_ptr()), cap, self.R, ctypes.c_void_p(self.render_norm.data_ptr()), st),
                 "mp_render_normals_async")
         if self.netC is not None:

@@ -227,20 +227,53 @@ def _visible_world_points(X, Y, Z, resolution, b_min, b_max, device):
     return orthogonal(samples, make_mat_color(resolution, b_min, b_max, device).unsqueeze(0))
 
 
+def _surface_normals_device(net, feat, X, Y, Z, calib_tensor, resolution, b_min, b_max, precision):
+    """surface_normals in "tc" / "auto": one mp_surface_normals_async call with the vertex count on the device"""
+    import ctypes
+    from . import _lib
+    from .modeling.MonoPortNet import _MODES
+    from .modeling.geometry import perspective
+    device = calib_tensor.device
+    n = X.numel()
+    out = torch.empty((n, 3), dtype=torch.float32, device=device)
+    if n == 0:
+        return out
+    Xd, Yd = X.to(device=device, dtype=torch.int64).contiguous(), Y.to(device=device, dtype=torch.int64).contiguous()
+    Zd = Z.to(device=device, dtype=torch.float32).contiguous()
+    count = torch.tensor([n], dtype=torch.int64, device=device)
+    scratch = torch.empty(6 * n + 1, dtype=torch.float32, device=device)
+    with _lib.device_guard(device):
+        fh = net.feature_handle(feat)
+        proj = _lib.PROJ_PERSPECTIVE if net.projection is perspective else _lib.PROJ_ORTHOGONAL
+        _lib.check(_lib.load().mp_surface_normals_async(
+            net.surface_classifier.handle(), fh.ptr, ctypes.c_void_p(Xd.data_ptr()), ctypes.c_void_p(Yd.data_ptr()),
+            ctypes.c_void_p(Zd.data_ptr()), ctypes.c_void_p(count.data_ptr()), n, int(resolution), _lib.f3(b_min),
+            _lib.f3(b_max), _lib.calib12(calib_tensor), proj, ctypes.c_float(net.normalizer.scale), _MODES[precision],
+            ctypes.c_void_p(scratch.data_ptr()), ctypes.c_void_p(out.data_ptr()), _lib.stream_ptr(device)),
+            "mp_surface_normals_async")
+    return out
+
+
 @torch.no_grad()
-def surface_normals(net, feats, X, Y, Z, calib_tensor, resolution=257, b_min=(-1, -1, -1), b_max=(1, 1, 1)):
+def surface_normals(net, feats, X, Y, Z, calib_tensor, resolution=257, b_min=(-1, -1, -1), b_max=(1, 1, 1), precision="fp32"):
     """Exact normals of the visible surface of forward_vertices(sdf, "front"), for colorization(..., norm=...): the
     geometry net's gradient (MonoPortNet.query_gradient) at the points colorization() samples, (X, Y, R - Z) through
     mat_color, returned [N,3] in forward_vertices' frame and sign.  Its normals are -(d/dX, d/dY, d/dZ) of the volume
     in its (X, Y, Z) index axes (finite differences, RTL/recon.py:80-87); Z runs against the world z axis (R - Z above), so
     the normal is -(g_x L_x, g_y L_y, -g_z L_z) / R normalised, with g the world gradient and L = b_max - b_min.  A vertex
-    where the gradient vanishes gets a zero vector.  None when there is no surface (X is None)."""
+    where the gradient vanishes gets a zero vector.  None when there is no surface (X is None).  precision: that of
+    query_gradient ("fp32": the exact kernel; "tc" / "auto": the tensor-core program's forward-mode derivative, through
+    mp_surface_normals_async -- the launches FrameGraph(render_normals="gradient") captures, so both give the same bits)."""
+    if precision not in ("fp32", "tc", "auto"):
+        raise ValueError("precision must be one of 'fp32', 'tc', 'auto'; got %r" % (precision,))
     if X is None:
         return None
     device = calib_tensor.device
+    if precision != "fp32":
+        return _surface_normals_device(net, feats[-1][0].to(device), X, Y, Z, calib_tensor, resolution, b_min, b_max, precision)
     samples = _visible_world_points(X, Y, Z, resolution, b_min, b_max, device)
     feats = [[f.to(device) for f in fs] for fs in feats]
-    _, grad = net.query_gradient(feats, samples, calib_tensor)
+    _, grad = net.query_gradient(feats, samples, calib_tensor, precision=precision)
     length = (torch.as_tensor(np.asarray(b_max, dtype=np.float32)) - torch.as_tensor(np.asarray(b_min, dtype=np.float32)))
     axis = (length.view(3) / resolution * torch.tensor([1.0, 1.0, -1.0])).to(device)
     return _unit_or_zero(-(grad[0].t() * axis))

@@ -1,7 +1,9 @@
 """What the demo's whole frame costs -- geometry, the normal image and the netC colour image (RTL/main.py:417-441) --
 eager against the captured frame step (pipeline.FrameGraph with netC and render_normals, FrameGraphRing at 1, 2 and 4
 lanes), with the features given and with both encoders (HG for netG, ResBlk for netC with netG's map as its prior).
-The geometry-only captured graph is timed beside them.  Workload: bench.py's synthetic person, 257^3 Seg3dLossless
+The geometry-only captured graph is timed beside them, and so is the captured frame whose normal image comes from the
+geometry net's analytic normals (render_normals="gradient": the tensor-core gradient, mp_surface_normals_async) instead
+of forward_vertices' finite differences.  Workload: bench.py's synthetic person, 257^3 Seg3dLossless
 (faster=True), a seeded netC head on a 512-channel map.
 
     python tools/colour_frame_bench.py [--rounds 3] [--window 1.0]
@@ -29,7 +31,7 @@ def main():
     from monoport_b200.engine import Seg3dLossless, make_query_func
     from monoport_b200.modeling import PIFuNetC, PIFuNetG
     from monoport_b200.pipeline import FrameGraph, FrameGraphRing
-    from monoport_b200.recon import colorization, forward_vertices
+    from monoport_b200.recon import colorization, forward_vertices, surface_normals
 
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(dev)
@@ -90,6 +92,9 @@ def main():
             rings["graph + normals + colour, %s, %d lane(s)" % ("encoders" if enc else "features given", lanes)] = (FrameGraphRing(
                 lambda: FrameGraph(net, eng, cal, "front", with_encoder=enc, feature_hook=hook if enc else None, netC=netC,
                                    render_normals=True), n_lanes=lanes), (lambda e: lambda n: items(e, n))(enc))
+        rings["graph + analytic normals + colour, features given, %d lane(s)" % lanes] = (FrameGraphRing(
+            lambda: FrameGraph(net, eng, cal, "front", with_encoder=False, netC=netC, render_normals="gradient"),
+            n_lanes=lanes), lambda n: items(False, n))
 
     # ---- the outputs first: the captured frames equal the eager chain (features given: bit for bit; encoders: the set
     # pixels, and the values to the encoders' float noise under capture)
@@ -106,6 +111,13 @@ def main():
                     set_g, set_e = (out[6] != 1.0).any(-1), (rt != 1.0).any(-1)
                     print("encoders, %d lane(s), frame %d: %d / %d colour pixels set in both, max|graph - eager| %.2e"
                           % (lanes, i, int((set_g & set_e).sum()), int(set_e.sum()), (out[6] - rt)[set_g & set_e].abs().max().item()))
+    for lanes in (1, 2, 4):
+        ring, _ = rings["graph + analytic normals + colour, features given, %d lane(s)" % lanes]
+        for i, out in enumerate(ring.run(items(False, 4))):
+            sdf = eng(im_feat_list=[[feats[i % 4]]], calib_tensor=cal)
+            X, Y, Z, _ = forward_vertices(sdf, "front")
+            nrm = surface_normals(net, [[feats[i % 4]]], X, Y, Z, calg, resolution=R, precision="auto")
+            assert torch.equal(out[5], colorization(None, None, X, Y, Z, calg, norm=nrm, resolution=R)), "analytic normal image differs"
     print("outputs checked: the captured frames equal the eager chain")
 
     # ---- timing: warm-up, then alternating windows of at least args.window seconds

@@ -3,6 +3,9 @@
 For the geometry head (256-channel maps) and the colour head (512-channel maps) on 128 x 128 features, N in {10^4, 10^5,
 10^6} random points seen by the demo camera, in one call:
   grad      MonoPortNet.query_gradient (value + gradient, one launch of the fp32 gradient kernel)
+  grad-tc   MonoPortNet.query_gradient with precision "tc" (the tensor-core program's forward-mode derivative; its
+            per-frame texel products are rebuilt every call).  grad and grad-tc are timed twice, alternated, and the
+            faster round of each is reported
   fp32      query() with precision "fp32" (the forward half alone, the same CUDA-core arithmetic)
   tc        query() with precision "tc" (the tensor-core program; its per-frame texel products are rebuilt every call)
   autograd  a PyTorch restatement in this file: grid_sample + matmuls + autograd on the GPU, fp32
@@ -84,6 +87,9 @@ def main():
             def grad():
                 res["grad"] = net.query_gradient(feats, pts, calibs=cal)
 
+            def grad_tc():
+                res["grad_tc"] = net.query_gradient(feats, pts, calibs=cal, precision="tc")
+
             def fp32():
                 net.precision = "fp32"
                 net.query(feats, pts, calibs=cal)
@@ -99,6 +105,10 @@ def main():
                  "autograd": timed(autograd, args.reps, args.warmup)}
             if tc_ok:
                 t["tc"] = timed(tc, args.reps, args.warmup)
+                t["grad_tc"] = timed(grad_tc, args.reps, args.warmup)
+                g2 = timed(grad, args.reps, args.warmup)
+                t["grad"] = min(t["grad"], g2)
+                t["grad_tc"] = min(t["grad_tc"], timed(grad_tc, args.reps, args.warmup))
             ref = res["autograd"][1]
             err = (res["grad"][1][0] - ref).abs() / ref.abs().max()
             rel = err.max().item()
@@ -114,6 +124,12 @@ def main():
             line["autograd_over_grad"] = round(t["autograd"][0] / t["grad"][0], 3)
             line["max_rel_diff_vs_autograd"] = rel
             line["frac_within_2e-5_of_max_vs_autograd"] = round(frac, 6)
+            if tc_ok:
+                line["grad_tc_mpts_s"] = round(N / t["grad_tc"][0] / 1e3, 2)
+                line["grad_tc_speedup_over_grad"] = round(t["grad"][0] / t["grad_tc"][0], 2)
+                etc = (res["grad_tc"][1][0] - ref).abs() / ref.abs().max()
+                line["grad_tc_rel_diff_vs_autograd_median_p99_max"] = [etc.median().item(), etc.quantile(0.99).item()
+                                                                       if etc.numel() <= 1 << 24 else None, etc.max().item()]
             print(json.dumps(line), flush=True)
             del res
             torch.cuda.empty_cache()
