@@ -23,6 +23,8 @@
 // producer gives its registers to the consumers (setmaxnreg: 40 and 232 per thread).  The MMAs run asynchronously: the
 // role branches are warp-uniform by construction and the consumers wait for their MMAs at fixed points of a static
 // schedule (see the ring below), so layer-0 chunk c+1 is generated while the MMAs of chunk c are in flight.
+// query_wg_kernel and query_jvp_kernel (the point gradient, forward mode) share that producer, ring and trunk of layers
+// 1-3 (run_trunk); each passes in its own layer-0 chunks, hidden-layer epilogue and layer 4.
 #include "mp_common.cuh"
 #include "tc_ptx.cuh"
 #include <stdlib.h>
@@ -66,6 +68,9 @@ template <int C> struct Prog {
   static constexpr int Small = Wr + Ring * kStageBytes;       // zf[64], inimg[64], s4[RES][64]
   static constexpr int Bars = Small + (2 + RES) * kTile * 4;  // full[Slots], empty[Slots]
   static constexpr int Total = Bars + 2 * Slots * 8;
+  // slot of a tile's stage: layer 1 stage s -> s % Slots; step k of layers 2 and 3 (counted across both) -> 2 + k % Ring
+  __host__ __device__ static constexpr uint32_t l1_slot(uint32_t s) { return s % (uint32_t)Slots; }
+  __host__ __device__ static constexpr uint32_t l23_slot(uint32_t k) { return 2u + k % (uint32_t)Ring; }
 };
 static_assert(Prog<256>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
 static_assert(Prog<512>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
@@ -212,12 +217,194 @@ __device__ __forceinline__ uint32_t act_pack(float a, float b) {
   return *reinterpret_cast<const uint32_t*>(&r);
 }
 
+__device__ __forceinline__ void sync_consumers() { tc::bar_sync(1, kConsumers); }
+
 // ====================================================================================================================
-// The fused query program.  Register fragment of a 64 x N accumulator (wgmma m64nNk16, f32): thread t of the warpgroup
-// (warp wl = t/32, lane l) holds d[4j + e] = D[16 wl + l/4 + 8 (e>>1)][8 j + 2 (l%4) + (e&1)].
+// The weight ring and the trunk (layers 1-3) of the program, shared by query_wg_kernel and query_jvp_kernel: the same
+// stream, slots, wait schedule and MMAs, so the JVP's value rows are the query's rows bit for bit.
 // Hand-offs: every consumer takes EVERY stage of the stream (waits for it), uses the ones that carry its rows and
 // releases a stage once the MMAs that read it have completed (one arrival per consumer warp); the operand buffers written
 // by the consumers themselves are published with fence.proxy.async + a named barrier over the 256 consumer threads.
+
+// the ring's barriers (one thread): full[q] completes with the bulk copy into slot q, empty[q] with the release of slot q
+// by all 8 consumer warps
+template <int C>
+__device__ __forceinline__ void ring_init(uint64_t* full, uint64_t* empty) {
+  for (int s = 0; s < Prog<C>::Slots; ++s) {
+    tc::mbar_init(full + s, 1);
+    tc::mbar_init(empty + s, kConsumers / 32);
+  }
+  tc::fence_barrier_init();
+}
+
+// the producer thread: the weight stream of one tile into the ring.  phase: bit q is the parity of slot q's next refill.
+template <int C>
+__device__ __forceinline__ void produce_tile(uint8_t* smem, uint64_t* full, uint64_t* empty, const uint8_t* wsrc, uint32_t& phase) {
+  using P = Prog<C>;
+  for (int s = 0; s < P::StagesPerTile; ++s) {
+    const uint32_t slot = s < P::StagesL1 ? P::l1_slot(s) : P::l23_slot(s - P::StagesL1);
+    tc::mbar_wait(empty + slot, ((phase >> slot) & 1u) ^ 1u);
+    phase ^= 1u << slot;
+    tc::mbar_arrive_expect_tx(full + slot, kStageBytes);
+    tc::bulk_g2s(smem + P::H1 + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
+  }
+}
+
+// The consumers' part of one tile: layers 1-3 on the tile's 64 A-operand rows, from X (at P::X) and layer-0 chunk 0 (in the
+// first chunk buffer at P::H0), both written and published by the caller.  Register fragment of a 64 x N accumulator
+// (wgmma m64nNk16, f32): thread t of the warpgroup (warp wl = t/32, lane l) holds d[4j + e] = D[16 wl + l/4 + 8 (e>>1)][8 j
+// + 2 (l%4) + (e&1)].  The kernel passes in what differs between its programs:
+//   gen_chunk(c)   layer-0 chunk c (two K-blocks) into chunk buffer c & 1, fenced for the async proxy;
+//   epi(acc, side, col0, dst)   a hidden layer's epilogue: this warpgroup's outputs col0 .. (acc[128]: layer 1's 256, acc[64]:
+//                               layer 2's 128; bias and depth column at side) -> the fp16 K-major operand at shared offset dst;
+//   head(acc[32])  its 64 layer-3 outputs -> layer 4 and the stores (H1 is dead by then: scratch for the partial sums).
+// fphase: bit q is the parity of slot q's next fill, kept across the tiles of the CTA.
+template <int C, class GenChunk, class Epi, class Head>
+__device__ __forceinline__ void run_trunk(uint8_t* smem, uint64_t* full, uint64_t* empty, uint32_t& fphase, int lane, int wg,
+                                          GenChunk&& gen_chunk, Epi&& epi, Head&& head) {
+  using P = Prog<C>;
+  constexpr int Ring = P::Ring, XKB = P::XKB;
+  const uint32_t smem_base = tc::smem_u32(smem);
+  auto desc = [&](int off) { return tc::make_wdesc_sw128(smem_base + (uint32_t)off, 1024); };
+
+  // ---- the weight ring, consumer side.  Every consumer takes every stage of a tile (56 for the geometry head, 76 for the
+  // colour head) in a fixed order, so which stages a warpgroup still has in flight at any point is known at compile time:
+  // each wait below is a fixed wgmma_wait<N> and each release names its stage by arithmetic on its index in the tile.
+  // No stage is ever queued at run time; the parity of each slot's next fill is one bit per slot (fphase), flipped by
+  // every take, as the producer flips its own bit per refill.
+  // Layer 1 streams through Slots = Ring + 2 slots (H1's halves are slots 0 and 1), layers 2 and 3 through the Ring slots
+  // 2 .. Slots-1: the deeper ring lets the producer run one more K-block ahead in layer 1, where each warpgroup waits for
+  // its K-block's MMAs before it takes the next.  H1's slots are refilled with the next tile's stages 0 and 1 only once
+  // H1 is dead: their last layer-1 stages (Defer, Defer + 1) are released at the end of the tile, and the layer-1
+  // epilogue writes H1 only after both warpgroups retired every MMA that read those slots.
+  // Deadlock freedom: the producer refills a slot with stage s once all 8 consumer warps have released the stage that last
+  // used it, so every consumer must have released that stage before it waits for s.  Where that release needs the
+  // stage's MMAs complete, the wait for them comes first:
+  //   layer 1 (two stages per K-block i: 2i carries output half 0 for warpgroup 0, 2i+1 half 1 for warpgroup 1; each
+  //     warpgroup releases the other's stage right after taking it and its own once the K-block's MMAs completed):
+  //     taking 2i+1 needs 2i+1-Slots <= 2i-3, which both warpgroups released by the end of K-block i-1's takes (its
+  //     owner after its wait<0> there); taking 2i needs 2i-Slots, released a K-block earlier still.  The deferred stages
+  //     are last users of slots 0 and 1, whose next stages are the next tile's 0 and 1;
+  //   layers 2 and 3 (one stage per K-block step, read by both warpgroups): taking step k needs k - Ring (for k < Ring a
+  //     layer-1 stage of slot 2 + k, released in layer 1), so before it the warpgroup lets at most Ring - 1 groups stay
+  //     in flight (wait<Ring-1>) and releases k - Ring.
+  // Every layer ends with wait<0> and releases its own stages still held, so a layer starts with nothing in flight.
+  constexpr uint32_t Defer = P::StagesL1 - P::Slots;
+  auto release_if = [&](uint32_t slot, bool pred) {
+    __syncwarp();
+    tc::mbar_arrive_if(empty + slot, pred && lane == 0);
+  };
+  auto release = [&](uint32_t slot) { release_if(slot, true); };
+  auto l1_release = [&](uint32_t s) { release_if(P::l1_slot(s), s - Defer >= 2u); };
+  auto take = [&](uint32_t slot) {
+    tc::mbar_wait(full + slot, (fphase >> slot) & 1u);
+    fphase ^= 1u << slot;
+  };
+  auto slot_off = [&](uint32_t slot) { return P::H1 + (int)slot * kStageBytes; };
+  // layer 1, K-block i (A operand at shared offset a_off): this warpgroup's 256 outputs times its stage 2i + wg
+  auto l1_kblock = [&](float (&acc)[128], int i, int a_off) {
+    const uint32_t s0 = 2 * i, mine = s0 + wg, prev = mine - 2;
+    take(P::l1_slot(s0));
+    tc::wgmma_wait<0>();
+    if (i > 0) l1_release(prev);
+    take(P::l1_slot(s0 + 1));
+    l1_release(s0 + 1 - wg);                         // the other warpgroup's half
+    const uint64_t da = desc(a_off), db = desc(slot_off(P::l1_slot(mine)));
+    tc::wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
+    tc::wgmma_commit();
+  };
+  // layers 2 and 3, step k of a layer whose steps start at k_layer: frees the slot of step k (see above) and takes it
+  auto step_take = [&](uint32_t k_layer, int k) {
+    if (k >= Ring) {
+      tc::wgmma_wait<Ring - 1>();
+      release(P::l23_slot(k_layer + k - Ring));
+    }
+    take(P::l23_slot(k_layer + k));
+    tc::wgmma_fence();
+  };
+  // end of a layer of n steps (n >= Ring): all MMAs complete, the last Ring stages released
+  auto layer_end = [&](uint32_t k_layer, int n) {
+    tc::wgmma_wait<0>();
+#pragma unroll
+    for (int j = Ring; j > 0; --j) release(P::l23_slot(k_layer + n - j));
+  };
+
+  // ---- layer 1: 8 sampled layer-0 chunks (2 K-blocks each), then X; this warpgroup's 256 of the 512 outputs
+  {
+    float acc[128];
+#pragma unroll
+    for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+#pragma unroll 1
+    for (int c = 0; c < 8; ++c) {
+#pragma unroll
+      for (int kb = 0; kb < 2; ++kb) l1_kblock(acc, 2 * c + kb, P::H0 + ((c & 1) * 2 + kb) * kKb);
+      if (c < 7) {
+        // the other chunk buffer was last read by chunk c-1, whose MMAs completed before chunk c's second K-block was
+        // issued (in both warpgroups once they meet here); chunk c's second K-block stays in flight meanwhile
+        sync_consumers();
+        gen_chunk(c + 1);
+        sync_consumers();
+      }
+    }
+#pragma unroll 1
+    for (int kb = 0; kb < XKB; ++kb) l1_kblock(acc, 16 + kb, P::X + kb * kKb);
+    tc::wgmma_wait<0>();
+    l1_release(2 * (16 + XKB - 1) + wg);
+    sync_consumers();        // H1 was ring slots 0 and 1: every MMA that read them has retired in both warpgroups
+    epi(acc, side_off(1), wg * 256, P::H1);
+    tc::fence_proxy_async_smem();
+    sync_consumers();
+  }
+  // ---- layer 2: H1 (8 K-blocks), then X; this warpgroup's 128 of the 256 outputs -> H2 (over the chunk buffers)
+  {
+    float acc[64];
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+#pragma unroll 1
+    for (int kb = 0; kb < P::StagesL2; ++kb) {
+      step_take(0, kb);
+      const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(slot_off(P::l23_slot(kb)) + wg * 16384);
+#pragma unroll
+      for (int k = 0; k < 4; ++k) tc::wgmma_m64n128(acc, da + 2 * k, db + 2 * k);
+      tc::wgmma_commit();
+    }
+    layer_end(0, P::StagesL2);
+    epi(acc, side_off(2), wg * 128, P::H0);
+    tc::fence_proxy_async_smem();
+    sync_consumers();
+  }
+  // ---- layer 3: X, then H2 (two K-blocks per stage; colour: hi then lo pass); 64 of the 128 outputs
+  {
+    float acc[32];
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+#pragma unroll 1
+    for (int q = 0; q < P::StagesL3; ++q) {
+      step_take(P::StagesL2, q);
+#pragma unroll
+      for (int sub = 0; sub < 2; ++sub) {
+        const int kb = (2 * q + sub) % (XKB + 4);
+        const uint64_t da = desc(kb < XKB ? P::X + kb * kKb : P::H0 + (kb - XKB) * kKb);
+        const uint64_t db = desc(slot_off(P::l23_slot(P::StagesL2 + q)) + sub * 16384 + wg * 8192);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) tc::wgmma_m64n64(acc, da + 2 * k, db + 2 * k);
+      }
+      tc::wgmma_commit();
+    }
+    layer_end(P::StagesL2, P::StagesL3);
+    head(acc);
+  }
+  sync_consumers();        // the per-point scalars and X are rewritten by the next tile
+  // H1 (the layer-2 operand, then the partial sums) is dead: its slots may take the next tile's first stages
+  tc::fence_proxy_async_smem();
+  release(P::l1_slot(Defer));
+  release(P::l1_slot(Defer + 1));
+}
+
+// ====================================================================================================================
+// The fused query program: the trunk above, with the layer-0 chunks sampled from G0, the hidden epilogues and layer 4.
 // PEERS: also store channel 0 into the peer volumes of dst (fused slab exchange).
 // bt.B images of src.n points (more than one: MP_SRC_ROWS, [R,N] outputs); tile t is tile t % n_tiles of image t / n_tiles,
 // and the range guard skips the tiles of the images outside the head's range -- the producer and the consumers skip
@@ -226,7 +413,7 @@ template <int C, bool PEERS>
 __global__ void __launch_bounds__(kThreads, 1)
 query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpSurfaceSrc surf, MpBatch bt) {
   using P = Prog<C>;
-  constexpr int RES = P::RES, Ring = P::Ring, XKB = P::XKB;
+  constexpr int RES = P::RES;
   MP_DYN_SMEM(uint8_t, smem_raw);
   // aligned by an offset from the shared array itself (not through an integer cast), so the compiler keeps knowing that
   // every pointer below is a shared-memory pointer: 32-bit addresses and st.shared instead of 64-bit generic ones
@@ -261,26 +448,17 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   // consumer warps take lane 0's answer)
   auto image_skipped = [&](int b) { return mp_guard_skips(prm.amax + b, prm.amax_limit, prm.guard); };
 
-  if (tid == 0) {
-    for (int s = 0; s < P::Slots; ++s) {
-      tc::mbar_init(full + s, 1);
-      tc::mbar_init(empty + s, kConsumers / 32);
-    }
-    tc::fence_barrier_init();
-  }
+  if (tid == 0) ring_init<C>(full, empty);
   __syncthreads();
-  // slot of a tile's stage: layer 1 stage s -> s % Slots; step k of layers 2 and 3 (counted across both) -> 2 + k % Ring
-  auto l1_slot = [](uint32_t s) { return s % (uint32_t)P::Slots; };
-  auto l23_slot = [](uint32_t k) { return 2u + k % (uint32_t)Ring; };
 
   if (wg == 2) {
     // ============================== weight producer ==============================
     tc::setmaxnreg_dec<kProducerRegs>();
     if (warp == 8 && lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
-      uint32_t phase = 0;                  // bit q: parity of slot q's next refill
-      int guard_b = -1;
+      uint32_t phase = 0;
       bool skip = false;
+      int guard_b = -1;
       for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
         const int b = mp_tile_image(bt, t, n_tiles);
         if (b != guard_b) {
@@ -291,13 +469,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
           t = mp_skip_image(bt, t, b, n_tiles);
           continue;
         }
-        for (int s = 0; s < P::StagesPerTile; ++s) {
-          const uint32_t slot = s < P::StagesL1 ? l1_slot(s) : l23_slot(s - P::StagesL1);
-          tc::mbar_wait(empty + slot, ((phase >> slot) & 1u) ^ 1u);
-          phase ^= 1u << slot;
-          tc::mbar_arrive_expect_tx(full + slot, kStageBytes);
-          tc::bulk_g2s(smem + P::H1 + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
-        }
+        produce_tile<C>(smem, full, empty, wsrc, phase);
       }
     }
     return;
@@ -307,74 +479,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   tc::setmaxnreg_inc<kConsumerRegs>();
   const int wl = warp & 3;
   const int r0 = 16 * wl + (lane >> 2), cq = 2 * (lane & 3);
-  const uint32_t smem_base = tc::smem_u32(smem);
-  auto desc = [&](int off) { return tc::make_wdesc_sw128(smem_base + (uint32_t)off, 1024); };
-  auto sync_consumers = [&]() { tc::bar_sync(1, kConsumers); };
-
-  // ---- the weight ring, consumer side.  Every consumer takes every stage of a tile (56 for the geometry head, 76 for the
-  // colour head) in a fixed order, so which stages a warpgroup still has in flight at any point is known at compile time:
-  // each wait below is a fixed wgmma_wait<N> and each release names its stage by arithmetic on its index in the tile.
-  // No stage is ever queued at run time; the parity of each slot's next fill is one bit per slot (fphase), flipped by
-  // every take, as the producer flips its own bit per refill.
-  // Layer 1 streams through Slots = Ring + 2 slots (H1's halves are slots 0 and 1), layers 2 and 3 through the Ring slots
-  // 2 .. Slots-1: the deeper ring lets the producer run one more K-block ahead in layer 1, where each warpgroup waits for
-  // its K-block's MMAs before it takes the next.  H1's slots are refilled with the next tile's stages 0 and 1 only once
-  // H1 is dead: their last layer-1 stages (Defer, Defer + 1) are released at the end of the tile, and the layer-1
-  // epilogue writes H1 only after both warpgroups retired every MMA that read those slots.
-  // Deadlock freedom: the producer refills a slot with stage s once all 8 consumer warps have released the stage that last
-  // used it, so every consumer must have released that stage before it waits for s.  Where that release needs the
-  // stage's MMAs complete, the wait for them comes first:
-  //   layer 1 (two stages per K-block i: 2i carries output half 0 for warpgroup 0, 2i+1 half 1 for warpgroup 1; each
-  //     warpgroup releases the other's stage right after taking it and its own once the K-block's MMAs completed):
-  //     taking 2i+1 needs 2i+1-Slots <= 2i-3, which both warpgroups released by the end of K-block i-1's takes (its
-  //     owner after its wait<0> there); taking 2i needs 2i-Slots, released a K-block earlier still.  The deferred stages
-  //     are last users of slots 0 and 1, whose next stages are the next tile's 0 and 1;
-  //   layers 2 and 3 (one stage per K-block step, read by both warpgroups): taking step k needs k - Ring (for k < Ring a
-  //     layer-1 stage of slot 2 + k, released in layer 1), so before it the warpgroup lets at most Ring - 1 groups stay
-  //     in flight (wait<Ring-1>) and releases k - Ring.
-  // Every layer ends with wait<0> and releases its own stages still held, so a layer starts with nothing in flight.
-  constexpr uint32_t Defer = P::StagesL1 - P::Slots;
   uint32_t fphase = 0;
-  auto release_if = [&](uint32_t slot, bool pred) {
-    __syncwarp();
-    tc::mbar_arrive_if(empty + slot, pred && lane == 0);
-  };
-  auto release = [&](uint32_t slot) { release_if(slot, true); };
-  auto l1_release = [&](uint32_t s) { release_if(l1_slot(s), s - Defer >= 2u); };
-  auto take = [&](uint32_t slot) {
-    tc::mbar_wait(full + slot, (fphase >> slot) & 1u);
-    fphase ^= 1u << slot;
-  };
-  auto slot_off = [&](uint32_t slot) { return P::H1 + (int)slot * kStageBytes; };
-  // layer 1, K-block i (A operand at shared offset a_off): this warpgroup's 256 outputs times its stage 2i + wg
-  auto l1_kblock = [&](float (&acc)[128], int i, int a_off) {
-    const uint32_t s0 = 2 * i, mine = s0 + wg, prev = mine - 2;
-    take(l1_slot(s0));
-    tc::wgmma_wait<0>();
-    if (i > 0) l1_release(prev);
-    take(l1_slot(s0 + 1));
-    l1_release(s0 + 1 - wg);                         // the other warpgroup's half
-    const uint64_t da = desc(a_off), db = desc(slot_off(l1_slot(mine)));
-    tc::wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
-    tc::wgmma_commit();
-  };
-  // layers 2 and 3, step k of a layer whose steps start at k_layer: frees the slot of step k (see above) and takes it
-  auto step_take = [&](uint32_t k_layer, int k) {
-    if (k >= Ring) {
-      tc::wgmma_wait<Ring - 1>();
-      release(l23_slot(k_layer + k - Ring));
-    }
-    take(l23_slot(k_layer + k));
-    tc::wgmma_fence();
-  };
-  // end of a layer of n steps (n >= Ring): all MMAs complete, the last Ring stages released
-  auto layer_end = [&](uint32_t k_layer, int n) {
-    tc::wgmma_wait<0>();
-#pragma unroll
-    for (int j = Ring; j > 0; --j) release(l23_slot(k_layer + n - j));
-  };
 
   // ---- taps of this warp's 8 points for the layer-0 chunks: lane = (point 4 i + qw, channels 8 l8 .. and 64 + 8 l8 ..)
   const int l8 = lane & 7, qw = lane >> 3;
@@ -473,90 +578,22 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
     sync_consumers();
     const float zf0 = s_zf[r0], zf1 = s_zf[r0 + 8];
 
-    // ---- layer 1: 8 sampled layer-0 chunks (2 K-blocks each), then X; this warpgroup's 256 of the 512 outputs
-    {
-      float acc[128];
+    // hidden epilogue: + bias + w_z z, leaky ReLU -> fp16, K-major
+    auto epi = [&](const auto& acc, int side, int col0, int dst) {
 #pragma unroll
-      for (int j = 0; j < 128; ++j) acc[j] = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < 8; ++c) {
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb) l1_kblock(acc, 2 * c + kb, P::H0 + ((c & 1) * 2 + kb) * kKb);
-        if (c < 7) {
-          // the other chunk buffer was last read by chunk c-1, whose MMAs completed before chunk c's second K-block was
-          // issued (in both warpgroups once they meet here); chunk c's second K-block stays in flight meanwhile
-          sync_consumers();
-          gen_chunk(c + 1);
-          sync_consumers();
-        }
-      }
-#pragma unroll 1
-      for (int kb = 0; kb < XKB; ++kb) l1_kblock(acc, 16 + kb, P::X + kb * kKb);
-      tc::wgmma_wait<0>();
-      l1_release(2 * (16 + XKB - 1) + wg);
-      sync_consumers();        // H1 was ring slots 0 and 1: every MMA that read them has retired in both warpgroups
-      // epilogue -> H1 (fp16, K-major): + bias + w_z z, leaky ReLU
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const int col = wg * 256 + 8 * j + cq;
-        const float b0 = prm.bias_all[side_off(1) + col], b1 = prm.bias_all[side_off(1) + col + 1];
-        const float z0 = prm.wz_all[side_off(1) + col], z1 = prm.wz_all[side_off(1) + col + 1];
-        uint8_t* kbp = smem + P::H1 + (col >> 6) * kKb;
+      for (int j = 0; j < (int)(sizeof(acc) / sizeof(acc[0])) / 4; ++j) {
+        const int col = col0 + 8 * j + cq;
+        const float b0 = prm.bias_all[side + col], b1 = prm.bias_all[side + col + 1];
+        const float z0 = prm.wz_all[side + col], z1 = prm.wz_all[side + col + 1];
+        uint8_t* kbp = smem + dst + (col >> 6) * kKb;
         *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0, col & 63)) =
             act_pack(acc[4 * j + 0] + fmaf(z0, zf0, b0), acc[4 * j + 1] + fmaf(z1, zf0, b1));
         *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0 + 8, col & 63)) =
             act_pack(acc[4 * j + 2] + fmaf(z0, zf1, b0), acc[4 * j + 3] + fmaf(z1, zf1, b1));
       }
-      tc::fence_proxy_async_smem();
-      sync_consumers();
-    }
-    // ---- layer 2: H1 (8 K-blocks), then X; this warpgroup's 128 of the 256 outputs -> H2 (over the chunk buffers)
-    {
-      float acc[64];
-#pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-#pragma unroll 1
-      for (int kb = 0; kb < P::StagesL2; ++kb) {
-        step_take(0, kb);
-        const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(slot_off(l23_slot(kb)) + wg * 16384);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::wgmma_m64n128(acc, da + 2 * k, db + 2 * k);
-        tc::wgmma_commit();
-      }
-      layer_end(0, P::StagesL2);
-#pragma unroll
-      for (int j = 0; j < 16; ++j) {
-        const int col = wg * 128 + 8 * j + cq;
-        const float b0 = prm.bias_all[side_off(2) + col], b1 = prm.bias_all[side_off(2) + col + 1];
-        const float z0 = prm.wz_all[side_off(2) + col], z1 = prm.wz_all[side_off(2) + col + 1];
-        uint8_t* kbp = smem + P::H0 + (col >> 6) * kKb;
-        *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0, col & 63)) =
-            act_pack(acc[4 * j + 0] + fmaf(z0, zf0, b0), acc[4 * j + 1] + fmaf(z1, zf0, b1));
-        *reinterpret_cast<uint32_t*>(kbp + tc::sw128_offset(r0 + 8, col & 63)) =
-            act_pack(acc[4 * j + 2] + fmaf(z0, zf1, b0), acc[4 * j + 3] + fmaf(z1, zf1, b1));
-      }
-      tc::fence_proxy_async_smem();
-      sync_consumers();
-    }
-    // ---- layer 3: X, then H2 (two K-blocks per stage; colour: hi then lo pass); 64 of the 128 outputs; layer 4 in fp32
-    {
-      float acc[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-#pragma unroll 1
-      for (int q = 0; q < P::StagesL3; ++q) {
-        step_take(P::StagesL2, q);
-#pragma unroll
-        for (int sub = 0; sub < 2; ++sub) {
-          const int kb = (2 * q + sub) % (XKB + 4);
-          const uint64_t da = desc(kb < XKB ? P::X + kb * kKb : P::H0 + (kb - XKB) * kKb);
-          const uint64_t db = desc(slot_off(l23_slot(P::StagesL2 + q)) + sub * 16384 + wg * 8192);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::wgmma_m64n64(acc, da + 2 * k, db + 2 * k);
-        }
-        tc::wgmma_commit();
-      }
-      layer_end(P::StagesL2, P::StagesL3);
+    };
+    // layer 4 in fp32 and the stores
+    auto head = [&](const float (&acc)[32]) {
       float lg[2][RES];
 #pragma unroll
       for (int h = 0; h < 2; ++h)
@@ -613,12 +650,8 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
           }
         }
       }
-      sync_consumers();        // the per-point scalars and X are rewritten by the next tile
-      // H1 (the layer-2 operand, then the partial sums) is dead: its slots may take the next tile's first stages
-      tc::fence_proxy_async_smem();
-      release(l1_slot(Defer));
-      release(l1_slot(Defer + 1));
-    }
+    };
+    run_trunk<C>(smem, full, empty, fphase, lane, wg, gen_chunk, epi, head);
   }
 }
 
@@ -626,8 +659,9 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
 // F1‴: the gradient of the query program with respect to the points, forward mode (a JVP with three tangents).  The output
 // depends on a point only through its texel coordinates (ix, iy) and its depth feature zf, and a tangent goes through the
 // same weights as the value in the same order: so the tangents are three more rows of the A operand, and a tile of 64 rows
-// is 16 points x (value, d/dix, d/diy, d/dzf).  The weight stream, the ring, the wait schedule and every MMA are those of
-// query_wg_kernel; the value rows are its rows, bit for bit (same taps, same roundings, same layer-4 summation order).
+// is 16 points x (value, d/dix, d/diy, d/dzf).  It runs query_wg_kernel's trunk (run_trunk: the weight stream, the ring,
+// the wait schedule and every MMA) with its own operands and epilogues; the value rows are the query's rows, bit for bit
+// (same taps, same roundings, same layer-4 summation order).
 // Row map (jvp_row): point k (0..15) of the tile has its value on row 16 (k/4) + k%4, d/dix 8 rows below, d/diy 4 rows
 // below, d/dzf 12 rows below -- in the accumulator fragment, lanes 0-15 of warp k/4 hold (value, d/dix) and lanes 16-31
 // the same columns of (d/diy, d/dzf), so a value's leaky-ReLU branch reaches its tangents as packed sign bits through one
@@ -694,16 +728,16 @@ __device__ __forceinline__ JvpTaps jvp_taps(const MpPointSrc& src, const MpCalib
   return j;
 }
 
-// epilogue of hidden layer 1 or 2 (side = its side_off): this lane's NJ x 2 columns (from col0 + cq) of rows r0 and r0 + 8
+// epilogue of hidden layer 1 or 2 (side = its side_off): this lane's N / 4 column pairs (from col0 + cq) of rows r0 and r0 + 8
 // -> the fp16 K-major operand at buf.  isv: the lane holds (value, d/dix) rows, else (d/diy, d/dzf).  Column pair by column
 // pair, so that each accumulator dies at its first use (the value's signs cross to lanes 16-31 as two bits per pair).
 // zt: the depth feature's tangent on row r0 + 8 (0: d/dix, 1: d/dzf), a multiplier rather than a select, so that no
 // per-lane product of the weights is hoisted out of the tile loop.
-template <int NJ>
-__device__ __forceinline__ void jvp_hidden_epilogue(const TcParams& prm, const float (&acc)[4 * NJ], int side, int col0, uint8_t* buf,
+template <int N>
+__device__ __forceinline__ void jvp_hidden_epilogue(const TcParams& prm, const float (&acc)[N], int side, int col0, uint8_t* buf,
                                                     int r0, int cq, float zf, bool isv, float zt) {
 #pragma unroll
-  for (int j = 0; j < NJ; ++j) {
+  for (int j = 0; j < N / 4; ++j) {
     const int col = col0 + 8 * j + cq;
     const float z0 = prm.wz_all[side + col], z1 = prm.wz_all[side + col + 1];
     uint8_t* kbp = buf + (col >> 6) * kKb;
@@ -726,7 +760,7 @@ template <int C>
 __global__ void __launch_bounds__(kThreads, 1)
 query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, JvpOut jo) {
   using P = Prog<C>;
-  constexpr int RES = P::RES, Ring = P::Ring, XKB = P::XKB, NP = kJvpPts;
+  constexpr int RES = P::RES, NP = kJvpPts;
   static_assert((5 + 3 * RES) * NP <= (2 + RES) * kTile, "per-point scalars of a JVP tile fit the Small block");
   MP_DYN_SMEM(uint8_t, smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -748,85 +782,28 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
   const int skip = __shfl_sync(0xffffffffu, (int)mp_guard_skips(prm.amax, prm.amax_limit, prm.guard), 0);
   const long long n_tiles = skip ? 0 : (n + NP - 1) / NP;
 
-  if (tid == 0) {
-    for (int s = 0; s < P::Slots; ++s) {
-      tc::mbar_init(full + s, 1);
-      tc::mbar_init(empty + s, kConsumers / 32);
-    }
-    tc::fence_barrier_init();
-  }
+  if (tid == 0) ring_init<C>(full, empty);
   __syncthreads();
-  auto l1_slot = [](uint32_t s) { return s % (uint32_t)P::Slots; };
-  auto l23_slot = [](uint32_t k) { return 2u + k % (uint32_t)Ring; };
 
   if (wg == 2) {
-    // ============================== weight producer (query_wg_kernel's) ==============================
+    // ============================== weight producer ==============================
     tc::setmaxnreg_dec<kProducerRegs>();
     if (warp == 8 && lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
       uint32_t phase = 0;
-      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-        for (int s = 0; s < P::StagesPerTile; ++s) {
-          const uint32_t slot = s < P::StagesL1 ? l1_slot(s) : l23_slot(s - P::StagesL1);
-          tc::mbar_wait(empty + slot, ((phase >> slot) & 1u) ^ 1u);
-          phase ^= 1u << slot;
-          tc::mbar_arrive_expect_tx(full + slot, kStageBytes);
-          tc::bulk_g2s(smem + P::H1 + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
-        }
-      }
+      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) produce_tile<C>(smem, full, empty, wsrc, phase);
     }
     return;
   }
 
-  // ============================== consumers: query_wg_kernel's ring protocol ==============================
+  // ============================== consumers ==============================
   tc::setmaxnreg_inc<kConsumerRegs>();
   const int wl = warp & 3;
   const int r0 = 16 * wl + (lane >> 2), cq = 2 * (lane & 3);
   const bool isv = lane < 16;                         // rows r0, r0 + 8 hold (value, d/dix), else (d/diy, d/dzf)
   const int kpt = 4 * wl + ((lane >> 2) & 3);         // ... of point kpt
   const float zt = (float)(lane >> 4);                // the depth feature's tangent on row r0 + 8
-  const uint32_t smem_base = tc::smem_u32(smem);
-  auto desc = [&](int off) { return tc::make_wdesc_sw128(smem_base + (uint32_t)off, 1024); };
-  auto sync_consumers = [&]() { tc::bar_sync(1, kConsumers); };
-  constexpr uint32_t Defer = P::StagesL1 - P::Slots;
   uint32_t fphase = 0;
-  auto release_if = [&](uint32_t slot, bool pred) {
-    __syncwarp();
-    tc::mbar_arrive_if(empty + slot, pred && lane == 0);
-  };
-  auto release = [&](uint32_t slot) { release_if(slot, true); };
-  auto l1_release = [&](uint32_t s) { release_if(l1_slot(s), s - Defer >= 2u); };
-  auto take = [&](uint32_t slot) {
-    tc::mbar_wait(full + slot, (fphase >> slot) & 1u);
-    fphase ^= 1u << slot;
-  };
-  auto slot_off = [&](uint32_t slot) { return P::H1 + (int)slot * kStageBytes; };
-  auto l1_kblock = [&](float (&acc)[128], int i, int a_off) {
-    const uint32_t s0 = 2 * i, mine = s0 + wg, prev = mine - 2;
-    take(l1_slot(s0));
-    tc::wgmma_wait<0>();
-    if (i > 0) l1_release(prev);
-    take(l1_slot(s0 + 1));
-    l1_release(s0 + 1 - wg);
-    const uint64_t da = desc(a_off), db = desc(slot_off(l1_slot(mine)));
-    tc::wgmma_fence();
-#pragma unroll
-    for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
-    tc::wgmma_commit();
-  };
-  auto step_take = [&](uint32_t k_layer, int k) {
-    if (k >= Ring) {
-      tc::wgmma_wait<Ring - 1>();
-      release(l23_slot(k_layer + k - Ring));
-    }
-    take(l23_slot(k_layer + k));
-    tc::wgmma_fence();
-  };
-  auto layer_end = [&](uint32_t k_layer, int n_steps) {
-    tc::wgmma_wait<0>();
-#pragma unroll
-    for (int j = Ring; j > 0; --j) release(l23_slot(k_layer + n_steps - j));
-  };
 
   // ---- layer-0 chunks: lane = (point 2 warp + lane/16, K-block half (lane/8)%2, channels 8 (lane%8) ..), all four rows
   const int l8 = lane & 7, kbh = (lane >> 3) & 1, gq = 2 * warp + (lane >> 4);
@@ -976,67 +953,11 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
     int r0t = r0, cqt = cq;
     asm volatile("" : "+r"(r0t), "+r"(cqt));
 
-    // ---- layer 1 (query_wg_kernel's schedule)
-    {
-      float acc[128];
-#pragma unroll
-      for (int j = 0; j < 128; ++j) acc[j] = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < 8; ++c) {
-#pragma unroll
-        for (int kb = 0; kb < 2; ++kb) l1_kblock(acc, 2 * c + kb, P::H0 + ((c & 1) * 2 + kb) * kKb);
-        if (c < 7) {
-          sync_consumers();
-          gen_chunk(c + 1);
-          sync_consumers();
-        }
-      }
-#pragma unroll 1
-      for (int kb = 0; kb < XKB; ++kb) l1_kblock(acc, 16 + kb, P::X + kb * kKb);
-      tc::wgmma_wait<0>();
-      l1_release(2 * (16 + XKB - 1) + wg);
-      sync_consumers();
-      jvp_hidden_epilogue<32>(prm, acc, side_off(1), wg * 256, smem + P::H1, r0t, cqt, zf, isv, zt);
-      tc::fence_proxy_async_smem();
-      sync_consumers();
-    }
-    // ---- layer 2
-    {
-      float acc[64];
-#pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-#pragma unroll 1
-      for (int kb = 0; kb < P::StagesL2; ++kb) {
-        step_take(0, kb);
-        const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(slot_off(l23_slot(kb)) + wg * 16384);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) tc::wgmma_m64n128(acc, da + 2 * k, db + 2 * k);
-        tc::wgmma_commit();
-      }
-      layer_end(0, P::StagesL2);
-      jvp_hidden_epilogue<16>(prm, acc, side_off(2), wg * 128, smem + P::H0, r0t, cqt, zf, isv, zt);
-      tc::fence_proxy_async_smem();
-      sync_consumers();
-    }
-    // ---- layer 3, then layer 4 in fp32
-    {
-      float acc[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-#pragma unroll 1
-      for (int q = 0; q < P::StagesL3; ++q) {
-        step_take(P::StagesL2, q);
-#pragma unroll
-        for (int sub = 0; sub < 2; ++sub) {
-          const int kb = (2 * q + sub) % (XKB + 4);
-          const uint64_t da = desc(kb < XKB ? P::X + kb * kKb : P::H0 + (kb - XKB) * kKb);
-          const uint64_t db = desc(slot_off(l23_slot(P::StagesL2 + q)) + sub * 16384 + wg * 8192);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) tc::wgmma_m64n64(acc, da + 2 * k, db + 2 * k);
-        }
-        tc::wgmma_commit();
-      }
-      layer_end(P::StagesL2, P::StagesL3);
+    auto epi = [&](const auto& acc, int side, int col0, int dst) {
+      jvp_hidden_epilogue(prm, acc, side, col0, smem + dst, r0t, cqt, zf, isv, zt);
+    };
+    // layer 4 in fp32, the chain rule and the stores
+    auto head = [&](const float (&acc)[32]) {
       // row r0: the value's hidden dot exactly as query_wg_kernel sums it (lanes < 16), and the signs of its layer-3 outputs
       float lg[2][RES], lt[RES];
 #pragma unroll
@@ -1139,11 +1060,8 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
           for (int a = 0; a < 3; ++a) jo.dp[a * jo.ld_dp + i] = inimg != 0.f ? gp[a] : 0.f;     // outside the image: exactly 0
         }
       }
-      sync_consumers();
-      tc::fence_proxy_async_smem();
-      release(l1_slot(Defer));
-      release(l1_slot(Defer + 1));
-    }
+    };
+    run_trunk<C>(smem, full, empty, fphase, lane, wg, gen_chunk, epi, head);
   }
 }
 
@@ -1447,9 +1365,13 @@ int frame_products(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, cudaStrea
   return MP_OK;
 }
 
-// the kernel parameters of the head's program on the current frame of feat
-TcParams tc_params(const mp_mlp* mlp, const TcPack* pk, const mp_feat* feat, int guard) {
-  TcParams prm;
+// the per-frame products, the kernel parameters of the head's program on the current frame of feat and the persistent
+// grid (one CTA per SM, at most one per tile) of a launch over `tiles` tiles
+template <int C>
+int launch_setup(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, cudaStream_t st, int guard, long long tiles, TcParams& prm,
+                 int& grid) {
+  const int rp = frame_products<C>(mlp, pk, feat, st);
+  if (rp != MP_OK) return rp;
   memset(&prm, 0, sizeof(prm));
   prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
   prm.wstream = pk->wstream;
@@ -1464,7 +1386,11 @@ TcParams tc_params(const mp_mlp* mlp, const TcPack* pk, const mp_feat* feat, int
   prm.s4tex = feat->s4tex;
   prm.d_bias0 = pk->d_bias0;
   prm.d_wz0 = pk->d_wz0;
-  return prm;
+  int dev = 0, sms = 132;
+  MP_CUDA(cudaGetDevice(&dev));
+  MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  grid = (int)(tiles < (long long)sms ? tiles : sms);
+  return MP_OK;
 }
 
 // the per-frame products, then the fused query over the images of bt
@@ -1472,8 +1398,10 @@ template <int C>
 int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
            cudaStream_t st, const MpSurfaceSrc& surf, int guard, const MpBatch& bt) {
   using P = Prog<C>;
-  const int rp = frame_products<C>(mlp, pk, feat, st);
-  if (rp != MP_OK) return rp;
+  TcParams prm;
+  int grid = 0;
+  const int rs = launch_setup<C>(mlp, pk, feat, st, guard, bt.B * ((src.n + kTile - 1) / kTile), prm, grid);
+  if (rs != MP_OK) return rs;
   if (surf.X && guard == MP_GUARD_NONE && isfinite(mlp->tc_amax_limit)) {
     // the eager rendering (mp_colorize_surface): check the frame's feature range on the host (one 4-byte read-back per
     // frame) and let the caller take the unfused path when it is outside the validated range.  (The enqueue-only render,
@@ -1488,12 +1416,6 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
       return MP_E_RANGE;
     }
   }
-  const TcParams prm = tc_params(mlp, pk, feat, guard);
-  int dev = 0, sms = 132;
-  MP_CUDA(cudaGetDevice(&dev));
-  MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const long long tiles = bt.B * ((src.n + kTile - 1) / kTile);
-  const int grid = (int)(tiles < (long long)sms ? tiles : sms);
 #ifndef MP_CUDA_EMU
   if (dst.n_peers > 0) query_wg_kernel<C, true><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bt);      // fused slab exchange
   else query_wg_kernel<C, false><<<grid, kThreads, P::Total + 1024, st>>>(prm, src, cal, dst, surf, bt);
@@ -1510,20 +1432,36 @@ template <int C>
 int launch_jvp(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const JvpOut& jo,
                cudaStream_t st, int guard) {
   using P = Prog<C>;
-  const int rp = frame_products<C>(mlp, pk, feat, st);
-  if (rp != MP_OK) return rp;
-  const TcParams prm = tc_params(mlp, pk, feat, guard);
-  int dev = 0, sms = 132;
-  MP_CUDA(cudaGetDevice(&dev));
-  MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  const long long tiles = (src.n + kJvpPts - 1) / kJvpPts;
-  const int grid = (int)(tiles < (long long)sms ? tiles : sms);
+  TcParams prm;
+  int grid = 0;
+  const int rs = launch_setup<C>(mlp, pk, feat, st, guard, (src.n + kJvpPts - 1) / kJvpPts, prm, grid);
+  if (rs != MP_OK) return rs;
 #ifndef MP_CUDA_EMU
   query_jvp_kernel<C><<<grid, kThreads, P::Total + kJvpDwBytes + 1024, st>>>(prm, src, cal, jo);
 #else
   MP_EMU_LAUNCH(grid, kThreads, (query_jvp_kernel<C>(prm, src, cal, jo)));
 #endif
   MP_CUDA(cudaGetLastError());
+  return MP_OK;
+}
+
+// what the query and the gradient launches both need: the head's program prepared, a map of the head's channel count C
+// and of at most 65536 texels (texel indices travel as 16-bit pairs in registers, per map of a batch)
+int check_query(const mp_mlp* mlp, const mp_feat* feat, int& C) {
+  const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
+  if (!pk || !mlp->tc_ok) {
+    mp_set_error("tensor-core path not prepared for this head");
+    return MP_E_UNSUPPORTED;
+  }
+  C = pk->kind == 1 ? 512 : 256;
+  if (feat->C != C) {
+    mp_set_error("head expects %d input channels but the feature map has %d (+1 depth)", mlp->channels[0], feat->C);
+    return MP_E_INVALID;
+  }
+  if ((long long)feat->H * feat->W > 65536) {
+    mp_set_error("the tensor-core program handles feature maps of at most 65536 texels (got %d x %d); use MP_MODE_FP32", feat->H, feat->W);
+    return MP_E_UNSUPPORTED;
+  }
   return MP_OK;
 }
 
@@ -1589,20 +1527,10 @@ int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* 
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                        const MpOutDst& dst, cudaStream_t st, int guard, const MpBatch* bt) {
   if (src.n <= 0) return MP_OK;
+  int C = 0;
+  const int rc = check_query(mlp, feat, C);
+  if (rc != MP_OK) return rc;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
-  if (!pk || !mlp->tc_ok) {
-    mp_set_error("tensor-core path not prepared for this head");
-    return MP_E_UNSUPPORTED;
-  }
-  const int C = pk->kind == 1 ? 512 : 256;
-  if (feat->C != C) {
-    mp_set_error("head expects %d input channels but the feature map has %d (+1 depth)", mlp->channels[0], feat->C);
-    return MP_E_INVALID;
-  }
-  if ((long long)feat->H * feat->W > 65536) {      // texel indices travel as 16-bit pairs in registers (per map of a batch)
-    mp_set_error("the tensor-core program handles feature maps of at most 65536 texels (got %d x %d); use MP_MODE_FP32", feat->H, feat->W);
-    return MP_E_UNSUPPORTED;
-  }
   if (dst.n_peers > MP_MAX_PEERS) {
     mp_set_error("at most %d peer volumes", MP_MAX_PEERS);
     return MP_E_UNSUPPORTED;
@@ -1625,20 +1553,10 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
 int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
                            long long ld_grad, float* out, long long ld_out, float* dpoints, long long ld_dp, cudaStream_t st, int guard) {
   if (src.n <= 0) return MP_OK;
+  int C = 0;
+  const int rc = check_query(mlp, feat, C);
+  if (rc != MP_OK) return rc;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
-  if (!pk || !mlp->tc_ok) {
-    mp_set_error("tensor-core path not prepared for this head");
-    return MP_E_UNSUPPORTED;
-  }
-  const int C = pk->kind == 1 ? 512 : 256;
-  if (feat->C != C) {
-    mp_set_error("head expects %d input channels but the feature map has %d (+1 depth)", mlp->channels[0], feat->C);
-    return MP_E_INVALID;
-  }
-  if ((long long)feat->H * feat->W > 65536) {      // (as mp_launch_query_tc)
-    mp_set_error("the tensor-core program handles feature maps of at most 65536 texels (got %d x %d); use MP_MODE_FP32", feat->H, feat->W);
-    return MP_E_UNSUPPORTED;
-  }
   if (src.kind != MP_SRC_ROWS || feat->B != 1) {
     mp_set_error("the gradient program takes point rows of one map");
     return MP_E_UNSUPPORTED;

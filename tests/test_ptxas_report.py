@@ -1,9 +1,9 @@
 """The tensor-core query program compiles to asynchronous MMAs without local-memory traffic.
 
 ptxas reports C7520 when it has to serialize a kernel's wgmma instructions (every MMA completes before the next
-instruction, which removes the overlap the program is written for), and it reports spill stores per kernel.  This test
-compiles query_tc.cu for sm_90a with the library's own flags and checks both, for every instantiation of
-query_wg_kernel and g0_wg_kernel.  CPU only: it needs nvcc, not a GPU.
+instruction, which removes the overlap the program is written for), and it reports the stack frame and the spill stores
+and loads per kernel.  This test compiles query_tc.cu for sm_90a with the library's own flags and checks both, for every
+instantiation of query_wg_kernel, query_jvp_kernel and g0_wg_kernel.  CPU only: it needs nvcc, not a GPU.
 """
 import os
 import re
@@ -13,7 +13,7 @@ import pytest
 
 from monoport_b200 import build as lib_build
 
-KERNELS = ("query_wg_kernel", "g0_wg_kernel")
+KERNELS = ("query_wg_kernel", "query_jvp_kernel", "g0_wg_kernel")
 
 
 def _nvcc():
@@ -52,8 +52,9 @@ def _entries(log):
 
 def test_each_head_has_a_plain_and_a_peer_store_instantiation(ptxas_log):
     names = list(_entries(ptxas_log))
-    # query_wg_kernel: 2 heads x (plain, peer stores); g0_wg_kernel: 2 heads
+    # query_wg_kernel: 2 heads x (plain, peer stores); query_jvp_kernel, g0_wg_kernel: 2 heads
     assert sum("query_wg_kernel" in n for n in names) == 4, names
+    assert sum("query_jvp_kernel" in n for n in names) == 2, names
     assert sum("g0_wg_kernel" in n for n in names) == 2, names
 
 
@@ -65,6 +66,6 @@ def test_no_serialized_wgmma(ptxas_log):
 def test_no_spills(ptxas_log):
     for name, lines in _entries(ptxas_log).items():
         stats = " ".join(lines)
-        m = re.search(r"(\d+) bytes spill stores, (\d+) bytes spill loads", stats)
+        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", stats)
         assert m, (name, stats)
-        assert m.group(1) == "0" and m.group(2) == "0", (name, stats)
+        assert m.groups() == ("0", "0", "0"), (name, stats)

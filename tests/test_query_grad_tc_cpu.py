@@ -1,9 +1,9 @@
 """CPU checks of the tensor-core gradient program (query_jvp_kernel, mp_query_points_grad_mode in MP_MODE_TC), compiled
 unmodified on the CPU model of tests/emu: against the reference's fp64 autograd goldens, its value against the tensor-core
 query program bit for bit, across simulated SM counts and bulk-copy completion orders, outside the image, under the range
-guard and with a device-side point count.  Also the ptxas report of its sm_90a instantiations."""
+guard and with a device-side point count.  (Its ptxas report is checked with the rest of query_tc.cu in
+test_ptxas_report.py.)"""
 import os
-import re
 import shutil
 import struct
 import subprocess
@@ -280,29 +280,3 @@ def test_jvp_range_guard_and_device_count(emu, tmp_path):
     assert torch.equal(cut[0][:, :k], full[0][:, :k]) and torch.equal(cut[1][:, :k], full[1][:, :k])
     assert bool((cut[0][:, k:] == -4242).all()) and bool((cut[1][:, k:] == -4242).all())
 
-
-# ---- ptxas report ----------------------------------------------------------------------------------------------------------
-def test_jvp_kernel_has_no_spill_no_stack_frame_and_no_serialized_wgmma(tmp_path):
-    from monoport_b200 import build as lib_build
-    try:
-        nvcc = lib_build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    cmd = [nvcc] + lib_build.NVCC_FLAGS + ["-c", os.path.join(lib_build.CSRC, "query_tc.cu"), "-o", str(tmp_path / "q.o")]
-    p = subprocess.run(cmd, capture_output=True, text=True)
-    assert p.returncode == 0, p.stdout + p.stderr
-    log = p.stdout + p.stderr
-    found, current = {}, None
-    for line in log.splitlines():
-        m = re.search(r"Compiling entry function '([^']+)'", line)
-        if m:
-            current = m.group(1) if "query_jvp_kernel" in m.group(1) else None
-            if current:
-                found[current] = ""
-        elif current and ("spill" in line or "stack" in line):
-            found[current] += line
-    assert len(found) == 2, list(found)               # geometry and colour heads
-    for name, stats in found.items():
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", stats)
-        assert m and m.groups() == ("0", "0", "0"), (name, stats)
-    assert "C7520" not in log
