@@ -34,6 +34,7 @@ extern "C" {
 #define MP_E_CAPACITY (-4)  /* caller-provided output buffer too small       */
 #define MP_E_NOMEM (-5)
 #define MP_E_RANGE (-6)     /* inputs outside the validated range of the requested fast path; use the exact one */
+#define MP_E_TRUNCATED (-7) /* a device-driven loop stopped at its cap: the result is incomplete; use the eager call */
 
 /* last_op of the head: heads/SurfaceClassifier.py:68-69 (None / nn.Sigmoid / nn.Tanh) */
 #define MP_LAST_NONE 0
@@ -235,11 +236,20 @@ int mp_octree_run_fused(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const fl
  *                            [rank] is ignored).  world == 1 switches sharding off.  All ranks must then call
  *                            mp_octree_run_fused the same number of times with the same inputs. */
 /* The fused run in two halves for CUDA-graph captured frame steps: _async only enqueues (no host memory is read, no
- * synchronisation: capturable; engines without a conflict loop, i.e. faster != 0 or top-k), mp_octree_fetch reads the
- * non-empty flag and the per-level counts back afterwards (synchronises). */
+ * synchronisation: capturable, every engine mode), mp_octree_fetch reads the non-empty flag and the per-level counts back
+ * afterwards (synchronises).  In the lossless mode (faster == 0, no top-k) the conflict loop of each level runs as a
+ * conditional WHILE node of the graph whose body is one pass (query, scatter with conflict detection, next conflict list)
+ * and whose loop-control kernel decides on the device whether another pass runs -- the same nodes, order, values and
+ * counts as mp_octree_run_fused's host-driven loop.  A level stops after 8 x its resolution passes at most.  On a stream
+ * that is not being captured the call records its own sequence into a graph and launches that (still enqueue-only).
+ * A sharded lossless handle is refused (MP_E_UNSUPPORTED).
+ * mp_octree_fetch_loops: n_levels int32 = conflict-loop passes per level of the last _async run (0 for level 0 and for
+ * the other modes); MP_E_TRUNCATED when a level stopped at its cap with nodes left to evaluate (run that frame with
+ * mp_octree_run_fused).  Synchronises. */
 int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib12, int projection,
                               float z_scale, int mode, float* out_dev, void* stream);
 int mp_octree_fetch(mp_octree_t* h, int* nonempty, int64_t* stats_host, void* stream);
+int mp_octree_fetch_loops(mp_octree_t* h, int32_t* passes_per_level, void* stream);
 int mp_octree_shard_export(mp_octree_t* h, unsigned char* handles192);
 int mp_octree_shard_set(mp_octree_t* h, int rank, int world, float* const* vals0, float* const* vals1,
                         uint32_t* const* flags);

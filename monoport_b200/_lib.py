@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libmonoport_b200.so")
 
 MP_OK = 0
 MP_E_RANGE = -6
+MP_E_TRUNCATED = -7
 MODE_FP32, MODE_TC, MODE_AUTO, MODE_TC_V3 = 0, 1, 2, 4
 LAST_NONE, LAST_SIGMOID, LAST_TANH = 0, 1, 2
 PROJ_ORTHOGONAL, PROJ_PERSPECTIVE = 0, 1
@@ -74,6 +75,7 @@ SIGNATURES = {
                                     P(c_int), P(c_int64), c_void_p]),
     "mp_octree_run_fused_async": (c_int, [c_void_p, c_void_p, c_void_p, P(c_float), c_int, c_float, c_int, c_void_p, c_void_p]),
     "mp_octree_fetch": (c_int, [c_void_p, P(c_int), P(c_int64), c_void_p]),
+    "mp_octree_fetch_loops": (c_int, [c_void_p, P(ctypes.c_int32), c_void_p]),
     "mp_octree_shard_export": (c_int, [c_void_p, ctypes.c_char_p]),
     "mp_octree_shard_set": (c_int, [c_void_p, c_int, c_int, P(c_void_p), P(c_void_p), P(c_void_p)]),
     "mp_mcubes_create": (c_int, [c_int, c_int, c_int, P(c_void_p)]),

@@ -14,7 +14,7 @@
 //   (lossless mode)   conflict detection + 27-neighbourhood re-query loop
 // Top-k variant: 4-pass radix select on |occ - balance| with index-order tie break.
 #include "mp_common.cuh"
-#include "octree_kernels.cuh"
+#include "octree_loop.cuh"
 
 using namespace octree_k;
 
@@ -32,6 +32,11 @@ __global__ void node_points_kernel(MpPointSrc src, float* __restrict__ pts) {
 
 // per-level evaluated-node counters [MP_MAX_LAYERS + 4] + one slot for the non-empty flag
 constexpr int kStatSlots = MP_MAX_LAYERS + 5;
+// per-level pass counters of the device-driven conflict loop + one slot for the truncated level (level + 1, 0 = none)
+constexpr int kLoopSlots = MP_MAX_LAYERS + 5;
+// A level of `res` nodes per axis stops its device-driven conflict loop after kLoopPassesPerRes * res passes.  The loop
+// walks a thin feature about one node per pass: a one-voxel rod took 0.3 * res passes, 25x below the cap.
+constexpr int kLoopPassesPerRes = 8;
 
 // ---- multi-GPU list sharding (SURVEY.md §8e): every rank keeps the whole pyramid state and runs the cheap volume passes
 // itself (identical inputs => identical node lists on every rank, including the lossless conflict loop, which can walk
@@ -100,6 +105,10 @@ struct mp_octree {
   int* nonempty;              // device flag
   long long* stats;           // device [n_levels]
   SelectState* sel;
+  // lossless handles: the device-driven conflict loop of mp_octree_run_fused_async.  `loops` holds its pass counters;
+  // body_stream records the WHILE bodies, cap_stream the whole run when the caller's stream is not being captured.
+  int32_t* loops;
+  cudaStream_t body_stream, cap_stream;
   // stepping state
   int level;                  // level of the outstanding batch (-1 before begin)
   int cur;                    // which vol/known buffer holds `level`
@@ -129,6 +138,9 @@ extern "C" int mp_octree_destroy(mp_octree_t* h) {
   if (h->count) cudaFree(h->count);
   if (h->stats) cudaFree(h->stats);
   if (h->sel) cudaFree(h->sel);
+  if (h->loops) cudaFree(h->loops);
+  if (h->body_stream) cudaStreamDestroy(h->body_stream);
+  if (h->cap_stream) cudaStreamDestroy(h->cap_stream);
   delete h;
   return MP_OK;
 }
@@ -189,6 +201,12 @@ extern "C" int mp_octree_create(int n_levels, const int* resolutions, const floa
   // the non-empty flag lives in the last slot of the stats buffer: one memset resets both, one copy reads both back
   if (e == cudaSuccess) h->nonempty = reinterpret_cast<int*>(h->stats + kStatSlots - 1);
   if (e == cudaSuccess) e = cudaMalloc(&h->sel, sizeof(SelectState));
+  if (!h->use_topk && !h->faster) {   // (streams are created here, never while a caller's stream is being captured)
+    if (e == cudaSuccess) e = cudaMalloc(&h->loops, sizeof(int32_t) * kLoopSlots);
+    if (e == cudaSuccess) e = cudaMemset(h->loops, 0, sizeof(int32_t) * kLoopSlots);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->body_stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking);
+  }
   if (e != cudaSuccess) {
     mp_set_error("mp_octree_create: %s", cudaGetErrorString(e));
     mp_octree_destroy(h);
@@ -462,7 +480,91 @@ extern "C" int mp_octree_finish(mp_octree_t* h, float* out_dev, int* nonempty, v
 }
 
 // ---- fused run --------------------------------------------------------------------------------------
-static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode, cudaStream_t st) {
+// One evaluation pass of `level` over its node list (h->idx, count on the device): the query, then the scatter (lossless:
+// into the value list first, with conflict detection against the interpolated volume, then the next conflict list).
+static int level_pass(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode, cudaStream_t st) {
+  const bool lossless = !h->use_topk && !h->faster;
+  int rc = MP_OK;
+  MpPointSrc src;
+  fill_src_nodes(h, level, src, h->cap, true);
+  if (h->use_topk) {
+    long long k = h->topk[level];
+    const long long nf = (long long)h->res[level] * h->res[level] * h->res[level];
+    if (k > nf) k = nf;
+    if (k <= 0) return MP_OK;
+    src.n = k;
+    src.count_dev = nullptr;
+    set_i64_kernel<<<1, 1, 0, st>>>(h->stats + level, k);
+  }
+  const float* vals = h->vals;
+  const bool via_vals = lossless || h->shard_world > 1;
+  if (h->shard_world > 1) {
+    rc = sharded_query(h, mlp, feat, src, cal, mode, st, &vals);
+    if (rc != MP_OK) return rc;
+  } else {
+    MpOutDst dst;
+    dst.out = nullptr; dst.ld = 0; dst.scatter_vol = h->vol[h->cur];
+    if (lossless) {
+      // keep the interpolated values, evaluate into vals, then scatter+conflict-detect
+      dst.out = h->vals; dst.ld = h->cap; dst.scatter_vol = nullptr;
+    }
+    rc = mp_query_dispatch(mlp, feat, src, cal, dst, mode, st);
+    if (rc != MP_OK) return rc;
+  }
+  scatter_kernel<<<grid_for(h->cap > 1 << 20 ? 1 << 20 : h->cap), 256, 0, st>>>(
+      h->idx, src.count_dev, src.n, via_vals ? vals : h->vol[h->cur], h->vol[h->cur],
+      h->use_topk ? nullptr : h->known[h->cur], lossless ? h->conflict : nullptr, h->balance, via_vals);
+  MP_CUDA(cudaGetLastError());
+  if (lossless) return build_conflict_list(h, level, st);
+  return MP_OK;
+}
+
+// The conflict loop of a lossless level as a WHILE node of the graph being captured on `st`: the body is one level_pass
+// followed by loop_control_kernel, which decides on the device whether the body runs again.  The condition defaults to 1
+// on every launch of the graph, so the body runs at least once, as in the host-driven loop.
+static int device_conflict_loop(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode,
+                                cudaStream_t st) {
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  cudaGraph_t graph = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t n_deps = 0;
+  MP_CUDA(cudaStreamGetCaptureInfo(st, &cs, nullptr, &graph, &deps, &n_deps));
+  if (cs != cudaStreamCaptureStatusActive) {
+    mp_set_error("octree: the device-driven conflict loop needs a stream that is being captured");
+    return MP_E_CUDA;
+  }
+  cudaGraphConditionalHandle cond;
+  MP_CUDA(cudaGraphConditionalHandleCreate(&cond, graph, 1, cudaGraphCondAssignDefault));
+  cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
+  np.conditional.handle = cond;
+  np.conditional.type = cudaGraphCondTypeWhile;
+  np.conditional.size = 1;
+  cudaGraphNode_t node;
+  MP_CUDA(cudaGraphAddNode(&node, graph, deps, n_deps, &np));
+  MP_CUDA(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));   // the next level waits
+  MP_CUDA(cudaStreamBeginCaptureToGraph(h->body_stream, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                        cudaStreamCaptureModeRelaxed));
+  int rc = level_pass(h, level, mlp, feat, cal, mode, h->body_stream);
+  if (rc == MP_OK) {
+    loop_control_kernel<<<1, 1, 0, h->body_stream>>>(h->count, h->loops + level, h->loops + kLoopSlots - 1, level,
+                                                     kLoopPassesPerRes * h->res[level], cond);
+    const cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) {
+      mp_set_error("octree: loop_control_kernel: %s", cudaGetErrorString(le));
+      rc = MP_E_CUDA;
+    }
+  }
+  cudaGraph_t body = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(h->body_stream, &body);   // (always: the private stream stays usable)
+  if (rc != MP_OK) return rc;
+  MP_CUDA(e);
+  return MP_OK;
+}
+
+// device_loop: the lossless conflict loop of every level runs as a WHILE node of the graph captured on `st` (no host read);
+// otherwise it is driven from the host, which reads the list length back after every pass.
+static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode, cudaStream_t st,
+                            bool device_loop = false) {
   int rc = MP_OK;
   // level 0: dense
   {
@@ -496,40 +598,15 @@ static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const 
     const bool last = level == h->n_levels - 1;
     if (!h->use_topk && h->faster && last) break;
     const bool lossless = !h->use_topk && !h->faster;
-    for (int iter = 0;; ++iter) {
-      MpPointSrc src;
-      fill_src_nodes(h, level, src, h->cap, true);
-      if (h->use_topk) {
-        long long k = h->topk[level];
-        const long long nf = (long long)h->res[level] * h->res[level] * h->res[level];
-        if (k > nf) k = nf;
-        if (k <= 0) break;
-        src.n = k;
-        src.count_dev = nullptr;
-        set_i64_kernel<<<1, 1, 0, st>>>(h->stats + level, k);
-      }
-      const float* vals = h->vals;
-      const bool via_vals = lossless || h->shard_world > 1;
-      if (h->shard_world > 1) {
-        rc = sharded_query(h, mlp, feat, src, cal, mode, st, &vals);
-        if (rc != MP_OK) return rc;
-      } else {
-        MpOutDst dst;
-        dst.out = nullptr; dst.ld = 0; dst.scatter_vol = h->vol[h->cur];
-        if (lossless) {
-          // keep the interpolated values, evaluate into vals, then scatter+conflict-detect
-          dst.out = h->vals; dst.ld = h->cap; dst.scatter_vol = nullptr;
-        }
-        rc = mp_query_dispatch(mlp, feat, src, cal, dst, mode, st);
-        if (rc != MP_OK) return rc;
-      }
-      scatter_kernel<<<grid_for(h->cap > 1 << 20 ? 1 << 20 : h->cap), 256, 0, st>>>(
-          h->idx, src.count_dev, src.n, via_vals ? vals : h->vol[h->cur], h->vol[h->cur],
-          h->use_topk ? nullptr : h->known[h->cur], lossless ? h->conflict : nullptr, h->balance, via_vals);
-      MP_CUDA(cudaGetLastError());
-      if (!lossless) break;
-      rc = build_conflict_list(h, level, st);
+    if (lossless && device_loop) {
+      rc = device_conflict_loop(h, level, mlp, feat, cal, mode, st);
       if (rc != MP_OK) return rc;
+      continue;
+    }
+    for (;;) {
+      rc = level_pass(h, level, mlp, feat, cal, mode, st);
+      if (rc != MP_OK) return rc;
+      if (!lossless) break;
       int32_t cnt = 0;
       MP_CUDA(cudaMemcpyAsync(&cnt, h->count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
       MP_CUDA(cudaStreamSynchronize(st));
@@ -540,30 +617,70 @@ static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const 
   return MP_OK;
 }
 
-// The enqueue half of the fused run: everything is stream-ordered and no host memory is read, so the call can be captured
-// into a CUDA graph (engines without a conflict loop: `faster` and top-k).  Results (non-empty flag, per-level counts) stay
-// on the device until mp_octree_fetch.
-extern "C" int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib12, int projection,
-                                         float z_scale, int mode, float* out_dev, void* stream) {
-  MP_REQUIRE(h && mlp && feat && out_dev, "NULL argument");
-  MP_REQUIRE_SINGLE_MAP(feat, "the occupancy engine");
-  MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "the occupancy engine needs a single-channel head");
-  MP_REQUIRE(h->use_topk || h->faster, "the lossless engine's conflict loop reads counts on the host; use mp_octree_run_fused");
-  MpRange nvtx("monoport_b200: F2 coarse-to-fine engine (enqueue)");
-  cudaStream_t st = (cudaStream_t)stream;
+// The enqueue sequence of mp_octree_run_fused_async on `st`.
+static int enqueue_fused(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode, float* out_dev,
+                         cudaStream_t st) {
+  const bool lossless = !h->use_topk && !h->faster;
   int rc = reset_run(h, st);
   if (rc != MP_OK) return rc;
-  MpCalib cal;
-  mp_fill_calib(cal, calib12, projection, z_scale);
+  if (lossless) MP_CUDA(cudaMemsetAsync(h->loops, 0, sizeof(int32_t) * kLoopSlots, st));
   const int final_buf = (h->n_levels - 1) & 1;
   float* const own_buf = h->vol[final_buf];
   h->vol[final_buf] = out_dev;          // the last level lands in the caller's volume (see mp_octree_run_fused)
-  rc = run_fused_levels(h, mlp, feat, cal, mode, st);
+  rc = run_fused_levels(h, mlp, feat, cal, mode, st, lossless);
   const bool in_place = h->cur == final_buf;
   const float* result = h->vol[h->cur];
   h->vol[final_buf] = own_buf;
   if (rc != MP_OK) return rc;
   if (!in_place) MP_CUDA(cudaMemcpyAsync(out_dev, result, h->vol_elems * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  return MP_OK;
+}
+
+// The enqueue half of the fused run: everything is stream-ordered and no host memory is read, so the call can be captured
+// into a CUDA graph.  Results (non-empty flag, per-level counts, conflict-loop passes) stay on the device until
+// mp_octree_fetch / mp_octree_fetch_loops.  A lossless engine's conflict loop runs as a WHILE node per level; on a stream
+// that is not being captured the call records its sequence into a graph of its own and launches that on the stream.
+extern "C" int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib12, int projection,
+                                         float z_scale, int mode, float* out_dev, void* stream) {
+  MP_REQUIRE(h && mlp && feat && out_dev, "NULL argument");
+  MP_REQUIRE_SINGLE_MAP(feat, "the occupancy engine");
+  MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "the occupancy engine needs a single-channel head");
+  const bool lossless = !h->use_topk && !h->faster;
+  if (lossless && h->shard_world > 1) {
+    // (the barrier epochs of a sharded run are counted on the host: a replayed loop body would reuse one)
+    mp_set_error("a sharded lossless engine reads counts on the host; use mp_octree_run_fused");
+    return MP_E_UNSUPPORTED;
+  }
+  MpRange nvtx("monoport_b200: F2 coarse-to-fine engine (enqueue)");
+  cudaStream_t st = (cudaStream_t)stream;
+  MpCalib cal;
+  mp_fill_calib(cal, calib12, projection, z_scale);
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (lossless) MP_CUDA(cudaStreamIsCapturing(st, &cs));
+  if (!lossless || cs == cudaStreamCaptureStatusActive) {
+    const int rc = enqueue_fused(h, mlp, feat, cal, mode, out_dev, st);
+    if (rc != MP_OK) return rc;
+    h->phase = 2;
+    return MP_OK;
+  }
+  // not capturing: capture the sequence on the private stream (relaxed: the lazy allocations of a query stay legal),
+  // then launch it on the caller's stream
+  MP_CUDA(cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeRelaxed));
+  const int rc = enqueue_fused(h, mlp, feat, cal, mode, out_dev, h->cap_stream);
+  cudaGraph_t graph = nullptr;
+  cudaError_t e = cudaStreamEndCapture(h->cap_stream, &graph);
+  if (rc != MP_OK) {
+    if (graph) cudaGraphDestroy(graph);
+    return rc;
+  }
+  MP_CUDA(e);
+  cudaGraphExec_t exec = nullptr;
+  e = cudaGraphInstantiate(&exec, graph, 0);
+  cudaGraphDestroy(graph);
+  MP_CUDA(e);
+  e = cudaGraphLaunch(exec, st);
+  cudaGraphExecDestroy(exec);           // (released once the launch has completed)
+  MP_CUDA(e);
   h->phase = 2;
   return MP_OK;
 }
@@ -577,6 +694,26 @@ extern "C" int mp_octree_fetch(mp_octree_t* h, int* nonempty, int64_t* stats_hos
   MP_CUDA(cudaStreamSynchronize(st));
   *nonempty = *reinterpret_cast<const int*>(stats + kStatSlots - 1);
   if (stats_host) for (int l = 0; l < h->n_levels; ++l) stats_host[l] = stats[l];
+  return MP_OK;
+}
+
+// Conflict-loop passes per level of the last mp_octree_run_fused_async (0 for level 0 and for engines without the loop).
+// Synchronises.  MP_E_TRUNCATED when a level stopped at its cap with nodes still to evaluate.
+extern "C" int mp_octree_fetch_loops(mp_octree_t* h, int32_t* passes_per_level, void* stream) {
+  MP_REQUIRE(h && passes_per_level, "NULL argument");
+  for (int l = 0; l < h->n_levels; ++l) passes_per_level[l] = 0;
+  if (!h->loops) return MP_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  int32_t loops[kLoopSlots];
+  MP_CUDA(cudaMemcpyAsync(loops, h->loops, sizeof(loops), cudaMemcpyDeviceToHost, st));
+  MP_CUDA(cudaStreamSynchronize(st));
+  for (int l = 0; l < h->n_levels; ++l) passes_per_level[l] = loops[l];
+  const int t = loops[kLoopSlots - 1];
+  if (t > 0) {
+    mp_set_error("the conflict loop of level %d (resolution %d) stopped at its cap of %d passes with nodes left to evaluate",
+                 t - 1, h->res[t - 1], kLoopPassesPerRes * h->res[t - 1]);
+    return MP_E_TRUNCATED;
+  }
   return MP_OK;
 }
 

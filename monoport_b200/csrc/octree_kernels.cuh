@@ -207,6 +207,21 @@ __global__ void conflict_neighbours_kernel(const uint8_t* __restrict__ conflict,
   }
 }
 
+// ---- device-driven conflict loop (lossless engine, body of a CUDA-graph WHILE node) ---------------------------------
+// After one pass of a level (evaluate the list, scatter with conflict detection, build the next conflict list): count the
+// pass, and run another while the new list is non-empty.  A level that reaches `cap` passes with nodes still listed stops
+// and is reported in *truncated (level + 1).  Every continuing pass makes at least one unknown node known, so the loop ends
+// by itself; the cap only bounds how long a defect could keep the GPU busy.
+__device__ __forceinline__ unsigned conflict_loop_continue(const int32_t* count, int32_t* passes, int32_t* truncated,
+                                                           int level, int cap) {
+  const int32_t p = *passes + 1;
+  *passes = p;
+  if (*count <= 0) return 0u;
+  if (p >= cap) { *truncated = level + 1; return 0u; }
+  return 1u;
+}
+// (the kernel that hands this decision to the WHILE node is loop_control_kernel in octree_loop.cuh)
+
 // ---- top-k (Seg3dTopk): radix select of the k smallest |v - balance| with index tie-break ------------
 __device__ __forceinline__ uint32_t topk_key(float v, float balance) { return __float_as_uint(fabsf(v - balance)); }
 

@@ -56,8 +56,11 @@ class FrameGraph:
     between the tensor-core and the exact kernel is made on the device (range guard).  Several FrameGraphs own separate
     streams, workspaces and output buffers, so frame k+1's encoder overlaps frame k's reconstruction (`FrameGraphRing`).
 
-    engine: a Seg3dLossless(faster=True) / Seg3dTopk built with make_query_func(net) (engines with a conflict loop read
-    counts on the host and cannot be captured).  calib: [1,4,4] tensor (read once, at construction).
+    engine: a Seg3dLossless (faster=True, or the lossless faster=False) / Seg3dTopk built with make_query_func(net).  The
+    lossless engine's conflict loop runs inside the graph as a conditional WHILE node per level, decided on the device;
+    result() reads its passes per level into `last_conflict_loops` and raises RuntimeError for a frame whose loop stopped at
+    its cap (8 x the level's resolution passes) -- run that frame with the eager engine.  calib: [1,4,4] tensor (read once,
+    at construction).
     `feature_hook(feat) -> feat` (optional) runs inside the captured step on the encoder's last-stage map.
     launch(x) enqueues a frame (x = image [1,3,H,W] with an encoder, else the [1,C,h,w] feature map); result() waits for it
     and returns (sdf or None, X, Y, Z, norm) exactly like engine(...) followed by forward_vertices(sdf, direction).
@@ -79,8 +82,6 @@ class FrameGraph:
         from .modeling.MonoPortNet import FeatureHandle
         from .modeling.geometry import perspective
         from .recon import _DIRS
-        if not (engine.faster or engine.topk_points is not None):
-            raise ValueError("FrameGraph needs an engine without a conflict loop (faster=True or Seg3dTopk)")
         if getattr(engine.query_func, "__monoport_fused__", None) is not net:
             raise ValueError("the engine's query_func must be make_query_func(net)")
         self.net, self.engine = net, engine
@@ -144,6 +145,7 @@ class FrameGraph:
             with torch.cuda.graph(self.graph, stream=self.stream), torch.no_grad():
                 self._step()
         self.last_stats = None
+        self.last_conflict_loops = None
         self._nonempty = None
 
     def _step(self):
@@ -212,14 +214,24 @@ class FrameGraph:
         return self
 
     def result(self):
-        """Wait for the enqueued frame: (sdf or None, X, Y, Z, norm) -- views of this graph's buffers, valid until its next launch."""
+        """Wait for the enqueued frame: (sdf or None, X, Y, Z, norm) -- views of this graph's buffers, valid until its next launch.
+        Raises RuntimeError when the lossless conflict loop of the frame stopped at its cap."""
         n = len(self.engine.resolutions)
         nonempty = ctypes.c_int(0)
         stats = (ctypes.c_int64 * n)()
+        loops = (ctypes.c_int32 * n)()
         with torch.cuda.stream(self.stream):
-            _lib.check(self._lib.mp_octree_fetch(self._oct, ctypes.byref(nonempty), stats, _lib.stream_ptr(self.device)),
+            st = _lib.stream_ptr(self.device)
+            _lib.check(self._lib.mp_octree_fetch(self._oct, ctypes.byref(nonempty), stats, st),
                        "mp_octree_fetch")                                    # (synchronises the graph's stream)
+            rc = self._lib.mp_octree_fetch_loops(self._oct, loops, st)
         self.last_stats = list(stats)
+        self.last_conflict_loops = list(loops)
+        if rc == _lib.MP_E_TRUNCATED:
+            self._nonempty = None
+            raise RuntimeError("FrameGraph: %s; this frame's volume is incomplete -- run the eager engine for it"
+                               % self._lib.mp_last_error().decode())
+        _lib.check(rc, "mp_octree_fetch_loops")
         self._nonempty = bool(nonempty.value)
         if not nonempty.value:
             return None, None, None, None, None

@@ -1,6 +1,7 @@
 """Tiny invocation of every kernel family for compute-sanitizer (memcheck): both tensor-core programs, the fp32 kernel and
-its point-gradient kernel, the octree engine, marching cubes, the visible-surface kernel and the enqueue-only renders of
-captured frames (mp_colorize_surface_async on both programs, mp_render_normals_async)."""
+its point-gradient kernel, the octree engine (eager, and a captured lossless frame), marching cubes, the visible-surface
+kernel and the enqueue-only renders of captured frames (mp_colorize_surface_async on both programs,
+mp_render_normals_async)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -26,6 +27,13 @@ for faster in (True, False):
     eng = Seg3dLossless(make_query_func(net), b, -b, [9, 17, 33], balance_value=0.5, faster=faster).to("cuda")
     sdf = eng(im_feat_list=[[feat.cuda()]], calib_tensor=cal)
     print("engine faster=%s" % faster, eng.last_stats, None if sdf is None else float(sdf.sum()))
+# a captured lossless frame: the conflict loop of every level as a WHILE node decided on the device
+from monoport_b200.pipeline import FrameGraph
+eng = Seg3dLossless(make_query_func(net), b, -b, [9, 17, 33], balance_value=0.5, faster=False).to("cuda")
+fg = FrameGraph(net, eng, cal.cpu(), "front", with_encoder=False)
+sdf = fg.launch(feat.cuda()).result()[0]
+print("captured lossless frame", fg.last_stats, fg.last_conflict_loops, None if sdf is None else float(sdf.sum()))
+fg.close()
 eng = Seg3dTopk(make_query_func(net), b, -b, [9, 17, 33], num_points=[0, 500, 2000]).to("cuda")
 sdf = eng(im_feat_list=[[feat.cuda()]], calib_tensor=cal)
 X, Y, Z, n = forward_vertices(sdf, "front")
