@@ -147,6 +147,12 @@ int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const float* point
                               int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
                               int64_t ld_grad, float* out_dev, int64_t ld_out, float* dpoints_dev, int64_t ld_dpoints,
                               const int32_t* count_dev, int mode, void* stream);
+/* mp_query_points with an optional point count on the device (count_dev: one int32, or NULL): n is then the capacity and
+ * the points at or beyond min(*count_dev, n) are neither read nor written.  Enqueue-only like mp_query_points; the same
+ * modes, range guard and kernels.  Single-map handles only. */
+int mp_query_points_count(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                          int64_t point_stride, const float* calib12, int projection, float z_scale, float* out_dev,
+                          int64_t ld_out, const int32_t* count_dev, int mode, void* stream);
 /* Same call with HOST buffers (points [3,N], out [Res,N], feature map NCHW fp32 or NULL to reuse the
  * uploaded one): copies in, runs, copies out, synchronises.  This is what bench.py's e2e leg times. */
 int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,
@@ -265,6 +271,16 @@ int mp_mcubes_create(int D, int H, int W, mp_mcubes_t** out);
 int mp_mcubes_destroy(mp_mcubes_t* h);
 int mp_mcubes_count(mp_mcubes_t* h, const float* vol_dev, float iso, int64_t* n_verts, int64_t* n_faces, void* stream);
 int mp_mcubes_emit(mp_mcubes_t* h, const float* vol_dev, float iso, float* verts_dev, int32_t* faces_dev, void* stream);
+/* Count and emission in one enqueue-only call (no host read, no allocation, no synchronisation: graph-capturable, and a
+ * graph may replay it on the same handle).  The mesh is mp_mcubes_count + mp_mcubes_emit's, id for id, into caller buffers
+ * of v_cap vertices [v_cap][3] and f_cap faces [f_cap][3]: a vertex with id >= v_cap and a face with index >= f_cap are not
+ * written.  counts_dev (int64[2]) receives the true totals (nV, nF), so the caller can detect an overflow; count32_dev (one
+ * int32) receives min(nV, v_cap), the point count of mp_query_points_count / mp_mesh_normals_async at the vertices.
+ * world: NULL for index space, else 7 host floats {R, b_min[3], b_max[3]}: vertex v is stored as
+ * (v + 0.5) * ((b_max - b_min) / R) + b_min with torch's fp32 roundings (reconstruction()'s vertices bit for bit).
+ * Does not change what mp_mcubes_count / mp_mcubes_emit see on the handle. */
+int mp_mcubes_run_async(mp_mcubes_t* h, const float* vol_dev, float iso, const float* world, int64_t v_cap, int64_t f_cap,
+                        float* verts_dev, int32_t* faces_dev, int64_t* counts_dev, int32_t* count32_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Visible-surface extraction.  Replaces forward_vertices (RTL/recon.py:27-89).
@@ -315,6 +331,13 @@ int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_de
                              const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
                              const float* calib12, int projection, float z_scale, int mode, float* scratch_dev, float* norm_dev,
                              void* stream);
+/* Analytic normals at mesh vertices, enqueue-only: verts_dev = mp_mcubes_run_async's world-space [capacity][3] vertices,
+ * counts_dev / count32_dev its counts (the first min(counts_dev[0], capacity) vertices are evaluated).  norm_dev[i] =
+ * -g / |g| with g the geometry head's gradient at vertex i (zero where it vanishes), as reconstruction(normals=True) gives
+ * it.  mode: as mp_query_points_grad_mode.  scratch_dev: 3 * capacity floats.  Heads with one output, single-map handles. */
+int mp_mesh_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const float* verts_dev, const int64_t* counts_dev,
+                          const int32_t* count32_dev, int64_t capacity, const float* calib12, int projection, float z_scale,
+                          int mode, float* scratch_dev, float* norm_dev, void* stream);
 
 #ifdef __cplusplus
 }

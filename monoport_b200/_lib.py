@@ -45,6 +45,8 @@ SIGNATURES = {
                                       c_float, c_void_p, c_int64, c_int64, c_int, c_void_p]),
     "mp_query_points": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
                                 c_void_p, c_int64, c_int, c_void_p]),
+    "mp_query_points_count": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
+                                      c_void_p, c_int64, c_void_p, c_int, c_void_p]),
     "mp_query_points_grad": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
                                      c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
     "mp_query_points_grad_mode": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
@@ -82,6 +84,8 @@ SIGNATURES = {
     "mp_mcubes_destroy": (c_int, [c_void_p]),
     "mp_mcubes_count": (c_int, [c_void_p, c_void_p, c_float, P(c_int64), P(c_int64), c_void_p]),
     "mp_mcubes_emit": (c_int, [c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p]),
+    "mp_mcubes_run_async": (c_int, [c_void_p, c_void_p, c_float, P(c_float), c_int64, c_int64, c_void_p, c_void_p, c_void_p,
+                                    c_void_p, c_void_p]),
     "mp_colorize_surface": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, P(c_float), P(c_float),
                                     P(c_float), c_int, c_float, c_void_p, c_void_p]),
     "mp_colorize_surface_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, P(c_float),
@@ -89,6 +93,8 @@ SIGNATURES = {
     "mp_render_normals_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p]),
     "mp_surface_normals_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, P(c_float),
                                          P(c_float), P(c_float), c_int, c_float, c_int, c_void_p, c_void_p, c_void_p]),
+    "mp_mesh_normals_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, P(c_float), c_int, c_float,
+                                      c_int, c_void_p, c_void_p, c_void_p]),
     "mp_forward_vertices":(c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, P(c_int64),
                                     c_void_p]),
     "mp_forward_vertices_scratch_bytes": (c_int64, [c_int]),

@@ -11,6 +11,9 @@
 // emit :  mesh_emit_kernel, a warp per listed word, a lane per node: vertices from the volume (two loads per vertex); the
 //         cells' triangles go through a shared-memory queue and are resolved one thread per face corner (edge -> owning
 //         node -> id = the owning word's prefix + popcounts).
+// mp_mcubes_run_async: the same launches without the host (graph-capturable, replayable on one workspace): the emission grid
+//         is fixed at record time and reads the active-list length on the device; caller buffers with capacities, the true
+//         totals and the vertex count left on the device, optional world-space vertices.
 // Workspace: 1 bit + 24 B per 32 nodes (15 MB at 257^3; the round-1 byte-per-node design took 102 MB).
 #include "mp_common.cuh"
 #include <stdlib.h>
@@ -84,11 +87,10 @@ static int sm_count() {
   return sms;
 }
 
-extern "C" int mp_mcubes_count(mp_mcubes_t* h, const float* vol_dev, float iso, int64_t* n_verts, int64_t* n_faces,
-                               void* stream) {
-  MP_REQUIRE(h && vol_dev && n_verts && n_faces, "NULL argument");
-  MpRange nvtx("monoport_b200: F3 marching cubes (count)");
-  cudaStream_t st = (cudaStream_t)stream;
+// bits_kernel -> zeroed chunk sums (and n_active_dev) -> classify_sums_kernel -> the scan's emit half: the counts, the
+// prefixes and the active list on the device.  Enqueue-only; every per-run word is reset inside the sequence (the chunk
+// sums and n_active_dev by the memset, the scan ticket by the scan's last CTA), so a graph can replay it.
+static int enqueue_count(mp_mcubes* h, const float* vol_dev, float iso, cudaStream_t st) {
   {
     // a multiple of the SM count, 8 CTAs of 256 threads resident per SM: 8 x 128 B loads in flight per warp
     const long long warps_needed = (h->n_words + kBitsUnroll - 1) / kBitsUnroll;
@@ -107,6 +109,16 @@ extern "C" int mp_mcubes_count(mp_mcubes_t* h, const float* vol_dev, float iso, 
   PrefixEmit em{h->prefix, h->active, h->n_active_dev};
   mpscan::emit_kernel<WordCountF, PrefixEmit><<<nb, mpscan::kThreads, 0, st>>>(f2, em, h->n_words, h->sums);
   MP_CUDA(cudaGetLastError());
+  return MP_OK;
+}
+
+extern "C" int mp_mcubes_count(mp_mcubes_t* h, const float* vol_dev, float iso, int64_t* n_verts, int64_t* n_faces,
+                               void* stream) {
+  MP_REQUIRE(h && vol_dev && n_verts && n_faces, "NULL argument");
+  MpRange nvtx("monoport_b200: F3 marching cubes (count)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rc = enqueue_count(h, vol_dev, iso, st);
+  if (rc != MP_OK) return rc;
   unsigned long long tot = 0;
   MP_CUDA(cudaMemcpyAsync(&tot, h->total, sizeof(tot), cudaMemcpyDeviceToHost, st));
   MP_CUDA(cudaMemcpyAsync(&h->n_active, h->n_active_dev, sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
@@ -132,6 +144,42 @@ extern "C" int mp_mcubes_emit(mp_mcubes_t* h, const float* vol_dev, float iso, f
   if (blocks_needed > 0)
     mesh_emit_kernel<<<(unsigned)blocks_needed, kEmitThreads, 0, st>>>(vol_dev, h->bits, h->info, h->prefix, h->active, h->n_active,
                                                                      verts_dev, faces_dev, h->D, h->H, h->W, h->n, iso);
+  MP_CUDA(cudaGetLastError());
+  return MP_OK;
+}
+
+extern "C" int mp_mcubes_run_async(mp_mcubes_t* h, const float* vol_dev, float iso, const float* world, int64_t v_cap,
+                                   int64_t f_cap, float* verts_dev, int32_t* faces_dev, int64_t* counts_dev,
+                                   int32_t* count32_dev, void* stream) {
+  MP_REQUIRE(h && vol_dev && counts_dev && count32_dev, "NULL argument");
+  MP_REQUIRE(v_cap >= 0 && f_cap >= 0 && v_cap <= INT32_MAX && f_cap <= INT32_MAX, "bad capacities v_cap=%lld f_cap=%lld",
+             (long long)v_cap, (long long)f_cap);
+  MP_REQUIRE((verts_dev || v_cap == 0) && (faces_dev || f_cap == 0), "NULL output buffers");
+  MeshOut out;
+  memset(&out, 0, sizeof(out));
+  out.verts = verts_dev;
+  out.faces = faces_dev;
+  out.v_cap = (uint32_t)v_cap;
+  out.f_cap = (uint32_t)f_cap;
+  if (world) {
+    const float R = world[0];
+    MP_REQUIRE(R >= 1.f, "bad world mapping: R=%g", (double)R);
+    out.world = 1;
+    for (int a = 0; a < 3; ++a) {
+      out.scale[a] = (world[4 + a] - world[1 + a]) / R;          // torch's (b_max - b_min) / R in fp32
+      out.bmin[a] = world[1 + a];
+    }
+  }
+  MpRange nvtx("monoport_b200: F3 marching cubes (enqueue-only)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int rc = enqueue_count(h, vol_dev, iso, st);
+  if (rc != MP_OK) return rc;
+  // a persistent grid fixed at record time: 4 CTAs per SM, and no more warps than the volume has words
+  const long long blocks_needed = (h->n_words + kEmitWarps - 1) / kEmitWarps;
+  const long long cap = (long long)sm_count() * 4;
+  mesh_emit_async_kernel<<<(unsigned)(blocks_needed < cap ? blocks_needed : cap), kEmitThreads, 0, st>>>(
+      vol_dev, h->bits, h->info, h->prefix, h->active, h->n_active_dev, h->total, out,
+      reinterpret_cast<long long*>(counts_dev), count32_dev, h->D, h->H, h->W, h->n, iso);
   MP_CUDA(cudaGetLastError());
   return MP_OK;
 }

@@ -211,10 +211,28 @@ __device__ __forceinline__ int32_t vertex_id(const WordInfo* __restrict__ info, 
 constexpr int kEmitThreads = 256;
 constexpr int kEmitWarps = kEmitThreads / 32;
 constexpr int kEmitQueue = kEmitWarps * 32 * MC_MAX_TRI;
-__global__ void __launch_bounds__(kEmitThreads)
-mesh_emit_kernel(const float* __restrict__ vol, const uint32_t* __restrict__ bits, const WordInfo* __restrict__ info,
-                 const unsigned long long* __restrict__ prefix, const uint32_t* __restrict__ active, uint32_t n_active,
-                 float* __restrict__ verts, int32_t* __restrict__ faces, int D, int H, int W, long long n, float iso) {
+
+// Where the emission writes, for the enqueue-only run (mesh_emit_async_kernel): vertex ids >= v_cap and face indices >=
+// f_cap are not written, and with `world` set a vertex v is stored as (v + 0.5) * scale + b_min -- reconstruction()'s
+// node-centre mapping, with torch's three fp32 roundings (intrinsics, so that no FMA contraction fuses them).
+struct MeshOut {
+  float* verts;
+  int32_t* faces;
+  uint32_t v_cap, f_cap;
+  int world;
+  float scale[3], bmin[3];
+};
+
+// The emission of one grid (the algorithm above), shared by the eager kernel (kCapped = false: every id is written, index
+// space, n_active from the host) and the enqueue-only one (kCapped = true: MeshOut's capacities and world mapping, n_active
+// read from the device).  `n_active` must be the same for every thread of the grid (it sets the uniform round count).
+template <bool kCapped>
+__device__ __forceinline__ void mesh_emit_body(const float* __restrict__ vol, const uint32_t* __restrict__ bits,
+                                               const WordInfo* __restrict__ info, const unsigned long long* __restrict__ prefix,
+                                               const uint32_t* __restrict__ active, uint32_t n_active, const MeshOut& out,
+                                               int D, int H, int W, long long n, float iso) {
+  float* __restrict__ verts = out.verts;
+  int32_t* __restrict__ faces = out.faces;
   __shared__ uint32_t q_node[kEmitQueue], q_tri[kEmitQueue], q_edges[kEmitQueue];
   __shared__ uint32_t q_count;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -246,8 +264,14 @@ mesh_emit_kernel(const float* __restrict__ vol, const uint32_t* __restrict__ bit
           const float t = __fdiv_rn(__fsub_rn(iso, va), __fsub_rn(vb, va));
           float p[3] = {(float)x, (float)y, (float)z};
           p[axis] = __fadd_rn(p[axis], t);
-          float* o = verts + 3ull * vi;
-          o[0] = p[0]; o[1] = p[1]; o[2] = p[2];
+          if (!kCapped || vi < out.v_cap) {
+            if (kCapped && out.world) {
+#pragma unroll
+              for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(__fmul_rn(__fadd_rn(p[a], 0.5f), out.scale[a]), out.bmin[a]);
+            }
+            float* o = verts + 3ull * vi;
+            o[0] = p[0]; o[1] = p[1]; o[2] = p[2];
+          }
           ++vi;
         }
       }
@@ -292,10 +316,40 @@ mesh_emit_kernel(const float* __restrict__ vol, const uint32_t* __restrict__ bit
       else if (axis == 1) { ox = q & 1; oz = q >> 1; }
       else { ox = q & 1; oy = q >> 1; }
       const uint32_t node = q_node[tq] + (oz * (uint32_t)H + oy) * (uint32_t)W + ox;
-      faces[3ull * q_tri[tq] + c] = vertex_id(info, prefix, node, axis);
+      if (!kCapped || q_tri[tq] < out.f_cap) faces[3ull * q_tri[tq] + c] = vertex_id(info, prefix, node, axis);
     }
     __syncthreads();
   }
+}
+
+__global__ void __launch_bounds__(kEmitThreads)
+mesh_emit_kernel(const float* __restrict__ vol, const uint32_t* __restrict__ bits, const WordInfo* __restrict__ info,
+                 const unsigned long long* __restrict__ prefix, const uint32_t* __restrict__ active, uint32_t n_active,
+                 float* __restrict__ verts, int32_t* __restrict__ faces, int D, int H, int W, long long n, float iso) {
+  MeshOut out;
+  out.verts = verts;
+  out.faces = faces;
+  mesh_emit_body<false>(vol, bits, info, prefix, active, n_active, out, D, H, W, n, iso);
+}
+
+// ---- pass 4 without the host (mp_mcubes_run_async): the grid is fixed when the launch is recorded, every thread reads the
+// active-list length the scan left on the device, and the rounds cover it.  Block 0 also publishes the totals of the packed
+// scan total (low 32 bits vertices, high 32 faces): counts[0..1] = (nv, nf), the true ones even when they exceed the
+// capacities, and count32 = min(nv, v_cap), the point count of the queries at the vertices.
+__global__ void __launch_bounds__(kEmitThreads)
+mesh_emit_async_kernel(const float* __restrict__ vol, const uint32_t* __restrict__ bits, const WordInfo* __restrict__ info,
+                       const unsigned long long* __restrict__ prefix, const uint32_t* __restrict__ active,
+                       const uint32_t* __restrict__ n_active_dev, const unsigned long long* __restrict__ total, MeshOut out,
+                       long long* __restrict__ counts, int32_t* __restrict__ count32, int D, int H, int W, long long n,
+                       float iso) {
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    const unsigned long long tot = *total;
+    const uint32_t nv = (uint32_t)(tot & 0xffffffffull), nf = (uint32_t)(tot >> 32);
+    counts[0] = (long long)nv;
+    counts[1] = (long long)nf;
+    *count32 = (int32_t)(nv < out.v_cap ? nv : out.v_cap);
+  }
+  mesh_emit_body<true>(vol, bits, info, prefix, active, *n_active_dev, out, D, H, W, n, iso);
 }
 
 }  // namespace mcubes

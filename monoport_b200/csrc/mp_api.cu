@@ -294,7 +294,7 @@ int mp_query_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const M
 static int query_points(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n, int64_t batch_stride,
                         int64_t row_stride, int64_t point_stride, const float* calib12, const float* calibs_dev, int projection,
                         float z_scale, float* out_dev, int64_t out_batch_stride, int64_t ld_out, int mode, void* stream,
-                        bool batched) {
+                        bool batched, const int32_t* count_dev = nullptr) {
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE(n >= 0 && row_stride >= 1 && point_stride >= 1 && ld_out >= n, "bad sizes n=%lld strides=%lld,%lld ld_out=%lld",
              (long long)n, (long long)row_stride, (long long)point_stride, (long long)ld_out);
@@ -315,6 +315,7 @@ static int query_points(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* poin
   src.px = points_dev; src.py = points_dev + row_stride; src.pz = points_dev + 2 * row_stride;
   src.pstride = point_stride;
   src.n = n;
+  src.count_dev = count_dev;
   MpCalib cal;
   mp_fill_calib(cal, calib12, projection, z_scale);
   MpOutDst dst;
@@ -335,6 +336,13 @@ extern "C" int mp_query_points(mp_mlp_t* mlp, mp_feat_t* feat, const float* poin
                                float* out_dev, int64_t ld_out, int mode, void* stream) {
   return query_points(mlp, feat, 1, points_dev, n, 0, row_stride, point_stride, calib12, nullptr, projection, z_scale, out_dev, 0,
                       ld_out, mode, stream, false);
+}
+
+extern "C" int mp_query_points_count(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                                     int64_t point_stride, const float* calib12, int projection, float z_scale, float* out_dev,
+                                     int64_t ld_out, const int32_t* count_dev, int mode, void* stream) {
+  return query_points(mlp, feat, 1, points_dev, n, 0, row_stride, point_stride, calib12, nullptr, projection, z_scale, out_dev, 0,
+                      ld_out, mode, stream, false, count_dev);
 }
 
 extern "C" int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
@@ -465,6 +473,30 @@ extern "C" int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const in
   float a[3];
   for (int k = 0; k < 3; ++k) a[k] = (b_max3[k] - b_min3[k]) / (float)R;
   normals_finish_kernel<<<grid, 256, 0, st>>>(grad, reinterpret_cast<const long long*>(count_dev), capacity, a[0], a[1], -a[2], norm_dev);
+  MP_CUDA(cudaGetLastError());
+  return MP_OK;
+}
+
+// Analytic normals at the vertices of a mesh (mp_mcubes_run_async's world-space [cap][3] vertices), enqueue-only: the
+// gradient launches of mp_surface_normals_async read the vertex rows in place (row stride 1, point stride 3) with the int32
+// count of the emission, and normals_finish_kernel takes unit axes: -g / |g|, zero where g vanishes.
+extern "C" int mp_mesh_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const float* verts_dev, const int64_t* counts_dev,
+                                     const int32_t* count32_dev, int64_t capacity, const float* calib12, int projection,
+                                     float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
+  MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE_SINGLE_MAP(feat, "mp_mesh_normals_async");
+  MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "mesh normals need a head with one output (got %d)", mlp->cout[mlp->n_layers - 1]);
+  MP_REQUIRE(capacity >= 0, "bad capacity %lld", (long long)capacity);
+  MP_REQUIRE(verts_dev && counts_dev && count32_dev && scratch_dev && norm_dev, "NULL argument");
+  if (capacity == 0) return MP_OK;
+  float* grad = scratch_dev;
+  const int rc = query_points_grad(mlp, feat, verts_dev, capacity, 1, 3, calib12, projection, z_scale, nullptr, 0, nullptr, 0, grad,
+                                   capacity, count32_dev, mode, stream, "mp_mesh_normals_async");
+  if (rc != MP_OK) return rc;
+  const long long blocks = (capacity + 255) / 256;
+  const int grid = (int)(blocks < 1024 ? blocks : 1024);
+  normals_finish_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(grad, reinterpret_cast<const long long*>(counts_dev), capacity,
+                                                                1.f, 1.f, 1.f, norm_dev);
   MP_CUDA(cudaGetLastError());
   return MP_OK;
 }

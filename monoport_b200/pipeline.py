@@ -75,10 +75,21 @@ class FrameGraph:
         finite-difference normals (the norm result() returns); "gradient": N = the analytic normals of the geometry net,
         surface_normals(..., precision="auto") computed inside the step (mp_surface_normals_async, the count on the device);
       canvas: the background of both images ([R,R,3], default ones).
-    launch(x, x_colour) then takes the netC input too, and rendered() (after result()) returns (render_norm, render_tex)."""
+    launch(x, x_colour) then takes the netC input too, and rendered() (after result()) returns (render_norm, render_tex).
+
+    The mesh of the frame can be extracted inside the same captured step:
+      mesh: marching cubes at 0.5 on the frame's volume, in world space (marching_cubes_async on a workspace the graph
+        owns): the vertices and faces reconstruction(use_octree=True, engine=engine) returns for the frame, bit for bit;
+      mesh_normals: their analytic normals, mesh_normals(net, ..., precision="auto") computed inside the step;
+      mesh_colours: their colours, mesh_colours(netC, ...) computed inside the step (needs netC);
+      mesh_capacity: (vertices, faces) the buffers hold, default (8 R^2, 16 R^2).
+    mesh() (after result()) then returns (verts [V,3], faces [F,3] int32, normals or None, colours or None) -- views of this
+    graph's buffers, valid until its next launch -- or None for a frame without a surface, and raises RuntimeError for a
+    frame whose mesh exceeds the capacity (run reconstruction() eagerly for that frame)."""
 
     def __init__(self, net, engine, calib, direction="front", with_encoder=True, input_shape=None, feature_hook=None,
-                 netC=None, render_normals=False, canvas=None):
+                 netC=None, render_normals=False, canvas=None, mesh=False, mesh_normals=False, mesh_colours=False,
+                 mesh_capacity=None):
         from .modeling.MonoPortNet import FeatureHandle
         from .modeling.geometry import perspective
         from .recon import _DIRS
@@ -98,6 +109,11 @@ class FrameGraph:
         if render_normals not in (False, True, "gradient"):
             raise ValueError("render_normals must be False, True or 'gradient'; got %r" % (render_normals,))
         self.render_normals = render_normals
+        if (mesh_normals or mesh_colours or mesh_capacity is not None) and not mesh:
+            raise ValueError("mesh_normals, mesh_colours and mesh_capacity need mesh=True")
+        if mesh_colours and netC is None:
+            raise ValueError("mesh_colours needs netC")
+        self.with_mesh, self.with_mesh_normals, self.with_mesh_colours = bool(mesh), bool(mesh_normals), bool(mesh_colours)
         lib = self._lib = _lib.load()
         with torch.cuda.device(dev):
             self.stream = torch.cuda.Stream(dev)
@@ -131,6 +147,23 @@ class FrameGraph:
                 self.N_grad = torch.empty((cap, 3), dtype=torch.float32, device=dev)
                 self._nscratch = torch.empty(6 * cap + 1, dtype=torch.float32, device=dev)
             self._scratch = torch.empty(int(lib.mp_forward_vertices_scratch_bytes(R)), dtype=torch.uint8, device=dev)
+            self._mcubes = None
+            if mesh:
+                from .recon import McubesWorkspace
+                v_cap, f_cap = (8 * R * R, 16 * R * R) if mesh_capacity is None else (int(c) for c in mesh_capacity)
+                if v_cap < 0 or f_cap < 0:
+                    raise ValueError("mesh_capacity must be (vertices, faces) >= 0; got %r" % (mesh_capacity,))
+                self._mcubes = McubesWorkspace((R, R, R), dev)
+                self.mesh_verts = torch.empty((v_cap, 3), dtype=torch.float32, device=dev)
+                self.mesh_faces = torch.empty((f_cap, 3), dtype=torch.int32, device=dev)
+                self.mesh_counts = torch.zeros(2, dtype=torch.int64, device=dev)
+                self._mesh_count32 = torch.zeros(1, dtype=torch.int32, device=dev)
+                if mesh_normals:
+                    self.mesh_norm = torch.empty((v_cap, 3), dtype=torch.float32, device=dev)
+                    self._mesh_nscratch = torch.empty(3 * v_cap, dtype=torch.float32, device=dev)
+                if mesh_colours:
+                    self._mesh_pred = torch.empty((3, v_cap), dtype=torch.float32, device=dev)
+                    self._mesh_rgb = torch.empty((3, v_cap), dtype=torch.float32, device=dev)
             self._oct = engine._new_handle(dev)            # private workspace: graphs of different lanes overlap
             self._fh = None
             self._head = net.surface_classifier.handle()
@@ -198,6 +231,29 @@ class FrameGraph:
                 ctypes.c_void_p(self.Z.data_ptr()), ctypes.c_void_p(self.count.data_ptr()), cap, self.R, self._bmin3,
                 self._bmax3, self._cal12, self._projC, ctypes.c_float(self.netC.normalizer.scale), self.netC._mode(),
                 ctypes.c_void_p(self.render_tex.data_ptr()), st), "mp_colorize_surface_async")
+        if self.with_mesh:
+            self._mesh_step(st)
+
+    def _mesh_step(self, st):
+        from .recon import marching_cubes_async
+        lib = self._lib
+        marching_cubes_async(self.volume, self.mesh_verts, self.mesh_faces, self.mesh_counts, self._mesh_count32, 0.5,
+                             list(self._bmin3), list(self._bmax3), workspace=self._mcubes)
+        v_cap = self.mesh_verts.shape[0]
+        verts, counts, count32 = (ctypes.c_void_p(t.data_ptr()) for t in (self.mesh_verts, self.mesh_counts, self._mesh_count32))
+        if self.with_mesh_normals:
+            _lib.check(lib.mp_mesh_normals_async(
+                self._head, self._fh.ptr, verts, counts, count32, v_cap, self._cal12, self._proj,
+                ctypes.c_float(self.net.normalizer.scale), _lib.MODE_AUTO, ctypes.c_void_p(self._mesh_nscratch.data_ptr()),
+                ctypes.c_void_p(self.mesh_norm.data_ptr()), st), "mp_mesh_normals_async")
+        if self.with_mesh_colours:
+            # netC at the vertex rows (row stride 1, point stride 3), then mesh_colours' pred * 0.5 + 0.5
+            _lib.check(lib.mp_query_points_count(
+                self._headC, self._fhc.ptr, verts, v_cap, 1, 3, self._cal12, self._projC,
+                ctypes.c_float(self.netC.normalizer.scale), ctypes.c_void_p(self._mesh_pred.data_ptr()), v_cap, count32,
+                self.netC._mode(), st), "mp_query_points_count")
+            torch.mul(self._mesh_pred, 0.5, out=self._mesh_rgb)
+            self._mesh_rgb.add_(0.5)
 
     def launch(self, x, x_colour=None):
         """Enqueue one frame (returns at once).  x_colour: netC's input (its image with the encoder, else its map), required
@@ -248,11 +304,35 @@ class FrameGraph:
             return None, None
         return self.render_norm, self.render_tex
 
+    def mesh(self):
+        """After result(): (verts [V,3] world, faces [F,3] int32, normals [V,3] or None, colours [V,3] or None) of the frame
+        -- views of this graph's buffers, valid until its next launch -- or None when the frame has no surface.  Raises
+        RuntimeError when the frame's mesh does not fit the graph's capacity."""
+        if not self.with_mesh:
+            raise RuntimeError("FrameGraph.mesh() needs a graph built with mesh=True")
+        if self._nonempty is None:
+            raise RuntimeError("FrameGraph.mesh() needs the frame's result() first")
+        if not self._nonempty:
+            return None
+        nv, nf = self.mesh_counts.tolist()              # (result() has synchronised the graph's stream)
+        v_cap, f_cap = self.mesh_verts.shape[0], self.mesh_faces.shape[0]
+        if nv > v_cap or nf > f_cap:
+            raise RuntimeError("FrameGraph: the frame's mesh has %d vertices and %d faces, above the capacity of %d and %d "
+                               "(mesh_capacity) -- run reconstruction() eagerly for this frame" % (nv, nf, v_cap, f_cap))
+        if nv == 0:
+            return None
+        return (self.mesh_verts[:nv], self.mesh_faces[:nf], self.mesh_norm[:nv] if self.with_mesh_normals else None,
+                self._mesh_rgb.t()[:nv] if self.with_mesh_colours else None)
+
     def close(self):
         if self._oct is not None:
             self.stream.synchronize()
             self._lib.mp_octree_destroy(self._oct)
             self._oct = None
+        if self._mcubes is not None:
+            self.stream.synchronize()
+            self._mcubes.close()
+            self._mcubes = None
 
     def __del__(self):
         try:
@@ -264,7 +344,8 @@ class FrameGraph:
 class FrameGraphRing:
     """`n_lanes` FrameGraphs used round-robin: up to n_lanes frames in flight, results in input order (the graph-captured
     counterpart of FramePipeline for the stages of this library).  Lanes built with netC take (x, x_colour) items and yield
-    result() + rendered(): (sdf, X, Y, Z, norm, render_norm, render_tex)."""
+    result() + rendered(): (sdf, X, Y, Z, norm, render_norm, render_tex).  Lanes built with mesh=True append mesh()'s
+    (verts, faces, normals, colours), four Nones for a frame without a surface."""
 
     def __init__(self, make_graph, n_lanes=2):
         self.lanes = [make_graph() for _ in range(int(n_lanes))]
@@ -274,6 +355,8 @@ class FrameGraphRing:
         out = lane.result()
         if lane.netC is not None or lane.render_normals:
             out = out + lane.rendered()
+        if lane.with_mesh:
+            out = out + (lane.mesh() or (None,) * 4)
         return out
 
     def run(self, iterable):

@@ -3,7 +3,9 @@
   pifu_calib, forward_vertices : same signatures/returns as RTL/recon.py:4-25 / :27-89 (the reference file itself can
                                  also be used unchanged on the volumes the engines return);
   marching_cubes, reconstruction: additions asked for by the north star (the reference has no marching cubes;
-                                 `reconstruction` follows upstream PIFu's signature).
+                                 `reconstruction` follows upstream PIFu's signature);
+  marching_cubes_async, mesh_normals, mesh_colours: the mesh of a captured frame (FrameGraph(mesh=True)) and its eager
+                                 twins -- normals and upstream PIFu's gen_mesh_color vertex colours at the vertices.
 """
 import ctypes
 import threading
@@ -95,6 +97,121 @@ def marching_cubes(vol, iso=0.5):
                                       ctypes.c_void_p(verts.data_ptr()), ctypes.c_void_p(faces.data_ptr()), st),
                    "mp_mcubes_emit")
     return verts, faces
+
+
+class McubesWorkspace:
+    """A marching-cubes workspace (mp_mcubes_t) for volumes of one [D,H,W] shape, owned by the caller: what
+    marching_cubes_async runs on.  Runs that may be in flight together (the lanes of a FrameGraphRing, which share a thread)
+    need one workspace each.  close() frees it once the work enqueued on it has completed."""
+
+    def __init__(self, shape, device):
+        self.shape = tuple(int(s) for s in shape)
+        self.device = torch.device(device)
+        self.ptr = ctypes.c_void_p()
+        with _lib.device_guard(self.device):
+            _lib.check(_lib.load().mp_mcubes_create(*self.shape, ctypes.byref(self.ptr)), "mp_mcubes_create")
+
+    def close(self):
+        if self.ptr:
+            _lib.load().mp_mcubes_destroy(self.ptr)
+            self.ptr = ctypes.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def _require(t, dtype, shape, what):
+    if t.dtype != dtype or t.device.type != "cuda" or not t.is_contiguous() or (shape is not None and tuple(t.shape) != shape):
+        raise ValueError("%s must be a contiguous %s CUDA tensor%s; got %s %s %s" % (
+            what, dtype, "" if shape is None else " of shape %s" % (shape,), t.dtype, t.device, tuple(t.shape)))
+
+
+@torch.no_grad()
+def marching_cubes_async(vol, verts, faces, counts, count32, iso=0.5, b_min=None, b_max=None, *, workspace):
+    """marching_cubes() without the host: enqueue-only (no read-back, no allocation, no synchronisation), so a CUDA graph
+    can capture it (FrameGraph(mesh=True)).  The mesh goes into the caller's buffers verts [V_cap,3] float32 and faces
+    [F_cap,3] int32 -- the same ids and order as marching_cubes(); vertices with id >= V_cap and faces with index >= F_cap are
+    not written.  counts (int64 [2]) receives the true totals (nV, nF): the mesh is complete when they fit.  count32 (int32
+    [1]) receives min(nV, V_cap), the vertex count of mesh_normals / netC queries on the device.
+    b_min / b_max: None for index space, else the vertices are reconstruction()'s world points
+    (v + 0.5) * ((b_max - b_min) / R) + b_min, bit for bit (cubic volumes, R = the side).
+    workspace: a McubesWorkspace of the volume's shape (not shared with a run that may still be in flight)."""
+    if vol.dim() == 5:
+        vol = vol[0, 0]
+    _require(vol, torch.float32, None, "vol")
+    if vol.dim() != 3:
+        raise ValueError("vol must be [D,H,W] or [1,1,D,H,W]; got %s" % (tuple(vol.shape),))
+    if not isinstance(workspace, McubesWorkspace) or workspace.shape != tuple(vol.shape) or not workspace.ptr:
+        raise ValueError("workspace must be an open McubesWorkspace of shape %s" % (tuple(vol.shape),))
+    if verts.dim() != 2 or faces.dim() != 2:
+        raise ValueError("verts must be [V_cap,3] and faces [F_cap,3]")
+    _require(verts, torch.float32, (verts.shape[0], 3), "verts")
+    _require(faces, torch.int32, (faces.shape[0], 3), "faces")
+    _require(counts, torch.int64, (2,), "counts")
+    _require(count32, torch.int32, (1,), "count32")
+    for t in (verts, faces, counts, count32):
+        if t.device != vol.device:
+            raise ValueError("the volume and the output buffers live on different devices")
+    world = None
+    if (b_min is None) != (b_max is None):
+        raise ValueError("pass both b_min and b_max, or neither")
+    if b_min is not None:
+        D, H, W = vol.shape
+        if not D == H == W:
+            raise ValueError("world-space vertices need a cubic volume; got %s" % (tuple(vol.shape),))
+        world = (ctypes.c_float * 7)(float(W), *_lib.f3(b_min), *_lib.f3(b_max))
+    with _lib.device_guard(vol.device):
+        _lib.check(_lib.load().mp_mcubes_run_async(
+            workspace.ptr, ctypes.c_void_p(vol.data_ptr()), ctypes.c_float(iso), world, verts.shape[0], faces.shape[0],
+            ctypes.c_void_p(verts.data_ptr()), ctypes.c_void_p(faces.data_ptr()), ctypes.c_void_p(counts.data_ptr()),
+            ctypes.c_void_p(count32.data_ptr()), _lib.stream_ptr(vol.device)), "mp_mcubes_run_async")
+
+
+@torch.no_grad()
+def mesh_normals(net, feats, verts, calib_tensor, precision="auto"):
+    """Outward unit normals -grad sigma / |grad sigma| of the geometry net at mesh vertices verts [V,3] (world space, e.g.
+    reconstruction()'s), zero where the gradient vanishes -- through mp_mesh_normals_async, the call FrameGraph(mesh_normals=
+    True) captures, so both give the same bits.  precision: that of query_gradient ("fp32": the exact kernel, what
+    reconstruction(normals=True) uses; "tc" / "auto": the tensor-core program's forward-mode derivative, a frame above the
+    head's feature limit differentiated exactly, decided on the device)."""
+    from .modeling.MonoPortNet import _MODES
+    from .modeling.geometry import perspective
+    if precision not in ("fp32", "tc", "auto"):
+        raise ValueError("precision must be one of 'fp32', 'tc', 'auto'; got %r" % (precision,))
+    feat = feats[-1][0]
+    if verts.dim() != 2 or verts.shape[1] != 3:
+        raise ValueError("verts must be [V,3]; got %s" % (tuple(verts.shape),))
+    if verts.device != feat.device:
+        raise ValueError("verts and features live on different devices")
+    device = feat.device
+    n = verts.shape[0]
+    out = torch.empty((n, 3), dtype=torch.float32, device=device)
+    if n == 0:
+        return out
+    v = verts.detach().to(torch.float32).contiguous()
+    counts = torch.tensor([n, 0], dtype=torch.int64, device=device)
+    count32 = torch.tensor([n], dtype=torch.int32, device=device)
+    scratch = torch.empty(3 * n, dtype=torch.float32, device=device)
+    with _lib.device_guard(device):
+        fh = net.feature_handle(feat)
+        proj = _lib.PROJ_PERSPECTIVE if net.projection is perspective else _lib.PROJ_ORTHOGONAL
+        _lib.check(_lib.load().mp_mesh_normals_async(
+            net.surface_classifier.handle(), fh.ptr, ctypes.c_void_p(v.data_ptr()), ctypes.c_void_p(counts.data_ptr()),
+            ctypes.c_void_p(count32.data_ptr()), n, _lib.calib12(calib_tensor), proj, ctypes.c_float(net.normalizer.scale),
+            _MODES[precision], ctypes.c_void_p(scratch.data_ptr()), ctypes.c_void_p(out.data_ptr()), _lib.stream_ptr(device)),
+            "mp_mesh_normals_async")
+    return out
+
+
+@torch.no_grad()
+def mesh_colours(netC, feats_C, verts, calib_tensor):
+    """Vertex colours of a mesh, upstream PIFu's gen_mesh_color: netC queried at the vertices verts [V,3] (world space),
+    pred * 0.5 + 0.5, as [V,3] -- for mesh_util.save_obj_mesh_with_color / save_ply_mesh(colors=).  FrameGraph(mesh_colours=
+    True) computes the same bits inside the captured step."""
+    return (netC.query(feats_C, verts.t()[None], calib_tensor)[0][0] * 0.5 + 0.5).t()
 
 
 def _unit_or_zero(v):
