@@ -331,8 +331,9 @@ static int build_level_list(mp_octree* h, int level, cudaStream_t st) {
     TopkF f{h->vol[dst_buf], h->balance, h->sel};
     TopkEmit em{h->idx, h->sel};
     MP_CUDA(mpscan::scan_emit(f, em, nf, h->sums, h->total, st));
-    // count = k exactly
-    set_i32_kernel<<<1, 1, 0, st>>>(h->count, (int32_t)k);
+    // count = k exactly, or 0 when level 0 found nothing occupied
+    topk_count_kernel<<<1, 1, 0, st>>>(h->count, h->stats + level, h->nonempty, (int32_t)k);
+    MP_CUDA(cudaGetLastError());
     return MP_OK;
   }
   if (interp_only) {
@@ -487,14 +488,12 @@ static int level_pass(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, c
   int rc = MP_OK;
   MpPointSrc src;
   fill_src_nodes(h, level, src, h->cap, true);
-  if (h->use_topk) {
+  if (h->use_topk) {   // (the count on the device is k, or 0 after an empty level 0: build_level_list)
     long long k = h->topk[level];
     const long long nf = (long long)h->res[level] * h->res[level] * h->res[level];
     if (k > nf) k = nf;
     if (k <= 0) return MP_OK;
     src.n = k;
-    src.count_dev = nullptr;
-    set_i64_kernel<<<1, 1, 0, st>>>(h->stats + level, k);
   }
   const float* vals = h->vals;
   const bool via_vals = lossless || h->shard_world > 1;

@@ -155,7 +155,6 @@ __global__ void iota_kernel(int32_t* idx, int n) {
 }
 
 // a scalar parameter -> device memory (instead of a host-to-device copy from a stack variable: graph-capturable)
-__global__ void set_i32_kernel(int32_t* p, int32_t v) { *p = v; }
 __global__ void set_i64_kernel(long long* p, long long v) { *p = v; }
 
 __global__ void set_u8_kernel(uint8_t* p, long long n, uint8_t v) {
@@ -269,6 +268,14 @@ __global__ void select_pick_kernel(SelectState* s, int pass) {
   }
   __syncthreads();
   if (threadIdx.x < 256) s->hist[threadIdx.x] = 0;
+}
+
+// A top-k level's node count: k after a non-empty level 0, else 0 (the generic run stops there and evaluates nothing
+// more); decided on the device so that a captured frame needs no host read.  Also the level's evaluated-node stat.
+__global__ void topk_count_kernel(int32_t* count, long long* stat, const int* nonempty, int32_t k) {
+  const int32_t n = *nonempty ? k : 0;
+  *count = n;
+  if (stat) *stat = n;
 }
 
 struct TopkF {   // low 32 bits: key < T ; high 32 bits: key == T

@@ -141,8 +141,9 @@ def bilinear_ref(feat, u, v):
 
     def tap(xx, yy, w):
         ok = (xx >= 0) & (xx <= W - 1) & (yy >= 0) & (yy <= H - 1)
-        xi = xx.clamp(0, W - 1).long()
-        yi = yy.clamp(0, H - 1).long()
+        # (a NaN coordinate -- a point with a NaN depth -- reads texel 0 with a NaN weight: the value stays NaN)
+        xi = xx.nan_to_num(0.0).clamp(0, W - 1).long()
+        yi = yy.nan_to_num(0.0).clamp(0, H - 1).long()
         return flat[:, yi * W + xi] * (w * ok.to(w.dtype))[None]
 
     return tap(x0, y0, w_nw) + tap(x1, y0, w_ne) + tap(x0, y1, w_sw) + tap(x1, y1, w_se)
@@ -329,7 +330,7 @@ def seg3d_lossless_ref(query_fn, resolutions, b_min=(-1, -1, -1), b_max=(1, 1, 1
         stats.append(dict(res=res, idx=idx))
         if idx.numel() == 0:
             continue
-        occ, known, extra = _eval_scatter(query_fn, occ, known, idx, res, stride, R, b_min, b_max)
+        occ, known, extra = _eval_scatter(query_fn, occ, known, idx, res, stride, R, b_min, b_max, balance)
         if not faster:
             # conflict loop
             interp_sign = None
@@ -342,7 +343,7 @@ def seg3d_lossless_ref(query_fn, resolutions, b_min=(-1, -1, -1), b_max=(1, 1, 1
                 if idx2.numel() == 0:
                     break
                 stats[-1]["idx"] = torch.cat([stats[-1]["idx"], idx2])
-                occ, known, extra = _eval_scatter(query_fn, occ, known, idx2, res, stride, R, b_min, b_max)
+                occ, known, extra = _eval_scatter(query_fn, occ, known, idx2, res, stride, R, b_min, b_max, balance)
     return (occ, stats) if return_stats else occ
 
 
@@ -353,7 +354,7 @@ def _xmajor_indices(mask):
     return p[:, 2] * res * res + p[:, 1] * res + p[:, 0]
 
 
-def _eval_scatter(query_fn, occ, known, idx, res, stride, R, b_min, b_max, balance=0.5):
+def _eval_scatter(query_fn, occ, known, idx, res, stride, R, b_min, b_max, balance):
     x = idx % res
     y = (idx // res) % res
     z = idx // (res * res)
@@ -454,10 +455,29 @@ def marching_cubes_ref(vol, iso=0.5):
 
 
 def analytic_volume(R, kind="sphere"):
-    """Deterministic float32 test volumes built from correctly-rounded IEEE ops only (+,-,*,/,sqrt)."""
+    """Deterministic float32 test volumes built from correctly-rounded IEEE ops only (+,-,*,/,sqrt) or a seeded generator.
+    sphere / ellipsoid / two_blobs lie inside the box; the others reach its faces:
+      corner  ball of radius 0.9 centred on the corner (1, 1, 1)
+      slab    |x| < 0.3, cut by four faces
+      ball01  {0, 1}-valued ball of radius 1.05 (every face and edge cuts it)
+      steps   a shell field quantised to {0, .25, .5, .75, 1}: nodes equal 0.5 (and any balance of that set) exactly
+      noise   uniform [0, 1) noise"""
     r = (np.arange(R, dtype=np.float32) + np.float32(0.5)) / np.float32(R) * np.float32(2) - np.float32(1)
     z, y, x = np.meshgrid(r, r, r, indexing="ij")
-    if kind == "sphere":
+    if kind == "noise":
+        return np.random.default_rng(R).random((R, R, R), dtype=np.float32)
+    if kind == "ball01":
+        return (np.sqrt(x * x + y * y + z * z) < np.float32(1.05)).astype(np.float32)
+    if kind == "steps":
+        d = np.sqrt(x * x + y * y + z * z)
+        f = np.clip(np.float32(0.5) + np.float32(1.5) * (np.float32(0.7) - d), np.float32(0), np.float32(1))
+        return (np.floor(f * np.float32(4) + np.float32(0.5)) / np.float32(4)).astype(np.float32)
+    if kind == "corner":
+        one = np.float32(1)
+        f = np.float32(0.9) - np.sqrt((x - one) ** 2 + (y - one) ** 2 + (z - one) ** 2)
+    elif kind == "slab":
+        f = np.float32(0.3) - np.abs(x)
+    elif kind == "sphere":
         d = np.sqrt(x * x + y * y + z * z)
         f = np.float32(0.6) - d
     elif kind == "ellipsoid":

@@ -1,9 +1,10 @@
 // TEST INFRASTRUCTURE ONLY: the surface render of monoport_b200/csrc/query_fp32.cu (the exact twin of the tensor-core colour
 // render) compiled unmodified on the CPU emulation layer.
-//   emu_colour_surface_fp32 in.bin out.f32 sms surface R count      mp_launch_surface_fp32: the N "points" of in.bin are
-//                                                                    vertex rows X, Y, Z (capacity N, count on the device);
-//                                                                    out = the [R,R,3] canvas (background EMU_CANVAS_BG,
-//                                                                    default 1)
+//   emu_colour_surface_fp32 in.bin out.f32 sms surface R count bx0 by0 bz0 bx1 by1 bz1
+//                                                                    mp_launch_surface_fp32 over the box [b_min, b_max]: the
+//                                                                    N "points" of in.bin are vertex rows X, Y, Z (capacity N,
+//                                                                    count on the device); out = the [R,R,3] canvas
+//                                                                    (background EMU_CANVAS_BG, default 1)
 //   emu_colour_surface_fp32 in.bin out.f32 sms rows                  mp_launch_query_fp32 on the N world points of in.bin;
 //                                                                    out = [res][N]
 // in.bin as for emu_query_fp32.  Range guard: EMU_GUARD (sense), EMU_TC_LIMIT (the head's limit, default +inf) and
@@ -42,9 +43,9 @@ void mp_set_error(const char* fmt, ...) {
 #include "../../monoport_b200/csrc/query_fp32.cu"
 
 int main(int argc, char** argv) {
-  const bool surface = argc == 7 && !strcmp(argv[4], "surface");
+  const bool surface = argc == 13 && !strcmp(argv[4], "surface");
   if (!surface && !(argc == 5 && !strcmp(argv[4], "rows"))) {
-    fprintf(stderr, "usage: emu_colour_surface_fp32 in.bin out.f32 sms (surface R count | rows)\n");
+    fprintf(stderr, "usage: emu_colour_surface_fp32 in.bin out.f32 sms (surface R count bx0 by0 bz0 bx1 by1 bz1 | rows)\n");
     return 2;
   }
   g_fake_sms = atoi(argv[3]);
@@ -102,7 +103,8 @@ int main(int argc, char** argv) {
     const float bg = getenv("EMU_CANVAS_BG") ? (float)atof(getenv("EMU_CANVAS_BG")) : 1.0f;
     out.assign((size_t)R * R * 3 + 1, bg);
     out.back() = -4242.f;
-    const float bmin[3] = {-1.f, -1.f, -1.f}, bmax[3] = {1.f, 1.f, 1.f};
+    float bmin[3], bmax[3];
+    for (int a = 0; a < 3; ++a) { bmin[a] = strtof(argv[7 + a], nullptr); bmax[a] = strtof(argv[10 + a], nullptr); }
     const MpSurfaceSrc surf = mp_surface_src(X.data(), Y.data(), Z.data(), &count, R, bmin, bmax, out.data());
     rc = mp_launch_surface_fp32(&mlp, &feat, surf, N, cal, nullptr, guard);
   } else {

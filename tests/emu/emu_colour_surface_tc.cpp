@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE ONLY: the surface render of monoport_b200/csrc/query_tc.cu (the colour head's tensor-core program
 // writing the visible-surface colours into a canvas) compiled UNMODIFIED for the CPU against the execution-model emulation
 // (cuda_emu.h) and the functional model of the wgmma / mbarrier / bulk-copy layer (tc_ptx_emu.h).
-//   emu_colour_surface_tc in.bin out.f32 sms R count [host]
+//   emu_colour_surface_tc in.bin out.f32 sms R count bx0 by0 bz0 bx1 by1 bz1 [host]      (the box [b_min, b_max])
 // in.bin as for emu_query_tc (header, z_scale, calib[12], feature map NCHW, "points" [3*N], the 5 layers); the N points are
 // the capacity of the vertex buffers: rows X, Y (integers) and Z (index space).
 //   default: mp_launch_surface_tc with the vertex count on the device (`count`, an int64 that may exceed N) and the range
@@ -68,11 +68,13 @@ int mp_launch_query_fp32(const mp_mlp*, const mp_feat*, const MpPointSrc&, const
                          const MpBatch*) { return MP_E_UNSUPPORTED; }
 
 int main(int argc, char** argv) {
-  if (argc < 6) { fprintf(stderr, "usage: emu_colour_surface_tc in.bin out.f32 sms R count [host]\n"); return 2; }
+  if (argc < 12) { fprintf(stderr, "usage: emu_colour_surface_tc in.bin out.f32 sms R count bx0 by0 bz0 bx1 by1 bz1 [host]\n"); return 2; }
   g_fake_sms = atoi(argv[3]);
   const int R = atoi(argv[4]);
   const long long count = atoll(argv[5]);
-  const bool host = argc >= 7 && !strcmp(argv[6], "host");
+  float bmin[3], bmax[3];
+  for (int a = 0; a < 3; ++a) { bmin[a] = strtof(argv[6 + a], nullptr); bmax[a] = strtof(argv[9 + a], nullptr); }
+  const bool host = argc >= 13 && !strcmp(argv[12], "host");
   FILE* f = fopen(argv[1], "rb");
   if (!f) { perror(argv[1]); return 2; }
   int32_t hd[8];
@@ -121,7 +123,6 @@ int main(int argc, char** argv) {
   const float bg = getenv("EMU_CANVAS_BG") ? (float)atof(getenv("EMU_CANVAS_BG")) : 1.0f;
   std::vector<float> canvas((size_t)R * R * 3 + 1, bg);
   canvas[(size_t)R * R * 3] = -4242.f;
-  const float bmin[3] = {-1.f, -1.f, -1.f}, bmax[3] = {1.f, 1.f, 1.f};
   int rc;
   if (host) {
     rc = mp_launch_colour_surface(&mlp, &feat, X.data(), Y.data(), Z.data(), count, R, bmin, bmax, cal, canvas.data(), nullptr);

@@ -33,6 +33,7 @@ struct Eng {
   std::vector<unsigned long long> sums;
   unsigned long long total[2] = {0, 0};
   int32_t count = 0;
+  int nonempty = 0;
   std::vector<long long> stats;
   SelectState sel;
   int cur = 0;
@@ -78,7 +79,7 @@ static void build_level_list(Eng& e, int level) {
       cuda_emu::launch(dim3(1), dim3(256), [&] { select_pick_kernel(sp, pass); });
     }
     scan_emit(TopkF{vf, bal, sp}, TopkEmit{e.idx.data(), sp}, nf, e, mpscan::NoPost());
-    e.count = (int32_t)k;
+    topk_count_kernel(&e.count, &e.stats[level], &e.nonempty, (int32_t)k);   // a <<<1, 1>>> launch: one call
     return;
   }
   if (interp_only) { e.count = 0; return; }
@@ -162,13 +163,14 @@ int main(int argc, char** argv) {
     uint8_t* kp = e.known[e.cur].data();
     cuda_emu::launch(dim3(grid_for(n0)), dim3(256), [&] { set_u8_kernel(kp, n0, 1); });
   }
-  int nonempty = 0;
   {
     const float* vp = e.vol[e.cur].data();
     const float bal = e.balance;
-    cuda_emu::launch(dim3(grid_for(n0)), dim3(256), [&] { any_gt_kernel(vp, n0, bal, &nonempty); });
+    int* ne = &e.nonempty;
+    cuda_emu::launch(dim3(grid_for(n0)), dim3(256), [&] { any_gt_kernel(vp, n0, bal, ne); });
   }
-  for (int level = 1; level < e.n_levels && nonempty; ++level) {
+  // like run_fused_levels, the levels run whatever level 0 found: an empty frame must produce empty node lists
+  for (int level = 1; level < e.n_levels; ++level) {
     build_level_list(e, level);
     const bool last = level == e.n_levels - 1;
     if (!e.use_topk && e.faster && last) break;
@@ -177,8 +179,9 @@ int main(int argc, char** argv) {
       long long n = e.count;
       if (e.use_topk) {
         const long long nf = (long long)e.res[level] * e.res[level] * e.res[level];
-        n = e.topk[level] > nf ? nf : e.topk[level];
-        if (n <= 0) break;
+        const long long k = e.topk[level] > nf ? nf : e.topk[level];
+        if (k <= 0) break;
+        n = n < k ? n : k;
       }
       float* volp = e.vol[e.cur].data();
       query_nodes(e, level, n, lossless ? e.vals.data() : nullptr, lossless ? nullptr : volp);
@@ -187,7 +190,7 @@ int main(int argc, char** argv) {
       uint8_t* kn = e.use_topk ? nullptr : e.known[e.cur].data();
       uint8_t* cf = lossless ? e.conflict.data() : nullptr;
       const float bal = e.balance;
-      const int32_t* cnt = e.use_topk ? nullptr : &e.count;
+      const int32_t* cnt = &e.count;
       const long long nmax = e.use_topk ? n : e.cap;
       cuda_emu::launch(dim3(grid_for(e.cap > (1 << 20) ? (1 << 20) : e.cap)), dim3(256),
                        [&] { scatter_kernel(ip, cnt, nmax, vsrc, volp, kn, cf, bal, lossless); });
@@ -198,7 +201,7 @@ int main(int argc, char** argv) {
   }
   if (e.total[1] != 0) { fprintf(stderr, "scan ticket not reset\n"); return 3; }
   // outputs
-  printf("%d", nonempty);
+  printf("%d", e.nonempty);
   FILE* fi = fopen(argv[5], "wb");
   for (int l = 0; l < e.n_levels; ++l) {
     printf(" %zu", e.evaluated[l].size());
@@ -207,7 +210,7 @@ int main(int argc, char** argv) {
   fclose(fi);
   printf("\n");
   FILE* fv = fopen(argv[4], "wb");
-  if (nonempty) fwrite(e.vol[e.cur].data(), 4, e.V, fv);
+  if (e.nonempty) fwrite(e.vol[e.cur].data(), 4, e.V, fv);
   fclose(fv);
   return 0;
 }

@@ -58,13 +58,16 @@ def build_net(case_or_net, Ws=None, bs=None, device="cuda", proj="orthogonal"):
     return net.eval()
 
 
-def lookup_query(field):
-    """query_func that reads a dense [R,R,R] field at the node nearest to each world point in [-1,1]^3
-    (bit-exact on CPU and GPU: pure gather).  Returns (fn_oracle(points[N,3])->[N], fn_engine(points=[1,N,3])->[1,1,N])."""
+def lookup_query(field, b_min=(-1, -1, -1), b_max=(1, 1, 1)):
+    """query_func that reads a dense [R,R,R] field at the node nearest to each world point of the box [b_min, b_max]
+    (bit-exact on CPU and GPU: pure gather).  The node is recovered in float64 from level_points' convention
+    p = (c + 0.5) / R * (b_max - b_min) + b_min.  Returns (fn_oracle(points[N,3])->[N], fn_engine(points=[1,N,3])->[1,1,N])."""
     R = field.shape[0]
+    lo = torch.tensor(b_min, dtype=torch.float64)
+    ext = torch.tensor(b_max, dtype=torch.float64) - lo
 
     def idx(p):
-        i = ((p.double() + 1) / 2 * R - 0.5).round().long().clamp(0, R - 1)
+        i = ((p.double() - lo.to(p.device)) / ext.to(p.device) * R - 0.5).round().long().clamp(0, R - 1)
         return i[..., 2], i[..., 1], i[..., 0]
 
     def fn_oracle(p):

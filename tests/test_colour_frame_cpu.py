@@ -21,6 +21,8 @@ pytestmark = pytest.mark.skipif(shutil.which("g++") is None or not os.path.exist
                                 reason="g++ / CUDA headers not available")
 
 R = 65
+UNIT = ((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0))
+B1 = ((-0.83, -1.17, -0.61), (0.91, 1.06, 0.77))     # asymmetric, no power-of-two extent: the axes cannot stand in for each other
 GUARD_NONE, GUARD_IN_RANGE, GUARD_OUT_OF_RANGE = 0, 1, 2
 
 
@@ -86,32 +88,37 @@ def _run(args, env=None, out_shape=(R, R, 3)):
     return torch.from_numpy(np.fromfile(args[2], dtype=np.float32)).reshape(out_shape), r.stdout
 
 
-def _fp32_surface(exe, tmp_path, sc, count, sms=3, n=200, env=None, feat=None):
+def _box_args(box):
+    return ["%.9g" % np.float32(v) for v in box[0] + box[1]]
+
+
+def _fp32_surface(exe, tmp_path, sc, count, sms=3, n=200, env=None, feat=None, box=UNIT):
     fin, fout = str(tmp_path / "s.bin"), str(tmp_path / "s.f32")
     _write(fin, sc, _vertex_rows(sc, n), feat)
-    return _run([exe, fin, fout, str(sms), "surface", str(R), str(count)], env)[0]
+    return _run([exe, fin, fout, str(sms), "surface", str(R), str(count)] + _box_args(box), env)[0]
 
 
-def _tc_surface(exe, tmp_path, sc, count, sms=2, n=200, env=None, host=False, feat=None):
+def _tc_surface(exe, tmp_path, sc, count, sms=2, n=200, env=None, host=False, feat=None, box=UNIT):
     fin, fout = str(tmp_path / "t.bin"), str(tmp_path / "t.f32")
     _write(fin, sc, _vertex_rows(sc, n), feat)
-    img, out = _run([exe, fin, fout, str(sms), str(R), str(count)] + (["host"] if host else []), env)
+    img, out = _run([exe, fin, fout, str(sms), str(R), str(count)] + _box_args(box) + (["host"] if host else []), env)
     return img, float(out.split()[0])
 
 
-def _want(sc, n=200):
+def _want(sc, n=200, box=UNIT):
     def query_c(points, calib):
         return spec.query_ref(sc["feat"], points, calib, sc["Ws"], sc["bs"], spec.LAST_TANH)
-    return spec.colorization_ref(query_c, sc["X"][:n], sc["Y"][:n], sc["Z"][:n], sc["cal"], resolution=R)
+    return spec.colorization_ref(query_c, sc["X"][:n], sc["Y"][:n], sc["Z"][:n], sc["cal"], resolution=R, b_min=box[0],
+                                 b_max=box[1])
 
 
 # ---- the exact fp32 render ---------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("sms", [1, 3])
-def test_exact_surface_render_matches_restatement(emu_fp32, tmp_path, scene, sms):
+@pytest.mark.parametrize("sms,box", [pytest.param(1, UNIT, id="1"), pytest.param(3, UNIT, id="3"), pytest.param(3, B1, id="3-B1")])
+def test_exact_surface_render_matches_restatement(emu_fp32, tmp_path, scene, sms, box):
     """colorization (RTL/main.py:212-249) with the exact kernel: within the fp32 query bar of the restatement driven by the
     oracle's query, and pixels without a vertex keep the canvas colour."""
-    got = _fp32_surface(emu_fp32, tmp_path, scene, 200, sms=sms)
-    want = _want(scene)
+    got = _fp32_surface(emu_fp32, tmp_path, scene, 200, sms=sms, box=box)
+    want = _want(scene, box=box)
     assert (got - want).abs().max().item() <= 2e-5
     untouched = torch.ones(R, R, dtype=torch.bool)
     untouched[scene["X"], scene["Y"]] = False
@@ -119,20 +126,23 @@ def test_exact_surface_render_matches_restatement(emu_fp32, tmp_path, scene, sms
 
 
 def test_exact_surface_render_is_the_rows_query_plus_scatter(emu_fp32, tmp_path, scene):
-    """Bit for bit: the fused render = the exact ROWS query on world points made with the same two fp32 roundings
-    (index * (b_max - b_min) / R, then + b_min), followed by the same scatter of v * 0.5 + 0.5."""
-    got = _fp32_surface(emu_fp32, tmp_path, scene, 200)
-    f32 = np.float32
-    scale = (f32(1) - f32(-1)) / f32(R)
-    v = _vertex_rows(scene).astype(f32)
-    v[2] = f32(R) - v[2]
-    world = (v * scale).astype(f32) + f32(-1)
-    fin, fout = str(tmp_path / "w.bin"), str(tmp_path / "w.f32")
-    _write(fin, scene, world)
-    vals = _run([emu_fp32, fin, fout, "3", "rows"], out_shape=(3, 200))[0].numpy()
-    want = np.ones((R, R, 3), f32)
-    want[scene["X"].numpy(), scene["Y"].numpy(), :] = ((vals * f32(0.5)).astype(f32) + f32(0.5)).T
-    assert np.array_equal(got.numpy().view(np.int32), want.view(np.int32))
+    """Bit for bit: the fused render = the exact ROWS query on world points made with the same two fp32 roundings per axis
+    (index * (b_max - b_min) / R, then + b_min), followed by the same scatter of v * 0.5 + 0.5 -- over the unit cube and a
+    box whose three extents differ."""
+    for box in (UNIT, B1):
+        got = _fp32_surface(emu_fp32, tmp_path, scene, 200, box=box)
+        f32 = np.float32
+        lo, hi = np.asarray(box[0], f32), np.asarray(box[1], f32)
+        scale = ((hi - lo) / f32(R)).astype(f32)[:, None]
+        v = _vertex_rows(scene).astype(f32)
+        v[2] = f32(R) - v[2]
+        world = (v * scale).astype(f32) + lo[:, None]
+        fin, fout = str(tmp_path / "w.bin"), str(tmp_path / "w.f32")
+        _write(fin, scene, world)
+        vals = _run([emu_fp32, fin, fout, "3", "rows"], out_shape=(3, 200))[0].numpy()
+        want = np.ones((R, R, 3), f32)
+        want[scene["X"].numpy(), scene["Y"].numpy(), :] = ((vals * f32(0.5)).astype(f32) + f32(0.5)).T
+        assert np.array_equal(got.numpy().view(np.int32), want.view(np.int32)), box
 
 
 def test_exact_surface_render_device_count(emu_fp32, tmp_path, scene):
@@ -161,14 +171,16 @@ def test_exact_surface_render_guard_sense(emu_fp32, tmp_path, scene, limit, writ
 # ---- the tensor-core render with the count on the device ---------------------------------------------------------------
 def test_tc_surface_render_device_count_equals_host_count(emu_tc, tmp_path, scene):
     """The render of a captured step (count read on the device, capacity n) equals the eager launch given the same count on
-    the host, bit for bit; vertices past the count keep the background, and a count above the capacity is clamped."""
+    the host, bit for bit, over the unit cube and a box whose three extents differ; vertices past the count keep the
+    background, and a count above the capacity is clamped."""
     n, k = 130, 100
-    dev, _ = _tc_surface(emu_tc, tmp_path, scene, k, n=n, env={"EMU_CANVAS_BG": "0.25"})
-    host, _ = _tc_surface(emu_tc, tmp_path, scene, k, n=n, host=True, env={"EMU_CANVAS_BG": "0.25"})
-    assert torch.equal(dev, host)
     X, Y = scene["X"], scene["Y"]
-    assert bool((dev[X[k:n], Y[k:n]] == 0.25).all())
-    assert (dev[X[:k], Y[:k]] - _want(scene, k)[X[:k], Y[:k]]).abs().max().item() <= 1e-4
+    for box in (B1, UNIT):
+        dev, _ = _tc_surface(emu_tc, tmp_path, scene, k, n=n, env={"EMU_CANVAS_BG": "0.25"}, box=box)
+        host, _ = _tc_surface(emu_tc, tmp_path, scene, k, n=n, host=True, env={"EMU_CANVAS_BG": "0.25"}, box=box)
+        assert torch.equal(dev, host)
+        assert bool((dev[X[k:n], Y[k:n]] == 0.25).all())
+        assert (dev[X[:k], Y[:k]] - _want(scene, k, box)[X[:k], Y[:k]]).abs().max().item() <= 1e-4, box
     clamped, _ = _tc_surface(emu_tc, tmp_path, scene, 10 ** 9, n=n, env={"EMU_CANVAS_BG": "0.25"})
     host_all, _ = _tc_surface(emu_tc, tmp_path, scene, n, n=n, host=True, env={"EMU_CANVAS_BG": "0.25"})
     assert torch.equal(clamped, host_all)

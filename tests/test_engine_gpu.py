@@ -13,23 +13,35 @@ from helpers import GOLDEN, build_net, lookup_query
 pytestmark = pytest.mark.gpu
 
 RES = [9, 17, 33, 65]
+UNIT = ((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0))
+B1 = ((-0.83, -1.17, -0.61), (0.91, 1.06, 0.77))          # asymmetric, no power-of-two extent
+B_PIFU = ((-128.0, -28.0, -128.0), (128.0, 228.0, 128.0))  # upstream PIFu's reconstruction box
 
 
-def _engine(kind, fn, **kw):
+def _engine(kind, fn, box=UNIT, balance=0.5, **kw):
     from monoport_b200.engine import Seg3dLossless, Seg3dTopk
-    b_min = np.array([[-1.0, -1.0, -1.0]], dtype=np.float32)
-    b_max = np.array([[1.0, 1.0, 1.0]], dtype=np.float32)
+    b_min = np.array([box[0]], dtype=np.float32)
+    b_max = np.array([box[1]], dtype=np.float32)
     if kind == "topk":
-        return Seg3dTopk(query_func=fn, b_min=b_min, b_max=b_max, resolutions=RES, **kw).to("cuda")
-    return Seg3dLossless(query_func=fn, b_min=b_min, b_max=b_max, resolutions=RES, balance_value=0.5,
+        return Seg3dTopk(query_func=fn, b_min=b_min, b_max=b_max, resolutions=RES, balance_value=balance, **kw).to("cuda")
+    return Seg3dLossless(query_func=fn, b_min=b_min, b_max=b_max, resolutions=RES, balance_value=balance,
                          use_cuda_impl=False, faster=(kind == "faster")).to("cuda")
 
 
-@pytest.mark.parametrize("field_kind", ["sphere", "two_blobs", "ellipsoid"])
+@pytest.mark.parametrize("field_kind,box,balance", [
+    pytest.param("sphere", UNIT, 0.5, id="sphere"), pytest.param("two_blobs", UNIT, 0.5, id="two_blobs"),
+    pytest.param("ellipsoid", UNIT, 0.5, id="ellipsoid"),
+    # boxes whose three extents differ (a swapped or shared axis extent changes the points), other balances, fields that
+    # reach the box and nodes equal to the balance
+    pytest.param("sphere", B1, 0.5, id="sphere-B1"), pytest.param("corner", B1, 0.3, id="corner-B1-0.3"),
+    pytest.param("slab", B1, 0.7, id="slab-B1-0.7"), pytest.param("steps", B1, 0.3, id="steps-B1-0.3"),
+    pytest.param("noise", B1, 0.7, id="noise-B1-0.7"), pytest.param("steps", B_PIFU, 0.5, id="steps-PIFU"),
+    pytest.param("noise", B_PIFU, 0.3, id="noise-PIFU-0.3"), pytest.param("corner", B_PIFU, 0.7, id="corner-PIFU-0.7"),
+    pytest.param("slab", B_PIFU, 0.5, id="slab-PIFU")])
 @pytest.mark.parametrize("kind", ["faster", "lossless", "topk"])
-def test_engine_matches_oracle_bit_exact(kind, field_kind):
+def test_engine_matches_oracle_bit_exact(kind, field_kind, box, balance):
     field = torch.from_numpy(spec.analytic_volume(65, field_kind))
-    fn_o, fn_e = lookup_query(field)
+    fn_o, fn_e = lookup_query(field, *box)
     recorded = []
 
     def fn_rec(points, **kw):
@@ -38,11 +50,11 @@ def test_engine_matches_oracle_bit_exact(kind, field_kind):
 
     if kind == "topk":
         kpts = [0, 2500, 9000, 40000]
-        want, stats = spec.seg3d_topk_ref(fn_o, RES, kpts, return_stats=True)
-        eng = _engine("topk", fn_rec, num_points=kpts)
+        want, stats = spec.seg3d_topk_ref(fn_o, RES, kpts, *box, balance=balance, return_stats=True)
+        eng = _engine("topk", fn_rec, box, balance, num_points=kpts)
     else:
-        want, stats = spec.seg3d_lossless_ref(fn_o, RES, faster=(kind == "faster"), return_stats=True)
-        eng = _engine(kind, fn_rec)
+        want, stats = spec.seg3d_lossless_ref(fn_o, RES, *box, balance=balance, faster=(kind == "faster"), return_stats=True)
+        eng = _engine(kind, fn_rec, box, balance)
     got = eng(anything="goes")                        # unknown kwargs are forwarded (RTL/main.py:392-394)
     assert got.shape == (1, 1, 65, 65, 65) and got.device.type == "cuda"
     assert torch.equal(got[0, 0].cpu(), want), "volume must be bit-identical to the restatement"
@@ -56,7 +68,7 @@ def test_engine_matches_oracle_bit_exact(kind, field_kind):
             continue
         stride = 64 // (res - 1)
         c = torch.stack([idx % res, (idx // res) % res, idx // (res * res)], 1) * stride
-        want_pts.append(spec.level_points(c, 65, (-1, -1, -1), (1, 1, 1)))
+        want_pts.append(spec.level_points(c, 65, *box))
     assert torch.equal(got_pts, torch.cat(want_pts)), "evaluated node sets / order differ"
 
 
@@ -117,12 +129,23 @@ def test_fused_engine_equals_generic_engine_with_mlp():
                 assert ((a[0, 0].cpu() > 0.5) != (want > 0.5)).sum().item() <= 2   # fp32 summation-order ties only
 
 
-@pytest.mark.parametrize("kind,R", [("sphere", 33), ("two_blobs", 65), ("ellipsoid", 40)])
-def test_marching_cubes_matches_oracle(kind, R):
+@pytest.mark.parametrize("kind,R,iso", [
+    pytest.param("sphere", 33, 0.5, id="sphere-33"), pytest.param("two_blobs", 65, 0.5, id="two_blobs-65"),
+    pytest.param("ellipsoid", 40, 0.5, id="ellipsoid-40"),
+    # nodes equal to the iso value; surfaces cut by the volume's faces; dense noise on odd and tiny shapes
+    pytest.param("steps", 33, 0.5, id="steps-33"), pytest.param("steps", 33, 0.25, id="steps-33-iso0.25"),
+    pytest.param("corner", 65, 0.5, id="corner-65"), pytest.param("noise", (20, 17, 23), 0.5, id="noise-20x17x23"),
+    pytest.param("noise", (3, 70, 2), 0.5, id="noise-3x70x2"), pytest.param("noise", (2, 3, 257), 0.5, id="noise-2x3x257"),
+    pytest.param("noise", (9, 40, 35), 0.5, id="noise-9x40x35")])
+def test_marching_cubes_matches_oracle(kind, R, iso):
     from monoport_b200.recon import marching_cubes
-    vol = spec.analytic_volume(R, kind)
-    V, F = spec.marching_cubes_ref(vol)
-    v, f = marching_cubes(torch.from_numpy(vol).cuda())
+    if kind == "noise":          # (the shapes of the CPU model's noise cases, same generator)
+        vol = np.random.default_rng(sum(R)).random(R, dtype=np.float32)
+    else:
+        vol = spec.analytic_volume(R, kind)
+    V, F = spec.marching_cubes_ref(vol, iso)
+    v, f = marching_cubes(torch.from_numpy(vol).cuda(), iso)
+    assert len(F) > 0
     assert f.dtype == torch.int32 and np.array_equal(f.cpu().numpy(), F), "topology must be bit-exact"
     assert np.abs(v.cpu().numpy() - V).max() <= 1e-6
 

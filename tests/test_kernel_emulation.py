@@ -49,11 +49,17 @@ def _run_mcubes(exe, vol, tmp_path, iso=0.5):
     return v, f
 
 
-@pytest.mark.parametrize("kind,R", [("sphere", 33), ("ellipsoid", 40), ("two_blobs", 49)])
-def test_mcubes_kernels_match_oracle_on_analytic_volumes(emu_mcubes, tmp_path, kind, R):
+@pytest.mark.parametrize("kind,R,iso", [
+    pytest.param("sphere", 33, 0.5, id="sphere-33"), pytest.param("ellipsoid", 40, 0.5, id="ellipsoid-40"),
+    pytest.param("two_blobs", 49, 0.5, id="two_blobs-49"), pytest.param("steps", 33, 0.5, id="steps-33"),
+    pytest.param("steps", 33, 0.25, id="steps-33-iso0.25"), pytest.param("corner", 33, 0.5, id="corner-33"),
+    pytest.param("ball01", 17, 0.5, id="ball01-17")])
+def test_mcubes_kernels_match_oracle_on_analytic_volumes(emu_mcubes, tmp_path, kind, R, iso):
+    """steps: nodes equal to the iso value (not inside: t = 0 or 1 on the edge); corner / ball01: cut by the box faces."""
     vol = spec.analytic_volume(R, kind)
-    V, F = spec.marching_cubes_ref(vol)
-    v, f = _run_mcubes(emu_mcubes, vol, tmp_path)
+    V, F = spec.marching_cubes_ref(vol, iso)
+    v, f = _run_mcubes(emu_mcubes, vol, tmp_path, iso)
+    assert len(F) > 0
     assert np.array_equal(f, F), "topology must be bit-exact"
     assert v.shape == V.shape and np.array_equal(v, V)
     if kind == "sphere":
@@ -124,10 +130,10 @@ def emu_octree(tmp_path_factory):
     return _build(str(tmp_path_factory.mktemp("emu_octree")), "emu_octree")
 
 
-def _run_octree(exe, tmp_path, mode, field, res, kpts=None):
+def _run_octree(exe, tmp_path, mode, field, res, kpts=None, balance=0.5):
     fin, fvol, fidx = (str(tmp_path / n) for n in ("dense.f32", "vol.f32", "idx.i32"))
     np.ascontiguousarray(field, dtype=np.float32).tofile(fin)
-    args = [exe, mode, "0.5", fin, fvol, fidx, str(len(res))] + [str(r) for r in res] + [str(k) for k in (kpts or [])]
+    args = [exe, mode, repr(float(balance)), fin, fvol, fidx, str(len(res))] + [str(r) for r in res] + [str(k) for k in (kpts or [])]
     r = subprocess.run(args, capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stderr
     out = [int(x) for x in r.stdout.split()]
@@ -135,11 +141,21 @@ def _run_octree(exe, tmp_path, mode, field, res, kpts=None):
     return out[0], out[1:], vol, np.fromfile(fidx, dtype=np.int32)
 
 
-@pytest.mark.parametrize("mode,field_kind,res", [
-    ("faster", "sphere", [9, 17, 33, 65]), ("faster", "two_blobs", [5, 9, 17, 33, 65]), ("faster", "ellipsoid", [9, 17, 33]),
-    pytest.param("lossless", "two_blobs", [9, 17, 33], marks=full_only), pytest.param("lossless", "sphere", [9, 17], marks=()),
-    pytest.param("topk", "sphere", [9, 17, 33], marks=full_only), pytest.param("topk", "sphere", [9, 17], marks=())])
-def test_octree_kernels_match_restatement(emu_octree, tmp_path, mode, field_kind, res):
+@pytest.mark.parametrize("mode,field_kind,res,balance", [
+    pytest.param("faster", "sphere", [9, 17, 33, 65], 0.5, id="faster-sphere-res0"),
+    pytest.param("faster", "two_blobs", [5, 9, 17, 33, 65], 0.5, id="faster-two_blobs-res1"),
+    pytest.param("faster", "ellipsoid", [9, 17, 33], 0.5, id="faster-ellipsoid-res2"),
+    pytest.param("lossless", "two_blobs", [9, 17, 33], 0.5, marks=full_only, id="lossless-two_blobs-res3"),
+    pytest.param("lossless", "sphere", [9, 17], 0.5, id="lossless-sphere-res4"),
+    pytest.param("topk", "sphere", [9, 17, 33], 0.5, marks=full_only, id="topk-sphere-res5"),
+    pytest.param("topk", "sphere", [9, 17], 0.5, id="topk-sphere-res6"),
+    # fields that reach the box (clamped dilation boxes with mixed neighbourhoods), nodes equal to the balance, other balances
+    ("lossless", "noise", [5, 9, 17], 0.3), ("lossless", "noise", [5, 9, 17], 0.7), ("faster", "noise", [5, 9, 17, 33], 0.3),
+    ("faster", "corner", [9, 17, 33], 0.5), ("faster", "slab", [9, 17, 33], 0.7), ("faster", "steps", [5, 9, 17, 33], 0.5),
+    ("lossless", "corner", [9, 17], 0.3), ("lossless", "steps", [9, 17], 0.5), ("lossless", "slab", [5, 9, 17], 0.7),
+    ("lossless", "ball01", [5, 9, 17], 0.5), ("topk", "noise", [5, 9, 17], 0.3), ("topk", "steps", [9, 17], 0.5),
+    ("topk", "corner", [9, 17], 0.7)])
+def test_octree_kernels_match_restatement(emu_octree, tmp_path, mode, field_kind, res, balance):
     import torch
     from helpers import lookup_query
     R = res[-1]
@@ -147,10 +163,10 @@ def test_octree_kernels_match_restatement(emu_octree, tmp_path, mode, field_kind
     fn_o, _ = lookup_query(torch.from_numpy(field))
     kpts = [0, 1500, 5000][:len(res)] if mode == "topk" else None
     if mode == "topk":
-        want, stats = spec.seg3d_topk_ref(fn_o, res, kpts, return_stats=True)
+        want, stats = spec.seg3d_topk_ref(fn_o, res, kpts, balance=balance, return_stats=True)
     else:
-        want, stats = spec.seg3d_lossless_ref(fn_o, res, faster=(mode == "faster"), return_stats=True)
-    nonempty, counts, vol, idx = _run_octree(emu_octree, tmp_path, mode, field, res, kpts)
+        want, stats = spec.seg3d_lossless_ref(fn_o, res, balance=balance, faster=(mode == "faster"), return_stats=True)
+    nonempty, counts, vol, idx = _run_octree(emu_octree, tmp_path, mode, field, res, kpts, balance)
     assert nonempty == 1 and want is not None
     assert counts == [int(s["idx"].numel()) for s in stats]
     assert np.array_equal(vol.reshape(R, R, R), want.numpy()), "volume must be bit-identical to the restatement"
@@ -158,8 +174,13 @@ def test_octree_kernels_match_restatement(emu_octree, tmp_path, mode, field_kind
 
 
 def test_octree_kernels_empty_field(emu_octree, tmp_path):
-    nonempty, counts, vol, idx = _run_octree(emu_octree, tmp_path, "faster", np.zeros((33, 33, 33), np.float32), [9, 17, 33])
-    assert nonempty == 0 and counts[0] == 729 and sum(counts[1:]) == 0 and vol.size == 0
+    """Level 0 finds nothing occupied: the levels still run (no host read of the flag, as in a captured frame) but evaluate
+    nothing -- also the top-k levels, whose node count is gated on the device-side flag."""
+    for mode in ("faster", "lossless", "topk"):
+        kpts = [0, 100, 2000] if mode == "topk" else None
+        nonempty, counts, vol, idx = _run_octree(emu_octree, tmp_path, mode, np.zeros((33, 33, 33), np.float32), [9, 17, 33],
+                                                 kpts)
+        assert nonempty == 0 and counts[0] == 729 and sum(counts[1:]) == 0 and vol.size == 0, mode
 
 
 # ---- visible-surface kernels (surface_kernels.cuh) against the goldens produced by the unmodified RTL/recon.py -------------
@@ -168,7 +189,8 @@ def emu_surface(tmp_path_factory):
     return _build(str(tmp_path_factory.mktemp("emu_surface")), "emu_surface")
 
 
-@pytest.mark.parametrize("golden", ["fv_sphere_33", "fv_two_blobs_65", "fv_ellipsoid_65"])
+@pytest.mark.parametrize("golden", ["fv_sphere_33", "fv_two_blobs_65", "fv_ellipsoid_65"] + [
+    "fv_%s_%d" % (k, R) for k in ("corner", "slab", "ball01", "noise") for R in (33, 65)])
 def test_surface_kernels_match_reference_golden(emu_surface, tmp_path, golden_dir, golden):
     g = np.load(os.path.join(golden_dir, golden + ".npz"))
     R = int(g["R"])

@@ -263,6 +263,7 @@ def test_colour_surface_render_on_a_non_square_map(emu_surface, tmp_path, progra
     fin, fout = str(tmp_path / "s.bin"), str(tmp_path / "s.f32")
     _write_input(fin, c["feat"], rows, c["calib"], c["proj"], 3, c["last_op"], c["Ws"], c["bs"])
     args = [fin, fout, "2", str(R_CANVAS), str(n)] if program == "tc" else [fin, fout, "2", "surface", str(R_CANVAS), str(n)]
+    args += ["-1", "-1", "-1", "1", "1", "1"]                 # the render box [b_min, b_max]
     r = subprocess.run([emu_surface[program]] + args, capture_output=True, text=True, timeout=3600)
     assert r.returncode == 0, r.stderr[-2000:]
     got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(R_CANVAS, R_CANVAS, 3)

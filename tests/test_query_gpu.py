@@ -84,26 +84,42 @@ def test_calib_3x4_and_4x4_agree():
     assert torch.equal(a, b)
 
 
+def _box_calib(cal, b_min, b_max):
+    """the calibration that sees the box [b_min, b_max] as the scene calib sees [-1,1]^3: cal @ (scale, translate)"""
+    lo, hi = np.asarray(b_min, np.float64), np.asarray(b_max, np.float64)
+    M = np.eye(4)
+    M[:3, :3] = np.diag(2.0 / (hi - lo))
+    M[:3, 3] = -(hi + lo) / (hi - lo)
+    return torch.from_numpy(cal[0].double().numpy() @ M).float()[None]
+
+
 def test_random_case_vs_oracle_and_grid_mode():
-    """Fresh seeded case not in the goldens + dense-grid mode == points mode on the same node centres."""
+    """Fresh seeded case not in the goldens + dense-grid mode == points mode on the same node centres, over the unit cube, an
+    asymmetric box without a power-of-two extent, and upstream PIFu's box (with the calibration that maps it onto the
+    scene's): the grid's node centres are level_points' three fp32 roundings per axis."""
     Ws, bs = spec.make_weights(spec.G_CHANNELS, 1234)
     feat = spec.make_feat(256, 128, 128, 77)
-    cal = spec.scene_calib(20, -50)
+    cal0 = spec.scene_calib(20, -50)
     net = build_net("G", Ws, bs)
     R = 21
     coords = spec._grid_coords(R, 1)
-    world = spec.level_points(coords, R, (-1, -1, -1), (1, 1, 1))          # [N,3]
-    want = spec.query_ref(feat, world.t().contiguous(), cal, Ws, bs, spec.LAST_SIGMOID)[0]
-    for mode in _modes(net):
-        net.precision = mode
-        vol = net.query_grid(feat.cuda(), cal.cuda(), R, (-1, -1, -1), (1, 1, 1))
-        assert vol.shape == (R, R, R)
-        assert (vol.reshape(-1).cpu() - want).abs().max().item() <= TOL[mode]
-        pts = net.query([[feat.cuda()]], world.t().contiguous()[None].cuda(), calibs=cal.cuda())[0][0, 0]
-        assert torch.equal(pts, vol.reshape(-1)), "grid mode and points mode must agree bit-for-bit"
-        # slab == rows of the full volume
-        slab = net.query_grid(feat.cuda(), cal.cuda(), R, (-1, -1, -1), (1, 1, 1), z0=5, nz=7)
-        assert torch.equal(slab, vol[5:12])
+    for b_min, b_max in (((-1, -1, -1), (1, 1, 1)), ((-0.83, -1.17, -0.61), (0.91, 1.06, 0.77)),
+                         ((-128, -28, -128), (128, 228, 128))):
+        cal = _box_calib(cal0, b_min, b_max)
+        world = spec.level_points(coords, R, b_min, b_max)          # [N,3]
+        want = spec.query_ref(feat, world.t().contiguous(), cal, Ws, bs, spec.LAST_SIGMOID)[0]
+        for mode in _modes(net):
+            net.precision = mode
+            vol = net.query_grid(feat.cuda(), cal.cuda(), R, b_min, b_max)
+            assert vol.shape == (R, R, R)
+            assert (vol.reshape(-1).cpu() - want).abs().max().item() <= TOL[mode], (b_min, mode)
+            pts = net.query([[feat.cuda()]], world.t().contiguous()[None].cuda(), calibs=cal.cuda())[0][0, 0]
+            assert torch.equal(pts, vol.reshape(-1)), "grid mode and points mode must agree bit-for-bit"
+            # slab == rows of the full volume
+            slab = net.query_grid(feat.cuda(), cal.cuda(), R, b_min, b_max, z0=5, nz=7)
+            assert torch.equal(slab, vol[5:12])
+            part = net.query_grid_range(feat.cuda(), cal.cuda(), R, b_min, b_max, lin0=1234, n=4321)
+            assert torch.equal(part, vol.reshape(-1)[1234:1234 + 4321])
 
 
 def test_host_buffer_entry_point():
