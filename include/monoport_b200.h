@@ -153,6 +153,15 @@ int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const float* point
 int mp_query_points_count(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
                           int64_t point_stride, const float* calib12, int projection, float z_scale, float* out_dev,
                           int64_t ld_out, const int32_t* count_dev, int mode, void* stream);
+/* Device-calibration twins (_dcal) of the enqueue-only calls mp_query_points_count, mp_octree_run_fused_async,
+ * mp_colorize_surface_async, mp_surface_normals_async and mp_mesh_normals_async: calib_dev in place of calib12 is 12 float32
+ * values in DEVICE memory, rows 0..2 of [R|t] like calib12, read by the kernels when they run -- a captured CUDA graph
+ * then follows whatever camera the caller writes there before each replay.  NULL is refused (a call without a camera is
+ * its twin with calib12 == NULL).  projection and z_scale stay arguments.  Everything else -- arguments, modes, range guard,
+ * refusals -- is the twin's, and so are the results: bit for bit what the twin gives with the same 12 floats. */
+int mp_query_points_count_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                               int64_t point_stride, const float* calib_dev, int projection, float z_scale, float* out_dev,
+                               int64_t ld_out, const int32_t* count_dev, int mode, void* stream);
 /* Same call with HOST buffers (points [3,N], out [Res,N], feature map NCHW fp32 or NULL to reuse the
  * uploaded one): copies in, runs, copies out, synchronises.  This is what bench.py's e2e leg times. */
 int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,
@@ -254,6 +263,10 @@ int mp_octree_run_fused(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const fl
  * mp_octree_run_fused).  Synchronises. */
 int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib12, int projection,
                               float z_scale, int mode, float* out_dev, void* stream);
+/* mp_octree_run_fused_async with the camera in device memory (see mp_query_points_count_dcal): every query launch of the
+ * run, the bodies of the lossless WHILE nodes included, reads calib_dev when it runs.  A sharded handle is refused. */
+int mp_octree_run_fused_async_dcal(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib_dev, int projection,
+                                   float z_scale, int mode, float* out_dev, void* stream);
 int mp_octree_fetch(mp_octree_t* h, int* nonempty, int64_t* stats_host, void* stream);
 int mp_octree_fetch_loops(mp_octree_t* h, int32_t* passes_per_level, void* stream);
 int mp_octree_shard_export(mp_octree_t* h, unsigned char* handles192);
@@ -316,6 +329,11 @@ int mp_colorize_surface(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, co
 int mp_colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev, const float* z_dev,
                               const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
                               const float* calib12, int projection, float z_scale, int mode, float* canvas_dev, void* stream);
+/* mp_colorize_surface_async with the camera in device memory (see mp_query_points_count_dcal). */
+int mp_colorize_surface_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev, const float* z_dev,
+                                   const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
+                                   const float* calib_dev, int projection, float z_scale, int mode, float* canvas_dev,
+                                   void* stream);
 /* The normal image of the demo (RTL/main.py:212-228, colorization(norm=...)): canvas[X[i], Y[i], :] =
  * clamp((norm[i] + 1) / 2, 0, 1) for the first min(*count_dev, capacity) vertices, bit for bit what torch gives (NaN
  * normals stay NaN).  Enqueue-only like the call above; capacity <= R*R. */
@@ -331,6 +349,11 @@ int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_de
                              const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
                              const float* calib12, int projection, float z_scale, int mode, float* scratch_dev, float* norm_dev,
                              void* stream);
+/* mp_surface_normals_async with the camera in device memory (see mp_query_points_count_dcal). */
+int mp_surface_normals_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev, const float* z_dev,
+                                  const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
+                                  const float* calib_dev, int projection, float z_scale, int mode, float* scratch_dev,
+                                  float* norm_dev, void* stream);
 /* Analytic normals at mesh vertices, enqueue-only: verts_dev = mp_mcubes_run_async's world-space [capacity][3] vertices,
  * counts_dev / count32_dev its counts (the first min(counts_dev[0], capacity) vertices are evaluated).  norm_dev[i] =
  * -g / |g| with g the geometry head's gradient at vertex i (zero where it vanishes), as reconstruction(normals=True) gives
@@ -338,6 +361,10 @@ int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_de
 int mp_mesh_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const float* verts_dev, const int64_t* counts_dev,
                           const int32_t* count32_dev, int64_t capacity, const float* calib12, int projection, float z_scale,
                           int mode, float* scratch_dev, float* norm_dev, void* stream);
+/* mp_mesh_normals_async with the camera in device memory (see mp_query_points_count_dcal). */
+int mp_mesh_normals_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const float* verts_dev, const int64_t* counts_dev,
+                               const int32_t* count32_dev, int64_t capacity, const float* calib_dev, int projection,
+                               float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -95,6 +95,18 @@ SIGNATURES = {
                                          P(c_float), P(c_float), c_int, c_float, c_int, c_void_p, c_void_p, c_void_p]),
     "mp_mesh_normals_async": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, P(c_float), c_int, c_float,
                                       c_int, c_void_p, c_void_p, c_void_p]),
+    # the device-calibration twins: calib_dev (12 float32 in device memory) in place of calib12
+    "mp_query_points_count_dcal": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, c_void_p, c_int, c_float,
+                                           c_void_p, c_int64, c_void_p, c_int, c_void_p]),
+    "mp_octree_run_fused_async_dcal": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_int, c_void_p,
+                                               c_void_p]),
+    "mp_colorize_surface_async_dcal": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
+                                               P(c_float), P(c_float), c_void_p, c_int, c_float, c_int, c_void_p, c_void_p]),
+    "mp_surface_normals_async_dcal": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
+                                              P(c_float), P(c_float), c_void_p, c_int, c_float, c_int, c_void_p, c_void_p,
+                                              c_void_p]),
+    "mp_mesh_normals_async_dcal": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_int, c_float,
+                                           c_int, c_void_p, c_void_p, c_void_p]),
     "mp_forward_vertices":(c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, P(c_int64),
                                     c_void_p]),
     "mp_forward_vertices_scratch_bytes": (c_int64, [c_int]),

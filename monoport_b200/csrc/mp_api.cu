@@ -249,6 +249,22 @@ void mp_fill_calib(MpCalib& c, const float* calib12, int projection, float z_sca
   c.z_scale = z_scale;
 }
 
+// The camera of a single-map call: calib12 (host memory, or none) in the kernel parameters, or -- calib_dev set, the _dcal
+// entry points -- 12 floats in device memory that the kernels read when they run.  Returns the batch to launch with
+// (nullptr: the by-value camera).
+const MpBatch* mp_single_calib(MpCalib& cal, MpBatch& bt, const float* calib12, const float* calib_dev, int projection,
+                               float z_scale) {
+  if (!calib_dev) {
+    mp_fill_calib(cal, calib12, projection, z_scale);
+    return nullptr;
+  }
+  mp_fill_calib(cal, nullptr, projection, z_scale);
+  cal.has = 1;
+  cal.perspective = projection == MP_PROJ_PERSPECTIVE;
+  bt = mp_device_calib(calib_dev);
+  return &bt;
+}
+
 void mp_fill_grid_geom(MpPointSrc& s, int res, int node_stride, int r_final, const float* bmin, const float* bmax) {
   s.res = res;
   s.node_stride = node_stride;
@@ -294,7 +310,7 @@ int mp_query_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const M
 static int query_points(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n, int64_t batch_stride,
                         int64_t row_stride, int64_t point_stride, const float* calib12, const float* calibs_dev, int projection,
                         float z_scale, float* out_dev, int64_t out_batch_stride, int64_t ld_out, int mode, void* stream,
-                        bool batched, const int32_t* count_dev = nullptr) {
+                        bool batched, const int32_t* count_dev = nullptr, const float* calib_dev = nullptr) {
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE(n >= 0 && row_stride >= 1 && point_stride >= 1 && ld_out >= n, "bad sizes n=%lld strides=%lld,%lld ld_out=%lld",
              (long long)n, (long long)row_stride, (long long)point_stride, (long long)ld_out);
@@ -317,10 +333,11 @@ static int query_points(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* poin
   src.n = n;
   src.count_dev = count_dev;
   MpCalib cal;
-  mp_fill_calib(cal, calib12, projection, z_scale);
+  MpBatch one;
+  const MpBatch* single = mp_single_calib(cal, one, calib12, calib_dev, projection, z_scale);
   MpOutDst dst;
   dst.out = out_dev; dst.ld = ld_out; dst.scatter_vol = nullptr;
-  if (!batched) return mp_query_dispatch(mlp, feat, src, cal, dst, mode, (cudaStream_t)stream);
+  if (!batched) return mp_query_dispatch(mlp, feat, src, cal, dst, mode, (cudaStream_t)stream, single);
   MpBatch bt;
   bt.B = B;
   bt.pt_stride = batch_stride;
@@ -345,6 +362,14 @@ extern "C" int mp_query_points_count(mp_mlp_t* mlp, mp_feat_t* feat, const float
                       ld_out, mode, stream, false, count_dev);
 }
 
+extern "C" int mp_query_points_count_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
+                                          int64_t point_stride, const float* calib_dev, int projection, float z_scale, float* out_dev,
+                                          int64_t ld_out, const int32_t* count_dev, int mode, void* stream) {
+  MP_REQUIRE(calib_dev, "NULL calib_dev");
+  return query_points(mlp, feat, 1, points_dev, n, 0, row_stride, point_stride, nullptr, nullptr, projection, z_scale, out_dev, 0,
+                      ld_out, mode, stream, false, count_dev, calib_dev);
+}
+
 extern "C" int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
                                      int64_t batch_stride, int64_t row_stride, int64_t point_stride, const float* calibs_dev,
                                      int projection, float z_scale, float* out_dev, int64_t out_batch_stride, int64_t ld_out,
@@ -357,7 +382,8 @@ extern "C" int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, cons
 static int query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
                              int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
                              int64_t ld_grad, float* out_dev, int64_t ld_out, float* dpoints_dev, int64_t ld_dpoints,
-                             const int32_t* count_dev, int mode, void* stream, const char* what) {
+                             const int32_t* count_dev, int mode, void* stream, const char* what,
+                             const float* calib_dev = nullptr) {
   MpRange nvtx("monoport_b200: F1'' query gradient");
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE_SINGLE_MAP(feat, what);
@@ -375,7 +401,8 @@ static int query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points
   src.n = n;
   src.count_dev = count_dev;
   MpCalib cal;
-  mp_fill_calib(cal, calib12, projection, z_scale);
+  MpBatch one;
+  const MpBatch* single = mp_single_calib(cal, one, calib12, calib_dev, projection, z_scale);
   cudaStream_t st = (cudaStream_t)stream;
   // the rule of mp_query_dispatch: the tensor-core program covers maps of at most 65536 texels, and a frame above the head's
   // feature limit is taken by the exact kernel, decided on the device
@@ -388,13 +415,14 @@ static int query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points
     }
     const bool guarded = isfinite(mlp->tc_amax_limit);
     int rc = mp_launch_query_jvp_tc(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st,
-                                    guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE);
+                                    guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE, single);
     if (rc != MP_OK || !guarded) return rc;
     return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st,
-                                MP_GUARD_OUT_OF_RANGE);
+                                MP_GUARD_OUT_OF_RANGE, single);
   }
   MP_REQUIRE(mode == MP_MODE_FP32, "bad mode %d", mode);
-  return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st);
+  return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st, MP_GUARD_NONE,
+                              single);
 }
 
 extern "C" int mp_query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
@@ -446,10 +474,10 @@ __global__ void normals_finish_kernel(const float* __restrict__ g, const long lo
   }
 }
 
-extern "C" int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev,
-                                        const float* z_dev, const int64_t* count_dev, int64_t capacity, int R,
-                                        const float* b_min3, const float* b_max3, const float* calib12, int projection,
-                                        float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
+static int surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev, const float* z_dev,
+                                 const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
+                                 const float* calib12, const float* calib_dev, int projection, float z_scale, int mode,
+                                 float* scratch_dev, float* norm_dev, void* stream) {
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE_SINGLE_MAP(feat, "mp_surface_normals_async");
   MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "surface normals need a head with one output (got %d)", mlp->cout[mlp->n_layers - 1]);
@@ -467,7 +495,7 @@ extern "C" int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const in
   normals_points_kernel<<<grid, 256, 0, st>>>(surf, capacity, pts, count32);
   MP_CUDA(cudaGetLastError());
   const int rc = query_points_grad(mlp, feat, pts, capacity, capacity, 1, calib12, projection, z_scale, nullptr, 0, nullptr, 0, grad,
-                                   capacity, count32, mode, stream, "mp_surface_normals_async");
+                                   capacity, count32, mode, stream, "mp_surface_normals_async", calib_dev);
   if (rc != MP_OK) return rc;
   // forward_vertices' frame: its (X, Y, Z) index axes are the world axes scaled by R / (b_max - b_min), Z reversed
   float a[3];
@@ -477,12 +505,29 @@ extern "C" int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const in
   return MP_OK;
 }
 
+extern "C" int mp_surface_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev,
+                                        const float* z_dev, const int64_t* count_dev, int64_t capacity, int R,
+                                        const float* b_min3, const float* b_max3, const float* calib12, int projection,
+                                        float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
+  return surface_normals_async(mlp, feat, x_dev, y_dev, z_dev, count_dev, capacity, R, b_min3, b_max3, calib12, nullptr, projection,
+                               z_scale, mode, scratch_dev, norm_dev, stream);
+}
+
+extern "C" int mp_surface_normals_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev,
+                                             const float* z_dev, const int64_t* count_dev, int64_t capacity, int R,
+                                             const float* b_min3, const float* b_max3, const float* calib_dev, int projection,
+                                             float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
+  MP_REQUIRE(calib_dev, "NULL calib_dev");
+  return surface_normals_async(mlp, feat, x_dev, y_dev, z_dev, count_dev, capacity, R, b_min3, b_max3, nullptr, calib_dev, projection,
+                               z_scale, mode, scratch_dev, norm_dev, stream);
+}
+
 // Analytic normals at the vertices of a mesh (mp_mcubes_run_async's world-space [cap][3] vertices), enqueue-only: the
 // gradient launches of mp_surface_normals_async read the vertex rows in place (row stride 1, point stride 3) with the int32
 // count of the emission, and normals_finish_kernel takes unit axes: -g / |g|, zero where g vanishes.
-extern "C" int mp_mesh_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const float* verts_dev, const int64_t* counts_dev,
-                                     const int32_t* count32_dev, int64_t capacity, const float* calib12, int projection,
-                                     float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
+static int mesh_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const float* verts_dev, const int64_t* counts_dev,
+                              const int32_t* count32_dev, int64_t capacity, const float* calib12, const float* calib_dev,
+                              int projection, float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE_SINGLE_MAP(feat, "mp_mesh_normals_async");
   MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "mesh normals need a head with one output (got %d)", mlp->cout[mlp->n_layers - 1]);
@@ -491,7 +536,7 @@ extern "C" int mp_mesh_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const float
   if (capacity == 0) return MP_OK;
   float* grad = scratch_dev;
   const int rc = query_points_grad(mlp, feat, verts_dev, capacity, 1, 3, calib12, projection, z_scale, nullptr, 0, nullptr, 0, grad,
-                                   capacity, count32_dev, mode, stream, "mp_mesh_normals_async");
+                                   capacity, count32_dev, mode, stream, "mp_mesh_normals_async", calib_dev);
   if (rc != MP_OK) return rc;
   const long long blocks = (capacity + 255) / 256;
   const int grid = (int)(blocks < 1024 ? blocks : 1024);
@@ -499,6 +544,21 @@ extern "C" int mp_mesh_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const float
                                                                 1.f, 1.f, 1.f, norm_dev);
   MP_CUDA(cudaGetLastError());
   return MP_OK;
+}
+
+extern "C" int mp_mesh_normals_async(mp_mlp_t* mlp, mp_feat_t* feat, const float* verts_dev, const int64_t* counts_dev,
+                                     const int32_t* count32_dev, int64_t capacity, const float* calib12, int projection,
+                                     float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
+  return mesh_normals_async(mlp, feat, verts_dev, counts_dev, count32_dev, capacity, calib12, nullptr, projection, z_scale, mode,
+                            scratch_dev, norm_dev, stream);
+}
+
+extern "C" int mp_mesh_normals_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const float* verts_dev, const int64_t* counts_dev,
+                                          const int32_t* count32_dev, int64_t capacity, const float* calib_dev, int projection,
+                                          float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream) {
+  MP_REQUIRE(calib_dev, "NULL calib_dev");
+  return mesh_normals_async(mlp, feat, verts_dev, counts_dev, count32_dev, capacity, nullptr, calib_dev, projection, z_scale, mode,
+                            scratch_dev, norm_dev, stream);
 }
 
 extern "C" int mp_query_points_host(mp_mlp_t* mlp, mp_feat_t* feat, const float* feat_nchw_host, const float* points_host,
@@ -620,10 +680,10 @@ extern "C" int mp_colorize_surface(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t
 // The same render, enqueue-only (graph-capturable): the vertex count stays on the device and the range guard is decided
 // there, exactly as mp_query_dispatch decides it for a query -- the tensor-core launch renders a frame inside the head's
 // range, its exact fp32 twin one outside it, and the other launch returns at once.
-extern "C" int mp_colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev,
-                                         const float* z_dev, const int64_t* count_dev, int64_t capacity, int R, const float* b_min3,
-                                         const float* b_max3, const float* calib12, int projection, float z_scale, int mode,
-                                         float* canvas_dev, void* stream) {
+static int colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev, const float* z_dev,
+                                  const int64_t* count_dev, int64_t capacity, int R, const float* b_min3, const float* b_max3,
+                                  const float* calib12, const float* calib_dev, int projection, float z_scale, int mode,
+                                  float* canvas_dev, void* stream) {
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE_SINGLE_MAP(feat, "mp_colorize_surface_async");
   MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 3, "surface colourisation needs a head with 3 outputs (got %d)",
@@ -633,7 +693,8 @@ extern "C" int mp_colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const i
   if (capacity == 0) return MP_OK;
   MpRange nvtx("monoport_b200: F1 fused surface colourisation");
   MpCalib cal;
-  mp_fill_calib(cal, calib12, projection, z_scale);
+  MpBatch one;
+  const MpBatch* single = mp_single_calib(cal, one, calib12, calib_dev, projection, z_scale);
   const MpSurfaceSrc surf = mp_surface_src(reinterpret_cast<const long long*>(x_dev), reinterpret_cast<const long long*>(y_dev), z_dev,
                                            reinterpret_cast<const long long*>(count_dev), R, b_min3, b_max3, canvas_dev);
   cudaStream_t st = (cudaStream_t)stream;
@@ -645,12 +706,29 @@ extern "C" int mp_colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const i
       return MP_E_UNSUPPORTED;
     }
     const bool guarded = isfinite(mlp->tc_amax_limit);
-    int rc = mp_launch_surface_tc(mlp, feat, surf, capacity, cal, st, guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE);
+    int rc = mp_launch_surface_tc(mlp, feat, surf, capacity, cal, st, guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE, single);
     if (rc != MP_OK || !guarded) return rc;
-    return mp_launch_surface_fp32(mlp, feat, surf, capacity, cal, st, MP_GUARD_OUT_OF_RANGE);
+    return mp_launch_surface_fp32(mlp, feat, surf, capacity, cal, st, MP_GUARD_OUT_OF_RANGE, single);
   }
   MP_REQUIRE(mode == MP_MODE_FP32, "bad mode %d", mode);
-  return mp_launch_surface_fp32(mlp, feat, surf, capacity, cal, st, MP_GUARD_NONE);
+  return mp_launch_surface_fp32(mlp, feat, surf, capacity, cal, st, MP_GUARD_NONE, single);
+}
+
+extern "C" int mp_colorize_surface_async(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev,
+                                         const float* z_dev, const int64_t* count_dev, int64_t capacity, int R, const float* b_min3,
+                                         const float* b_max3, const float* calib12, int projection, float z_scale, int mode,
+                                         float* canvas_dev, void* stream) {
+  return colorize_surface_async(mlp, feat, x_dev, y_dev, z_dev, count_dev, capacity, R, b_min3, b_max3, calib12, nullptr, projection,
+                                z_scale, mode, canvas_dev, stream);
+}
+
+extern "C" int mp_colorize_surface_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const int64_t* x_dev, const int64_t* y_dev,
+                                              const float* z_dev, const int64_t* count_dev, int64_t capacity, int R,
+                                              const float* b_min3, const float* b_max3, const float* calib_dev, int projection,
+                                              float z_scale, int mode, float* canvas_dev, void* stream) {
+  MP_REQUIRE(calib_dev, "NULL calib_dev");
+  return colorize_surface_async(mlp, feat, x_dev, y_dev, z_dev, count_dev, capacity, R, b_min3, b_max3, nullptr, calib_dev,
+                                projection, z_scale, mode, canvas_dev, stream);
 }
 
 // Volumes that other processes of the node write into: plain cudaMalloc blocks (exportable; the caching allocators of

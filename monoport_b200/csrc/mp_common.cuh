@@ -154,7 +154,9 @@ struct MpCalib {
 // (tile t belongs to image t / tiles_per_image).  Image b reads its points at px/py/pz + b * pt_stride, its calibration
 // (rows 0..2 of [R|t], when MpCalib::has) from calibs[12 b ..] in device memory (null: MpCalib::m), its map's per-texel
 // arrays at the per-image offsets of mp_feat, and writes its outputs at out + b * out_stride.  The default is a
-// single-map launch.
+// single-map launch.  B == 1 with calibs set is a single-map launch whose camera is read from device memory when the kernel
+// runs (a captured frame whose camera changes between replays): every point source and output of a single-map launch, the
+// projection and z_scale still from MpCalib (has = 1).
 struct MpBatch {
   int B = 1;
   long long pt_stride = 0;
@@ -359,7 +361,8 @@ __device__ __forceinline__ float mp_lrelu(float v) { return v > 0.f ? v : v * MP
 // `guard`: the launch is conditional on the frame's feature range (feat->amax vs mlp->tc_amax_limit), evaluated on the device:
 //   MP_GUARD_NONE always run, MP_GUARD_IN_RANGE run when max|feature| <= limit, MP_GUARD_OUT_OF_RANGE run when it is above.
 // `bt` (batched launches; nullptr = one map): the launch covers bt->B images of src.n points.  The guard is decided per tile
-// from the maximum of the tile's own image (feat->amax[b]).
+// from the maximum of the tile's own image (feat->amax[b]).  A bt with B == 1 only moves the camera to device memory
+// (MpBatch::calibs); the gradient and surface launchers take such a bt too.
 enum { MP_GUARD_NONE = 0, MP_GUARD_IN_RANGE = 1, MP_GUARD_OUT_OF_RANGE = 2 };
 int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
@@ -371,12 +374,12 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
 // src.count_dev (when set) is the point count on the device; `guard` as for the query launchers.
 int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
-                         long long ld_dp, cudaStream_t st, int guard = MP_GUARD_NONE);
+                         long long ld_dp, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
 // the same outputs from the tensor-core program's forward-mode derivative (query_tc.cu: query_jvp_kernel), whose value is
 // the tensor-core query's bit for bit; the shipped heads, MP_SRC_ROWS, one map of at most 65536 texels
 int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
                            long long ld_grad, float* out, long long ld_out, float* dpoints, long long ld_dp, cudaStream_t st,
-                           int guard);
+                           int guard, const MpBatch* bt = nullptr);
 // device-side predicate shared by the kernels: true = the tiles of this image (amax = its entry) must do nothing.  In the
 // tensor-core program the weight producer and the consumers both take it, per tile, from the same word.
 __device__ __forceinline__ bool mp_guard_skips(const unsigned* amax, float limit, int guard) {
@@ -392,9 +395,15 @@ int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* 
 // range guard decided on the device (`guard` as above).  _tc: the colour head's tensor-core program (query_tc.cu); _fp32: the
 // exact kernel (query_fp32.cu), any head with 3 outputs.
 int mp_launch_surface_tc(const mp_mlp* mlp, mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
-                         cudaStream_t st, int guard);
+                         cudaStream_t st, int guard, const MpBatch* bt = nullptr);
 int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
-                           cudaStream_t st, int guard);
+                           cudaStream_t st, int guard, const MpBatch* bt = nullptr);
+// the single-map MpBatch whose camera is the 12 floats at calib_dev (device memory); nullptr: the camera in MpCalib
+inline MpBatch mp_device_calib(const float* calib_dev) {
+  MpBatch b;
+  b.calibs = calib_dev;
+  return b;
+}
 int mp_tc_prepare(mp_mlp* mlp);     // builds mlp->tc; sets tc_ok
 void mp_tc_release(mp_mlp* mlp);
 
@@ -402,4 +411,6 @@ void mp_tc_release(mp_mlp* mlp);
 int mp_query_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
                       int mode, cudaStream_t st, const MpBatch* bt = nullptr);
 void mp_fill_calib(MpCalib& c, const float* calib12, int projection, float z_scale);
+const MpBatch* mp_single_calib(MpCalib& cal, MpBatch& bt, const float* calib12, const float* calib_dev, int projection,
+                               float z_scale);
 void mp_fill_grid_geom(MpPointSrc& s, int res, int node_stride, int r_final, const float* bmin, const float* bmax);

@@ -483,7 +483,8 @@ extern "C" int mp_octree_finish(mp_octree_t* h, float* out_dev, int* nonempty, v
 // ---- fused run --------------------------------------------------------------------------------------
 // One evaluation pass of `level` over its node list (h->idx, count on the device): the query, then the scatter (lossless:
 // into the value list first, with conflict detection against the interpolated volume, then the next conflict list).
-static int level_pass(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode, cudaStream_t st) {
+static int level_pass(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, const MpBatch* bt, int mode,
+                      cudaStream_t st) {
   const bool lossless = !h->use_topk && !h->faster;
   int rc = MP_OK;
   MpPointSrc src;
@@ -507,7 +508,7 @@ static int level_pass(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, c
       // keep the interpolated values, evaluate into vals, then scatter+conflict-detect
       dst.out = h->vals; dst.ld = h->cap; dst.scatter_vol = nullptr;
     }
-    rc = mp_query_dispatch(mlp, feat, src, cal, dst, mode, st);
+    rc = mp_query_dispatch(mlp, feat, src, cal, dst, mode, st, bt);
     if (rc != MP_OK) return rc;
   }
   scatter_kernel<<<grid_for(h->cap > 1 << 20 ? 1 << 20 : h->cap), 256, 0, st>>>(
@@ -521,8 +522,8 @@ static int level_pass(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, c
 // The conflict loop of a lossless level as a WHILE node of the graph being captured on `st`: the body is one level_pass
 // followed by loop_control_kernel, which decides on the device whether the body runs again.  The condition defaults to 1
 // on every launch of the graph, so the body runs at least once, as in the host-driven loop.
-static int device_conflict_loop(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode,
-                                cudaStream_t st) {
+static int device_conflict_loop(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, const MpBatch* bt,
+                                int mode, cudaStream_t st) {
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   cudaGraph_t graph = nullptr;
   const cudaGraphNode_t* deps = nullptr;
@@ -543,7 +544,7 @@ static int device_conflict_loop(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_
   MP_CUDA(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));   // the next level waits
   MP_CUDA(cudaStreamBeginCaptureToGraph(h->body_stream, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
                                         cudaStreamCaptureModeRelaxed));
-  int rc = level_pass(h, level, mlp, feat, cal, mode, h->body_stream);
+  int rc = level_pass(h, level, mlp, feat, cal, bt, mode, h->body_stream);
   if (rc == MP_OK) {
     loop_control_kernel<<<1, 1, 0, h->body_stream>>>(h->count, h->loops + level, h->loops + kLoopSlots - 1, level,
                                                      kLoopPassesPerRes * h->res[level], cond);
@@ -562,8 +563,8 @@ static int device_conflict_loop(mp_octree* h, int level, mp_mlp_t* mlp, mp_feat_
 
 // device_loop: the lossless conflict loop of every level runs as a WHILE node of the graph captured on `st` (no host read);
 // otherwise it is driven from the host, which reads the list length back after every pass.
-static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode, cudaStream_t st,
-                            bool device_loop = false) {
+static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, const MpBatch* bt, int mode,
+                            cudaStream_t st, bool device_loop = false) {
   int rc = MP_OK;
   // level 0: dense
   {
@@ -582,7 +583,7 @@ static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const 
     } else {
       MpOutDst dst;
       dst.out = h->vol[h->cur]; dst.ld = n; dst.scatter_vol = nullptr;
-      rc = mp_query_dispatch(mlp, feat, src, cal, dst, mode, st);
+      rc = mp_query_dispatch(mlp, feat, src, cal, dst, mode, st, bt);
       if (rc != MP_OK) return rc;
     }
     set_u8_kernel<<<grid_for(n), 256, 0, st>>>(h->known[h->cur], n, 1);
@@ -598,12 +599,12 @@ static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const 
     if (!h->use_topk && h->faster && last) break;
     const bool lossless = !h->use_topk && !h->faster;
     if (lossless && device_loop) {
-      rc = device_conflict_loop(h, level, mlp, feat, cal, mode, st);
+      rc = device_conflict_loop(h, level, mlp, feat, cal, bt, mode, st);
       if (rc != MP_OK) return rc;
       continue;
     }
     for (;;) {
-      rc = level_pass(h, level, mlp, feat, cal, mode, st);
+      rc = level_pass(h, level, mlp, feat, cal, bt, mode, st);
       if (rc != MP_OK) return rc;
       if (!lossless) break;
       int32_t cnt = 0;
@@ -617,8 +618,8 @@ static int run_fused_levels(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const 
 }
 
 // The enqueue sequence of mp_octree_run_fused_async on `st`.
-static int enqueue_fused(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, int mode, float* out_dev,
-                         cudaStream_t st) {
+static int enqueue_fused(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpCalib& cal, const MpBatch* bt, int mode,
+                         float* out_dev, cudaStream_t st) {
   const bool lossless = !h->use_topk && !h->faster;
   int rc = reset_run(h, st);
   if (rc != MP_OK) return rc;
@@ -626,7 +627,7 @@ static int enqueue_fused(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpC
   const int final_buf = (h->n_levels - 1) & 1;
   float* const own_buf = h->vol[final_buf];
   h->vol[final_buf] = out_dev;          // the last level lands in the caller's volume (see mp_octree_run_fused)
-  rc = run_fused_levels(h, mlp, feat, cal, mode, st, lossless);
+  rc = run_fused_levels(h, mlp, feat, cal, bt, mode, st, lossless);
   const bool in_place = h->cur == final_buf;
   const float* result = h->vol[h->cur];
   h->vol[final_buf] = own_buf;
@@ -639,8 +640,10 @@ static int enqueue_fused(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const MpC
 // into a CUDA graph.  Results (non-empty flag, per-level counts, conflict-loop passes) stay on the device until
 // mp_octree_fetch / mp_octree_fetch_loops.  A lossless engine's conflict loop runs as a WHILE node per level; on a stream
 // that is not being captured the call records its sequence into a graph of its own and launches that on the stream.
-extern "C" int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib12, int projection,
-                                         float z_scale, int mode, float* out_dev, void* stream) {
+// calib_dev (the _dcal twin): the camera's 12 floats in device memory, read by the query launches when they run -- a
+// captured run, the lossless WHILE bodies included, then reads the current camera at every replay.
+static int run_fused_async(mp_octree* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib12, const float* calib_dev,
+                           int projection, float z_scale, int mode, float* out_dev, void* stream) {
   MP_REQUIRE(h && mlp && feat && out_dev, "NULL argument");
   MP_REQUIRE_SINGLE_MAP(feat, "the occupancy engine");
   MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "the occupancy engine needs a single-channel head");
@@ -650,14 +653,17 @@ extern "C" int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_
     mp_set_error("a sharded lossless engine reads counts on the host; use mp_octree_run_fused");
     return MP_E_UNSUPPORTED;
   }
+  // (the value lists of a sharded engine go through sharded_query, which takes the camera by value)
+  MP_REQUIRE(!calib_dev || h->shard_world == 1, "a sharded engine takes its calib by value");
   MpRange nvtx("monoport_b200: F2 coarse-to-fine engine (enqueue)");
   cudaStream_t st = (cudaStream_t)stream;
   MpCalib cal;
-  mp_fill_calib(cal, calib12, projection, z_scale);
+  MpBatch one;
+  const MpBatch* bt = mp_single_calib(cal, one, calib12, calib_dev, projection, z_scale);
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
   if (lossless) MP_CUDA(cudaStreamIsCapturing(st, &cs));
   if (!lossless || cs == cudaStreamCaptureStatusActive) {
-    const int rc = enqueue_fused(h, mlp, feat, cal, mode, out_dev, st);
+    const int rc = enqueue_fused(h, mlp, feat, cal, bt, mode, out_dev, st);
     if (rc != MP_OK) return rc;
     h->phase = 2;
     return MP_OK;
@@ -665,7 +671,7 @@ extern "C" int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_
   // not capturing: capture the sequence on the private stream (relaxed: the lazy allocations of a query stay legal),
   // then launch it on the caller's stream
   MP_CUDA(cudaStreamBeginCapture(h->cap_stream, cudaStreamCaptureModeRelaxed));
-  const int rc = enqueue_fused(h, mlp, feat, cal, mode, out_dev, h->cap_stream);
+  const int rc = enqueue_fused(h, mlp, feat, cal, bt, mode, out_dev, h->cap_stream);
   cudaGraph_t graph = nullptr;
   cudaError_t e = cudaStreamEndCapture(h->cap_stream, &graph);
   if (rc != MP_OK) {
@@ -682,6 +688,17 @@ extern "C" int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_
   MP_CUDA(e);
   h->phase = 2;
   return MP_OK;
+}
+
+extern "C" int mp_octree_run_fused_async(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib12, int projection,
+                                         float z_scale, int mode, float* out_dev, void* stream) {
+  return run_fused_async(h, mlp, feat, calib12, nullptr, projection, z_scale, mode, out_dev, stream);
+}
+
+extern "C" int mp_octree_run_fused_async_dcal(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* feat, const float* calib_dev,
+                                              int projection, float z_scale, int mode, float* out_dev, void* stream) {
+  MP_REQUIRE(calib_dev, "NULL calib_dev");
+  return run_fused_async(h, mlp, feat, nullptr, calib_dev, projection, z_scale, mode, out_dev, stream);
 }
 
 // The read-back half: non-empty flag and per-level evaluated-node counts of the last (async) run.  Synchronises.
@@ -733,7 +750,7 @@ extern "C" int mp_octree_run_fused(mp_octree_t* h, mp_mlp_t* mlp, mp_feat_t* fea
   const int final_buf = (h->n_levels - 1) & 1;
   float* const own_buf = h->vol[final_buf];
   h->vol[final_buf] = out_dev;
-  rc = run_fused_levels(h, mlp, feat, cal, mode, st);
+  rc = run_fused_levels(h, mlp, feat, cal, nullptr, mode, st);
   const bool in_place = h->cur == final_buf;
   const float* result = h->vol[h->cur];
   h->vol[final_buf] = own_buf;

@@ -313,6 +313,7 @@ struct GradParams {
   long long ld_grad;
   float* dp;                       // [3][ld_dp]
   long long ld_dp;
+  const float* calib;              // rows 0..2 of [R|t] in device memory, read when the kernel runs (null: MpCalib::m)
 };
 
 template <int P>
@@ -397,7 +398,8 @@ query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
   }
   // the range guard, decided per launch as query_fp32_kernel decides it (uniform over the grid)
   const long long n_tiles = mp_guard_skips(prm.amax, prm.amax_limit, prm.guard) ? 0 : (n + P - 1) / P;
-  const MpBatch one;                                 // (a single map)
+  MpBatch one;                                       // (a single map; its camera in device memory when gp.calib is set)
+  one.calibs = gp.calib;
 
   for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const long long p0 = tile * P;
@@ -444,9 +446,11 @@ query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
         if (lane < 3) dp[lane * gp.ld_dp] = 0.f;
         continue;
       }
+      // the projection and its Jacobian below: one MpCalib, the camera tile_sample projected with
+      const MpCalib c = mp_image_calib(cal, one, 0);
       float x, y, z, u, v, w;
       mp_load_point(src, one, 0, i, x, y, z);
-      mp_project(cal, x, y, z, u, v, w);
+      mp_project(c, x, y, z, u, v, w);
       // the tap cell of mp_taps; a tap outside the map is zero padding and contributes nothing
       const float ix = ((u + 1.f) / 2.f) * (float)(prm.W - 1);
       const float iy = ((v + 1.f) / 2.f) * (float)(prm.H - 1);
@@ -478,18 +482,18 @@ query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
       if (lane == 0) {
         du *= 0.5f * (float)(prm.W - 1);
         dv *= 0.5f * (float)(prm.H - 1);
-        const float dw = cal.z_scale * sX[(size_t)prm.C * P + p];
+        const float dw = c.z_scale * sX[(size_t)prm.C * P + p];
         float g[3];
-        if (!cal.has) {
+        if (!c.has) {
           g[0] = du; g[1] = dv; g[2] = dw;
-        } else if (!cal.perspective) {                   // J = R
+        } else if (!c.perspective) {                     // J = R
 #pragma unroll
-          for (int a = 0; a < 3; ++a) g[a] = cal.m[a] * du + cal.m[4 + a] * dv + cal.m[8 + a] * dw;
+          for (int a = 0; a < 3; ++a) g[a] = c.m[a] * du + c.m[4 + a] * dv + c.m[8 + a] * dw;
         } else {                                         // J rows: (R0 - u R2) / w, (R1 - v R2) / w, R2
           const float su = du / w, sv = dv / w;
           const float s2 = dw - su * u - sv * v;
 #pragma unroll
-          for (int a = 0; a < 3; ++a) g[a] = cal.m[a] * su + cal.m[4 + a] * sv + cal.m[8 + a] * s2;
+          for (int a = 0; a < 3; ++a) g[a] = c.m[a] * su + c.m[4 + a] * sv + c.m[8 + a] * s2;
         }
 #pragma unroll
         for (int a = 0; a < 3; ++a) dp[a * gp.ld_dp] = g[a];
@@ -606,7 +610,7 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
   if (rc != MP_OK) return rc;
   prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
   const int ping = prm.h_ping, pong = prm.h_pong;
-  if (bt && (src.kind != MP_SRC_ROWS || dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
+  if (bt && bt->B > 1 && (src.kind != MP_SRC_ROWS || dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
     mp_set_error("batched launches take point rows and write [R,N] outputs");
     return MP_E_UNSUPPORTED;
   }
@@ -619,11 +623,15 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
 }
 
 int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
-                           cudaStream_t st, int guard) {
+                           cudaStream_t st, int guard, const MpBatch* bt) {
   if (n <= 0) return MP_OK;
   if (mlp->cout[mlp->n_layers - 1] != 3) {
     mp_set_error("surface colourisation needs a head with 3 outputs (got %d)", mlp->cout[mlp->n_layers - 1]);
     return MP_E_INVALID;
+  }
+  if (bt && bt->B != 1) {
+    mp_set_error("the surface render takes one map");
+    return MP_E_UNSUPPORTED;
   }
   Fp32Params prm;
   int sms = 0, max_smem = 0;
@@ -636,7 +644,7 @@ int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfa
   src.n = n;
   MpOutDst dst;
   dst.out = nullptr; dst.ld = 0; dst.scatter_vol = nullptr;
-  const MpBatch one;
+  const MpBatch one = bt ? *bt : MpBatch();         // (one map, its camera in device memory when one.calibs is set)
   const int ping = prm.h_ping, pong = prm.h_pong;
   if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32, true>(prm, src, cal, dst, st, sms, max_smem, one, surf);
   if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16, true>(prm, src, cal, dst, st, sms, max_smem, one, surf);
@@ -647,10 +655,10 @@ int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfa
 
 int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
-                         long long ld_dp, cudaStream_t st, int guard) {
+                         long long ld_dp, cudaStream_t st, int guard, const MpBatch* bt) {
   if (src.n <= 0) return MP_OK;
-  if (src.kind != MP_SRC_ROWS) {
-    mp_set_error("the gradient kernel takes point rows");
+  if (src.kind != MP_SRC_ROWS || (bt && bt->B != 1)) {
+    mp_set_error("the gradient kernel takes point rows of one map");
     return MP_E_UNSUPPORTED;
   }
   Fp32Params prm;
@@ -669,10 +677,11 @@ int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
   gp.mask_words = words;
   gp.grad_out = grad_out; gp.ld_grad = ld_grad;
   gp.dp = dpoints; gp.ld_dp = ld_dp;
+  gp.calib = bt ? bt->calibs : nullptr;
   if (out) {                                      // the value: query_fp32_kernel's own, bit for bit
     MpOutDst dst;
     dst.out = out; dst.ld = ld_out; dst.scatter_vol = nullptr;
-    const int rq = mp_launch_query_fp32(mlp, feat, src, cal, dst, st, guard);
+    const int rq = mp_launch_query_fp32(mlp, feat, src, cal, dst, st, guard, bt);
     if (rq != MP_OK) return rq;
   }
   const int res = prm.cout[prm.n_layers - 1];

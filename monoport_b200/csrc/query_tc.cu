@@ -687,6 +687,7 @@ struct JvpOut {
   long long ld_dp;
   const float* grad_out;  // [Res][ld_grad], or null (ones)
   long long ld_grad;
+  const float* calib;     // rows 0..2 of [R|t] in device memory, read when the kernel runs (null: MpCalib::m)
 };
 
 // A-operand row of tangent t (0 value, 1 d/dix, 2 d/diy, 3 d/dzf) of point k of a tile
@@ -698,17 +699,19 @@ struct JvpTaps {
   float u, v, w;          // the projected point
 };
 
-__device__ __forceinline__ JvpTaps jvp_taps(const MpPointSrc& src, const MpCalib& cal, int H, int W, long long i, long long n) {
+__device__ __forceinline__ JvpTaps jvp_taps(const MpPointSrc& src, const MpCalib& cal, const float* calib, int H, int W, long long i,
+                                            long long n) {
   JvpTaps j;
   MpSurfaceSrc nosurf;
   memset(&nosurf, 0, sizeof(nosurf));
-  const MpBatch one;
+  MpBatch one;                                       // (a single map; its camera in device memory when calib is set)
+  one.calibs = calib;
   j.pt = point_taps(nosurf, src, cal, one, 0, H, W, i, n);
   float u = 0.f, v = 0.f, w = 0.f;
   if (i < n) {
     float x, y, z;
     mp_load_point(src, one, 0, i, x, y, z);
-    mp_project<true>(cal, x, y, z, u, v, w);
+    mp_project<true>(mp_image_calib(cal, one, 0), x, y, z, u, v, w);
   }
   j.u = u; j.v = v; j.w = w;
   // the tap cell of mp_taps
@@ -862,7 +865,7 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
   for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
     const long long p0 = t * NP;
     // ---- this lane's point (lane % 16) of the tile; X and the per-point scalars: warp w samples points 2w, 2w + 1
-    const JvpTaps jt = jvp_taps(src, cal, prm.H, prm.W, p0 + (lane & 15), n);
+    const JvpTaps jt = jvp_taps(src, cal, jo.calib, prm.H, prm.W, p0 + (lane & 15), n);
 #pragma unroll 1
     for (int qq = 0; qq < 2; ++qq) {
       const int q = 2 * warp + qq;
@@ -1046,15 +1049,21 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
           float gp[3];
           if (!cal.has) {
             gp[0] = du; gp[1] = dv; gp[2] = dw;
-          } else if (!cal.perspective) {                 // J = R
+          } else {
+            // the camera jvp_taps projected with (device memory when jo.calib is set), read where the Jacobian needs it
+            MpBatch one;
+            one.calibs = jo.calib;
+            const MpCalib c = mp_image_calib(cal, one, 0);
+            if (!c.perspective) {                        // J = R
 #pragma unroll
-            for (int a = 0; a < 3; ++a) gp[a] = cal.m[a] * du + cal.m[4 + a] * dv + cal.m[8 + a] * dw;
-          } else {                                       // J rows: (R0 - u R2) / w, (R1 - v R2) / w, R2
-            const float u = s_uvw[kpt], v = s_uvw[NP + kpt], w = s_uvw[2 * NP + kpt];
-            const float su = du / w, sv = dv / w;
-            const float s2 = dw - su * u - sv * v;
+              for (int a = 0; a < 3; ++a) gp[a] = c.m[a] * du + c.m[4 + a] * dv + c.m[8 + a] * dw;
+            } else {                                     // J rows: (R0 - u R2) / w, (R1 - v R2) / w, R2
+              const float u = s_uvw[kpt], v = s_uvw[NP + kpt], w = s_uvw[2 * NP + kpt];
+              const float su = du / w, sv = dv / w;
+              const float s2 = dw - su * u - sv * v;
 #pragma unroll
-            for (int a = 0; a < 3; ++a) gp[a] = cal.m[a] * su + cal.m[4 + a] * sv + cal.m[8 + a] * s2;
+              for (int a = 0; a < 3; ++a) gp[a] = c.m[a] * su + c.m[4 + a] * sv + c.m[8 + a] * s2;
+            }
           }
 #pragma unroll
           for (int a = 0; a < 3; ++a) jo.dp[a * jo.ld_dp + i] = inimg != 0.f ? gp[a] : 0.f;     // outside the image: exactly 0
@@ -1498,11 +1507,15 @@ void mp_tc_release(mp_mlp* mlp) {
 }
 
 int mp_launch_surface_tc(const mp_mlp* mlp, mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
-                         cudaStream_t st, int guard) {
+                         cudaStream_t st, int guard, const MpBatch* bt) {
   if (n <= 0) return MP_OK;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
   if (!pk || !mlp->tc_ok || pk->kind != 1) {
     mp_set_error("fused surface colourisation needs the tensor-core program of the colour head");
+    return MP_E_UNSUPPORTED;
+  }
+  if (bt && bt->B != 1) {
+    mp_set_error("the surface render takes one map");
     return MP_E_UNSUPPORTED;
   }
   if (feat->C != 512 || (long long)feat->H * feat->W > 65536) {
@@ -1515,7 +1528,7 @@ int mp_launch_surface_tc(const mp_mlp* mlp, mp_feat* feat, const MpSurfaceSrc& s
   src.n = n;
   MpOutDst dst;
   dst.out = nullptr; dst.ld = 0; dst.scatter_vol = nullptr;
-  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, MpBatch());
+  return launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, bt ? *bt : MpBatch());
 }
 
 int mp_launch_colour_surface(const mp_mlp* mlp, mp_feat* feat, const long long* X, const long long* Y, const float* Z, long long n,
@@ -1541,7 +1554,7 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
   }
   MpSurfaceSrc surf;
   memset(&surf, 0, sizeof(surf));
-  if (bt && (src.kind != MP_SRC_ROWS || dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
+  if (bt && bt->B > 1 && (src.kind != MP_SRC_ROWS || dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
     mp_set_error("batched launches take point rows and write [R,N] outputs");
     return MP_E_UNSUPPORTED;
   }
@@ -1551,13 +1564,14 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
 }
 
 int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
-                           long long ld_grad, float* out, long long ld_out, float* dpoints, long long ld_dp, cudaStream_t st, int guard) {
+                           long long ld_grad, float* out, long long ld_out, float* dpoints, long long ld_dp, cudaStream_t st, int guard,
+                           const MpBatch* bt) {
   if (src.n <= 0) return MP_OK;
   int C = 0;
   const int rc = check_query(mlp, feat, C);
   if (rc != MP_OK) return rc;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
-  if (src.kind != MP_SRC_ROWS || feat->B != 1) {
+  if (src.kind != MP_SRC_ROWS || feat->B != 1 || (bt && bt->B != 1)) {
     mp_set_error("the gradient program takes point rows of one map");
     return MP_E_UNSUPPORTED;
   }
@@ -1565,5 +1579,6 @@ int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& s
   jo.out = out; jo.ld_out = ld_out;
   jo.dp = dpoints; jo.ld_dp = ld_dp;
   jo.grad_out = grad_out; jo.ld_grad = ld_grad;
+  jo.calib = bt ? bt->calibs : nullptr;
   return C == 256 ? launch_jvp<256>(mlp, pk, feat, src, cal, jo, st, guard) : launch_jvp<512>(mlp, pk, feat, src, cal, jo, st, guard);
 }

@@ -59,11 +59,14 @@ class FrameGraph:
     engine: a Seg3dLossless (faster=True, or the lossless faster=False) / Seg3dTopk built with make_query_func(net).  The
     lossless engine's conflict loop runs inside the graph as a conditional WHILE node per level, decided on the device;
     result() reads its passes per level into `last_conflict_loops` and raises RuntimeError for a frame whose loop stopped at
-    its cap (8 x the level's resolution passes) -- run that frame with the eager engine.  calib: [1,4,4] tensor (read once,
-    at construction).
+    its cap (8 x the level's resolution passes) -- run that frame with the eager engine.
+    calib: [1,4,4] tensor, the graph's default camera.  The graph reads its camera from a 12-float device buffer when it runs
+    (the _dcal entry points), so every frame can have its own: launch(x, calib=...) writes the frame's camera there before
+    the replay, launch(x) the default one.  Orthographic or perspective projection stays the net's, fixed at construction.
     `feature_hook(feat) -> feat` (optional) runs inside the captured step on the encoder's last-stage map.
     launch(x) enqueues a frame (x = image [1,3,H,W] with an encoder, else the [1,C,h,w] feature map); result() waits for it
-    and returns (sdf or None, X, Y, Z, norm) exactly like engine(...) followed by forward_vertices(sdf, direction).
+    and returns (sdf or None, X, Y, Z, norm) exactly like engine(..., calib_tensor=<the frame's camera>) followed by
+    forward_vertices(sdf, direction).
 
     The demo's two images (RTL/main.py:417-441) can be rendered inside the same captured step:
       netC: the colour net.  Its map is netC.filter(x_colour, feat_prior=<the geometry map the engine receives>) with the
@@ -102,7 +105,7 @@ class FrameGraph:
         self.R = R = engine.resolutions[-1]
         self._dir = _DIRS[direction]
         self._proj = _lib.PROJ_PERSPECTIVE if net.projection is perspective else _lib.PROJ_ORTHOGONAL
-        self._cal12 = _lib.calib12(calib.detach().cpu())
+        cal12 = _lib.calib12(calib.detach().cpu())
         if input_shape is None:
             input_shape = (1, 3, 512, 512) if with_encoder else (1, net.surface_classifier.filter_channels[0] - 1, 128, 128)
         self.netC = netC
@@ -118,6 +121,10 @@ class FrameGraph:
         with torch.cuda.device(dev):
             self.stream = torch.cuda.Stream(dev)
             self.static_in = torch.zeros(input_shape, dtype=torch.float32, device=dev)
+            # the camera the captured step reads when it runs (rows 0..2 of [R|t]), and the constructor's, for launch(calib=None)
+            self._cal_default = torch.tensor(list(cal12), dtype=torch.float32).to(dev)
+            self._cal_dev = self._cal_default.clone()
+            self._cal_is_default = True           # (only launch() writes the buffer, in stream order)
             self.render_tex = self.render_norm = None
             if netC is not None or self.render_normals:
                 bg = torch.ones((R, R, 3), dtype=torch.float32) if canvas is None else canvas.detach()
@@ -195,9 +202,10 @@ class FrameGraph:
         self._fh.key = None                      # always upload: the map changes with every replay
         self._fh.upload(feat)
         st = _lib.stream_ptr(dev)
-        _lib.check(lib.mp_octree_run_fused_async(
-            self._oct, self._head, self._fh.ptr, self._cal12, self._proj, ctypes.c_float(self.net.normalizer.scale),
-            self.net._mode(), ctypes.c_void_p(self.volume.data_ptr()), st), "mp_octree_run_fused_async")
+        cal = ctypes.c_void_p(self._cal_dev.data_ptr())
+        _lib.check(lib.mp_octree_run_fused_async_dcal(
+            self._oct, self._head, self._fh.ptr, cal, self._proj, ctypes.c_float(self.net.normalizer.scale),
+            self.net._mode(), ctypes.c_void_p(self.volume.data_ptr()), st), "mp_octree_run_fused_async_dcal")
         _lib.check(lib.mp_forward_vertices_async(
             ctypes.c_void_p(self.volume.data_ptr()), self.R, self._dir, ctypes.c_void_p(self.X.data_ptr()),
             ctypes.c_void_p(self.Y.data_ptr()), ctypes.c_void_p(self.Z.data_ptr()), ctypes.c_void_p(self.N.data_ptr()),
@@ -207,11 +215,12 @@ class FrameGraph:
             norm = self.N
             if self.render_normals == "gradient":
                 norm = self.N_grad
-                _lib.check(lib.mp_surface_normals_async(
+                _lib.check(lib.mp_surface_normals_async_dcal(
                     self._head, self._fh.ptr, ctypes.c_void_p(self.X.data_ptr()), ctypes.c_void_p(self.Y.data_ptr()),
                     ctypes.c_void_p(self.Z.data_ptr()), ctypes.c_void_p(self.count.data_ptr()), cap, self.R, self._bmin3,
-                    self._bmax3, self._cal12, self._proj, ctypes.c_float(self.net.normalizer.scale), _lib.MODE_AUTO,
-                    ctypes.c_void_p(self._nscratch.data_ptr()), ctypes.c_void_p(norm.data_ptr()), st), "mp_surface_normals_async")
+                    self._bmax3, cal, self._proj, ctypes.c_float(self.net.normalizer.scale), _lib.MODE_AUTO,
+                    ctypes.c_void_p(self._nscratch.data_ptr()), ctypes.c_void_p(norm.data_ptr()), st),
+                    "mp_surface_normals_async_dcal")
             self.render_norm.copy_(self._bg)
             _lib.check(lib.mp_render_normals_async(
                 ctypes.c_void_p(self.X.data_ptr()), ctypes.c_void_p(self.Y.data_ptr()), ctypes.c_void_p(norm.data_ptr()),
@@ -226,15 +235,15 @@ class FrameGraph:
             self._fhc.key = None
             self._fhc.upload(featc)
             self.render_tex.copy_(self._bg)
-            _lib.check(lib.mp_colorize_surface_async(
+            _lib.check(lib.mp_colorize_surface_async_dcal(
                 self._headC, self._fhc.ptr, ctypes.c_void_p(self.X.data_ptr()), ctypes.c_void_p(self.Y.data_ptr()),
                 ctypes.c_void_p(self.Z.data_ptr()), ctypes.c_void_p(self.count.data_ptr()), cap, self.R, self._bmin3,
-                self._bmax3, self._cal12, self._projC, ctypes.c_float(self.netC.normalizer.scale), self.netC._mode(),
-                ctypes.c_void_p(self.render_tex.data_ptr()), st), "mp_colorize_surface_async")
+                self._bmax3, cal, self._projC, ctypes.c_float(self.netC.normalizer.scale), self.netC._mode(),
+                ctypes.c_void_p(self.render_tex.data_ptr()), st), "mp_colorize_surface_async_dcal")
         if self.with_mesh:
-            self._mesh_step(st)
+            self._mesh_step(st, cal)
 
-    def _mesh_step(self, st):
+    def _mesh_step(self, st, cal):
         from .recon import marching_cubes_async
         lib = self._lib
         marching_cubes_async(self.volume, self.mesh_verts, self.mesh_faces, self.mesh_counts, self._mesh_count32, 0.5,
@@ -242,26 +251,58 @@ class FrameGraph:
         v_cap = self.mesh_verts.shape[0]
         verts, counts, count32 = (ctypes.c_void_p(t.data_ptr()) for t in (self.mesh_verts, self.mesh_counts, self._mesh_count32))
         if self.with_mesh_normals:
-            _lib.check(lib.mp_mesh_normals_async(
-                self._head, self._fh.ptr, verts, counts, count32, v_cap, self._cal12, self._proj,
+            _lib.check(lib.mp_mesh_normals_async_dcal(
+                self._head, self._fh.ptr, verts, counts, count32, v_cap, cal, self._proj,
                 ctypes.c_float(self.net.normalizer.scale), _lib.MODE_AUTO, ctypes.c_void_p(self._mesh_nscratch.data_ptr()),
-                ctypes.c_void_p(self.mesh_norm.data_ptr()), st), "mp_mesh_normals_async")
+                ctypes.c_void_p(self.mesh_norm.data_ptr()), st), "mp_mesh_normals_async_dcal")
         if self.with_mesh_colours:
             # netC at the vertex rows (row stride 1, point stride 3), then mesh_colours' pred * 0.5 + 0.5
-            _lib.check(lib.mp_query_points_count(
-                self._headC, self._fhc.ptr, verts, v_cap, 1, 3, self._cal12, self._projC,
+            _lib.check(lib.mp_query_points_count_dcal(
+                self._headC, self._fhc.ptr, verts, v_cap, 1, 3, cal, self._projC,
                 ctypes.c_float(self.netC.normalizer.scale), ctypes.c_void_p(self._mesh_pred.data_ptr()), v_cap, count32,
-                self.netC._mode(), st), "mp_query_points_count")
+                self.netC._mode(), st), "mp_query_points_count_dcal")
             torch.mul(self._mesh_pred, 0.5, out=self._mesh_rgb)
             self._mesh_rgb.add_(0.5)
 
-    def launch(self, x, x_colour=None):
+    def _calib_rows(self, calib):
+        """calib ([1,4,4], [4,4] or [3,4], any float dtype, on the CPU or on the graph's device) -> its rows 0..2 as a
+        [3,4] tensor, the reduction of _lib.calib12 (the float32 rounding happens in the copy into the buffer)."""
+        if not torch.is_tensor(calib) or not calib.is_floating_point():
+            raise ValueError("calib must be a floating-point tensor; got %r" % (type(calib) if not torch.is_tensor(calib)
+                                                                               else calib.dtype,))
+        c = calib.detach()
+        if c.dim() == 3:
+            if c.shape[0] != 1:
+                raise ValueError("calib: batch size must be 1; got %d" % c.shape[0])
+            c = c[0]
+        if c.dim() != 2 or c.shape[1] != 4 or c.shape[0] not in (3, 4):
+            raise ValueError("calib must be [1,4,4], [4,4] or [3,4]; got %s" % (tuple(calib.shape),))
+        if c.device.type != "cpu" and c.device != self._cal_dev.device:
+            raise ValueError("calib is on %s; the FrameGraph runs on %s (or pass a CPU tensor)" % (c.device, self._cal_dev.device))
+        if c.device.type == "cpu":
+            # a private copy: the caller may change its tensor as soon as launch() returns
+            c = c[:3, :4].to(torch.float32, copy=True)
+        return c[:3, :4]
+
+    def launch(self, x, x_colour=None, calib=None):
         """Enqueue one frame (returns at once).  x_colour: netC's input (its image with the encoder, else its map), required
-        exactly when the graph was built with netC."""
+        exactly when the graph was built with netC.  calib: the frame's camera ([1,4,4], [4,4] or [3,4], CPU or this graph's
+        device; rows 0..2 are used, in float32 like calib12), None for the constructor's.  ValueError for another shape, a
+        batch of more than one or another device."""
         if (x_colour is None) != (self.netC is None):
             raise ValueError("x_colour is required exactly when the FrameGraph renders with netC")
+        rows = None if calib is None else self._calib_rows(calib)
         self.stream.wait_stream(torch.cuda.current_stream(self.device))     # x may still be produced on the caller's stream
         with torch.cuda.stream(self.stream):
+            if rows is None:
+                if not self._cal_is_default:      # a fixed camera costs nothing per frame
+                    self._cal_dev.copy_(self._cal_default, non_blocking=True)
+                    self._cal_is_default = True
+            else:
+                self._cal_is_default = False
+                if rows.device.type != "cpu":
+                    rows.record_stream(self.stream)      # (read on this stream: its memory is not reused before the copy)
+                self._cal_dev.view(3, 4).copy_(rows, non_blocking=True)
             self.static_in.copy_(x, non_blocking=True)
             if x_colour is not None:
                 self.static_in_c.copy_(x_colour, non_blocking=True)
@@ -345,7 +386,8 @@ class FrameGraphRing:
     """`n_lanes` FrameGraphs used round-robin: up to n_lanes frames in flight, results in input order (the graph-captured
     counterpart of FramePipeline for the stages of this library).  Lanes built with netC take (x, x_colour) items and yield
     result() + rendered(): (sdf, X, Y, Z, norm, render_norm, render_tex).  Lanes built with mesh=True append mesh()'s
-    (verts, faces, normals, colours), four Nones for a frame without a surface."""
+    (verts, faces, normals, colours), four Nones for a frame without a surface.  run(items, calibs) takes the cameras of the
+    frames too (zipped with items; see FrameGraph.launch)."""
 
     def __init__(self, make_graph, n_lanes=2):
         self.lanes = [make_graph() for _ in range(int(n_lanes))]
@@ -359,13 +401,14 @@ class FrameGraphRing:
             out = out + (lane.mesh() or (None,) * 4)
         return out
 
-    def run(self, iterable):
+    def run(self, iterable, calibs=None):
         inflight = deque()
-        for i, x in enumerate(iterable):
+        pairs = zip(iterable, calibs) if calibs is not None else ((x, None) for x in iterable)
+        for i, (x, calib) in enumerate(pairs):
             lane = self.lanes[i % len(self.lanes)]
             if len(inflight) >= len(self.lanes):
                 yield self._out(inflight.popleft())
-            inflight.append(lane.launch(*x) if lane.netC is not None else lane.launch(x))
+            inflight.append(lane.launch(*x, calib=calib) if lane.netC is not None else lane.launch(x, calib=calib))
         while inflight:
             yield self._out(inflight.popleft())
 
