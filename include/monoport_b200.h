@@ -310,6 +310,19 @@ int mp_forward_vertices_async(const float* vol_dev, int R, int direction, int64_
                               float* norm_dev, int64_t* count_dev, void* scratch_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * The demo's display images (visulization, RTL/main.py:252-281), enqueue-only (graph-capturable): the [R,R,3] float32
+ * canvases norm_dev / tex_dev (either may be NULL, not both) become [S,S,3] float32 images C * 255, rotated by
+ * torch.rot90(k=1, dims [0,1]) and resized by nearest F.interpolate, bit for bit what torch gives (NaN stays NaN); and an
+ * [S,S] uint8 mask, 0 where the three values of the reference image (the texture image if present, else the normal
+ * image) all equal 255 and 1 elsewhere.  One kernel into staging_dev (3 * S*S floats per present image + S*S floats),
+ * then one device-to-host copy per output into page-locked host memory (norm_host / tex_host for the present images,
+ * mask_host always).  Refuses (MP_E_INVALID) NULL for both images, R < 1 or S < 1, a NULL output or staging buffer,
+ * and a host output that is not page-locked.  The host outputs hold the result once the stream has reached this call.
+ * ------------------------------------------------------------------------------------------- */
+int mp_display_async(const float* norm_dev, const float* tex_dev, int R, int S, float* norm_host, float* tex_host,
+                     uint8_t* mask_host, float* staging_dev, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Direct rendering of the visible surface with the colour head.  Replaces colorization (RTL/main.py:212-249): vertex i =
  * (X[i], Y[i], R - Z[i]) of mp_forward_vertices -> world space by mat_color (:201-210) -> netC.query -> pred*0.5+0.5 ->
  * canvas[X[i], Y[i], :]  ([R,R,3] float32, prepared by the caller), in ONE launch without intermediate tensors.

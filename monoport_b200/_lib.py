@@ -112,6 +112,7 @@ SIGNATURES = {
     "mp_forward_vertices_scratch_bytes": (c_int64, [c_int]),
     "mp_forward_vertices_async": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p]),
+    "mp_display_async": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -57,6 +57,41 @@ extern "C" int mp_render_normals_async(const int64_t* x_dev, const int64_t* y_de
   return MP_OK;
 }
 
+static bool pinned_host(const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();                                        // (not sticky: clear it for the caller's next check)
+    return false;
+  }
+  return a.type == cudaMemoryTypeHost;
+}
+
+// The demo's display images, enqueue-only (graph-capturable): display_kernel into staging_dev, then one device-to-host copy
+// per output.  Staging layout: [S,S,3] floats of the normal image (if any), [S,S,3] of the texture image (if any), S*S bytes
+// of the mask.
+extern "C" int mp_display_async(const float* norm_dev, const float* tex_dev, int R, int S, float* norm_host, float* tex_host,
+                                uint8_t* mask_host, float* staging_dev, void* stream) {
+  MP_REQUIRE(norm_dev || tex_dev, "mp_display_async: both images are NULL");
+  MP_REQUIRE(R >= 1 && S >= 1, "mp_display_async: bad sizes R=%d S=%d", R, S);
+  MP_REQUIRE(mask_host && staging_dev, "NULL argument");
+  MP_REQUIRE(!norm_dev || norm_host, "mp_display_async: the normal image has no host output");
+  MP_REQUIRE(!tex_dev || tex_host, "mp_display_async: the texture image has no host output");
+  MP_REQUIRE((!norm_dev || pinned_host(norm_host)) && (!tex_dev || pinned_host(tex_host)) && pinned_host(mask_host),
+             "mp_display_async: host outputs must be page-locked (cudaHostAlloc / pin_memory)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t px = (size_t)S * S;
+  float* norm_st = norm_dev ? staging_dev : nullptr;
+  float* tex_st = tex_dev ? staging_dev + (norm_dev ? 3 * px : 0) : nullptr;
+  uint8_t* mask_st = reinterpret_cast<uint8_t*>(staging_dev + (norm_dev ? 3 * px : 0) + (tex_dev ? 3 * px : 0));
+  const long long blocks = ((long long)px + kDispThreads - 1) / kDispThreads;
+  display_kernel<<<(unsigned)blocks, kDispThreads, 0, st>>>(norm_dev, tex_dev, R, S, norm_st, tex_st, mask_st);
+  MP_CUDA(cudaGetLastError());
+  if (norm_dev) MP_CUDA(cudaMemcpyAsync(norm_host, norm_st, 3 * px * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (tex_dev) MP_CUDA(cudaMemcpyAsync(tex_host, tex_st, 3 * px * sizeof(float), cudaMemcpyDeviceToHost, st));
+  MP_CUDA(cudaMemcpyAsync(mask_host, mask_st, px, cudaMemcpyDeviceToHost, st));
+  return MP_OK;
+}
+
 extern "C" int mp_forward_vertices(const float* vol_dev, int R, int direction, int64_t* x_dev, int64_t* y_dev,
                                    float* z_dev, float* norm_dev, int64_t* n_out, void* stream) {
   MP_REQUIRE(vol_dev && x_dev && y_dev && z_dev && norm_dev && n_out, "NULL argument");

@@ -117,4 +117,36 @@ render_normals_kernel(const long long* __restrict__ X, const long long* __restri
   }
 }
 
+// The display images of the demo (visulization, RTL/main.py:252-281) for one S x S output: each [R,R,3] canvas C (either
+// may be NULL, not both) becomes C * 255 rotated by torch.rot90(k=1, dims [0,1]) and resized by nearest F.interpolate,
+// i.e. out[y][x] = C[nx][R-1-ny] * 255 with upsample_nearest2d's index n = min((int)floorf(dst * (R / S)), R - 1) (its
+// S == R and S == 2R special cases select the same texels).  mask[y][x] = 0 iff the three values of the reference image
+// (the texture image if present, else the normal image) all equal 255 after the multiply -- a NaN value is foreground.
+// One thread per output pixel when launched with ceil(S^2 / kDispThreads) blocks (grid-stride for smaller grids).
+constexpr int kDispThreads = 256;
+__global__ void __launch_bounds__(kDispThreads)
+display_kernel(const float* __restrict__ norm, const float* __restrict__ tex, int R, int S, float* __restrict__ norm_out,
+               float* __restrict__ tex_out, uint8_t* __restrict__ mask) {
+  const float scale = (float)R / (float)S;
+  const long long n = (long long)S * S;
+  const long long step = (long long)gridDim.x * blockDim.x;
+  for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < n; p += step) {
+    const int y = (int)(p / S), x = (int)(p % S);
+    const int ny = min((int)floorf(__fmul_rn((float)y, scale)), R - 1);
+    const int nx = min((int)floorf(__fmul_rn((float)x, scale)), R - 1);
+    const size_t src = ((size_t)nx * R + (size_t)(R - 1 - ny)) * 3;
+    float nv[3] = {0.f, 0.f, 0.f}, tv[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      if (norm) norm_out[3 * p + c] = nv[c] = __fmul_rn(norm[src + c], 255.0f);
+      if (tex) tex_out[3 * p + c] = tv[c] = __fmul_rn(tex[src + c], 255.0f);
+    }
+    const bool from_tex = tex != nullptr;             // the mask's reference image
+    bool bg = true;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) bg = bg && (from_tex ? tv[c] : nv[c]) == 255.0f;
+    mask[p] = bg ? 0 : 1;
+  }
+}
+
 }  // namespace surface_k

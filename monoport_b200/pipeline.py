@@ -88,11 +88,16 @@ class FrameGraph:
       mesh_capacity: (vertices, faces) the buffers hold, default (8 R^2, 16 R^2).
     mesh() (after result()) then returns (verts [V,3], faces [F,3] int32, normals or None, colours or None) -- views of this
     graph's buffers, valid until its next launch -- or None for a frame without a surface, and raises RuntimeError for a
-    frame whose mesh exceeds the capacity (run reconstruction() eagerly for that frame)."""
+    frame whose mesh exceeds the capacity (run reconstruction() eagerly for that frame).
+
+    display: the step ends with the demo's display images (RTL/main.py:252-281) of the rendered images, copied into
+      page-locked host buffers of this graph (mp_display_async; needs netC and/or render_normals).  displayed() (after
+      result()) returns them as recon.visulization(*rendered()) does -- numpy views of those buffers, valid until the next
+      launch -- with no device work of its own."""
 
     def __init__(self, net, engine, calib, direction="front", with_encoder=True, input_shape=None, feature_hook=None,
                  netC=None, render_normals=False, canvas=None, mesh=False, mesh_normals=False, mesh_colours=False,
-                 mesh_capacity=None):
+                 mesh_capacity=None, display=False):
         from .modeling.MonoPortNet import FeatureHandle
         from .modeling.geometry import perspective
         from .recon import _DIRS
@@ -117,6 +122,9 @@ class FrameGraph:
         if mesh_colours and netC is None:
             raise ValueError("mesh_colours needs netC")
         self.with_mesh, self.with_mesh_normals, self.with_mesh_colours = bool(mesh), bool(mesh_normals), bool(mesh_colours)
+        if display and netC is None and not render_normals:
+            raise ValueError("display needs an image to show: netC and/or render_normals")
+        self.with_display = bool(display)
         lib = self._lib = _lib.load()
         with torch.cuda.device(dev):
             self.stream = torch.cuda.Stream(dev)
@@ -171,6 +179,9 @@ class FrameGraph:
                 if mesh_colours:
                     self._mesh_pred = torch.empty((3, v_cap), dtype=torch.float32, device=dev)
                     self._mesh_rgb = torch.empty((3, v_cap), dtype=torch.float32, device=dev)
+            if display:
+                from .recon import DisplayBuffers
+                self._display = DisplayBuffers(self.render_norm is not None, self.render_tex is not None, dev)
             self._oct = engine._new_handle(dev)            # private workspace: graphs of different lanes overlap
             self._fh = None
             self._head = net.surface_classifier.handle()
@@ -242,6 +253,8 @@ class FrameGraph:
                 ctypes.c_void_p(self.render_tex.data_ptr()), st), "mp_colorize_surface_async_dcal")
         if self.with_mesh:
             self._mesh_step(st, cal)
+        if self.with_display:
+            self._display.enqueue(self.render_norm, self.render_tex, self.R, st)
 
     def _mesh_step(self, st, cal):
         from .recon import marching_cubes_async
@@ -365,6 +378,18 @@ class FrameGraph:
         return (self.mesh_verts[:nv], self.mesh_faces[:nf], self.mesh_norm[:nv] if self.with_mesh_normals else None,
                 self._mesh_rgb.t()[:nv] if self.with_mesh_colours else None)
 
+    def displayed(self):
+        """After result(): (render_norm [256,256,3] float32, render_tex likewise, mask [256,256,1] bool) -- numpy views of
+        this graph's page-locked buffers, valid until its next launch, equal to recon.visulization(*rendered()).  An image
+        the graph does not render is None; all three are None for an empty frame."""
+        if not self.with_display:
+            raise RuntimeError("FrameGraph.displayed() needs a graph built with display=True")
+        if self._nonempty is None:
+            raise RuntimeError("FrameGraph.displayed() needs the frame's result() first")
+        if not self._nonempty:
+            return None, None, None
+        return self._display.arrays
+
     def close(self):
         if self._oct is not None:
             self.stream.synchronize()
@@ -386,8 +411,9 @@ class FrameGraphRing:
     """`n_lanes` FrameGraphs used round-robin: up to n_lanes frames in flight, results in input order (the graph-captured
     counterpart of FramePipeline for the stages of this library).  Lanes built with netC take (x, x_colour) items and yield
     result() + rendered(): (sdf, X, Y, Z, norm, render_norm, render_tex).  Lanes built with mesh=True append mesh()'s
-    (verts, faces, normals, colours), four Nones for a frame without a surface.  run(items, calibs) takes the cameras of the
-    frames too (zipped with items; see FrameGraph.launch)."""
+    (verts, faces, normals, colours), four Nones for a frame without a surface.  Lanes built with display=True then append
+    displayed()'s (render_norm, render_tex, mask).  run(items, calibs) takes the cameras of the frames too (zipped with
+    items; see FrameGraph.launch)."""
 
     def __init__(self, make_graph, n_lanes=2):
         self.lanes = [make_graph() for _ in range(int(n_lanes))]
@@ -399,6 +425,8 @@ class FrameGraphRing:
             out = out + lane.rendered()
         if lane.with_mesh:
             out = out + (lane.mesh() or (None,) * 4)
+        if lane.with_display:
+            out = out + lane.displayed()
         return out
 
     def run(self, iterable, calibs=None):

@@ -5,7 +5,9 @@
   marching_cubes, reconstruction: additions asked for by the north star (the reference has no marching cubes;
                                  `reconstruction` follows upstream PIFu's signature);
   marching_cubes_async, mesh_normals, mesh_colours: the mesh of a captured frame (FrameGraph(mesh=True)) and its eager
-                                 twins -- normals and upstream PIFu's gen_mesh_color vertex colours at the vertices.
+                                 twins -- normals and upstream PIFu's gen_mesh_color vertex colours at the vertices;
+  visulization                 : the demo's display images (RTL/main.py:252-281), the eager twin of
+                                 FrameGraph(display=True).
 """
 import ctypes
 import threading
@@ -369,6 +371,57 @@ def _surface_normals_device(net, feat, X, Y, Z, calib_tensor, resolution, b_min,
             ctypes.c_void_p(scratch.data_ptr()), ctypes.c_void_p(out.data_ptr()), _lib.stream_ptr(device)),
             "mp_surface_normals_async")
     return out
+
+
+DISPLAY_SIZE = 256          # render_size of the demo's display images (RTL/main.py:257)
+
+
+class DisplayBuffers:
+    """What mp_display_async writes for [R,R,3] canvases on `device`: page-locked host images norm / tex ([S,S,3] float32,
+    None for an absent image) and mask ([S,S,1] bool), with their numpy views `arrays`, and the device staging buffer."""
+
+    def __init__(self, has_norm, has_tex, device, size=DISPLAY_SIZE):
+        S = self.size = int(size)
+        self.norm = torch.empty((S, S, 3), dtype=torch.float32, pin_memory=True) if has_norm else None
+        self.tex = torch.empty((S, S, 3), dtype=torch.float32, pin_memory=True) if has_tex else None
+        self.mask = torch.empty((S, S, 1), dtype=torch.bool, pin_memory=True)
+        self.staging = torch.empty((3 * (int(has_norm) + int(has_tex)) + 1) * S * S, dtype=torch.float32, device=device)
+        self.arrays = tuple(None if t is None else t.numpy() for t in (self.norm, self.tex, self.mask))
+
+    def enqueue(self, norm_dev, tex_dev, R, stream):
+        """mp_display_async of the canvases (device tensors or None, matching the buffers) on `stream`"""
+        def p(t):
+            return None if t is None else ctypes.c_void_p(t.data_ptr())
+        _lib.check(_lib.load().mp_display_async(p(norm_dev), p(tex_dev), int(R), self.size, p(self.norm), p(self.tex),
+                                                p(self.mask), p(self.staging), stream), "mp_display_async")
+
+
+@torch.no_grad()
+def visulization(render_norm, render_tex=None):
+    """The demo's display images (RTL/main.py:252-281, the reference's name and return types): each [R,R,3] float32 CUDA
+    canvas (either may be None) x255, rotated by torch.rot90(k=1) over dims (0, 1) and resized to 256 x 256 by nearest
+    F.interpolate, as numpy float32 [256,256,3]; and mask, numpy bool [256,256,1], False where the three channels of the
+    texture image (else the normal image) all equal 255.  (None, None, None) without any image.  One kernel and the
+    device-to-host copies of mp_display_async (what FrameGraph(display=True) captures, so both give the same bits) on the
+    current stream, then a synchronisation."""
+    if render_norm is None and render_tex is None:
+        return None, None, None
+    imgs = [t for t in (render_norm, render_tex) if t is not None]
+    if any(t.device.type != "cuda" for t in imgs):
+        raise RuntimeError("monoport_b200.visulization: CUDA tensors only (no CPU path)")
+    R = imgs[0].shape[0]
+    for t in imgs:
+        if t.dtype != torch.float32 or t.dim() != 3 or tuple(t.shape) != (R, R, 3) or t.device != imgs[0].device:
+            raise ValueError("visulization takes float32 [R,R,3] canvases of one size on one device; got %s" % (
+                [(t.dtype, tuple(t.shape), str(t.device)) for t in imgs],))
+    norm = None if render_norm is None else render_norm.detach().contiguous()
+    tex = None if render_tex is None else render_tex.detach().contiguous()
+    dev = imgs[0].device
+    with _lib.device_guard(dev):
+        buf = DisplayBuffers(norm is not None, tex is not None, dev)
+        buf.enqueue(norm, tex, R, _lib.stream_ptr(dev))
+        torch.cuda.current_stream(dev).synchronize()
+    return buf.arrays
 
 
 @torch.no_grad()
