@@ -87,11 +87,9 @@ extern "C" int mp_mlp_create(int n_layers, const int* channels, const float* con
   static std::atomic<unsigned long long> next_gen{1};
   h->gen = next_gen.fetch_add(1);
   {
-    // validated feature range of the tensor-core programs (DESIGN.md, precision): measured error ~2.7e-5 x (max|feature| / 5)
-    // for the geometry head, 5.6e-5 x (max|feature| / 5) for the colour head; the limits keep both under 1e-4 with margin
-    const bool colour = channels[n_layers] == 3;
+    // validated feature range of the tensor-core programs, per output count and last op (DESIGN.md, precision)
     const char* v = getenv("MONOPORT_B200_TC_FEATURE_LIMIT");
-    h->tc_amax_limit = v ? (float)atof(v) : (colour ? 8.0f : 12.0f);
+    h->tc_amax_limit = v ? (float)atof(v) : mp_tc_default_feature_limit(channels[n_layers], last_op);
   }
   cudaGetDevice(&h->device);
   for (int l = 0; l <= n_layers; ++l) h->channels[l] = channels[l];

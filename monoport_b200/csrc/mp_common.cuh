@@ -88,6 +88,17 @@ struct mp_mlp {
   float tc_amax_limit;
 };
 
+// Default tc_amax_limit of a head with `res` outputs and last op `last_op` (DESIGN.md §5, "Feature limit per last op").  The
+// tensor-core programs run the geometry widths (res 1) and the colour widths (res 3) with any last op; the error of the
+// logit reaches the output times the last op's slope (Sigmoid 1/4, Tanh and none 1), so the validated range depends on
+// both.  The geometry head's Sigmoid (12) and the colour head's Tanh (8) are the shipped limits; the others were measured on
+// the CPU model of the wgmma program to keep the geometry head's Sigmoid margin under the 1e-4 bar.
+inline float mp_tc_default_feature_limit(int res, int last_op) {
+  if (last_op == MP_LAST_SIGMOID) return 12.0f;
+  if (res == 3) return last_op == MP_LAST_TANH ? 8.0f : 4.0f;
+  return 3.0f;                                       // the geometry widths with Tanh or no last op
+}
+
 struct mp_feat {
   int C, H, W;
   int B;            // maps held (mp_feat_create: 1; mp_feat_create_batch: B).  Every per-texel array below is B

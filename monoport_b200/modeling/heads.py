@@ -27,8 +27,9 @@ class SurfaceClassifier(nn.Module):
             self.filters.append(nn.Conv1d(cin, filter_channels[l + 1], 1))
         self._handle = None
         self._handle_key = None
-        # largest |feature| a frame may have for the tensor-core program to be used (None = the library default: 12 for the
-        # geometry head, 8 for the colour head; float("inf") disables the guard); larger frames take the exact fp32 kernel
+        # largest |feature| a frame may have for the tensor-core program to be used (None = the library default, by output
+        # count and last op: 12 with Sigmoid, 8 for the colour head's Tanh, 4 for a 3-output head with no last op, 3 for a
+        # 1-output head with Tanh or none; float("inf") disables the guard); larger frames take the exact fp32 kernel
         self.tc_feature_limit = None
 
     # ---- autograd / stand-alone module forward (training scaffolding, not the hot path) ----------------
