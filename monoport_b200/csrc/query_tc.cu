@@ -19,8 +19,9 @@
 // layer 2: 128; layer 3: 64); both sample the operands (X, the layer-0 chunks) and run the epilogues.  Warpgroup 2 is the
 // producer: one thread of it streams the weights L2 -> shared memory through a ring of 32 KB stages (cp.async.bulk on
 // mbarriers), pre-packed on the host as K-major SWIZZLE_128B tiles in exactly the order the consumers take them; in layer
-// 1 the ring also borrows the two halves of H1, the layer-2 operand, two more stages in flight where they matter.  The
-// producer gives its registers to the consumers (setmaxnreg: 40 and 232 per thread).  The MMAs run asynchronously: the
+// 1 the ring also borrows the two halves of H1, the layer-2 operand (two more stages in flight where they matter), and in
+// layer 2 the layer-0 chunk buffers (one more).  The producer gives its registers to the consumers (setmaxnreg: 40 and
+// 232 per thread).  The MMAs run asynchronously: the
 // role branches are warp-uniform by construction and the consumers wait for their MMAs at fixed points of a static
 // schedule (see the ring below), so layer-0 chunk c+1 is generated while the MMAs of chunk c are in flight.
 // query_wg_kernel and query_jvp_kernel (the point gradient, forward mode) share that producer, ring and trunk of layers
@@ -60,17 +61,31 @@ template <int C> struct Prog {
   // Layer 1 streams through Slots = Ring + 2: H1 is only written by layer 1's epilogue, so until then its two 32 KB
   // halves are ring slots 0 and 1 and the ring slots proper are 2 .. Slots-1 (slot q at H1 + q x 32 KB)
   static constexpr int Slots = Ring + 2;
+  // Layer 2 streams through Ring2 = Ring + 1 slots: the chunk buffers (32 KB, one stage) are dead from the end of layer 1
+  // until layer 2's epilogue writes H2 there, so during layer 2 they are one more slot, SlotH0 = Slots (at H0).  Layer 2
+  // keeps layer 3's wait depth (Ring - 1 groups in flight), so the extra slot lets the producer refill one step earlier.
+  static constexpr int Ring2 = Ring + 1;
+  static constexpr uint32_t SlotH0 = Slots;
+  // SlotH0's last layer-2 stage is the one whose release waits for the next tile's end of layer 1: it must be among the
+  // Ring stages still held when layer 2 ends, i.e. not the one residue of the last Ring2 steps released in the loop
+  static constexpr bool H0LastHeld = (StagesL2 - 1 - Ring) % Ring2 < Ring;
   // shared memory (offsets inside the 1024-aligned dynamic block)
   static constexpr int X = 0;                                 // XKB x 8 KB
-  static constexpr int H0 = X + XKB * kKb;                    // 2 chunk buffers x 2 K-blocks; H2 (4 K-blocks) after layer 1
+  static constexpr int H0 = X + XKB * kKb;                    // 2 chunk buffers x 2 K-blocks; H2 (4 K-blocks) after layer 2 (layer 2: ring slot SlotH0)
   static constexpr int H1 = H0 + 4 * kKb;                     // 8 K-blocks (layer 1: ring slots 0, 1); the last layer's partial sums after layer 2
   static constexpr int Wr = H1 + 8 * kKb;                     // Ring x 32 KB
   static constexpr int Small = Wr + Ring * kStageBytes;       // zf[64], inimg[64], s4[RES][64]
-  static constexpr int Bars = Small + (2 + RES) * kTile * 4;  // full[Slots], empty[Slots]
-  static constexpr int Total = Bars + 2 * Slots * 8;
-  // slot of a tile's stage: layer 1 stage s -> s % Slots; step k of layers 2 and 3 (counted across both) -> 2 + k % Ring
+  static constexpr int Bars = Small + (2 + RES) * kTile * 4;  // full[Slots + 1], empty[Slots + 1]
+  static constexpr int Total = Bars + 2 * (Slots + 1) * 8;
+  // slot of a tile's stage: layer 1 stage s -> s % Slots; layer 2 step k -> 2 + k % Ring2 (SlotH0 = 2 + Ring: the last
+  // slot of each round, the one that frees last, at the end of layer 1); layer 3 step j -> 2 + j % Ring
   __host__ __device__ static constexpr uint32_t l1_slot(uint32_t s) { return s % (uint32_t)Slots; }
-  __host__ __device__ static constexpr uint32_t l23_slot(uint32_t k) { return 2u + k % (uint32_t)Ring; }
+  __host__ __device__ static constexpr uint32_t l2_slot(uint32_t k) { return 2u + k % (uint32_t)Ring2; }
+  __host__ __device__ static constexpr uint32_t l3_slot(uint32_t j) { return 2u + j % (uint32_t)Ring; }
+  __host__ __device__ static constexpr int slot_off(uint32_t q) { return q == SlotH0 ? H0 : H1 + (int)q * kStageBytes; }
+  // The producer's parity bit of SlotH0 starts at 1: its first fill of a tile waits for the release at the end of that
+  // tile's layer 1 (the other slots start free)
+  static constexpr uint32_t ProducerPhase0 = 1u << SlotH0;
 };
 static_assert(Prog<256>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
 static_assert(Prog<512>::Total + 1024 <= 232448, "shared memory budget (227 KB per CTA)");
@@ -79,6 +94,10 @@ static_assert(Prog<256>::StagesL3 >= Prog<256>::Ring && Prog<512>::StagesL3 >= P
 static_assert(Prog<256>::H1 + 2 * kStageBytes == Prog<256>::Wr && Prog<512>::H1 + 2 * kStageBytes == Prog<512>::Wr, "H1 = ring slots 0, 1");
 static_assert(Prog<256>::StagesL1 % Prog<256>::Slots == 0 && Prog<512>::StagesL1 % Prog<512>::Slots == 0,
               "layer 1's last stages in slots 0 and 1 are StagesL1 - Slots and the one after it");
+static_assert(Prog<256>::H0 + kStageBytes == Prog<256>::H1 && Prog<512>::H0 + kStageBytes == Prog<512>::H1, "the chunk buffers = one stage");
+static_assert(Prog<256>::SlotH0 == 2 + Prog<256>::Ring && Prog<512>::SlotH0 == 2 + Prog<512>::Ring, "l2_slot maps the last step of a round to SlotH0");
+static_assert(Prog<256>::H0LastHeld && Prog<512>::H0LastHeld, "SlotH0's last layer-2 stage is held to the end of layer 2");
+static_assert(Prog<256>::StagesL2 >= Prog<256>::Ring2 && Prog<512>::StagesL2 >= Prog<512>::Ring2, "layer 2 ends by releasing its last Ring2 stages");
 
 struct TcPack {
   __half* wstream;        // stage stream of a tile: Prog<C>::StagesPerTile x 32 KB
@@ -230,23 +249,25 @@ __device__ __forceinline__ void sync_consumers() { tc::bar_sync(1, kConsumers); 
 // by all 8 consumer warps
 template <int C>
 __device__ __forceinline__ void ring_init(uint64_t* full, uint64_t* empty) {
-  for (int s = 0; s < Prog<C>::Slots; ++s) {
+  for (int s = 0; s <= Prog<C>::Slots; ++s) {
     tc::mbar_init(full + s, 1);
     tc::mbar_init(empty + s, kConsumers / 32);
   }
   tc::fence_barrier_init();
 }
 
-// the producer thread: the weight stream of one tile into the ring.  phase: bit q is the parity of slot q's next refill.
+// the producer thread: the weight stream of one tile into the ring.  phase: bit q is the parity of slot q's next refill
+// (P::ProducerPhase0 before the first tile).
 template <int C>
 __device__ __forceinline__ void produce_tile(uint8_t* smem, uint64_t* full, uint64_t* empty, const uint8_t* wsrc, uint32_t& phase) {
   using P = Prog<C>;
   for (int s = 0; s < P::StagesPerTile; ++s) {
-    const uint32_t slot = s < P::StagesL1 ? P::l1_slot(s) : P::l23_slot(s - P::StagesL1);
+    const uint32_t slot = s < P::StagesL1 ? P::l1_slot(s)
+                          : s < P::StagesL1 + P::StagesL2 ? P::l2_slot(s - P::StagesL1) : P::l3_slot(s - P::StagesL1 - P::StagesL2);
     tc::mbar_wait(empty + slot, ((phase >> slot) & 1u) ^ 1u);
     phase ^= 1u << slot;
     tc::mbar_arrive_expect_tx(full + slot, kStageBytes);
-    tc::bulk_g2s(smem + P::H1 + slot * kStageBytes, wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
+    tc::bulk_g2s(smem + P::slot_off(slot), wsrc + (size_t)s * kStageBytes, kStageBytes, full + slot);
   }
 }
 
@@ -272,9 +293,10 @@ __device__ __forceinline__ void run_trunk(uint8_t* smem, uint64_t* full, uint64_
   // each wait below is a fixed wgmma_wait<N> and each release names its stage by arithmetic on its index in the tile.
   // No stage is ever queued at run time; the parity of each slot's next fill is one bit per slot (fphase), flipped by
   // every take, as the producer flips its own bit per refill.
-  // Layer 1 streams through Slots = Ring + 2 slots (H1's halves are slots 0 and 1), layers 2 and 3 through the Ring slots
-  // 2 .. Slots-1: the deeper ring lets the producer run one more K-block ahead in layer 1, where each warpgroup waits for
-  // its K-block's MMAs before it takes the next.  H1's slots are refilled with the next tile's stages 0 and 1 only once
+  // Layer 1 streams through Slots = Ring + 2 slots (H1's halves are slots 0 and 1), layer 2 through the Ring slots
+  // 2 .. Slots-1 and SlotH0 (the chunk buffers), layer 3 through the Ring slots alone: the deeper ring lets the producer
+  // run one more K-block ahead in layer 1, where each warpgroup waits for its K-block's MMAs before it takes the next,
+  // and one step further ahead in layer 2.  H1's slots are refilled with the next tile's stages 0 and 1 only once
   // H1 is dead: their last layer-1 stages (Defer, Defer + 1) are released at the end of the tile, and the layer-1
   // epilogue writes H1 only after both warpgroups retired every MMA that read those slots.
   // Deadlock freedom: the producer refills a slot with stage s once all 8 consumer warps have released the stage that last
@@ -285,9 +307,13 @@ __device__ __forceinline__ void run_trunk(uint8_t* smem, uint64_t* full, uint64_
   //     taking 2i+1 needs 2i+1-Slots <= 2i-3, which both warpgroups released by the end of K-block i-1's takes (its
   //     owner after its wait<0> there); taking 2i needs 2i-Slots, released a K-block earlier still.  The deferred stages
   //     are last users of slots 0 and 1, whose next stages are the next tile's 0 and 1;
-  //   layers 2 and 3 (one stage per K-block step, read by both warpgroups): taking step k needs k - Ring (for k < Ring a
-  //     layer-1 stage of slot 2 + k, released in layer 1), so before it the warpgroup lets at most Ring - 1 groups stay
-  //     in flight (wait<Ring-1>) and releases k - Ring.
+  //   layers 2 and 3 (one stage per K-block step, read by both warpgroups, through R = Ring2 slots in layer 2 and Ring in
+  //     layer 3): before taking step k the warpgroup lets at most Ring - 1 groups stay in flight (wait<Ring-1>) and
+  //     releases k - Ring; taking step k needs k - R, which is released at step k - R + Ring <= k.  For k < R the slot's
+  //     last stage came before the layer: a layer-1 stage of slots 2 .. Slots-1 (released in layer 1), a layer-2 stage
+  //     (released at the end of layer 2), or, for SlotH0, the release at the end of this tile's layer 1, once no MMA
+  //     reads the chunk buffers.  The last layer-2 stage in SlotH0 is not released at the end of layer 2 (H2 is written
+  //     there): its release is the next tile's end of layer 1.
   // Every layer ends with wait<0> and releases its own stages still held, so a layer starts with nothing in flight.
   constexpr uint32_t Defer = P::StagesL1 - P::Slots;
   auto release_if = [&](uint32_t slot, bool pred) {
@@ -300,7 +326,7 @@ __device__ __forceinline__ void run_trunk(uint8_t* smem, uint64_t* full, uint64_
     tc::mbar_wait(full + slot, (fphase >> slot) & 1u);
     fphase ^= 1u << slot;
   };
-  auto slot_off = [&](uint32_t slot) { return P::H1 + (int)slot * kStageBytes; };
+  auto slot_off = [&](uint32_t slot) { return P::slot_off(slot); };
   // layer 1, K-block i (A operand at shared offset a_off): this warpgroup's 256 outputs times its stage 2i + wg
   auto l1_kblock = [&](float (&acc)[128], int i, int a_off) {
     const uint32_t s0 = 2 * i, mine = s0 + wg, prev = mine - 2;
@@ -315,21 +341,23 @@ __device__ __forceinline__ void run_trunk(uint8_t* smem, uint64_t* full, uint64_
     for (int k = 0; k < 4; ++k) tc::wgmma_m64n256(acc, da + 2 * k, db + 2 * k);
     tc::wgmma_commit();
   };
-  // layers 2 and 3, step k of a layer whose steps start at k_layer: frees the slot of step k (see above) and takes it
-  auto step_take = [&](uint32_t k_layer, int k) {
+  // layers 2 and 3, step k of a layer whose slots are slot(k): retires and releases step k - Ring (see above), takes step k
+  auto step_take = [&](auto slot, int k) {
     if (k >= Ring) {
       tc::wgmma_wait<Ring - 1>();
-      release(P::l23_slot(k_layer + k - Ring));
+      release(slot(k - Ring));
     }
-    take(P::l23_slot(k_layer + k));
+    take(slot(k));
     tc::wgmma_fence();
   };
-  // end of a layer of n steps (n >= Ring): all MMAs complete, the last Ring stages released
-  auto layer_end = [&](uint32_t k_layer, int n) {
+  // end of a layer of n steps (n >= Ring): all MMAs complete, the last Ring stages released (but not SlotH0's)
+  auto layer_end = [&](auto slot, int n) {
     tc::wgmma_wait<0>();
 #pragma unroll
-    for (int j = Ring; j > 0; --j) release(P::l23_slot(k_layer + n - j));
+    for (int j = Ring; j > 0; --j) release_if(slot(n - j), slot(n - j) != P::SlotH0);
   };
+  auto l2_slot = [](int k) { return P::l2_slot((uint32_t)k); };
+  auto l3_slot = [](int j) { return P::l3_slot((uint32_t)j); };
 
   // ---- layer 1: 8 sampled layer-0 chunks (2 K-blocks each), then X; this warpgroup's 256 of the 512 outputs
   {
@@ -352,6 +380,7 @@ __device__ __forceinline__ void run_trunk(uint8_t* smem, uint64_t* full, uint64_
     for (int kb = 0; kb < XKB; ++kb) l1_kblock(acc, 16 + kb, P::X + kb * kKb);
     tc::wgmma_wait<0>();
     l1_release(2 * (16 + XKB - 1) + wg);
+    release(P::SlotH0);      // this warpgroup's MMAs reading the chunk buffers have retired: layer 2 may stream into them
     sync_consumers();        // H1 was ring slots 0 and 1: every MMA that read them has retired in both warpgroups
     epi(acc, side_off(1), wg * 256, P::H1);
     tc::fence_proxy_async_smem();
@@ -364,13 +393,14 @@ __device__ __forceinline__ void run_trunk(uint8_t* smem, uint64_t* full, uint64_
     for (int j = 0; j < 64; ++j) acc[j] = 0.f;
 #pragma unroll 1
     for (int kb = 0; kb < P::StagesL2; ++kb) {
-      step_take(0, kb);
-      const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(slot_off(P::l23_slot(kb)) + wg * 16384);
+      step_take(l2_slot, kb);
+      const uint64_t da = desc(kb < 8 ? P::H1 + kb * kKb : P::X + (kb - 8) * kKb), db = desc(slot_off(l2_slot(kb)) + wg * 16384);
 #pragma unroll
       for (int k = 0; k < 4; ++k) tc::wgmma_m64n128(acc, da + 2 * k, db + 2 * k);
       tc::wgmma_commit();
     }
-    layer_end(0, P::StagesL2);
+    layer_end(l2_slot, P::StagesL2);
+    sync_consumers();        // H2 overwrites SlotH0's last stage: every consumer warp has retired the MMAs that read it
     epi(acc, side_off(2), wg * 128, P::H0);
     tc::fence_proxy_async_smem();
     sync_consumers();
@@ -382,18 +412,18 @@ __device__ __forceinline__ void run_trunk(uint8_t* smem, uint64_t* full, uint64_
     for (int j = 0; j < 32; ++j) acc[j] = 0.f;
 #pragma unroll 1
     for (int q = 0; q < P::StagesL3; ++q) {
-      step_take(P::StagesL2, q);
+      step_take(l3_slot, q);
 #pragma unroll
       for (int sub = 0; sub < 2; ++sub) {
         const int kb = (2 * q + sub) % (XKB + 4);
         const uint64_t da = desc(kb < XKB ? P::X + kb * kKb : P::H0 + (kb - XKB) * kKb);
-        const uint64_t db = desc(slot_off(P::l23_slot(P::StagesL2 + q)) + sub * 16384 + wg * 8192);
+        const uint64_t db = desc(slot_off(l3_slot(q)) + sub * 16384 + wg * 8192);
 #pragma unroll
         for (int k = 0; k < 4; ++k) tc::wgmma_m64n64(acc, da + 2 * k, db + 2 * k);
       }
       tc::wgmma_commit();
     }
-    layer_end(P::StagesL2, P::StagesL3);
+    layer_end(l3_slot, P::StagesL3);
     head(acc);
   }
   sync_consumers();        // the per-point scalars and X are rewritten by the next tile
@@ -419,7 +449,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   // every pointer below is a shared-memory pointer: 32-bit addresses and st.shared instead of 64-bit generic ones
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::Bars);
-  uint64_t* empty = full + P::Slots;
+  uint64_t* empty = full + P::Slots + 1;
   float* s_zf = reinterpret_cast<float*>(smem + P::Small);
   float* s_in = s_zf + kTile;
   float* s_s4 = s_in + kTile;
@@ -456,7 +486,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
     tc::setmaxnreg_dec<kProducerRegs>();
     if (warp == 8 && lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
-      uint32_t phase = 0;
+      uint32_t phase = P::ProducerPhase0;
       bool skip = false;
       int guard_b = -1;
       for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
@@ -768,7 +798,7 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
   MP_DYN_SMEM(uint8_t, smem_raw);
   uint8_t* smem = smem_raw + ((1024u - (tc::smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + P::Bars);
-  uint64_t* empty = full + P::Slots;
+  uint64_t* empty = full + P::Slots + 1;
   float* s_zf = reinterpret_cast<float*>(smem + P::Small);   // [NP]
   float* s_in = s_zf + NP;                                    // [NP]
   float* s_uvw = s_in + NP;                                   // [3][NP]
@@ -793,7 +823,7 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
     tc::setmaxnreg_dec<kProducerRegs>();
     if (warp == 8 && lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
-      uint32_t phase = 0;
+      uint32_t phase = P::ProducerPhase0;
       for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) produce_tile<C>(smem, full, empty, wsrc, phase);
     }
     return;
