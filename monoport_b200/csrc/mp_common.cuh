@@ -421,7 +421,40 @@ void mp_tc_release(mp_mlp* mlp);
 // generic query dispatch (mode handling) used by the API and the octree engine
 int mp_query_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst,
                       int mode, cudaStream_t st, const MpBatch* bt = nullptr);
-void mp_fill_calib(MpCalib& c, const float* calib12, int projection, float z_scale);
-const MpBatch* mp_single_calib(MpCalib& cal, MpBatch& bt, const float* calib12, const float* calib_dev, int projection,
-                               float z_scale);
-void mp_fill_grid_geom(MpPointSrc& s, int res, int node_stride, int r_final, const float* bmin, const float* bmax);
+
+// Host helpers of the launches (header-only, so that the CPU model of tests/emu runs these very lines)
+inline void mp_fill_calib(MpCalib& c, const float* calib12, int projection, float z_scale) {
+  memset(&c, 0, sizeof(c));
+  c.has = calib12 != nullptr;
+  if (calib12) memcpy(c.m, calib12, 12 * sizeof(float));
+  c.perspective = (projection == MP_PROJ_PERSPECTIVE) && c.has;
+  c.z_scale = z_scale;
+}
+
+// The camera of a single-map call: calib12 (host memory, or none) in the kernel parameters, or -- calib_dev set, the _dcal
+// entry points -- 12 floats in device memory that the kernels read when they run.  Returns the batch to launch with
+// (nullptr: the by-value camera).
+inline const MpBatch* mp_single_calib(MpCalib& cal, MpBatch& bt, const float* calib12, const float* calib_dev, int projection,
+                                      float z_scale) {
+  if (!calib_dev) {
+    mp_fill_calib(cal, calib12, projection, z_scale);
+    return nullptr;
+  }
+  mp_fill_calib(cal, nullptr, projection, z_scale);
+  cal.has = 1;
+  cal.perspective = projection == MP_PROJ_PERSPECTIVE;
+  bt = mp_device_calib(calib_dev);
+  return &bt;
+}
+
+inline void mp_fill_grid_geom(MpPointSrc& s, int res, int node_stride, int r_final, const float* bmin, const float* bmax) {
+  s.res = res;
+  s.node_stride = node_stride;
+  s.r_final = r_final;
+  s.inv_r = 1.0f / (float)r_final;
+  s.half_inv_r = (float)(1.0 / (2.0 * (double)r_final));
+  for (int a = 0; a < 3; ++a) {
+    s.bmin[a] = bmin[a];
+    s.bext[a] = bmax[a] - bmin[a];   // fp32 subtraction, like torch's (b_max - b_min)
+  }
+}

@@ -3,100 +3,30 @@
 //   emu_query_grad in.bin out.f32 [sms] [grad_out.f32]
 // in.bin as for emu_query_fp32; grad_out.f32 (optional): [Res][N] fp32, otherwise all ones.  out.f32 = value [Res][N]
 // followed by the point gradient [3][N].  sms = simulated SM count (grid size), default 3.
-#include <cuda_runtime.h>
-#include <stdarg.h>
-
-#define MP_EMU_CUDA_TYPES 1
-#include "cuda_emu.h"
-
-alignas(1024) static float g_dyn_smem[240 * 1024 / 4];        // the kernel's dynamic shared memory
-void* mp_emu_dyn_smem() { return g_dyn_smem; }
-
-static int g_sms = 3;
-extern "C" {
-cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
-cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) {
-  *v = a == cudaDevAttrMultiProcessorCount ? g_sms : (a == cudaDevAttrMaxSharedMemoryPerBlockOptin ? 232448 : 0);
-  return cudaSuccess;
-}
-cudaError_t cudaGetLastError(void) { return cudaSuccess; }
-const char* cudaGetErrorString(cudaError_t) { return "emulated"; }
-}
-template <class T> static cudaError_t cudaFuncSetAttribute(T*, cudaFuncAttribute, int) { return cudaSuccess; }
-#define MP_EMU_LAUNCH(grid, block, call) cuda_emu::launch(dim3((unsigned)(grid)), dim3((unsigned)(block)), [&] { call; })
-
-static char g_err[512];
-void mp_set_error(const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-}
-
+#include "emu_host.h"
 #include "../../monoport_b200/csrc/query_fp32.cu"
 
 int main(int argc, char** argv) {
   if (argc < 3 || argc > 5) { fprintf(stderr, "usage: emu_query_grad in.bin out.f32 [sms] [grad_out.f32]\n"); return 2; }
-  if (argc >= 4) g_sms = atoi(argv[3]);
-  FILE* f = fopen(argv[1], "rb");
-  if (!f) { perror(argv[1]); return 2; }
-  int32_t hd[8];
-  float zs, calib[12];
-  if (fread(hd, 4, 8, f) != 8 || fread(&zs, 4, 1, f) != 1 || fread(calib, 4, 12, f) != 12) { fprintf(stderr, "short header\n"); return 2; }
-  const int C = hd[0], H = hd[1], W = hd[2], N = hd[3], has_calib = hd[4], persp = hd[5], res = hd[6], last_op = hd[7];
-  auto rd = [&](FILE* g, size_t n) { std::vector<float> v(n); if (fread(v.data(), 4, n, g) != n) { fprintf(stderr, "short file\n"); exit(2); } return v; };
-  std::vector<float> nchw = rd(f, (size_t)C * H * W), pts = rd(f, (size_t)3 * N);
-  const int chans[6] = {C + 1, 1024, 512, 256, 128, res};
-  mp_mlp mlp;
-  memset(&mlp, 0, sizeof(mlp));
-  mlp.n_layers = 5; mlp.skip = 1; mlp.last_op = last_op;
-  std::vector<std::vector<float>> Ws(5), Wt(5), Bs(5);
-  for (int l = 0; l <= 5; ++l) mlp.channels[l] = chans[l];
-  for (int l = 0; l < 5; ++l) {
-    const int cin = chans[l] + (l ? chans[0] : 0), cout = chans[l + 1];
-    mlp.cin[l] = cin; mlp.cout[l] = cout;
-    Ws[l] = rd(f, (size_t)cin * cout);
-    Bs[l] = rd(f, cout);
-    Wt[l].resize((size_t)cin * cout);                    // what transpose_w_kernel produces: [cin][cout]
-    for (int o = 0; o < cout; ++o)
-      for (int k = 0; k < cin; ++k) Wt[l][(size_t)k * cout + o] = Ws[l][(size_t)o * cin + k];
-    mlp.w[l] = Ws[l].data(); mlp.wt[l] = Wt[l].data(); mlp.bias[l] = Bs[l].data();
-  }
-  fclose(f);
+  if (argc >= 4) g_fake_sms = atoi(argv[3]);
+  EmuInput in = emu_read_input(argv[1]);
+  const int N = in.N, res = in.res;
+  EmuMlp m = emu_make_mlp(in);
   std::vector<float> gout;
   if (argc >= 5) {
     FILE* g = fopen(argv[4], "rb");
     if (!g) { perror(argv[4]); return 2; }
-    gout = rd(g, (size_t)res * N);
+    gout = emu_read(g, (size_t)res * N);
     fclose(g);
   }
-  std::vector<float> nhwc((size_t)C * H * W);
-  for (int c = 0; c < C; ++c)
-    for (int p = 0; p < H * W; ++p) nhwc[(size_t)p * C + c] = nchw[(size_t)c * H * W + p];
-  mp_feat feat;
-  memset(&feat, 0, sizeof(feat));
-  feat.C = C; feat.H = H; feat.W = W; feat.nhwc32 = nhwc.data(); feat.B = 1;
-  MpPointSrc src;
-  memset(&src, 0, sizeof(src));
-  src.kind = MP_SRC_ROWS;
-  src.px = pts.data(); src.py = pts.data() + N; src.pz = pts.data() + 2 * (size_t)N;
-  src.pstride = 1;
-  src.n = N;
-  MpCalib cal;
-  memset(&cal, 0, sizeof(cal));
-  cal.has = has_calib;
-  memcpy(cal.m, calib, sizeof(calib));
-  cal.perspective = persp && has_calib;
-  cal.z_scale = zs;
+  EmuFeat ef = emu_make_feat(in);
   // one buffer: value [res][N], gradient [3][N], then a sentinel
   std::vector<float> out((size_t)(res + 3) * N + 1, -4242.f);
   float* dp = out.data() + (size_t)res * N;
-  const int rc = mp_launch_query_grad(&mlp, &feat, src, cal, gout.empty() ? nullptr : gout.data(), N, out.data(), N, dp, N,
-                                      nullptr);
+  const int rc = mp_launch_query_grad(&m.mlp, &ef.feat, emu_rows_src(in), in.cal, gout.empty() ? nullptr : gout.data(), N,
+                                      out.data(), N, dp, N, nullptr);
   if (rc != MP_OK) { fprintf(stderr, "mp_launch_query_grad: %s\n", g_err); return 3; }
   if (out[(size_t)(res + 3) * N] != -4242.f) { fprintf(stderr, "wrote past the output\n"); return 3; }
-  f = fopen(argv[2], "wb");
-  fwrite(out.data(), 4, (size_t)(res + 3) * N, f);
-  fclose(f);
+  emu_write(argv[2], out.data(), (size_t)(res + 3) * N);
   return 0;
 }

@@ -9,6 +9,7 @@ import torch
 
 from oracle import spec
 from helpers import GOLDEN, checksum
+from shape_cases import load_shape_grad_case
 
 
 def query_grad_ref(feat, points, calib, Ws, bs, last_op, projection="orthogonal", z_scale=spec.Z_SCALE, grad_output=None,
@@ -65,3 +66,31 @@ def within_bar(got, ref):
     frac = (err <= 2e-5 * scale).double().mean().item()
     worst = err.max().item() / scale
     return worst <= 1e-3 and frac >= 0.99, "max|err|/max|g| = %.2e, fraction within 2e-5: %.4f" % (worst, frac)
+
+
+# ---- the tensor-core gradient program (query_jvp_kernel) -------------------------------------------------------------------
+# the first 8 points of every case are border_points(): on the image border / corners and far outside
+GOLDEN_CASES = [("grad", "g_rot", 64), ("grad", "g_persp", 48), ("grad", "g_nocalib", 48), ("grad", "g_bigfeat", 48),
+                ("grad", "c_rot", 32), ("shape", "g_wide", 72), ("shape", "g_tiny", 72)]
+
+
+def load_golden(kind, name):
+    """a case of GOLDEN_CASES: kind "grad" (tests/golden/grad_*.npz) or "shape" (shape_grad_*.npz)"""
+    return load_grad_case(name) if kind == "grad" else load_shape_grad_case(name)
+
+
+# Goldens on which the fp16 restatement (tc_jvp_ref, all points of the golden) does not pass the bar below with a 2x margin
+# get its own distance from grad64 + 10 % as their bar: shape_grad_g_wide's largest component is 2.85e-2 max|g| away
+# (a leaky-ReLU kink taken on the other side in fp16).  Every other golden keeps the bar (DESIGN.md, section F1 triple-prime).
+MAX_BAR = {"g_wide": 3.1e-2}
+
+
+def tc_bar(got, g64, name=None):
+    """The error bar of the tensor-core gradient against the reference's fp64 gradient: median <= 5e-5 max|g|, 99 % of the
+    components <= 5e-3 max|g|, every component <= 5e-2 max|g| (MAX_BAR for the goldens named there).  (The tail comes
+    from fp16 taking the other side of a leaky-ReLU kink.)  -> (ok, message)"""
+    scale = g64.abs().max().item()
+    err = (got.double() - g64.double()).abs().flatten() / scale
+    med, p99, worst = err.median().item(), torch.quantile(err, 0.99).item(), err.max().item()
+    return (med <= 5e-5 and p99 <= 5e-3 and worst <= MAX_BAR.get(name, 5e-2),
+            "|err|/max|g|: median %.2e, p99 %.2e, max %.2e" % (med, p99, worst))

@@ -3,8 +3,6 @@ and its exact fp32 twin) and the normal-image kernel, compiled unmodified agains
 the vertex count on the device and the range guard decided there; and the compiler report of the new fp32 instantiations."""
 import os
 import re
-import shutil
-import struct
 import subprocess
 
 import numpy as np
@@ -12,13 +10,9 @@ import pytest
 import torch
 
 from oracle import spec
+from emu_harness import build, needs_emu, ptxas_report, write_input
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-CUDA_INC = "/usr/local/cuda/include"
-
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None or not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")),
-                                reason="g++ / CUDA headers not available")
+pytestmark = needs_emu
 
 R = 65
 UNIT = ((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0))
@@ -26,28 +20,19 @@ B1 = ((-0.83, -1.17, -0.61), (0.91, 1.06, 0.77))     # asymmetric, no power-of-t
 GUARD_NONE, GUARD_IN_RANGE, GUARD_OUT_OF_RANGE = 0, 1, 2
 
 
-def _build(tmp, name, extra):
-    exe = os.path.join(tmp, name)
-    cmd = ["g++", "-std=c++17", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas", "-fno-strict-aliasing",
-           "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU] + list(extra) + ["-o", exe, os.path.join(EMU, name + ".cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
-
-
 @pytest.fixture(scope="module")
 def emu_tc(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu_cs_tc")), "emu_colour_surface_tc", ["-O3", "-march=native"])
+    return build(tmp_path_factory, "emu_colour_surface_tc")
 
 
 @pytest.fixture(scope="module")
 def emu_fp32(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu_cs_fp32")), "emu_colour_surface_fp32", ["-O2"])
+    return build(tmp_path_factory, "emu_colour_surface_fp32")
 
 
 @pytest.fixture(scope="module")
 def emu_normals(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu_rn")), "emu_render_normals", ["-O1"])
+    return build(tmp_path_factory, "emu_render_normals")
 
 
 @pytest.fixture(scope="module")
@@ -65,17 +50,7 @@ def scene():
 
 def _write(path, sc, rows, feat=None):
     """emu input: header, z_scale, calib, the map, three rows of N floats, the head"""
-    feat = sc["feat"] if feat is None else feat
-    n = rows.shape[1]
-    with open(path, "wb") as f:
-        f.write(struct.pack("8i", 512, 32, 32, n, 1, 0, 3, spec.LAST_TANH))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        f.write(struct.pack("12f", *sc["cal"][0, :3, :4].reshape(-1).tolist()))
-        f.write(feat.numpy().tobytes())
-        f.write(np.ascontiguousarray(rows, dtype=np.float32).tobytes())
-        for W, b in zip(sc["Ws"], sc["bs"]):
-            f.write(W.numpy().tobytes())
-            f.write(b.numpy().tobytes())
+    write_input(path, sc["feat"] if feat is None else feat, rows, sc["cal"], "orthogonal", 3, spec.LAST_TANH, sc["Ws"], sc["bs"])
 
 
 def _vertex_rows(sc, n=200):
@@ -226,27 +201,13 @@ def test_normal_image_is_torchs(emu_normals, tmp_path, count, blocks):
 
 # ---- compiler report of the exact program -----------------------------------------------------------------------------
 @pytest.fixture(scope="module")
-def fp32_ptxas(tmp_path_factory):
-    from monoport_b200 import build as lib_build
-    try:
-        nvcc = lib_build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    out = tmp_path_factory.mktemp("ptxas_fp32") / "query_fp32.o"
-    p = subprocess.run([nvcc] + lib_build.NVCC_FLAGS + ["-c", os.path.join(lib_build.CSRC, "query_fp32.cu"), "-o", str(out)],
-                       capture_output=True, text=True)
-    assert p.returncode == 0, p.stdout + p.stderr
+def fp32_ptxas():
+    """{(tile P, surface instantiation): its ptxas lines} of query_fp32_kernel"""
     stats = {}
-    current = None
-    for line in (p.stdout + p.stderr).splitlines():
-        m = re.search(r"Compiling entry function '([^']*query_fp32_kernelILi(\d+)ELb([01])E[^']*)'", line)
+    for name, lines in ptxas_report("query_fp32.cu")[0]:
+        m = re.search(r"query_fp32_kernelILi(\d+)ELb([01])E", name)
         if m:
-            current = (int(m.group(2)), m.group(3) == "1")
-            stats[current] = ""
-        elif "Compiling entry function" in line:
-            current = None
-        elif current and ("stack frame" in line or "registers" in line):
-            stats[current] += line
+            stats[(int(m.group(1)), m.group(2) == "1")] = " ".join(lines)
     return stats
 
 

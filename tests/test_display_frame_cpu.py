@@ -5,7 +5,6 @@ compiler report of the kernel; and the refusals of mp_display_async that need no
 import ctypes
 import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -13,25 +12,15 @@ import pytest
 import torch
 
 from display_cases import display_canvases, visulization_ref
+from emu_harness import build, needs_emu, ptxas_report
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-GOLDEN = os.path.join(HERE, "golden")
-CUDA_INC = "/usr/local/cuda/include"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 S = 256
-
-emu_available = pytest.mark.skipif(shutil.which("g++") is None or not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")),
-                                   reason="g++ / CUDA headers not available")
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("emu_display") / "emu_display")
-    cmd = ["g++", "-std=c++17", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas", "-fno-strict-aliasing", "-O1",
-           "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU, "-o", exe, os.path.join(EMU, "emu_display.cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
+    return build(tmp_path_factory, "emu_display")
 
 
 def _display(exe, tmp_path, norm, tex, blocks, size=S):
@@ -86,7 +75,7 @@ def _golden_want(g, case):
 
 
 # ---- the kernel against the reference's outputs ------------------------------------------------------------------------
-@emu_available
+@needs_emu
 @pytest.mark.parametrize("case", CASES)
 @pytest.mark.parametrize("R", [257, 129, 33])
 def test_kernel_matches_reference_goldens(emu, tmp_path, R, case):
@@ -126,7 +115,7 @@ def test_restatement_matches_reference_goldens(R):
 
 
 # ---- the kernel against the restatement over every nearest path ----------------------------------------------------------
-@emu_available
+@needs_emu
 @pytest.mark.parametrize("R,size", [(17, S), (33, S), (128, S), (129, S), (256, S), (257, S), (513, S), (33, 100)])
 def test_kernel_matches_restatement(emu, tmp_path, R, size):
     """Downscale (513, 257), identity (256), x2 (128) and general nearest upscales, each case on its own CTA count: bit for
@@ -144,19 +133,10 @@ def test_kernel_matches_restatement(emu, tmp_path, R, size):
 
 
 # ---- compiler report ---------------------------------------------------------------------------------------------------
-def test_display_kernel_has_no_frame_and_no_spills(tmp_path):
-    from monoport_b200 import build as lib_build
-    try:
-        nvcc = lib_build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    p = subprocess.run([nvcc] + lib_build.NVCC_FLAGS + ["-c", os.path.join(lib_build.CSRC, "surface.cu"), "-o",
-                                                        str(tmp_path / "surface.o")], capture_output=True, text=True)
-    assert p.returncode == 0, p.stdout + p.stderr
-    log = (p.stdout + p.stderr).splitlines()
-    at = [i for i, line in enumerate(log) if re.search(r"Compiling entry function '\w*display_kernel\w*'", line)]
+def test_display_kernel_has_no_frame_and_no_spills():
+    at = [lines for name, lines in ptxas_report("surface.cu")[0] if re.fullmatch(r"\w*display_kernel\w*", name)]
     assert len(at) == 1, at
-    stats = " ".join(log[at[0]:at[0] + 4])
+    stats = " ".join(at[0])
     assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in stats, stats
 
 

@@ -5,8 +5,6 @@ query over a node list with the volume scatter, the tensor-core query over a nod
 surface render of both programs, and both gradient programs.  Every case runs two launches through one buffer rewritten
 between them, and each must give its own camera's result."""
 import os
-import shutil
-import struct
 import subprocess
 
 import numpy as np
@@ -14,34 +12,18 @@ import pytest
 import torch
 
 from oracle import spec
+from emu_harness import build, needs_emu, write_input
 from grad_cases import load_grad_case
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-CUDA_INC = "/usr/local/cuda/include"
-
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None or not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")),
-                                reason="g++ / CUDA headers not available")
+pytestmark = needs_emu
 
 R = 65
 UNIT = ["-1", "-1", "-1", "1", "1", "1"]
 
 
-def _build(tmp, name, opt):
-    exe = os.path.join(tmp, name)
-    cmd = ["g++", "-std=c++17", opt, "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas", "-fno-strict-aliasing",
-           "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU, "-o", exe, os.path.join(EMU, name + ".cpp")]
-    if opt == "-O3":
-        cmd.insert(3, "-march=native")
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("emu_dcal"))
-    return dict(fp32=_build(d, "emu_dcal_fp32", "-O2"), tc=_build(d, "emu_dcal_tc", "-O3"))
+    return {k: build(tmp_path_factory, "emu_dcal_" + k) for k in ("fp32", "tc")}
 
 
 def _case(name, proj):
@@ -62,19 +44,8 @@ def _second_camera(c):
 
 def _write(path, c, rows, calib=None):
     """in.bin of the harnesses: header, z_scale, calib rows 0..2, the map, three rows of N floats, the head"""
-    calib = c["calib"] if calib is None else calib
-    C, H, W = c["feat"].shape[1:]
-    rows = np.ascontiguousarray(rows, dtype=np.float32)
-    with open(path, "wb") as f:
-        f.write(struct.pack("8i", C, H, W, rows.shape[1], 1, 1 if c["proj"] == "perspective" else 0, c["chans"][-1],
-                            c["last_op"]))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        f.write(struct.pack("12f", *calib[0, :3, :4].reshape(-1).tolist()))
-        f.write(c["feat"].contiguous().numpy().tobytes())
-        f.write(rows.tobytes())
-        for Wl, bl in zip(c["Ws"], c["bs"]):
-            f.write(Wl.numpy().tobytes())
-            f.write(bl.numpy().tobytes())
+    write_input(path, c["feat"], rows, c["calib"] if calib is None else calib, c["proj"], c["chans"][-1], c["last_op"], c["Ws"],
+                c["bs"])
 
 
 def _run(tmp_path, tag, exe, args, c, rows, env=None):

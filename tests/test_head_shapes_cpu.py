@@ -12,9 +12,9 @@ import torch
 
 from oracle import spec
 from grad_cases import query_grad_ref, within_bar
+from emu_harness import build, write_input
 from head_cases import (fp32_tile, head_cases, head_grad_cases, head_widths, load_head_case, load_head_grad_case,
                         shipped_widths)
-from test_map_shapes_cpu import _build, _write_input
 
 TC_PAIRS = [(net, op) for net in ("G", "C") for op in (spec.LAST_SIGMOID, spec.LAST_TANH, spec.LAST_NONE)]
 
@@ -25,15 +25,14 @@ def _widths(chans, no_residual=False):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("emu_heads"))
-    return dict(heads=_build(d, "emu_heads_fp32", "-O2"), tc=_build(d, "emu_query_tc"))
+    return dict(heads=build(tmp_path_factory, "emu_heads_fp32"), tc=build(tmp_path_factory, "emu_query_tc"))
 
 
 def _launch(exe, tmp_path, c, n, mode, sms=3, extra=(), widths=None, points=None):
     """-> (returncode, stdout, stderr, out array or None)"""
     fin, fout = str(tmp_path / "h.bin"), str(tmp_path / "h.f32")
     pts = c["points"][:, :, :n] if points is None else points
-    _write_input(fin, c["feat"], pts, c["calib"], c["proj"], c["chans"][-1], c["last_op"], c["Ws"], c["bs"])
+    write_input(fin, c["feat"], pts, c["calib"], c["proj"], c["chans"][-1], c["last_op"], c["Ws"], c["bs"])
     if os.path.exists(fout):
         os.remove(fout)
     r = subprocess.run([exe, fin, fout, widths or _widths(c["chans"]), str(sms), mode] + [str(a) for a in extra],
@@ -230,7 +229,7 @@ def test_tc_program_within_the_bar_at_the_default_limit(emu, tmp_path, net, last
     pts = spec.make_points(512, 3000 + seed)
     cal = spec.scene_calib(20, -60 + 17 * seed)
     fin, fout = str(tmp_path / "tc.bin"), str(tmp_path / "tc.f32")
-    _write_input(fin, feat, pts, cal, "orthogonal", chans[-1], last_op, Ws, bs)
+    write_input(fin, feat, pts, cal, "orthogonal", chans[-1], last_op, Ws, bs)
     r = subprocess.run([emu["tc"], fin, fout, "0", "2"], capture_output=True, text=True, timeout=3600)
     assert r.returncode == 0, r.stderr[-2000:]
     got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(chans[-1], 512)

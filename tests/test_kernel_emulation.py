@@ -3,36 +3,24 @@ are compiled UNMODIFIED against tests/emu/cuda_emu.h (one OS thread per CUDA thr
 warp shuffles) and compared with the oracle.  The build container has no GPU; this catches indexing / scan / table
 mistakes before a kernel is sent to an H100.  The `-m gpu` tests remain the parity tests of the real library."""
 import os
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
 from oracle import spec
+from emu_harness import build, needs_gxx, write_input
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
+pytestmark = needs_gxx
 # one OS thread per CUDA thread is slow: the heaviest cases only run with MONOPORT_B200_EMU_FULL=1 (they pass; the default
 # set keeps the CPU tier at a few minutes)
 FULL = os.environ.get("MONOPORT_B200_EMU_FULL", "0") == "1"
 full_only = pytest.mark.skipif(not FULL, reason="heavy emulation case: set MONOPORT_B200_EMU_FULL=1")
 
 
-def _build(tmp, name, extra=()):
-    exe = os.path.join(tmp, name)
-    cmd = ["g++", "-std=c++17", "-O1", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas"] + list(extra) + [
-        "-o", exe, os.path.join(EMU, name + ".cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
-
-
 @pytest.fixture(scope="module")
 def emu_mcubes(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu")), "emu_mcubes")
+    return build(tmp_path_factory, "emu_mcubes")
 
 
 def _run_mcubes(exe, vol, tmp_path, iso=0.5):
@@ -95,7 +83,7 @@ def test_mcubes_kernels_empty_volume(emu_mcubes, tmp_path, fill):
 # ---- the ordered scan itself (mp_scan.cuh): exclusive prefixes of two packed counters -----------------------------------
 @pytest.fixture(scope="module")
 def emu_scan(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu_scan")), "emu_scan")
+    return build(tmp_path_factory, "emu_scan")
 
 
 @pytest.mark.parametrize("vec", [0, 1])
@@ -127,7 +115,7 @@ def _check_scan(exe, tmp_path, n, vec):
 # ---- coarse-to-fine engine kernels (octree_kernels.cuh) against the restatement: volume AND evaluated node lists --------
 @pytest.fixture(scope="module")
 def emu_octree(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu_octree")), "emu_octree")
+    return build(tmp_path_factory, "emu_octree")
 
 
 def _run_octree(exe, tmp_path, mode, field, res, kpts=None, balance=0.5):
@@ -186,7 +174,7 @@ def test_octree_kernels_empty_field(emu_octree, tmp_path):
 # ---- visible-surface kernels (surface_kernels.cuh) against the goldens produced by the unmodified RTL/recon.py -------------
 @pytest.fixture(scope="module")
 def emu_surface(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu_surface")), "emu_surface")
+    return build(tmp_path_factory, "emu_surface")
 
 
 @pytest.mark.parametrize("golden", ["fv_sphere_33", "fv_two_blobs_65", "fv_ellipsoid_65"] + [
@@ -213,35 +201,17 @@ def test_surface_kernels_match_reference_golden(emu_surface, tmp_path, golden_di
 # ---- the flagship kernels: query_tc.cu (weight packing, launch logic, G0 GEMM kernel, fused wgmma sample+MLP program) on
 #      the functional model of the wgmma / mbarrier / bulk-copy layer (tests/emu/tc_ptx_emu.h), with asynchronous operations
 #      deferred adversarially, against the goldens of the UNMODIFIED reference ---------------------------------------------
-CUDA_INC = "/usr/local/cuda/include"
-
-
 @pytest.fixture(scope="module")
 def emu_query_tc(tmp_path_factory):
-    if not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")):
-        pytest.skip("CUDA headers not found")
-    # the kernels type-pun registers through reinterpret_cast like all CUDA code: no strict aliasing on the host build
-    return _build(str(tmp_path_factory.mktemp("emu_tc")), "emu_query_tc",
-                  ["-O3", "-march=native", "-fno-strict-aliasing", "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU])
+    return build(tmp_path_factory, "emu_query_tc")
 
 
 def _run_query_tc(exe, tmp_path, case, n, program, sms, extra_env=None):
-    import struct
     import torch
-    pts = case["points"][:, :, :n].contiguous()
-    cal, feat = case["calib"], case["feat"]
-    hw, res = feat.shape[2], case["expected"].shape[0]
+    res = case["expected"].shape[0]
     fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    with open(fin, "wb") as f:
-        f.write(struct.pack("8i", feat.shape[1], hw, hw, n, 1 if cal is not None else 0,
-                            1 if case["proj"] == "perspective" else 0, res, case["last_op"]))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        f.write(struct.pack("12f", *(cal[0, :3, :4].reshape(-1).tolist() if cal is not None else [0.0] * 12)))
-        f.write(feat.numpy().tobytes())
-        f.write(pts[0].numpy().tobytes())
-        for W, b in zip(case["Ws"], case["bs"]):
-            f.write(W.numpy().tobytes())
-            f.write(b.numpy().tobytes())
+    write_input(fin, case["feat"], case["points"][:, :, :n], case["calib"], case["proj"], res, case["last_op"], case["Ws"],
+                case["bs"])
     env = dict(os.environ)
     env.update(extra_env or {})
     r = subprocess.run([exe, fin, fout, str(program), str(sms)], capture_output=True, text=True, timeout=900, env=env)
@@ -301,18 +271,8 @@ def test_tcgen05_colour_head_matches_reference_golden(emu_query_tc, tmp_path, or
 
 
 def _write_tc_input(path, case, n):
-    import struct
-    cal, feat = case["calib"], case["feat"]
-    hw = feat.shape[2]
-    with open(path, "wb") as f:
-        f.write(struct.pack("8i", feat.shape[1], hw, hw, n, 1, 0, 1, case["last_op"]))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        f.write(struct.pack("12f", *cal[0, :3, :4].reshape(-1).tolist()))
-        f.write(feat.numpy().tobytes())
-        f.write(np.zeros(3 * n, np.float32).tobytes())
-        for W, b in zip(case["Ws"], case["bs"]):
-            f.write(W.numpy().tobytes())
-            f.write(b.numpy().tobytes())
+    """n points at the origin (the grid and node-list sources make their own)"""
+    write_input(path, case["feat"], np.zeros((3, n)), case["calib"], "orthogonal", 1, case["last_op"], case["Ws"], case["bs"])
 
 
 @pytest.mark.parametrize("program", [3, 103])
@@ -380,7 +340,6 @@ def test_tcgen05_list_sharding_is_bit_identical(emu_query_tc, tmp_path, kind, wo
 def test_tcgen05_colour_head_fused_surface_rendering(emu_query_tc, tmp_path):
     """mp_colorize_surface: visible-surface vertices (X, Y, R - Z) -> world (mat_color) -> netC -> pred*0.5+0.5 -> canvas, one
     launch, against the restatement of RTL/main.py:212-249 driven by the oracle's query (32 x 32 colour map)."""
-    import struct
     import torch
     Ws, bs = spec.make_weights(spec.C_CHANNELS, 77)
     feat = spec.make_feat(512, 32, 32, 78)
@@ -391,15 +350,7 @@ def test_tcgen05_colour_head_fused_surface_rendering(emu_query_tc, tmp_path):
     X, Y = cols // R, cols % R
     Z = torch.rand(n, generator=g) * (R - 1)
     fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    with open(fin, "wb") as f:
-        f.write(struct.pack("8i", 512, 32, 32, n, 1, 0, 3, spec.LAST_TANH))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        f.write(struct.pack("12f", *cal[0, :3, :4].reshape(-1).tolist()))
-        f.write(feat.numpy().tobytes())
-        f.write(torch.stack([X.float(), Y.float(), Z]).numpy().astype(np.float32).tobytes())
-        for W, b in zip(Ws, bs):
-            f.write(W.numpy().tobytes())
-            f.write(b.numpy().tobytes())
+    write_input(fin, feat, torch.stack([X.float(), Y.float(), Z]), cal, "orthogonal", 3, spec.LAST_TANH, Ws, bs)
     r = subprocess.run([emu_query_tc, fin, fout, "0", "2", "surface", str(R)], capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stderr[-2000:]
     got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(R, R, 3)
@@ -417,32 +368,18 @@ def test_tcgen05_colour_head_fused_surface_rendering(emu_query_tc, tmp_path):
 # ---- the exact CUDA-core kernel (query_fp32.cu): default path of the colour head, fallback for every other head shape ----
 @pytest.fixture(scope="module")
 def emu_query_fp32(tmp_path_factory):
-    if not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")):
-        pytest.skip("CUDA headers not found")
-    return _build(str(tmp_path_factory.mktemp("emu_fp32")), "emu_query_fp32",
-                  ["-O2", "-fno-strict-aliasing", "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU])
+    return build(tmp_path_factory, "emu_query_fp32")
 
 
 @pytest.mark.parametrize("name,n", [("c_rot33", 200), ("c_identity", 100), ("g_persp", 150), ("g_nocalib", 77), ("g_identity", 130)])
 def test_fp32_kernel_matches_reference_golden(emu_query_fp32, tmp_path, name, n):
-    import struct
     import torch
     from helpers import load_query_case
     case = load_query_case(name)
-    pts = case["points"][:, :, :n].contiguous()
-    cal, feat = case["calib"], case["feat"]
     res = case["expected"].shape[0]
     fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    with open(fin, "wb") as f:
-        f.write(struct.pack("8i", feat.shape[1], feat.shape[2], feat.shape[3], n, 1 if cal is not None else 0,
-                            1 if case["proj"] == "perspective" else 0, res, case["last_op"]))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        f.write(struct.pack("12f", *(cal[0, :3, :4].reshape(-1).tolist() if cal is not None else [0.0] * 12)))
-        f.write(feat.numpy().tobytes())
-        f.write(pts[0].numpy().tobytes())
-        for W, b in zip(case["Ws"], case["bs"]):
-            f.write(W.numpy().tobytes())
-            f.write(b.numpy().tobytes())
+    write_input(fin, case["feat"], case["points"][:, :, :n], case["calib"], case["proj"], res, case["last_op"], case["Ws"],
+                case["bs"])
     r = subprocess.run([emu_query_fp32, fin, fout], capture_output=True, text=True, timeout=900)
     assert r.returncode == 0, r.stderr[-2000:]
     got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(res, n)

@@ -3,9 +3,7 @@ loop_control_kernel included, run unmodified on the CPU model (tests/emu/emu_oct
 deciding whether another pass runs, as the WHILE node's condition does on the GPU.  Volume, node lists and per-level counts
 must equal the restatement's, and the passes per level its query calls per level.  A cap below the walk's length stops the
 level and sets the truncated flag.  Also: loop_control_kernel compiles for sm_90a without a stack frame or spills."""
-import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -13,10 +11,8 @@ import pytest
 import torch
 
 from oracle import spec
+from emu_harness import build, ptxas_report
 from helpers import lookup_query
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
 
 
 def rod_field(R):
@@ -32,14 +28,7 @@ def rod_field(R):
 
 @pytest.fixture(scope="module")
 def emu_octree(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    exe = str(tmp_path_factory.mktemp("emu_loop") / "emu_octree_loop")
-    cmd = ["g++", "-std=c++17", "-O1", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(EMU, "emu_octree_loop.cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
+    return build(tmp_path_factory, "emu_octree_loop")
 
 
 def _run_loop(exe, tmp_path, field, res, cap=0):
@@ -101,18 +90,9 @@ def test_device_loop_stops_at_its_cap(emu_octree, tmp_path):
     assert counts[-1] < int(stats[-1]["idx"].numel())
 
 
-def test_loop_control_kernel_has_no_stack_frame(tmp_path):
-    from monoport_b200 import build as lib_build
-    try:
-        nvcc = lib_build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    cmd = [nvcc] + lib_build.NVCC_FLAGS + ["-c", os.path.join(lib_build.CSRC, "octree.cu"), "-o", str(tmp_path / "octree.o")]
-    p = subprocess.run(cmd, capture_output=True, text=True)
-    assert p.returncode == 0, p.stdout + p.stderr
-    log = (p.stdout + p.stderr).splitlines()
-    at = [i for i, line in enumerate(log) if re.search(r"Compiling entry function '[^']*loop_control_kernel", line)]
+def test_loop_control_kernel_has_no_stack_frame():
+    at = [lines for name, lines in ptxas_report("octree.cu")[0] if "loop_control_kernel" in name]
     assert len(at) == 1, "loop_control_kernel not compiled"
-    stats = " ".join(log[at[0] + 1:at[0] + 4])
+    stats = " ".join(at[0])
     m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", stats)
     assert m and m.groups() == ("0", "0", "0"), stats

@@ -4,8 +4,6 @@ or that sit at or above the tensor-core program's 65536 texels.  The restatement
 them, and the query kernels -- compiled unmodified on the CPU model of tests/emu -- against the reference and the restatement:
 the tensor-core program with its per-texel products, the exact fp32 kernel, the point gradient and the colour surface render."""
 import os
-import shutil
-import struct
 import subprocess
 
 import numpy as np
@@ -13,13 +11,10 @@ import pytest
 import torch
 
 from oracle import spec
+from emu_harness import build, write_input
 from grad_cases import query_grad_ref, within_bar
 from shape_cases import (TC_TEXEL_LIMIT, load_shape_batch_case, load_shape_case, load_shape_grad_case, shape_batch_cases,
                          shape_cases, shape_grad_cases, within_fp32_bar)
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-CUDA_INC = "/usr/local/cuda/include"
 # one OS thread per CUDA thread is slow: the heaviest cases only run with MONOPORT_B200_EMU_FULL=1
 FULL = os.environ.get("MONOPORT_B200_EMU_FULL", "0") == "1"
 full_only = pytest.mark.skipif(not FULL, reason="heavy emulation case: set MONOPORT_B200_EMU_FULL=1")
@@ -91,48 +86,16 @@ def test_restatement_per_image_matches_batched_shape_golden(name):
 
 
 # ---- the kernels on the CPU model --------------------------------------------------------------------------------------------
-def _build(tmp, name, opt="-O3"):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    if not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")):
-        pytest.skip("CUDA headers not found")
-    exe = os.path.join(tmp, name)
-    cmd = ["g++", "-std=c++17", opt, "-march=native", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas",
-           "-fno-strict-aliasing", "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU, "-o", exe, os.path.join(EMU, name + ".cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("emu_shapes"))
-    return dict(tc=_build(d, "emu_query_tc"), fp32=_build(d, "emu_query_fp32", "-O2"), grad=_build(d, "emu_query_grad"))
-
-
-def _write_input(path, feat, points, calib, proj, res, last_op, Ws, bs, batched=False):
-    """in.bin of the emulation harnesses: feat [B,C,H,W], points [B,3,N], calib [B,4,4] | None (B = 1 unless batched)"""
-    B, C, H, W = feat.shape
-    n = points.shape[2]
-    with open(path, "wb") as f:
-        f.write(struct.pack("8i", C, H, W, n, 1 if calib is not None else 0, 1 if proj == "perspective" else 0, res, last_op))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        head = calib[0, :3, :4].reshape(-1).tolist() if (calib is not None and not batched) else [0.0] * 12
-        f.write(struct.pack("12f", *head))
-        f.write(feat.contiguous().numpy().tobytes())
-        f.write(points.contiguous().numpy().tobytes())
-        if batched and calib is not None:
-            f.write(calib[:, :3, :4].contiguous().numpy().astype(np.float32).tobytes())
-        for Wl, bl in zip(Ws, bs):
-            f.write(Wl.numpy().tobytes())
-            f.write(bl.numpy().tobytes())
+    return {k: build(tmp_path_factory, "emu_query_" + k) for k in ("tc", "fp32", "grad")}
 
 
 def _run(exe, tmp_path, c, n, args, batched=False, env=None, tag="x"):
     """-> [B,Res,n] (batched) or [Res,n] from emu_query_tc / emu_query_fp32"""
     res = c["chans"][-1]
     fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    _write_input(fin, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], res, c["last_op"], c["Ws"], c["bs"], batched)
+    write_input(fin, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], res, c["last_op"], c["Ws"], c["bs"], batched)
     r = subprocess.run([exe, fin, fout] + [str(a) for a in args], capture_output=True, text=True, timeout=3600,
                        env=dict(os.environ, **(env or {})))
     assert r.returncode == 0 and "DEADLOCK" not in r.stderr, r.stderr[-2000:]
@@ -228,7 +191,7 @@ def test_grad_kernel_matches_reference_shape_golden(emu, tmp_path, name):
     c = load_shape_grad_case(name)
     n = 136
     fin, fout = str(tmp_path / "in_g.bin"), str(tmp_path / "out_g.f32")
-    _write_input(fin, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], 1, c["last_op"], c["Ws"], c["bs"])
+    write_input(fin, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], 1, c["last_op"], c["Ws"], c["bs"])
     r = subprocess.run([emu["grad"], fin, fout, "3"], capture_output=True, text=True, timeout=3600)
     assert r.returncode == 0, r.stderr[-2000:]
     out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
@@ -245,8 +208,7 @@ R_CANVAS = 65
 
 @pytest.fixture(scope="module")
 def emu_surface(tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("emu_shapes_cs"))
-    return dict(tc=_build(d, "emu_colour_surface_tc"), fp32=_build(d, "emu_colour_surface_fp32", "-O2"))
+    return {k: build(tmp_path_factory, "emu_colour_surface_" + k) for k in ("tc", "fp32")}
 
 
 @pytest.mark.parametrize("program", ["tc", "fp32"])
@@ -261,7 +223,7 @@ def test_colour_surface_render_on_a_non_square_map(emu_surface, tmp_path, progra
     Z = torch.rand(n, generator=g) * (R_CANVAS - 1)
     rows = torch.stack([X.float(), Y.float(), Z])[None]
     fin, fout = str(tmp_path / "s.bin"), str(tmp_path / "s.f32")
-    _write_input(fin, c["feat"], rows, c["calib"], c["proj"], 3, c["last_op"], c["Ws"], c["bs"])
+    write_input(fin, c["feat"], rows, c["calib"], c["proj"], 3, c["last_op"], c["Ws"], c["bs"])
     args = [fin, fout, "2", str(R_CANVAS), str(n)] if program == "tc" else [fin, fout, "2", "surface", str(R_CANVAS), str(n)]
     args += ["-1", "-1", "-1", "1", "1", "1"]                 # the render box [b_min, b_max]
     r = subprocess.run([emu_surface[program]] + args, capture_output=True, text=True, timeout=3600)

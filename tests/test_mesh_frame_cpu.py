@@ -4,9 +4,7 @@ every CTA walks several rounds of the active list.  The mesh must be the eager e
 (spec.marching_cubes_ref) bit for bit, in index space and in reconstruction()'s world space; the capacities must cut the
 writes exactly while the true totals are still reported; two runs on one workspace must each equal a fresh run.  Also:
 mesh_emit_async_kernel compiles for sm_90a without a stack frame or spills."""
-import os
 import re
-import shutil
 import subprocess
 
 import numpy as np
@@ -14,26 +12,14 @@ import pytest
 import torch
 
 from oracle import spec
+from emu_harness import build, needs_gxx, ptxas_report
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-
-pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="g++ not available")
-
-
-def _build(tmp, name):
-    exe = os.path.join(tmp, name)
-    cmd = ["g++", "-std=c++17", "-O1", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas", "-o", exe,
-           os.path.join(EMU, name + ".cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
+pytestmark = needs_gxx
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    tmp = str(tmp_path_factory.mktemp("emu_mesh"))
-    return _build(tmp, "emu_mcubes_async"), _build(tmp, "emu_mcubes")
+    return build(tmp_path_factory, "emu_mcubes_async"), build(tmp_path_factory, "emu_mcubes")
 
 
 def _run_async(exe, vols, tmp_path, v_cap=None, f_cap=None, blocks=2, world=None, iso=0.5):
@@ -157,18 +143,9 @@ def test_replay_on_one_workspace(emu, tmp_path):
     assert runs[0][2] > runs[1][2] > 0 and runs[2][2] == 0
 
 
-def test_async_emission_kernel_has_no_stack_frame(tmp_path):
-    from monoport_b200 import build as lib_build
-    try:
-        nvcc = lib_build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    cmd = [nvcc] + lib_build.NVCC_FLAGS + ["-c", os.path.join(lib_build.CSRC, "mcubes.cu"), "-o", str(tmp_path / "mcubes.o")]
-    p = subprocess.run(cmd, capture_output=True, text=True)
-    assert p.returncode == 0, p.stdout + p.stderr
-    log = (p.stdout + p.stderr).splitlines()
-    at = [i for i, line in enumerate(log) if re.search(r"Compiling entry function '[^']*mesh_emit_async_kernel", line)]
+def test_async_emission_kernel_has_no_stack_frame():
+    at = [lines for name, lines in ptxas_report("mcubes.cu")[0] if "mesh_emit_async_kernel" in name]
     assert len(at) == 1, "mesh_emit_async_kernel not compiled"
-    stats = " ".join(log[at[0] + 1:at[0] + 4])
+    stats = " ".join(at[0])
     m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", stats)
     assert m and m.groups() == ("0", "0", "0"), stats

@@ -2,8 +2,6 @@
 the reference, and both query kernels -- compiled unmodified on the CPU model of tests/emu -- against those goldens and
 against B = 1 runs of each image, bit for bit, including the per-image range guard of the tensor-core program."""
 import os
-import shutil
-import struct
 import subprocess
 
 import numpy as np
@@ -12,10 +10,7 @@ import torch
 
 from oracle import spec
 from batch_cases import batch_cases, load_batch_case
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-CUDA_INC = "/usr/local/cuda/include"
+from emu_harness import build, write_input
 
 
 @pytest.mark.parametrize("name", batch_cases())
@@ -36,46 +31,14 @@ def test_batched_goldens_cover_the_issue_cases():
 
 
 # ---- the kernels on the CPU model ------------------------------------------------------------------------------------------
-def _build(tmp, name):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    if not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")):
-        pytest.skip("CUDA headers not found")
-    exe = os.path.join(tmp, name)
-    cmd = ["g++", "-std=c++17", "-O3", "-march=native", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas",
-           "-fno-strict-aliasing", "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU, "-o", exe, os.path.join(EMU, name + ".cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
-
-
 @pytest.fixture(scope="module")
 def emu_tc(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu_batch_tc")), "emu_query_tc")
+    return build(tmp_path_factory, "emu_query_tc")
 
 
 @pytest.fixture(scope="module")
 def emu_fp32(tmp_path_factory):
-    return _build(str(tmp_path_factory.mktemp("emu_batch_fp32")), "emu_query_fp32")
-
-
-def _write_input(path, feat, points, calib, proj, res, last_op, Ws, bs, batched):
-    """in.bin of the emulation harnesses: feat [B,C,H,W], points [B,3,N], calib [B,4,4] | None (batched: B maps, point sets
-    and calibs; otherwise B must be 1 and the calib goes in the header)."""
-    B, C, H, W = feat.shape
-    n = points.shape[2]
-    with open(path, "wb") as f:
-        f.write(struct.pack("8i", C, H, W, n, 1 if calib is not None else 0, 1 if proj == "perspective" else 0, res, last_op))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        head = calib[0, :3, :4].reshape(-1).tolist() if (calib is not None and not batched) else [0.0] * 12
-        f.write(struct.pack("12f", *head))
-        f.write(feat.contiguous().numpy().tobytes())
-        f.write(points.contiguous().numpy().tobytes())
-        if batched and calib is not None:
-            f.write(calib[:, :3, :4].contiguous().numpy().astype(np.float32).tobytes())
-        for Wl, bl in zip(Ws, bs):
-            f.write(Wl.numpy().tobytes())
-            f.write(bl.numpy().tobytes())
+    return build(tmp_path_factory, "emu_query_fp32")
 
 
 def _run(exe, tmp_path, case, n, args, batched, env=None, feat=None, tag="x"):
@@ -83,8 +46,8 @@ def _run(exe, tmp_path, case, n, args, batched, env=None, feat=None, tag="x"):
     feat = case["feat"] if feat is None else feat
     res = case["expected"].shape[1]
     fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    _write_input(fin, feat, case["points"][:, :, :n], case["calib"], case["proj"], res, case["last_op"], case["Ws"], case["bs"],
-                 batched)
+    write_input(fin, feat, case["points"][:, :, :n], case["calib"], case["proj"], res, case["last_op"], case["Ws"], case["bs"],
+                batched)
     e = dict(os.environ)
     e.update(env or {})
     r = subprocess.run([exe, fin, fout] + [str(a) for a in args], capture_output=True, text=True, timeout=1800, env=e)

@@ -2,10 +2,7 @@
 autograd goldens, and the gradient kernel -- compiled unmodified on the CPU model of tests/emu -- against those goldens, against
 the fp32 query kernel's values bit for bit, across simulated SM counts, and outside the image.  Also the ptxas report of the
 kernel's sm_90a instantiations."""
-import os
 import re
-import shutil
-import struct
 import subprocess
 
 import numpy as np
@@ -13,11 +10,8 @@ import pytest
 import torch
 
 from oracle import spec
+from emu_harness import build, ptxas_report, write_input
 from grad_cases import grad_cases, load_grad_case, query_grad_ref, within_bar
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-CUDA_INC = "/usr/local/cuda/include"
 
 
 def test_grad_goldens_cover_the_cases():
@@ -39,41 +33,14 @@ def test_restatement_matches_reference_grad_golden(name):
 
 
 # ---- the kernel on the CPU model -------------------------------------------------------------------------------------------
-def _build(tmp, name):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    if not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")):
-        pytest.skip("CUDA headers not found")
-    exe = os.path.join(tmp, name)
-    cmd = ["g++", "-std=c++17", "-O3", "-march=native", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas",
-           "-fno-strict-aliasing", "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU, "-o", exe, os.path.join(EMU, name + ".cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
     """(gradient harness, fp32 query harness)"""
-    d = str(tmp_path_factory.mktemp("emu_grad"))
-    return _build(d, "emu_query_grad"), _build(d, "emu_query_fp32")
+    return build(tmp_path_factory, "emu_query_grad"), build(tmp_path_factory, "emu_query_fp32")
 
 
 def _write_input(path, c, n):
-    """in.bin of the emulation harnesses (the layout of emu_query_fp32)"""
-    C, H, W = c["feat"].shape[1:]
-    res = c["chans"][-1]
-    with open(path, "wb") as f:
-        f.write(struct.pack("8i", C, H, W, n, 1 if c["calib"] is not None else 0, 1 if c["proj"] == "perspective" else 0,
-                            res, c["last_op"]))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        head = c["calib"][0, :3, :4].reshape(-1).tolist() if c["calib"] is not None else [0.0] * 12
-        f.write(struct.pack("12f", *head))
-        f.write(c["feat"].contiguous().numpy().tobytes())
-        f.write(c["points"][0, :, :n].contiguous().numpy().tobytes())
-        for Wl, bl in zip(c["Ws"], c["bs"]):
-            f.write(Wl.numpy().tobytes())
-            f.write(bl.numpy().tobytes())
+    write_input(path, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], c["chans"][-1], c["last_op"], c["Ws"], c["bs"])
 
 
 def _run_grad(emu, tmp_path, c, n, sms=3, tag="g"):
@@ -140,24 +107,8 @@ def test_kernel_gradient_is_exactly_zero_outside_the_image(emu, tmp_path):
 
 
 # ---- ptxas report ----------------------------------------------------------------------------------------------------------
-def test_grad_kernel_has_no_spill_and_no_stack_frame(tmp_path):
-    from monoport_b200 import build as lib_build
-    try:
-        nvcc = lib_build._nvcc()
-    except RuntimeError:
-        pytest.skip("nvcc not available")
-    cmd = [nvcc] + lib_build.NVCC_FLAGS + ["-c", os.path.join(lib_build.CSRC, "query_fp32.cu"), "-o", str(tmp_path / "q.o")]
-    p = subprocess.run(cmd, capture_output=True, text=True)
-    assert p.returncode == 0, p.stdout + p.stderr
-    found, current = {}, None
-    for line in (p.stdout + p.stderr).splitlines():
-        m = re.search(r"Compiling entry function '([^']+)'", line)
-        if m:
-            current = m.group(1) if "query_grad_kernel" in m.group(1) else None
-            if current:
-                found[current] = ""
-        elif current and ("spill" in line or "stack" in line):
-            found[current] += line
+def test_grad_kernel_has_no_spill_and_no_stack_frame():
+    found = {name: " ".join(lines) for name, lines in ptxas_report("query_fp32.cu")[0] if "query_grad_kernel" in name}
     assert len(found) == 3, list(found)               # P = 32, 16, 8
     for name, stats in found.items():
         m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", stats)

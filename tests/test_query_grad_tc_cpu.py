@@ -4,8 +4,6 @@ query program bit for bit, across simulated SM counts and bulk-copy completion o
 guard and with a device-side point count.  (Its ptxas report is checked with the rest of query_tc.cu in
 test_ptxas_report.py.)"""
 import os
-import shutil
-import struct
 import subprocess
 
 import numpy as np
@@ -13,47 +11,17 @@ import pytest
 import torch
 
 from oracle import spec
-from grad_cases import load_grad_case
-from shape_cases import load_shape_grad_case
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-EMU = os.path.join(HERE, "emu")
-CUDA_INC = "/usr/local/cuda/include"
-
-
-def _build(tmp, name):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    if not os.path.exists(os.path.join(CUDA_INC, "cuda_fp16.h")):
-        pytest.skip("CUDA headers not found")
-    exe = os.path.join(tmp, name)
-    cmd = ["g++", "-std=c++17", "-O3", "-march=native", "-pthread", "-ffp-contract=off", "-Wno-unknown-pragmas",
-           "-fno-strict-aliasing", "-DMP_CUDA_EMU=1", "-I" + CUDA_INC, "-I" + EMU, "-o", exe, os.path.join(EMU, name + ".cpp")]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr[-3000:]
-    return exe
+from emu_harness import build, write_input
+from grad_cases import GOLDEN_CASES, load_golden, load_grad_case, tc_bar
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("emu_jvp"))
-    return dict(jvp=_build(d, "emu_query_jvp_tc"), tc=_build(d, "emu_query_tc"))
+    return dict(jvp=build(tmp_path_factory, "emu_query_jvp_tc"), tc=build(tmp_path_factory, "emu_query_tc"))
 
 
 def _write_input(path, c, n):
-    """in.bin of emu_query_tc / emu_query_jvp_tc (one map)"""
-    C, H, W = c["feat"].shape[1:]
-    with open(path, "wb") as f:
-        f.write(struct.pack("8i", C, H, W, n, 1 if c["calib"] is not None else 0, 1 if c["proj"] == "perspective" else 0,
-                            c["chans"][-1], c["last_op"]))
-        f.write(struct.pack("f", spec.Z_SCALE))
-        head = c["calib"][0, :3, :4].reshape(-1).tolist() if c["calib"] is not None else [0.0] * 12
-        f.write(struct.pack("12f", *head))
-        f.write(c["feat"].contiguous().numpy().tobytes())
-        f.write(c["points"][0, :, :n].contiguous().numpy().tobytes())
-        for Wl, bl in zip(c["Ws"], c["bs"]):
-            f.write(Wl.numpy().tobytes())
-            f.write(bl.numpy().tobytes())
+    write_input(path, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], c["chans"][-1], c["last_op"], c["Ws"], c["bs"])
 
 
 def _run_jvp(emu, tmp_path, c, n, sms=3, env=None, tag="j"):
@@ -81,23 +49,6 @@ def _run_tc(emu, tmp_path, c, n, env=None):
                        timeout=3600, env=dict(os.environ, **(env or {})))
     assert r.returncode == 0, r.stderr[-2000:]
     return torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(c["chans"][-1], n)
-
-
-# Goldens on which the fp16 restatement (tc_jvp_ref, all points of the golden) does not pass the bar below with a 2x margin
-# get its own distance from grad64 + 10 % as their bar: shape_grad_g_wide's largest component is 2.85e-2 max|g| away
-# (a leaky-ReLU kink taken on the other side in fp16).  Every other golden keeps the bar (DESIGN.md, section F1 triple-prime).
-MAX_BAR = {"g_wide": 3.1e-2}
-
-
-def tc_bar(got, g64, name=None):
-    """The error bar of the tensor-core gradient against the reference's fp64 gradient: median <= 5e-5 max|g|, 99 % of the
-    components <= 5e-3 max|g|, every component <= 5e-2 max|g| (MAX_BAR for the goldens named there).  (The tail comes
-    from fp16 taking the other side of a leaky-ReLU kink.)  -> (ok, message)"""
-    scale = g64.abs().max().item()
-    err = (got.double() - g64.double()).abs().flatten() / scale
-    med, p99, worst = err.median().item(), torch.quantile(err, 0.99).item(), err.max().item()
-    return (med <= 5e-5 and p99 <= 5e-3 and worst <= MAX_BAR.get(name, 5e-2),
-            "|err|/max|g|: median %.2e, p99 %.2e, max %.2e" % (med, p99, worst))
 
 
 # ---- a torch restatement of the kernel's fp16 roundings ------------------------------------------------------------------
@@ -194,18 +145,9 @@ def tc_jvp_ref(feat, points, calib, Ws, bs, last_op, projection="orthogonal", z_
     return torch.where(in_img[None], gp, 0.0)
 
 
-# the first 8 points of every case are border_points(): on the image border / corners and far outside
-GOLDEN_CASES = [("grad", "g_rot", 64), ("grad", "g_persp", 48), ("grad", "g_nocalib", 48), ("grad", "g_bigfeat", 48),
-                ("grad", "c_rot", 32), ("shape", "g_wide", 72), ("shape", "g_tiny", 72)]
-
-
-def _load(kind, name):
-    return load_grad_case(name) if kind == "grad" else load_shape_grad_case(name)
-
-
 @pytest.mark.parametrize("kind,name,n", GOLDEN_CASES)
 def test_jvp_kernel_matches_reference_grad_golden(emu, tmp_path, kind, name, n):
-    c = _load(kind, name)
+    c = load_golden(kind, name)
     val, dp = _run_jvp(emu, tmp_path, c, n)
     assert (val - c["value"][:, :n]).abs().max().item() <= 1e-4
     ok, msg = tc_bar(dp, c["grad64"][:, :n], name)
@@ -217,7 +159,7 @@ def test_jvp_kernel_matches_reference_grad_golden(emu, tmp_path, kind, name, n):
 def test_jvp_kernel_is_closer_to_its_fp16_restatement_than_the_restatement_to_fp64(emu, tmp_path, kind, name, n):
     """The kernel against tc_jvp_ref: the median and the 99th percentile of |kernel - restatement| are at most half those of
     |restatement - grad64|.  The restatement itself passes every golden's bar."""
-    c = _load(kind, name)
+    c = load_golden(kind, name)
     _, dp = _run_jvp(emu, tmp_path, c, n)
     ref = tc_jvp_ref(c["feat"], c["points"][:, :, :n], c["calib"], c["Ws"], c["bs"], c["last_op"], c["proj"],
                      grad_output=c["grad_output"][:, :n] if c["grad_output"] is not None else None)

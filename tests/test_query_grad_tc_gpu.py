@@ -11,9 +11,8 @@ import torch
 
 from oracle import spec
 from helpers import build_net
-from grad_cases import load_grad_case
+from grad_cases import GOLDEN_CASES, load_golden, load_grad_case, tc_bar
 from shape_cases import load_shape_case, load_shape_grad_case
-from test_query_grad_tc_cpu import GOLDEN_CASES, _load, tc_bar
 
 pytestmark = pytest.mark.gpu
 
@@ -29,7 +28,7 @@ def _inputs(c):
 
 @pytest.mark.parametrize("kind,name,n", GOLDEN_CASES)
 def test_tc_gradient_matches_reference_grad_golden(kind, name, n):
-    c = _load(kind, name)
+    c = load_golden(kind, name)
     net, feats, pts, cal, gout = _inputs(c)
     for precision in ("tc", "auto"):
         val, dp = net.query_gradient(feats, pts, calibs=cal, grad_output=gout, precision=precision)
