@@ -147,6 +147,30 @@ int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const float* point
                               int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
                               int64_t ld_grad, float* out_dev, int64_t ld_out, float* dpoints_dev, int64_t ld_dpoints,
                               const int32_t* count_dev, int mode, void* stream);
+/* The vector-Jacobian product of MonoPortNet.query in MP_MODE_FP32, for training: with S = sum(grad_out * query(feats,
+ * points, calibs)) over B images (the exact values, mp_query_points / mp_query_points_batch), every requested one of
+ *   dfeat_dev      [B][C][H][W] = dS / d features (NCHW, like the map mp_feat_upload takes),
+ *   dpoints_dev    [B][3][n]    = dS / d points (what mp_query_points_grad gives for B = 1, bit for bit),
+ *   dweights_dev   n_layers device pointers, [Cout_l][Cin_l] = dS / d filters.l.weight (mp_mlp_create's layout),
+ *   dbiases_dev    n_layers device pointers, [Cout_l]       = dS / d filters.l.bias
+ * (NULL, or a NULL entry: not computed, and costs nothing).  Exact fp32 on CUDA cores, every head the exact kernel takes; the
+ * feature handle may hold one map or B (mp_feat_create_batch).  Points as for mp_query_points_batch; calibs_dev: [B][12] fp32
+ * in device memory (rows 0..2 of [R|t]) or NULL for calibs=None.  grad_out_dev: [B][Res][n] fp32 (NULL: all ones).  Points
+ * outside the image contribute nothing (in_img multiplies the output, MonoPortNet.py:89).  Outputs are overwritten.
+ * The weight gradients are contracted chunk by chunk from rows the kernel saves in scratch_dev; the feature gradient is
+ * gathered in it before its layout step.  scratch_bytes: at least mp_query_points_vjp_scratch_bytes(...) for the same
+ * requests; a larger scratch holds larger chunks.  The weight, bias and point gradients are deterministic for one scratch
+ * size; the feature gradient is accumulated with atomics (like grid_sample's backward) and is not.  No range guard, no
+ * tensor-core variant.  Enqueue-only: nothing is read back to the host. */
+int mp_query_points_vjp(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n, int64_t batch_stride,
+                        int64_t row_stride, int64_t point_stride, const float* calibs_dev, int projection, float z_scale,
+                        const float* grad_out_dev, float* dfeat_dev, float* dpoints_dev, float* const* dweights_dev,
+                        float* const* dbiases_dev, void* scratch_dev, int64_t scratch_bytes, void* stream);
+/* Scratch bytes of mp_query_points_vjp for B images of n points, the weight gradients contracted in chunks of chunk_points
+ * points (<= 0: all points in one chunk; about 16 KB per point for the geometry head), want_dfeat / want_dweights: whether
+ * the feature / weight gradients are requested (neither: 0 bytes).  Negative: an MP_E_* code. */
+int64_t mp_query_points_vjp_scratch_bytes(mp_mlp_t* mlp, mp_feat_t* feat, int B, int64_t n, int64_t chunk_points, int want_dfeat,
+                                          int want_dweights);
 /* mp_query_points with an optional point count on the device (count_dev: one int32, or NULL): n is then the capacity and
  * the points at or beyond min(*count_dev, n) are neither read nor written.  Enqueue-only like mp_query_points; the same
  * modes, range guard and kernels.  Single-map handles only. */

@@ -51,7 +51,10 @@ SIGNATURES = {
                                      c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
     "mp_query_points_grad_mode": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
                                           c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int, c_void_p]),
-    "mp_query_points_host": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, P(c_float), c_int, c_float,
+    "mp_query_points_vjp": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int,
+                                    c_float, c_void_p, c_void_p, c_void_p, P(c_void_p), P(c_void_p), c_void_p, c_int64, c_void_p]),
+    "mp_query_points_vjp_scratch_bytes": (c_int64, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_int]),
+    "mp_query_points_host":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, P(c_float), c_int, c_float,
                                      c_void_p, c_int, c_void_p]),
     "mp_query_grid": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, P(c_float), P(c_float), P(c_float), c_int,
                               c_float, c_void_p, c_int, c_void_p]),

@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libmonoport_b200.so")
-SOURCES = ["mp_api.cu", "query_fp32.cu", "query_tc.cu", "octree.cu", "mcubes.cu", "surface.cu"]
+SOURCES = ["mp_api.cu", "query_fp32.cu", "query_tc.cu", "query_vjp.cu", "octree.cu", "mcubes.cu", "surface.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-v",

@@ -404,6 +404,48 @@ extern "C" int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const f
 }
 
 // ---------------------------------------------------------------------------------------------
+// the vector-Jacobian product of the exact query, for training (query_vjp.cu)
+// ---------------------------------------------------------------------------------------------
+extern "C" int64_t mp_query_points_vjp_scratch_bytes(mp_mlp_t* mlp, mp_feat_t* feat, int B, int64_t n, int64_t chunk_points,
+                                                     int want_dfeat, int want_dweights) {
+  MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE(B == feat->B && n >= 0, "bad batch %d (the handle holds %d maps) or n=%lld", B, feat->B, (long long)n);
+  return mp_vjp_scratch_bytes(mlp, feat, B, n, chunk_points, want_dfeat != 0, want_dweights != 0);
+}
+
+extern "C" int mp_query_points_vjp(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
+                                   int64_t batch_stride, int64_t row_stride, int64_t point_stride, const float* calibs_dev,
+                                   int projection, float z_scale, const float* grad_out_dev, float* dfeat_dev, float* dpoints_dev,
+                                   float* const* dweights_dev, float* const* dbiases_dev, void* scratch_dev,
+                                   int64_t scratch_bytes, void* stream) {
+  MpRange nvtx("monoport_b200: F1'''' query VJP");
+  MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE(B == feat->B, "batch size %d does not match the feature handle's %d maps", B, feat->B);
+  MP_REQUIRE(n >= 0 && row_stride >= 1 && point_stride >= 1 && (B == 1 || batch_stride >= 1) && scratch_bytes >= 0,
+             "bad sizes n=%lld strides=%lld,%lld,%lld scratch=%lld", (long long)n, (long long)batch_stride, (long long)row_stride,
+             (long long)point_stride, (long long)scratch_bytes);
+  // (the kernel finds a tile's image with a 32-bit division: at most 2^31 tiles of 8 points per launch)
+  MP_REQUIRE((long long)B * ((n + 7) / 8) < (1ll << 31), "batch too large: %d x %lld points", B, (long long)n);
+  MP_REQUIRE(n == 0 || points_dev, "NULL points");
+  MpPointSrc src;
+  memset(&src, 0, sizeof(src));
+  src.kind = MP_SRC_ROWS;
+  src.px = points_dev; src.py = points_dev + row_stride; src.pz = points_dev + 2 * row_stride;
+  src.pstride = point_stride;
+  src.n = n;
+  MpCalib cal;
+  mp_fill_calib(cal, nullptr, projection, z_scale);
+  cal.has = calibs_dev != nullptr;
+  cal.perspective = projection == MP_PROJ_PERSPECTIVE && cal.has;
+  MpBatch bt;
+  bt.B = B;
+  bt.pt_stride = batch_stride;
+  bt.calibs = calibs_dev;
+  return mp_launch_query_vjp(mlp, feat, src, cal, bt, grad_out_dev, dfeat_dev, dpoints_dev, dweights_dev, dbiases_dev, scratch_dev,
+                             scratch_bytes, (cudaStream_t)stream);
+}
+
+// ---------------------------------------------------------------------------------------------
 // analytic normals of the visible surface, enqueue-only (mp_surface_normals_async)
 // ---------------------------------------------------------------------------------------------
 // step 1: vertex i -> its world point (mp_surface_point's two roundings) in rows [3][cap]; the count, clamped to the

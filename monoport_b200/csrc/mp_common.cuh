@@ -366,6 +366,24 @@ __device__ __forceinline__ float mp_last_op(float v, int last_op) {
   return v;
 }
 
+// atomicAdd on a float (the VJP kernel's feature-gradient scatter).  The CPU model of tests/emu runs the threads of a CTA
+// concurrently and models only the integer atomics: there it is a compare-and-swap loop on the float's bits.
+__device__ __forceinline__ float mp_atomic_add(float* p, float v) {
+#ifndef MP_CUDA_EMU
+  return atomicAdd(p, v);
+#else
+  unsigned* u = reinterpret_cast<unsigned*>(p);
+  unsigned old = __atomic_load_n(u, __ATOMIC_SEQ_CST), upd;
+  float f;
+  do {
+    memcpy(&f, &old, 4);
+    const float sum = f + v;
+    memcpy(&upd, &sum, 4);
+  } while (!__atomic_compare_exchange_n(u, &old, upd, false, __ATOMIC_SEQ_CST, __ATOMIC_SEQ_CST));
+  return f;
+#endif
+}
+
 __device__ __forceinline__ float mp_lrelu(float v) { return v > 0.f ? v : v * MP_LEAKY_SLOPE; }
 
 // host-side launchers implemented in the kernel files
@@ -391,6 +409,36 @@ int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
 int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
                            long long ld_grad, float* out, long long ld_out, float* dpoints, long long ld_dp, cudaStream_t st,
                            int guard, const MpBatch* bt = nullptr);
+// The vector-Jacobian product of the exact query (query_fp32.cu: query_vjp_kernel; query_vjp.cu drives it).  The caller of
+// mp_launch_query_vjp_tiles fills the outputs, the row tables and the chunk; the launcher fills w, mask_off and mask_words.
+struct MpVjpParams {
+  const float* w[MP_MAX_LAYERS];   // [cout][cin] row-major
+  int mask_off[MP_MAX_LAYERS];     // words (of P points) before hidden layer l's sign mask
+  int mask_words;
+  const float* grad_out;           // image b, channel r, point i at grad_out[b * gout_stride + r * ld_grad + i]; null = ones
+  long long ld_grad, gout_stride;
+  float* dp;                       // null, or d points: image b, coordinate a, point i at dp[b * dp_stride + a * ld_dp + i]
+  long long ld_dp, dp_stride;
+  float* dfeat;                    // null, or [B][H][W][C] fp32, accumulated with atomicAdd
+  float* rows;                     // null, or the saved rows [act rows ; delta rows][ld_rows] of the chunk's points
+  long long ld_rows;
+  int act_row[MP_MAX_LAYERS];      // row of hidden layer l's activations (the input X: rows 0 .. c0-1)
+  int delta_row[MP_MAX_LAYERS];    // row of layer l's δ
+  long long tile0, tile1;          // the chunk: tiles [tile0, tile1) of the B * ceil(n / P) tiles of the batch
+};
+// P of the VJP kernel for this head on the current device (a positive tile size), or an MP_E_* code
+int mp_query_vjp_tile(const mp_mlp* mlp);
+// one launch of query_vjp_kernel over the chunk of `outs` (src: MP_SRC_ROWS, n points per image; bt: the batch)
+int mp_launch_query_vjp_tiles(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
+                              const MpBatch& bt, const MpVjpParams& outs, cudaStream_t st);
+// the whole VJP (query_vjp.cu): outputs zeroed, then chunk by chunk the kernel and the weight-gradient contraction, then the
+// feature gradient's layout step.  dweights / dbiases: n_layers device pointers each, or null; scratch as sized by
+// mp_vjp_scratch_bytes for the same requests.
+long long mp_vjp_scratch_bytes(const mp_mlp* mlp, const mp_feat* feat, int B, long long n, long long chunk_points, bool dfeat,
+                               bool dweights);
+int mp_launch_query_vjp(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
+                        const float* grad_out, float* dfeat_nchw, float* dpoints, float* const* dweights, float* const* dbiases,
+                        void* scratch, long long scratch_bytes, cudaStream_t st);
 // device-side predicate shared by the kernels: true = the tiles of this image (amax = its entry) must do nothing.  In the
 // tensor-core program the weight producer and the consumers both take it, per tile, from the same word.
 __device__ __forceinline__ bool mp_guard_skips(const unsigned* amax, float limit, int guard) {

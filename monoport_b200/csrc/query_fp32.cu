@@ -184,11 +184,18 @@ __device__ __forceinline__ void tile_sample(const Fp32Params& prm, const MpPoint
   __syncthreads();
 }
 
+// what tile_hidden hands every finished hidden layer (l, its [cout][P] activations): nothing, except in the VJP kernel
+struct NoLayerSink {
+  __device__ __forceinline__ void operator()(int, const float*) const {}
+};
+
 // 3. hidden layers, ping-ponging between sA and sB (layer l writes sA for even l, sB for odd l); returns the last hidden
-// layer's activations.  MASK: layer l also stores its pre-activation signs at sMask + mask_off[l].
-template <int P, bool MASK>
+// layer's activations.  MASK: layer l also stores its pre-activation signs at sMask + mask_off[l].  `sink` sees each layer's
+// activations after the barrier that ends it, before the next-but-one layer overwrites them.
+template <int P, bool MASK, class Sink = NoLayerSink>
 __device__ __forceinline__ const float* tile_hidden(const Fp32Params& prm, const float* sX, float* sA, float* sB,
-                                                    unsigned* sMask = nullptr, const int* mask_off = nullptr) {
+                                                    unsigned* sMask = nullptr, const int* mask_off = nullptr,
+                                                    const Sink& sink = Sink()) {
   const float* sIn = sX;
   float* sOut = sA;
   for (int l = 0; l < prm.n_layers - 1; ++l) {
@@ -203,6 +210,7 @@ __device__ __forceinline__ const float* tile_hidden(const Fp32Params& prm, const
       dense_layer<P, 1, MASK>(prm.wt[l], prm.bias[l], hid, skipw, prm.cout[l], sIn, sX, sOut, m);
     }
     __syncthreads();
+    sink(l, sOut);
     sIn = sOut;
     sOut = (sOut == sA) ? sB : sA;
   }
@@ -377,6 +385,78 @@ __device__ void transposed_layer(const float* __restrict__ w, int cin, int cout,
   }
 }
 
+// the input gradient dX (in sX) of the tile's points of image b -> d(u,v,w) -> d point, written at dp[a * ld_dp + i]: warp
+// per point, lanes over channels.  The same arithmetic as the last step of query_grad_kernel below, which keeps its own
+// copy of these lines: calling this function there changes that kernel's register allocation.
+template <int P>
+__device__ __forceinline__ void tile_point_grad(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
+                                                int b, const float* feat, long long p0, long long n, const float* sX,
+                                                const float* sMeta, const int (&sOff)[4][P], float* dp_img, long long ld_dp) {
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  for (int p = warp; p < P; p += kThreads / 32) {
+    const long long i = p0 + p;
+    if (i >= n) continue;
+    float* dp = dp_img + i;
+    if (sMeta[p] == 0.f) {                             // outside the image: exactly 0
+      if (lane < 3) dp[lane * ld_dp] = 0.f;
+      continue;
+    }
+    // the projection and its Jacobian below: one MpCalib, the camera tile_sample projected with
+    const MpCalib c = mp_image_calib(cal, bt, b);
+    float x, y, z, u, v, w;
+    mp_load_point(src, bt, b, i, x, y, z);
+    mp_project(c, x, y, z, u, v, w);
+    // the tap cell of mp_taps; a tap outside the map is zero padding and contributes nothing
+    const float ix = ((u + 1.f) / 2.f) * (float)(prm.W - 1);
+    const float iy = ((v + 1.f) / 2.f) * (float)(prm.H - 1);
+    const float x0 = floorf(ix), y0 = floorf(iy);
+    const float fx = ix - x0, fy = iy - y0;
+    const float x1 = x0 + 1.f, y1 = y0 + 1.f;
+    const bool x0ok = (x0 >= 0.f) && (x0 <= (float)(prm.W - 1));
+    const bool x1ok = (x1 >= 0.f) && (x1 <= (float)(prm.W - 1));
+    const bool y0ok = (y0 >= 0.f) && (y0 <= (float)(prm.H - 1));
+    const bool y1ok = (y1 >= 0.f) && (y1 <= (float)(prm.H - 1));
+    const bool ok_nw = x0ok && y0ok, ok_ne = x1ok && y0ok, ok_sw = x0ok && y1ok, ok_se = x1ok && y1ok;
+    const float* f0 = feat + (size_t)sOff[0][p] * prm.C;
+    const float* f1 = feat + (size_t)sOff[1][p] * prm.C;
+    const float* f2 = feat + (size_t)sOff[2][p] * prm.C;
+    const float* f3 = feat + (size_t)sOff[3][p] * prm.C;
+    float du = 0.f, dv = 0.f;
+    for (int c = lane; c < prm.C; c += 32) {
+      const float fnw = ok_nw ? __ldg(f0 + c) : 0.f, fne = ok_ne ? __ldg(f1 + c) : 0.f;
+      const float fsw = ok_sw ? __ldg(f2 + c) : 0.f, fse = ok_se ? __ldg(f3 + c) : 0.f;
+      const float dx = sX[(size_t)c * P + p];
+      du = fmaf(dx, (1.f - fy) * (fne - fnw) + fy * (fse - fsw), du);
+      dv = fmaf(dx, (1.f - fx) * (fsw - fnw) + fx * (fse - fne), dv);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      du += __shfl_xor_sync(0xffffffffu, du, o);
+      dv += __shfl_xor_sync(0xffffffffu, dv, o);
+    }
+    if (lane == 0) {
+      du *= 0.5f * (float)(prm.W - 1);
+      dv *= 0.5f * (float)(prm.H - 1);
+      const float dw = c.z_scale * sX[(size_t)prm.C * P + p];
+      float g[3];
+      if (!c.has) {
+        g[0] = du; g[1] = dv; g[2] = dw;
+      } else if (!c.perspective) {                     // J = R
+#pragma unroll
+        for (int a = 0; a < 3; ++a) g[a] = c.m[a] * du + c.m[4 + a] * dv + c.m[8 + a] * dw;
+      } else {                                         // J rows: (R0 - u R2) / w, (R1 - v R2) / w, R2
+        const float su = du / w, sv = dv / w;
+        const float s2 = dw - su * u - sv * v;
+#pragma unroll
+        for (int a = 0; a < 3; ++a) g[a] = c.m[a] * su + c.m[4 + a] * sv + c.m[8 + a] * s2;
+      }
+#pragma unroll
+      for (int a = 0; a < 3; ++a) dp[a * ld_dp] = g[a];
+    }
+  }
+}
+
 template <int P>
 __global__ void __launch_bounds__(kThreads, 1)
 query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
@@ -521,6 +601,134 @@ int launch_grad(const Fp32Params& prm, const GradParams& gp, const MpPointSrc& s
   query_grad_kernel<P><<<grid, kThreads, smem, st>>>(prm, gp, src, cal);
 #else
   MP_EMU_LAUNCH(grid, kThreads, query_grad_kernel<P>(prm, gp, src, cal));
+#endif
+  MP_CUDA(cudaGetLastError());
+  return MP_OK;
+}
+
+// ---- F1'''': the vector-Jacobian product of the query, for training ------------------------------------------------------
+// query_grad_kernel's tile steps over the B * ceil(n / P) tiles of a batch (tile t of image t / ceil(n / P), as
+// query_fp32_kernel maps them), for the tiles [vp.tile0, vp.tile1) of one chunk.  Besides d points it can
+//   - save the rows the weight gradient contracts: the input X and every hidden activation in the forward half, every δ_l
+//     (the last layer's g included) in the reverse half -- column (t - tile0) * P + p of vp.rows (query_vjp.cu sums them);
+//   - scatter dX[:C] of each in-image point onto its four taps with grid_sample's weights (atomicAdd into [B][H][W][C]).
+// It writes no values.
+template <int P>
+__device__ __forceinline__ void save_rows(float* dst, long long ld, const float* src, int rows) {
+  for (int e = threadIdx.x; e < rows * P; e += kThreads) {
+    const int r = e / P, p = e % P;
+    dst[(long long)r * ld + p] = src[(size_t)r * P + p];
+  }
+}
+
+template <int P>
+struct SaveActivations {
+  float* rows;                 // this tile's first column, or null
+  long long ld;
+  const int* act_row;
+  const int* cout;
+  __device__ __forceinline__ void operator()(int l, const float* sOut) const {
+    if (rows) save_rows<P>(rows + (long long)act_row[l] * ld, ld, sOut, cout[l]);
+  }
+};
+
+template <int P>
+__global__ void __launch_bounds__(kThreads, 1)
+query_vjp_kernel(Fp32Params prm, MpVjpParams vp, MpPointSrc src, MpCalib cal, MpBatch bt) {
+  MP_DYN_SMEM_ALIGNED(float, smem, 16);
+  float* sX = smem;                                  // [c0][P]: sampled input, then dX
+  float* sA = sX + (size_t)prm.c0 * P;               // [h_ping][P]: activations of even layers, then their δ
+  float* sB = sA + (size_t)prm.h_ping * P;           // [h_pong][P]: odd layers
+  float* sMeta = sB + (size_t)prm.h_pong * P;        // [8][P]: in_img
+  unsigned* sMask = reinterpret_cast<unsigned*>(sMeta + 8 * P);          // [mask_words][P]
+  float* sG = reinterpret_cast<float*>(sMask + (size_t)vp.mask_words * P);   // [Res][P]
+  const int tid = threadIdx.x;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int L = prm.n_layers;
+  const int res = prm.cout[L - 1];
+  const long long n = src.n;
+  const long long n_tiles = (n + P - 1) / P;         // (per image)
+  const bool need_dx = vp.dp || vp.dfeat;            // (else the reverse pass stops at δ_0)
+
+  for (long long at = vp.tile0 + blockIdx.x; at < vp.tile1; at += gridDim.x) {
+    const int b = mp_tile_image(bt, at, n_tiles);
+    const long long p0 = (at - (long long)b * n_tiles) * P;
+    const float* feat = prm.feat + (size_t)b * prm.H * prm.W * prm.C;
+    float* rows = vp.rows ? vp.rows + (at - vp.tile0) * P : nullptr;
+    // ---- forward half ----------------------------------------------------------------------------
+    __shared__ int sOff[4][P];
+    __shared__ float sWgt[4][P];
+    tile_sample<P>(prm, src, cal, bt, b, feat, p0, n, sX, sMeta, sOff, sWgt);
+    if (rows) save_rows<P>(rows, vp.ld_rows, sX, prm.c0);
+    const float* sIn = tile_hidden<P, true>(prm, sX, sA, sB, sMask, vp.mask_off,
+                                            SaveActivations<P>{rows, vp.ld_rows, vp.act_row, prm.cout});
+    for (int job = warp; job < P * res; job += kThreads / 32) {
+      const int p = job % P, r = job / P;
+      const float acc = last_layer_dot<P>(prm, sX, sIn, p, r, lane);
+      if (lane == 0) {
+        const long long i = p0 + p;
+        float g = 0.f;
+        if (i < n) {
+          const float y = mp_last_op(acc + __ldg(prm.bias[L - 1] + r), prm.last_op);
+          const float d = prm.last_op == MP_LAST_SIGMOID ? y * (1.f - y) : (prm.last_op == MP_LAST_TANH ? 1.f - y * y : 1.f);
+          g = (vp.grad_out ? __ldg(vp.grad_out + b * vp.gout_stride + (long long)r * vp.ld_grad + i) : 1.f) * d;
+          if (sMeta[p] == 0.f) g = 0.f;                  // in_img multiplies the output (and y may be NaN/inf there)
+        }
+        sG[r * P + p] = g;
+      }
+    }
+    __syncthreads();
+    if (rows) save_rows<P>(rows + (long long)vp.delta_row[L - 1] * vp.ld_rows, vp.ld_rows, sG, res);
+    // ---- reverse half: last layer down to layer 0 (layer 0 only for dX) ----------------------------
+    const float* sDelta = sG;
+    for (int l = L - 1; l >= (need_dx ? 0 : 1); --l) {
+      const int hid = l == 0 ? 0 : prm.hid[l];
+      float* sHid = l == 0 ? nullptr : (((l - 1) & 1) ? sB : sA);
+      const unsigned* m = l == 0 ? nullptr : sMask + vp.mask_off[l - 1];
+      if (prm.cin[l] > kThreads)
+        transposed_layer<P, 2>(vp.w[l], prm.cin[l], prm.cout[l], hid, sDelta, sHid, m, sX, l == L - 1);
+      else
+        transposed_layer<P, 1>(vp.w[l], prm.cin[l], prm.cout[l], hid, sDelta, sHid, m, sX, l == L - 1);
+      __syncthreads();
+      if (rows && l > 0) save_rows<P>(rows + (long long)vp.delta_row[l - 1] * vp.ld_rows, vp.ld_rows, sHid, prm.cout[l - 1]);
+      sDelta = sHid;
+    }
+    // ---- dX -> d points, and dX[:C] -> the four taps of the feature map -----------------------------
+    if (vp.dp) tile_point_grad<P>(prm, src, cal, bt, b, feat, p0, n, sX, sMeta, sOff, vp.dp + b * vp.dp_stride, vp.ld_dp);
+    if (vp.dfeat) {
+      float* df = vp.dfeat + (size_t)b * prm.H * prm.W * prm.C;
+      for (int p = warp; p < P; p += kThreads / 32) {
+        if (p0 + p >= n || sMeta[p] == 0.f) continue;          // outside the image: nothing, anywhere
+        for (int a = 0; a < 4; ++a) {
+          const float wa = sWgt[a][p];
+          if (wa == 0.f) continue;                             // (a tap off the map has weight 0)
+          float* t = df + (size_t)sOff[a][p] * prm.C;
+          for (int c = lane; c < prm.C; c += 32) mp_atomic_add(t + c, wa * sX[(size_t)c * P + p]);
+        }
+      }
+    }
+    __syncthreads();
+  }
+}
+
+template <int P>
+int launch_vjp(const Fp32Params& prm, const MpVjpParams& vp, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
+               cudaStream_t st, int sm_count, int max_smem) {
+  const size_t smem = GradSmem<P>::bytes(prm.c0, prm.h_ping, prm.h_pong, vp.mask_words, prm.cout[prm.n_layers - 1]);
+  const int opt_in = max_smem - 2048;             // one device-wide bound, as in launch() below
+  static thread_local bool opted[64] = {};
+  int dev_ = 0;
+  MP_CUDA(cudaGetDevice(&dev_));
+  if (dev_ < 0 || dev_ >= 64 || !opted[dev_]) {
+    MP_CUDA(cudaFuncSetAttribute(query_vjp_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
+    if (dev_ >= 0 && dev_ < 64) opted[dev_] = true;
+  }
+  const long long tiles = vp.tile1 - vp.tile0;
+  const int grid = (int)(tiles < (long long)sm_count ? (tiles > 0 ? tiles : 1) : sm_count);
+#ifndef MP_CUDA_EMU
+  query_vjp_kernel<P><<<grid, kThreads, smem, st>>>(prm, vp, src, cal, bt);
+#else
+  MP_EMU_LAUNCH(grid, kThreads, query_vjp_kernel<P>(prm, vp, src, cal, bt));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -695,5 +903,56 @@ int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
   if (fits(GradSmem<16>::bytes(prm.c0, prm.h_ping, prm.h_pong, words, res))) return launch_grad<16>(prm, scaled(16), src, cal, st, sms, max_smem);
   if (fits(GradSmem<8>::bytes(prm.c0, prm.h_ping, prm.h_pong, words, res))) return launch_grad<8>(prm, scaled(8), src, cal, st, sms, max_smem);
   mp_set_error("head too wide for the gradient kernel's shared-memory tiling");
+  return MP_E_UNSUPPORTED;
+}
+
+// the VJP kernel's tile: the largest P of 32, 16, 8 whose shared memory fits (query_grad_kernel's footprint); 0: too wide
+static int vjp_tile(const mp_mlp* mlp, int max_smem) {
+  int ping = 0, pong = 0, words = 0;
+  for (int l = 0; l + 1 < mlp->n_layers; ++l) {
+    if (l % 2 == 0) ping = ping > mlp->cout[l] ? ping : mlp->cout[l];
+    else pong = pong > mlp->cout[l] ? pong : mlp->cout[l];
+    words += (mlp->cout[l] + 31) / 32;
+  }
+  const int c0 = mlp->channels[0], res = mlp->cout[mlp->n_layers - 1];
+  if (GradSmem<32>::bytes(c0, ping, pong, words, res) + 2048 <= (size_t)max_smem) return 32;
+  if (GradSmem<16>::bytes(c0, ping, pong, words, res) + 2048 <= (size_t)max_smem) return 16;
+  if (GradSmem<8>::bytes(c0, ping, pong, words, res) + 2048 <= (size_t)max_smem) return 8;
+  return 0;
+}
+
+int mp_query_vjp_tile(const mp_mlp* mlp) {
+  int dev = 0, max_smem = 0;
+  MP_CUDA(cudaGetDevice(&dev));
+  MP_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const int P = vjp_tile(mlp, max_smem);
+  if (!P) {
+    mp_set_error("head too wide for the VJP kernel's shared-memory tiling");
+    return MP_E_UNSUPPORTED;
+  }
+  return P;
+}
+
+int mp_launch_query_vjp_tiles(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
+                              const MpBatch& bt, const MpVjpParams& outs, cudaStream_t st) {
+  Fp32Params prm;
+  int sms = 0, max_smem = 0;
+  const int rc = fill_params(mlp, feat, prm, sms, max_smem);
+  if (rc != MP_OK) return rc;
+  prm.guard = MP_GUARD_NONE;
+  MpVjpParams vp = outs;
+  int words = 0;
+  for (int l = 0; l < mlp->n_layers; ++l) {
+    vp.w[l] = mlp->w[l];
+    vp.mask_off[l] = words;                      // (words per point here; scaled to words of a P-point tile below)
+    if (l < mlp->n_layers - 1) words += (mlp->cout[l] + 31) / 32;
+  }
+  vp.mask_words = words;
+  const int P = vjp_tile(mlp, max_smem);
+  for (int l = 0; l < mlp->n_layers; ++l) vp.mask_off[l] *= P;
+  if (P == 32) return launch_vjp<32>(prm, vp, src, cal, bt, st, sms, max_smem);
+  if (P == 16) return launch_vjp<16>(prm, vp, src, cal, bt, st, sms, max_smem);
+  if (P == 8) return launch_vjp<8>(prm, vp, src, cal, bt, st, sms, max_smem);
+  mp_set_error("head too wide for the VJP kernel's shared-memory tiling");
   return MP_E_UNSUPPORTED;
 }

@@ -9,6 +9,7 @@ import threading
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch.autograd.function import once_differentiable
 
 from .. import _lib
 from ..config import CN
@@ -71,6 +72,36 @@ class FeatureHandle:
                 _lib.load().mp_feat_destroy(self.ptr)
         except Exception:
             pass
+
+
+class _QueryStage(torch.autograd.Function):
+    """One stage of MonoPortNet.query_stages: the exact fp32 query in the forward, mp_query_points_vjp in the backward --
+    d features, d points and the head's d weights / d biases, each only when autograd asks for it."""
+
+    @staticmethod
+    def forward(ctx, net, feat, points, calibs, *params):
+        ctx.net = net
+        ctx.has_calibs = calibs is not None
+        ctx.save_for_backward(feat, points, *([calibs] if calibs is not None else []), *params)
+        return net._query_fp32(feat, points, calibs)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad):
+        saved = ctx.saved_tensors            # (raises if an optimizer step changed the head since the forward)
+        feat, points = saved[0], saved[1]
+        calibs = saved[2] if ctx.has_calibs else None
+        want_feat, want_points = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
+        want_head = any(ctx.needs_input_grad[4:])
+        dfeat, dpoints, dws, dbs = ctx.net._query_vjp(feat, points, calibs, grad, want_feat, want_points, want_head)
+        dparams = [None] * (len(saved) - (3 if ctx.has_calibs else 2))
+        if want_head:
+            head = ctx.net.surface_classifier
+            for l, f in enumerate(head.filters):
+                dparams[2 * l] = dws[l].reshape(f.weight.shape).to(f.weight.dtype)
+                dparams[2 * l + 1] = dbs[l].to(f.bias.dtype)
+        return (None, None if dfeat is None else dfeat.to(feat.dtype),
+                None if dpoints is None else dpoints.to(points.dtype), None, *dparams)
 
 
 class MonoPortNet(nn.Module):
@@ -148,7 +179,7 @@ class MonoPortNet(nn.Module):
         demo; B > 1 evaluates all images in one launch (mp_query_points_batch)."""
         if self.training:
             raise NotImplementedError("training-mode (multi-stage, autograd) query is outside the accelerated hot path; "
-                                      "call .eval() (RTL/main.py:116)")
+                                      "call .eval() (RTL/main.py:116), or query_stages() for the differentiable query")
         if transforms is not None:
             raise NotImplementedError("`transforms` is not supported (never passed on the recon path, RTL/main.py:179-182)")
         feats = feats_stages[-1]
@@ -242,6 +273,130 @@ class MonoPortNet(nn.Module):
                 ctypes.c_void_p(out.data_ptr()), n, ctypes.c_void_p(dp.data_ptr()), n, None, _MODES[precision],
                 _lib.stream_ptr(feat.device)), "mp_query_points_grad_mode")
         return out, dp
+
+    # ---- training: the differentiable query ---------------------------------------------------------------
+    # points per chunk of the weight-gradient contraction (its scratch: about 16 KB per point for the geometry head); the
+    # weight, bias and point gradients are the same bits from run to run for one chunk size
+    vjp_chunk_points = 8192
+
+    def query_stages(self, feats_stages, points, calibs=None, transforms=None):
+        """list(list([B,C,H,W])), points [B,3,N], calibs [B,4,4]|[B,3,4]|None -> [ [B,Res,N] for every stage ]
+        What the reference's train-mode query() computes (MonoPortNet.py:63-91: every hourglass stage), in either module
+        mode, differentiable with respect to every stage's feature map, the points and the head's `filters.{l}.weight` /
+        `filters.{l}.bias`.  The values are the exact fp32 kernel's (query() with precision "fp32", bit for bit); the
+        backward is one fused sm_90a VJP launch per chunk of points plus the weight-gradient contraction
+        (mp_query_points_vjp).  The feature gradient is accumulated with atomics (like grid_sample's backward) and so is
+        not bit-reproducible; the others are.  No double backward, no calib gradient."""
+        if transforms is not None:
+            raise NotImplementedError("`transforms` is not supported (never passed on the recon path, RTL/main.py:179-182)")
+        if calibs is not None and calibs.requires_grad:
+            raise ValueError("query_stages gives no gradient with respect to calibs; pass calibs.detach()")
+        head = self.surface_classifier
+        params = [t for f in head.filters for t in (f.weight, f.bias)]
+        preds = []
+        for feats in feats_stages:
+            if len(feats) != 1:
+                raise NotImplementedError("multi-level feature lists (HRNet) are not supported")
+            feat = feats[0]
+            if feat.device.type != "cuda":
+                raise RuntimeError("monoport_b200.query_stages: features must be CUDA tensors (there is no CPU path)")
+            B = feat.shape[0] if feat.dim() == 4 else -1
+            if feat.dim() != 4 or points.dim() != 3 or points.shape[0] != B or points.shape[1] != 3:
+                raise ValueError("features must be [B,C,H,W] and points [B,3,N]; got %s and %s"
+                                 % (tuple(feat.shape), tuple(points.shape)))
+            if calibs is not None and (calibs.dim() != 3 or calibs.shape[0] != B or calibs.shape[1] not in (3, 4)
+                                       or calibs.shape[2] != 4):
+                raise ValueError("calibs must be [B,4,4] or [B,3,4] with the features' B=%d; got %s"
+                                 % (B, tuple(calibs.shape)))
+            if points.device != feat.device:
+                raise ValueError("points and features live on different devices")
+            preds.append(_QueryStage.apply(self, feat, points, calibs, *params))
+        return preds
+
+    def _points_rows(self, points):
+        p = points.detach()
+        if p.dtype != torch.float32:
+            p = p.float()
+        if p.shape[2] > 0 and min(p.stride()) < 1:
+            p = p.contiguous()
+        return p
+
+    def _query_fp32(self, feat, points, calibs):
+        """the values of query_stages: query() with precision "fp32" (B = 1: mp_query_points, else mp_query_points_batch)"""
+        B, n = feat.shape[0], points.shape[2]
+        res = self.surface_classifier.filter_channels[-1]
+        out = torch.empty((B, res, n), dtype=torch.float32, device=feat.device)
+        if n == 0:
+            return out
+        p = self._points_rows(points)
+        s = p.stride()
+        proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
+        with _lib.device_guard(feat.device):
+            lib = _lib.load()
+            if B == 1:
+                fh = self.feature_handle(feat.detach())
+                _lib.check(lib.mp_query_points(
+                    self.surface_classifier.handle(), fh.ptr, ctypes.c_void_p(p.data_ptr()), n, s[1], s[2],
+                    _lib.calib12(None if calibs is None else calibs.detach()), proj, ctypes.c_float(self.normalizer.scale),
+                    ctypes.c_void_p(out.data_ptr()), n, _lib.MODE_FP32, _lib.stream_ptr(feat.device)), "mp_query_points")
+            else:
+                cal = None if calibs is None else calibs.detach()[:, :3, :4].to(device=feat.device, dtype=torch.float32).contiguous()
+                fh = self.batch_feature_handle(feat.detach())
+                _lib.check(lib.mp_query_points_batch(
+                    self.surface_classifier.handle(), fh.ptr, B, ctypes.c_void_p(p.data_ptr()), n, s[0], s[1], s[2],
+                    None if cal is None else ctypes.c_void_p(cal.data_ptr()), proj, ctypes.c_float(self.normalizer.scale),
+                    ctypes.c_void_p(out.data_ptr()), res * n, n, _lib.MODE_FP32, _lib.stream_ptr(feat.device)),
+                    "mp_query_points_batch")
+        return out
+
+    def _query_vjp(self, feat, points, calibs, grad, want_feat, want_points, want_head):
+        """-> (d feat [B,C,H,W] | None, d points [B,3,N] | None, [d W_l [Cout,Cin]] | None, [d b_l] | None) of
+        sum(grad * query) (mp_query_points_vjp).  The map is uploaded again: a query since the forward may have replaced
+        the handle's contents."""
+        B, C, H, W = feat.shape
+        n = points.shape[2]
+        head = self.surface_classifier
+        dev = feat.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        dfeat = torch.empty((B, C, H, W), **f32) if want_feat else None
+        dpoints = torch.empty((B, 3, n), **f32) if want_points else None
+        dws = [torch.empty(f.weight.shape[:2], **f32) for f in head.filters] if want_head else None
+        dbs = [torch.empty(f.bias.shape, **f32) for f in head.filters] if want_head else None
+        if n == 0:
+            for t in [dfeat, dpoints] + (dws or []) + (dbs or []):
+                if t is not None:
+                    t.zero_()
+            return dfeat, dpoints, dws, dbs
+        p = self._points_rows(points)
+        s = p.stride()
+        gout = grad.detach().to(torch.float32).contiguous()
+        proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
+        with _lib.device_guard(dev):
+            lib = _lib.load()
+            cal = None if calibs is None else calibs.detach()[:, :3, :4].to(**f32).contiguous()
+            key = ((C, H, W, dev.index, threading.get_ident()) if B == 1 else
+                   ("batch", B, C, H, W, dev.index, threading.get_ident()))
+            fh = self._feat_handles.get(key)
+            if fh is None:
+                fh = self._feat_handles[key] = FeatureHandle(C, H, W, dev, B=B)
+            fh.invalidate()
+            fh.upload(feat.detach())
+            mlp = head.handle()
+            nbytes = lib.mp_query_points_vjp_scratch_bytes(mlp, fh.ptr, B, n, int(self.vjp_chunk_points), int(want_feat),
+                                                           int(want_head))
+            if nbytes < 0:
+                _lib.check(int(nbytes), "mp_query_points_vjp_scratch_bytes")
+            scratch = torch.empty(int(nbytes), dtype=torch.uint8, device=dev) if nbytes > 0 else None
+            L = len(head.filters)
+            ptrs = (lambda ts: None if ts is None else (ctypes.c_void_p * L)(*[t.data_ptr() for t in ts]))
+            _lib.check(lib.mp_query_points_vjp(
+                mlp, fh.ptr, B, ctypes.c_void_p(p.data_ptr()), n, s[0], s[1], s[2],
+                None if cal is None else ctypes.c_void_p(cal.data_ptr()), proj, ctypes.c_float(self.normalizer.scale),
+                ctypes.c_void_p(gout.data_ptr()), None if dfeat is None else ctypes.c_void_p(dfeat.data_ptr()),
+                None if dpoints is None else ctypes.c_void_p(dpoints.data_ptr()), ptrs(dws), ptrs(dbs),
+                None if scratch is None else ctypes.c_void_p(scratch.data_ptr()), int(nbytes), _lib.stream_ptr(dev)),
+                "mp_query_points_vjp")
+        return dfeat, dpoints, dws, dbs
 
     def _query_batch(self, feat, points, calibs):
         """query() of B > 1 images: one launch; the calibs stay on the device (no read-back, no synchronisation)."""
