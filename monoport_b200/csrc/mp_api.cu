@@ -180,8 +180,9 @@ extern "C" int mp_feat_create_batch(int B, int C, int H, int W, mp_feat_t** out)
   cudaError_t e = cudaMalloc(&h->nhwc_own, n * sizeof(float));
   h->nhwc32 = h->nhwc_own;
   if (e == cudaSuccess) e = cudaMalloc(&h->staging, n * sizeof(float));
-  if (e == cudaSuccess) e = cudaMalloc(&h->amax, B * sizeof(unsigned));
-  if (e == cudaSuccess) e = cudaMemset(h->amax, 0, B * sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMalloc(&h->amax, 2 * B * sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMemset(h->amax, 0, 2 * B * sizeof(unsigned));
+  if (e == cudaSuccess) h->nonfinite = h->amax + B;
   if (e != cudaSuccess) {
     mp_set_error("mp_feat_create: %s", cudaGetErrorString(e));
     mp_feat_destroy(h);
@@ -208,7 +209,7 @@ extern "C" int mp_feat_upload(mp_feat_t* h, const float* nchw, int on_device, vo
   h->nhwc32 = h->nhwc_own;
   for (int b = 0; b < h->B; ++b) nchw_to_nhwc_kernel<<<grid, block, 0, st>>>(src + b * per_map, h->nhwc32 + b * per_map, h->C, HW);
   MP_CUDA(cudaGetLastError());
-  MP_CUDA(cudaMemsetAsync(h->amax, 0, h->B * sizeof(unsigned), st));
+  MP_CUDA(cudaMemsetAsync(h->amax, 0, 2 * h->B * sizeof(unsigned), st));
   h->version += 1;
   return MP_OK;
 }
@@ -220,7 +221,7 @@ extern "C" int mp_feat_upload_nhwc(mp_feat_t* h, const float* nhwc_dev, void* st
   const size_t n = (size_t)h->B * h->C * h->H * h->W;
   h->nhwc32 = h->nhwc_own;
   MP_CUDA(cudaMemcpyAsync(h->nhwc32, nhwc_dev, n * sizeof(float), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
-  MP_CUDA(cudaMemsetAsync(h->amax, 0, h->B * sizeof(unsigned), (cudaStream_t)stream));
+  MP_CUDA(cudaMemsetAsync(h->amax, 0, 2 * h->B * sizeof(unsigned), (cudaStream_t)stream));
   h->version += 1;
   return MP_OK;
 }
@@ -231,7 +232,7 @@ extern "C" int mp_feat_bind_nhwc(mp_feat_t* h, const float* nhwc_dev, void* stre
   MP_REQUIRE(h && nhwc_dev, "NULL handle or data");
   MP_REQUIRE((reinterpret_cast<uintptr_t>(nhwc_dev) & 15) == 0, "the channel-last map must be 16-byte aligned");
   h->nhwc32 = const_cast<float*>(nhwc_dev);
-  MP_CUDA(cudaMemsetAsync(h->amax, 0, h->B * sizeof(unsigned), (cudaStream_t)stream));
+  MP_CUDA(cudaMemsetAsync(h->amax, 0, 2 * h->B * sizeof(unsigned), (cudaStream_t)stream));
   h->version += 1;
   return MP_OK;
 }
@@ -629,7 +630,28 @@ static int query_grid_range(mp_mlp_t* mlp, mp_feat_t* feat, int R, long long lin
   dst.peer_off = lin0;        // the range's position inside every full [R,R,R] volume
   // (the value of a node never depends on the range it is evaluated in, so a sharded volume is bit-identical to the
   // single-GPU volume for every rank count)
-  return mp_query_dispatch(mlp, feat, src, cal, dst, mode, (cudaStream_t)stream);
+  // With a Sigmoid head on the tensor-core route a node outside the image has the value 0 * act = +0, so the program runs
+  // over the list of in-image nodes only (DESIGN.md §F1).  Other heads carry act's sign in that zero, and node indices
+  // are int32: those keep the dense launch.
+  const bool tc_route = mlp->tc_ok && (long long)feat->H * feat->W <= 65536 &&
+                        (mode == MP_MODE_AUTO || mode == MP_MODE_TC || mode == MP_MODE_TC_V3);
+  if (!tc_route || mlp->last_op != MP_LAST_SIGMOID || (long long)R * R * R >= (1ll << 31))
+    return mp_query_dispatch(mlp, feat, src, cal, dst, mode, (cudaStream_t)stream);
+  MpRange nvtx("monoport_b200: F1 fused sample+MLP query, in-image nodes");
+  // mp_query_dispatch's two guarded launches: the compaction's zero stores come first, the list launch skips an
+  // out-of-range frame on the device, and the exact launch then overwrites every node of the range
+  const cudaStream_t st = (cudaStream_t)stream;
+  void* scratch = nullptr;
+  mp_ensure_pool();
+  MP_CUDA(cudaMallocAsync(&scratch, mp_tc_grid_scratch_bytes(n), st));
+  const bool guarded = isfinite(mlp->tc_amax_limit);
+  cudaError_t e = cudaMemsetAsync(scratch, 0, 16, st);
+  int rc = e == cudaSuccess ? mp_launch_query_tc_grid(mlp, feat, src, cal, dst, scratch, st, guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE)
+                            : MP_E_CUDA;
+  if (e != cudaSuccess) mp_set_error("scratch of the grid query: %s", cudaGetErrorString(e));
+  if (rc == MP_OK && guarded) rc = mp_launch_query_fp32(mlp, feat, src, cal, dst, st, MP_GUARD_OUT_OF_RANGE);
+  cudaFreeAsync(scratch, st);
+  return rc;
 }
 
 extern "C" int mp_query_grid(mp_mlp_t* mlp, mp_feat_t* feat, int R, int z0, int nz, const float* b_min3, const float* b_max3,

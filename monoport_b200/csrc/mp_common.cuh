@@ -122,6 +122,9 @@ struct mp_feat {
   // max |feature| of the current frame as float bits (non-negative floats order like unsigned integers): zeroed by every
   // upload, raised by the staging pass of the per-frame G0 kernels; read by the range guard of the query kernels
   unsigned* amax;
+  // [B] after amax (the same allocation, zeroed with it): nonzero when the current map holds a NaN or an infinity (raised by
+  // the same staging pass); the in-image grid launch then lists every node
+  unsigned* nonfinite;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -232,6 +235,10 @@ struct MpOutDst {
   float* peer[MP_MAX_PEERS] = {};
   long long peer_off = 0;
   int n_peers = 0;
+  // MP_SRC_NODES over the full volumes (the in-image list of a grid query): if set, the peer stores of point i go to
+  // peer[p][nodes[i]] instead of peer[p][peer_off + i].  (An int in the struct's tail padding: the exact kernel keeps a
+  // copy of dst on its stack.)
+  int peer_by_node = 0;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -397,6 +404,14 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
                          const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                        const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
+// The tensor-core program over the nodes of an MP_SRC_GRID range that project into the image, for a head whose last op is
+// Sigmoid (there a node outside the image has the value 0 * act = +0 exactly).  An ordered compaction lists those nodes and
+// stores +0 for the others into dst (out[i] and / or peer[p][peer_off + i]); the program then runs over the list with a
+// device-side count.  One map, calib by value; the output is the dense launch's bit for bit.  `guard` as above.  scratch:
+// mp_tc_grid_scratch_bytes(grid.n) bytes of device memory whose first 16 are zero (they are left at zero).
+size_t mp_tc_grid_scratch_bytes(long long n);
+int mp_launch_query_tc_grid(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& grid, const MpCalib& cal, const MpOutDst& dst,
+                            void* scratch, cudaStream_t st, int guard);
 // gradient of the fp32 query with respect to the points (query_fp32.cu): value -> out[r*ld_out+i] (out may be null; written
 // by a query_fp32_kernel launch, so it is that kernel's value bit for bit),
 // d(sum_r grad_out[r*ld_grad+i] * value_r)/d point_i -> dpoints[a*ld_dp+i] (grad_out null = ones); MP_SRC_ROWS, one map.

@@ -27,6 +27,7 @@
 // query_wg_kernel and query_jvp_kernel (the point gradient, forward mode) share that producer, ring and trunk of layers
 // 1-3 (run_trunk); each passes in its own layer-0 chunks, hidden-layer epilogue and layer 4.
 #include "mp_common.cuh"
+#include "mp_scan.cuh"
 #include "tc_ptx.cuh"
 #include <stdlib.h>
 
@@ -148,13 +149,22 @@ struct PointTaps {
   bool in_img;      // MonoPortNet.py:74
 };
 
-// projection (geometry.py:19-55) + mask + taps of point i of image b (i >= n: masked-out padding point), projected with
-// image b's calibration; surface vertices when surf.X.
+// The program's projection (geometry.py:19-55, m0 x rounded first) of the world point (x, y, z) and its mask
+// (MonoPortNet.py:74): the taps below and the in-image list of a grid query (InImage) both take it, so the list holds
+// exactly the nodes the dense launch does not multiply by 0.
+__device__ __forceinline__ bool tc_project_in_image(const MpCalib& cal, float x, float y, float z, float& u, float& v, float& w) {
+  mp_project<true>(cal, x, y, z, u, v, w);
+  return (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);
+}
+
+// projection + mask + taps of point i of image b (i >= n: masked-out padding point), projected with image b's calibration;
+// surface vertices when surf.X.
 __device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
                                                 int b, int H, int W, long long i, long long n) {
   PointTaps pt;
   float u = 0.f, v = 0.f, w = 0.f;
   const bool valid = i < n;
+  bool in_img = false;
   if (valid) {
     float x, y, z;
     if (surf.X) {
@@ -162,9 +172,9 @@ __device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const 
     } else {
       mp_load_point(src, bt, b, i, x, y, z);
     }
-    mp_project<true>(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
+    in_img = tc_project_in_image(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
   }
-  pt.in_img = valid && (u >= -1.f) && (u <= 1.f) && (v >= -1.f) && (v <= 1.f);
+  pt.in_img = in_img;
   const MpTaps t = mp_taps(valid ? u : 0.f, valid ? v : 0.f, H, W);
   const bool dead = !valid || !(u == u) || !(v == v);      // NaN coordinates (perspective with w == 0): keep taps finite
 #pragma unroll
@@ -672,9 +682,10 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
             if (dst.scatter_vol && r == 0) dst.scatter_vol[__ldg(src.nodes + i)] = val;
             if constexpr (PEERS) {
               if (r == 0) {
+                const long long at = dst.peer_by_node ? (long long)__ldg(src.nodes + i) : dst.peer_off + i;
 #pragma unroll
                 for (int pp = 0; pp < MP_MAX_PEERS; ++pp)
-                  if (pp < dst.n_peers) dst.peer[pp][dst.peer_off + i] = val;
+                  if (pp < dst.n_peers) dst.peer[pp][at] = val;
               }
             }
           }
@@ -1123,7 +1134,8 @@ template <int C> struct G0Cfg {
 template <int C>
 __global__ void __launch_bounds__(kG0Threads, 1)
 g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half* __restrict__ G, int M,
-             __half* __restrict__ F16, float* __restrict__ S4, const float* __restrict__ w4s, unsigned* __restrict__ amax) {
+             __half* __restrict__ F16, float* __restrict__ S4, const float* __restrict__ w4s, unsigned* __restrict__ amax,
+             unsigned* __restrict__ nonfinite) {
   using Cfg = G0Cfg<C>;
   constexpr int RES = Prog<C>::RES, KB = Cfg::KB;
   MP_DYN_SMEM(uint8_t, g0_smem_raw);
@@ -1144,6 +1156,7 @@ g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half
     F16 += img * M * C;
     S4 += img * M * RES;
     if (amax) amax += img;
+    if (nonfinite) nonfinite += img;
   }
   if (tid == 0) {
     for (int i = 0; i < kG0Stages; ++i) { tc::mbar_init(&b_full[i], 1); tc::mbar_init(&b_empty[i], kConsumers / 32); }
@@ -1170,6 +1183,7 @@ g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half
     const float* frow = F + (size_t)(live ? m0 + row : 0) * C + half * 32;
     float s4acc[RES];
     float fmax_abs = 0.f;             // range guard: the largest |feature| this thread stages
+    float nf_probe = 0.f;             // x - x summed over the same features: NaN once one of them is a NaN or an infinity
 #pragma unroll
     for (int r = 0; r < RES; ++r) s4acc[r] = 0.f;
 #pragma unroll 1
@@ -1179,6 +1193,8 @@ g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half
       for (int j = 0; j < 8; ++j) v[j] = live ? __ldg(reinterpret_cast<const float4*>(frow + kb * 64) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) fmax_abs = fmaxf(fmax_abs, fmaxf(fmaxf(fabsf(v[j].x), fabsf(v[j].y)), fmaxf(fabsf(v[j].z), fabsf(v[j].w))));
+#pragma unroll
+      for (int j = 0; j < 8; ++j) nf_probe += ((v[j].x - v[j].x) + (v[j].y - v[j].y)) + ((v[j].z - v[j].z) + (v[j].w - v[j].w));
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
         uint4 pk;
@@ -1206,6 +1222,8 @@ g0_wg_kernel(const float* __restrict__ F, const uint8_t* __restrict__ Wt, __half
       for (int o = 16; o > 0; o >>= 1) fmax_abs = fmaxf(fmax_abs, __shfl_xor_sync(0xffffffffu, fmax_abs, o));
       if (lane == 0) atomicMax(amax, __float_as_uint(fmax_abs));       // non-negative floats order like their bit patterns
     }
+    // (fmaxf drops a NaN, so the maximum above cannot tell a map with a NaN: this flag can)
+    if (nonfinite && __any_sync(0xffffffffu, !(nf_probe == 0.f)) && lane == 0) atomicMax(nonfinite, 1u);
 #pragma unroll
     for (int r = 0; r < RES; ++r) {
       const float tot = s4acc[r] + __shfl_xor_sync(0xffffffffu, s4acc[r], 1);
@@ -1391,11 +1409,12 @@ int frame_products(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, cudaStrea
     const dim3 g0_grid((unsigned)((HW + 127) / 128), (unsigned)maps);
 #ifndef MP_CUDA_EMU
     g0_wg_kernel<C><<<g0_grid, kG0Threads, G0Cfg<C>::Smem, st>>>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s,
-                                                              feat->amax);
+                                                              feat->amax, feat->nonfinite);
 #else
     // (a 2-D grid: the CPU model's launcher of tests/emu takes the dim3 itself)
     cuda_emu::launch(g0_grid, dim3((unsigned)kG0Threads),
-                     [&] { g0_wg_kernel<C>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, feat->amax); });
+                     [&] { g0_wg_kernel<C>(feat->nhwc32, pk->d_w0t, feat->g0, (int)HW, feat->f16, feat->s4tex, pk->w4s, feat->amax,
+                                          feat->nonfinite); });
 #endif
     MP_CUDA(cudaGetLastError());
     feat->g0_owner = mlp->gen;
@@ -1483,6 +1502,48 @@ int launch_jvp(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPoint
   MP_CUDA(cudaGetLastError());
   return MP_OK;
 }
+
+// ---- the in-image list of a grid range (mp_launch_query_tc_grid), on the ordered scan of mp_scan.cuh
+// f(i) = 1 when node lin0 + i projects into the image.  When the map holds a NaN or an infinity every node counts: the
+// range guard does not send every such frame to the exact kernel (its maximum ignores a NaN), and then 0 * act need not
+// be +0 outside the image.
+struct InImage {
+  static constexpr bool kVec8 = false;
+  MpPointSrc grid;
+  MpCalib cal;
+  const unsigned* nonfinite;
+  __device__ unsigned long long operator()(long long i) const {
+    if (nonfinite && *nonfinite) return 1ull;
+    float x, y, z, u, v, w;
+    mp_load_point(grid, MpBatch(), 0, i, x, y, z);
+    return tc_project_in_image(cal, x, y, z, u, v, w) ? 1ull : 0ull;
+  }
+};
+
+// a listed node goes to the list at its prefix (ascending node order, so the program's scattered stores stay nearly
+// coalesced); any other node gets the value the dense launch gives it, +0
+struct ListOrZero {
+  int32_t* list;
+  float* out;                       // the range's outputs, or null
+  float* peer[MP_MAX_PEERS];
+  int n_peers;
+  long long lin0, peer_off;
+  __device__ void operator()(long long i, unsigned long long in, unsigned long long at) const {
+    if (in) {
+      list[at] = (int32_t)(lin0 + i);
+      return;
+    }
+    if (out) out[i] = 0.f;
+#pragma unroll
+    for (int p = 0; p < MP_MAX_PEERS; ++p)
+      if (p < n_peers) peer[p][peer_off + i] = 0.f;
+  }
+};
+
+struct StoreCount {
+  int32_t* count;
+  __device__ void operator()(unsigned long long total) const { *count = (int32_t)total; }
+};
 
 // what the query and the gradient launches both need: the head's program prepared, a map of the head's channel count C
 // and of at most 65536 texels (texel indices travel as 16-bit pairs in registers, per map of a batch)
@@ -1591,6 +1652,61 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
   const MpBatch& b = bt ? *bt : MpBatch();
   return C == 256 ? launch<256>(mlp, pk, feat, src, cal, dst, st, surf, guard, b)
                   : launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, b);
+}
+
+// scratch of mp_launch_query_tc_grid: total[2] (grand total, ticket), the chunk sums, the count, the list
+static size_t grid_list_offset(long long n) { return 16 + 8 * (size_t)mpscan::num_blocks(n) + 16; }
+
+size_t mp_tc_grid_scratch_bytes(long long n) { return grid_list_offset(n) + 4 * (size_t)n; }
+
+// Three launches: the compaction's two (its zero stores first on the stream), then the program over the list.  Node
+// coordinates are integers, so MP_SRC_NODES gives each node the world point MP_SRC_GRID gives it, bit for bit.
+int mp_launch_query_tc_grid(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& grid, const MpCalib& cal, const MpOutDst& dst,
+                            void* scratch, cudaStream_t st, int guard) {
+  const long long n = grid.n;
+  if (n <= 0) return MP_OK;
+  int C = 0;
+  int rc = check_query(mlp, feat, C);
+  if (rc != MP_OK) return rc;
+  if (C != 256 || mlp->last_op != MP_LAST_SIGMOID || grid.kind != MP_SRC_GRID || grid.lin0 + n > (1ll << 31) ||
+      dst.n_peers > MP_MAX_PEERS || (dst.n_peers > 0 && dst.peer_off != grid.lin0) || dst.scatter_vol || dst.peer_by_node) {
+    mp_set_error("the in-image grid launch takes a grid range of int32 node indices and a single-output Sigmoid head");
+    return MP_E_UNSUPPORTED;
+  }
+  const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
+  // the map's non-finite flag, which the compaction reads, comes with the per-frame products
+  rc = frame_products<256>(mlp, pk, feat, st);
+  if (rc != MP_OK) return rc;
+  const int nb = mpscan::num_blocks(n);
+  unsigned long long* total = static_cast<unsigned long long*>(scratch);
+  int32_t* list = reinterpret_cast<int32_t*>(static_cast<uint8_t*>(scratch) + grid_list_offset(n));
+  int32_t* count = list - 4;                     // (the 16 bytes before the list)
+  const InImage f{grid, cal, feat->nonfinite};
+  ListOrZero em;
+  em.list = list;
+  em.out = dst.out;
+  for (int p = 0; p < MP_MAX_PEERS; ++p) em.peer[p] = dst.peer[p];
+  em.n_peers = dst.n_peers;
+  em.lin0 = grid.lin0;
+  em.peer_off = dst.peer_off;
+#ifndef MP_CUDA_EMU
+  MP_CUDA(mpscan::scan_emit(f, em, n, total + 2, total, st, StoreCount{count}));
+#else
+  MP_EMU_LAUNCH(nb, mpscan::kThreads, (mpscan::block_sums_kernel<InImage, StoreCount>(f, n, total + 2, nb, total, StoreCount{count})));
+  MP_EMU_LAUNCH(nb, mpscan::kThreads, (mpscan::emit_kernel<InImage, ListOrZero>(f, em, n, total + 2)));
+#endif
+  MpPointSrc src = grid;                         // (n stays the upper bound of the device-side count)
+  src.kind = MP_SRC_NODES;
+  src.nodes = list;
+  src.count_dev = count;
+  MpOutDst ldst = dst;                           // values by node index: out through the node scatter, the peers by peer_by_node
+  ldst.out = nullptr;
+  ldst.ld = 0;
+  ldst.scatter_vol = dst.out ? dst.out - grid.lin0 : nullptr;
+  ldst.peer_by_node = 1;
+  MpSurfaceSrc surf;
+  memset(&surf, 0, sizeof(surf));
+  return launch<256>(mlp, pk, feat, src, cal, ldst, st, surf, guard, MpBatch());
 }
 
 int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
