@@ -414,8 +414,9 @@ int mp_launch_query_tc_grid(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& 
                             void* scratch, cudaStream_t st, int guard);
 // gradient of the fp32 query with respect to the points (query_fp32.cu): value -> out[r*ld_out+i] (out may be null; written
 // by a query_fp32_kernel launch, so it is that kernel's value bit for bit),
-// d(sum_r grad_out[r*ld_grad+i] * value_r)/d point_i -> dpoints[a*ld_dp+i] (grad_out null = ones); MP_SRC_ROWS, one map.
-// src.count_dev (when set) is the point count on the device; `guard` as for the query launchers.
+// d(sum_r grad_out[r*ld_grad+i] * value_r)/d point_i -> dpoints[a*ld_dp+i] (grad_out null = ones): one launch of the VJP
+// kernel below, for d points only; MP_SRC_ROWS, one map.  src.count_dev (when set) is the point count on the device;
+// `guard` as for the query launchers.
 int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
                          long long ld_dp, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
@@ -443,9 +444,10 @@ struct MpVjpParams {
 };
 // P of the VJP kernel for this head on the current device (a positive tile size), or an MP_E_* code
 int mp_query_vjp_tile(const mp_mlp* mlp);
-// one launch of query_vjp_kernel over the chunk of `outs` (src: MP_SRC_ROWS, n points per image; bt: the batch)
+// one launch of query_vjp_kernel over the chunk of `outs` (src: MP_SRC_ROWS, n points per image -- src.count_dev, when set,
+// the count on the device of a single-map launch; bt: the batch); `guard` as for the query launchers
 int mp_launch_query_vjp_tiles(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
-                              const MpBatch& bt, const MpVjpParams& outs, cudaStream_t st);
+                              const MpBatch& bt, const MpVjpParams& outs, cudaStream_t st, int guard = MP_GUARD_NONE);
 // the whole VJP (query_vjp.cu): outputs zeroed, then chunk by chunk the kernel and the weight-gradient contraction, then the
 // feature gradient's layout step.  dweights / dbiases: n_layers device pointers each, or null; scratch as sized by
 // mp_vjp_scratch_bytes for the same requests.

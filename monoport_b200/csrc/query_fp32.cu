@@ -17,14 +17,6 @@ namespace {
 
 constexpr int kThreads = 256;
 
-template <int P>
-struct Fp32Smem {
-  // sizes in floats
-  static __host__ __device__ size_t bytes(int c0, int h_ping, int h_pong) {
-    return (size_t)(c0 + h_ping + h_pong) * P * sizeof(float) + (size_t)P * 8 * sizeof(float);
-  }
-};
-
 struct Fp32Params {
   int n_layers;
   int c0;                       // input width (C + 1)
@@ -58,7 +50,7 @@ __device__ __forceinline__ void fma_rows(float (&acc)[NCO][P], const float* __re
 }
 
 // One hidden layer: out[co][p] = lrelu(b[co] + sum_k Wt[k][co] * in[k][p]),  in = [hidden rows ; skip rows]
-// MASK (the gradient kernel): also store the sign of every pre-activation, bit co % 32 of sMask[(co / 32) * P + p]
+// MASK (the VJP kernel): also store the sign of every pre-activation, bit co % 32 of sMask[(co / 32) * P + p]
 template <int P, int NCO, bool MASK = false>
 __device__ void dense_layer(const float* __restrict__ wt, const float* __restrict__ bias, int cin_hidden, int cin_skip,
                             int cout, const float* sHidden, const float* sSkip, float* sOut, unsigned* sMask = nullptr) {
@@ -134,7 +126,7 @@ __device__ void dense_layer(const float* __restrict__ wt, const float* __restric
   }
 }
 
-// ---- the steps of a tile, shared by query_fp32_kernel and the forward half of query_grad_kernel ------------------------
+// ---- the steps of a tile, shared by query_fp32_kernel and the forward half of query_vjp_kernel --------------------------
 // 1. projection, mask, taps of image b's points; 2. bilinear gather from its map `feat`: sX = [sampled features ;
 // z * z_scale], sMeta[p] = in_img.  SURF: the points are the vertices of *surf (one map) instead of src's.
 template <int P, bool SURF = false>
@@ -304,7 +296,7 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpB
   }
 }
 
-// ---- F1'': gradient of the query with respect to the points -----------------------------------------------------------
+// ---- F1'' and F1'''': the reverse pass of the query (the point gradient, and the vector-Jacobian product for training) ---
 // Forward half = the fp32 kernel's tile steps (tile_sample / tile_hidden / last_layer_dot above), which also record the sign
 // of every hidden pre-activation as bit masks (1920 bits per point for the shipped heads).  Reverse half, per tile:
 //   g      = grad_out * last_op'(value) * in_img                                    -> sG    [Res][P]
@@ -313,23 +305,6 @@ query_fp32_kernel(Fp32Params prm, MpPointSrc src, MpCalib cal, MpOutDst dst, MpB
 //   d(u,v) = sum_c dX_c * dX_c/d(u,v)   (grid_sample's backward: the tap differences), dw = z_scale * dX_C
 //   dp     = J^T d(u,v,w),  J = d(u,v,w)/dp of the projection
 // The transposed products read the row-major [cout][cin] weight copy: the thread that owns input channel k reads w[co][k].
-struct GradParams {
-  const float* w[MP_MAX_LAYERS];   // [cout][cin] row-major
-  int mask_off[MP_MAX_LAYERS];     // words (of P points) before hidden layer l's sign mask
-  int mask_words;
-  const float* grad_out;           // [Res][ld_grad] or null (= ones)
-  long long ld_grad;
-  float* dp;                       // [3][ld_dp]
-  long long ld_dp;
-  const float* calib;              // rows 0..2 of [R|t] in device memory, read when the kernel runs (null: MpCalib::m)
-};
-
-template <int P>
-struct GradSmem {
-  static __host__ __device__ size_t bytes(int c0, int h_ping, int h_pong, int mask_words, int res) {
-    return Fp32Smem<P>::bytes(c0, h_ping, h_pong) + (size_t)mask_words * P * sizeof(unsigned) + (size_t)res * P * sizeof(float);
-  }
-};
 
 // out[k][p] = sum_co W[co][k] * delta[co][p] for the cin input channels k of a layer; rows k < hid are the previous layer's
 // δ (times lrelu' from its mask), rows k >= hid go to dX[k - hid] (assigned when `first`, accumulated otherwise)
@@ -386,8 +361,7 @@ __device__ void transposed_layer(const float* __restrict__ w, int cin, int cout,
 }
 
 // the input gradient dX (in sX) of the tile's points of image b -> d(u,v,w) -> d point, written at dp[a * ld_dp + i]: warp
-// per point, lanes over channels.  The same arithmetic as the last step of query_grad_kernel below, which keeps its own
-// copy of these lines: calling this function there changes that kernel's register allocation.
+// per point, lanes over channels
 template <int P>
 __device__ __forceinline__ void tile_point_grad(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
                                                 int b, const float* feat, long long p0, long long n, const float* sX,
@@ -457,158 +431,10 @@ __device__ __forceinline__ void tile_point_grad(const Fp32Params& prm, const MpP
   }
 }
 
-template <int P>
-__global__ void __launch_bounds__(kThreads, 1)
-query_grad_kernel(Fp32Params prm, GradParams gp, MpPointSrc src, MpCalib cal) {
-  MP_DYN_SMEM_ALIGNED(float, smem, 16);
-  float* sX = smem;                                  // [c0][P]: sampled input, then dX
-  float* sA = sX + (size_t)prm.c0 * P;               // [h_ping][P]: activations of even layers, then their δ
-  float* sB = sA + (size_t)prm.h_ping * P;           // [h_pong][P]: odd layers
-  float* sMeta = sB + (size_t)prm.h_pong * P;        // [8][P]: in_img
-  unsigned* sMask = reinterpret_cast<unsigned*>(sMeta + 8 * P);          // [mask_words][P]
-  float* sG = reinterpret_cast<float*>(sMask + (size_t)gp.mask_words * P);   // [Res][P]
-  const int tid = threadIdx.x;
-  const int warp = tid >> 5, lane = tid & 31;
-  const int L = prm.n_layers;
-  const int res = prm.cout[L - 1];
-  long long n = src.n;
-  if (src.count_dev) {                               // (the point count on the device: src.n is then the capacity)
-    const long long c = *src.count_dev;
-    n = c < n ? c : n;
-  }
-  // the range guard, decided per launch as query_fp32_kernel decides it (uniform over the grid)
-  const long long n_tiles = mp_guard_skips(prm.amax, prm.amax_limit, prm.guard) ? 0 : (n + P - 1) / P;
-  MpBatch one;                                       // (a single map; its camera in device memory when gp.calib is set)
-  one.calibs = gp.calib;
-
-  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-    const long long p0 = tile * P;
-    // ---- forward half: the fp32 kernel's steps, plus the sign masks --------------------------------
-    __shared__ int sOff[4][P];
-    __shared__ float sWgt[4][P];
-    tile_sample<P>(prm, src, cal, one, 0, prm.feat, p0, n, sX, sMeta, sOff, sWgt);
-    const float* sIn = tile_hidden<P, true>(prm, sX, sA, sB, sMask, gp.mask_off);
-    for (int job = warp; job < P * res; job += kThreads / 32) {
-      const int p = job % P, r = job / P;
-      const float acc = last_layer_dot<P>(prm, sX, sIn, p, r, lane);
-      if (lane == 0) {
-        const long long i = p0 + p;
-        float g = 0.f;
-        if (i < n) {
-          const float y = mp_last_op(acc + __ldg(prm.bias[L - 1] + r), prm.last_op);
-          const float d = prm.last_op == MP_LAST_SIGMOID ? y * (1.f - y) : (prm.last_op == MP_LAST_TANH ? 1.f - y * y : 1.f);
-          g = (gp.grad_out ? __ldg(gp.grad_out + (long long)r * gp.ld_grad + i) : 1.f) * d;
-          if (sMeta[p] == 0.f) g = 0.f;                  // in_img multiplies the output (and y may be NaN/inf there)
-        }
-        sG[r * P + p] = g;
-      }
-    }
-    __syncthreads();
-    // ---- reverse half: last layer down to layer 0 -------------------------------------------------
-    const float* sDelta = sG;
-    for (int l = L - 1; l >= 0; --l) {
-      const int hid = l == 0 ? 0 : prm.hid[l];
-      float* sHid = l == 0 ? nullptr : (((l - 1) & 1) ? sB : sA);
-      const unsigned* m = l == 0 ? nullptr : sMask + gp.mask_off[l - 1];
-      if (prm.cin[l] > kThreads)
-        transposed_layer<P, 2>(gp.w[l], prm.cin[l], prm.cout[l], hid, sDelta, sHid, m, sX, l == L - 1);
-      else
-        transposed_layer<P, 1>(gp.w[l], prm.cin[l], prm.cout[l], hid, sDelta, sHid, m, sX, l == L - 1);
-      __syncthreads();
-      sDelta = sHid;
-    }
-    // ---- input gradient -> d(u,v,w) -> dp: warp per point, lanes over channels ---------------------
-    for (int p = warp; p < P; p += kThreads / 32) {
-      const long long i = p0 + p;
-      if (i >= n) continue;
-      float* dp = gp.dp + i;
-      if (sMeta[p] == 0.f) {                             // outside the image: exactly 0
-        if (lane < 3) dp[lane * gp.ld_dp] = 0.f;
-        continue;
-      }
-      // the projection and its Jacobian below: one MpCalib, the camera tile_sample projected with
-      const MpCalib c = mp_image_calib(cal, one, 0);
-      float x, y, z, u, v, w;
-      mp_load_point(src, one, 0, i, x, y, z);
-      mp_project(c, x, y, z, u, v, w);
-      // the tap cell of mp_taps; a tap outside the map is zero padding and contributes nothing
-      const float ix = ((u + 1.f) / 2.f) * (float)(prm.W - 1);
-      const float iy = ((v + 1.f) / 2.f) * (float)(prm.H - 1);
-      const float x0 = floorf(ix), y0 = floorf(iy);
-      const float fx = ix - x0, fy = iy - y0;
-      const float x1 = x0 + 1.f, y1 = y0 + 1.f;
-      const bool x0ok = (x0 >= 0.f) && (x0 <= (float)(prm.W - 1));
-      const bool x1ok = (x1 >= 0.f) && (x1 <= (float)(prm.W - 1));
-      const bool y0ok = (y0 >= 0.f) && (y0 <= (float)(prm.H - 1));
-      const bool y1ok = (y1 >= 0.f) && (y1 <= (float)(prm.H - 1));
-      const bool ok_nw = x0ok && y0ok, ok_ne = x1ok && y0ok, ok_sw = x0ok && y1ok, ok_se = x1ok && y1ok;
-      const float* f0 = prm.feat + (size_t)sOff[0][p] * prm.C;
-      const float* f1 = prm.feat + (size_t)sOff[1][p] * prm.C;
-      const float* f2 = prm.feat + (size_t)sOff[2][p] * prm.C;
-      const float* f3 = prm.feat + (size_t)sOff[3][p] * prm.C;
-      float du = 0.f, dv = 0.f;
-      for (int c = lane; c < prm.C; c += 32) {
-        const float fnw = ok_nw ? __ldg(f0 + c) : 0.f, fne = ok_ne ? __ldg(f1 + c) : 0.f;
-        const float fsw = ok_sw ? __ldg(f2 + c) : 0.f, fse = ok_se ? __ldg(f3 + c) : 0.f;
-        const float dx = sX[(size_t)c * P + p];
-        du = fmaf(dx, (1.f - fy) * (fne - fnw) + fy * (fse - fsw), du);
-        dv = fmaf(dx, (1.f - fx) * (fsw - fnw) + fx * (fse - fne), dv);
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        du += __shfl_xor_sync(0xffffffffu, du, o);
-        dv += __shfl_xor_sync(0xffffffffu, dv, o);
-      }
-      if (lane == 0) {
-        du *= 0.5f * (float)(prm.W - 1);
-        dv *= 0.5f * (float)(prm.H - 1);
-        const float dw = c.z_scale * sX[(size_t)prm.C * P + p];
-        float g[3];
-        if (!c.has) {
-          g[0] = du; g[1] = dv; g[2] = dw;
-        } else if (!c.perspective) {                     // J = R
-#pragma unroll
-          for (int a = 0; a < 3; ++a) g[a] = c.m[a] * du + c.m[4 + a] * dv + c.m[8 + a] * dw;
-        } else {                                         // J rows: (R0 - u R2) / w, (R1 - v R2) / w, R2
-          const float su = du / w, sv = dv / w;
-          const float s2 = dw - su * u - sv * v;
-#pragma unroll
-          for (int a = 0; a < 3; ++a) g[a] = c.m[a] * su + c.m[4 + a] * sv + c.m[8 + a] * s2;
-        }
-#pragma unroll
-        for (int a = 0; a < 3; ++a) dp[a * gp.ld_dp] = g[a];
-      }
-    }
-    __syncthreads();
-  }
-}
-
-template <int P>
-int launch_grad(const Fp32Params& prm, const GradParams& gp, const MpPointSrc& src, const MpCalib& cal, cudaStream_t st,
-                int sm_count, int max_smem) {
-  const size_t smem = GradSmem<P>::bytes(prm.c0, prm.h_ping, prm.h_pong, gp.mask_words, prm.cout[prm.n_layers - 1]);
-  const int opt_in = max_smem - 2048;             // one device-wide bound, as in launch() below
-  static thread_local bool opted[64] = {};
-  int dev_ = 0;
-  MP_CUDA(cudaGetDevice(&dev_));
-  if (dev_ < 0 || dev_ >= 64 || !opted[dev_]) {
-    MP_CUDA(cudaFuncSetAttribute(query_grad_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
-    if (dev_ >= 0 && dev_ < 64) opted[dev_] = true;
-  }
-  const long long tiles = (src.n + P - 1) / P;
-  const int grid = (int)(tiles < (long long)sm_count ? (tiles > 0 ? tiles : 1) : sm_count);
-#ifndef MP_CUDA_EMU
-  query_grad_kernel<P><<<grid, kThreads, smem, st>>>(prm, gp, src, cal);
-#else
-  MP_EMU_LAUNCH(grid, kThreads, query_grad_kernel<P>(prm, gp, src, cal));
-#endif
-  MP_CUDA(cudaGetLastError());
-  return MP_OK;
-}
-
-// ---- F1'''': the vector-Jacobian product of the query, for training ------------------------------------------------------
-// query_grad_kernel's tile steps over the B * ceil(n / P) tiles of a batch (tile t of image t / ceil(n / P), as
-// query_fp32_kernel maps them), for the tiles [vp.tile0, vp.tile1) of one chunk.  Besides d points it can
+// query_vjp_kernel runs these steps over the B * ceil(n / P) tiles of a batch (tile t of image t / ceil(n / P), as
+// query_fp32_kernel maps them), for the tiles [vp.tile0, vp.tile1) of one chunk.  n is src.n, or the count on the device
+// when src.count_dev is set (single-map launches: the tile bound follows the count); the range guard skips an image as in
+// query_fp32_kernel.  Besides d points it can
 //   - save the rows the weight gradient contracts: the input X and every hidden activation in the forward half, every δ_l
 //     (the last layer's g included) in the reverse half -- column (t - tile0) * P + p of vp.rows (query_vjp.cu sums them);
 //   - scatter dX[:C] of each in-image point onto its four taps with grid_sample's weights (atomicAdd into [B][H][W][C]).
@@ -646,12 +472,21 @@ query_vjp_kernel(Fp32Params prm, MpVjpParams vp, MpPointSrc src, MpCalib cal, Mp
   const int warp = tid >> 5, lane = tid & 31;
   const int L = prm.n_layers;
   const int res = prm.cout[L - 1];
-  const long long n = src.n;
+  long long n = src.n;
+  if (src.count_dev) {                               // (the point count on the device: src.n is then the capacity)
+    const long long c = *src.count_dev;
+    n = c < n ? c : n;
+  }
   const long long n_tiles = (n + P - 1) / P;         // (per image)
+  const long long tile1 = vp.tile1 < n_tiles * bt.B ? vp.tile1 : n_tiles * bt.B;
   const bool need_dx = vp.dp || vp.dfeat;            // (else the reverse pass stops at δ_0)
 
-  for (long long at = vp.tile0 + blockIdx.x; at < vp.tile1; at += gridDim.x) {
+  for (long long at = vp.tile0 + blockIdx.x; at < tile1; at += gridDim.x) {
     const int b = mp_tile_image(bt, at, n_tiles);
+    if (mp_guard_skips(prm.amax + b, prm.amax_limit, prm.guard)) {      // (uniform over the CTA)
+      at = mp_skip_image(bt, at, b, n_tiles);
+      continue;
+    }
     const long long p0 = (at - (long long)b * n_tiles) * P;
     const float* feat = prm.feat + (size_t)b * prm.H * prm.W * prm.C;
     float* rows = vp.rows ? vp.rows + (at - vp.tile0) * P : nullptr;
@@ -711,61 +546,59 @@ query_vjp_kernel(Fp32Params prm, MpVjpParams vp, MpPointSrc src, MpCalib cal, Mp
   }
 }
 
-template <int P>
-int launch_vjp(const Fp32Params& prm, const MpVjpParams& vp, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
-               cudaStream_t st, int sm_count, int max_smem) {
-  const size_t smem = GradSmem<P>::bytes(prm.c0, prm.h_ping, prm.h_pong, vp.mask_words, prm.cout[prm.n_layers - 1]);
-  const int opt_in = max_smem - 2048;             // one device-wide bound, as in launch() below
-  static thread_local bool opted[64] = {};
-  int dev_ = 0;
-  MP_CUDA(cudaGetDevice(&dev_));
-  if (dev_ < 0 || dev_ >= 64 || !opted[dev_]) {
-    MP_CUDA(cudaFuncSetAttribute(query_vjp_kernel<P>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
-    if (dev_ >= 0 && dev_ < 64) opted[dev_] = true;
+// ---- host side ------------------------------------------------------------------------------------------------------------
+struct DeviceLimits {
+  int sms, max_smem;            // SM count, shared-memory opt-in limit per block
+};
+
+// The shared memory of a head's tiles: the widest even and odd hidden layers (the ping / pong blocks sA / sB) and, for the
+// reverse pass, the sign-mask words per point of the hidden layers (mask_off[l]: the words before hidden layer l's).
+struct HeadLayout {
+  int c0, ping, pong, res;
+  int mask_words, mask_off[MP_MAX_LAYERS];
+  // bytes of a P-point tile: sX, sA, sB and sMeta [8][P]; the reverse pass adds sMask and sG [res][P]
+  size_t tile_bytes(int P, bool reverse) const {
+    return (size_t)(c0 + ping + pong + 8 + (reverse ? mask_words + res : 0)) * P * sizeof(float);
   }
-  const long long tiles = vp.tile1 - vp.tile0;
-  const int grid = (int)(tiles < (long long)sm_count ? (tiles > 0 ? tiles : 1) : sm_count);
-#ifndef MP_CUDA_EMU
-  query_vjp_kernel<P><<<grid, kThreads, smem, st>>>(prm, vp, src, cal, bt);
-#else
-  MP_EMU_LAUNCH(grid, kThreads, query_vjp_kernel<P>(prm, vp, src, cal, bt));
-#endif
-  MP_CUDA(cudaGetLastError());
+  // the largest tile of 32, 16 or 8 points that fits beside the 2 KB kept for the kernels' static shared memory; 0: none
+  int fit_tile(bool reverse, int max_smem) const {
+    for (int P = 32; P >= 8; P /= 2)
+      if (tile_bytes(P, reverse) + 2048 <= (size_t)max_smem) return P;
+    return 0;
+  }
+};
+
+HeadLayout head_layout(const mp_mlp* mlp) {
+  HeadLayout h;
+  memset(&h, 0, sizeof(h));
+  h.c0 = mlp->channels[0];
+  h.res = mlp->cout[mlp->n_layers - 1];
+  for (int l = 0; l + 1 < mlp->n_layers; ++l) {
+    int& width = l % 2 == 0 ? h.ping : h.pong;
+    width = width > mlp->cout[l] ? width : mlp->cout[l];
+    h.mask_off[l] = h.mask_words;
+    h.mask_words += (mlp->cout[l] + 31) / 32;
+  }
+  return h;
+}
+
+// the current device's limits, read once per device and thread
+int device_limits(DeviceLimits& dev) {
+  static thread_local DeviceLimits cached[64] = {};
+  int d = 0;
+  MP_CUDA(cudaGetDevice(&d));
+  if (d >= 0 && d < 64 && cached[d].sms) {
+    dev = cached[d];
+    return MP_OK;
+  }
+  MP_CUDA(cudaDeviceGetAttribute(&dev.sms, cudaDevAttrMultiProcessorCount, d));
+  MP_CUDA(cudaDeviceGetAttribute(&dev.max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, d));
+  if (d >= 0 && d < 64) cached[d] = dev;
   return MP_OK;
 }
 
-template <int P, bool SURF = false>
-int launch(const Fp32Params& prm, const MpPointSrc& src, const MpCalib& cal, const MpOutDst& dst, cudaStream_t st,
-           int sm_count, int max_smem, const MpBatch& bt, const MpSurfaceSrc& surf = MpSurfaceSrc()) {
-  const size_t smem = Fp32Smem<P>::bytes(prm.c0, prm.h_ping, prm.h_pong);
-  // The opt-in is a property of the kernel, shared by every thread, and heads of different widths launch the same
-  // instantiation with different sizes: it is always set to the same bound -- the device's maximum less the 2 KB the size
-  // selection below keeps free for the kernel's static shared memory -- so no thread lowers it under another thread's
-  // launch.  (Sticky per device: raising it again for every launch costs a driver call per query.)
-  const int opt_in = max_smem - 2048;
-  static thread_local bool opted[64] = {};
-  int dev_ = 0;
-  MP_CUDA(cudaGetDevice(&dev_));
-  if (dev_ < 0 || dev_ >= 64 || !opted[dev_]) {
-    MP_CUDA(cudaFuncSetAttribute(query_fp32_kernel<P, SURF>, cudaFuncAttributeMaxDynamicSharedMemorySize, opt_in));
-    if (dev_ >= 0 && dev_ < 64) opted[dev_] = true;
-  }
-  long long tiles = bt.B * ((src.n + P - 1) / P);
-  int grid = (int)(tiles < (long long)sm_count ? (tiles > 0 ? tiles : 1) : sm_count);
-#ifndef MP_CUDA_EMU
-  query_fp32_kernel<P, SURF><<<grid, kThreads, smem, st>>>(prm, src, cal, dst, bt, surf);
-#else
-  // tests/emu: CPU model of the execution model
-  MP_EMU_LAUNCH(grid, kThreads, (query_fp32_kernel<P, SURF>(prm, src, cal, dst, bt, surf)));
-#endif
-  MP_CUDA(cudaGetLastError());
-  return MP_OK;
-}
-
-}  // namespace
-
-// Fp32Params of a head and a map, and the device's SM count and shared-memory opt-in limit (both kernels)
-static int fill_params(const mp_mlp* mlp, const mp_feat* feat, Fp32Params& prm, int& sms, int& max_smem) {
+// Fp32Params of a head and a map, with the range guard `guard` on the map's maxima; the head's layout; the device's limits
+int fill_params(const mp_mlp* mlp, const mp_feat* feat, int guard, Fp32Params& prm, HeadLayout& h, DeviceLimits& dev) {
   memset(&prm, 0, sizeof(prm));
   prm.n_layers = mlp->n_layers;
   prm.c0 = mlp->channels[0];
@@ -774,17 +607,12 @@ static int fill_params(const mp_mlp* mlp, const mp_feat* feat, Fp32Params& prm, 
     mp_set_error("head expects %d input channels but the feature map has %d (+1 depth)", prm.c0, feat->C);
     return MP_E_INVALID;
   }
-  int ping = 0, pong = 0;
   for (int l = 0; l < mlp->n_layers; ++l) {
     prm.cin[l] = mlp->cin[l];
     prm.cout[l] = mlp->cout[l];
     prm.hid[l] = (l == 0) ? 0 : mlp->channels[l];
     prm.wt[l] = mlp->wt[l];
     prm.bias[l] = mlp->bias[l];
-    if (l < mlp->n_layers - 1) {
-      if (l % 2 == 0) ping = ping > mlp->cout[l] ? ping : mlp->cout[l];
-      else pong = pong > mlp->cout[l] ? pong : mlp->cout[l];
-    }
     if (l > 0 && !mlp->skip) {
       mp_set_error("no_residual heads are not supported");
       return MP_E_UNSUPPORTED;
@@ -792,42 +620,83 @@ static int fill_params(const mp_mlp* mlp, const mp_feat* feat, Fp32Params& prm, 
   }
   prm.w_last = mlp->w[mlp->n_layers - 1];
   prm.last_op = mlp->last_op;
-  prm.h_ping = ping; prm.h_pong = pong;
+  h = head_layout(mlp);
+  prm.h_ping = h.ping; prm.h_pong = h.pong;
   prm.feat = feat->nhwc32;
-  int dev = 0;
-  sms = 148; max_smem = 0;
-  MP_CUDA(cudaGetDevice(&dev));
-  {
-    static thread_local int c_sms[64] = {}, c_smem[64] = {};
-    if (dev >= 0 && dev < 64 && c_sms[dev]) { sms = c_sms[dev]; max_smem = c_smem[dev]; }
-    else {
-      MP_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-      MP_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-      if (dev >= 0 && dev < 64) { c_sms[dev] = sms; c_smem[dev] = max_smem; }
-    }
+  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
+  return device_limits(dev);
+}
+
+// One launch of Kernel, an exact kernel whose tiles are P points, on min(tiles, SMs) CTAs (at least one) with `smem` bytes
+// of dynamic shared memory.  The opt-in is a property of the kernel instantiation, shared by every thread, and heads of
+// different widths launch the same instantiation with different sizes: it is always set to the same bound -- the device's
+// maximum less the 2 KB HeadLayout::fit_tile keeps free for the kernel's static shared memory -- so no thread lowers it
+// under another thread's launch.  (Sticky per device, and recorded per instantiation: Kernel is a template argument, so each
+// one has its own `opted`.  Raising it again for every launch costs a driver call per query.)
+template <int P, auto Kernel, class... Args>
+int launch(long long tiles, size_t smem, const DeviceLimits& dev, cudaStream_t st, const Args&... args) {
+  static thread_local bool opted[64] = {};
+  int d = 0;
+  MP_CUDA(cudaGetDevice(&d));
+  if (d < 0 || d >= 64 || !opted[d]) {
+    MP_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dev.max_smem - 2048));
+    if (d >= 0 && d < 64) opted[d] = true;
   }
+  const int grid = (int)(tiles < (long long)dev.sms ? (tiles > 0 ? tiles : 1) : dev.sms);
+#ifndef MP_CUDA_EMU
+  Kernel<<<grid, kThreads, smem, st>>>(args...);
+#else
+  // tests/emu: CPU model of the execution model
+  MP_EMU_LAUNCH(grid, kThreads, Kernel(args...));
+#endif
+  MP_CUDA(cudaGetLastError());
   return MP_OK;
 }
+
+// query_fp32_kernel over bt.B images of src.n points
+template <bool SURF>
+int launch_query(const Fp32Params& prm, const HeadLayout& h, const DeviceLimits& dev, const MpPointSrc& src, const MpCalib& cal,
+                 const MpOutDst& dst, const MpBatch& bt, const MpSurfaceSrc& surf, cudaStream_t st) {
+  const int P = h.fit_tile(false, dev.max_smem);
+  if (!P) {
+    mp_set_error("head too wide for the fp32 kernel's shared-memory tiling");
+    return MP_E_UNSUPPORTED;
+  }
+  const long long tiles = bt.B * ((src.n + P - 1) / P);
+  const size_t smem = h.tile_bytes(P, false);
+  if (P == 32) return launch<32, query_fp32_kernel<32, SURF>>(tiles, smem, dev, st, prm, src, cal, dst, bt, surf);
+  if (P == 16) return launch<16, query_fp32_kernel<16, SURF>>(tiles, smem, dev, st, prm, src, cal, dst, bt, surf);
+  return launch<8, query_fp32_kernel<8, SURF>>(tiles, smem, dev, st, prm, src, cal, dst, bt, surf);
+}
+
+// the VJP kernel's tile for this head on the current device, or an MP_E_* code (`what` names the kernel in the refusal)
+int reverse_tile(const mp_mlp* mlp, const char* what) {
+  DeviceLimits dev;
+  const int rc = device_limits(dev);
+  if (rc != MP_OK) return rc;
+  const int P = head_layout(mlp).fit_tile(true, dev.max_smem);
+  if (!P) {
+    mp_set_error("head too wide for the %s's shared-memory tiling", what);
+    return MP_E_UNSUPPORTED;
+  }
+  return P;
+}
+
+}  // namespace
 
 int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const MpOutDst& dst, cudaStream_t st, int guard, const MpBatch* bt) {
   if (src.n <= 0) return MP_OK;
   Fp32Params prm;
-  int sms = 0, max_smem = 0;
-  const int rc = fill_params(mlp, feat, prm, sms, max_smem);
+  HeadLayout h;
+  DeviceLimits dev;
+  const int rc = fill_params(mlp, feat, guard, prm, h, dev);
   if (rc != MP_OK) return rc;
-  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
-  const int ping = prm.h_ping, pong = prm.h_pong;
   if (bt && bt->B > 1 && (src.kind != MP_SRC_ROWS || dst.scatter_vol || dst.n_peers > 0 || !dst.out)) {
     mp_set_error("batched launches take point rows and write [R,N] outputs");
     return MP_E_UNSUPPORTED;
   }
-  const MpBatch& b = bt ? *bt : MpBatch();
-  if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32>(prm, src, cal, dst, st, sms, max_smem, b);
-  if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16>(prm, src, cal, dst, st, sms, max_smem, b);
-  if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8>(prm, src, cal, dst, st, sms, max_smem, b);
-  mp_set_error("head too wide for the fp32 kernel's shared-memory tiling");
-  return MP_E_UNSUPPORTED;
+  return launch_query<false>(prm, h, dev, src, cal, dst, bt ? *bt : MpBatch(), MpSurfaceSrc(), st);
 }
 
 int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfaceSrc& surf, long long n, const MpCalib& cal,
@@ -842,23 +711,18 @@ int mp_launch_surface_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpSurfa
     return MP_E_UNSUPPORTED;
   }
   Fp32Params prm;
-  int sms = 0, max_smem = 0;
-  const int rc = fill_params(mlp, feat, prm, sms, max_smem);
+  HeadLayout h;
+  DeviceLimits dev;
+  const int rc = fill_params(mlp, feat, guard, prm, h, dev);
   if (rc != MP_OK) return rc;
-  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
   MpPointSrc src;
   memset(&src, 0, sizeof(src));
   src.kind = MP_SRC_ROWS;
   src.n = n;
   MpOutDst dst;
   dst.out = nullptr; dst.ld = 0; dst.scatter_vol = nullptr;
-  const MpBatch one = bt ? *bt : MpBatch();         // (one map, its camera in device memory when one.calibs is set)
-  const int ping = prm.h_ping, pong = prm.h_pong;
-  if (Fp32Smem<32>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<32, true>(prm, src, cal, dst, st, sms, max_smem, one, surf);
-  if (Fp32Smem<16>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<16, true>(prm, src, cal, dst, st, sms, max_smem, one, surf);
-  if (Fp32Smem<8>::bytes(prm.c0, ping, pong) + 2048 <= (size_t)max_smem) return launch<8, true>(prm, src, cal, dst, st, sms, max_smem, one, surf);
-  mp_set_error("head too wide for the fp32 kernel's shared-memory tiling");
-  return MP_E_UNSUPPORTED;
+  // (one map, its camera in device memory when bt->calibs is set)
+  return launch_query<true>(prm, h, dev, src, cal, dst, bt ? *bt : MpBatch(), surf, st);
 }
 
 int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
@@ -869,90 +733,42 @@ int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
     mp_set_error("the gradient kernel takes point rows of one map");
     return MP_E_UNSUPPORTED;
   }
-  Fp32Params prm;
-  int sms = 0, max_smem = 0;
-  const int rc = fill_params(mlp, feat, prm, sms, max_smem);
-  if (rc != MP_OK) return rc;
-  prm.amax = feat->amax; prm.amax_limit = mlp->tc_amax_limit; prm.guard = guard;
-  GradParams gp;
-  memset(&gp, 0, sizeof(gp));
-  int words = 0;
-  for (int l = 0; l < mlp->n_layers; ++l) {
-    gp.w[l] = mlp->w[l];
-    gp.mask_off[l] = words;                      // (mask words per point here; scaled to words of a P-point tile below)
-    if (l < mlp->n_layers - 1) words += (mlp->cout[l] + 31) / 32;
-  }
-  gp.mask_words = words;
-  gp.grad_out = grad_out; gp.ld_grad = ld_grad;
-  gp.dp = dpoints; gp.ld_dp = ld_dp;
-  gp.calib = bt ? bt->calibs : nullptr;
   if (out) {                                      // the value: query_fp32_kernel's own, bit for bit
     MpOutDst dst;
     dst.out = out; dst.ld = ld_out; dst.scatter_vol = nullptr;
     const int rq = mp_launch_query_fp32(mlp, feat, src, cal, dst, st, guard, bt);
     if (rq != MP_OK) return rq;
   }
-  const int res = prm.cout[prm.n_layers - 1];
-  auto fits = [&](size_t bytes) { return bytes + 2048 <= (size_t)max_smem; };
-  auto scaled = [&](int P) {
-    GradParams g = gp;
-    for (int l = 0; l < mlp->n_layers; ++l) g.mask_off[l] = gp.mask_off[l] * P;
-    return g;
-  };
-  if (fits(GradSmem<32>::bytes(prm.c0, prm.h_ping, prm.h_pong, words, res))) return launch_grad<32>(prm, scaled(32), src, cal, st, sms, max_smem);
-  if (fits(GradSmem<16>::bytes(prm.c0, prm.h_ping, prm.h_pong, words, res))) return launch_grad<16>(prm, scaled(16), src, cal, st, sms, max_smem);
-  if (fits(GradSmem<8>::bytes(prm.c0, prm.h_ping, prm.h_pong, words, res))) return launch_grad<8>(prm, scaled(8), src, cal, st, sms, max_smem);
-  mp_set_error("head too wide for the gradient kernel's shared-memory tiling");
-  return MP_E_UNSUPPORTED;
+  const int P = reverse_tile(mlp, "gradient kernel");
+  if (P < 0) return P;
+  MpVjpParams vp;                                 // d points of every tile of the map; no rows, no feature gradient
+  memset(&vp, 0, sizeof(vp));
+  vp.grad_out = grad_out; vp.ld_grad = ld_grad;
+  vp.dp = dpoints; vp.ld_dp = ld_dp;
+  vp.tile1 = (src.n + P - 1) / P;
+  return mp_launch_query_vjp_tiles(mlp, feat, src, cal, bt ? *bt : MpBatch(), vp, st, guard);
 }
 
-// the VJP kernel's tile: the largest P of 32, 16, 8 whose shared memory fits (query_grad_kernel's footprint); 0: too wide
-static int vjp_tile(const mp_mlp* mlp, int max_smem) {
-  int ping = 0, pong = 0, words = 0;
-  for (int l = 0; l + 1 < mlp->n_layers; ++l) {
-    if (l % 2 == 0) ping = ping > mlp->cout[l] ? ping : mlp->cout[l];
-    else pong = pong > mlp->cout[l] ? pong : mlp->cout[l];
-    words += (mlp->cout[l] + 31) / 32;
-  }
-  const int c0 = mlp->channels[0], res = mlp->cout[mlp->n_layers - 1];
-  if (GradSmem<32>::bytes(c0, ping, pong, words, res) + 2048 <= (size_t)max_smem) return 32;
-  if (GradSmem<16>::bytes(c0, ping, pong, words, res) + 2048 <= (size_t)max_smem) return 16;
-  if (GradSmem<8>::bytes(c0, ping, pong, words, res) + 2048 <= (size_t)max_smem) return 8;
-  return 0;
-}
-
-int mp_query_vjp_tile(const mp_mlp* mlp) {
-  int dev = 0, max_smem = 0;
-  MP_CUDA(cudaGetDevice(&dev));
-  MP_CUDA(cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  const int P = vjp_tile(mlp, max_smem);
-  if (!P) {
-    mp_set_error("head too wide for the VJP kernel's shared-memory tiling");
-    return MP_E_UNSUPPORTED;
-  }
-  return P;
-}
+int mp_query_vjp_tile(const mp_mlp* mlp) { return reverse_tile(mlp, "VJP kernel"); }
 
 int mp_launch_query_vjp_tiles(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
-                              const MpBatch& bt, const MpVjpParams& outs, cudaStream_t st) {
+                              const MpBatch& bt, const MpVjpParams& outs, cudaStream_t st, int guard) {
   Fp32Params prm;
-  int sms = 0, max_smem = 0;
-  const int rc = fill_params(mlp, feat, prm, sms, max_smem);
+  HeadLayout h;
+  DeviceLimits dev;
+  const int rc = fill_params(mlp, feat, guard, prm, h, dev);
   if (rc != MP_OK) return rc;
-  prm.guard = MP_GUARD_NONE;
+  const int P = mp_query_vjp_tile(mlp);
+  if (P < 0) return P;
   MpVjpParams vp = outs;
-  int words = 0;
   for (int l = 0; l < mlp->n_layers; ++l) {
     vp.w[l] = mlp->w[l];
-    vp.mask_off[l] = words;                      // (words per point here; scaled to words of a P-point tile below)
-    if (l < mlp->n_layers - 1) words += (mlp->cout[l] + 31) / 32;
+    vp.mask_off[l] = h.mask_off[l] * P;           // (in words of a P-point tile)
   }
-  vp.mask_words = words;
-  const int P = vjp_tile(mlp, max_smem);
-  for (int l = 0; l < mlp->n_layers; ++l) vp.mask_off[l] *= P;
-  if (P == 32) return launch_vjp<32>(prm, vp, src, cal, bt, st, sms, max_smem);
-  if (P == 16) return launch_vjp<16>(prm, vp, src, cal, bt, st, sms, max_smem);
-  if (P == 8) return launch_vjp<8>(prm, vp, src, cal, bt, st, sms, max_smem);
-  mp_set_error("head too wide for the VJP kernel's shared-memory tiling");
-  return MP_E_UNSUPPORTED;
+  vp.mask_words = h.mask_words;
+  const long long tiles = vp.tile1 - vp.tile0;
+  const size_t smem = h.tile_bytes(P, true);
+  if (P == 32) return launch<32, query_vjp_kernel<32>>(tiles, smem, dev, st, prm, vp, src, cal, bt);
+  if (P == 16) return launch<16, query_vjp_kernel<16>>(tiles, smem, dev, st, prm, vp, src, cal, bt);
+  return launch<8, query_vjp_kernel<8>>(tiles, smem, dev, st, prm, vp, src, cal, bt);
 }

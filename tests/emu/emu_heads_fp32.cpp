@@ -13,7 +13,7 @@
 // no_residual head.  in.bin as for emu_query_fp32 (the header's res is the last width), with the weights of these widths.
 // Every launch prints "launch P=<tile size>" on stdout: the instantiation the launcher's shared-memory fit chose.
 
-// both launch sites (launch<P> and launch_grad<P>) expand this inside their template: P is the tile size they launch
+// the launcher (launch<P, Kernel>) expands this inside its template: P is the tile size it launches
 #define MP_EMU_LAUNCH(grid, block, call)                                                                                 \
   (printf("launch P=%d\n", P), cuda_emu::launch(dim3((unsigned)(grid)), dim3((unsigned)(block)), [&] { call; }))
 #include "emu_host.h"

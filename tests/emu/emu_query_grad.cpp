@@ -1,8 +1,11 @@
-// TEST INFRASTRUCTURE ONLY: the gradient kernel of monoport_b200/csrc/query_fp32.cu (query_grad_kernel) compiled unmodified
-// on the CPU emulation layer.
+// TEST INFRASTRUCTURE ONLY: the exact point gradient of monoport_b200/csrc/query_fp32.cu (mp_launch_query_grad: the value
+// by query_fp32_kernel, d points by query_vjp_kernel) compiled unmodified on the CPU emulation layer.
 //   emu_query_grad in.bin out.f32 [sms] [grad_out.f32]
 // in.bin as for emu_query_fp32; grad_out.f32 (optional): [Res][N] fp32, otherwise all ones.  out.f32 = value [Res][N]
-// followed by the point gradient [3][N].  sms = simulated SM count (grid size), default 3.
+// followed by the point gradient [3][N], pre-filled with -4242 (what a guarded launch skips, and the points at or beyond the
+// device-side count, keep it).  sms = simulated SM count (grid size), default 3.  Range guard: EMU_GUARD (sense),
+// EMU_TC_LIMIT (the head's limit, default +inf) and EMU_AMAX (the map's max |feature|); EMU_COUNT=k: the point count on
+// the device (n = N is then the capacity).
 #include "emu_host.h"
 #include "../../monoport_b200/csrc/query_fp32.cu"
 
@@ -20,11 +23,20 @@ int main(int argc, char** argv) {
     fclose(g);
   }
   EmuFeat ef = emu_make_feat(in);
+  const int guard = getenv("EMU_GUARD") ? atoi(getenv("EMU_GUARD")) : MP_GUARD_NONE;
+  const float amax_f = getenv("EMU_AMAX") ? (float)atof(getenv("EMU_AMAX")) : 0.f;
+  memcpy(&ef.amax[0], &amax_f, 4);
+  MpPointSrc src = emu_rows_src(in);
+  int32_t count = 0;
+  if (getenv("EMU_COUNT")) {
+    count = atoi(getenv("EMU_COUNT"));
+    src.count_dev = &count;
+  }
   // one buffer: value [res][N], gradient [3][N], then a sentinel
   std::vector<float> out((size_t)(res + 3) * N + 1, -4242.f);
   float* dp = out.data() + (size_t)res * N;
-  const int rc = mp_launch_query_grad(&m.mlp, &ef.feat, emu_rows_src(in), in.cal, gout.empty() ? nullptr : gout.data(), N,
-                                      out.data(), N, dp, N, nullptr);
+  const int rc = mp_launch_query_grad(&m.mlp, &ef.feat, src, in.cal, gout.empty() ? nullptr : gout.data(), N, out.data(), N,
+                                      dp, N, nullptr, guard);
   if (rc != MP_OK) { fprintf(stderr, "mp_launch_query_grad: %s\n", g_err); return 3; }
   if (out[(size_t)(res + 3) * N] != -4242.f) { fprintf(stderr, "wrote past the output\n"); return 3; }
   emu_write(argv[2], out.data(), (size_t)(res + 3) * N);

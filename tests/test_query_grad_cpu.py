@@ -1,8 +1,8 @@
 """CPU checks of the point gradient of query() (mp_query_points_grad): the differentiable restatement against the reference's
 autograd goldens, and the gradient kernel -- compiled unmodified on the CPU model of tests/emu -- against those goldens, against
-the fp32 query kernel's values bit for bit, across simulated SM counts, and outside the image.  Also the ptxas report of the
-kernel's sm_90a instantiations."""
-import re
+the fp32 query kernel's values bit for bit, across simulated SM counts, outside the image, and under the range guard and a
+device-side point count."""
+import os
 import subprocess
 
 import numpy as np
@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from oracle import spec
-from emu_harness import build, ptxas_report, write_input
+from emu_harness import build, write_input
 from grad_cases import grad_cases, load_grad_case, query_grad_ref, within_bar
 
 
@@ -43,7 +43,7 @@ def _write_input(path, c, n):
     write_input(path, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], c["chans"][-1], c["last_op"], c["Ws"], c["bs"])
 
 
-def _run_grad(emu, tmp_path, c, n, sms=3, tag="g"):
+def _run_grad(emu, tmp_path, c, n, sms=3, tag="g", env=None):
     """-> (value [Res,n], dpoints [3,n]) of the gradient kernel"""
     res = c["chans"][-1]
     fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
@@ -53,7 +53,7 @@ def _run_grad(emu, tmp_path, c, n, sms=3, tag="g"):
         fg = str(tmp_path / ("gout_%s.f32" % tag))
         c["grad_output"][:, :n].contiguous().numpy().astype(np.float32).tofile(fg)
         args.append(fg)
-    r = subprocess.run(args, capture_output=True, text=True, timeout=1800)
+    r = subprocess.run(args, capture_output=True, text=True, timeout=1800, env=dict(os.environ, **(env or {})))
     assert r.returncode == 0, r.stderr[-2000:]
     out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
     assert out.numel() == (res + 3) * n
@@ -106,10 +106,22 @@ def test_kernel_gradient_is_exactly_zero_outside_the_image(emu, tmp_path):
     assert bool((dp[:, ~outside].abs().sum(0) > 0).all())
 
 
-# ---- ptxas report ----------------------------------------------------------------------------------------------------------
-def test_grad_kernel_has_no_spill_and_no_stack_frame():
-    found = {name: " ".join(lines) for name, lines in ptxas_report("query_fp32.cu")[0] if "query_grad_kernel" in name}
-    assert len(found) == 3, list(found)               # P = 32, 16, 8
-    for name, stats in found.items():
-        m = re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads", stats)
-        assert m and m.groups() == ("0", "0", "0"), (name, stats)
+def test_kernel_range_guard_and_device_count(emu, tmp_path):
+    """One map above the head's feature limit and one below: a launch guarded out of range writes the value and d points
+    only for the map above, one guarded in range only for the map below.  The device-side count stops the launch at that
+    point."""
+    c = load_grad_case("g_rot")
+    n = 40
+    full = _run_grad(emu, tmp_path, c, n)
+    for guard, runs_above in (("2", True), ("1", False)):
+        for amax, above in (("2", True), ("0.5", False)):
+            got = _run_grad(emu, tmp_path, c, n, tag="g%s%s" % (guard, amax),
+                            env={"EMU_GUARD": guard, "EMU_TC_LIMIT": "1", "EMU_AMAX": amax})
+            if above == runs_above:
+                assert torch.equal(got[0], full[0]) and torch.equal(got[1], full[1]), (guard, amax)
+            else:
+                assert bool((got[0] == -4242).all()) and bool((got[1] == -4242).all()), (guard, amax)
+    k = 21
+    cut = _run_grad(emu, tmp_path, c, n, tag="cnt", env={"EMU_COUNT": str(k)})
+    assert torch.equal(cut[0][:, :k], full[0][:, :k]) and torch.equal(cut[1][:, :k], full[1][:, :k])
+    assert bool((cut[0][:, k:] == -4242).all()) and bool((cut[1][:, k:] == -4242).all())
