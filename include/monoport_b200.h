@@ -160,8 +160,8 @@ int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const float* point
  * The weight gradients are contracted chunk by chunk from rows the kernel saves in scratch_dev; the feature gradient is
  * gathered in it before its layout step.  scratch_bytes: at least mp_query_points_vjp_scratch_bytes(...) for the same
  * requests; a larger scratch holds larger chunks.  The weight, bias and point gradients are deterministic for one scratch
- * size; the feature gradient is accumulated with atomics (like grid_sample's backward) and is not.  No range guard, no
- * tensor-core variant.  Enqueue-only: nothing is read back to the host. */
+ * size; the feature gradient is accumulated with atomics (like grid_sample's backward) and is not, unless it is asked for
+ * in order (mp_query_points_vjp_ex, MP_VJP_DETERMINISTIC).  No range guard, no tensor-core variant.  Enqueue-only: nothing is read back to the host. */
 int mp_query_points_vjp(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n, int64_t batch_stride,
                         int64_t row_stride, int64_t point_stride, const float* calibs_dev, int projection, float z_scale,
                         const float* grad_out_dev, float* dfeat_dev, float* dpoints_dev, float* const* dweights_dev,
@@ -171,6 +171,22 @@ int mp_query_points_vjp(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* poin
  * the feature / weight gradients are requested (neither: 0 bytes).  Negative: an MP_E_* code. */
 int64_t mp_query_points_vjp_scratch_bytes(mp_mlp_t* mlp, mp_feat_t* feat, int B, int64_t n, int64_t chunk_points, int want_dfeat,
                                           int want_dweights);
+/* flags of mp_query_points_vjp_ex.  MP_VJP_DETERMINISTIC: the feature gradient is summed in a fixed order instead of with
+ * atomics -- per chunk of chunk_points points, the points are sorted by the cell of their nw tap (stably, so in point order
+ * within a cell) and each element of dfeat is summed by one thread over the four cells whose points reach it, in point
+ * order, then added to the previous chunks' sum.  dfeat is then the same bits from run to run and whatever else is
+ * requested, for one chunk size. */
+#define MP_VJP_DETERMINISTIC 1
+/* mp_query_points_vjp and its scratch size with flags (0: exactly the calls above).  With MP_VJP_DETERMINISTIC the scratch
+ * also holds, per chunk, dX[:C], the tap weights and the cell key of every point and the buffers of the sort, and the
+ * feature gradient is chunked by chunk_points whether or not the weight gradients are requested; B * H * W must be below
+ * 2^32 - 1.  Enqueue-only. */
+int mp_query_points_vjp_ex(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n, int64_t batch_stride,
+                           int64_t row_stride, int64_t point_stride, const float* calibs_dev, int projection, float z_scale,
+                           const float* grad_out_dev, float* dfeat_dev, float* dpoints_dev, float* const* dweights_dev,
+                           float* const* dbiases_dev, void* scratch_dev, int64_t scratch_bytes, int flags, void* stream);
+int64_t mp_query_points_vjp_scratch_bytes_ex(mp_mlp_t* mlp, mp_feat_t* feat, int B, int64_t n, int64_t chunk_points,
+                                             int want_dfeat, int want_dweights, int flags);
 /* mp_query_points with an optional point count on the device (count_dev: one int32, or NULL): n is then the capacity and
  * the points at or beyond min(*count_dev, n) are neither read nor written.  Enqueue-only like mp_query_points; the same
  * modes, range guard and kernels.  Single-map handles only. */

@@ -16,6 +16,7 @@ MP_E_TRUNCATED = -7
 MODE_FP32, MODE_TC, MODE_AUTO, MODE_TC_V3 = 0, 1, 2, 4
 LAST_NONE, LAST_SIGMOID, LAST_TANH = 0, 1, 2
 PROJ_ORTHOGONAL, PROJ_PERSPECTIVE = 0, 1
+VJP_DETERMINISTIC = 1
 
 
 class MonoportLibraryError(RuntimeError):
@@ -54,6 +55,10 @@ SIGNATURES = {
     "mp_query_points_vjp": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int,
                                     c_float, c_void_p, c_void_p, c_void_p, P(c_void_p), P(c_void_p), c_void_p, c_int64, c_void_p]),
     "mp_query_points_vjp_scratch_bytes": (c_int64, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_int]),
+    "mp_query_points_vjp_ex": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int,
+                                       c_float, c_void_p, c_void_p, c_void_p, P(c_void_p), P(c_void_p), c_void_p, c_int64, c_int,
+                                       c_void_p]),
+    "mp_query_points_vjp_scratch_bytes_ex": (c_int64, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_int, c_int]),
     "mp_query_points_host":(c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, P(c_float), c_int, c_float,
                                      c_void_p, c_int, c_void_p]),
     "mp_query_grid": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, P(c_float), P(c_float), P(c_float), c_int,

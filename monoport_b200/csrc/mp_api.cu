@@ -407,18 +407,24 @@ extern "C" int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const f
 // ---------------------------------------------------------------------------------------------
 // the vector-Jacobian product of the exact query, for training (query_vjp.cu)
 // ---------------------------------------------------------------------------------------------
-extern "C" int64_t mp_query_points_vjp_scratch_bytes(mp_mlp_t* mlp, mp_feat_t* feat, int B, int64_t n, int64_t chunk_points,
-                                                     int want_dfeat, int want_dweights) {
+extern "C" int64_t mp_query_points_vjp_scratch_bytes_ex(mp_mlp_t* mlp, mp_feat_t* feat, int B, int64_t n, int64_t chunk_points,
+                                                        int want_dfeat, int want_dweights, int flags) {
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE(B == feat->B && n >= 0, "bad batch %d (the handle holds %d maps) or n=%lld", B, feat->B, (long long)n);
-  return mp_vjp_scratch_bytes(mlp, feat, B, n, chunk_points, want_dfeat != 0, want_dweights != 0);
+  MP_REQUIRE((flags & ~MP_VJP_DETERMINISTIC) == 0, "unknown VJP flags %d", flags);
+  return mp_vjp_scratch_bytes(mlp, feat, B, n, chunk_points, want_dfeat != 0, want_dweights != 0, flags);
 }
 
-extern "C" int mp_query_points_vjp(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
-                                   int64_t batch_stride, int64_t row_stride, int64_t point_stride, const float* calibs_dev,
-                                   int projection, float z_scale, const float* grad_out_dev, float* dfeat_dev, float* dpoints_dev,
-                                   float* const* dweights_dev, float* const* dbiases_dev, void* scratch_dev,
-                                   int64_t scratch_bytes, void* stream) {
+extern "C" int64_t mp_query_points_vjp_scratch_bytes(mp_mlp_t* mlp, mp_feat_t* feat, int B, int64_t n, int64_t chunk_points,
+                                                     int want_dfeat, int want_dweights) {
+  return mp_query_points_vjp_scratch_bytes_ex(mlp, feat, B, n, chunk_points, want_dfeat, want_dweights, 0);
+}
+
+extern "C" int mp_query_points_vjp_ex(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
+                                      int64_t batch_stride, int64_t row_stride, int64_t point_stride, const float* calibs_dev,
+                                      int projection, float z_scale, const float* grad_out_dev, float* dfeat_dev,
+                                      float* dpoints_dev, float* const* dweights_dev, float* const* dbiases_dev, void* scratch_dev,
+                                      int64_t scratch_bytes, int flags, void* stream) {
   MpRange nvtx("monoport_b200: F1'''' query VJP");
   MP_REQUIRE(mlp && feat, "NULL handle");
   MP_REQUIRE(B == feat->B, "batch size %d does not match the feature handle's %d maps", B, feat->B);
@@ -443,7 +449,17 @@ extern "C" int mp_query_points_vjp(mp_mlp_t* mlp, mp_feat_t* feat, int B, const 
   bt.pt_stride = batch_stride;
   bt.calibs = calibs_dev;
   return mp_launch_query_vjp(mlp, feat, src, cal, bt, grad_out_dev, dfeat_dev, dpoints_dev, dweights_dev, dbiases_dev, scratch_dev,
-                             scratch_bytes, (cudaStream_t)stream);
+                             scratch_bytes, (cudaStream_t)stream, flags);
+}
+
+extern "C" int mp_query_points_vjp(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
+                                   int64_t batch_stride, int64_t row_stride, int64_t point_stride, const float* calibs_dev,
+                                   int projection, float z_scale, const float* grad_out_dev, float* dfeat_dev, float* dpoints_dev,
+                                   float* const* dweights_dev, float* const* dbiases_dev, void* scratch_dev,
+                                   int64_t scratch_bytes, void* stream) {
+  return mp_query_points_vjp_ex(mlp, feat, B, points_dev, n, batch_stride, row_stride, point_stride, calibs_dev, projection,
+                                z_scale, grad_out_dev, dfeat_dev, dpoints_dev, dweights_dev, dbiases_dev, scratch_dev, scratch_bytes,
+                                0, stream);
 }
 
 // ---------------------------------------------------------------------------------------------

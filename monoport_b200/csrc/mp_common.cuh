@@ -436,6 +436,12 @@ struct MpVjpParams {
   float* dp;                       // null, or d points: image b, coordinate a, point i at dp[b * dp_stride + a * ld_dp + i]
   long long ld_dp, dp_stride;
   float* dfeat;                    // null, or [B][H][W][C] fp32, accumulated with atomicAdd
+  // the ordered feature gradient (query_vjp.cu): when dx_rows is set, dfeat is not touched and column j of the chunk gets
+  // dX[:C] at dx_rows[j * C ..] (in-image points only), its four tap weights at dx_wgt[4 j ..] and its cell key at dx_key[j]:
+  // b * H * W + (the nw tap's texel) for an in-image point, B * H * W for a point at or beyond n or outside the image
+  float* dx_rows;
+  float* dx_wgt;
+  unsigned* dx_key;
   float* rows;                     // null, or the saved rows [act rows ; delta rows][ld_rows] of the chunk's points
   long long ld_rows;
   int act_row[MP_MAX_LAYERS];      // row of hidden layer l's activations (the input X: rows 0 .. c0-1)
@@ -448,14 +454,15 @@ int mp_query_vjp_tile(const mp_mlp* mlp);
 // the count on the device of a single-map launch; bt: the batch); `guard` as for the query launchers
 int mp_launch_query_vjp_tiles(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                               const MpBatch& bt, const MpVjpParams& outs, cudaStream_t st, int guard = MP_GUARD_NONE);
-// the whole VJP (query_vjp.cu): outputs zeroed, then chunk by chunk the kernel and the weight-gradient contraction, then the
-// feature gradient's layout step.  dweights / dbiases: n_layers device pointers each, or null; scratch as sized by
-// mp_vjp_scratch_bytes for the same requests.
+// the whole VJP (query_vjp.cu): outputs zeroed, then chunk by chunk the kernel and the weight-gradient contraction (and, with
+// MP_VJP_DETERMINISTIC in flags, the ordered feature gradient's sort and gather), then the feature gradient's layout step.
+// dweights / dbiases: n_layers device pointers each, or null; scratch as sized by mp_vjp_scratch_bytes for the same requests
+// and flags.
 long long mp_vjp_scratch_bytes(const mp_mlp* mlp, const mp_feat* feat, int B, long long n, long long chunk_points, bool dfeat,
-                               bool dweights);
+                               bool dweights, int flags = 0);
 int mp_launch_query_vjp(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
                         const float* grad_out, float* dfeat_nchw, float* dpoints, float* const* dweights, float* const* dbiases,
-                        void* scratch, long long scratch_bytes, cudaStream_t st);
+                        void* scratch, long long scratch_bytes, cudaStream_t st, int flags = 0);
 // device-side predicate shared by the kernels: true = the tiles of this image (amax = its entry) must do nothing.  In the
 // tensor-core program the weight producer and the consumers both take it, per tile, from the same word.
 __device__ __forceinline__ bool mp_guard_skips(const unsigned* amax, float limit, int guard) {

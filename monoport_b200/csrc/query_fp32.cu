@@ -437,7 +437,8 @@ __device__ __forceinline__ void tile_point_grad(const Fp32Params& prm, const MpP
 // query_fp32_kernel.  Besides d points it can
 //   - save the rows the weight gradient contracts: the input X and every hidden activation in the forward half, every δ_l
 //     (the last layer's g included) in the reverse half -- column (t - tile0) * P + p of vp.rows (query_vjp.cu sums them);
-//   - scatter dX[:C] of each in-image point onto its four taps with grid_sample's weights (atomicAdd into [B][H][W][C]).
+//   - scatter dX[:C] of each in-image point onto its four taps with grid_sample's weights (atomicAdd into [B][H][W][C]), or,
+//     with vp.dx_rows set, record dX[:C], the tap weights and the cell key of each column for query_vjp.cu's ordered gather.
 // It writes no values.
 template <int P>
 __device__ __forceinline__ void save_rows(float* dst, long long ld, const float* src, int rows) {
@@ -530,7 +531,20 @@ query_vjp_kernel(Fp32Params prm, MpVjpParams vp, MpPointSrc src, MpCalib cal, Mp
     }
     // ---- dX -> d points, and dX[:C] -> the four taps of the feature map -----------------------------
     if (vp.dp) tile_point_grad<P>(prm, src, cal, bt, b, feat, p0, n, sX, sMeta, sOff, vp.dp + b * vp.dp_stride, vp.ld_dp);
-    if (vp.dfeat) {
+    if (vp.dx_rows) {
+      // the ordered path: the chunk's columns for the sort and gather of query_vjp.cu, no atomics
+      const long long HW = (long long)prm.H * prm.W;
+      for (int p = warp; p < P; p += kThreads / 32) {
+        const long long col = (at - vp.tile0) * P + p;
+        const bool in = p0 + p < n && sMeta[p] != 0.f;
+        if (in) {
+          float* d = vp.dx_rows + col * prm.C;
+          for (int c = lane; c < prm.C; c += 32) d[c] = sX[(size_t)c * P + p];
+        }
+        if (lane < 4) vp.dx_wgt[col * 4 + lane] = sWgt[lane][p];
+        if (lane == 0) vp.dx_key[col] = (unsigned)(in ? b * HW + sOff[0][p] : bt.B * HW);
+      }
+    } else if (vp.dfeat) {
       float* df = vp.dfeat + (size_t)b * prm.H * prm.W * prm.C;
       for (int p = warp; p < P; p += kThreads / 32) {
         if (p0 + p >= n || sMeta[p] == 0.f) continue;          // outside the image: nothing, anywhere

@@ -12,8 +12,10 @@
 // Determinism: every element of dW / db is owned by one thread of wgrad_kernel, which sums the chunk's points in column
 // order; chunks follow one another on the stream in point order.  For one scratch size (one chunk size) the weight, bias and
 // point gradients are the same bits from run to run.  The feature gradient is accumulated with atomicAdd, like torch's
-// grid_sample backward, and its roundings depend on the order in which the points' taps land.
+// grid_sample backward, and its roundings depend on the order in which the points' taps land -- unless it is requested
+// ordered (MP_VJP_DETERMINISTIC, below): then it is the same bits too, for one chunk size.
 #include "mp_common.cuh"
+#include "mp_scan.cuh"
 
 namespace {
 
@@ -124,6 +126,230 @@ __global__ void __launch_bounds__(256) nhwc_to_nchw_kernel(const float* in, floa
   }
 }
 
+// ---- the ordered feature gradient (MP_VJP_DETERMINISTIC) ------------------------------------------------------------------
+// Per chunk, query_vjp_kernel records column j (one point) as dX[:C], its four tap weights and its cell key: b * H * W plus the
+// texel of its nw tap (always on the map for an in-image point), or B * H * W for a point that contributes nothing.  Then:
+//  1. A stable LSD radix sort of the chunk's columns by key, 8 bits per pass: radix_count_kernel counts the digits of each
+//     block of 2048 columns (shared-memory integer atomics, which only count), the ordered scan of mp_scan.cuh turns the
+//     digit-major [256][blocks] counts into offsets, and radix_scatter_kernel places each block's columns in column order
+//     (ranks from warp ballots).  So within a cell the columns stay in ascending order, whatever the keys.
+//  2. dfeat_gather_kernel: the thread of texel (b, y, x) and channel c owns that element of the [B][H][W][C] buffer.  It
+//     sums, over the cells (y-1, x-1), (y-1, x), (y, x-1), (y, x) in that order -- whose points have the texel as their se,
+//     sw, ne and nw tap -- and within a cell over its columns j in ascending order, with w the weight of that tap:
+//         if (w != 0) s = fmaf(w, dX_j[c], s)            (s = +0 at the start; a tap of weight 0 is off the map)
+//     and adds s to the buffer when some term was taken.  Chunks follow one another on the stream in point order.
+// The feature gradient is then a function of the chunk size alone: not of the SM count, the schedule or the other requests.
+constexpr int kRadixBits = 8;
+constexpr int kRadixBins = 1 << kRadixBits;
+constexpr int kRadixThreads = 256;
+constexpr int kRadixItems = 8;
+constexpr int kRadixBlock = kRadixThreads * kRadixItems;   // columns per CTA
+static_assert(kRadixBins == kRadixThreads, "thread t owns digit t");
+
+// counts[d * nb + block] = the columns of the block whose digit (key >> shift) & 255 is d
+__global__ void __launch_bounds__(kRadixThreads) radix_count_kernel(const unsigned* __restrict__ keys, int n, int shift,
+                                                                    unsigned* __restrict__ counts, int nb) {
+  __shared__ unsigned hist[kRadixBins];
+  hist[threadIdx.x] = 0u;
+  __syncthreads();
+  for (int r = 0; r < kRadixItems; ++r) {
+    const int i = (int)blockIdx.x * kRadixBlock + r * kRadixThreads + (int)threadIdx.x;
+    if (i < n) atomicAdd(&hist[(keys[i] >> shift) & (kRadixBins - 1)], 1u);
+  }
+  __syncthreads();
+  counts[threadIdx.x * nb + blockIdx.x] = hist[threadIdx.x];
+}
+
+// the ordered scan over the digit-major counts
+struct DigitCounts {
+  static constexpr bool kVec8 = false;
+  const unsigned* counts;
+  __device__ unsigned long long operator()(long long i) const { return counts[i]; }
+};
+struct DigitOffsets {
+  unsigned* offsets;
+  __device__ void operator()(long long i, unsigned long long, unsigned long long prefix) const { offsets[i] = (unsigned)prefix; }
+};
+
+// One pass: the block's columns, 256 at a time in column order, go to offsets[d * nb + block] plus their rank among the
+// block's earlier columns of digit d.  vals null: the values are the column indices.
+__global__ void __launch_bounds__(kRadixThreads) radix_scatter_kernel(const unsigned* __restrict__ keys,
+                                                                      const unsigned* __restrict__ vals, int n, int shift,
+                                                                      const unsigned* __restrict__ offsets, int nb,
+                                                                      unsigned* __restrict__ keys_out,
+                                                                      unsigned* __restrict__ vals_out) {
+  constexpr int kWarps = kRadixThreads / 32;
+  __shared__ unsigned base[kRadixBins];              // digit t: where the block's next column of that digit goes
+  __shared__ unsigned wcount[kWarps][kRadixBins];    // per warp: its columns of each digit, then where they start
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  base[tid] = offsets[tid * nb + blockIdx.x];
+  for (int r = 0; r < kRadixItems; ++r) {
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) wcount[w][tid] = 0u;
+    __syncthreads();
+    const int i = (int)blockIdx.x * kRadixBlock + r * kRadixThreads + tid;
+    const bool valid = i < n;
+    const unsigned key = valid ? keys[i] : 0u;
+    const unsigned d = (key >> shift) & (kRadixBins - 1);
+    // the lanes holding the same digit, then this lane's rank among them
+    unsigned peers = __ballot_sync(0xffffffffu, valid);
+#pragma unroll
+    for (int bit = 0; bit < kRadixBits; ++bit) {
+      const unsigned set = __ballot_sync(0xffffffffu, (d >> bit) & 1u);
+      peers &= ((d >> bit) & 1u) ? set : ~set;
+    }
+    const unsigned rank = __popc(peers & ((1u << lane) - 1u));
+    if (valid && rank == 0) wcount[warp][d] = __popc(peers);
+    __syncthreads();
+    unsigned run = base[tid];
+#pragma unroll
+    for (int w = 0; w < kWarps; ++w) {
+      const unsigned c = wcount[w][tid];
+      wcount[w][tid] = run;
+      run += c;
+    }
+    base[tid] = run;
+    __syncthreads();
+    if (valid) {
+      const unsigned dst = wcount[warp][d] + rank;
+      keys_out[dst] = key;
+      vals_out[dst] = vals ? vals[i] : (unsigned)i;
+    }
+    __syncthreads();
+  }
+}
+
+struct GatherParams {
+  const float* dx;             // [cols][C]
+  const float* wgt;            // [cols][4]: nw, ne, sw, se
+  const unsigned* keys;        // the sorted keys
+  const unsigned* cols;        // the columns in that order
+  int n;                       // columns of the chunk
+  float* nhwc;                 // [B][H][W][C]
+  int C, H, W;
+  long long texels;            // B * H * W
+};
+
+// the first of the n sorted keys that is >= k
+__device__ __forceinline__ int lower_bound_key(const unsigned* keys, int n, unsigned k) {
+  int lo = 0, hi = n;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (__ldg(keys + mid) < k) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
+
+// one warp per texel, lanes over channels (the order at the top of this section)
+__global__ void __launch_bounds__(256) dfeat_gather_kernel(GatherParams gp) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long t = (long long)blockIdx.x * 8 + warp;
+  if (t >= gp.texels) return;
+  const long long r = t % ((long long)gp.H * gp.W);
+  const bool up = r >= gp.W, left = r % gp.W != 0;
+  int lo[4], hi[4];
+  bool any = false;
+#pragma unroll
+  for (int a = 0; a < 4; ++a) {
+    const bool ok = a == 0 ? up && left : (a == 1 ? up : (a == 2 ? left : true));
+    const long long cell = t - (a < 2 ? gp.W : 0) - (a % 2 == 0 ? 1 : 0);
+    lo[a] = hi[a] = 0;
+    if (ok) {
+      lo[a] = lower_bound_key(gp.keys, gp.n, (unsigned)cell);
+      hi[a] = lower_bound_key(gp.keys, gp.n, (unsigned)cell + 1u);
+    }
+    any |= lo[a] < hi[a];
+  }
+  if (!any) return;
+  float* out = gp.nhwc + t * gp.C;
+  for (int c = lane; c < gp.C; c += 32) {
+    float s = 0.f;
+    bool took = false;
+#pragma unroll
+    for (int a = 0; a < 4; ++a) {
+      const int tap = 3 - a;                         // se, sw, ne, nw
+      for (int j = lo[a]; j < hi[a]; ++j) {
+        const unsigned col = __ldg(gp.cols + j);
+        const float w = __ldg(gp.wgt + (size_t)col * 4 + tap);
+        if (w == 0.f) continue;
+        s = fmaf(w, __ldg(gp.dx + (size_t)col * gp.C + c), s);
+        took = true;
+      }
+    }
+    if (took) out[c] += s;
+  }
+}
+
+size_t round256(size_t b) { return (b + 255) / 256 * 256; }
+
+// The ordered path's part of the scratch for a chunk of `cols` columns (byte offsets from its start): the scan's words first
+// (total[2], whose ticket total[1] must be zero before the first scan, then the chunk sums), the recorded columns, the two
+// key / column buffers of the sort and the digit counts and offsets.
+struct OrderedLayout {
+  size_t scan, dx, wgt, key[2], col[2], counts, offsets, bytes;
+  int blocks;                  // radix blocks of the chunk
+};
+
+OrderedLayout ordered_layout(long long cols, int C) {
+  OrderedLayout o;
+  size_t at = 0;
+  auto take = [&at](size_t b) {
+    const size_t p = at;
+    at += round256(b);
+    return p;
+  };
+  o.blocks = (int)((cols + kRadixBlock - 1) / kRadixBlock);
+  const long long digits = (long long)kRadixBins * o.blocks;
+  o.scan = take(8 * (size_t)(2 + mpscan::num_blocks(digits)));
+  o.dx = take((size_t)cols * C * sizeof(float));
+  o.wgt = take((size_t)cols * 4 * sizeof(float));
+  for (int k = 0; k < 2; ++k) o.key[k] = take((size_t)cols * sizeof(unsigned));
+  for (int k = 0; k < 2; ++k) o.col[k] = take((size_t)cols * sizeof(unsigned));
+  o.counts = take((size_t)digits * sizeof(unsigned));
+  o.offsets = take((size_t)digits * sizeof(unsigned));
+  o.bytes = at;
+  return o;
+}
+
+// radix passes for keys up to max_key; the sorted keys and columns end in buffer (passes & 1)
+int radix_passes(unsigned long long max_key) {
+  int p = 1;
+  while (p < 4 && (max_key >> (kRadixBits * p)) != 0) ++p;
+  return p;
+}
+
+// the sort of one chunk's n columns (keys in buffer 0)
+int sort_columns(char* area, const OrderedLayout& o, int n, int passes, cudaStream_t st) {
+  unsigned* keys[2] = {reinterpret_cast<unsigned*>(area + o.key[0]), reinterpret_cast<unsigned*>(area + o.key[1])};
+  unsigned* cols[2] = {reinterpret_cast<unsigned*>(area + o.col[0]), reinterpret_cast<unsigned*>(area + o.col[1])};
+  unsigned* counts = reinterpret_cast<unsigned*>(area + o.counts);
+  unsigned* offsets = reinterpret_cast<unsigned*>(area + o.offsets);
+  unsigned long long* total = reinterpret_cast<unsigned long long*>(area + o.scan);
+  const int nb = (n + kRadixBlock - 1) / kRadixBlock;
+  const long long digits = (long long)kRadixBins * nb;
+  const DigitCounts f{counts};
+  const DigitOffsets em{offsets};
+  for (int p = 0; p < passes; ++p) {
+    const int in = p & 1, out = in ^ 1, shift = kRadixBits * p;
+    const unsigned* vals = p == 0 ? nullptr : cols[in];
+#ifndef MP_CUDA_EMU
+    radix_count_kernel<<<nb, kRadixThreads, 0, st>>>(keys[in], n, shift, counts, nb);
+    MP_CUDA(mpscan::scan_emit(f, em, digits, total + 2, total, st));
+    radix_scatter_kernel<<<nb, kRadixThreads, 0, st>>>(keys[in], vals, n, shift, offsets, nb, keys[out], cols[out]);
+#else
+    const int sb = mpscan::num_blocks(digits);
+    MP_EMU_LAUNCH(nb, kRadixThreads, radix_count_kernel(keys[in], n, shift, counts, nb));
+    MP_EMU_LAUNCH(sb, mpscan::kThreads, (mpscan::block_sums_kernel<DigitCounts, mpscan::NoPost>(f, digits, total + 2, sb, total,
+                                                                                              mpscan::NoPost())));
+    MP_EMU_LAUNCH(sb, mpscan::kThreads, (mpscan::emit_kernel<DigitCounts, DigitOffsets>(f, em, digits, total + 2)));
+    MP_EMU_LAUNCH(nb, kRadixThreads, radix_scatter_kernel(keys[in], vals, n, shift, offsets, nb, keys[out], cols[out]));
+#endif
+    MP_CUDA(cudaGetLastError());
+  }
+  return MP_OK;
+}
+
 // the scratch rows of a head: act_row / delta_row (see the top of this file) and their total
 struct RowLayout {
   int act_row[MP_MAX_LAYERS];
@@ -141,35 +367,46 @@ RowLayout row_layout(const mp_mlp* mlp) {
   return r;
 }
 
-size_t round256(size_t b) { return (b + 255) / 256 * 256; }
+// the scratch of one chunk of `chunk` tiles after the NHWC buffer: the saved rows, then the ordered path's part
+size_t chunk_bytes(const RowLayout& rl, int P, int C, bool want_w, bool ordered, long long chunk) {
+  const size_t rows = want_w ? (size_t)rl.total * P * sizeof(float) * (size_t)chunk : 0;
+  return ordered ? round256(rows) + ordered_layout(chunk * P, C).bytes : rows;
+}
+
+// the chunk of a request, in tiles: chunk_points rounded up to tiles (<= 0: every tile), at most every tile
+long long chunk_tiles(long long chunk_points, int P, long long tiles) {
+  const long long chunk = chunk_points > 0 ? (chunk_points + P - 1) / P : tiles;
+  return chunk < tiles ? chunk : tiles;
+}
 
 }  // namespace
 
 long long mp_vjp_scratch_bytes(const mp_mlp* mlp, const mp_feat* feat, int B, long long n, long long chunk_points, bool dfeat,
-                               bool dweights) {
+                               bool dweights, int flags) {
   const int P = mp_query_vjp_tile(mlp);
   if (P < 0) return P;
+  const bool ordered = dfeat && (flags & MP_VJP_DETERMINISTIC);
   size_t bytes = dfeat ? round256((size_t)B * feat->H * feat->W * feat->C * sizeof(float)) : 0;
-  if (dweights) {
+  if (dweights || ordered) {
     const long long tiles = (long long)B * ((n + P - 1) / P);
-    long long chunk = chunk_points > 0 ? (chunk_points + P - 1) / P : tiles;
-    chunk = chunk < tiles ? chunk : tiles;
-    bytes += (size_t)row_layout(mlp).total * P * sizeof(float) * (size_t)chunk;
+    bytes += chunk_bytes(row_layout(mlp), P, feat->C, dweights, ordered, chunk_tiles(chunk_points, P, tiles));
   }
   return (long long)bytes;
 }
 
 int mp_launch_query_vjp(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt,
                         const float* grad_out, float* dfeat_nchw, float* dpoints, float* const* dweights, float* const* dbiases,
-                        void* scratch, long long scratch_bytes, cudaStream_t st) {
+                        void* scratch, long long scratch_bytes, cudaStream_t st, int flags) {
   const int L = mlp->n_layers;
   bool want_w = false;
   for (int l = 0; l < L; ++l) want_w |= (dweights && dweights[l]) || (dbiases && dbiases[l]);
   if (!want_w && !dfeat_nchw && !dpoints) return MP_OK;
+  MP_REQUIRE((flags & ~MP_VJP_DETERMINISTIC) == 0, "unknown VJP flags %d", flags);
   const int P = mp_query_vjp_tile(mlp);
   if (P < 0) return P;
   const long long n = src.n;
   const long long tiles = (long long)bt.B * ((n + P - 1) / P);
+  const bool ordered = dfeat_nchw && (flags & MP_VJP_DETERMINISTIC) && tiles > 0;
   const long long HW = (long long)feat->H * feat->W;
   const size_t dfeat_elems = dfeat_nchw ? (size_t)bt.B * HW * feat->C : 0;
   const size_t dfeat_bytes = round256(dfeat_elems * sizeof(float));
@@ -178,7 +415,22 @@ int mp_launch_query_vjp(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc
   MP_REQUIRE(scratch_bytes >= (long long)dfeat_bytes, "scratch of %lld bytes is smaller than the feature gradient's %lld",
              scratch_bytes, (long long)dfeat_bytes);
   long long chunk = tiles;
-  if (want_w) {
+  if (ordered) {
+    // the largest chunk whose scratch fits: the chunk mp_vjp_scratch_bytes sized for the same requests
+    MP_REQUIRE((unsigned long long)bt.B * HW < 0xFFFFFFFFull, "%d maps of %lld texels: too many cells for the ordered feature gradient",
+               bt.B, HW);
+    const long long room = scratch_bytes - (long long)dfeat_bytes;
+    MP_REQUIRE((long long)chunk_bytes(rl, P, feat->C, want_w, true, 1) <= room,
+               "scratch of %lld bytes holds no chunk (see mp_query_points_vjp_scratch_bytes_ex)", scratch_bytes);
+    long long lo = 1, hi = tiles;
+    while (lo < hi) {
+      const long long mid = lo + (hi - lo + 1) / 2;
+      if ((long long)chunk_bytes(rl, P, feat->C, want_w, true, mid) <= room) lo = mid;
+      else hi = mid - 1;
+    }
+    chunk = lo;
+    MP_REQUIRE(chunk * P < (1ll << 31), "a chunk of %lld points is too large for the ordered feature gradient", chunk * P);
+  } else if (want_w) {
     chunk = (scratch_bytes - (long long)dfeat_bytes) / ((long long)rl.total * P * (long long)sizeof(float));
     MP_REQUIRE(chunk >= 1, "scratch of %lld bytes holds no chunk (%lld bytes per %d points; see mp_query_points_vjp_scratch_bytes)",
                scratch_bytes, (long long)rl.total * P * (long long)sizeof(float), P);
@@ -196,6 +448,18 @@ int mp_launch_query_vjp(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc
   vp.ld_rows = chunk * P;
   memcpy(vp.act_row, rl.act_row, sizeof(vp.act_row));
   memcpy(vp.delta_row, rl.delta_row, sizeof(vp.delta_row));
+  char* area = nullptr;                             // the ordered path's part of the scratch
+  OrderedLayout ol;
+  memset(&ol, 0, sizeof(ol));
+  const int passes = radix_passes((unsigned long long)bt.B * HW);
+  if (ordered) {
+    area = static_cast<char*>(scratch) + dfeat_bytes + round256(want_w ? (size_t)rl.total * P * sizeof(float) * chunk : 0);
+    ol = ordered_layout(chunk * P, feat->C);
+    vp.dx_rows = reinterpret_cast<float*>(area + ol.dx);
+    vp.dx_wgt = reinterpret_cast<float*>(area + ol.wgt);
+    vp.dx_key = reinterpret_cast<unsigned*>(area + ol.key[0]);
+    MP_CUDA(cudaMemsetAsync(area + ol.scan, 0, 16, st));   // the scan's ticket (the scans leave it at zero)
+  }
 
   // outputs: the feature gradient accumulates into the zeroed NHWC buffer, the weight gradients chunk by chunk
   if (nhwc) MP_CUDA(cudaMemsetAsync(nhwc, 0, dfeat_elems * sizeof(float), st));
@@ -234,6 +498,26 @@ int mp_launch_query_vjp(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc
       wgrad_kernel<<<grid_w, 256, 0, st>>>(wp);
 #else
       MP_EMU_LAUNCH(grid_w, 256, wgrad_kernel(wp));
+#endif
+      MP_CUDA(cudaGetLastError());
+    }
+    if (ordered) {
+      const int cols = (int)((vp.tile1 - vp.tile0) * P);
+      const int rs = sort_columns(area, ol, cols, passes, st);
+      if (rs != MP_OK) return rs;
+      GatherParams gp;
+      gp.dx = vp.dx_rows; gp.wgt = vp.dx_wgt;
+      gp.keys = reinterpret_cast<const unsigned*>(area + ol.key[passes & 1]);
+      gp.cols = reinterpret_cast<const unsigned*>(area + ol.col[passes & 1]);
+      gp.n = cols;
+      gp.nhwc = nhwc;
+      gp.C = feat->C; gp.H = feat->H; gp.W = feat->W;
+      gp.texels = (long long)bt.B * HW;
+      const long long grid = (gp.texels + 7) / 8;
+#ifndef MP_CUDA_EMU
+      dfeat_gather_kernel<<<(unsigned)grid, 256, 0, st>>>(gp);
+#else
+      MP_EMU_LAUNCH(grid, 256, dfeat_gather_kernel(gp));
 #endif
       MP_CUDA(cudaGetLastError());
     }

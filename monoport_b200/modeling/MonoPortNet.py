@@ -93,7 +93,8 @@ class _QueryStage(torch.autograd.Function):
         calibs = saved[2] if ctx.has_calibs else None
         want_feat, want_points = ctx.needs_input_grad[1], ctx.needs_input_grad[2]
         want_head = any(ctx.needs_input_grad[4:])
-        dfeat, dpoints, dws, dbs = ctx.net._query_vjp(feat, points, calibs, grad, want_feat, want_points, want_head)
+        dfeat, dpoints, dws, dbs = ctx.net._query_vjp(feat, points, calibs, grad, want_feat, want_points, want_head,
+                                                      torch.are_deterministic_algorithms_enabled())
         dparams = [None] * (len(saved) - (3 if ctx.has_calibs else 2))
         if want_head:
             head = ctx.net.surface_classifier
@@ -275,8 +276,9 @@ class MonoPortNet(nn.Module):
         return out, dp
 
     # ---- training: the differentiable query ---------------------------------------------------------------
-    # points per chunk of the weight-gradient contraction (its scratch: about 16 KB per point for the geometry head); the
-    # weight, bias and point gradients are the same bits from run to run for one chunk size
+    # points per chunk of the weight-gradient contraction (its scratch: about 16 KB per point for the geometry head) and, in
+    # torch's deterministic mode, of the ordered feature gradient; the gradients that are bit-reproducible are so for one
+    # chunk size
     vjp_chunk_points = 8192
 
     def query_stages(self, feats_stages, points, calibs=None, transforms=None):
@@ -285,8 +287,13 @@ class MonoPortNet(nn.Module):
         mode, differentiable with respect to every stage's feature map, the points and the head's `filters.{l}.weight` /
         `filters.{l}.bias`.  The values are the exact fp32 kernel's (query() with precision "fp32", bit for bit); the
         backward is one fused sm_90a VJP launch per chunk of points plus the weight-gradient contraction
-        (mp_query_points_vjp).  The feature gradient is accumulated with atomics (like grid_sample's backward) and so is
-        not bit-reproducible; the others are.  No double backward, no calib gradient."""
+        (mp_query_points_vjp_ex).  The weight, bias and point gradients are bit-reproducible for one `vjp_chunk_points`.
+        The feature gradient is accumulated with atomics (like grid_sample's backward) and so is not -- unless torch's
+        deterministic mode is on (torch.use_deterministic_algorithms(True), read when the backward runs): then it is summed in
+        a fixed order (per chunk of `vjp_chunk_points` points, sorted by cell; DESIGN §F1⁗), the same bits from run to run
+        and whichever other gradients are requested, and the other gradients are the same bits as without it.  That covers
+        the query's share of a training step only: torch flags some ops of the shipped encoders' backward passes (HG's
+        bicubic upsampling, ResBlk's reflection padding) as nondeterministic.  No double backward, no calib gradient."""
         if transforms is not None:
             raise NotImplementedError("`transforms` is not supported (never passed on the recon path, RTL/main.py:179-182)")
         if calibs is not None and calibs.requires_grad:
@@ -349,10 +356,11 @@ class MonoPortNet(nn.Module):
                     "mp_query_points_batch")
         return out
 
-    def _query_vjp(self, feat, points, calibs, grad, want_feat, want_points, want_head):
+    def _query_vjp(self, feat, points, calibs, grad, want_feat, want_points, want_head, deterministic=False):
         """-> (d feat [B,C,H,W] | None, d points [B,3,N] | None, [d W_l [Cout,Cin]] | None, [d b_l] | None) of
-        sum(grad * query) (mp_query_points_vjp).  The map is uploaded again: a query since the forward may have replaced
-        the handle's contents."""
+        sum(grad * query) (mp_query_points_vjp_ex).  deterministic: the feature gradient in a fixed order
+        (MP_VJP_DETERMINISTIC), chunked by `vjp_chunk_points` whatever else is requested; the other gradients are the same
+        bits either way.  The map is uploaded again: a query since the forward may have replaced the handle's contents."""
         B, C, H, W = feat.shape
         n = points.shape[2]
         head = self.surface_classifier
@@ -382,20 +390,21 @@ class MonoPortNet(nn.Module):
             fh.invalidate()
             fh.upload(feat.detach())
             mlp = head.handle()
-            nbytes = lib.mp_query_points_vjp_scratch_bytes(mlp, fh.ptr, B, n, int(self.vjp_chunk_points), int(want_feat),
-                                                           int(want_head))
+            flags = _lib.VJP_DETERMINISTIC if deterministic else 0
+            nbytes = lib.mp_query_points_vjp_scratch_bytes_ex(mlp, fh.ptr, B, n, int(self.vjp_chunk_points), int(want_feat),
+                                                              int(want_head), flags)
             if nbytes < 0:
-                _lib.check(int(nbytes), "mp_query_points_vjp_scratch_bytes")
+                _lib.check(int(nbytes), "mp_query_points_vjp_scratch_bytes_ex")
             scratch = torch.empty(int(nbytes), dtype=torch.uint8, device=dev) if nbytes > 0 else None
             L = len(head.filters)
             ptrs = (lambda ts: None if ts is None else (ctypes.c_void_p * L)(*[t.data_ptr() for t in ts]))
-            _lib.check(lib.mp_query_points_vjp(
+            _lib.check(lib.mp_query_points_vjp_ex(
                 mlp, fh.ptr, B, ctypes.c_void_p(p.data_ptr()), n, s[0], s[1], s[2],
                 None if cal is None else ctypes.c_void_p(cal.data_ptr()), proj, ctypes.c_float(self.normalizer.scale),
                 ctypes.c_void_p(gout.data_ptr()), None if dfeat is None else ctypes.c_void_p(dfeat.data_ptr()),
                 None if dpoints is None else ctypes.c_void_p(dpoints.data_ptr()), ptrs(dws), ptrs(dbs),
-                None if scratch is None else ctypes.c_void_p(scratch.data_ptr()), int(nbytes), _lib.stream_ptr(dev)),
-                "mp_query_points_vjp")
+                None if scratch is None else ctypes.c_void_p(scratch.data_ptr()), int(nbytes), flags, _lib.stream_ptr(dev)),
+                "mp_query_points_vjp_ex")
         return dfeat, dpoints, dws, dbs
 
     def _query_batch(self, feat, points, calibs):
