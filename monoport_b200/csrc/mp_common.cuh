@@ -405,10 +405,11 @@ int mp_launch_query_fp32(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
 int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                        const MpOutDst& dst, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
 // The tensor-core program over the nodes of an MP_SRC_GRID range that project into the image, for a head whose last op is
-// Sigmoid (there a node outside the image has the value 0 * act = +0 exactly).  An ordered compaction lists those nodes and
-// stores +0 for the others into dst (out[i] and / or peer[p][peer_off + i]); the program then runs over the list with a
-// device-side count.  One map, calib by value; the output is the dense launch's bit for bit.  `guard` as above.  scratch:
-// mp_tc_grid_scratch_bytes(grid.n) bytes of device memory whose first 16 are zero (they are left at zero).
+// Sigmoid (there a node outside the image has the value 0 * act = +0 exactly).  An ordered compaction lists those nodes in
+// 4x4x4-brick order and stores +0 for the others into dst (out[i] and / or peer[p][peer_off + i]); the program then runs
+// over the list with a device-side count.  One map, calib by value, R^3 < 2^31; the output is the dense launch's bit for
+// bit.  `guard` as above.  scratch: mp_tc_grid_scratch_bytes(grid.n) bytes of device memory (a bound for every R) whose
+// first 16 are zero (they are left at zero).
 size_t mp_tc_grid_scratch_bytes(long long n);
 int mp_launch_query_tc_grid(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& grid, const MpCalib& cal, const MpOutDst& dst,
                             void* scratch, cudaStream_t st, int guard);

@@ -1504,15 +1504,53 @@ int launch_jvp(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPoint
 }
 
 // ---- the in-image list of a grid range (mp_launch_query_tc_grid), on the ordered scan of mp_scan.cuh
-// f(i) = 1 when node lin0 + i projects into the image.  When the map holds a NaN or an infinity every node counts: the
-// range guard does not send every such frame to the exact kernel (its maximum ignores a NaN), and then 0 * act need not
-// be +0 outside the image.
+// The scan runs over a brick-major index space j: the 4x4x4 bricks of the brick layers that the range's z planes cross,
+// x fastest inside a brick, then the bricks along x, y and z.  So a 64-point tile of the program is one brick wherever a
+// brick lies wholly in the image, and its bilinear taps touch about 3x fewer texels than a run of 64 nodes along an x row
+// (DESIGN.md §F1; tools/tile_texels.py counts them).  The program stores by node, so the order changes no value.
+constexpr int kBrick = 4;   // the edge of a brick, in nodes (kBrick^3 = 64 = the program's tile)
+static_assert(kBrick * kBrick * kBrick == kTile, "a brick is one tile of the program");
+
+struct BrickSpace {
+  int R, rb, bz0;           // nodes per axis, bricks per axis, the first brick layer
+  long long lin0, n, size;  // the range [lin0, lin0 + n) and the number of indices j
+  static BrickSpace of(int R, long long lin0, long long n) {
+    BrickSpace s;
+    s.R = R;
+    s.rb = (R + kBrick - 1) / kBrick;
+    const long long plane = (long long)R * R;
+    s.bz0 = (int)(lin0 / plane) / kBrick;
+    const int layers = (int)((lin0 + n - 1) / plane) / kBrick - s.bz0 + 1;
+    s.lin0 = lin0;
+    s.n = n;
+    s.size = (long long)layers * s.rb * s.rb * (kBrick * kBrick * kBrick);
+    return s;
+  }
+  // the range index (node - lin0) of index j, or -1 for padding past R and for nodes outside the range
+  __device__ __forceinline__ long long node(long long j) const {
+    const int b = (int)(j / (kBrick * kBrick * kBrick)), w = (int)(j % (kBrick * kBrick * kBrick));
+    const int t = b / rb;
+    const int ix = (b - t * rb) * kBrick + w % kBrick;
+    const int iy = (t % rb) * kBrick + (w / kBrick) % kBrick;
+    const int iz = (bz0 + t / rb) * kBrick + w / (kBrick * kBrick);
+    if (ix >= R || iy >= R || iz >= R) return -1;
+    const long long i = ((long long)iz * R + iy) * R + ix - lin0;
+    return i >= 0 && i < n ? i : -1;
+  }
+};
+
+// f(j) = 1 when j's node is in the range and projects into the image.  When the map holds a NaN or an infinity every
+// node of the range counts: the range guard does not send every such frame to the exact kernel (its maximum ignores a
+// NaN), and then 0 * act need not be +0 outside the image.
 struct InImage {
   static constexpr bool kVec8 = false;
+  BrickSpace bs;
   MpPointSrc grid;
   MpCalib cal;
   const unsigned* nonfinite;
-  __device__ unsigned long long operator()(long long i) const {
+  __device__ unsigned long long operator()(long long j) const {
+    const long long i = bs.node(j);
+    if (i < 0) return 0ull;
     if (nonfinite && *nonfinite) return 1ull;
     float x, y, z, u, v, w;
     mp_load_point(grid, MpBatch(), 0, i, x, y, z);
@@ -1520,19 +1558,22 @@ struct InImage {
   }
 };
 
-// a listed node goes to the list at its prefix (ascending node order, so the program's scattered stores stay nearly
-// coalesced); any other node gets the value the dense launch gives it, +0
+// a listed node goes to the list at its prefix (brick order: the program's stores by node are 16-byte runs); any other
+// node of the range gets the value the dense launch gives it, +0
 struct ListOrZero {
+  BrickSpace bs;
   int32_t* list;
   float* out;                       // the range's outputs, or null
   float* peer[MP_MAX_PEERS];
   int n_peers;
-  long long lin0, peer_off;
-  __device__ void operator()(long long i, unsigned long long in, unsigned long long at) const {
+  long long peer_off;
+  __device__ void operator()(long long j, unsigned long long in, unsigned long long at) const {
+    const long long i = bs.node(j);
     if (in) {
-      list[at] = (int32_t)(lin0 + i);
+      list[at] = (int32_t)(bs.lin0 + i);
       return;
     }
+    if (i < 0) return;
     if (out) out[i] = 0.f;
 #pragma unroll
     for (int p = 0; p < MP_MAX_PEERS; ++p)
@@ -1654,8 +1695,14 @@ int mp_launch_query_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, 
                   : launch<512>(mlp, pk, feat, src, cal, dst, st, surf, guard, b);
 }
 
-// scratch of mp_launch_query_tc_grid: total[2] (grand total, ticket), the chunk sums, the count, the list
-static size_t grid_list_offset(long long n) { return 16 + 8 * (size_t)mpscan::num_blocks(n) + 16; }
+// scratch of mp_launch_query_tc_grid: total[2] (grand total, ticket), the chunk sums, the count, the list.  The chunk
+// sums cover the brick space, whose size depends on R and lin0 as well as n; this bounds it for every range of n nodes
+// with R^3 < 2^31 (so R <= 1290): at most ((n - 1) / R^2 + 8) / 4 brick layers of at most 4 (R + 3)^2 indices each,
+// which is under 16 n + 8 * 1293^2 (the factor (R + 3)^2 / R^2 is largest, 16, at R = 1).  That is 1.6 % more than the
+// list, plus 52 KB.
+static size_t grid_list_offset(long long n) {
+  return 16 + 8 * (size_t)mpscan::num_blocks(16 * n + 8ll * 1293 * 1293) + 16;
+}
 
 size_t mp_tc_grid_scratch_bytes(long long n) { return grid_list_offset(n) + 4 * (size_t)n; }
 
@@ -1668,7 +1715,8 @@ int mp_launch_query_tc_grid(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& 
   int C = 0;
   int rc = check_query(mlp, feat, C);
   if (rc != MP_OK) return rc;
-  if (C != 256 || mlp->last_op != MP_LAST_SIGMOID || grid.kind != MP_SRC_GRID || grid.lin0 + n > (1ll << 31) ||
+  if (C != 256 || mlp->last_op != MP_LAST_SIGMOID || grid.kind != MP_SRC_GRID || grid.lin0 < 0 ||
+      grid.lin0 + n > (long long)grid.res * grid.res * grid.res || (long long)grid.res * grid.res * grid.res >= (1ll << 31) ||
       dst.n_peers > MP_MAX_PEERS || (dst.n_peers > 0 && dst.peer_off != grid.lin0) || dst.scatter_vol || dst.peer_by_node) {
     mp_set_error("the in-image grid launch takes a grid range of int32 node indices and a single-output Sigmoid head");
     return MP_E_UNSUPPORTED;
@@ -1677,23 +1725,24 @@ int mp_launch_query_tc_grid(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& 
   // the map's non-finite flag, which the compaction reads, comes with the per-frame products
   rc = frame_products<256>(mlp, pk, feat, st);
   if (rc != MP_OK) return rc;
-  const int nb = mpscan::num_blocks(n);
+  const BrickSpace bs = BrickSpace::of(grid.res, grid.lin0, n);
   unsigned long long* total = static_cast<unsigned long long*>(scratch);
   int32_t* list = reinterpret_cast<int32_t*>(static_cast<uint8_t*>(scratch) + grid_list_offset(n));
   int32_t* count = list - 4;                     // (the 16 bytes before the list)
-  const InImage f{grid, cal, feat->nonfinite};
+  const InImage f{bs, grid, cal, feat->nonfinite};
   ListOrZero em;
+  em.bs = bs;
   em.list = list;
   em.out = dst.out;
   for (int p = 0; p < MP_MAX_PEERS; ++p) em.peer[p] = dst.peer[p];
   em.n_peers = dst.n_peers;
-  em.lin0 = grid.lin0;
   em.peer_off = dst.peer_off;
 #ifndef MP_CUDA_EMU
-  MP_CUDA(mpscan::scan_emit(f, em, n, total + 2, total, st, StoreCount{count}));
+  MP_CUDA(mpscan::scan_emit(f, em, bs.size, total + 2, total, st, StoreCount{count}));
 #else
-  MP_EMU_LAUNCH(nb, mpscan::kThreads, (mpscan::block_sums_kernel<InImage, StoreCount>(f, n, total + 2, nb, total, StoreCount{count})));
-  MP_EMU_LAUNCH(nb, mpscan::kThreads, (mpscan::emit_kernel<InImage, ListOrZero>(f, em, n, total + 2)));
+  const int nb = mpscan::num_blocks(bs.size);
+  MP_EMU_LAUNCH(nb, mpscan::kThreads, (mpscan::block_sums_kernel<InImage, StoreCount>(f, bs.size, total + 2, nb, total, StoreCount{count})));
+  MP_EMU_LAUNCH(nb, mpscan::kThreads, (mpscan::emit_kernel<InImage, ListOrZero>(f, em, bs.size, total + 2)));
 #endif
   MpPointSrc src = grid;                         // (n stays the upper bound of the device-side count)
   src.kind = MP_SRC_NODES;
