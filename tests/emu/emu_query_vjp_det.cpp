@@ -9,7 +9,13 @@
 // [B][C][H][W], d points [B][3][N], d W_l [cout][cin] for every layer, d b_l for every layer (zeros where not requested).
 // EMU_VJP_FLAGS: the flags (default 0).  EMU_VJP_DUMP=path (with MP_VJP_DETERMINISTIC, want f and one chunk): the ordered
 // feature gradient's scratch after the run -- int64 {columns, C}, then fp32 dX rows [columns][C] (zero for a column that
-// contributes nothing), fp32 tap weights [columns][4], the sorted uint32 keys and their columns.
+// contributes nothing), fp32 tap weights [columns][4], the sorted uint32 keys and their columns; and "radix passes <p>" on
+// stdout.
+// EMU_VJP_WMASK / EMU_VJP_BMASK (with want w): bit l set = d W_l / d b_l requested, every other entry of the launcher's
+// dweights / dbiases arrays null (default: all layers).  Either variable fills every d W / d b output with -7 first, so
+// that what the launcher did not write stays -7.
+#include <algorithm>
+
 #include "emu_host.h"
 
 extern "C" cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t) { memset(d, v, n); return cudaSuccess; }
@@ -52,6 +58,16 @@ int main(int argc, char** argv) {
   float* q = dp + n_p;
   for (int l = 0; l < L; ++l) { dw[l] = q; q += (size_t)m.mlp.cout[l] * m.mlp.cin[l]; }
   for (int l = 0; l < L; ++l) { db[l] = q; q += m.mlp.cout[l]; }
+  const char* wmask = getenv("EMU_VJP_WMASK");
+  const char* bmask = getenv("EMU_VJP_BMASK");
+  if (wmask || bmask) {
+    std::fill(dp + n_p, q, -7.f);
+    const long wm = wmask ? atol(wmask) : -1, bm = bmask ? atol(bmask) : -1;
+    for (int l = 0; l < L; ++l) {
+      if (!((wm >> l) & 1)) dw[l] = nullptr;
+      if (!((bm >> l) & 1)) db[l] = nullptr;
+    }
+  }
 
   MpPointSrc src = emu_rows_src(in);
   MpBatch bt;
@@ -74,7 +90,8 @@ int main(int argc, char** argv) {
     const size_t rows = ww ? (size_t)row_layout(&m.mlp).total * P * sizeof(float) * (size_t)(cols / P) : 0;
     const char* area = reinterpret_cast<const char*>(scratch.data()) + round256((size_t)B * HW * in.C * sizeof(float)) + round256(rows);
     const OrderedLayout ol = ordered_layout(cols, in.C);
-    const int sorted = radix_passes((unsigned long long)B * HW) & 1;
+    const int passes = radix_passes((unsigned long long)B * HW), sorted = passes & 1;
+    printf("radix passes %d\n", passes);
     FILE* f = fopen(dump, "wb");
     const long long hd[2] = {cols, in.C};
     fwrite(hd, 8, 2, f);

@@ -57,6 +57,9 @@ HEAD_CASES = [
          calib="rot33", proj="orthogonal", grad=True, amax=None),
     dict(name="p8_full", chans=[1025, 4096, 2071, 1], last_op=S, H=5, W=4, wseed=671, fseed=672, pseed=673, N=72,
          calib="rot33", proj="orthogonal", grad=False, amax=None),
+    # the gradient's tile 8 (the query's too), with several outer passes of the transposed layers
+    dict(name="p8", chans=[65, 3000, 600, 1], last_op=S, H=8, W=11, wseed=721, fseed=722, pseed=723, N=120,
+         calib="rot33", proj="orthogonal", grad=True, amax=None),
     # the shipped widths with the other last ops, the map at 0.99 x the head's default feature limit
     dict(name="sdf", chans=G, last_op=NONE, H=48, W=40, wseed=681, fseed=682, pseed=683, N=520, calib="rot33",
          proj="orthogonal", grad=False, amax=0.99 * 3.0),

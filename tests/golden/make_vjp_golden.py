@@ -45,14 +45,44 @@ VJP_CASES = [
          wseed=441, fseed=442, pseed=443),
     dict(name="narrow_b3_persp", chans=NARROW, last_op="sigmoid", B=3, S=2, N=211, H=20, W=12, calib="persp", gseed=454,
          wseed=451, fseed=452, pseed=453),
+    # heads other than the shipped two on the training path: the reverse tile 8 (several outer passes of the transposed
+    # layers), the reverse tiles 8 / 16 / 32 exactly full (one more unit in the second hidden layer takes the next tile or
+    # is refused), layer inputs with cin % 64 == 0 (the bias alone in wgrad_kernel's last k-tile) and cin % 64 == 63 (the
+    # bias the last column of a full tile), outputs of 64 and 65, no last op, one layer and eight
+    dict(name="p8_b2_persp", chans=[65, 3000, 600, 1], last_op="sigmoid", B=2, S=1, N=77, H=12, W=9, calib="persp",
+         gseed=464, wseed=461, fseed=462, pseed=463),
+    dict(name="p8_full_reverse", chans=[1025, 4096, 1883, 1], last_op="sigmoid", B=1, S=1, N=24, H=5, W=4, calib="rot",
+         gseed=-1, wseed=471, fseed=472, pseed=473),
+    dict(name="p16_full_reverse", chans=[513, 2048, 936, 1], last_op="sigmoid", B=1, S=1, N=40, H=6, W=5, calib="rot",
+         gseed=484, wseed=481, fseed=482, pseed=483),
+    dict(name="p32_full_reverse", chans=[129, 1024, 587, 1], last_op="sigmoid", B=1, S=1, N=50, H=6, W=7, calib="rot",
+         gseed=494, wseed=491, fseed=492, pseed=493),
+    dict(name="odd_b2_persp", chans=[20, 300, 77, 130, 5, 2], last_op="none", B=2, S=1, N=61, H=11, W=6, calib="persp",
+         gseed=504, wseed=501, fseed=502, pseed=503),
+    dict(name="tiles_b1_rot", chans=[127, 64, 65, 2], last_op="tanh", B=1, S=1, N=90, H=9, W=8, calib="rot", gseed=514,
+         wseed=511, fseed=512, pseed=513),
+    dict(name="single_b2_nocalib", chans=[65, 3], last_op="tanh", B=2, S=1, N=53, H=7, W=10, calib="none", gseed=524,
+         wseed=521, fseed=522, pseed=523),
+    dict(name="deep_b1_rot", chans=[40, 32, 32, 33, 31, 64, 16, 8, 1], last_op="sigmoid", B=1, S=1, N=70, H=12, W=5,
+         calib="rot", gseed=534, wseed=531, fseed=532, pseed=533),
+    # maps one texel high or wide (an axis whose scale H - 1 or W - 1 is 0), and B = 3 maps of 5 x 7: fewer texels than one
+    # 32-texel tile of the layout step, and B * H * W = 105 keys, one radix pass of the ordered feature gradient
+    dict(name="row_b1_rot", chans=NARROW, last_op="sigmoid", B=1, S=1, N=120, H=1, W=200, calib="rot", gseed=544,
+         wseed=541, fseed=542, pseed=543),
+    dict(name="col_b2_nocalib", chans=NARROW, last_op="sigmoid", B=2, S=1, N=90, H=200, W=1, calib="none", gseed=554,
+         wseed=551, fseed=552, pseed=553),
+    dict(name="tiny_b3", chans=NARROW, last_op="sigmoid", B=3, S=1, N=45, H=5, W=7, calib="persp", gseed=564, wseed=561,
+         fseed=562, pseed=563),
 ]
+
+LAST_OPS = {"sigmoid": nn.Sigmoid, "tanh": nn.Tanh, "none": lambda: None}
 
 
 def reference_vjp(ns, c, inp, dtype):
     """the reference's train-mode query() over every stage, differentiated by autograd -> (values [S,B,Res,N], grads dict)"""
     net = ns.PIFuNetC() if c["chans"] == spec.C_CHANNELS else ns.PIFuNetG()
     if c["chans"] not in (spec.G_CHANNELS, spec.C_CHANNELS):
-        net.surface_classifier = ns.SurfaceClassifier(c["chans"], 1, False, nn.Sigmoid())
+        net.surface_classifier = ns.SurfaceClassifier(c["chans"], 1, False, LAST_OPS[c["last_op"]]())
     if inp["proj"] == "perspective":
         net.projection = ns.perspective
     net.surface_classifier.load_state_dict(

@@ -94,3 +94,67 @@ def restate_ordered_dfeat(dx, wgt, keys, order, B, H, W):
         if took:
             out[t] = out[t] + s
     return torch.from_numpy(out.reshape(B, H, W, C).transpose(0, 3, 1, 2).copy())
+
+
+# ---- every radix-pass count of the ordered feature gradient ------------------------------------------------------------------
+# a head whose maps have one channel: cheap at every map size
+ONE_CHANNEL = [2, 16, 8, 1]
+
+
+def radix_passes_rule(texels):
+    """the passes of the sort over keys up to B * H * W (the key of a point that contributes nothing): 8 bits each, so
+    1 + #{k in 1..3 : B * H * W >= 2^(8k)}"""
+    return 1 + sum(texels >= 1 << (8 * k) for k in (1, 2, 3))
+
+
+def spread_case(B, N, H, W, chans=ONE_CHANNEL, seed=0, bands=()):
+    """B images of N points, calibs=None: uniform over [-1.1, 1.1]^2 (so some outside the image), the first 8 on the last
+    column, the last row, the far corner and outside, the next N // 4 crowded into one cell (the last row of cells in the
+    last image, the middle one in the others) and, in the last image, N // 8 more in each band (y0, y1) of texel rows.
+    -> the dict of one_cell_case"""
+    g = torch.Generator().manual_seed(2000 + seed)
+    Ws, bs = spec.make_weights(chans, 2010 + seed)
+    feat = torch.cat([spec.make_feat(chans[0] - 1, H, W, 2020 + seed + b) for b in range(B)])
+    pts = (torch.rand(B, 3, N, generator=g) * 2.2 - 1.1).contiguous()
+    for b in range(B):
+        pts[b, :2, :8] = torch.tensor([[1.0, 0.3, 1.0, 1.5, -0.2, 1.0, -1.0, 0.0],
+                                       [-0.1, 1.0, 1.0, 0.0, -1.2, 0.999, 1.0, 1.0]])
+        k = N // 4
+        f = torch.rand(2, k, generator=g, dtype=torch.float64) * 0.9 + 0.05
+        pts[b, 0, 8:8 + k] = cell_coord(W // 3, f[0], W).float()
+        pts[b, 1, 8:8 + k] = cell_coord(H - 2 if b == B - 1 else H // 2, f[1], H).float()
+    o = 8 + N // 4
+    for y0, y1 in bands:
+        k = N // 8
+        y = torch.randint(y0, y1, (k,), generator=g).double()
+        f = torch.rand(2, k, generator=g, dtype=torch.float64)
+        pts[B - 1, 0, o:o + k] = (f[0] * 2 - 1).float()
+        pts[B - 1, 1, o:o + k] = cell_coord(y, f[1], H).clamp(max=1.0).float()
+        o += k
+    assert o <= N
+    gout = torch.randn(B, chans[-1], N, generator=g)
+    return dict(feats=[feat], points=pts, calib=None, Ws=Ws, bs=bs, grad_output=[gout], last_op=spec.LAST_SIGMOID,
+                chans=list(chans), proj="orthogonal")
+
+
+# the GPU's batch-against-alone cases: (B, H, W, N, bands of the last image) -> the passes of the batch and of one image.
+# B = 3 of 2400 x 2400 reaches keys >= 2^24 in the last image's rows from 2191 on: bands above and below that row.
+GPU_RADIX_CASES = {
+    "three_vs_two": (2, 200, 200, 3000, ()),
+    "four_vs_three": (3, 2400, 2400, 4000, ((2191, 2400), (2100, 2191))),
+}
+
+
+def zero_unit_case(seed=0):
+    """the narrow head, calibs=None, where some hidden units have a pre-activation of exactly 0: units 0-7 of layer 0 and
+    0-3 of layer 1 have zero weights and bias (0 at every point), units 8-11 of layer 0 see only the depth feature (0 at
+    the points with z = 0, a quarter of them).  -> (the dict of one_cell_case, {layer: zero rows})"""
+    c = spread_case(2, 400, 16, 20, chans=NARROW, seed=50 + seed)
+    Ws, bs = [w.clone() for w in c["Ws"]], [b.clone() for b in c["bs"]]
+    Ws[0][:12] = 0.0
+    bs[0][:12] = 0.0
+    Ws[0][8:12, -1] = torch.tensor([0.7, -0.4, 1.1, -0.9])
+    Ws[1][:4] = 0.0
+    bs[1][:4] = 0.0
+    c["points"][:, 2, ::4] = 0.0
+    return dict(c, Ws=Ws, bs=bs), {0: list(range(12)), 1: list(range(4))}

@@ -173,12 +173,15 @@ def test_tile_fits_follow_the_device_opt_in():
     shared-memory opt-in, read from the device."""
     optin = _optin()
     cases = [([1025, 512, 255, 1], False), ([1025, 512, 256, 1], False), ([1025, 4096, 2071, 1], False),
-             ([1025, 4096, 2072, 1], False), ([1025, 4096, 2071, 1], True), ([1025, 512, 255, 1], True)]
+             ([1025, 4096, 2072, 1], False), ([1025, 4096, 2071, 1], True), ([1025, 512, 255, 1], True),
+             # the gradient's tiles 32, 16 and 8 exactly full, and one more unit in the second hidden layer
+             ([129, 1024, 587, 1], True), ([129, 1024, 588, 1], True), ([513, 2048, 936, 1], True),
+             ([513, 2048, 937, 1], True), ([1025, 4096, 1883, 1], True), ([1025, 4096, 1884, 1], True)]
     if optin == 232448:
-        assert [fp32_tile(ch, optin, g) for ch, g in cases] == [32, 16, 8, None, None, 16]
-    feat = torch.zeros(1, 1024, 5, 4, device="cuda")
+        assert [fp32_tile(ch, optin, g) for ch, g in cases] == [32, 16, 8, None, None, 16, 32, 16, 16, 8, 8, None]
     pts = torch.zeros(1, 3, 40, device="cuda")
     for chans, grad in cases:
+        feat = torch.zeros(1, chans[0] - 1, 5, 4, device="cuda")
         net = build_head_net(_zero_head(chans))
         call = (lambda: net.query_gradient([[feat]], pts)) if grad else (lambda: net.query([[feat]], pts))
         net.precision = "fp32"

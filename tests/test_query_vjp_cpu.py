@@ -12,7 +12,9 @@ import pytest
 import torch
 
 import emu_harness
+from oracle import spec
 from emu_harness import build, ptxas_report, write_input
+from head_cases import fp32_tile
 from vjp_cases import GRAD_NAMES, flat, golden_bar, load_vjp_case, query_vjp_ref, vjp_cases
 
 emu_harness.HARNESSES.setdefault("emu_query_vjp", ("-O3", True))
@@ -26,6 +28,25 @@ def test_vjp_goldens_cover_the_cases():
     assert {c["proj"] for c in cs} == {"orthogonal", "perspective"} and any(c["calib"] is None for c in cs)
     assert any(c["feats"][0].shape[2] != c["feats"][0].shape[3] for c in cs)
     assert any(c["grad_output"] is not None for c in cs) and {c["chans"][-1] for c in cs} >= {1, 3}
+    # the reverse tiles 8, 16 and 32, each exactly full once: one more unit in the second hidden layer takes another tile
+    chans = [c["chans"] for c in cs]
+    tiles = {fp32_tile(ch, grad=True) for ch in chans}
+    assert tiles >= {8, 16, 32}, tiles
+    for P in (8, 16, 32):
+        assert any(fp32_tile(ch, grad=True) == P and fp32_tile(ch[:2] + [ch[2] + 1] + ch[3:], grad=True) != P
+                   for ch in chans if len(ch) >= 4), P
+    # one layer and MP_MAX_LAYERS; wgrad_kernel's bias column alone in the last k-tile and last in a full one; outputs of
+    # 64 and 65 channels; a map of fewer than 32 channels; no last op
+    assert {len(ch) - 1 for ch in chans} >= {1, 8}
+    cins = {ch[l] + (ch[0] if l else 0) for ch in chans for l in range(len(ch) - 1)}
+    assert {k % 64 for k in cins} >= {0, 63}, sorted(cins)
+    assert {w for ch in chans for w in ch[1:]} >= {64, 65}
+    assert any(ch[0] - 1 < 32 for ch in chans)
+    assert any(c["last_op"] == spec.LAST_NONE for c in cs)
+    # maps one texel high and one wide; B * H * W <= 255, one radix pass of the ordered feature gradient
+    shapes = [c["feats"][0].shape for c in cs]
+    assert any(s[2] == 1 for s in shapes) and any(s[3] == 1 for s in shapes)
+    assert any(s[0] * s[2] * s[3] <= 255 for s in shapes)
 
 
 @pytest.mark.parametrize("name", vjp_cases())
@@ -76,7 +97,8 @@ def _run_vjp(emu, tmp_path, c, stage=0, chunk=0, sms=3, want="fpw", tag="v"):
 
 
 # the single-stage goldens (a multi-stage golden's head gradient sums over its stages: the restatement covers those)
-SINGLE = ["g_b1_rot", "g_b1_nocalib_nonsquare", "c_b3_rot"]
+SINGLE = ["g_b1_rot", "g_b1_nocalib_nonsquare", "c_b3_rot", "p8_b2_persp", "odd_b2_persp", "tiles_b1_rot", "single_b2_nocalib",
+          "deep_b1_rot", "row_b1_rot", "col_b2_nocalib", "tiny_b3"]
 
 
 @pytest.mark.parametrize("name", SINGLE)
