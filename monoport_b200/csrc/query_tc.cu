@@ -183,60 +183,45 @@ __device__ __forceinline__ PointTaps point_taps(const MpSurfaceSrc& surf, const 
   return pt;
 }
 
-// Whole warp: the 16 points whose taps sit in lanes 0..15 (duplicated in lanes 16..31), channels [phase*256, +256) of the
-// fp16 copy of the map, into rows [pbase, pbase+16) of the fp16 X tile (K-major SWIZZLE_128B; a lane covers 8 channels).
+// The skip operand X of a warp's 8 points, in two halves so that the caller can issue every gather before it uses one.
+// Whole warp: the points whose taps sit in lanes 0..7 (duplicated in lanes 8..31), channels [phase*256, +256) of the
+// fp16 copy of the map (feat16: the tile's image's), a lane covering 8 channels.
+//   load_x8   the 8 x 4 taps of the lane's channels into raw[point][tap];
+//   store_x8  the bilinear samples from raw into rows [pbase, pbase+8) of the fp16 X tile (K-major SWIZZLE_128B).
 // The last layer's direct feature access is NOT derived from these samples but from S4 (fp32, per texel), which the lane
-// owning the point interpolates in fp32 (phase 0).
-// (feat16 / s4tex: the fp16 map and the S4 products of the tile's image)
+// owning the point interpolates in fp32.
 template <int C>
-__device__ __forceinline__ void sample_x16(const TcParams& prm, const __half* feat16, const float* s4tex, uint8_t* smem_x, float* s_zf,
-                                           float* s_in, float* s_s4, const PointTaps& pt, int pbase, int lane, int phase) {
-  constexpr int RES = Prog<C>::RES;
+__device__ __forceinline__ void load_x8(const __half* feat16, const PointTaps& pt, int lane, int phase, uint4 (&raw)[8][4]) {
   const int cbase = phase * 256 + lane * 8;
-#pragma unroll 1
-  for (int q0 = 0; q0 < 16; q0 += 4) {
-    uint4 raw[4][4];                         // [point][tap] 8 fp16 channels
-    float wgt[4][4];
 #pragma unroll
-    for (int qq = 0; qq < 4; ++qq)
+  for (int q = 0; q < 8; ++q)
 #pragma unroll
-      for (int a = 0; a < 4; ++a) {
-        const int off = __shfl_sync(0xffffffffu, pt.off[a], q0 + qq);
-        wgt[qq][a] = __shfl_sync(0xffffffffu, pt.wgt[a], q0 + qq);
-        raw[qq][a] = __ldg(reinterpret_cast<const uint4*>(feat16 + (size_t)off * C + cbase));
-      }
-#pragma unroll
-    for (int qq = 0; qq < 4; ++qq) {
-      const int p = pbase + q0 + qq;
-      float2 acc[4];
-#pragma unroll
-      for (int a = 0; a < 4; ++a) {                   // same accumulation order as grid_sample: nw, ne, sw, se
-        const float2 w2 = make_float2(wgt[qq][a], wgt[qq][a]);
-        const __half2* h2 = reinterpret_cast<const __half2*>(&raw[qq][a]);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float2 f = __half22float2(h2[j]);
-          acc[j] = (a == 0) ? make_float2(__fmul_rn(f.x, w2.x), __fmul_rn(f.y, w2.y)) : make_float2(fmaf(f.x, w2.x, acc[j].x), fmaf(f.y, w2.y, acc[j].y));
-        }
-      }
-      uint4 packed;
-      packed.x = tc::pack_half2(acc[0].x, acc[0].y);
-      packed.y = tc::pack_half2(acc[1].x, acc[1].y);
-      packed.z = tc::pack_half2(acc[2].x, acc[2].y);
-      packed.w = tc::pack_half2(acc[3].x, acc[3].y);
-      *reinterpret_cast<uint4*>(smem_x + (phase * 4 + (lane >> 3)) * kKb + tc::sw128_offset(p, (lane & 7) * 8)) = packed;
+    for (int a = 0; a < 4; ++a) {
+      const int off = __shfl_sync(0xffffffffu, pt.off[a], q);
+      raw[q][a] = __ldg(reinterpret_cast<const uint4*>(feat16 + (size_t)off * C + cbase));
     }
-  }
-  if (phase == 0 && lane < 16) {
+}
+
+__device__ __forceinline__ void store_x8(uint8_t* smem_x, const PointTaps& pt, const uint4 (&raw)[8][4], int pbase, int lane, int phase) {
 #pragma unroll
-    for (int r = 0; r < RES; ++r) {
-      float s = 0.f;
+  for (int q = 0; q < 8; ++q) {
+    float2 acc[4];
 #pragma unroll
-      for (int a = 0; a < 4; ++a) s = fmaf(pt.wgt[a], __ldg(s4tex + (size_t)pt.off[a] * RES + r), s);
-      s_s4[r * kTile + pbase + lane] = s + __ldg(prm.w4z + r) * pt.zf + __ldg(prm.b4 + r);
+    for (int a = 0; a < 4; ++a) {                   // same accumulation order as grid_sample: nw, ne, sw, se
+      const float w = __shfl_sync(0xffffffffu, pt.wgt[a], q);
+      const __half2* h2 = reinterpret_cast<const __half2*>(&raw[q][a]);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float2 f = __half22float2(h2[j]);
+        acc[j] = (a == 0) ? make_float2(__fmul_rn(f.x, w), __fmul_rn(f.y, w)) : make_float2(fmaf(f.x, w, acc[j].x), fmaf(f.y, w, acc[j].y));
+      }
     }
-    s_zf[pbase + lane] = pt.zf;
-    s_in[pbase + lane] = pt.in_img ? 1.f : 0.f;
+    uint4 packed;
+    packed.x = tc::pack_half2(acc[0].x, acc[0].y);
+    packed.y = tc::pack_half2(acc[1].x, acc[1].y);
+    packed.z = tc::pack_half2(acc[2].x, acc[2].y);
+    packed.w = tc::pack_half2(acc[3].x, acc[3].y);
+    *reinterpret_cast<uint4*>(smem_x + (phase * 4 + (lane >> 3)) * kKb + tc::sw128_offset(pbase + q, (lane & 7) * 8)) = packed;
   }
 }
 
@@ -518,13 +503,29 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
   // ============================== consumers ==============================
   tc::setmaxnreg_inc<kConsumerRegs>();
   const int wl = warp & 3;
-  const int r0 = 16 * wl + (lane >> 2), cq = 2 * (lane & 3);
+  const int cq = 2 * (lane & 3);
   uint32_t fphase = 0;
 
   // ---- taps of this warp's 8 points for the layer-0 chunks: lane = (point 4 i + qw, channels 8 l8 .. and 64 + 8 l8 ..)
   const int l8 = lane & 7, qw = lane >> 3;
   uint32_t t_off[2][2], t_wgt[2][2], t_z[2];
   const __half* g0 = prm.g0;         // the tile's image's block of G0
+  // The G0 taps of the next chunk are loaded one chunk ahead: chunk c+1's loads are issued as soon as chunk c is written,
+  // so they are in flight under chunk c's MMAs instead of between the two barriers of the generation point.
+  uint4 raw[2][4][2];                // [point][tap][K-block]: the taps of the chunk generated next
+  auto load_chunk = [&](int c) {
+    const int ch = c * 128 + l8 * 8;
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int a = 0; a < 4; ++a) {
+        const uint32_t off = (a & 1) ? (t_off[i][a >> 1] >> 16) : (t_off[i][a >> 1] & 0xFFFFu);
+        const uint4* srcp = reinterpret_cast<const uint4*>(g0 + (size_t)off * kL0 + ch);
+        raw[i][a][0] = __ldg(srcp);
+        raw[i][a][1] = __ldg(srcp + 8);      // + 64 channels
+      }
+  };
+  // chunk c from the taps load_chunk(c) left in raw; then chunk c+1's loads
   auto gen_chunk = [&](int c) {
     const int ch = c * 128 + l8 * 8;
     __half2 b8[8], z8[8];
@@ -536,16 +537,6 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
     }
     uint8_t* dstp = smem + P::H0 + (c & 1) * 2 * kKb;
     const __half2 slope2 = __float2half2_rn(MP_LEAKY_SLOPE);
-    uint4 raw[2][4][2];                  // [point][tap][K-block]
-#pragma unroll
-    for (int i = 0; i < 2; ++i)
-#pragma unroll
-      for (int a = 0; a < 4; ++a) {
-        const uint32_t off = (a & 1) ? (t_off[i][a >> 1] >> 16) : (t_off[i][a >> 1] & 0xFFFFu);
-        const uint4* srcp = reinterpret_cast<const uint4*>(g0 + (size_t)off * kL0 + ch);
-        raw[i][a][0] = __ldg(srcp);
-        raw[i][a][1] = __ldg(srcp + 8);      // + 64 channels
-      }
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int p = warp * 8 + 4 * i + qw;
@@ -574,6 +565,7 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
       *reinterpret_cast<uint4*>(dstp + tc::sw128_offset(p, l8 * 8)) = make_uint4(o[0], o[1], o[2], o[3]);
       *reinterpret_cast<uint4*>(dstp + kKb + tc::sw128_offset(p, l8 * 8)) = make_uint4(o[4], o[5], o[6], o[7]);
     }
+    if (c < 7) load_chunk(c + 1);
     tc::fence_proxy_async_smem();
   };
 
@@ -591,15 +583,13 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
     const long long p0 = win0 + (t - (long long)b * n_tiles) * kTile;
     const size_t texel0 = (size_t)b * prm.H * prm.W;
     g0 = prm.g0 + texel0 * kL0;
-    // ---- X (skip operand) + per-point scalars: 4 groups of 16 points x C/256 channel phases over the 8 warps
-#pragma unroll 1
-    for (int job = warp; job < 4 * (C / 256); job += 8) {
-      const int grp = job & 3, phase = job >> 2;
-      const PointTaps pt = point_taps(surf, src, cal, bt, b, prm.H, prm.W, p0 + grp * 16 + (lane & 15), n);
-      sample_x16<C>(prm, prm.feat16 + texel0 * C, prm.s4tex + texel0 * RES, smem + P::X, s_zf, s_in, s_s4, pt, grp * 16, lane, phase);
-    }
+    // ---- tile start, in one round of gathers: each warp projects its 8 points once (lane l8 = point warp * 8 + l8), issues
+    // the X taps, the S4 taps and the taps of layer-0 chunk 0 of those points, and only then uses them.  The chunk taps
+    // are shuffled into their lanes (t_off, t_wgt, t_z); X takes its taps and weights by shuffle from lanes 0..7; lanes 0..7
+    // write the per-point scalars.
     {
-      const PointTaps pt = point_taps(surf, src, cal, bt, b, prm.H, prm.W, p0 + warp * 8 + l8, n);
+      const int pbase = warp * 8;
+      const PointTaps pt = point_taps(surf, src, cal, bt, b, prm.H, prm.W, p0 + pbase + l8, n);
       const uint32_t o01 = (uint32_t)pt.off[0] | ((uint32_t)pt.off[1] << 16), o23 = (uint32_t)pt.off[2] | ((uint32_t)pt.off[3] << 16);
       const uint32_t w01 = tc::pack_half2(pt.wgt[0], pt.wgt[1]), w23 = tc::pack_half2(pt.wgt[2], pt.wgt[3]);
       const uint32_t zz = tc::pack_half2(pt.zf, pt.zf);
@@ -612,10 +602,44 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
         t_wgt[i][1] = __shfl_sync(0xffffffffu, w23, q);
         t_z[i] = __shfl_sync(0xffffffffu, zz, q);
       }
+      load_chunk(0);
+      const __half* feat16 = prm.feat16 + texel0 * C;
+      const float* s4tex = prm.s4tex + texel0 * RES;
+      uint4 xraw[8][4];
+      load_x8<C>(feat16, pt, lane, 0, xraw);
+      float s4raw[RES][4], w4z[RES], b4[RES];
+#pragma unroll
+      for (int r = 0; r < RES; ++r) {
+#pragma unroll
+        for (int a = 0; a < 4; ++a) s4raw[r][a] = __ldg(s4tex + (size_t)pt.off[a] * RES + r);
+        w4z[r] = __ldg(prm.w4z + r);
+        b4[r] = __ldg(prm.b4 + r);
+      }
+      store_x8(smem + P::X, pt, xraw, pbase, lane, 0);
+#pragma unroll 1
+      for (int phase = 1; phase < C / 256; ++phase) {      // colour: the second 256 channels of X, one more round
+        load_x8<C>(feat16, pt, lane, phase, xraw);
+        store_x8(smem + P::X, pt, xraw, pbase, lane, phase);
+      }
+      if (lane < 8) {
+#pragma unroll
+        for (int r = 0; r < RES; ++r) {
+          float s = 0.f;
+#pragma unroll
+          for (int a = 0; a < 4; ++a) s = fmaf(pt.wgt[a], s4raw[r][a], s);
+          s_s4[r * kTile + pbase + lane] = s + w4z[r] * pt.zf + b4[r];
+        }
+        s_zf[pbase + lane] = pt.zf;
+        s_in[pbase + lane] = pt.in_img ? 1.f : 0.f;
+      }
     }
     tc::fence_proxy_async_smem();
     gen_chunk(0);
     sync_consumers();
+    // rows r0 and r0 + 8 of the accumulator fragments.  Taken through a shuffle in every tile, so that the compiler does not
+    // hoist the epilogues' shared-memory addresses out of the tile loop: held across it they would take the registers the
+    // gathers of the tile start have in flight, and spill.
+    const int r0 = __shfl_sync(0xffffffffu, 16 * wl + (lane >> 2), lane);
     const float zf0 = s_zf[r0], zf1 = s_zf[r0 + 8];
 
     // hidden epilogue: + bias + w_z z, leaky ReLU -> fp16, K-major
@@ -927,7 +951,7 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
         for (int a = 0; a < 4; ++a) raw[a] = __ldg(reinterpret_cast<const uint4*>(prm.feat16 + (size_t)off[a] * C + cbase));
         float2 acc[4], ax[4], ay[4];
 #pragma unroll
-        for (int a = 0; a < 4; ++a) {        // the value as sample_x16 takes it: nw, ne, sw, se
+        for (int a = 0; a < 4; ++a) {        // the value as store_x8 takes it: nw, ne, sw, se
           const float2 w2 = make_float2(wgt[a], wgt[a]);
           const __half2* h2 = reinterpret_cast<const __half2*>(&raw[a]);
 #pragma unroll
@@ -949,7 +973,7 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
         *reinterpret_cast<uint4*>(xkb + tc::sw128_offset(jvp_row(q, 3), k8)) = make_uint4(0u, 0u, 0u, 0u);
       }
     }
-    if (lane < 16 && (lane >> 1) == warp) {          // point `lane`: its scalars (S4 as sample_x16 samples it)
+    if (lane < 16 && (lane >> 1) == warp) {          // point `lane`: its scalars (S4 as query_wg_kernel samples it)
       const PointTaps& pt = jt.pt;
 #pragma unroll
       for (int r = 0; r < RES; ++r) {
