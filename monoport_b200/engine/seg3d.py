@@ -160,12 +160,10 @@ class _Seg3dBase(nn.Module):
         out = self._new_volume(device)
         nonempty = ctypes.c_int(0)
         stats = (ctypes.c_int64 * len(self.resolutions))()
-        from ..modeling.geometry import perspective
         with _lib.device_guard(device):
             fh = net.feature_handle(feat)
-            proj = _lib.PROJ_PERSPECTIVE if net.projection is perspective else _lib.PROJ_ORTHOGONAL
             _lib.check(lib.mp_octree_run_fused(
-                self._handle(device), net.surface_classifier.handle(), fh.ptr, _lib.calib12(calib_tensor), proj,
+                self._handle(device), net.surface_classifier.handle(), fh.ptr, _lib.calib12(calib_tensor), net._proj(),
                 ctypes.c_float(net.normalizer.scale), net._mode(), ctypes.c_void_p(out.data_ptr()),
                 ctypes.byref(nonempty), stats, _lib.stream_ptr(device)), "mp_octree_run_fused")
         self.last_stats = list(stats)

@@ -83,7 +83,7 @@ class _QueryStage(torch.autograd.Function):
         ctx.net = net
         ctx.has_calibs = calibs is not None
         ctx.save_for_backward(feat, points, *([calibs] if calibs is not None else []), *params)
-        return net._query_fp32(feat, points, calibs)
+        return net._query_points(feat.detach(), points, calibs, _lib.MODE_FP32)
 
     @staticmethod
     @once_differentiable
@@ -141,24 +141,27 @@ class MonoPortNet(nn.Module):
             raise ValueError("feature map must be [1,C,H,W] (batch 1, RTL/main.py:175); got %s" % (tuple(feat.shape),))
         if feat.device.type != "cuda":
             raise RuntimeError("monoport_b200.query: features must be CUDA tensors (there is no CPU path)")
-        _, C, H, W = feat.shape
-        # one handle per calling thread: the handle carries the channel-last copies of the CURRENT frame, and the
-        # demo-style pipelines query different frames from different threads (RTL/dataloader.py:734-751)
-        key = (C, H, W, feat.device.index, threading.get_ident())
-        h = self._feat_handles.get(key)
-        if h is None:
-            h = self._feat_handles[key] = FeatureHandle(C, H, W, feat.device)
-        h.upload(feat, trust_identity=self.feature_cache)
-        return h
+        return self._feature_handle(feat)
 
     def batch_feature_handle(self, feat):
         """The handle of a [B,C,H,W] batch (B > 1) for query(): B maps, evaluated together by mp_query_points_batch.  The
         single-map entry points (feature_handle, the grid queries, the engines) do not take it."""
+        return self._feature_handle(feat)
+
+    def _feature_handle(self, feat, reupload=False):
+        """The calling thread's handle of the [B,C,H,W] map `feat`, with `feat` uploaded under FeatureHandle.upload's
+        identity policy, or in any case when `reupload`."""
         B, C, H, W = feat.shape
-        key = ("batch", B, C, H, W, feat.device.index, threading.get_ident())
+        # one handle per calling thread: the handle carries the channel-last copies of the CURRENT frame, and the
+        # demo-style pipelines query different frames from different threads (RTL/dataloader.py:734-751)
+        key = (C, H, W, feat.device.index, threading.get_ident())
+        if B != 1:
+            key = ("batch", B) + key
         h = self._feat_handles.get(key)
         if h is None:
             h = self._feat_handles[key] = FeatureHandle(C, H, W, feat.device, B=B)
+        if reupload:
+            h.invalidate()
         h.upload(feat, trust_identity=self.feature_cache)
         return h
 
@@ -173,6 +176,77 @@ class MonoPortNet(nn.Module):
         except KeyError:
             raise ValueError("precision must be one of %s" % sorted(_MODES))
 
+    def _proj(self):
+        """the C-ABI's code of `projection` (a plain attribute, so read at each call)"""
+        return _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
+
+    @staticmethod
+    def _checked_map(feats, points, calibs, what, calib_rows):
+        """-> the one map [B,C,H,W] of a stage's feature list `feats`, checked for a query by `what` against points [B,3,N]
+        and calibs [B,4,4] | [B,3,4] | None, all on one device.  The calibs' shape is left to _lib.calib12 (which also takes
+        one [4,4] or [3,4] matrix) where a single map's launch reads them by value, i.e. for B == 1 unless `calib_rows`."""
+        if len(feats) != 1:
+            raise NotImplementedError("multi-level feature lists (HRNet) are not supported")
+        feat = feats[0]
+        if feat.device.type != "cuda":
+            raise RuntimeError("monoport_b200.%s: features must be CUDA tensors (there is no CPU path)" % what)
+        B = feat.shape[0] if feat.dim() == 4 else -1
+        if feat.dim() != 4 or points.dim() != 3 or points.shape[0] != B or points.shape[1] != 3:
+            raise ValueError("features must be [B,C,H,W] and points [B,3,N]; got %s and %s"
+                             % (tuple(feat.shape), tuple(points.shape)))
+        if calibs is not None and (calib_rows or B != 1):
+            if calibs.dim() != 3 or calibs.shape[0] != B or calibs.shape[1] not in (3, 4) or calibs.shape[2] != 4:
+                raise ValueError("calibs must be [B,4,4] or [B,3,4] with the features' B=%d; got %s"
+                                 % (B, tuple(calibs.shape)))
+        if points.device != feat.device:
+            raise ValueError("points and features live on different devices")
+        return feat
+
+    @staticmethod
+    def _points_rows(points):
+        """points [B,3,N] as the C-ABI reads them: float32, detached, made contiguous only when a stride it reads is < 1 (the
+        row and point strides, and the batch stride for B > 1)"""
+        p = points.detach() if points.requires_grad else points      # (detach() alone costs a microsecond per query)
+        if p.dtype != torch.float32:
+            p = p.float()
+        s = p.stride()
+        if p.shape[2] > 0 and (s[1] < 1 or s[2] < 1 or (p.shape[0] > 1 and s[0] < 1)):
+            p = p.contiguous()
+        return p
+
+    @staticmethod
+    def _calib_rows(calibs, device):
+        """calibs [B,3|4,4] | None -> their [B,3,4] float32 rows on `device`, as the batched entry points read them"""
+        return None if calibs is None else calibs.detach()[:, :3, :4].to(device=device, dtype=torch.float32).contiguous()
+
+    def _query_points(self, feat, points, calibs, mode):
+        """[B,C,H,W] map, points [B,3,N], calibs -> [B,Res,N] in one launch of `mode`: mp_query_points for B == 1 (the camera
+        by value, read back once per frame scope), else mp_query_points_batch (the calibs stay on the device: no read-back,
+        no synchronisation)."""
+        B, n = feat.shape[0], points.shape[2]
+        head = self.surface_classifier
+        res = head.filter_channels[-1]
+        out = torch.empty((B, res, n), dtype=torch.float32, device=feat.device)
+        if n == 0:
+            return out
+        p = self._points_rows(points)
+        s = p.stride()
+        with _lib.device_guard(feat.device):
+            fh = self._feature_handle(feat)
+            if B == 1:
+                _lib.check(_lib.load().mp_query_points(
+                    head.handle(), fh.ptr, ctypes.c_void_p(p.data_ptr()), n, s[1], s[2], _lib.calib12(calibs), self._proj(),
+                    ctypes.c_float(self.normalizer.scale), ctypes.c_void_p(out.data_ptr()), n, mode,
+                    _lib.stream_ptr(feat.device)), "mp_query_points")
+            else:
+                cal = self._calib_rows(calibs, feat.device)
+                _lib.check(_lib.load().mp_query_points_batch(
+                    head.handle(), fh.ptr, B, ctypes.c_void_p(p.data_ptr()), n, s[0], s[1], s[2],
+                    None if cal is None else ctypes.c_void_p(cal.data_ptr()), self._proj(),
+                    ctypes.c_float(self.normalizer.scale), ctypes.c_void_p(out.data_ptr()), res * n, n, mode,
+                    _lib.stream_ptr(feat.device)), "mp_query_points_batch")
+        return out
+
     @torch.no_grad()
     def query(self, feats_stages, points, calibs=None, transforms=None):
         """list(list([B,C,H,W])), points [B,3,N], calibs [B,4,4]|[B,3,4]|None -> [ [B,Res,N] ]
@@ -183,38 +257,8 @@ class MonoPortNet(nn.Module):
                                       "call .eval() (RTL/main.py:116), or query_stages() for the differentiable query")
         if transforms is not None:
             raise NotImplementedError("`transforms` is not supported (never passed on the recon path, RTL/main.py:179-182)")
-        feats = feats_stages[-1]
-        if len(feats) != 1:
-            raise NotImplementedError("multi-level feature lists (HRNet) are not supported")
-        feat = feats[0]
-        if feat.device.type != "cuda":
-            raise RuntimeError("monoport_b200.query: features must be CUDA tensors (there is no CPU path)")
-        if feat.dim() == 4 and feat.shape[0] > 1:
-            return self._query_batch(feat, points, calibs)
-        if points.dim() != 3 or points.shape[0] != 1 or points.shape[1] != 3:
-            raise ValueError("points must be [1,3,N]; got %s" % (tuple(points.shape),))
-        if points.device != feat.device:
-            raise ValueError("points and features live on different devices")
-        if points.dtype != torch.float32:
-            points = points.float()
-        n = points.shape[2]
-        s = points.stride()
-        if n > 0 and (s[1] < 1 or s[2] < 1):
-            points = points.contiguous()
-            s = points.stride()
-        head = self.surface_classifier
-        res = head.filter_channels[-1]
-        out = torch.empty((1, res, n), dtype=torch.float32, device=feat.device)
-        if n == 0:
-            return [out]
-        with _lib.device_guard(feat.device):
-            fh = self.feature_handle(feat)
-            proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
-            _lib.check(_lib.load().mp_query_points(
-                head.handle(), fh.ptr, ctypes.c_void_p(points.data_ptr()), n, s[1], s[2], _lib.calib12(calibs), proj,
-                ctypes.c_float(self.normalizer.scale), ctypes.c_void_p(out.data_ptr()), n, self._mode(),
-                _lib.stream_ptr(feat.device)), "mp_query_points")
-        return [out]
+        feat = self._checked_map(feats_stages[-1], points, calibs, "query", calib_rows=False)
+        return [self._query_points(feat, points, calibs, self._mode())]
 
     @torch.no_grad()
     def query_gradient(self, feats_stages, points, calibs=None, grad_output=None, precision="fp32"):
@@ -232,26 +276,12 @@ class MonoPortNet(nn.Module):
         if self.training:
             raise NotImplementedError("query_gradient is eval-mode only (the gradient of the last stage, like query()); "
                                       "call .eval()")
-        feats = feats_stages[-1]
-        if len(feats) != 1:
-            raise NotImplementedError("multi-level feature lists (HRNet) are not supported")
-        feat = feats[0]
-        if feat.device.type != "cuda":
-            raise RuntimeError("monoport_b200.query_gradient: features must be CUDA tensors (there is no CPU path)")
-        if feat.dim() != 4 or feat.shape[0] != 1:
+        feat = self._checked_map(feats_stages[-1], points, calibs, "query_gradient", calib_rows=False)
+        if feat.shape[0] != 1:
             raise ValueError("query_gradient takes one feature map [1,C,H,W]; got %s" % (tuple(feat.shape),))
-        if points.dim() != 3 or points.shape[0] != 1 or points.shape[1] != 3:
-            raise ValueError("points must be [1,3,N]; got %s" % (tuple(points.shape),))
-        if points.device != feat.device:
-            raise ValueError("points and features live on different devices")
-        points = points.detach()
-        if points.dtype != torch.float32:
-            points = points.float()
+        points = self._points_rows(points)
         n = points.shape[2]
         s = points.stride()
-        if n > 0 and (s[1] < 1 or s[2] < 1):
-            points = points.contiguous()
-            s = points.stride()
         head = self.surface_classifier
         res = head.filter_channels[-1]
         gout = None
@@ -267,9 +297,8 @@ class MonoPortNet(nn.Module):
             return out, dp
         with _lib.device_guard(feat.device):
             fh = self.feature_handle(feat)
-            proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
             _lib.check(_lib.load().mp_query_points_grad_mode(
-                head.handle(), fh.ptr, ctypes.c_void_p(points.data_ptr()), n, s[1], s[2], _lib.calib12(calibs), proj,
+                head.handle(), fh.ptr, ctypes.c_void_p(points.data_ptr()), n, s[1], s[2], _lib.calib12(calibs), self._proj(),
                 ctypes.c_float(self.normalizer.scale), None if gout is None else ctypes.c_void_p(gout.data_ptr()), n,
                 ctypes.c_void_p(out.data_ptr()), n, ctypes.c_void_p(dp.data_ptr()), n, None, _MODES[precision],
                 _lib.stream_ptr(feat.device)), "mp_query_points_grad_mode")
@@ -302,59 +331,9 @@ class MonoPortNet(nn.Module):
         params = [t for f in head.filters for t in (f.weight, f.bias)]
         preds = []
         for feats in feats_stages:
-            if len(feats) != 1:
-                raise NotImplementedError("multi-level feature lists (HRNet) are not supported")
-            feat = feats[0]
-            if feat.device.type != "cuda":
-                raise RuntimeError("monoport_b200.query_stages: features must be CUDA tensors (there is no CPU path)")
-            B = feat.shape[0] if feat.dim() == 4 else -1
-            if feat.dim() != 4 or points.dim() != 3 or points.shape[0] != B or points.shape[1] != 3:
-                raise ValueError("features must be [B,C,H,W] and points [B,3,N]; got %s and %s"
-                                 % (tuple(feat.shape), tuple(points.shape)))
-            if calibs is not None and (calibs.dim() != 3 or calibs.shape[0] != B or calibs.shape[1] not in (3, 4)
-                                       or calibs.shape[2] != 4):
-                raise ValueError("calibs must be [B,4,4] or [B,3,4] with the features' B=%d; got %s"
-                                 % (B, tuple(calibs.shape)))
-            if points.device != feat.device:
-                raise ValueError("points and features live on different devices")
+            feat = self._checked_map(feats, points, calibs, "query_stages", calib_rows=True)
             preds.append(_QueryStage.apply(self, feat, points, calibs, *params))
         return preds
-
-    def _points_rows(self, points):
-        p = points.detach()
-        if p.dtype != torch.float32:
-            p = p.float()
-        if p.shape[2] > 0 and min(p.stride()) < 1:
-            p = p.contiguous()
-        return p
-
-    def _query_fp32(self, feat, points, calibs):
-        """the values of query_stages: query() with precision "fp32" (B = 1: mp_query_points, else mp_query_points_batch)"""
-        B, n = feat.shape[0], points.shape[2]
-        res = self.surface_classifier.filter_channels[-1]
-        out = torch.empty((B, res, n), dtype=torch.float32, device=feat.device)
-        if n == 0:
-            return out
-        p = self._points_rows(points)
-        s = p.stride()
-        proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
-        with _lib.device_guard(feat.device):
-            lib = _lib.load()
-            if B == 1:
-                fh = self.feature_handle(feat.detach())
-                _lib.check(lib.mp_query_points(
-                    self.surface_classifier.handle(), fh.ptr, ctypes.c_void_p(p.data_ptr()), n, s[1], s[2],
-                    _lib.calib12(None if calibs is None else calibs.detach()), proj, ctypes.c_float(self.normalizer.scale),
-                    ctypes.c_void_p(out.data_ptr()), n, _lib.MODE_FP32, _lib.stream_ptr(feat.device)), "mp_query_points")
-            else:
-                cal = None if calibs is None else calibs.detach()[:, :3, :4].to(device=feat.device, dtype=torch.float32).contiguous()
-                fh = self.batch_feature_handle(feat.detach())
-                _lib.check(lib.mp_query_points_batch(
-                    self.surface_classifier.handle(), fh.ptr, B, ctypes.c_void_p(p.data_ptr()), n, s[0], s[1], s[2],
-                    None if cal is None else ctypes.c_void_p(cal.data_ptr()), proj, ctypes.c_float(self.normalizer.scale),
-                    ctypes.c_void_p(out.data_ptr()), res * n, n, _lib.MODE_FP32, _lib.stream_ptr(feat.device)),
-                    "mp_query_points_batch")
-        return out
 
     def _query_vjp(self, feat, points, calibs, grad, want_feat, want_points, want_head, deterministic=False):
         """-> (d feat [B,C,H,W] | None, d points [B,3,N] | None, [d W_l [Cout,Cin]] | None, [d b_l] | None) of
@@ -378,17 +357,10 @@ class MonoPortNet(nn.Module):
         p = self._points_rows(points)
         s = p.stride()
         gout = grad.detach().to(torch.float32).contiguous()
-        proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
         with _lib.device_guard(dev):
             lib = _lib.load()
-            cal = None if calibs is None else calibs.detach()[:, :3, :4].to(**f32).contiguous()
-            key = ((C, H, W, dev.index, threading.get_ident()) if B == 1 else
-                   ("batch", B, C, H, W, dev.index, threading.get_ident()))
-            fh = self._feat_handles.get(key)
-            if fh is None:
-                fh = self._feat_handles[key] = FeatureHandle(C, H, W, dev, B=B)
-            fh.invalidate()
-            fh.upload(feat.detach())
+            cal = self._calib_rows(calibs, dev)
+            fh = self._feature_handle(feat.detach(), reupload=True)
             mlp = head.handle()
             flags = _lib.VJP_DETERMINISTIC if deterministic else 0
             nbytes = lib.mp_query_points_vjp_scratch_bytes_ex(mlp, fh.ptr, B, n, int(self.vjp_chunk_points), int(want_feat),
@@ -400,46 +372,12 @@ class MonoPortNet(nn.Module):
             ptrs = (lambda ts: None if ts is None else (ctypes.c_void_p * L)(*[t.data_ptr() for t in ts]))
             _lib.check(lib.mp_query_points_vjp_ex(
                 mlp, fh.ptr, B, ctypes.c_void_p(p.data_ptr()), n, s[0], s[1], s[2],
-                None if cal is None else ctypes.c_void_p(cal.data_ptr()), proj, ctypes.c_float(self.normalizer.scale),
+                None if cal is None else ctypes.c_void_p(cal.data_ptr()), self._proj(), ctypes.c_float(self.normalizer.scale),
                 ctypes.c_void_p(gout.data_ptr()), None if dfeat is None else ctypes.c_void_p(dfeat.data_ptr()),
                 None if dpoints is None else ctypes.c_void_p(dpoints.data_ptr()), ptrs(dws), ptrs(dbs),
                 None if scratch is None else ctypes.c_void_p(scratch.data_ptr()), int(nbytes), flags, _lib.stream_ptr(dev)),
                 "mp_query_points_vjp_ex")
         return dfeat, dpoints, dws, dbs
-
-    def _query_batch(self, feat, points, calibs):
-        """query() of B > 1 images: one launch; the calibs stay on the device (no read-back, no synchronisation)."""
-        B = feat.shape[0]
-        if points.dim() != 3 or points.shape[1] != 3 or points.shape[0] != B:
-            raise ValueError("points must be [B,3,N] with the features' B=%d; got %s" % (B, tuple(points.shape)))
-        if calibs is not None and (calibs.dim() != 3 or calibs.shape[0] != B or calibs.shape[1] not in (3, 4)
-                                   or calibs.shape[2] != 4):
-            raise ValueError("calibs must be [B,4,4] or [B,3,4] with the features' B=%d; got %s" % (B, tuple(calibs.shape)))
-        if points.device != feat.device:
-            raise ValueError("points and features live on different devices")
-        if points.dtype != torch.float32:
-            points = points.float()
-        n = points.shape[2]
-        s = points.stride()
-        if n > 0 and min(s) < 1:
-            points = points.contiguous()
-            s = points.stride()
-        res = self.surface_classifier.filter_channels[-1]
-        out = torch.empty((B, res, n), dtype=torch.float32, device=feat.device)
-        if n == 0:
-            return [out]
-        with _lib.device_guard(feat.device):
-            cal = None
-            if calibs is not None:
-                cal = calibs.detach()[:, :3, :4].to(device=feat.device, dtype=torch.float32).contiguous()
-            fh = self.batch_feature_handle(feat)
-            proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
-            _lib.check(_lib.load().mp_query_points_batch(
-                self.surface_classifier.handle(), fh.ptr, B, ctypes.c_void_p(points.data_ptr()), n, s[0], s[1], s[2],
-                None if cal is None else ctypes.c_void_p(cal.data_ptr()), proj, ctypes.c_float(self.normalizer.scale),
-                ctypes.c_void_p(out.data_ptr()), res * n, n, self._mode(), _lib.stream_ptr(feat.device)),
-                "mp_query_points_batch")
-        return [out]
 
     def query_grid(self, feat, calibs, resolution, b_min, b_max, z0=0, nz=None, out=None, fh=None):
         """Dense occupancy slab [nz,R,R] of an R^3 grid over [b_min,b_max] (points generated in-kernel).
@@ -451,10 +389,9 @@ class MonoPortNet(nn.Module):
         with _lib.device_guard(feat.device):
             if fh is None:
                 fh = self.feature_handle(feat)
-            proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
             _lib.check(_lib.load().mp_query_grid(
                 self.surface_classifier.handle(), fh.ptr, R, int(z0), nz, _lib.f3(b_min), _lib.f3(b_max),
-                _lib.calib12(calibs), proj, ctypes.c_float(self.normalizer.scale), ctypes.c_void_p(out.data_ptr()),
+                _lib.calib12(calibs), self._proj(), ctypes.c_float(self.normalizer.scale), ctypes.c_void_p(out.data_ptr()),
                 self._mode(), _lib.stream_ptr(feat.device)), "mp_query_grid")
         return out
 
@@ -469,10 +406,9 @@ class MonoPortNet(nn.Module):
         with _lib.device_guard(feat.device):
             if fh is None:
                 fh = self.feature_handle(feat)
-            proj = _lib.PROJ_PERSPECTIVE if self.projection is perspective else _lib.PROJ_ORTHOGONAL
             _lib.check(_lib.load().mp_query_grid_range(
                 self.surface_classifier.handle(), fh.ptr, R, lin0, n, _lib.f3(b_min), _lib.f3(b_max),
-                _lib.calib12(calibs), proj, ctypes.c_float(self.normalizer.scale), ctypes.c_void_p(out.data_ptr()),
+                _lib.calib12(calibs), self._proj(), ctypes.c_float(self.normalizer.scale), ctypes.c_void_p(out.data_ptr()),
                 self._mode(), _lib.stream_ptr(feat.device)), "mp_query_grid_range")
         return out
 

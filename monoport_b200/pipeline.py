@@ -99,7 +99,6 @@ class FrameGraph:
                  netC=None, render_normals=False, canvas=None, mesh=False, mesh_normals=False, mesh_colours=False,
                  mesh_capacity=None, display=False):
         from .modeling.MonoPortNet import FeatureHandle
-        from .modeling.geometry import perspective
         from .recon import _DIRS
         if getattr(engine.query_func, "__monoport_fused__", None) is not net:
             raise ValueError("the engine's query_func must be make_query_func(net)")
@@ -109,7 +108,7 @@ class FrameGraph:
         self.feature_hook = feature_hook
         self.R = R = engine.resolutions[-1]
         self._dir = _DIRS[direction]
-        self._proj = _lib.PROJ_PERSPECTIVE if net.projection is perspective else _lib.PROJ_ORTHOGONAL
+        self._proj = net._proj()
         cal12 = _lib.calib12(calib.detach().cpu())
         if input_shape is None:
             input_shape = (1, 3, 512, 512) if with_encoder else (1, net.surface_classifier.filter_channels[0] - 1, 128, 128)
@@ -149,7 +148,7 @@ class FrameGraph:
                 self.render_tex = torch.empty_like(self._bg)
                 self._fhc = None
                 self._headC = netC.surface_classifier.handle()
-                self._projC = _lib.PROJ_PERSPECTIVE if netC.projection is perspective else _lib.PROJ_ORTHOGONAL
+                self._projC = netC._proj()
             self._bmin3, self._bmax3 = _lib.f3(engine.b_min), _lib.f3(engine.b_max)
             self.volume = torch.empty((1, 1, R, R, R), dtype=torch.float32, device=dev)
             cap = R * R

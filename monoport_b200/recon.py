@@ -180,7 +180,6 @@ def mesh_normals(net, feats, verts, calib_tensor, precision="auto"):
     reconstruction(normals=True) uses; "tc" / "auto": the tensor-core program's forward-mode derivative, a frame above the
     head's feature limit differentiated exactly, decided on the device)."""
     from .modeling.MonoPortNet import _MODES
-    from .modeling.geometry import perspective
     if precision not in ("fp32", "tc", "auto"):
         raise ValueError("precision must be one of 'fp32', 'tc', 'auto'; got %r" % (precision,))
     feat = feats[-1][0]
@@ -199,10 +198,9 @@ def mesh_normals(net, feats, verts, calib_tensor, precision="auto"):
     scratch = torch.empty(3 * n, dtype=torch.float32, device=device)
     with _lib.device_guard(device):
         fh = net.feature_handle(feat)
-        proj = _lib.PROJ_PERSPECTIVE if net.projection is perspective else _lib.PROJ_ORTHOGONAL
         _lib.check(_lib.load().mp_mesh_normals_async(
             net.surface_classifier.handle(), fh.ptr, ctypes.c_void_p(v.data_ptr()), ctypes.c_void_p(counts.data_ptr()),
-            ctypes.c_void_p(count32.data_ptr()), n, _lib.calib12(calib_tensor), proj, ctypes.c_float(net.normalizer.scale),
+            ctypes.c_void_p(count32.data_ptr()), n, _lib.calib12(calib_tensor), net._proj(), ctypes.c_float(net.normalizer.scale),
             _MODES[precision], ctypes.c_void_p(scratch.data_ptr()), ctypes.c_void_p(out.data_ptr()), _lib.stream_ptr(device)),
             "mp_mesh_normals_async")
     return out
@@ -305,7 +303,6 @@ def colorization(netC, feat_tensor_C, X, Y, Z, calib_tensor, norm=None, resoluti
     if norm is not None:
         image[X, Y, :] = ((norm + 1) / 2).clamp(0, 1)
         return image
-    from .modeling.geometry import perspective
     head = netC.surface_classifier
     feat = feat_tensor_C[-1][0]
     # the tensor-core program covers maps of at most 65536 texels: a larger map takes the generic route, whose query() runs
@@ -319,11 +316,10 @@ def colorization(netC, feat_tensor_C, X, Y, Z, calib_tensor, norm=None, resoluti
             Xc, Yc, Zc = X.contiguous(), Y.contiguous(), Z.float().contiguous()
             with _lib.device_guard(device):
                 fh = netC.feature_handle(feat)
-                proj = _lib.PROJ_PERSPECTIVE if netC.projection is perspective else _lib.PROJ_ORTHOGONAL
                 rc = _lib.load().mp_colorize_surface(
                     head.handle(), fh.ptr, ctypes.c_void_p(Xc.data_ptr()), ctypes.c_void_p(Yc.data_ptr()),
                     ctypes.c_void_p(Zc.data_ptr()), n, int(resolution), _lib.f3(b_min), _lib.f3(b_max), _lib.calib12(calib_tensor),
-                    proj, ctypes.c_float(netC.normalizer.scale), ctypes.c_void_p(image.data_ptr()), _lib.stream_ptr(device))
+                    netC._proj(), ctypes.c_float(netC.normalizer.scale), ctypes.c_void_p(image.data_ptr()), _lib.stream_ptr(device))
                 if rc != _lib.MP_E_RANGE:
                     _lib.check(rc, "mp_colorize_surface")
         if rc != _lib.MP_E_RANGE:
@@ -351,7 +347,6 @@ def _surface_normals_device(net, feat, X, Y, Z, calib_tensor, resolution, b_min,
     import ctypes
     from . import _lib
     from .modeling.MonoPortNet import _MODES
-    from .modeling.geometry import perspective
     device = calib_tensor.device
     n = X.numel()
     out = torch.empty((n, 3), dtype=torch.float32, device=device)
@@ -363,11 +358,10 @@ def _surface_normals_device(net, feat, X, Y, Z, calib_tensor, resolution, b_min,
     scratch = torch.empty(6 * n + 1, dtype=torch.float32, device=device)
     with _lib.device_guard(device):
         fh = net.feature_handle(feat)
-        proj = _lib.PROJ_PERSPECTIVE if net.projection is perspective else _lib.PROJ_ORTHOGONAL
         _lib.check(_lib.load().mp_surface_normals_async(
             net.surface_classifier.handle(), fh.ptr, ctypes.c_void_p(Xd.data_ptr()), ctypes.c_void_p(Yd.data_ptr()),
             ctypes.c_void_p(Zd.data_ptr()), ctypes.c_void_p(count.data_ptr()), n, int(resolution), _lib.f3(b_min),
-            _lib.f3(b_max), _lib.calib12(calib_tensor), proj, ctypes.c_float(net.normalizer.scale), _MODES[precision],
+            _lib.f3(b_max), _lib.calib12(calib_tensor), net._proj(), ctypes.c_float(net.normalizer.scale), _MODES[precision],
             ctypes.c_void_p(scratch.data_ptr()), ctypes.c_void_p(out.data_ptr()), _lib.stream_ptr(device)),
             "mp_surface_normals_async")
     return out

@@ -175,17 +175,15 @@ def query_grid_fused(net, feat, calibs, R, b_min, b_max, peers, fh=None):
     then make one barrier per frame sufficient)."""
     import ctypes
     from . import _lib
-    from .modeling.geometry import perspective
     assert R == peers.R
     lin0, n = range_bounds(R, peers.world)[0][peers.rank]          # balanced ranges of the linear node order
     ptrs, local = peers.next_set()
     with _lib.device_guard(feat.device):
         if fh is None:
             fh = net.feature_handle(feat)
-        proj = _lib.PROJ_PERSPECTIVE if net.projection is perspective else _lib.PROJ_ORTHOGONAL
         _lib.check(_lib.load().mp_query_grid_range_peers(
             net.surface_classifier.handle(), fh.ptr, int(R), int(lin0), int(n), _lib.f3(b_min), _lib.f3(b_max),
-            _lib.calib12(calibs), proj, ctypes.c_float(net.normalizer.scale), ptrs, peers.world, net._mode(),
+            _lib.calib12(calibs), net._proj(), ctypes.c_float(net.normalizer.scale), ptrs, peers.world, net._mode(),
             _lib.stream_ptr(feat.device)), "mp_query_grid_range_peers")
     peers.barrier()
     return local
