@@ -1,17 +1,25 @@
-// TEST INFRASTRUCTURE ONLY: the host side of the query harnesses (emu_query_*, emu_heads_fp32, emu_colour_surface_*,
-// emu_dcal_*), which compile monoport_b200/csrc/query_fp32.cu or query_tc.cu UNMODIFIED for the CPU against the
-// execution-model emulation (cuda_emu.h) and, for query_tc.cu, the functional model of the wgmma / mbarrier / bulk-copy
-// layer (tc_ptx_emu.h).  Include it first, then the kernel file.  It holds a host-memory stand-in for the CUDA runtime
-// calls of the launchers, the models of the device intrinsics the real headers only give to nvcc, and the in.bin reader.
+// TEST INFRASTRUCTURE ONLY: the host side of the two query harnesses, emu_fp32.cpp (query_fp32.cu and query_vjp.cu) and
+// emu_tc.cpp (query_tc.cu), which compile the library's kernel sources UNMODIFIED for the CPU against the execution-model
+// emulation (cuda_emu.h) and, for query_tc.cu, the functional model of the wgmma / mbarrier / bulk-copy layer
+// (tc_ptx_emu.h).  Include it first, then the kernel file.  It holds a host-memory stand-in for the CUDA runtime calls of
+// the launchers, the models of the device intrinsics the real headers only give to nvcc, the in.bin reader and the
+// command line both harnesses share:
+//   <harness> in.bin out.f32 op [op args] [--name value | --name=value | --flag ...]
+// Options every launching op reads: --sms N (the simulated SM count, default 3), --widths W (the head's widths after the
+// first, "64,48,1", "noskip:" in front for a no_residual head; default the shipped 1024,512,256,128,res) and --limit L
+// (the head's tensor-core feature limit, default +inf).  An option the op does not read exits 2.
 //
 // in.bin: int32 header {C, H, W, N, has_calib, perspective, res, last_op}, float z_scale, calib[12] (rows 0..2 of [R|t]),
 // then fp32 arrays: the feature maps NCHW [B*C*H*W], the points [B*3*N] (rows x, y, z of each image), when batched and
 // has_calib the B calibs [B*12] (instead of the header's), and per layer W_l [cout*cin] and b_l [cout].  B is 1 unless
-// the harness runs a batched launch.
+// the op runs a batched launch.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdarg.h>
+
+#include <string>
+#include <utility>
 
 #define MP_EMU_CUDA_TYPES 1
 #include <math.h>
@@ -41,6 +49,7 @@ cudaError_t cudaFree(void* p) { free(p); return cudaSuccess; }
 cudaError_t cudaMemcpy(void* d, const void* s, size_t n, cudaMemcpyKind) { memcpy(d, s, n); return cudaSuccess; }
 cudaError_t cudaMemset(void* d, int v, size_t n) { memset(d, v, n); return cudaSuccess; }
 cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, cudaMemcpyKind, cudaStream_t) { memcpy(d, s, n); return cudaSuccess; }
+cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t) { memset(d, v, n); return cudaSuccess; }
 cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) {
   if (a == cudaDevAttrComputeCapabilityMajor) *v = 9;
@@ -72,6 +81,51 @@ void mp_set_error(const char* fmt, ...) {
 }
 
 #include "../../monoport_b200/csrc/mp_common.cuh"
+
+// ---- the command line ---------------------------------------------------------------------------------------------------
+struct EmuArgs {
+  std::vector<const char*> pos;                               // in.bin, out.f32, the op, the op's arguments
+  std::vector<std::pair<std::string, const char*>> opts;      // --name value / --name=value; a flag's value is ""
+  std::vector<bool> used;
+
+  EmuArgs(int argc, char** argv) {
+    for (int i = 1; i < argc; ++i) {
+      if (strncmp(argv[i], "--", 2) != 0) { pos.push_back(argv[i]); continue; }
+      const char* eq = strchr(argv[i], '=');
+      if (eq) opts.emplace_back(std::string(argv[i] + 2, (size_t)(eq - argv[i] - 2)), eq + 1);
+      else if (i + 1 < argc && strncmp(argv[i + 1], "--", 2) != 0) { opts.emplace_back(argv[i] + 2, argv[i + 1]); ++i; }
+      else opts.emplace_back(argv[i] + 2, "");
+    }
+    used.assign(opts.size(), false);
+  }
+  // the op (exits 2 with the usage when in.bin, out.f32 or the op is missing)
+  const char* op(const char* usage) const {
+    if (pos.size() < 3) { fprintf(stderr, "usage: %s\n", usage); exit(2); }
+    return pos[2];
+  }
+  const char* arg(size_t i) const { return i + 3 < pos.size() ? pos[i + 3] : nullptr; }
+  const char* get(const char* name) {
+    for (size_t i = 0; i < opts.size(); ++i)
+      if (opts[i].first == name) { used[i] = true; return opts[i].second; }
+    return nullptr;
+  }
+  double num(const char* name, double dflt) { const char* v = get(name); return v ? atof(v) : dflt; }
+  // every option given must have been read by now: a stale or misspelt one fails loudly
+  void done() const {
+    for (size_t i = 0; i < opts.size(); ++i)
+      if (!used[i]) { fprintf(stderr, "option --%s is not read by %s\n", opts[i].first.c_str(), pos[2]); exit(2); }
+  }
+};
+
+// --guard none|in|out: the range guard's sense (mp_query_dispatch)
+static int emu_guard(EmuArgs& a) {
+  const char* g = a.get("guard");
+  if (!g || !strcmp(g, "none")) return MP_GUARD_NONE;
+  if (!strcmp(g, "in")) return MP_GUARD_IN_RANGE;
+  if (!strcmp(g, "out")) return MP_GUARD_OUT_OF_RANGE;
+  fprintf(stderr, "--guard none|in|out, not %s\n", g);
+  exit(2);
+}
 
 // ---- in.bin ---------------------------------------------------------------------------------------------------------------
 struct EmuInput {
@@ -115,15 +169,25 @@ struct EmuMlp {
   std::vector<std::vector<float>> w, wt, b;
 };
 
-// mp_mlp_create's layout for the widths after the first (channels[0] = C + 1) with the head's weights from in.bin: W [cout][cin]
-// and the [cin][cout] copy transpose_w_kernel makes.  The feature limit of the range guard is EMU_TC_LIMIT (default +inf).
-static EmuMlp emu_make_mlp(EmuInput& in, const std::vector<int>& widths, bool skip = true) {
+// mp_mlp_create's layout for --widths (channels[0] = C + 1) with the head's weights from in.bin: W [cout][cin] and the
+// [cin][cout] copy transpose_w_kernel makes.  The feature limit of the range guard is --limit (default +inf).
+static EmuMlp emu_make_mlp(EmuInput& in, EmuArgs& a) {
+  std::vector<int> widths = {1024, 512, 256, 128, in.res};
+  bool skip = true;
+  if (const char* w = a.get("widths")) {
+    const char* s = w;
+    skip = strncmp(s, "noskip:", 7) != 0;
+    if (!skip) s += 7;
+    widths.clear();
+    for (char* e; *s && (int)widths.size() < MP_MAX_LAYERS; s = *e ? e + 1 : e) widths.push_back((int)strtol(s, &e, 10));
+    if (widths.empty() || *s || widths.back() != in.res) { fprintf(stderr, "bad widths %s (res %d)\n", w, in.res); exit(2); }
+  }
   EmuMlp m;
   memset(&m.mlp, 0, sizeof(m.mlp));
   const int L = (int)widths.size();
   m.mlp.n_layers = L; m.mlp.skip = skip; m.mlp.last_op = in.last_op;
   m.mlp.gen = 1;
-  m.mlp.tc_amax_limit = getenv("EMU_TC_LIMIT") ? (float)atof(getenv("EMU_TC_LIMIT")) : INFINITY;
+  m.mlp.tc_amax_limit = (float)a.num("limit", INFINITY);
   m.mlp.channels[0] = in.C + 1;
   for (int l = 0; l < L; ++l) m.mlp.channels[l + 1] = widths[l];
   m.w.resize(L); m.wt.resize(L); m.b.resize(L);
@@ -141,9 +205,6 @@ static EmuMlp emu_make_mlp(EmuInput& in, const std::vector<int>& widths, bool sk
   in.f = nullptr;
   return m;
 }
-
-// the shipped widths: 1024, 512, 256, 128, res
-static EmuMlp emu_make_mlp(EmuInput& in) { return emu_make_mlp(in, {1024, 512, 256, 128, in.res}); }
 
 struct EmuFeat {
   mp_feat feat;
@@ -226,13 +287,64 @@ static EmuVerts emu_vertex_rows(const EmuInput& in) {
   return v;
 }
 
-// the box [bx0 by0 bz0] .. [bx1 by1 bz1] of six command-line arguments
-static void emu_box_args(char** argv, float* bmin, float* bmax) {
-  for (int a = 0; a < 3; ++a) { bmin[a] = strtof(argv[a], nullptr); bmax[a] = strtof(argv[3 + a], nullptr); }
+// the box [bx0 by0 bz0] .. [bx1 by1 bz1] of the op's arguments i .. i+5
+static void emu_box_args(const EmuArgs& a, size_t i, float* bmin, float* bmax) {
+  for (int k = 0; k < 3; ++k) { bmin[k] = strtof(a.arg(i + k), nullptr); bmax[k] = strtof(a.arg(i + 3 + k), nullptr); }
+}
+
+// n floats of a side file (a grad_output); nullptr: none, the launchers' ones
+static std::vector<float> emu_read_file(const char* path, size_t n) {
+  if (!path) return {};
+  FILE* f = fopen(path, "rb");
+  if (!f) { perror(path); exit(2); }
+  std::vector<float> v = emu_read(f, n);
+  fclose(f);
+  return v;
 }
 
 static void emu_write(const char* path, const float* data, size_t n) {
   FILE* f = fopen(path, "wb");
   fwrite(data, 4, n, f);
   fclose(f);
+}
+
+// The output of an op: launch(bt, out) fills out -- n floats pre-filled with `fill`, then a -4242 sentinel that must
+// survive -- and returns the launcher's code; the n floats go to out.f32.  bt is null (the by-value camera) unless dcal:
+//   --dcal         the launch reads its camera from "device" memory -- a single-map MpBatch whose calibs point at one
+//                  12-float buffer holding in.bin's calib -- while MpCalib::m holds NaNs, so any read of the by-value
+//                  camera shows in the output;
+//   --dcal=<file>  two launches read that one buffer: the first with the file's 12 float32 (its output goes to
+//                  <out>.first), the second, after the buffer has been rewritten, with in.bin's (to out.f32).
+// An op that does not read --dcal passes dcal = nullptr.
+template <class Launch>
+static int emu_output(const EmuArgs& a, MpCalib& cal, const char* dcal, size_t n, float fill, Launch launch) {
+  a.done();
+  auto one = [&](const MpBatch* bt, const std::string& path) {
+    std::vector<float> out(n + 1, fill);
+    out[n] = -4242.f;
+    const int rc = launch(bt, out.data());
+    if (rc != MP_OK) { fprintf(stderr, "launch refused: %s (%d)\n", g_err, rc); exit(3); }
+    if (out[n] != -4242.f) { fprintf(stderr, "wrote past the output\n"); exit(3); }
+    emu_write(path.c_str(), out.data(), n);
+  };
+  if (!dcal) {
+    one(nullptr, a.pos[1]);
+    return 0;
+  }
+  static float buf[12];
+  float calib[12];
+  memcpy(calib, cal.m, sizeof(calib));
+  for (int k = 0; k < 12; ++k) cal.m[k] = NAN;
+  MpBatch bt;
+  bt.calibs = buf;
+  if (*dcal) {
+    FILE* f = fopen(dcal, "rb");
+    const bool ok = f && fread(buf, 4, 12, f) == 12;
+    if (f) fclose(f);
+    if (!ok) { fprintf(stderr, "--dcal: cannot read 12 floats from %s\n", dcal); exit(2); }
+    one(&bt, std::string(a.pos[1]) + ".first");
+  }
+  memcpy(buf, calib, sizeof(buf));
+  one(&bt, a.pos[1]);
+  return 0;
 }

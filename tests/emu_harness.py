@@ -1,8 +1,9 @@
 """The CPU model's plumbing, shared by the test modules: one g++ recipe for the harnesses of tests/emu (each compiled at most
-once per pytest run), the writer of the query harnesses' in.bin (its layout: tests/emu/emu_host.h), and the ptxas report of a
-library source compiled with the library's own flags."""
+once per pytest run), the writer of the query harnesses' in.bin (its layout: tests/emu/emu_host.h), one runner of the query
+harnesses, and the ptxas report of a library source compiled with the library's own flags."""
 import functools
 import os
+import pathlib
 import re
 import shutil
 import struct
@@ -11,6 +12,7 @@ import tempfile
 
 import numpy as np
 import pytest
+import torch
 
 from oracle import spec
 
@@ -22,13 +24,10 @@ needs_gxx = pytest.mark.skipif(not HAVE_GXX, reason="g++ not available")
 needs_emu = pytest.mark.skipif(not (HAVE_GXX and HAVE_CUDA_INC), reason="g++ / CUDA headers not available")
 
 # harness -> (optimisation level, includes the CUDA headers).  The query harnesses run 5-layer heads with one OS thread per
-# CUDA thread: -O3 for the tensor-core programs and the gradient, -O2 for the other exact-kernel harnesses (their results
-# are the same bits at every level: -ffp-contract=off and no fast-math); the integer / byte harnesses are light.
+# CUDA thread: -O3 (their results are the same bits at every level: -ffp-contract=off and no fast-math); the integer /
+# byte harnesses are light.
 HARNESSES = {
-    "emu_query_tc": ("-O3", True), "emu_query_jvp_tc": ("-O3", True), "emu_colour_surface_tc": ("-O3", True),
-    "emu_dcal_tc": ("-O3", True), "emu_query_grad": ("-O3", True),
-    "emu_query_fp32": ("-O2", True), "emu_heads_fp32": ("-O2", True), "emu_colour_surface_fp32": ("-O2", True),
-    "emu_dcal_fp32": ("-O2", True),
+    "emu_tc": ("-O3", True), "emu_fp32": ("-O3", True),
     "emu_mcubes": ("-O1", False), "emu_mcubes_async": ("-O1", False), "emu_scan": ("-O1", False),
     "emu_octree": ("-O1", False), "emu_octree_loop": ("-O1", False), "emu_surface": ("-O1", False),
     "emu_display": ("-O1", False), "emu_render_normals": ("-O1", False),
@@ -37,13 +36,16 @@ HARNESSES = {
 
 def build(tmp_path_factory, name):
     """The executable of tests/emu/<name>.cpp, compiled on first use in this session (skips without g++ or, for the query
-    harnesses, the CUDA headers)."""
+    harnesses, the CUDA headers).  tmp_path_factory: pytest's, or a directory to build into."""
     opt, cuda = HARNESSES[name]
     if not HAVE_GXX:
         pytest.skip("g++ not available")
     if cuda and not HAVE_CUDA_INC:
         pytest.skip("CUDA headers not found")
-    exe = tmp_path_factory.getbasetemp() / "emu_bin" / name
+    if isinstance(tmp_path_factory, (str, pathlib.Path)):
+        exe = pathlib.Path(tmp_path_factory) / name
+    else:
+        exe = tmp_path_factory.getbasetemp() / "emu_bin" / name
     if not exe.exists():
         exe.parent.mkdir(exist_ok=True)
         # the kernels type-pun registers through reinterpret_cast like all CUDA code: no strict aliasing on the host build
@@ -53,6 +55,45 @@ def build(tmp_path_factory, name):
         r = subprocess.run(cmd, capture_output=True, text=True)
         assert r.returncode == 0, r.stderr[-3000:]
     return str(exe)
+
+
+def _side_file(path, x):
+    np.ascontiguousarray(x.numpy() if isinstance(x, torch.Tensor) else x, dtype=np.float32).tofile(path)
+    return str(path)
+
+
+def run(exe, tmp_path, op, *args, inp, shape, options=None, env=None, tag="x", returncode=0):
+    """One run of a query harness (tests/emu/emu_fp32.cpp or emu_tc.cpp): in.bin = write_input(**inp), then
+    `exe in.bin out.f32 op args --options`.  An array among args, or as an option's value, goes to a side file (a
+    grad_output, a --dcal camera) whose path takes its place.  options: {name: value} (canvas_bg for --canvas-bg), True
+    for a flag, None / False to leave it out.  env: the model's own knobs (EMU_TC_ORDER ...).  tag keeps the files of
+    several runs in one tmp_path apart.
+    -> (out, the finished process): out = out.f32 as a float32 tensor of `shape` (shape None: its raw bytes; None when
+    the harness is expected to fail with `returncode`)."""
+    fin, fout = tmp_path / ("in_%s.bin" % tag), tmp_path / ("out_%s.f32" % tag)
+    write_input(fin, **inp)
+    argv = [exe, str(fin), str(fout), op]
+    for i, a in enumerate(args):
+        is_array = isinstance(a, (np.ndarray, torch.Tensor))
+        argv.append(_side_file(tmp_path / ("arg%d_%s.f32" % (i, tag)), a) if is_array else str(a))
+    for k, v in (options or {}).items():
+        if isinstance(v, (np.ndarray, torch.Tensor)):
+            v = _side_file(tmp_path / ("%s_%s.f32" % (k, tag)), v)
+        if v is True:
+            argv.append("--" + k.replace("_", "-"))
+        elif v is not None and v is not False:
+            argv.append("--%s=%s" % (k.replace("_", "-"), v))
+    if fout.exists():
+        fout.unlink()
+    r = subprocess.run(argv, capture_output=True, text=True, timeout=3600, env=dict(os.environ, **(env or {})))
+    assert r.returncode == returncode and "DEADLOCK" not in r.stderr, r.stderr[-2000:]
+    if returncode:
+        return None, r
+    if shape is None:
+        return fout.read_bytes(), r
+    out = np.fromfile(fout, dtype=np.float32)
+    assert out.size == int(np.prod(shape)), (out.size, shape)
+    return torch.from_numpy(out).reshape(shape), r
 
 
 def write_input(path, feat, rows, calib, proj, res, last_op, Ws, bs, batched=False):

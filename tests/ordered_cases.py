@@ -1,6 +1,6 @@
 """The ordered feature gradient of the training query (MP_VJP_DETERMINISTIC, DESIGN §F1⁗): inputs that crowd the points of an
 image into one cell of its map, beside points on the map's last row and column and outside the image, and a restatement of
-the documented summation order over a dump of one chunk (tests/emu/emu_query_vjp_det.cpp, EMU_VJP_DUMP)."""
+the documented summation order over a dump of one chunk (the --dump option of tests/emu/emu_fp32.cpp's vjp op)."""
 from fractions import Fraction
 
 import numpy as np
@@ -54,7 +54,7 @@ def fma32(w, x, acc):
 
 
 def read_dump(path):
-    """EMU_VJP_DUMP -> (dX [cols, C], weights [cols, 4], sorted keys [cols], their columns [cols])"""
+    """a --dump file -> (dX [cols, C], weights [cols, 4], sorted keys [cols], their columns [cols])"""
     raw = open(path, "rb").read()
     cols, C = np.frombuffer(raw[:16], dtype=np.int64)
     o = 16

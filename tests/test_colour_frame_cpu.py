@@ -10,24 +10,23 @@ import pytest
 import torch
 
 from oracle import spec
-from emu_harness import build, needs_emu, ptxas_report, write_input
+from emu_harness import build, needs_emu, ptxas_report, run
 
 pytestmark = needs_emu
 
 R = 65
 UNIT = ((-1.0, -1.0, -1.0), (1.0, 1.0, 1.0))
 B1 = ((-0.83, -1.17, -0.61), (0.91, 1.06, 0.77))     # asymmetric, no power-of-two extent: the axes cannot stand in for each other
-GUARD_NONE, GUARD_IN_RANGE, GUARD_OUT_OF_RANGE = 0, 1, 2
 
 
 @pytest.fixture(scope="module")
 def emu_tc(tmp_path_factory):
-    return build(tmp_path_factory, "emu_colour_surface_tc")
+    return build(tmp_path_factory, "emu_tc")
 
 
 @pytest.fixture(scope="module")
 def emu_fp32(tmp_path_factory):
-    return build(tmp_path_factory, "emu_colour_surface_fp32")
+    return build(tmp_path_factory, "emu_fp32")
 
 
 @pytest.fixture(scope="module")
@@ -48,36 +47,29 @@ def scene():
     return dict(Ws=Ws, bs=bs, feat=feat, cal=cal, X=X, Y=Y, Z=Z)
 
 
-def _write(path, sc, rows, feat=None):
-    """emu input: header, z_scale, calib, the map, three rows of N floats, the head"""
-    write_input(path, sc["feat"] if feat is None else feat, rows, sc["cal"], "orthogonal", 3, spec.LAST_TANH, sc["Ws"], sc["bs"])
+def _input(sc, rows, feat=None):
+    """the harnesses' in.bin: the colour head and map, three rows of N floats"""
+    return dict(feat=sc["feat"] if feat is None else feat, rows=rows, calib=sc["cal"], proj="orthogonal", res=3,
+                last_op=spec.LAST_TANH, Ws=sc["Ws"], bs=sc["bs"])
 
 
 def _vertex_rows(sc, n=200):
     return torch.stack([sc["X"][:n].float(), sc["Y"][:n].float(), sc["Z"][:n]]).numpy()
 
 
-def _run(args, env=None, out_shape=(R, R, 3)):
-    r = subprocess.run(args, capture_output=True, text=True, timeout=1800, env=dict(os.environ, **(env or {})))
-    assert r.returncode == 0, r.stderr[-2000:]
-    return torch.from_numpy(np.fromfile(args[2], dtype=np.float32)).reshape(out_shape), r.stdout
-
-
 def _box_args(box):
     return ["%.9g" % np.float32(v) for v in box[0] + box[1]]
 
 
-def _fp32_surface(exe, tmp_path, sc, count, sms=3, n=200, env=None, feat=None, box=UNIT):
-    fin, fout = str(tmp_path / "s.bin"), str(tmp_path / "s.f32")
-    _write(fin, sc, _vertex_rows(sc, n), feat)
-    return _run([exe, fin, fout, str(sms), "surface", str(R), str(count)] + _box_args(box), env)[0]
+def _fp32_surface(exe, tmp_path, sc, count, sms=3, n=200, feat=None, box=UNIT, **options):
+    return run(exe, tmp_path, "surface", R, count, *_box_args(box), inp=_input(sc, _vertex_rows(sc, n), feat), shape=(R, R, 3),
+               options=dict(sms=sms, **options))[0]
 
 
-def _tc_surface(exe, tmp_path, sc, count, sms=2, n=200, env=None, host=False, feat=None, box=UNIT):
-    fin, fout = str(tmp_path / "t.bin"), str(tmp_path / "t.f32")
-    _write(fin, sc, _vertex_rows(sc, n), feat)
-    img, out = _run([exe, fin, fout, str(sms), str(R), str(count)] + _box_args(box) + (["host"] if host else []), env)
-    return img, float(out.split()[0])
+def _tc_surface(exe, tmp_path, sc, count, sms=2, n=200, host=False, feat=None, box=UNIT, **options):
+    img, r = run(exe, tmp_path, "surface", R, count, *_box_args(box), inp=_input(sc, _vertex_rows(sc, n), feat),
+                 shape=(R, R, 3), options=dict(sms=sms, eager=host, print_amax=True, **options))
+    return img, float(r.stdout.split()[0])
 
 
 def _want(sc, n=200, box=UNIT):
@@ -112,9 +104,7 @@ def test_exact_surface_render_is_the_rows_query_plus_scatter(emu_fp32, tmp_path,
         v = _vertex_rows(scene).astype(f32)
         v[2] = f32(R) - v[2]
         world = (v * scale).astype(f32) + lo[:, None]
-        fin, fout = str(tmp_path / "w.bin"), str(tmp_path / "w.f32")
-        _write(fin, scene, world)
-        vals = _run([emu_fp32, fin, fout, "3", "rows"], out_shape=(3, 200))[0].numpy()
+        vals = run(emu_fp32, tmp_path, "query", inp=_input(scene, world), shape=(3, 200), tag="w")[0].numpy()
         want = np.ones((R, R, 3), f32)
         want[scene["X"].numpy(), scene["Y"].numpy(), :] = ((vals * f32(0.5)).astype(f32) + f32(0.5)).T
         assert np.array_equal(got.numpy().view(np.int32), want.view(np.int32)), box
@@ -125,13 +115,13 @@ def test_exact_surface_render_device_count(emu_fp32, tmp_path, scene):
     valid vertices, whose pixels must keep the background), a count of 0 leaves the canvas untouched, and a count above the
     capacity is clamped to it."""
     n = 120
-    got = _fp32_surface(emu_fp32, tmp_path, scene, 90, n=n, env={"EMU_CANVAS_BG": "0.25"})
-    full = _fp32_surface(emu_fp32, tmp_path, scene, n, n=n, env={"EMU_CANVAS_BG": "0.25"})
+    got = _fp32_surface(emu_fp32, tmp_path, scene, 90, n=n, canvas_bg=0.25)
+    full = _fp32_surface(emu_fp32, tmp_path, scene, n, n=n, canvas_bg=0.25)
     X, Y = scene["X"], scene["Y"]
     assert torch.equal(got[X[:90], Y[:90]], full[X[:90], Y[:90]])
     assert bool((got[X[90:n], Y[90:n]] == 0.25).all()) and bool((full[X[90:n], Y[90:n]] != 0.25).all())
     assert bool((_fp32_surface(emu_fp32, tmp_path, scene, 0, n=n) == 1.0).all())
-    assert torch.equal(_fp32_surface(emu_fp32, tmp_path, scene, 10 ** 9, n=n, env={"EMU_CANVAS_BG": "0.25"}), full)
+    assert torch.equal(_fp32_surface(emu_fp32, tmp_path, scene, 10 ** 9, n=n, canvas_bg=0.25), full)
 
 
 @pytest.mark.parametrize("limit,writes", [("1.0", True), ("100.0", False)])
@@ -139,7 +129,7 @@ def test_exact_surface_render_guard_sense(emu_fp32, tmp_path, scene, limit, writ
     """MP_GUARD_OUT_OF_RANGE: the exact twin renders a frame whose max |feature| (here 5) is above the head's limit and
     leaves the canvas of an in-range frame to the tensor-core launch."""
     got = _fp32_surface(emu_fp32, tmp_path, scene, 40, n=40,
-                        env={"EMU_GUARD": str(GUARD_OUT_OF_RANGE), "EMU_TC_LIMIT": limit, "EMU_AMAX": "5.0"})
+                        guard="out", limit=limit, amax=5.0)
     assert bool((got == 1.0).all()) != writes
 
 
@@ -151,13 +141,13 @@ def test_tc_surface_render_device_count_equals_host_count(emu_tc, tmp_path, scen
     n, k = 130, 100
     X, Y = scene["X"], scene["Y"]
     for box in (B1, UNIT):
-        dev, _ = _tc_surface(emu_tc, tmp_path, scene, k, n=n, env={"EMU_CANVAS_BG": "0.25"}, box=box)
-        host, _ = _tc_surface(emu_tc, tmp_path, scene, k, n=n, host=True, env={"EMU_CANVAS_BG": "0.25"}, box=box)
+        dev, _ = _tc_surface(emu_tc, tmp_path, scene, k, n=n, canvas_bg=0.25, box=box)
+        host, _ = _tc_surface(emu_tc, tmp_path, scene, k, n=n, host=True, canvas_bg=0.25, box=box)
         assert torch.equal(dev, host)
         assert bool((dev[X[k:n], Y[k:n]] == 0.25).all())
         assert (dev[X[:k], Y[:k]] - _want(scene, k, box)[X[:k], Y[:k]]).abs().max().item() <= 1e-4, box
-    clamped, _ = _tc_surface(emu_tc, tmp_path, scene, 10 ** 9, n=n, env={"EMU_CANVAS_BG": "0.25"})
-    host_all, _ = _tc_surface(emu_tc, tmp_path, scene, n, n=n, host=True, env={"EMU_CANVAS_BG": "0.25"})
+    clamped, _ = _tc_surface(emu_tc, tmp_path, scene, 10 ** 9, n=n, canvas_bg=0.25)
+    host_all, _ = _tc_surface(emu_tc, tmp_path, scene, n, n=n, host=True, canvas_bg=0.25)
     assert torch.equal(clamped, host_all)
     zero, _ = _tc_surface(emu_tc, tmp_path, scene, 0, n=n)
     assert bool((zero == 1.0).all())
@@ -167,7 +157,7 @@ def test_tc_surface_render_device_count_equals_host_count(emu_tc, tmp_path, scen
 def test_tc_surface_render_guard_sense(emu_tc, tmp_path, scene, limit, writes):
     """MP_GUARD_IN_RANGE: the tensor-core launch renders a frame whose max |feature| is inside the head's limit and leaves
     the canvas of a frame above it untouched (the exact twin renders that one)."""
-    got, amax = _tc_surface(emu_tc, tmp_path, scene, 40, n=40, env={"EMU_TC_GUARD": str(GUARD_IN_RANGE), "EMU_TC_LIMIT": limit})
+    got, amax = _tc_surface(emu_tc, tmp_path, scene, 40, n=40, guard="in", limit=limit)
     assert abs(amax - scene["feat"].abs().max().item()) <= 1e-6 * amax
     assert bool((got == 1.0).all()) != writes
 

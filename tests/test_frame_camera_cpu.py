@@ -1,18 +1,15 @@
 """CPU tier of the per-frame camera: every program a captured frame launches, compiled unmodified against the CPU emulation
 layer (tests/emu), reads its camera from device memory (a single-map MpBatch whose calibs point at a 12-float buffer, the
-EMU_DCAL flag of tests/emu/emu_dcal_fp32.cpp and emu_dcal_tc.cpp) and must give, bit for bit, what its by-value launch gives with the same 12 floats -- the exact
-query over a node list with the volume scatter, the tensor-core query over a node list and over a grid range, the colour
-surface render of both programs, and both gradient programs.  Every case runs two launches through one buffer rewritten
-between them, and each must give its own camera's result."""
-import os
-import subprocess
-
+--dcal option of tests/emu/emu_fp32.cpp and emu_tc.cpp) and must give, bit for bit, what its by-value launch gives with the
+same 12 floats -- the exact query over a node list with the volume scatter, the tensor-core query over a node list and over
+a grid range, the colour surface render of both programs, and both gradient programs.  Every case runs two launches
+through one buffer rewritten between them, and each must give its own camera's result."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import spec
-from emu_harness import build, needs_emu, write_input
+from emu_harness import build, needs_emu, run
 from grad_cases import load_grad_case
 
 pytestmark = needs_emu
@@ -23,7 +20,7 @@ UNIT = ["-1", "-1", "-1", "1", "1", "1"]
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return {k: build(tmp_path_factory, "emu_dcal_" + k) for k in ("fp32", "tc")}
+    return {k: build(tmp_path_factory, "emu_" + k) for k in ("fp32", "tc")}
 
 
 def _case(name, proj):
@@ -42,30 +39,17 @@ def _second_camera(c):
     return spec.scene_calib(20, 63)
 
 
-def _write(path, c, rows, calib=None):
-    """in.bin of the harnesses: header, z_scale, calib rows 0..2, the map, three rows of N floats, the head"""
-    write_input(path, c["feat"], rows, c["calib"] if calib is None else calib, c["proj"], c["chans"][-1], c["last_op"], c["Ws"],
-                c["bs"])
-
-
-def _run(tmp_path, tag, exe, args, c, rows, env=None):
+def _run(tmp_path, tag, exe, args, c, rows, sms, size):
     """the by-value launches with camera A (the case's) and camera B, and the device-calib pair (B, then A) through one
-    buffer -> the four outputs as raw float32 arrays"""
+    buffer (--dcal) -> the four outputs as raw float32 arrays of `size` floats"""
     cal_b = _second_camera(c)
-    fa, fb = (str(tmp_path / ("%s_%s.bin" % (tag, k))) for k in "ab")
-    _write(fa, c, rows)
-    _write(fb, c, rows, cal_b)
-    first = str(tmp_path / ("%s_first.f32" % tag))
-    np.asarray(cal_b[0, :3, :4].reshape(-1).tolist(), dtype=np.float32).tofile(first)
     outs = {}
-    for key, fin, extra in (("a", fa, {}), ("b", fb, {}), ("d", fa, {"EMU_DCAL": first})):
-        fout = str(tmp_path / ("%s_out_%s.f32" % (tag, key)))
-        r = subprocess.run([exe, fin, fout] + args, capture_output=True, text=True, timeout=3600,
-                           env=dict(os.environ, **(env or {}), **extra))
-        assert r.returncode == 0 and "DEADLOCK" not in r.stderr, r.stderr[-2000:]
-        outs[key] = np.fromfile(fout, dtype=np.float32)
-        if key == "d":
-            outs["d_first"] = np.fromfile(fout + ".first", dtype=np.float32)
+    for key, calib, dcal in (("a", c["calib"], None), ("b", cal_b, None), ("d", c["calib"], cal_b[0, :3, :4].reshape(-1))):
+        inp = dict(feat=c["feat"], rows=rows, calib=calib, proj=c["proj"], res=c["chans"][-1], last_op=c["last_op"],
+                   Ws=c["Ws"], bs=c["bs"])
+        out, _ = run(exe, tmp_path, *args, inp=inp, shape=(size,), options=dict(sms=sms, dcal=dcal), tag=tag + key)
+        outs[key] = out.numpy()
+    outs["d_first"] = np.fromfile(str(tmp_path / ("out_%sd.f32.first" % tag)), dtype=np.float32)   # (run's out.f32 + .first)
     return outs
 
 
@@ -85,7 +69,7 @@ def _points(c, n):
 @pytest.mark.parametrize("proj,sms", [("orthogonal", 1), ("orthogonal", 3), ("perspective", 2)])
 def test_exact_nodes_scatter(emu, tmp_path, proj, sms):
     c = _case("g_rot", proj)
-    outs = _run(tmp_path, "fn", emu["fp32"], [str(sms), "nodes", "17", "9"], c, _points(c, 8))
+    outs = _run(tmp_path, "fn", emu["fp32"], ["nodes", 17, 9], c, _points(c, 8), sms, 9 ** 3)
     assert outs["a"].size == 9 ** 3
     _assert_bits(outs)
 
@@ -95,8 +79,8 @@ def test_exact_nodes_scatter(emu, tmp_path, proj, sms):
                                           ("grid", "orthogonal", 1), ("grid", "perspective", 2)])
 def test_tc_nodes_and_grid(emu, tmp_path, src, proj, sms):
     c = _case("g_rot", proj)
-    args = [str(sms)] + (["nodes", "17", "5"] if src == "nodes" else ["grid", "9", "3", "2"])
-    outs = _run(tmp_path, "t" + src, emu["tc"], args, c, _points(c, 8))
+    args, size = (["nodes", 17, 5], 5 ** 3) if src == "nodes" else (["grid", 9, 3, 2], 2 * 9 * 9)
+    outs = _run(tmp_path, "t" + src, emu["tc"], args, c, _points(c, 8), sms, size)
     assert outs["a"].size == (5 ** 3 if src == "nodes" else 2 * 9 * 9)
     _assert_bits(outs)
 
@@ -113,11 +97,8 @@ def _vertex_rows(n=120, seed=7):
 def test_colour_surface(emu, tmp_path, program, proj, sms):
     c = _case("c_rot", proj)
     rows = _vertex_rows()
-    count = str(rows.shape[1] - 5)                # (the count on the device, below the capacity)
-    if program == "fp32":
-        outs = _run(tmp_path, "sf", emu["fp32"], [str(sms), "surface", str(R), count] + UNIT, c, rows)
-    else:
-        outs = _run(tmp_path, "st", emu["tc"], [str(sms), "surface", str(R), count] + UNIT, c, rows)
+    count = rows.shape[1] - 5                     # (the count on the device, below the capacity)
+    outs = _run(tmp_path, "s" + program[0], emu[program], ["surface", R, count] + UNIT, c, rows, sms, R * R * 3)
     assert outs["a"].size == R * R * 3
     _assert_bits(outs)
 
@@ -126,14 +107,14 @@ def test_colour_surface(emu, tmp_path, program, proj, sms):
 @pytest.mark.parametrize("proj,sms", [("orthogonal", 1), ("orthogonal", 3), ("perspective", 2)])
 def test_exact_gradient(emu, tmp_path, proj, sms):
     c = _case("g_rot", proj)
-    outs = _run(tmp_path, "g", emu["fp32"], [str(sms), "grad"], c, _points(c, 37))
+    outs = _run(tmp_path, "g", emu["fp32"], ["grad"], c, _points(c, 37), sms, 4 * 37)
     _assert_bits(outs, min_distinct=37)
 
 
 @pytest.mark.parametrize("proj,sms", [("orthogonal", 2), ("perspective", 1), ("perspective", 3)])
 def test_tc_gradient(emu, tmp_path, proj, sms):
     c = _case("g_rot", proj)
-    outs = _run(tmp_path, "j", emu["tc"], [str(sms), "jvp"], c, _points(c, 35))
+    outs = _run(tmp_path, "j", emu["tc"], ["jvp"], c, _points(c, 35), sms, 4 * 35)
     _assert_bits(outs, min_distinct=35)
     # the gradient rows (after the value row) differ too: the Jacobian reads the buffer as well
     a, b = outs["a"][35:], outs["b"][35:]

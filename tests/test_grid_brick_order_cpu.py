@@ -1,27 +1,23 @@
 """CPU model of the brick order of the in-image list (mp_launch_query_tc_grid in query_tc.cu, compiled unmodified by
-tests/emu/emu_query_grid_brick.cpp): the compaction scans a brick-major index space over the brick layers that the
+the grid-brick op of tests/emu/emu_tc.cpp): the compaction scans a brick-major index space over the brick layers that the
 range's z planes cross.  On ranges whose ends are not on a plane, it must list each in-image node of the range exactly
 once, in 4x4x4-brick order, give every other node of the range +0, touch nothing else, and leave the volume of the
 dense launch bit for bit."""
 import struct
-import subprocess
 
 import numpy as np
 import pytest
 
-import emu_harness
-from emu_harness import needs_emu, write_input
+from emu_harness import build, needs_emu, run
 from oracle import spec
 from tools.tile_texels import brick_order
-
-emu_harness.HARNESSES.setdefault("emu_query_grid_brick", ("-O3", True))
 
 pytestmark = needs_emu
 
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    return emu_harness.build(tmp_path_factory, "emu_query_grid_brick")
+    return build(tmp_path_factory, "emu_tc")
 
 
 def _run(harness, tmp_path, R, lin0, n, sms=3, feat_edit=None):
@@ -31,12 +27,9 @@ def _run(harness, tmp_path, R, lin0, n, sms=3, feat_edit=None):
     feat = torch.nn.functional.avg_pool2d(feats[0], 4)[0].numpy()     # (a 32 x 32 map keeps the per-frame products cheap)
     if feat_edit is not None:
         feat = feat_edit(feat.copy())
-    fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.bin")
-    write_input(fin, feat, np.zeros((3, 1), np.float32), bench.scene_calib().numpy(), "orthogonal", 1, spec.LAST_SIGMOID,
-                Ws, bs)
-    r = subprocess.run([harness, fin, fout, str(sms), str(R), str(lin0), str(n)], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-2000:]
-    raw = open(fout, "rb").read()
+    inp = dict(feat=feat, rows=np.zeros((3, 1), np.float32), calib=bench.scene_calib().numpy(), proj="orthogonal", res=1,
+               last_op=spec.LAST_SIGMOID, Ws=Ws, bs=bs)
+    raw, _ = run(harness, tmp_path, "grid-brick", R, lin0, n, inp=inp, shape=None, options=dict(sms=sms))
     count, size = struct.unpack("2q", raw[:16])
     assert 0 <= count <= n, count
     o = 16

@@ -1,24 +1,19 @@
-"""CPU model of the in-image grid launch (mp_launch_query_tc_grid in query_tc.cu, compiled unmodified by
-tests/emu/emu_query_grid_in_image.cpp): the ordered compaction lists the nodes of a grid range that project into the image
-and stores +0 for the others, and the tensor-core program runs over the list.  The range must equal the dense MP_SRC_GRID
-launch bit for bit, compared as int32 views so that the sign of zero counts."""
-import subprocess
-
+"""CPU model of the in-image grid launch (mp_launch_query_tc_grid in query_tc.cu, compiled unmodified by the grid-in-image
+op of tests/emu/emu_tc.cpp): the ordered compaction lists the nodes of a grid range that project into the image and stores
++0 for the others, and the tensor-core program runs over the list.  The range must equal the dense MP_SRC_GRID launch bit
+for bit, compared as int32 views so that the sign of zero counts."""
 import numpy as np
 import pytest
 
-import emu_harness
-from emu_harness import needs_emu, write_input
+from emu_harness import build, needs_emu, run
 from oracle import spec
-
-emu_harness.HARNESSES.setdefault("emu_query_grid_in_image", ("-O3", True))
 
 pytestmark = needs_emu
 
 
 @pytest.fixture(scope="module")
 def harness(tmp_path_factory):
-    return emu_harness.build(tmp_path_factory, "emu_query_grid_in_image")
+    return build(tmp_path_factory, "emu_tc")
 
 
 def _bench_head_and_map():
@@ -34,12 +29,10 @@ def _run(harness, tmp_path, calib, R, lin0, n, sms=3, feat_edit=None, peers=Fals
     Ws, bs, feat = _bench_head_and_map()
     if feat_edit is not None:
         feat = feat_edit(feat.copy())
-    fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    write_input(fin, feat, np.zeros((3, 1), np.float32), calib, "orthogonal", 1, spec.LAST_SIGMOID, Ws, bs)
-    args = [harness, fin, fout, str(sms), str(R), str(lin0), str(n)] + (["peers"] if peers else [])
-    r = subprocess.run(args, capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = np.fromfile(fout, dtype=np.int32).reshape(2, n)
+    inp = dict(feat=feat, rows=np.zeros((3, 1), np.float32), calib=calib, proj="orthogonal", res=1, last_op=spec.LAST_SIGMOID,
+               Ws=Ws, bs=bs)
+    out, r = run(harness, tmp_path, "grid-in-image", R, lin0, n, inp=inp, shape=(2, n), options=dict(sms=sms, peers=peers))
+    out = out.numpy().view(np.int32)
     return out[0], out[1], int(r.stdout.split()[-1])
 
 

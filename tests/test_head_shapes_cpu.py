@@ -3,16 +3,14 @@ points, the two exactly full tiles and the next width up, widths that are not mu
 one layer and eight, outputs other than 1 and 3, no last op, no skip inputs -- through the exact kernels of query_fp32.cu
 compiled unmodified on the CPU model of tests/emu (the query, the point gradient and the surface render), against the
 reference and the restatement.  And the tensor-core program's default feature limit per last op, on the shipped widths."""
-import os
 import subprocess
 
-import numpy as np
 import pytest
 import torch
 
 from oracle import spec
 from grad_cases import query_grad_ref, within_bar
-from emu_harness import build, write_input
+from emu_harness import build, run
 from head_cases import (fp32_tile, head_cases, head_grad_cases, head_widths, load_head_case, load_head_grad_case,
                         shipped_widths)
 
@@ -25,20 +23,15 @@ def _widths(chans, no_residual=False):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return dict(heads=build(tmp_path_factory, "emu_heads_fp32"), tc=build(tmp_path_factory, "emu_query_tc"))
+    return dict(fp32=build(tmp_path_factory, "emu_fp32"), tc=build(tmp_path_factory, "emu_tc"))
 
 
-def _launch(exe, tmp_path, c, n, mode, sms=3, extra=(), widths=None, points=None):
-    """-> (returncode, stdout, stderr, out array or None)"""
-    fin, fout = str(tmp_path / "h.bin"), str(tmp_path / "h.f32")
-    pts = c["points"][:, :, :n] if points is None else points
-    write_input(fin, c["feat"], pts, c["calib"], c["proj"], c["chans"][-1], c["last_op"], c["Ws"], c["bs"])
-    if os.path.exists(fout):
-        os.remove(fout)
-    r = subprocess.run([exe, fin, fout, widths or _widths(c["chans"]), str(sms), mode] + [str(a) for a in extra],
-                       capture_output=True, text=True, timeout=3600)
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32)) if r.returncode == 0 else None
-    return r.returncode, r.stdout, r.stderr, out
+def _launch(exe, tmp_path, c, n, op, shape, sms=3, extra=(), widths=None, points=None, returncode=0):
+    """-> (out, the finished process) of emu_fp32 with the head's widths"""
+    inp = dict(feat=c["feat"], rows=c["points"][:, :, :n] if points is None else points, calib=c["calib"], proj=c["proj"],
+               res=c["chans"][-1], last_op=c["last_op"], Ws=c["Ws"], bs=c["bs"])
+    return run(exe, tmp_path, op, *extra, inp=inp, shape=shape, options=dict(widths=widths or _widths(c["chans"]), sms=sms),
+               returncode=returncode)
 
 
 def _tiles(stdout):
@@ -46,16 +39,14 @@ def _tiles(stdout):
 
 
 def _query(exe, tmp_path, c, n, sms=3):
-    rc, so, se, out = _launch(exe, tmp_path, c, n, "query", sms)
-    assert rc == 0, se[-2000:]
-    return out.reshape(c["chans"][-1], n), _tiles(so)
+    out, r = _launch(exe, tmp_path, c, n, "query", (c["chans"][-1], n), sms)
+    return out, _tiles(r.stdout)
 
 
 def _grad(exe, tmp_path, c, n, sms=3):
-    rc, so, se, out = _launch(exe, tmp_path, c, n, "grad", sms)
-    assert rc == 0, se[-2000:]
     res = c["chans"][-1]
-    return out[:res * n].reshape(res, n), out[res * n:].reshape(3, n), _tiles(so)
+    out, r = _launch(exe, tmp_path, c, n, "grad", ((res + 3) * n,), sms)
+    return out[:res * n].reshape(res, n), out[res * n:].reshape(3, n), _tiles(r.stdout)
 
 
 def _fp32_heads():
@@ -110,7 +101,7 @@ def _n(c):
 def test_fp32_kernel_matches_head_golden(emu, tmp_path, name):
     """within 2e-5 * max(1, max|ref|) of the reference, out-of-image points exactly 0, and the tile the footprint predicts"""
     c = load_head_case(name)
-    got, tiles = _query(emu["heads"], tmp_path, c, _n(c))
+    got, tiles = _query(emu["fp32"], tmp_path, c, _n(c))
     want = c["expected"]
     err = (got - want).abs().max().item()
     assert err <= 2e-5 * max(1.0, want.abs().max().item()), err
@@ -125,13 +116,13 @@ def test_grad_kernel_matches_head_golden(emu, tmp_path, name):
     gradient's tile the footprint predicts (the masks and g make it smaller than the query's for p32_full)"""
     c = load_head_grad_case(name)
     n = _n(c)
-    val, dp, tiles = _grad(emu["heads"], tmp_path, c, n)
+    val, dp, tiles = _grad(emu["fp32"], tmp_path, c, n)
     assert (val - c["value"]).abs().max().item() <= 2e-5 * max(1.0, c["value"].abs().max().item())
     ok, msg = within_bar(dp, c["grad32"])
     assert ok, msg
     ok, msg = within_bar(dp, c["grad64"])
     assert ok, "against fp64: " + msg
-    q, _ = _query(emu["heads"], tmp_path, c, n)
+    q, _ = _query(emu["fp32"], tmp_path, c, n)
     assert torch.equal(val, q)
     assert tiles == [fp32_tile(c["chans"]), fp32_tile(c["chans"], grad=True)]
 
@@ -141,8 +132,8 @@ def test_results_do_not_depend_on_the_sm_count(emu, tmp_path, name):
     """1, 2 and 3 simulated SMs (one CTA walks all 17 tiles, or they interleave): the same bits, query and gradient"""
     c = load_head_grad_case(name)
     n = _n(c)
-    q = [_query(emu["heads"], tmp_path, c, n, sms)[0] for sms in (1, 2, 3)]
-    g = [_grad(emu["heads"], tmp_path, c, n, sms)[1] for sms in (1, 2, 3)]
+    q = [_query(emu["fp32"], tmp_path, c, n, sms)[0] for sms in (1, 2, 3)]
+    g = [_grad(emu["fp32"], tmp_path, c, n, sms)[1] for sms in (1, 2, 3)]
     assert torch.equal(q[0], q[1]) and torch.equal(q[0], q[2])
     assert torch.equal(g[0], g[1]) and torch.equal(g[0], g[2])
 
@@ -161,9 +152,8 @@ def test_surface_render_of_a_three_output_head(emu, tmp_path, name):
     X, Y = cols // R_CANVAS, cols % R_CANVAS
     Z = torch.rand(n, generator=g) * (R_CANVAS - 1)
     rows = torch.stack([X.float(), Y.float(), Z])[None]
-    rc, _, se, out = _launch(emu["heads"], tmp_path, c, n, "surface", 2, [R_CANVAS, -1, -1, -1, 1, 1, 1], points=rows)
-    assert rc == 0, se[-2000:]
-    got = out.reshape(R_CANVAS, R_CANVAS, 3)
+    got, _ = _launch(emu["fp32"], tmp_path, c, n, "surface", (R_CANVAS, R_CANVAS, 3), 2, [R_CANVAS, n, -1, -1, -1, 1, 1, 1],
+                     points=rows)
 
     def query_c(points, calib):
         return spec.query_ref(c["feat"], points, calib, c["Ws"], c["bs"], c["last_op"], c["proj"])
@@ -190,16 +180,16 @@ def _zero_head(chans, last_op=spec.LAST_SIGMOID):
     ([1025, 4096, 2071, 1], "grad", "gradient kernel"),       # p8_full: its query runs, its gradient does not fit
 ])
 def test_one_past_each_fit_is_refused(emu, tmp_path, chans, mode, what):
-    rc, _, se, _ = _launch(emu["heads"], tmp_path, _zero_head(chans), 8, mode)
-    assert rc == 3 and "head too wide for the %s's shared-memory tiling (-3)" % what in se, se
+    _, r = _launch(emu["fp32"], tmp_path, _zero_head(chans), 8, mode, None, returncode=3)
+    assert r.returncode == 3 and "head too wide for the %s's shared-memory tiling (-3)" % what in r.stderr, r.stderr
 
 
 @pytest.mark.parametrize("mode", ["query", "grad"])
 def test_no_residual_head_is_refused(emu, tmp_path, mode):
     c = load_head_case("narrow")
     nr = dict(c, Ws=[torch.zeros(c["chans"][l + 1], c["chans"][l]) for l in range(3)])
-    rc, _, se, _ = _launch(emu["heads"], tmp_path, nr, 8, mode, widths=_widths(c["chans"], no_residual=True))
-    assert rc == 3 and "no_residual heads are not supported (-3)" in se, se
+    _, r = _launch(emu["fp32"], tmp_path, nr, 8, mode, None, widths=_widths(c["chans"], no_residual=True), returncode=3)
+    assert r.returncode == 3 and "no_residual heads are not supported (-3)" in r.stderr, r.stderr
 
 
 # ---- the tensor-core program's default feature limit, per last op -------------------------------------------------------
@@ -210,8 +200,8 @@ def _default_limit(exe, res, last_op):
 
 
 def test_shipped_pairs_keep_their_limits(emu):
-    assert _default_limit(emu["heads"], 1, spec.LAST_SIGMOID) == 12.0
-    assert _default_limit(emu["heads"], 3, spec.LAST_TANH) == 8.0
+    assert _default_limit(emu["fp32"], 1, spec.LAST_SIGMOID) == 12.0
+    assert _default_limit(emu["fp32"], 3, spec.LAST_TANH) == 8.0
 
 
 @pytest.mark.parametrize("seed", [0, 1])
@@ -222,16 +212,13 @@ def test_tc_program_within_the_bar_at_the_default_limit(emu, tmp_path, net, last
     is the harder case: scaled to the same max |feature|, its features are larger on average than a 128 x 128 map's.)
     The colour head's Tanh keeps its shipped limit of 8, which reaches 1.2e-4 here (DESIGN.md §F1, range guard)."""
     chans = spec.G_CHANNELS if net == "G" else spec.C_CHANNELS
-    limit = _default_limit(emu["heads"], chans[-1], last_op)
+    limit = _default_limit(emu["fp32"], chans[-1], last_op)
     Ws, bs = spec.make_weights(chans, 1000 + seed)
     feat = spec.make_feat(chans[0] - 1, 32, 32, 2000 + seed)
     feat = feat * (0.99 * limit / feat.abs().max().item())
     pts = spec.make_points(512, 3000 + seed)
     cal = spec.scene_calib(20, -60 + 17 * seed)
-    fin, fout = str(tmp_path / "tc.bin"), str(tmp_path / "tc.f32")
-    write_input(fin, feat, pts, cal, "orthogonal", chans[-1], last_op, Ws, bs)
-    r = subprocess.run([emu["tc"], fin, fout, "0", "2"], capture_output=True, text=True, timeout=3600)
-    assert r.returncode == 0, r.stderr[-2000:]
-    got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(chans[-1], 512)
+    inp = dict(feat=feat, rows=pts, calib=cal, proj="orthogonal", res=chans[-1], last_op=last_op, Ws=Ws, bs=bs)
+    got, _ = run(emu["tc"], tmp_path, "query", inp=inp, shape=(chans[-1], 512), options=dict(sms=2))
     err = (got - spec.query_ref(feat, pts, cal, Ws, bs, last_op)).abs().max().item()
     assert err <= 1e-4, (limit, err)

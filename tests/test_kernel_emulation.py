@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 from oracle import spec
-from emu_harness import build, needs_gxx, write_input
+from emu_harness import build, needs_gxx, run
 
 pytestmark = needs_gxx
 # one OS thread per CUDA thread is slow: the heaviest cases only run with MONOPORT_B200_EMU_FULL=1 (they pass; the default
@@ -202,21 +202,19 @@ def test_surface_kernels_match_reference_golden(emu_surface, tmp_path, golden_di
 #      the functional model of the wgmma / mbarrier / bulk-copy layer (tests/emu/tc_ptx_emu.h), with asynchronous operations
 #      deferred adversarially, against the goldens of the UNMODIFIED reference ---------------------------------------------
 @pytest.fixture(scope="module")
-def emu_query_tc(tmp_path_factory):
-    return build(tmp_path_factory, "emu_query_tc")
+def emu_tc(tmp_path_factory):
+    return build(tmp_path_factory, "emu_tc")
+
+
+def _case_input(case, n):
+    return dict(feat=case["feat"], rows=case["points"][:, :, :n], calib=case["calib"], proj=case["proj"],
+                res=case["expected"].shape[0], last_op=case["last_op"], Ws=case["Ws"], bs=case["bs"])
 
 
 def _run_query_tc(exe, tmp_path, case, n, program, sms, extra_env=None):
-    import torch
-    res = case["expected"].shape[0]
-    fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    write_input(fin, case["feat"], case["points"][:, :, :n], case["calib"], case["proj"], res, case["last_op"], case["Ws"],
-                case["bs"])
-    env = dict(os.environ)
-    env.update(extra_env or {})
-    r = subprocess.run([exe, fin, fout, str(program), str(sms)], capture_output=True, text=True, timeout=900, env=env)
-    assert r.returncode == 0, r.stderr[-2000:]
-    return torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(res, n)
+    """program 0 / 3: the tensor-core program; 103: with the peer stores of the fused slab exchange"""
+    return run(exe, tmp_path, "query", inp=_case_input(case, n), shape=(case["expected"].shape[0], n),
+               options=dict(sms=sms, peers=program >= 100), env=extra_env)[0]
 
 
 @pytest.mark.parametrize("name,n,program,sms", [
@@ -227,10 +225,10 @@ def _run_query_tc(exe, tmp_path, case, n, program, sms, extra_env=None):
     ("g_persp", 100, 3, 1),         # perspective projection
     ("g_nocalib", 150, 3, 3),       # calibs=None
 ])
-def test_tcgen05_kernels_match_reference_golden(emu_query_tc, tmp_path, name, n, program, sms):
+def test_tcgen05_kernels_match_reference_golden(emu_tc, tmp_path, name, n, program, sms):
     from helpers import load_query_case
     case = load_query_case(name)
-    got = _run_query_tc(emu_query_tc, tmp_path, case, n, program, sms)
+    got = _run_query_tc(emu_tc, tmp_path, case, n, program, sms)
     err = (got - case["expected"][:, :n]).abs().max().item()
     assert err <= 1e-4, err          # the GPU parity bar for the tensor-core programs (measured on the model: ~2e-5)
 
@@ -242,72 +240,63 @@ def test_tcgen05_kernels_match_reference_golden(emu_query_tc, tmp_path, name, n,
     ("c_rot33", 200, 0, 1),         # colour head: two-stage ring, (hi, lo) pass of layer 3
 ])
 @pytest.mark.parametrize("order", ["random:1", "random:2", "random:3"])
-def test_tcgen05_handoffs_survive_other_completion_orders(emu_query_tc, tmp_path, name, n, program, sms, order):
+def test_tcgen05_handoffs_survive_other_completion_orders(emu_tc, tmp_path, name, n, program, sms, order):
     """The model completes queued bulk copies in issue order by default.  The hand-off protocol (weight ring, operand
     buffers, wgmma groups) must not depend on that: random completion orders of the copies give the same bits, for both
     heads and for one or several CTAs."""
     import torch
     from helpers import load_query_case
     case = load_query_case(name)
-    want = _run_query_tc(emu_query_tc, tmp_path, case, n, program, sms)
-    got = _run_query_tc(emu_query_tc, tmp_path, case, n, program, sms, dict(EMU_TC_ORDER=order))
+    want = _run_query_tc(emu_tc, tmp_path, case, n, program, sms)
+    got = _run_query_tc(emu_tc, tmp_path, case, n, program, sms, dict(EMU_TC_ORDER=order))
     assert torch.equal(got, want)
     assert (got - case["expected"][:, :n]).abs().max().item() <= 1e-4
 
 
 @pytest.mark.parametrize("order", ["copies", "random:3"])
-def test_tcgen05_colour_head_matches_reference_golden(emu_query_tc, tmp_path, order):
+def test_tcgen05_colour_head_matches_reference_golden(emu_tc, tmp_path, order):
     """PIFuNetCMLP (513 -> 3, Tanh, 512-channel map): the 512-channel skip operand, the (hi, lo) pass of layer 3, eight-K-block
     G0 GEMM, three fp32 last-layer outputs; one emulated SM walks all four tiles (default completion order of the bulk
     copies and a random one)."""
     from helpers import load_query_case
     case = load_query_case("c_rot33")
     n = 200
-    got = _run_query_tc(emu_query_tc, tmp_path, case, n, 0, 1, {"EMU_TC_ORDER": order})
+    got = _run_query_tc(emu_tc, tmp_path, case, n, 0, 1, {"EMU_TC_ORDER": order})
     err = (got - case["expected"][:, :n]).abs().max().item()
     assert err <= 1e-4, err
     zero = case["expected"][:, :n] == 0
     assert (got[zero] == 0).all(), "out-of-image points must be exactly 0"
 
 
-def _write_tc_input(path, case, n):
+def _tc_input(case, n):
     """n points at the origin (the grid and node-list sources make their own)"""
-    write_input(path, case["feat"], np.zeros((3, n)), case["calib"], "orthogonal", 1, case["last_op"], case["Ws"], case["bs"])
+    return dict(feat=case["feat"], rows=np.zeros((3, n)), calib=case["calib"], proj="orthogonal", res=1,
+                last_op=case["last_op"], Ws=case["Ws"], bs=case["bs"])
 
 
 @pytest.mark.parametrize("program", [3, 103])
-def test_tcgen05_kernels_grid_source(emu_query_tc, tmp_path, program):
+def test_tcgen05_kernels_grid_source(emu_tc, tmp_path, program):
     """mp_query_grid's point source: node centres of a z slab generated in-kernel (103: also stored into the peer volumes
     at the slab's offset, the fused slab exchange)."""
-    import torch
     from helpers import load_query_case
     case = load_query_case("g_smallmap")
-    fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    _write_tc_input(fin, case, 4)
     R, z0, nz = 13, 3, 5
-    r = subprocess.run([emu_query_tc, fin, fout, str(program), "2", "grid", str(R), str(z0), str(nz)], capture_output=True,
-                       text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-2000:]
-    got = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
+    got, _ = run(emu_tc, tmp_path, "grid", R, z0, nz, inp=_tc_input(case, 4), shape=(nz * R * R,),
+                 options=dict(sms=2, peers=program >= 100))
     pts = spec.level_points(spec._grid_coords(R, 1), R, (-1, -1, -1), (1, 1, 1))[z0 * R * R:(z0 + nz) * R * R].t().contiguous()
     want = spec.query_ref(case["feat"], pts, case["calib"], case["Ws"], case["bs"], spec.LAST_SIGMOID)[0]
     assert got.numel() == nz * R * R and (got - want).abs().max().item() <= 1e-4
 
 
 @pytest.mark.parametrize("program", [3])
-def test_tcgen05_kernels_node_list_source(emu_query_tc, tmp_path, program):
+def test_tcgen05_kernels_node_list_source(emu_tc, tmp_path, program):
     """The octree engine's fused path: an index list with a device-side count below the list capacity, values scattered
     into the level volume; nodes that are not on the list stay untouched."""
     import torch
     from helpers import load_query_case
     case = load_query_case("g_smallmap")
-    fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    _write_tc_input(fin, case, 4)
     R, res = 33, 9
-    r = subprocess.run([emu_query_tc, fin, fout, str(program), "3", "nodes", str(R), str(res)], capture_output=True, text=True,
-                       timeout=900)
-    assert r.returncode == 0, r.stderr[-2000:]
-    got = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
+    got, _ = run(emu_tc, tmp_path, "nodes", R, res, inp=_tc_input(case, 4), shape=(res ** 3,), options=dict(sms=3))
     idx = torch.arange(0, res ** 3, 3)
     cc = torch.stack([idx % res, (idx // res) % res, idx // (res * res)], 1) * ((R - 1) // (res - 1))
     pts = spec.level_points(cc, R, (-1, -1, -1), (1, 1, 1)).t().contiguous()
@@ -318,26 +307,19 @@ def test_tcgen05_kernels_node_list_source(emu_query_tc, tmp_path, program):
 
 
 @pytest.mark.parametrize("kind,world", [("nodes", 2), ("nodes", 3), ("grid", 2)])
-def test_tcgen05_list_sharding_is_bit_identical(emu_query_tc, tmp_path, kind, world):
+def test_tcgen05_list_sharding_is_bit_identical(emu_tc, tmp_path, kind, world):
     """Multi-GPU list sharding of a query (octree levels, balanced dense ranges): `world` launches, launch r evaluating the
     r-th 128-aligned window of the point list -- also through the peer stores -- reproduce the unsharded launch bit for
     bit (243 nodes over 2 / 3 windows incl. an empty one; 5*13*13 grid nodes over 2)."""
     from helpers import load_query_case
     case = load_query_case("g_smallmap")
-    fin = str(tmp_path / "in.bin")
-    _write_tc_input(fin, case, 4)
-    args = ["nodes", "33", "9"] if kind == "nodes" else ["grid", "13", "3", "5"]
-    outs = []
-    for w in (1, world):
-        fout = str(tmp_path / ("w%d.f32" % w))
-        r = subprocess.run([emu_query_tc, fin, fout, "103", "2"] + args, capture_output=True, text=True, timeout=900,
-                           env=dict(os.environ, EMU_SHARD_WORLD=str(w)))
-        assert r.returncode == 0, r.stderr[-2000:]
-        outs.append(np.fromfile(fout, dtype=np.float32))
+    args, size = ((33, 9), 9 ** 3) if kind == "nodes" else ((13, 3, 5), 5 * 13 * 13)
+    outs = [run(emu_tc, tmp_path, kind, *args, inp=_tc_input(case, 4), shape=(size,), options=dict(sms=2, peers=True, shard=w),
+                tag="w%d" % w)[0].numpy() for w in (1, world)]
     assert outs[0].size > 0 and np.array_equal(outs[0], outs[1])
 
 
-def test_tcgen05_colour_head_fused_surface_rendering(emu_query_tc, tmp_path):
+def test_tcgen05_colour_head_fused_surface_rendering(emu_tc, tmp_path):
     """mp_colorize_surface: visible-surface vertices (X, Y, R - Z) -> world (mat_color) -> netC -> pred*0.5+0.5 -> canvas, one
     launch, against the restatement of RTL/main.py:212-249 driven by the oracle's query (32 x 32 colour map)."""
     import torch
@@ -349,11 +331,9 @@ def test_tcgen05_colour_head_fused_surface_rendering(emu_query_tc, tmp_path):
     cols = torch.randperm(R * R, generator=g)[:n]                     # at most one vertex per (x, y) column
     X, Y = cols // R, cols % R
     Z = torch.rand(n, generator=g) * (R - 1)
-    fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    write_input(fin, feat, torch.stack([X.float(), Y.float(), Z]), cal, "orthogonal", 3, spec.LAST_TANH, Ws, bs)
-    r = subprocess.run([emu_query_tc, fin, fout, "0", "2", "surface", str(R)], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-2000:]
-    got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(R, R, 3)
+    inp = dict(feat=feat, rows=torch.stack([X.float(), Y.float(), Z]), calib=cal, proj="orthogonal", res=3,
+               last_op=spec.LAST_TANH, Ws=Ws, bs=bs)
+    got, _ = run(emu_tc, tmp_path, "surface", R, inp=inp, shape=(R, R, 3), options=dict(sms=2, eager=True))
 
     def query_c(points, calib):
         return spec.query_ref(feat, points, calib, Ws, bs, spec.LAST_TANH)
@@ -367,22 +347,17 @@ def test_tcgen05_colour_head_fused_surface_rendering(emu_query_tc, tmp_path):
 
 # ---- the exact CUDA-core kernel (query_fp32.cu): default path of the colour head, fallback for every other head shape ----
 @pytest.fixture(scope="module")
-def emu_query_fp32(tmp_path_factory):
-    return build(tmp_path_factory, "emu_query_fp32")
+def emu_fp32(tmp_path_factory):
+    return build(tmp_path_factory, "emu_fp32")
 
 
 @pytest.mark.parametrize("name,n", [("c_rot33", 200), ("c_identity", 100), ("g_persp", 150), ("g_nocalib", 77), ("g_identity", 130)])
-def test_fp32_kernel_matches_reference_golden(emu_query_fp32, tmp_path, name, n):
+def test_fp32_kernel_matches_reference_golden(emu_fp32, tmp_path, name, n):
     import torch
     from helpers import load_query_case
     case = load_query_case(name)
     res = case["expected"].shape[0]
-    fin, fout = str(tmp_path / "in.bin"), str(tmp_path / "out.f32")
-    write_input(fin, case["feat"], case["points"][:, :, :n], case["calib"], case["proj"], res, case["last_op"], case["Ws"],
-                case["bs"])
-    r = subprocess.run([emu_query_fp32, fin, fout], capture_output=True, text=True, timeout=900)
-    assert r.returncode == 0, r.stderr[-2000:]
-    got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(res, n)
+    got, _ = run(emu_fp32, tmp_path, "query", inp=_case_input(case, n), shape=(res, n))
     want = case["expected"][:, :n]
     assert (got - want).abs().max().item() <= 2e-5          # the GPU bar of the fp32 mode
     assert torch.equal(got[want == 0], want[want == 0]), "out-of-image points must be exactly 0"

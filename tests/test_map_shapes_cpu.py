@@ -4,14 +4,13 @@ or that sit at or above the tensor-core program's 65536 texels.  The restatement
 them, and the query kernels -- compiled unmodified on the CPU model of tests/emu -- against the reference and the restatement:
 the tensor-core program with its per-texel products, the exact fp32 kernel, the point gradient and the colour surface render."""
 import os
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 from oracle import spec
-from emu_harness import build, write_input
+from emu_harness import build, run
 from grad_cases import query_grad_ref, within_bar
 from shape_cases import (TC_TEXEL_LIMIT, load_shape_batch_case, load_shape_case, load_shape_grad_case, shape_batch_cases,
                          shape_cases, shape_grad_cases, within_fp32_bar)
@@ -88,23 +87,20 @@ def test_restatement_per_image_matches_batched_shape_golden(name):
 # ---- the kernels on the CPU model --------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return {k: build(tmp_path_factory, "emu_query_" + k) for k in ("tc", "fp32", "grad")}
+    return {k: build(tmp_path_factory, "emu_" + k) for k in ("tc", "fp32")}
 
 
-def _run(exe, tmp_path, c, n, args, batched=False, env=None, tag="x"):
-    """-> [B,Res,n] (batched) or [Res,n] from emu_query_tc / emu_query_fp32"""
+def _input(c, n, batched=False, res=None, rows=None):
+    return dict(feat=c["feat"], rows=c["points"][:, :, :n] if rows is None else rows, calib=c["calib"], proj=c["proj"],
+                res=c["chans"][-1] if res is None else res, last_op=c["last_op"], Ws=c["Ws"], bs=c["bs"], batched=batched)
+
+
+def _run(exe, tmp_path, c, n, batch=None, tag="x", **options):
+    """-> [B,Res,n] (a batched launch of B images) or [Res,n] of the query of emu_tc / emu_fp32"""
     res = c["chans"][-1]
-    fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    write_input(fin, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], res, c["last_op"], c["Ws"], c["bs"], batched)
-    r = subprocess.run([exe, fin, fout] + [str(a) for a in args], capture_output=True, text=True, timeout=3600,
-                       env=dict(os.environ, **(env or {})))
-    assert r.returncode == 0 and "DEADLOCK" not in r.stderr, r.stderr[-2000:]
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
-    return out.reshape(c["feat"].shape[0], res, n) if batched else out.reshape(res, n)
-
-
-def _program(c):
-    return 0 if c["net"] == "C" else 3
+    shape = (batch, res, n) if batch else (res, n)
+    return run(exe, tmp_path, "query", inp=_input(c, n, batch is not None), shape=shape, options=dict(batch=batch, **options),
+               tag=tag)[0]
 
 
 # 136 points: the 8 border points, the 64-point corner cluster and 64 uniform ones -- three tiles of 64, the last one ragged
@@ -118,7 +114,7 @@ TC_CASES = [
 @pytest.mark.parametrize("name,n,sms", TC_CASES)
 def test_tc_program_matches_reference_shape_golden(emu, tmp_path, name, n, sms):
     c = load_shape_case(name)
-    got = _run(emu["tc"], tmp_path, c, n, [_program(c), sms])
+    got = _run(emu["tc"], tmp_path, c, n, sms=sms)
     want = c["expected"][:, :n]
     assert (got - want).abs().max().item() <= 1e-4
     assert torch.equal(got[want == 0], want[want == 0]), "out-of-image points must be exactly 0"
@@ -131,14 +127,14 @@ def test_tc_batch_on_non_square_maps(emu, tmp_path, name):
     for bit."""
     c = load_shape_batch_case(name)
     n = 100
-    got = _run(emu["tc"], tmp_path, c, n, [3, 2, "batch", c["B"]], batched=True)
+    got = _run(emu["tc"], tmp_path, c, n, batch=c["B"], sms=2)
     want = c["expected"][:, :, :n]
     assert (got - want).abs().max().item() <= 1e-4
     assert torch.equal(got[want == 0], want[want == 0])
     for b in range(c["B"]):
         one = dict(c, feat=c["feat"][b:b + 1], points=c["points"][b:b + 1],
                    calib=c["calib"][b:b + 1] if c["calib"] is not None else None)
-        assert torch.equal(got[b], _run(emu["tc"], tmp_path, one, n, [3, 2], tag="one%d" % b)), b
+        assert torch.equal(got[b], _run(emu["tc"], tmp_path, one, n, sms=2, tag="one%d" % b)), b
 
 
 @pytest.mark.parametrize("name", ["g_wide", "g_tiny"])
@@ -150,7 +146,7 @@ def test_g0_products_cover_every_texel(emu, tmp_path, name):
     C, H, W = c["feat"].shape[1:]
     M = H * W
     dump = str(tmp_path / "g0.bin")
-    _run(emu["tc"], tmp_path, c, 16, [3, 2], env={"EMU_TC_DUMP": dump})
+    _run(emu["tc"], tmp_path, c, 16, sms=2, dump=dump)
     raw = open(dump, "rb").read()
     assert len(raw) == M * 1024 * 2 + M * C * 2 + M * 4
     g0 = np.frombuffer(raw, np.float16, M * 1024).reshape(M, 1024).astype(np.float64)
@@ -178,7 +174,7 @@ FP32_CASES = [("g_wide", 136), ("g_tall", 136), ("g_tiny", 136), ("g_row", 136),
 @pytest.mark.parametrize("name,n", FP32_CASES)
 def test_fp32_kernel_matches_reference_shape_golden(emu, tmp_path, name, n):
     c = load_shape_case(name)
-    got = _run(emu["fp32"], tmp_path, c, n, [])
+    got = _run(emu["fp32"], tmp_path, c, n)
     want = c["expected"][:, :n]
     ok, msg = within_fp32_bar(got, dict(c, expected=want, expected64=c["expected64"][:, :n]))
     assert ok, msg
@@ -190,29 +186,20 @@ def test_grad_kernel_matches_reference_shape_golden(emu, tmp_path, name):
     """the point gradient within its bar of the reference's fp32 autograd, and its value the fp32 query's bit for bit"""
     c = load_shape_grad_case(name)
     n = 136
-    fin, fout = str(tmp_path / "in_g.bin"), str(tmp_path / "out_g.f32")
-    write_input(fin, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], 1, c["last_op"], c["Ws"], c["bs"])
-    r = subprocess.run([emu["grad"], fin, fout, "3"], capture_output=True, text=True, timeout=3600)
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
+    out, _ = run(emu["fp32"], tmp_path, "grad", inp=_input(c, n, res=1), shape=(4 * n,), options=dict(sms=3), tag="g")
     val, dp = out[:n].reshape(1, n), out[n:].reshape(3, n)
     assert (val - c["value"][:, :n]).abs().max().item() <= 2e-5
     ok, msg = within_bar(dp, c["grad32"][:, :n])
     assert ok, msg
-    assert torch.equal(val, _run(emu["fp32"], tmp_path, c, n, [], tag="q"))
+    assert torch.equal(val, _run(emu["fp32"], tmp_path, c, n, tag="q"))
 
 
 # ---- the colour surface render on a non-square map ------------------------------------------------------------------------
 R_CANVAS = 65
 
 
-@pytest.fixture(scope="module")
-def emu_surface(tmp_path_factory):
-    return {k: build(tmp_path_factory, "emu_colour_surface_" + k) for k in ("tc", "fp32")}
-
-
 @pytest.mark.parametrize("program", ["tc", "fp32"])
-def test_colour_surface_render_on_a_non_square_map(emu_surface, tmp_path, program):
+def test_colour_surface_render_on_a_non_square_map(emu, tmp_path, program):
     """colorization() of 120 visible vertices through the colour head on the 88 x 120 map, by the tensor-core render and by
     its exact fp32 twin, against the restatement driven by the oracle's query."""
     c = load_shape_case("c_wide")
@@ -222,13 +209,8 @@ def test_colour_surface_render_on_a_non_square_map(emu_surface, tmp_path, progra
     X, Y = cols // R_CANVAS, cols % R_CANVAS
     Z = torch.rand(n, generator=g) * (R_CANVAS - 1)
     rows = torch.stack([X.float(), Y.float(), Z])[None]
-    fin, fout = str(tmp_path / "s.bin"), str(tmp_path / "s.f32")
-    write_input(fin, c["feat"], rows, c["calib"], c["proj"], 3, c["last_op"], c["Ws"], c["bs"])
-    args = [fin, fout, "2", str(R_CANVAS), str(n)] if program == "tc" else [fin, fout, "2", "surface", str(R_CANVAS), str(n)]
-    args += ["-1", "-1", "-1", "1", "1", "1"]                 # the render box [b_min, b_max]
-    r = subprocess.run([emu_surface[program]] + args, capture_output=True, text=True, timeout=3600)
-    assert r.returncode == 0, r.stderr[-2000:]
-    got = torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(R_CANVAS, R_CANVAS, 3)
+    got, _ = run(emu[program], tmp_path, "surface", R_CANVAS, n, -1, -1, -1, 1, 1, 1,        # the render box [b_min, b_max]
+                 inp=_input(c, n, res=3, rows=rows), shape=(R_CANVAS, R_CANVAS, 3), options=dict(sms=2))
 
     def query_c(points, calib):
         return spec.query_ref(c["feat"], points, calib, c["Ws"], c["bs"], spec.LAST_TANH)

@@ -1,16 +1,12 @@
 """CPU checks of the batched query (mp_query_points_batch: B images in one launch): the oracle against the batched goldens of
 the reference, and both query kernels -- compiled unmodified on the CPU model of tests/emu -- against those goldens and
 against B = 1 runs of each image, bit for bit, including the per-image range guard of the tensor-core program."""
-import os
-import subprocess
-
-import numpy as np
 import pytest
 import torch
 
 from oracle import spec
 from batch_cases import batch_cases, load_batch_case
-from emu_harness import build, write_input
+from emu_harness import build, run
 
 
 @pytest.mark.parametrize("name", batch_cases())
@@ -33,27 +29,23 @@ def test_batched_goldens_cover_the_issue_cases():
 # ---- the kernels on the CPU model ------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu_tc(tmp_path_factory):
-    return build(tmp_path_factory, "emu_query_tc")
+    return build(tmp_path_factory, "emu_tc")
 
 
 @pytest.fixture(scope="module")
 def emu_fp32(tmp_path_factory):
-    return build(tmp_path_factory, "emu_query_fp32")
+    return build(tmp_path_factory, "emu_fp32")
 
 
-def _run(exe, tmp_path, case, n, args, batched, env=None, feat=None, tag="x"):
-    """-> [B,Res,n] (a batched launch: args end with "batch B") or [Res,n] (a single-image launch)"""
+def _run(exe, tmp_path, case, n, batched, env=None, feat=None, tag="x", **options):
+    """-> [B,Res,n] (a batched launch of every image of the case) or [Res,n] (a single-image launch)"""
     feat = case["feat"] if feat is None else feat
     res = case["expected"].shape[1]
-    fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    write_input(fin, feat, case["points"][:, :, :n], case["calib"], case["proj"], res, case["last_op"], case["Ws"], case["bs"],
-                batched)
-    e = dict(os.environ)
-    e.update(env or {})
-    r = subprocess.run([exe, fin, fout] + [str(a) for a in args], capture_output=True, text=True, timeout=1800, env=e)
-    assert r.returncode == 0 and "DEADLOCK" not in r.stderr, r.stderr[-2000:]
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
-    return out.reshape(feat.shape[0], res, n) if batched else out.reshape(res, n)
+    inp = dict(feat=feat, rows=case["points"][:, :, :n], calib=case["calib"], proj=case["proj"], res=res,
+               last_op=case["last_op"], Ws=case["Ws"], bs=case["bs"], batched=batched)
+    B = feat.shape[0]
+    return run(exe, tmp_path, "query", inp=inp, shape=(B, res, n) if batched else (res, n),
+               options=dict(batch=B if batched else None, **options), env=env, tag=tag)[0]
 
 
 def _single(case, b):
@@ -72,7 +64,7 @@ def _single(case, b):
 ])
 def test_tc_batch_matches_batched_reference_golden(emu_tc, tmp_path, name, n, sms):
     c = load_batch_case(name)
-    got = _run(emu_tc, tmp_path, c, n, [0 if c["net"] == "C" else 3, sms, "batch", c["B"]], True)
+    got = _run(emu_tc, tmp_path, c, n, True, sms=sms)
     want = c["expected"][:, :, :n]
     assert (got - want).abs().max().item() <= 1e-4
     assert torch.equal(got[want == 0], want[want == 0]), "out-of-image points must be exactly 0"
@@ -81,7 +73,7 @@ def test_tc_batch_matches_batched_reference_golden(emu_tc, tmp_path, name, n, sm
 @pytest.mark.parametrize("name,n", [("g_nocalib", 150), ("g_persp", 70), ("c_rot", 40), ("g_rot", 33)])
 def test_fp32_batch_matches_batched_reference_golden(emu_fp32, tmp_path, name, n):
     c = load_batch_case(name)
-    got = _run(emu_fp32, tmp_path, c, n, ["batch", c["B"]], True)
+    got = _run(emu_fp32, tmp_path, c, n, True)
     want = c["expected"][:, :, :n]
     assert (got - want).abs().max().item() <= 2e-5
     assert torch.equal(got[want == 0], want[want == 0])
@@ -90,9 +82,9 @@ def test_fp32_batch_matches_batched_reference_golden(emu_fp32, tmp_path, name, n
 def test_fp32_batch_image_equals_single_run(emu_fp32, tmp_path):
     c = load_batch_case("g_nocalib")
     n = 77
-    got = _run(emu_fp32, tmp_path, c, n, ["batch", c["B"]], True)
+    got = _run(emu_fp32, tmp_path, c, n, True)
     for b in range(c["B"]):
-        one = _run(emu_fp32, tmp_path, _single(c, b), n, [], False, tag="one%d" % b)
+        one = _run(emu_fp32, tmp_path, _single(c, b), n, False, tag="one%d" % b)
         assert torch.equal(got[b], one), b
 
 
@@ -102,9 +94,9 @@ def test_tc_batch_image_equals_single_run_bit_for_bit(emu_tc, tmp_path, sms):
     on one CTA, the weight ring running across images)."""
     c = load_batch_case("g_nocalib")
     n = 130
-    got = _run(emu_tc, tmp_path, c, n, [3, sms, "batch", c["B"]], True)
+    got = _run(emu_tc, tmp_path, c, n, True, sms=sms)
     for b in range(c["B"]):
-        one = _run(emu_tc, tmp_path, _single(c, b), n, [3, sms], False, tag="one%d" % b)
+        one = _run(emu_tc, tmp_path, _single(c, b), n, False, tag="one%d" % b, sms=sms)
         assert torch.equal(got[b], one), (sms, b)
 
 
@@ -112,11 +104,11 @@ def test_tc_batch_image_equals_single_run_bit_for_bit(emu_tc, tmp_path, sms):
 def test_tc_batch_bit_identity_under_other_completion_orders(emu_tc, tmp_path, order):
     c = load_batch_case("g_nocalib")
     n = 100
-    want = _run(emu_tc, tmp_path, c, n, [3, 2, "batch", c["B"]], True)
-    got = _run(emu_tc, tmp_path, c, n, [3, 2, "batch", c["B"]], True, env={"EMU_TC_ORDER": order}, tag="ord")
+    want = _run(emu_tc, tmp_path, c, n, True, sms=2)
+    got = _run(emu_tc, tmp_path, c, n, True, env={"EMU_TC_ORDER": order}, tag="ord", sms=2)
     assert torch.equal(got, want)
     for b in range(c["B"]):
-        one = _run(emu_tc, tmp_path, _single(c, b), n, [3, 2], False, env={"EMU_TC_ORDER": order}, tag="one%d" % b)
+        one = _run(emu_tc, tmp_path, _single(c, b), n, False, env={"EMU_TC_ORDER": order}, tag="one%d" % b, sms=2)
         assert torch.equal(got[b], one), b
 
 
@@ -133,11 +125,10 @@ def test_tc_batch_range_guard_skips_exactly_the_out_of_range_image(emu_tc, tmp_p
     limit = 12.0
     assert amax[1] > limit and amax[0] < limit and amax[2] < limit, amax
     n = 140
-    env = {"EMU_TC_LIMIT": str(limit), "EMU_TC_GUARD": "1"}
-    got = _run(emu_tc, tmp_path, case, n, [3, sms, "batch", 3], True, env=env)
+    got = _run(emu_tc, tmp_path, case, n, True, sms=sms, limit=limit, guard="in")
     assert bool((got[1] == -4242.0).all()), "the out-of-range image's outputs must stay untouched"
-    free = _run(emu_tc, tmp_path, case, n, [3, sms, "batch", 3], True, tag="free")      # no guard
+    free = _run(emu_tc, tmp_path, case, n, True, tag="free", sms=sms)      # no guard
     assert torch.equal(got[0], free[0]) and torch.equal(got[2], free[2])
     for b in (0, 2):
-        one = _run(emu_tc, tmp_path, _single(case, b), n, [3, sms], False, tag="one%d" % b)
+        one = _run(emu_tc, tmp_path, _single(case, b), n, False, tag="one%d" % b, sms=sms)
         assert torch.equal(got[b], one), b

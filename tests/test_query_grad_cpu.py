@@ -2,15 +2,11 @@
 autograd goldens, and the gradient kernel -- compiled unmodified on the CPU model of tests/emu -- against those goldens, against
 the fp32 query kernel's values bit for bit, across simulated SM counts, outside the image, and under the range guard and a
 device-side point count."""
-import os
-import subprocess
-
-import numpy as np
 import pytest
 import torch
 
 from oracle import spec
-from emu_harness import build, write_input
+from emu_harness import build, run
 from grad_cases import grad_cases, load_grad_case, query_grad_ref, within_bar
 
 
@@ -35,37 +31,25 @@ def test_restatement_matches_reference_grad_golden(name):
 # ---- the kernel on the CPU model -------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    """(gradient harness, fp32 query harness)"""
-    return build(tmp_path_factory, "emu_query_grad"), build(tmp_path_factory, "emu_query_fp32")
+    return build(tmp_path_factory, "emu_fp32")
 
 
-def _write_input(path, c, n):
-    write_input(path, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], c["chans"][-1], c["last_op"], c["Ws"], c["bs"])
+def _input(c, n):
+    return dict(feat=c["feat"], rows=c["points"][:, :, :n], calib=c["calib"], proj=c["proj"], res=c["chans"][-1],
+                last_op=c["last_op"], Ws=c["Ws"], bs=c["bs"])
 
 
-def _run_grad(emu, tmp_path, c, n, sms=3, tag="g", env=None):
+def _run_grad(emu, tmp_path, c, n, sms=3, tag="g", **options):
     """-> (value [Res,n], dpoints [3,n]) of the gradient kernel"""
     res = c["chans"][-1]
-    fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    _write_input(fin, c, n)
-    args = [emu[0], fin, fout, str(sms)]
-    if c["grad_output"] is not None:
-        fg = str(tmp_path / ("gout_%s.f32" % tag))
-        c["grad_output"][:, :n].contiguous().numpy().astype(np.float32).tofile(fg)
-        args.append(fg)
-    r = subprocess.run(args, capture_output=True, text=True, timeout=1800, env=dict(os.environ, **(env or {})))
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
-    assert out.numel() == (res + 3) * n
+    gout = [] if c["grad_output"] is None else [c["grad_output"][:, :n].contiguous()]
+    out, _ = run(emu, tmp_path, "grad", *gout, inp=_input(c, n), shape=((res + 3) * n,), options=dict(sms=sms, **options),
+                 tag=tag)
     return out[:res * n].reshape(res, n), out[res * n:].reshape(3, n)
 
 
 def _run_fp32(emu, tmp_path, c, n):
-    fin, fout = str(tmp_path / "in_q.bin"), str(tmp_path / "out_q.f32")
-    _write_input(fin, c, n)
-    r = subprocess.run([emu[1], fin, fout], capture_output=True, text=True, timeout=1800)
-    assert r.returncode == 0, r.stderr[-2000:]
-    return torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(c["chans"][-1], n)
+    return run(emu, tmp_path, "query", inp=_input(c, n), shape=(c["chans"][-1], n), tag="q")[0]
 
 
 # the first 8 points of every case are border_points(): on the image border / corners and far outside
@@ -113,15 +97,14 @@ def test_kernel_range_guard_and_device_count(emu, tmp_path):
     c = load_grad_case("g_rot")
     n = 40
     full = _run_grad(emu, tmp_path, c, n)
-    for guard, runs_above in (("2", True), ("1", False)):
+    for guard, runs_above in (("out", True), ("in", False)):
         for amax, above in (("2", True), ("0.5", False)):
-            got = _run_grad(emu, tmp_path, c, n, tag="g%s%s" % (guard, amax),
-                            env={"EMU_GUARD": guard, "EMU_TC_LIMIT": "1", "EMU_AMAX": amax})
+            got = _run_grad(emu, tmp_path, c, n, tag="g%s%s" % (guard, amax), guard=guard, limit=1, amax=amax)
             if above == runs_above:
                 assert torch.equal(got[0], full[0]) and torch.equal(got[1], full[1]), (guard, amax)
             else:
                 assert bool((got[0] == -4242).all()) and bool((got[1] == -4242).all()), (guard, amax)
     k = 21
-    cut = _run_grad(emu, tmp_path, c, n, tag="cnt", env={"EMU_COUNT": str(k)})
+    cut = _run_grad(emu, tmp_path, c, n, tag="cnt", count=k)
     assert torch.equal(cut[0][:, :k], full[0][:, :k]) and torch.equal(cut[1][:, :k], full[1][:, :k])
     assert bool((cut[0][:, k:] == -4242).all()) and bool((cut[1][:, k:] == -4242).all())

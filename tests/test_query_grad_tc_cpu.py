@@ -3,52 +3,37 @@ unmodified on the CPU model of tests/emu: against the reference's fp64 autograd 
 query program bit for bit, across simulated SM counts and bulk-copy completion orders, outside the image, under the range
 guard and with a device-side point count.  (Its ptxas report is checked with the rest of query_tc.cu in
 test_ptxas_report.py.)"""
-import os
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
 from oracle import spec
-from emu_harness import build, write_input
+from emu_harness import build, run
 from grad_cases import GOLDEN_CASES, load_golden, load_grad_case, tc_bar
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return dict(jvp=build(tmp_path_factory, "emu_query_jvp_tc"), tc=build(tmp_path_factory, "emu_query_tc"))
+    return build(tmp_path_factory, "emu_tc")
 
 
-def _write_input(path, c, n):
-    write_input(path, c["feat"], c["points"][:, :, :n], c["calib"], c["proj"], c["chans"][-1], c["last_op"], c["Ws"], c["bs"])
+def _input(c, n):
+    return dict(feat=c["feat"], rows=c["points"][:, :, :n], calib=c["calib"], proj=c["proj"], res=c["chans"][-1],
+                last_op=c["last_op"], Ws=c["Ws"], bs=c["bs"])
 
 
-def _run_jvp(emu, tmp_path, c, n, sms=3, env=None, tag="j"):
+def _run_jvp(emu, tmp_path, c, n, sms=3, env=None, tag="j", **options):
     """-> (value [Res,n], dpoints [3,n]) of the tensor-core gradient program"""
     res = c["chans"][-1]
-    fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    _write_input(fin, c, n)
-    args = [emu["jvp"], fin, fout, str(sms)]
-    if c["grad_output"] is not None:
-        fg = str(tmp_path / ("gout_%s.f32" % tag))
-        c["grad_output"][:, :n].contiguous().numpy().astype(np.float32).tofile(fg)
-        args.append(fg)
-    r = subprocess.run(args, capture_output=True, text=True, timeout=3600, env=dict(os.environ, **(env or {})))
-    assert r.returncode == 0 and "DEADLOCK" not in r.stderr, r.stderr[-2000:]
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
-    assert out.numel() == (res + 3) * n
+    gout = [] if c["grad_output"] is None else [c["grad_output"][:, :n].contiguous()]
+    out, _ = run(emu, tmp_path, "jvp", *gout, inp=_input(c, n), shape=((res + 3) * n,), options=dict(sms=sms, **options),
+                 env=env, tag=tag)
     return out[:res * n].reshape(res, n), out[res * n:].reshape(3, n)
 
 
-def _run_tc(emu, tmp_path, c, n, env=None):
+def _run_tc(emu, tmp_path, c, n, **options):
     """-> [Res,n] of the tensor-core query program"""
-    fin, fout = str(tmp_path / "in_q.bin"), str(tmp_path / "out_q.f32")
-    _write_input(fin, c, n)
-    r = subprocess.run([emu["tc"], fin, fout, "3" if c["net"] == "G" else "0", "2"], capture_output=True, text=True,
-                       timeout=3600, env=dict(os.environ, **(env or {})))
-    assert r.returncode == 0, r.stderr[-2000:]
-    return torch.from_numpy(np.fromfile(fout, dtype=np.float32)).reshape(c["chans"][-1], n)
+    return run(emu, tmp_path, "query", inp=_input(c, n), shape=(c["chans"][-1], n), options=dict(sms=2, **options), tag="q")[0]
 
 
 # ---- a torch restatement of the kernel's fp16 roundings ------------------------------------------------------------------
@@ -210,15 +195,14 @@ def test_jvp_range_guard_and_device_count(emu, tmp_path):
     amax = c["feat"].abs().max().item()
     below = float(np.nextafter(np.float32(amax), np.float32(0)))
     full = _run_jvp(emu, tmp_path, c, n)
-    at = _run_jvp(emu, tmp_path, c, n, env={"EMU_TC_LIMIT": repr(amax), "EMU_TC_GUARD": "1"}, tag="at")
+    at = _run_jvp(emu, tmp_path, c, n, limit=repr(amax), guard="in", tag="at")
     assert torch.equal(at[0], full[0]) and torch.equal(at[1], full[1])
-    for guard, limit in (("1", below), ("2", amax)):
-        env = {"EMU_TC_LIMIT": repr(limit), "EMU_TC_GUARD": guard}
-        skipped = _run_jvp(emu, tmp_path, c, n, env=env, tag="sk" + guard)
+    for guard, limit in (("in", below), ("out", amax)):
+        skipped = _run_jvp(emu, tmp_path, c, n, limit=repr(limit), guard=guard, tag="sk" + guard)
         assert bool((skipped[0] == -4242).all()) and bool((skipped[1] == -4242).all()), guard
-        assert bool((_run_tc(emu, tmp_path, c, n, env=env) == -4242).all()), guard
+        assert bool((_run_tc(emu, tmp_path, c, n, limit=repr(limit), guard=guard) == -4242).all()), guard
     k = 21
-    cut = _run_jvp(emu, tmp_path, c, n, env={"EMU_COUNT": str(k)}, tag="cnt")
+    cut = _run_jvp(emu, tmp_path, c, n, count=k, tag="cnt")
     assert torch.equal(cut[0][:, :k], full[0][:, :k]) and torch.equal(cut[1][:, :k], full[1][:, :k])
     assert bool((cut[0][:, k:] == -4242).all()) and bool((cut[1][:, k:] == -4242).all())
 

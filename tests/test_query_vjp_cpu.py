@@ -3,21 +3,15 @@ train-mode autograd goldens, and the VJP kernel with its weight-gradient contrac
 tests/emu -- against those goldens, its point gradient against the single-map gradient launch's bit for bit, its determinism
 across chunk sizes and SM counts.  Also the ptxas report: no spill and no stack frame for the new kernels, and the register
 counts of the query kernel."""
-import os
 import re
-import subprocess
 
-import numpy as np
 import pytest
 import torch
 
-import emu_harness
 from oracle import spec
-from emu_harness import build, ptxas_report, write_input
+from emu_harness import build, ptxas_report, run
 from head_cases import fp32_tile
-from vjp_cases import GRAD_NAMES, flat, golden_bar, load_vjp_case, query_vjp_ref, vjp_cases
-
-emu_harness.HARNESSES.setdefault("emu_query_vjp", ("-O3", True))
+from vjp_cases import GRAD_NAMES, flat, golden_bar, load_vjp_case, query_vjp_ref, run_vjp, vjp_cases
 
 
 def test_vjp_goldens_cover_the_cases():
@@ -62,38 +56,13 @@ def test_restatement_matches_reference_vjp_golden(name):
 # ---- the kernels on the CPU model ------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    """(VJP harness, point-gradient harness)"""
-    return build(tmp_path_factory, "emu_query_vjp"), build(tmp_path_factory, "emu_query_grad")
+    return build(tmp_path_factory, "emu_fp32")
 
 
 def _run_vjp(emu, tmp_path, c, stage=0, chunk=0, sms=3, want="fpw", tag="v"):
     """one stage of a golden on the CPU model -> (dfeat [B,C,H,W], dpoints [B,3,N], [dW_l], [db_l])"""
-    feat, pts, chans = c["feats"][stage], c["points"], c["chans"]
-    B, C, H, W = feat.shape
-    N = pts.shape[2]
-    fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    write_input(fin, feat, pts, c["calib"], c["proj"], chans[-1], c["last_op"], c["Ws"], c["bs"], batched=True)
-    fg = "-"
-    if c["grad_output"] is not None:
-        fg = str(tmp_path / ("gout_%s.f32" % tag))
-        c["grad_output"][stage].contiguous().numpy().astype(np.float32).tofile(fg)
-    r = subprocess.run([emu[0], fin, fout, str(B), ",".join(str(x) for x in chans[1:]), fg, str(chunk), str(sms), want],
-                       capture_output=True, text=True, timeout=3600)
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
-    o = 0
-
-    def take(shape):
-        nonlocal o
-        k = int(np.prod(shape))
-        t = out[o:o + k].reshape(shape)
-        o += k
-        return t
-    dfeat, dp = take((B, C, H, W)), take((B, 3, N))
-    dW = [take((chans[l + 1], c["Ws"][l].shape[1])) for l in range(len(c["Ws"]))]
-    db = [take((chans[l + 1],)) for l in range(len(c["Ws"]))]
-    assert o == out.numel()
-    return dfeat, dp, dW, db
+    gout = "-" if c["grad_output"] is None else c["grad_output"][stage].contiguous()
+    return run_vjp(emu, tmp_path, c, c["feats"][stage], gout, chunk, want, options=dict(sms=sms), tag=tag)[:4]
 
 
 # the single-stage goldens (a multi-stage golden's head gradient sums over its stages: the restatement covers those)
@@ -131,13 +100,12 @@ def test_kernel_point_gradient_is_the_gradient_kernels_bit_for_bit(emu, tmp_path
     the point count on the device"""
     c = load_vjp_case("g_b1_rot")
     _, dp, _, _ = _run_vjp(emu, tmp_path, c, want="p")
-    fin, fout = str(tmp_path / "in_g.bin"), str(tmp_path / "out_g.f32")
-    write_input(fin, c["feats"][0], c["points"][0], c["calib"], c["proj"], 1, c["last_op"], c["Ws"], c["bs"])
     N = c["points"].shape[2]
-    env = dict(os.environ, EMU_GUARD="2", EMU_TC_LIMIT="1", EMU_AMAX="2", EMU_COUNT=str(N))
-    r = subprocess.run([emu[1], fin, fout, "3"], capture_output=True, text=True, timeout=3600, env=env)
-    assert r.returncode == 0, r.stderr[-2000:]
-    want = torch.from_numpy(np.fromfile(fout, dtype=np.float32))[N:].reshape(3, N)
+    inp = dict(feat=c["feats"][0], rows=c["points"][0], calib=c["calib"], proj=c["proj"], res=1, last_op=c["last_op"],
+               Ws=c["Ws"], bs=c["bs"])
+    out, _ = run(emu, tmp_path, "grad", inp=inp, shape=(4 * N,), options=dict(sms=3, guard="out", limit=1, amax=2, count=N),
+                 tag="g")
+    want = out[N:].reshape(3, N)
     assert torch.equal(dp[0], want)
 
 

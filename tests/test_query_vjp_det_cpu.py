@@ -2,61 +2,29 @@
 kernel, the radix sort and the gather of query_vjp.cu compiled unmodified on the CPU model of tests/emu.  d features against
 the reference's goldens and the atomic path, the same bits at every SM count and for every request, the other gradients
 the flag-off bits, crowded cells and the map's edges, a restatement of the documented order from a dump of the scratch
-(tests/emu/emu_query_vjp_det.cpp), and the ptxas report of the new kernels."""
-import os
+(the --dump option of tests/emu/emu_fp32.cpp's vjp op), and the ptxas report of the new kernels."""
 import re
-import subprocess
 
-import numpy as np
 import pytest
 import torch
 
-import emu_harness
-from emu_harness import build, ptxas_report, write_input
+from emu_harness import build, ptxas_report
 from ordered_cases import one_cell_case, read_dump, restate_ordered_dfeat
-from vjp_cases import flat, golden_bar, load_vjp_case, query_vjp_ref, rel_dist, vjp_bar
-
-emu_harness.HARNESSES.setdefault("emu_query_vjp_det", ("-O3", True))
+from vjp_cases import flat, golden_bar, load_vjp_case, query_vjp_ref, rel_dist, run_vjp, vjp_bar
 
 DET = 1                                     # MP_VJP_DETERMINISTIC
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return build(tmp_path_factory, "emu_query_vjp_det")
+    return build(tmp_path_factory, "emu_fp32")
 
 
 def _run(emu, tmp_path, c, flags, chunk=0, sms=3, want="fpw", tag="v", dump=None):
     """stage 0 of a case on the CPU model -> (dfeat [B,C,H,W], dpoints [B,3,N], [dW_l], [db_l])"""
-    feat, pts, chans = c["feats"][0], c["points"], c["chans"]
-    B, C, H, W = feat.shape
-    N = pts.shape[2]
-    fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    write_input(fin, feat, pts, c["calib"], c["proj"], chans[-1], c["last_op"], c["Ws"], c["bs"], batched=True)
-    fg = "-"
-    if c["grad_output"] is not None:
-        fg = str(tmp_path / ("gout_%s.f32" % tag))
-        c["grad_output"][0].contiguous().numpy().astype(np.float32).tofile(fg)
-    env = dict(os.environ, EMU_VJP_FLAGS=str(flags))
-    if dump:
-        env["EMU_VJP_DUMP"] = dump
-    r = subprocess.run([emu, fin, fout, str(B), ",".join(str(x) for x in chans[1:]), fg, str(chunk), str(sms), want],
-                       capture_output=True, text=True, timeout=3600, env=env)
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
-    o = 0
-
-    def take(shape):
-        nonlocal o
-        k = int(np.prod(shape))
-        t = out[o:o + k].reshape(shape)
-        o += k
-        return t
-    dfeat, dp = take((B, C, H, W)), take((B, 3, N))
-    dW = [take((chans[l + 1], c["Ws"][l].shape[1])) for l in range(len(c["Ws"]))]
-    db = [take((chans[l + 1],)) for l in range(len(c["Ws"]))]
-    assert o == out.numel()
-    return dfeat, dp, dW, db
+    gout = "-" if c["grad_output"] is None else c["grad_output"][0].contiguous()
+    return run_vjp(emu, tmp_path, c, c["feats"][0], gout, chunk, want, options=dict(sms=sms, vjp_flags=flags, dump=dump),
+                   tag=tag)[:4]
 
 
 def _close_to_atomic(det, atomic):

@@ -1,57 +1,29 @@
 """CPU checks of the training query's backward (mp_launch_query_vjp) off the goldens' shapes, on the CPU model of tests/emu
-(tests/emu/emu_query_vjp_det.cpp: query_vjp_kernel, wgrad_kernel, the radix sort, the gather and the layout step compiled
+(the vjp op of tests/emu/emu_fp32.cpp: query_vjp_kernel, wgrad_kernel, the radix sort, the gather and the layout step compiled
 unmodified): the ordered feature gradient at one, two and three radix passes and with several radix blocks, an image of a
 batch against the same image alone where the two take different pass counts, per-layer partial weight / bias requests, and
 hidden units whose pre-activation is exactly 0."""
-import os
 import re
-import subprocess
 
-import numpy as np
 import pytest
 import torch
 
-import emu_harness
-from emu_harness import build, write_input
+from emu_harness import build
 from ordered_cases import GPU_RADIX_CASES, radix_passes_rule, read_dump, restate_ordered_dfeat, spread_case, zero_unit_case
-from vjp_cases import query_vjp_ref, rel_dist, vjp_bar
-
-emu_harness.HARNESSES.setdefault("emu_query_vjp_det", ("-O3", True))
+from vjp_cases import query_vjp_ref, rel_dist, run_vjp, vjp_bar
 
 DET = 1                                     # MP_VJP_DETERMINISTIC
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return build(tmp_path_factory, "emu_query_vjp_det")
+    return build(tmp_path_factory, "emu_fp32")
 
 
-def _run(emu, tmp_path, c, flags, chunk=0, sms=3, want="fpw", tag="v", env=None):
+def _run(emu, tmp_path, c, flags, chunk=0, sms=3, want="fpw", tag="v", **options):
     """stage 0 of a case on the CPU model -> (dfeat [B,C,H,W], dpoints [B,3,N], [dW_l], [db_l], stdout)"""
-    feat, pts, chans = c["feats"][0], c["points"], c["chans"]
-    B, C, H, W = feat.shape
-    N = pts.shape[2]
-    fin, fout = str(tmp_path / ("in_%s.bin" % tag)), str(tmp_path / ("out_%s.f32" % tag))
-    write_input(fin, feat, pts, c["calib"], c["proj"], chans[-1], c["last_op"], c["Ws"], c["bs"], batched=True)
-    fg = str(tmp_path / ("gout_%s.f32" % tag))
-    c["grad_output"][0].contiguous().numpy().astype(np.float32).tofile(fg)
-    r = subprocess.run([emu, fin, fout, str(B), ",".join(str(x) for x in chans[1:]), fg, str(chunk), str(sms), want],
-                       capture_output=True, text=True, timeout=3600, env=dict(os.environ, EMU_VJP_FLAGS=str(flags), **(env or {})))
-    assert r.returncode == 0, r.stderr[-2000:]
-    out = torch.from_numpy(np.fromfile(fout, dtype=np.float32))
-    o = 0
-
-    def take(shape):
-        nonlocal o
-        k = int(np.prod(shape))
-        t = out[o:o + k].reshape(shape)
-        o += k
-        return t
-    dfeat, dp = take((B, C, H, W)), take((B, 3, N))
-    dW = [take(tuple(w.shape)) for w in c["Ws"]]
-    db = [take(tuple(b.shape)) for b in c["bs"]]
-    assert o == out.numel()
-    return dfeat, dp, dW, db, r.stdout
+    return run_vjp(emu, tmp_path, c, c["feats"][0], c["grad_output"][0].contiguous(), chunk, want,
+                   options=dict(sms=sms, vjp_flags=flags, **options), tag=tag)
 
 
 def _ref(c, dtype):
@@ -88,7 +60,7 @@ def test_ordered_feature_gradient_at_every_radix_pass_count(emu, tmp_path, name)
     B, H, W, N, bands, passes = RADIX[name]
     c = spread_case(B, N, H, W, bands=bands, seed=len(name))
     dump = str(tmp_path / "dump.bin")
-    det = _run(emu, tmp_path, c, DET, want="f", tag="det", env=dict(EMU_VJP_DUMP=dump))
+    det = _run(emu, tmp_path, c, DET, want="f", tag="det", dump=dump)
     assert re.search(r"radix passes (\d)", det[4]).group(1) == str(passes)
     dx, wgt, keys, order = read_dump(dump)
     assert len(keys) > 2048                                    # several radix blocks
@@ -105,11 +77,11 @@ def test_ordered_feature_gradient_at_every_radix_pass_count(emu, tmp_path, name)
 def test_an_image_of_a_batch_is_that_image_alone_at_another_pass_count(emu, tmp_path):
     """one chunk: B = 3 maps of 10 x 10 take 2 passes, one of them alone 1; image b's columns keep their order"""
     c = spread_case(3, 150, 10, 10, seed=7)
-    batch = _run(emu, tmp_path, c, DET, want="f", tag="batch", env=dict(EMU_VJP_DUMP=str(tmp_path / "b.bin")))
+    batch = _run(emu, tmp_path, c, DET, want="f", tag="batch", dump=tmp_path / "b.bin")
     assert "radix passes 2" in batch[4]
     for b in range(3):
         cb = dict(c, feats=[c["feats"][0][b:b + 1]], points=c["points"][b:b + 1], grad_output=[c["grad_output"][0][b:b + 1]])
-        alone = _run(emu, tmp_path, cb, DET, want="f", tag="a%d" % b, env=dict(EMU_VJP_DUMP=str(tmp_path / "a.bin")))
+        alone = _run(emu, tmp_path, cb, DET, want="f", tag="a%d" % b, dump=tmp_path / "a.bin")
         assert "radix passes 1" in alone[4]
         assert torch.equal(batch[0][b:b + 1], alone[0]), b
 
@@ -129,7 +101,7 @@ def test_partial_requests_write_exactly_the_requested_layers(emu, tmp_path, flag
     full = _run(emu, tmp_path, c, flags, chunk=64, tag="full")
     assert all(bool((t != 0).any()) for t in full[2] + full[3])
     for i, (wm, bm) in enumerate(PARTIAL):
-        got = _run(emu, tmp_path, c, flags, chunk=64, tag="p%d" % i, env=dict(EMU_VJP_WMASK=str(wm), EMU_VJP_BMASK=str(bm)))
+        got = _run(emu, tmp_path, c, flags, chunk=64, tag="p%d" % i, wmask=wm, bmask=bm)
         assert torch.equal(got[1], full[1])
         for l in range(8):
             for mask, g, f in ((wm, got[2][l], full[2][l]), (bm, got[3][l], full[3][l])):

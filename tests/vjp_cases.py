@@ -1,6 +1,7 @@
 """The differentiable query for training (MonoPortNet.query_stages -> mp_query_points_vjp): a float64 / float32 restatement of
 the reference's train-mode query() differentiated by autograd (`query_vjp_ref`), the error bar of its gradients, the
-reference goldens (tests/golden/vjp_*.npz, tests/golden/make_vjp_golden.py) and the regeneration of their seeded inputs."""
+reference goldens (tests/golden/vjp_*.npz, tests/golden/make_vjp_golden.py), the regeneration of their seeded inputs, and
+the backward of one stage on the CPU model (`run_vjp`)."""
 import glob
 import os
 
@@ -9,6 +10,7 @@ import torch
 import torch.nn as nn
 
 from oracle import spec
+from emu_harness import run
 from helpers import GOLDEN
 
 GRAD_NAMES = ("dfeat", "dpoints", "dW", "db")
@@ -140,6 +142,22 @@ def load_vjp_case(name):
         c["dist_" + g] = float(z["dist_" + g])
     c["value"] = torch.from_numpy(z["value"])
     return c
+
+
+def run_vjp(exe, tmp_path, c, feat, grad_output, chunk, want="fpw", options=None, env=None, tag="v"):
+    """The backward of one stage -- the map feat [B,C,H,W], the case's points, head and camera -- by emu_fp32's vjp op.
+    grad_output: [B,Res,N] or "-" (ones).  -> (dfeat [B,C,H,W], dpoints [B,3,N], [dW_l], [db_l], stdout)"""
+    B, C, H, W = feat.shape
+    N = c["points"].shape[2]
+    inp = dict(feat=feat, rows=c["points"], calib=c["calib"], proj=c["proj"], res=c["chans"][-1], last_op=c["last_op"],
+               Ws=c["Ws"], bs=c["bs"], batched=True)
+    shapes = [(B, C, H, W), (B, 3, N)] + [tuple(w.shape) for w in c["Ws"]] + [tuple(b.shape) for b in c["bs"]]
+    sizes = [int(np.prod(s)) for s in shapes]
+    out, r = run(exe, tmp_path, "vjp", B, grad_output, chunk, want, inp=inp, shape=(sum(sizes),),
+                 options=dict(widths=",".join(str(x) for x in c["chans"][1:]), **(options or {})), env=env, tag=tag)
+    parts = [t.reshape(s) for t, s in zip(out.split(sizes), shapes)]
+    L = len(c["Ws"])
+    return parts[0], parts[1], parts[2:2 + L], parts[2 + L:], r.stdout
 
 
 def golden_bar(got_flat, c, g):
