@@ -97,8 +97,9 @@ int mp_feat_destroy(mp_feat_t* h);
 /* A handle that holds B maps of [C,H,W] -- the features of a batch [B,C,H,W] (MonoPortNet.py:48-91 takes any B).
  * mp_feat_create(C,H,W) is the B = 1 case.  On such a handle the three calls above read B contiguous maps: mp_feat_upload a
  * [B,C,H,W] NCHW block, mp_feat_upload_nhwc / mp_feat_bind_nhwc a [B,H,W,C] block (the memory of a torch.channels_last
- * [B,C,H,W] tensor).  Only mp_query_points_batch evaluates a handle with B > 1; every other entry point that takes an
- * mp_feat_t* returns MP_E_INVALID for it.
+ * [B,C,H,W] tensor).  Only mp_query_points_batch, mp_query_points_grad_batch and the VJP (mp_query_points_vjp,
+ * mp_query_points_vjp_ex) evaluate a handle with B > 1; every other entry point that takes an mp_feat_t* returns
+ * MP_E_INVALID for it.
  * Memory: besides the B fp32 maps (and a staging copy for host uploads) the tensor-core program keeps per-texel products for
  * every map -- per 128 x 128 map, G0 = 33.5 MB and the fp16 copy of the map 8.4 MB (16.8 MB for the colour head's 512
  * channels): a batch of 8 geometry maps holds about 0.34 GB of them. */
@@ -147,6 +148,19 @@ int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const float* point
                               int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
                               int64_t ld_grad, float* out_dev, int64_t ld_out, float* dpoints_dev, int64_t ld_dpoints,
                               const int32_t* count_dev, int mode, void* stream);
+/* mp_query_points_grad_mode over B images in one launch of each program: the value and the point gradient of
+ * MonoPortNet.query(feats[B,C,H,W], points[B,3,N], calibs[B,3|4,4]).  B must equal the handle's batch (a single-map handle
+ * is a batch of 1).  Points and calibs_dev as for mp_query_points_batch (calibs in DEVICE memory, or NULL for
+ * calibs=None).  grad_out_dev: [B][Res][n] dense (NULL: all ones); out_dev: [B][Res][n] dense, the value (NULL: not
+ * written); dpoints_dev: [B][3][n] dense.  Modes as mp_query_points_grad_mode, with the range guard decided per image on
+ * the device: in MP_MODE_TC / MP_MODE_AUTO the images whose largest |feature| is above the head's limit are differentiated
+ * by the exact kernel, the others by the tensor-core program; MP_MODE_AUTO takes the exact kernel for maps above 65536
+ * texels, which MP_MODE_TC refuses.  Image b's outputs are those of the single-map call on image b, bit for bit.
+ * Enqueue-only: nothing is read back to the host and the call does not synchronise. */
+int mp_query_points_grad_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
+                               int64_t batch_stride, int64_t row_stride, int64_t point_stride, const float* calibs_dev,
+                               int projection, float z_scale, const float* grad_out_dev, float* out_dev,
+                               float* dpoints_dev, int mode, void* stream);
 /* The vector-Jacobian product of MonoPortNet.query in MP_MODE_FP32, for training: with S = sum(grad_out * query(feats,
  * points, calibs)) over B images (the exact values, mp_query_points / mp_query_points_batch), every requested one of
  *   dfeat_dev      [B][C][H][W] = dS / d features (NCHW, like the map mp_feat_upload takes),

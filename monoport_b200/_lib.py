@@ -52,6 +52,8 @@ SIGNATURES = {
                                      c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p]),
     "mp_query_points_grad_mode": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_int64, P(c_float), c_int, c_float,
                                           c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int, c_void_p]),
+    "mp_query_points_grad_batch": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p,
+                                           c_int, c_float, c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "mp_query_points_vjp": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int64, c_int64, c_int64, c_int64, c_void_p, c_int,
                                     c_float, c_void_p, c_void_p, c_void_p, P(c_void_p), P(c_void_p), c_void_p, c_int64, c_void_p]),
     "mp_query_points_vjp_scratch_bytes": (c_int64, [c_void_p, c_void_p, c_int, c_int64, c_int64, c_int, c_int]),

@@ -341,6 +341,30 @@ extern "C" int mp_query_points_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, cons
                       out_dev, out_batch_stride, ld_out, mode, stream, true);
 }
 
+// The point gradient in `mode` over the images of bt (nullptr: one map; the layout of mp_launch_query_grad).  The rule of
+// mp_query_dispatch: the tensor-core program covers maps of at most 65536 texels, and an image above the head's feature
+// limit is taken by the exact kernel, decided on the device per image.
+static int grad_dispatch(mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
+                         int64_t ld_grad, float* out, int64_t ld_out, float* dpoints, int64_t ld_dpoints, int mode, cudaStream_t st,
+                         const MpBatch* bt) {
+  const bool tc_can = mlp->tc_ok && (long long)feat->H * feat->W <= 65536;
+  if (mode == MP_MODE_AUTO) mode = tc_can ? MP_MODE_TC : MP_MODE_FP32;
+  if (mode == MP_MODE_TC || mode == MP_MODE_TC_V3) {
+    if (!mlp->tc_ok) {
+      mp_set_error("MP_MODE_TC requested but the tensor-core kernel does not support this head/device");
+      return MP_E_UNSUPPORTED;
+    }
+    const bool guarded = isfinite(mlp->tc_amax_limit);
+    int rc = mp_launch_query_jvp_tc(mlp, feat, src, cal, grad_out, ld_grad, out, ld_out, dpoints, ld_dpoints, st,
+                                    guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE, bt);
+    if (rc != MP_OK || !guarded) return rc;
+    return mp_launch_query_grad(mlp, feat, src, cal, grad_out, ld_grad, out, ld_out, dpoints, ld_dpoints, st, MP_GUARD_OUT_OF_RANGE,
+                                bt);
+  }
+  MP_REQUIRE(mode == MP_MODE_FP32, "bad mode %d", mode);
+  return mp_launch_query_grad(mlp, feat, src, cal, grad_out, ld_grad, out, ld_out, dpoints, ld_dpoints, st, MP_GUARD_NONE, bt);
+}
+
 // mp_query_points_grad and mp_query_points_grad_mode
 static int query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
                              int64_t point_stride, const float* calib12, int projection, float z_scale, const float* grad_out_dev,
@@ -366,26 +390,8 @@ static int query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points
   MpCalib cal;
   MpBatch one;
   const MpBatch* single = mp_single_calib(cal, one, calib12, calib_dev, projection, z_scale);
-  cudaStream_t st = (cudaStream_t)stream;
-  // the rule of mp_query_dispatch: the tensor-core program covers maps of at most 65536 texels, and a frame above the head's
-  // feature limit is taken by the exact kernel, decided on the device
-  const bool tc_can = mlp->tc_ok && (long long)feat->H * feat->W <= 65536;
-  if (mode == MP_MODE_AUTO) mode = tc_can ? MP_MODE_TC : MP_MODE_FP32;
-  if (mode == MP_MODE_TC || mode == MP_MODE_TC_V3) {
-    if (!mlp->tc_ok) {
-      mp_set_error("MP_MODE_TC requested but the tensor-core kernel does not support this head/device");
-      return MP_E_UNSUPPORTED;
-    }
-    const bool guarded = isfinite(mlp->tc_amax_limit);
-    int rc = mp_launch_query_jvp_tc(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st,
-                                    guarded ? MP_GUARD_IN_RANGE : MP_GUARD_NONE, single);
-    if (rc != MP_OK || !guarded) return rc;
-    return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st,
-                                MP_GUARD_OUT_OF_RANGE, single);
-  }
-  MP_REQUIRE(mode == MP_MODE_FP32, "bad mode %d", mode);
-  return mp_launch_query_grad(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, st, MP_GUARD_NONE,
-                              single);
+  return grad_dispatch(mlp, feat, src, cal, grad_out_dev, ld_grad, out_dev, ld_out, dpoints_dev, ld_dpoints, mode,
+                       (cudaStream_t)stream, single);
 }
 
 extern "C" int mp_query_points_grad(mp_mlp_t* mlp, mp_feat_t* feat, const float* points_dev, int64_t n, int64_t row_stride,
@@ -402,6 +408,37 @@ extern "C" int mp_query_points_grad_mode(mp_mlp_t* mlp, mp_feat_t* feat, const f
                                          float* dpoints_dev, int64_t ld_dpoints, const int32_t* count_dev, int mode, void* stream) {
   return query_points_grad(mlp, feat, points_dev, n, row_stride, point_stride, calib12, projection, z_scale, grad_out_dev, ld_grad,
                            out_dev, ld_out, dpoints_dev, ld_dpoints, count_dev, mode, stream, "mp_query_points_grad_mode");
+}
+
+extern "C" int mp_query_points_grad_batch(mp_mlp_t* mlp, mp_feat_t* feat, int B, const float* points_dev, int64_t n,
+                                          int64_t batch_stride, int64_t row_stride, int64_t point_stride, const float* calibs_dev,
+                                          int projection, float z_scale, const float* grad_out_dev, float* out_dev,
+                                          float* dpoints_dev, int mode, void* stream) {
+  MpRange nvtx("monoport_b200: F1'' query gradient");
+  MP_REQUIRE(mlp && feat, "NULL handle");
+  MP_REQUIRE(B == feat->B, "batch size %d does not match the feature handle's %d maps", B, feat->B);
+  MP_REQUIRE(n >= 0 && row_stride >= 1 && point_stride >= 1 && (B == 1 || batch_stride >= 1),
+             "bad sizes n=%lld strides=%lld,%lld,%lld", (long long)n, (long long)batch_stride, (long long)row_stride,
+             (long long)point_stride);
+  // (the kernels find a tile's image with a 32-bit division: at most 2^31 tiles of 8 points per launch)
+  MP_REQUIRE((long long)B * ((n + 7) / 8) < (1ll << 31), "batch too large: %d x %lld points", B, (long long)n);
+  if (n == 0) return MP_OK;
+  MP_REQUIRE(points_dev && dpoints_dev, "NULL points/dpoints");
+  MpPointSrc src;
+  memset(&src, 0, sizeof(src));
+  src.kind = MP_SRC_ROWS;
+  src.px = points_dev; src.py = points_dev + row_stride; src.pz = points_dev + 2 * row_stride;
+  src.pstride = point_stride;
+  src.n = n;
+  MpCalib cal;
+  mp_fill_calib(cal, nullptr, projection, z_scale);
+  cal.has = calibs_dev != nullptr;
+  cal.perspective = projection == MP_PROJ_PERSPECTIVE && cal.has;
+  MpBatch bt;
+  bt.B = B;
+  bt.pt_stride = batch_stride;
+  bt.calibs = calibs_dev;
+  return grad_dispatch(mlp, feat, src, cal, grad_out_dev, n, out_dev, n, dpoints_dev, n, mode, (cudaStream_t)stream, &bt);
 }
 
 // ---------------------------------------------------------------------------------------------

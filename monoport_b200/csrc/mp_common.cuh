@@ -416,13 +416,15 @@ int mp_launch_query_tc_grid(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& 
 // gradient of the fp32 query with respect to the points (query_fp32.cu): value -> out[r*ld_out+i] (out may be null; written
 // by a query_fp32_kernel launch, so it is that kernel's value bit for bit),
 // d(sum_r grad_out[r*ld_grad+i] * value_r)/d point_i -> dpoints[a*ld_dp+i] (grad_out null = ones): one launch of the VJP
-// kernel below, for d points only; MP_SRC_ROWS, one map.  src.count_dev (when set) is the point count on the device;
-// `guard` as for the query launchers.
+// kernel below, for d points only; MP_SRC_ROWS.  bt: the images, as many as the handle's maps (nullptr: one map); image b's
+// rows follow image b-1's, at grad_out + b*Res*ld_grad, out + b*Res*ld_out and dpoints + b*3*ld_dp (bt->out_stride is
+// not read).  src.count_dev (when set) is the point count on the device; `guard` as for the query launchers.
 int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSrc& src, const MpCalib& cal,
                          const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
                          long long ld_dp, cudaStream_t st, int guard = MP_GUARD_NONE, const MpBatch* bt = nullptr);
-// the same outputs from the tensor-core program's forward-mode derivative (query_tc.cu: query_jvp_kernel), whose value is
-// the tensor-core query's bit for bit; the shipped heads, MP_SRC_ROWS, one map of at most 65536 texels
+// the same outputs, for the same images and layout, from the tensor-core program's forward-mode derivative (query_tc.cu:
+// query_jvp_kernel), whose value is the tensor-core query's bit for bit; the shipped heads, MP_SRC_ROWS, maps of at most
+// 65536 texels
 int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const float* grad_out,
                            long long ld_grad, float* out, long long ld_out, float* dpoints, long long ld_dp, cudaStream_t st,
                            int guard, const MpBatch* bt = nullptr);

@@ -743,24 +743,27 @@ int mp_launch_query_grad(const mp_mlp* mlp, const mp_feat* feat, const MpPointSr
                          const float* grad_out, long long ld_grad, float* out, long long ld_out, float* dpoints,
                          long long ld_dp, cudaStream_t st, int guard, const MpBatch* bt) {
   if (src.n <= 0) return MP_OK;
-  if (src.kind != MP_SRC_ROWS || (bt && bt->B != 1)) {
-    mp_set_error("the gradient kernel takes point rows of one map");
+  MpBatch b = bt ? *bt : MpBatch();
+  if (src.kind != MP_SRC_ROWS || feat->B != b.B) {
+    mp_set_error("the gradient kernel takes point rows, one set per map of the handle");
     return MP_E_UNSUPPORTED;
   }
+  const long long res = mlp->cout[mlp->n_layers - 1];
+  b.out_stride = res * ld_out;
   if (out) {                                      // the value: query_fp32_kernel's own, bit for bit
     MpOutDst dst;
     dst.out = out; dst.ld = ld_out; dst.scatter_vol = nullptr;
-    const int rq = mp_launch_query_fp32(mlp, feat, src, cal, dst, st, guard, bt);
+    const int rq = mp_launch_query_fp32(mlp, feat, src, cal, dst, st, guard, &b);
     if (rq != MP_OK) return rq;
   }
   const int P = reverse_tile(mlp, "gradient kernel");
   if (P < 0) return P;
-  MpVjpParams vp;                                 // d points of every tile of the map; no rows, no feature gradient
+  MpVjpParams vp;                                 // d points of every tile of the images; no rows, no feature gradient
   memset(&vp, 0, sizeof(vp));
-  vp.grad_out = grad_out; vp.ld_grad = ld_grad;
-  vp.dp = dpoints; vp.ld_dp = ld_dp;
-  vp.tile1 = (src.n + P - 1) / P;
-  return mp_launch_query_vjp_tiles(mlp, feat, src, cal, bt ? *bt : MpBatch(), vp, st, guard);
+  vp.grad_out = grad_out; vp.ld_grad = ld_grad; vp.gout_stride = res * ld_grad;
+  vp.dp = dpoints; vp.ld_dp = ld_dp; vp.dp_stride = 3 * ld_dp;
+  vp.tile1 = b.B * ((src.n + P - 1) / P);
+  return mp_launch_query_vjp_tiles(mlp, feat, src, cal, b, vp, st, guard);
 }
 
 int mp_query_vjp_tile(const mp_mlp* mlp) { return reverse_tile(mlp, "VJP kernel"); }

@@ -739,20 +739,21 @@ query_wg_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib ca
 //   layer 4:  the same fp32 hidden dot for every row, plus S4's value / x / y derivative, or w4z for the zf row.
 // Per point: g = grad_out * act'(y), d/d(ix, iy, zf) = sum_r g_r * y'_r, then d/du = d/dix (W-1)/2, d/dv = d/diy (H-1)/2,
 // d/dw = d/dzf z_scale and the projection's Jacobian as in query_grad_kernel.  Points outside the image get 0 for both.
-// One map; the range guard is decided per launch from amax[0] (producer and consumers take the same predicate).
+// bt.B images of src.n points, as query_wg_kernel covers a batch: tile t is tile t % n_tiles of image t / n_tiles, which
+// supplies its points, camera, per-texel products and output rows; the range guard skips the images outside the head's
+// range, the producer and the consumers deciding it from the same amax word (so the ring's stage counters stay in step).
 constexpr int kJvpPts = kTile / 4;      // points per tile
 constexpr int kJvpDwBytes = kJvpPts * 8 * 4;   // d wgt / d(ix, iy) of the tile's points, after Prog<C>::Total
 static_assert(Prog<256>::Total + kJvpDwBytes + 1024 <= 232448 && Prog<512>::Total + kJvpDwBytes + 1024 <= 232448,
               "shared memory budget of query_jvp_kernel (227 KB per CTA)");
 
 struct JvpOut {
-  float* out;             // [Res][ld_out] value, or null
+  float* out;             // image b: [Res][ld_out] value at out + b * MpBatch::out_stride, or null
   long long ld_out;
-  float* dp;              // [3][ld_dp]
-  long long ld_dp;
-  const float* grad_out;  // [Res][ld_grad], or null (ones)
-  long long ld_grad;
-  const float* calib;     // rows 0..2 of [R|t] in device memory, read when the kernel runs (null: MpCalib::m)
+  float* dp;              // image b: [3][ld_dp] at dp + b * dp_stride
+  long long ld_dp, dp_stride;
+  const float* grad_out;  // image b: [Res][ld_grad] at grad_out + b * gout_stride, or null (ones)
+  long long ld_grad, gout_stride;
 };
 
 // A-operand row of tangent t (0 value, 1 d/dix, 2 d/diy, 3 d/dzf) of point k of a tile
@@ -764,19 +765,18 @@ struct JvpTaps {
   float u, v, w;          // the projected point
 };
 
-__device__ __forceinline__ JvpTaps jvp_taps(const MpPointSrc& src, const MpCalib& cal, const float* calib, int H, int W, long long i,
-                                            long long n) {
+// point i of image b
+__device__ __forceinline__ JvpTaps jvp_taps(const MpPointSrc& src, const MpCalib& cal, const MpBatch& bt, int b, int H, int W,
+                                            long long i, long long n) {
   JvpTaps j;
   MpSurfaceSrc nosurf;
   memset(&nosurf, 0, sizeof(nosurf));
-  MpBatch one;                                       // (a single map; its camera in device memory when calib is set)
-  one.calibs = calib;
-  j.pt = point_taps(nosurf, src, cal, one, 0, H, W, i, n);
+  j.pt = point_taps(nosurf, src, cal, bt, b, H, W, i, n);
   float u = 0.f, v = 0.f, w = 0.f;
   if (i < n) {
     float x, y, z;
-    mp_load_point(src, one, 0, i, x, y, z);
-    mp_project<true>(mp_image_calib(cal, one, 0), x, y, z, u, v, w);
+    mp_load_point(src, bt, b, i, x, y, z);
+    mp_project<true>(mp_image_calib(cal, bt, b), x, y, z, u, v, w);
   }
   j.u = u; j.v = v; j.w = w;
   // the tap cell of mp_taps
@@ -826,7 +826,7 @@ __device__ __forceinline__ void jvp_hidden_epilogue(const TcParams& prm, const f
 
 template <int C>
 __global__ void __launch_bounds__(kThreads, 1)
-query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, JvpOut jo) {
+query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib cal, JvpOut jo, MpBatch bt) {
   using P = Prog<C>;
   constexpr int RES = P::RES, NP = kJvpPts;
   static_assert((5 + 3 * RES) * NP <= (2 + RES) * kTile, "per-point scalars of a JVP tile fit the Small block");
@@ -847,8 +847,10 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
     const long long c = __shfl_sync(0xffffffffu, *src.count_dev, 0);
     n = c < n ? c : n;
   }
-  const int skip = __shfl_sync(0xffffffffu, (int)mp_guard_skips(prm.amax, prm.amax_limit, prm.guard), 0);
-  const long long n_tiles = skip ? 0 : (n + NP - 1) / NP;
+  const long long n_tiles = (n + NP - 1) / NP;      // (per image)
+  const long long all_tiles = n_tiles * bt.B;
+  // the range guard of image b, read once per image a CTA meets (the consumer warps take lane 0's answer)
+  auto image_skipped = [&](int b) { return mp_guard_skips(prm.amax + b, prm.amax_limit, prm.guard); };
 
   if (tid == 0) ring_init<C>(full, empty);
   __syncthreads();
@@ -859,7 +861,20 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
     if (warp == 8 && lane == 0) {
       const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(prm.wstream);
       uint32_t phase = P::ProducerPhase0;
-      for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) produce_tile<C>(smem, full, empty, wsrc, phase);
+      bool skip = false;
+      int guard_b = -1;
+      for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
+        const int b = mp_tile_image(bt, t, n_tiles);
+        if (b != guard_b) {
+          skip = image_skipped(b);
+          guard_b = b;
+        }
+        if (skip) {
+          t = mp_skip_image(bt, t, b, n_tiles);
+          continue;
+        }
+        produce_tile<C>(smem, full, empty, wsrc, phase);
+      }
     }
     return;
   }
@@ -927,10 +942,24 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
     tc::fence_proxy_async_smem();
   };
 
-  for (long long t = blockIdx.x; t < n_tiles; t += gridDim.x) {
-    const long long p0 = t * NP;
+  int guard_b = -1, skip = 0;
+  for (long long t = blockIdx.x; t < all_tiles; t += gridDim.x) {
+    const int b = mp_tile_image(bt, t, n_tiles);
+    if (b != guard_b) {
+      skip = __shfl_sync(0xffffffffu, (int)image_skipped(b), 0);
+      guard_b = b;
+    }
+    if (skip) {
+      t = mp_skip_image(bt, t, b, n_tiles);
+      continue;
+    }
+    const long long p0 = (t - (long long)b * n_tiles) * NP;
+    const size_t texel0 = (size_t)b * prm.H * prm.W;
+    g0 = prm.g0 + texel0 * kL0;
+    const __half* feat16 = prm.feat16 + texel0 * C;
+    const float* s4tex = prm.s4tex + texel0 * RES;
     // ---- this lane's point (lane % 16) of the tile; X and the per-point scalars: warp w samples points 2w, 2w + 1
-    const JvpTaps jt = jvp_taps(src, cal, jo.calib, prm.H, prm.W, p0 + (lane & 15), n);
+    const JvpTaps jt = jvp_taps(src, cal, bt, b, prm.H, prm.W, p0 + (lane & 15), n);
 #pragma unroll 1
     for (int qq = 0; qq < 2; ++qq) {
       const int q = 2 * warp + qq;
@@ -948,7 +977,7 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
         const int cbase = phase * 256 + lane * 8;
         uint4 raw[4];
 #pragma unroll
-        for (int a = 0; a < 4; ++a) raw[a] = __ldg(reinterpret_cast<const uint4*>(prm.feat16 + (size_t)off[a] * C + cbase));
+        for (int a = 0; a < 4; ++a) raw[a] = __ldg(reinterpret_cast<const uint4*>(feat16 + (size_t)off[a] * C + cbase));
         float2 acc[4], ax[4], ay[4];
 #pragma unroll
         for (int a = 0; a < 4; ++a) {        // the value as store_x8 takes it: nw, ne, sw, se
@@ -980,7 +1009,7 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
         float s = 0.f, sx = 0.f, sy = 0.f;
 #pragma unroll
         for (int a = 0; a < 4; ++a) {
-          const float s4 = __ldg(prm.s4tex + (size_t)pt.off[a] * RES + r);
+          const float s4 = __ldg(s4tex + (size_t)pt.off[a] * RES + r);
           s = fmaf(pt.wgt[a], s4, s);
           sx = fmaf(jt.dx[a], s4, sx);
           sy = fmaf(jt.dy[a], s4, sy);
@@ -1098,14 +1127,15 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
         }
         const long long i = p0 + kpt;
         if (isv && mine == 0 && i < n) {
+          const int b = mp_tile_image(bt, t, n_tiles);       // (re-derived: not held across the trunk)
           const float inimg = s_in[kpt];
           float gx = 0.f, gy = 0.f, gz = 0.f;
 #pragma unroll
           for (int r = 0; r < RES; ++r) {
             const float act = mp_last_op(y[r], prm.last_op);
-            if (jo.out) jo.out[(long long)r * jo.ld_out + i] = inimg * act;
+            if (jo.out) jo.out[b * bt.out_stride + (long long)r * jo.ld_out + i] = inimg * act;
             const float d = prm.last_op == MP_LAST_SIGMOID ? act * (1.f - act) : (prm.last_op == MP_LAST_TANH ? 1.f - act * act : 1.f);
-            const float g = (jo.grad_out ? __ldg(jo.grad_out + (long long)r * jo.ld_grad + i) : 1.f) * d;
+            const float g = (jo.grad_out ? __ldg(jo.grad_out + b * jo.gout_stride + (long long)r * jo.ld_grad + i) : 1.f) * d;
             gx = fmaf(g, yx[r], gx);
             gy = fmaf(g, yy[r], gy);
             gz = fmaf(g, yz[r], gz);
@@ -1115,10 +1145,9 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
           if (!cal.has) {
             gp[0] = du; gp[1] = dv; gp[2] = dw;
           } else {
-            // the camera jvp_taps projected with (device memory when jo.calib is set), read where the Jacobian needs it
-            MpBatch one;
-            one.calibs = jo.calib;
-            const MpCalib c = mp_image_calib(cal, one, 0);
+            // the camera jvp_taps projected with (image b's, in device memory when bt.calibs is set), read where the
+            // Jacobian needs it
+            const MpCalib c = mp_image_calib(cal, bt, b);
             if (!c.perspective) {                        // J = R
 #pragma unroll
               for (int a = 0; a < 3; ++a) gp[a] = c.m[a] * du + c.m[4 + a] * dv + c.m[8 + a] * dw;
@@ -1131,7 +1160,7 @@ query_jvp_kernel(const __grid_constant__ TcParams prm, MpPointSrc src, MpCalib c
             }
           }
 #pragma unroll
-          for (int a = 0; a < 3; ++a) jo.dp[a * jo.ld_dp + i] = inimg != 0.f ? gp[a] : 0.f;     // outside the image: exactly 0
+          for (int a = 0; a < 3; ++a) jo.dp[b * jo.dp_stride + a * jo.ld_dp + i] = inimg != 0.f ? gp[a] : 0.f;   // outside the image: exactly 0
         }
       }
     };
@@ -1509,19 +1538,19 @@ int launch(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc&
   return MP_OK;
 }
 
-// the per-frame products, then the JVP program over src.n points of the single map of feat (16 points per tile)
+// the per-frame products, then the JVP program over the images of bt, src.n points each (16 points per tile)
 template <int C>
 int launch_jvp(const mp_mlp* mlp, const TcPack* pk, mp_feat* feat, const MpPointSrc& src, const MpCalib& cal, const JvpOut& jo,
-               cudaStream_t st, int guard) {
+               cudaStream_t st, int guard, const MpBatch& bt) {
   using P = Prog<C>;
   TcParams prm;
   int grid = 0;
-  const int rs = launch_setup<C>(mlp, pk, feat, st, guard, (src.n + kJvpPts - 1) / kJvpPts, prm, grid);
+  const int rs = launch_setup<C>(mlp, pk, feat, st, guard, bt.B * ((src.n + kJvpPts - 1) / kJvpPts), prm, grid);
   if (rs != MP_OK) return rs;
 #ifndef MP_CUDA_EMU
-  query_jvp_kernel<C><<<grid, kThreads, P::Total + kJvpDwBytes + 1024, st>>>(prm, src, cal, jo);
+  query_jvp_kernel<C><<<grid, kThreads, P::Total + kJvpDwBytes + 1024, st>>>(prm, src, cal, jo, bt);
 #else
-  MP_EMU_LAUNCH(grid, kThreads, (query_jvp_kernel<C>(prm, src, cal, jo)));
+  MP_EMU_LAUNCH(grid, kThreads, (query_jvp_kernel<C>(prm, src, cal, jo, bt)));
 #endif
   MP_CUDA(cudaGetLastError());
   return MP_OK;
@@ -1790,14 +1819,21 @@ int mp_launch_query_jvp_tc(const mp_mlp* mlp, mp_feat* feat, const MpPointSrc& s
   const int rc = check_query(mlp, feat, C);
   if (rc != MP_OK) return rc;
   const TcPack* pk = static_cast<const TcPack*>(mlp->tc);
-  if (src.kind != MP_SRC_ROWS || feat->B != 1 || (bt && bt->B != 1)) {
-    mp_set_error("the gradient program takes point rows of one map");
+  MpBatch b = bt ? *bt : MpBatch();
+  if (src.kind != MP_SRC_ROWS || feat->B != b.B) {
+    mp_set_error("the gradient program takes point rows, one set per map of the handle");
     return MP_E_UNSUPPORTED;
   }
+  // (the kernel finds a tile's image with a 32-bit division)
+  if (b.B > 1 && b.B * ((src.n + kJvpPts - 1) / kJvpPts) >= (1ll << 31)) {
+    mp_set_error("batch too large for the gradient program: %d x %lld points", b.B, src.n);
+    return MP_E_UNSUPPORTED;
+  }
+  const long long res = pk->res;
+  b.out_stride = res * ld_out;
   JvpOut jo;
   jo.out = out; jo.ld_out = ld_out;
-  jo.dp = dpoints; jo.ld_dp = ld_dp;
-  jo.grad_out = grad_out; jo.ld_grad = ld_grad;
-  jo.calib = bt ? bt->calibs : nullptr;
-  return C == 256 ? launch_jvp<256>(mlp, pk, feat, src, cal, jo, st, guard) : launch_jvp<512>(mlp, pk, feat, src, cal, jo, st, guard);
+  jo.dp = dpoints; jo.ld_dp = ld_dp; jo.dp_stride = 3 * ld_dp;
+  jo.grad_out = grad_out; jo.ld_grad = ld_grad; jo.gout_stride = res * ld_grad;
+  return C == 256 ? launch_jvp<256>(mlp, pk, feat, src, cal, jo, st, guard, b) : launch_jvp<512>(mlp, pk, feat, src, cal, jo, st, guard, b);
 }

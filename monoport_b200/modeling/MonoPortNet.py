@@ -262,13 +262,15 @@ class MonoPortNet(nn.Module):
 
     @torch.no_grad()
     def query_gradient(self, feats_stages, points, calibs=None, grad_output=None, precision="fp32"):
-        """query() and its gradient with respect to the points (mp_query_points_grad_mode).  feats/points/calibs as for
-        query() with B == 1; grad_output [1,Res,N] or None (ones).
-        precision "fp32" (default): one launch of the exact fp32 kernel; preds bit-identical to query() with precision "fp32".
-        "tc": the tensor-core program's forward-mode derivative; preds bit-identical to query() with precision "tc", and a
-        frame above the head's feature limit is differentiated exactly (decided on the GPU).  Maps above 65536 texels are
-        refused.  "auto": "tc" where the head and the map allow it, else "fp32".
-        -> (preds [1,Res,N], dpoints [1,3,N] = d sum(grad_output * preds) / d points; for the geometry head and
+        """query() and its gradient with respect to the points.  feats/points/calibs as for query(); grad_output [B,Res,N] or
+        None (ones).  B == 1: one map (mp_query_points_grad_mode, the camera by value, read back once per frame scope).
+        B > 1: the B images in one launch of each program (mp_query_points_grad_batch): the calibs stay on the device, nothing
+        is read back and nothing synchronises; image b's results are those of the B == 1 call on image b, bit for bit.
+        precision "fp32" (default): the exact fp32 kernel; preds bit-identical to query() with precision "fp32".
+        "tc": the tensor-core program's forward-mode derivative; preds bit-identical to query() with precision "tc", and an
+        image above the head's feature limit is differentiated exactly (decided on the GPU, per image).  Maps above 65536
+        texels are refused.  "auto": "tc" where the head and the map allow it, else "fp32".
+        -> (preds [B,Res,N], dpoints [B,3,N] = d sum(grad_output * preds) / d points; for the geometry head and
             grad_output=None, grad sigma).
         Points outside the image get 0 for both.  Autograd is not involved: `points.requires_grad` is ignored."""
         if precision not in ("fp32", "tc", "auto"):
@@ -277,8 +279,7 @@ class MonoPortNet(nn.Module):
             raise NotImplementedError("query_gradient is eval-mode only (the gradient of the last stage, like query()); "
                                       "call .eval()")
         feat = self._checked_map(feats_stages[-1], points, calibs, "query_gradient", calib_rows=False)
-        if feat.shape[0] != 1:
-            raise ValueError("query_gradient takes one feature map [1,C,H,W]; got %s" % (tuple(feat.shape),))
+        B = feat.shape[0]
         points = self._points_rows(points)
         n = points.shape[2]
         s = points.stride()
@@ -286,22 +287,32 @@ class MonoPortNet(nn.Module):
         res = head.filter_channels[-1]
         gout = None
         if grad_output is not None:
-            if tuple(grad_output.shape) != (1, res, n):
-                raise ValueError("grad_output must be [1,%d,%d]; got %s" % (res, n, tuple(grad_output.shape)))
+            if tuple(grad_output.shape) != (B, res, n):
+                raise ValueError("grad_output must be [%d,%d,%d]; got %s" % (B, res, n, tuple(grad_output.shape)))
             if grad_output.device != feat.device:
                 raise ValueError("grad_output and features live on different devices")
-            gout = grad_output.detach()[0].to(torch.float32).contiguous()
-        out = torch.empty((1, res, n), dtype=torch.float32, device=feat.device)
-        dp = torch.empty((1, 3, n), dtype=torch.float32, device=feat.device)
+            gout = grad_output.detach().to(torch.float32).contiguous()
+        out = torch.empty((B, res, n), dtype=torch.float32, device=feat.device)
+        dp = torch.empty((B, 3, n), dtype=torch.float32, device=feat.device)
         if n == 0:
             return out, dp
+        gptr = None if gout is None else ctypes.c_void_p(gout.data_ptr())
         with _lib.device_guard(feat.device):
-            fh = self.feature_handle(feat)
-            _lib.check(_lib.load().mp_query_points_grad_mode(
-                head.handle(), fh.ptr, ctypes.c_void_p(points.data_ptr()), n, s[1], s[2], _lib.calib12(calibs), self._proj(),
-                ctypes.c_float(self.normalizer.scale), None if gout is None else ctypes.c_void_p(gout.data_ptr()), n,
-                ctypes.c_void_p(out.data_ptr()), n, ctypes.c_void_p(dp.data_ptr()), n, None, _MODES[precision],
-                _lib.stream_ptr(feat.device)), "mp_query_points_grad_mode")
+            fh = self._feature_handle(feat)
+            if B == 1:
+                _lib.check(_lib.load().mp_query_points_grad_mode(
+                    head.handle(), fh.ptr, ctypes.c_void_p(points.data_ptr()), n, s[1], s[2], _lib.calib12(calibs),
+                    self._proj(), ctypes.c_float(self.normalizer.scale), gptr, n, ctypes.c_void_p(out.data_ptr()), n,
+                    ctypes.c_void_p(dp.data_ptr()), n, None, _MODES[precision], _lib.stream_ptr(feat.device)),
+                    "mp_query_points_grad_mode")
+            else:
+                cal = self._calib_rows(calibs, feat.device)
+                _lib.check(_lib.load().mp_query_points_grad_batch(
+                    head.handle(), fh.ptr, B, ctypes.c_void_p(points.data_ptr()), n, s[0], s[1], s[2],
+                    None if cal is None else ctypes.c_void_p(cal.data_ptr()), self._proj(),
+                    ctypes.c_float(self.normalizer.scale), gptr, ctypes.c_void_p(out.data_ptr()),
+                    ctypes.c_void_p(dp.data_ptr()), _MODES[precision], _lib.stream_ptr(feat.device)),
+                    "mp_query_points_grad_batch")
         return out, dp
 
     # ---- training: the differentiable query ---------------------------------------------------------------

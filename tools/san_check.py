@@ -1,7 +1,7 @@
 """Tiny invocation of every kernel family for compute-sanitizer (memcheck): both tensor-core programs, the fp32 kernel and
-its point-gradient kernel, the octree engine (eager, and a captured lossless frame), marching cubes, the visible-surface
-kernel and the enqueue-only renders of captured frames (mp_colorize_surface_async on both programs,
-mp_render_normals_async)."""
+its point-gradient kernel (single maps and batches), the octree engine (eager, and a captured lossless frame), marching
+cubes, the visible-surface kernel and the enqueue-only renders of captured frames (mp_colorize_surface_async on both
+programs, mp_render_normals_async)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
@@ -77,6 +77,12 @@ for mode in ("fp32", "tc", "auto"):
     ob = net.query([[fb]], pb, calibs=cb)[0]
     torch.cuda.synchronize()
     print("batch", mode, float(ob.sum()))
+# the batched point gradient (one launch of each program over the three images): in "tc" image 1 is differentiated by the
+# exact kernel, the others by the tensor-core program
+for precision in ("fp32", "tc"):
+    vb, db = net.query_gradient([[fb]], pb, calibs=cb, precision=precision)
+    torch.cuda.synchronize()
+    print("batch grad", precision, float(db.abs().sum()))
 # the point-gradient kernel: geometry head (ragged last tile), colour head with a grad_output and [N,3]-strided points
 vg, dg = net.query_gradient([[feat.cuda()]], pts[:, :, :123], calibs=cal)
 pv = pts[0, :, :77].t().contiguous().t()[None]
