@@ -433,6 +433,28 @@ int mp_mesh_normals_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, const float* vert
                                const int32_t* count32_dev, int64_t capacity, const float* calib_dev, int projection,
                                float z_scale, int mode, float* scratch_dev, float* norm_dev, void* stream);
 
+/* Mesh refinement (DESIGN.md §F3.1): move the vertices of a marching-cubes mesh onto the geometry network's own iso-surface
+ * along their edges, enqueue-only (graph-capturable).  Vertex v lies on the +axis edge of its owning node a; the edge's
+ * volume values va, vb bracket iso.  `rounds` rounds of regula falsi with the Illinois modification inside that bracket each
+ * evaluate the network once per vertex through the query program (`mode`, the range guard decided on the device, like
+ * mp_query_points_count), starting at the emitted vertex; the candidate with the smallest |sigma - iso| is then written
+ * over verts_dev[v] in world space.  A refined vertex stays on its edge, so faces and topology are marching cubes'.
+ * Precondition: `ws` is the workspace whose last run (mp_mcubes_run_async, or mp_mcubes_count + mp_mcubes_emit) read
+ * vol_dev at iso, and verts_dev [v_cap][3] holds that run's world-space vertices under `world` (7 host floats {R, b_min[3],
+ * b_max[3]} as mp_mcubes_run_async; R must be the side of the workspace's cubic volume).  count32_dev: the vertex count on
+ * the device (mp_mcubes_run_async's min(nV, v_cap)); vertices at or beyond min(count32, v_cap), faces and counts are never
+ * touched.  rounds = 0 enqueues nothing; rounds = 1 rewrites every vertex with its own bits.  scratch_dev: at least
+ * mp_mesh_refine_scratch_bytes(v_cap) bytes of device memory (about 50 B per vertex of capacity), private to the call until
+ * it completes.  The head must have one output; batch handles are refused. */
+int64_t mp_mesh_refine_scratch_bytes(int64_t v_cap);
+int mp_mesh_refine_async(mp_mlp_t* mlp, mp_feat_t* feat, mp_mcubes_t* ws, const float* vol_dev, float iso, const float* world,
+                         float* verts_dev, const int32_t* count32_dev, int64_t v_cap, int rounds, const float* calib12,
+                         int projection, float z_scale, int mode, void* scratch_dev, void* stream);
+/* mp_mesh_refine_async with the camera in device memory (see mp_query_points_count_dcal). */
+int mp_mesh_refine_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, mp_mcubes_t* ws, const float* vol_dev, float iso,
+                              const float* world, float* verts_dev, const int32_t* count32_dev, int64_t v_cap, int rounds,
+                              const float* calib_dev, int projection, float z_scale, int mode, void* scratch_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

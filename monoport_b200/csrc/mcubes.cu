@@ -14,10 +14,14 @@
 // mp_mcubes_run_async: the same launches without the host (graph-capturable, replayable on one workspace): the emission grid
 //         is fixed at record time and reads the active-list length on the device; caller buffers with capacities, the true
 //         totals and the vertex count left on the device, optional world-space vertices.
+// refine: mp_mesh_refine_async moves the vertices of the last run onto the network's own iso-surface along their edges
+//         (DESIGN.md §F3.1): mesh_edges_kernel (vertex -> owning node + axis, the emission's walk), refine_init_kernel, then
+//         per round the query program at the candidates and refine_step_kernel (refine_kernels.cuh).
 // Workspace: 1 bit + 24 B per 32 nodes (15 MB at 257^3; the round-1 byte-per-node design took 102 MB).
 #include "mp_common.cuh"
 #include <stdlib.h>
 #include "mcubes_kernels.cuh"
+#include "refine_kernels.cuh"
 
 using namespace mcubes;
 
@@ -35,6 +39,7 @@ struct mp_mcubes {
   unsigned long long* total;
   long long nv, nf;
   int counted;
+  int ran;                     // a count has been enqueued: the prefixes and the active list are defined
 };
 
 extern "C" int mp_mcubes_destroy(mp_mcubes_t* h) {
@@ -109,6 +114,7 @@ static int enqueue_count(mp_mcubes* h, const float* vol_dev, float iso, cudaStre
   PrefixEmit em{h->prefix, h->active, h->n_active_dev};
   mpscan::emit_kernel<WordCountF, PrefixEmit><<<nb, mpscan::kThreads, 0, st>>>(f2, em, h->n_words, h->sums);
   MP_CUDA(cudaGetLastError());
+  h->ran = 1;
   return MP_OK;
 }
 
@@ -182,4 +188,92 @@ extern "C" int mp_mcubes_run_async(mp_mcubes_t* h, const float* vol_dev, float i
       reinterpret_cast<long long*>(counts_dev), count32_dev, h->D, h->H, h->W, h->n, iso);
   MP_CUDA(cudaGetLastError());
   return MP_OK;
+}
+
+// ---- mesh refinement (DESIGN.md §F3.1)
+// scratch layout (mrefine::State), each array 256-byte aligned: 3 + 1 + 7 float rows, the node records, the flag bytes
+static size_t refine_align(size_t b) { return (b + 255) & ~(size_t)255; }
+
+extern "C" int64_t mp_mesh_refine_scratch_bytes(int64_t v_cap) {
+  if (v_cap < 0 || v_cap > INT32_MAX) return -1;
+  const size_t c = (size_t)v_cap;
+  return (int64_t)(11 * refine_align(c * sizeof(float)) + refine_align(c * sizeof(uint32_t)) + refine_align(c));
+}
+
+static int mesh_refine_async(mp_mlp_t* mlp, mp_feat_t* feat, mp_mcubes_t* h, const float* vol_dev, float iso, const float* world,
+                             float* verts_dev, const int32_t* count32_dev, int64_t v_cap, int rounds, const float* calib12,
+                             const float* calib_dev, int projection, float z_scale, int mode, void* scratch_dev, void* stream,
+                             const char* what) {
+  MP_REQUIRE(mlp && feat && h && vol_dev && world && count32_dev, "%s: NULL argument", what);
+  MP_REQUIRE(rounds >= 0, "%s: bad rounds %d", what, rounds);
+  MP_REQUIRE(v_cap >= 0 && v_cap <= INT32_MAX, "%s: bad capacity v_cap=%lld", what, (long long)v_cap);
+  MP_REQUIRE((verts_dev && scratch_dev) || v_cap == 0, "%s: NULL argument", what);
+  MP_REQUIRE(mlp->cout[mlp->n_layers - 1] == 1, "mesh refinement needs a head with one output (got %d)", mlp->cout[mlp->n_layers - 1]);
+  MP_REQUIRE_SINGLE_MAP(feat, what);
+  const float R = world[0];
+  MP_REQUIRE(h->D == h->H && h->H == h->W && R == (float)h->W,
+             "%s: the world mapping's R=%g is not the side of the workspace's %dx%dx%d volume", what, (double)R, h->D, h->H, h->W);
+  MP_REQUIRE(h->ran, "%s: the workspace has not run marching cubes", what);
+  if (rounds == 0 || v_cap == 0) return MP_OK;
+  MpRange nvtx("monoport_b200: F3.1 mesh refinement (enqueue-only)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t c = (size_t)v_cap;
+  char* base = static_cast<char*>(scratch_dev);
+  float* rows[11];
+  for (int k = 0; k < 11; ++k) rows[k] = reinterpret_cast<float*>(base + k * refine_align(c * sizeof(float)));
+  mrefine::State s;
+  s.pts = rows[0];                                    // rows 0..2: the query's point rows
+  s.sigma = rows[3];
+  s.ta = rows[4]; s.fa = rows[5]; s.tb = rows[6]; s.fb = rows[7];
+  s.tbest = rows[8]; s.fbest = rows[9]; s.tcur = rows[10];
+  s.node = reinterpret_cast<uint32_t*>(base + 11 * refine_align(c * sizeof(float)));
+  s.flags = reinterpret_cast<uint8_t*>(base + 11 * refine_align(c * sizeof(float)) + refine_align(c * sizeof(uint32_t)));
+  s.cap = (uint32_t)v_cap;
+  mrefine::Geom g;
+  g.H = h->H; g.W = h->W;
+  g.iso = iso;
+  for (int a = 0; a < 3; ++a) {
+    g.scale[a] = (world[4 + a] - world[1 + a]) / R;          // mp_mcubes_run_async's mapping
+    g.bmin[a] = world[1 + a];
+  }
+  {
+    // the emission's persistent grid: 4 CTAs per SM, and no more warps than the volume has words
+    const long long blocks_needed = (h->n_words + kEdgesThreads / 32 - 1) / (kEdgesThreads / 32);
+    const long long cap = (long long)sm_count() * 4;
+    mesh_edges_kernel<<<(unsigned)(blocks_needed < cap ? blocks_needed : cap), kEdgesThreads, 0, st>>>(
+        h->info, h->prefix, h->active, h->n_active_dev, (uint32_t)v_cap, s.node, s.flags);
+  }
+  MP_CUDA(cudaGetLastError());
+  const long long blocks = (v_cap + mrefine::kThreads - 1) / mrefine::kThreads;
+  const long long cap = (long long)sm_count() * 8;
+  const unsigned grid = (unsigned)(blocks < cap ? blocks : cap);
+  mrefine::refine_init_kernel<<<grid, mrefine::kThreads, 0, st>>>(vol_dev, count32_dev, s, g);
+  MP_CUDA(cudaGetLastError());
+  for (int r = 0; r < rounds; ++r) {
+    // the query program at the candidates: rows [3][v_cap], the count and the range guard on the device
+    const int rc = calib_dev ? mp_query_points_count_dcal(mlp, feat, s.pts, v_cap, v_cap, 1, calib_dev, projection, z_scale, s.sigma,
+                                                          v_cap, count32_dev, mode, stream)
+                             : mp_query_points_count(mlp, feat, s.pts, v_cap, v_cap, 1, calib12, projection, z_scale, s.sigma, v_cap,
+                                                     count32_dev, mode, stream);
+    if (rc != MP_OK) return rc;
+    mrefine::refine_step_kernel<<<grid, mrefine::kThreads, 0, st>>>(count32_dev, s, g, r == rounds - 1, verts_dev);
+    MP_CUDA(cudaGetLastError());
+  }
+  return MP_OK;
+}
+
+extern "C" int mp_mesh_refine_async(mp_mlp_t* mlp, mp_feat_t* feat, mp_mcubes_t* ws, const float* vol_dev, float iso,
+                                    const float* world, float* verts_dev, const int32_t* count32_dev, int64_t v_cap, int rounds,
+                                    const float* calib12, int projection, float z_scale, int mode, void* scratch_dev, void* stream) {
+  return mesh_refine_async(mlp, feat, ws, vol_dev, iso, world, verts_dev, count32_dev, v_cap, rounds, calib12, nullptr, projection,
+                           z_scale, mode, scratch_dev, stream, "mp_mesh_refine_async");
+}
+
+extern "C" int mp_mesh_refine_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, mp_mcubes_t* ws, const float* vol_dev, float iso,
+                                         const float* world, float* verts_dev, const int32_t* count32_dev, int64_t v_cap,
+                                         int rounds, const float* calib_dev, int projection, float z_scale, int mode,
+                                         void* scratch_dev, void* stream) {
+  MP_REQUIRE(calib_dev, "NULL calib_dev");
+  return mesh_refine_async(mlp, feat, ws, vol_dev, iso, world, verts_dev, count32_dev, v_cap, rounds, nullptr, calib_dev, projection,
+                           z_scale, mode, scratch_dev, stream, "mp_mesh_refine_async_dcal");
 }

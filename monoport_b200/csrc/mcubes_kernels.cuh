@@ -198,6 +198,43 @@ __device__ __forceinline__ int32_t vertex_id(const WordInfo* __restrict__ info, 
   return (int32_t)id;
 }
 
+// The vertex arithmetic of the emission, shared with mesh_edges_kernel and the refinement (refine_kernels.cuh), which must
+// reproduce the emitted vertices bit for bit.
+// (x, y, z) of node i (32-bit: mp_mcubes_create bounds the volume below 2^31 nodes)
+__device__ __forceinline__ void node_xyz(uint32_t i, uint32_t plane, int W, uint32_t& x, uint32_t& y, uint32_t& z) {
+  z = i / plane;
+  const uint32_t r = i - z * plane;
+  y = r / (uint32_t)W;
+  x = r - y * (uint32_t)W;
+}
+
+// id of the first vertex owned by node `lane` of a word: the word's prefix + the owned edges of the nodes below it
+__device__ __forceinline__ uint32_t word_vertex_base(unsigned long long pre, uint32_t ex, uint32_t ey, uint32_t ez, int lane) {
+  const uint32_t below = (1u << lane) - 1u;
+  return (uint32_t)pre + __popc(ex & below) + __popc(ey & below) + __popc(ez & below);
+}
+
+// the owned edges of node `lane` of a word: bit a = its +a edge is active
+__device__ __forceinline__ uint32_t lane_edge_code(uint32_t ex, uint32_t ey, uint32_t ez, int lane) {
+  return ((ex >> lane) & 1u) | (((ey >> lane) & 1u) << 1) | (((ez >> lane) & 1u) << 2);
+}
+
+// the linear interpolation of marching cubes: the parameter of iso between va (t = 0) and vb (t = 1)
+__device__ __forceinline__ float edge_t0(float va, float vb, float iso) { return __fdiv_rn(__fsub_rn(iso, va), __fsub_rn(vb, va)); }
+
+// index-space point at parameter t on the +axis edge of node (x, y, z)
+__device__ __forceinline__ void edge_point(uint32_t x, uint32_t y, uint32_t z, int axis, float t, float (&p)[3]) {
+  p[0] = (float)x; p[1] = (float)y; p[2] = (float)z;
+  p[axis] = __fadd_rn(p[axis], t);
+}
+
+// index space -> reconstruction()'s world point (p + 0.5) * scale + b_min, with torch's three fp32 roundings (intrinsics, so
+// that no FMA contraction fuses them)
+__device__ __forceinline__ void world_point(const float (&scale)[3], const float (&bmin)[3], float (&p)[3]) {
+#pragma unroll
+  for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(__fmul_rn(__fadd_rn(p[a], 0.5f), scale[a]), bmin[a]);
+}
+
 // ---- pass 4: emission, two phases per round of a CTA.
 // (a) one warp per word with a surface inside (the active list), one lane per node: up to three vertices (vertex id = rank of
 //     (node, axis) in node order), and the cell's triangles are QUEUED in shared memory -- (corner-0 node, triangle index,
@@ -249,26 +286,22 @@ __device__ __forceinline__ void mesh_emit_body(const float* __restrict__ vol, co
       const uint32_t ex = wi.x, ey = wi.y, ez = wi.z, nt = wi.w;
       const unsigned long long pre = __ldg(prefix + w);
       const uint32_t i = 32u * w + (uint32_t)lane;                                // this lane's node
-      const uint32_t z = i / plane, r = i - z * plane, y = r / (uint32_t)W, x = r - y * (uint32_t)W;
+      uint32_t x, y, z;
+      node_xyz(i, plane, W, x, y, z);
       // ---- vertices on the owned edges
-      const uint32_t below = (1u << lane) - 1u;
-      const uint32_t code = ((ex >> lane) & 1u) | (((ey >> lane) & 1u) << 1) | (((ez >> lane) & 1u) << 2);
+      const uint32_t code = lane_edge_code(ex, ey, ez, lane);
       if (code) {
-        uint32_t vi = (uint32_t)pre + __popc(ex & below) + __popc(ey & below) + __popc(ez & below);
+        uint32_t vi = word_vertex_base(pre, ex, ey, ez, lane);
         const float va = __ldg(vol + i);
 #pragma unroll
         for (int axis = 0; axis < 3; ++axis) {
           if (!((code >> axis) & 1u)) continue;
           const uint32_t step = axis == 0 ? 1u : (axis == 1 ? (uint32_t)W : plane);
           const float vb = __ldg(vol + i + step);
-          const float t = __fdiv_rn(__fsub_rn(iso, va), __fsub_rn(vb, va));
-          float p[3] = {(float)x, (float)y, (float)z};
-          p[axis] = __fadd_rn(p[axis], t);
+          float p[3];
+          edge_point(x, y, z, axis, edge_t0(va, vb, iso), p);
           if (!kCapped || vi < out.v_cap) {
-            if (kCapped && out.world) {
-#pragma unroll
-              for (int a = 0; a < 3; ++a) p[a] = __fadd_rn(__fmul_rn(__fadd_rn(p[a], 0.5f), out.scale[a]), out.bmin[a]);
-            }
+            if (kCapped && out.world) world_point(out.scale, out.bmin, p);
             float* o = verts + 3ull * vi;
             o[0] = p[0]; o[1] = p[1]; o[2] = p[2];
           }
@@ -350,6 +383,36 @@ mesh_emit_async_kernel(const float* __restrict__ vol, const uint32_t* __restrict
     *count32 = (int32_t)(nv < out.v_cap ? nv : out.v_cap);
   }
   mesh_emit_body<true>(vol, bits, info, prefix, active, *n_active_dev, out, D, H, W, n, iso);
+}
+
+// ---- edge records of the vertices (mp_mesh_refine_async): vertex v -> (owning node, axis), for every id < v_cap.  The walk
+// of pass 4: a warp per listed word, a lane per node, the id from the word's prefix + popcounts.  It reads the active-list
+// length on the device, so it follows both mp_mcubes_run_async and the eager count + emit.  A persistent grid of any size.
+constexpr int kEdgesThreads = 256;
+__global__ void __launch_bounds__(kEdgesThreads)
+mesh_edges_kernel(const WordInfo* __restrict__ info, const unsigned long long* __restrict__ prefix, const uint32_t* __restrict__ active,
+                  const uint32_t* __restrict__ n_active_dev, uint32_t v_cap, uint32_t* __restrict__ edge_node,
+                  uint8_t* __restrict__ edge_axis) {
+  const uint32_t n_active = *n_active_dev;
+  const int lane = threadIdx.x & 31;
+  const uint32_t n_warps = gridDim.x * (kEdgesThreads / 32);
+  for (uint32_t e = blockIdx.x * (kEdgesThreads / 32) + (threadIdx.x >> 5); e < n_active; e += n_warps) {
+    const uint32_t w = __ldg(active + e);
+    const uint4 wi = __ldg(reinterpret_cast<const uint4*>(info + w));
+    const uint32_t code = lane_edge_code(wi.x, wi.y, wi.z, lane);
+    if (!code) continue;
+    uint32_t vi = word_vertex_base(__ldg(prefix + w), wi.x, wi.y, wi.z, lane);
+    const uint32_t i = 32u * w + (uint32_t)lane;
+#pragma unroll
+    for (int axis = 0; axis < 3; ++axis) {
+      if (!((code >> axis) & 1u)) continue;
+      if (vi < v_cap) {
+        edge_node[vi] = i;
+        edge_axis[vi] = (uint8_t)axis;
+      }
+      ++vi;
+    }
+  }
 }
 
 }  // namespace mcubes

@@ -85,7 +85,10 @@ class FrameGraph:
         owns): the vertices and faces reconstruction(use_octree=True, engine=engine) returns for the frame, bit for bit;
       mesh_normals: their analytic normals, mesh_normals(net, ..., precision="auto") computed inside the step;
       mesh_colours: their colours, mesh_colours(netC, ...) computed inside the step (needs netC);
-      mesh_capacity: (vertices, faces) the buffers hold, default (8 R^2, 16 R^2).
+      mesh_capacity: (vertices, faces) the buffers hold, default (8 R^2, 16 R^2);
+      mesh_refine: K > 0 moves the vertices onto the geometry net's own iso-surface along their edges, K rounds of
+        refine_mesh_async at the net's precision, between marching cubes and the mesh normals and colours (which are then
+        evaluated at the refined vertices): reconstruction(..., refine=K)'s vertices, bit for bit.
     mesh() (after result()) then returns (verts [V,3], faces [F,3] int32, normals or None, colours or None) -- views of this
     graph's buffers, valid until its next launch -- or None for a frame without a surface, and raises RuntimeError for a
     frame whose mesh exceeds the capacity (run reconstruction() eagerly for that frame).
@@ -97,7 +100,7 @@ class FrameGraph:
 
     def __init__(self, net, engine, calib, direction="front", with_encoder=True, input_shape=None, feature_hook=None,
                  netC=None, render_normals=False, canvas=None, mesh=False, mesh_normals=False, mesh_colours=False,
-                 mesh_capacity=None, display=False):
+                 mesh_capacity=None, display=False, mesh_refine=0):
         from .modeling.MonoPortNet import FeatureHandle
         from .recon import _DIRS
         if getattr(engine.query_func, "__monoport_fused__", None) is not net:
@@ -118,6 +121,10 @@ class FrameGraph:
         self.render_normals = render_normals
         if (mesh_normals or mesh_colours or mesh_capacity is not None) and not mesh:
             raise ValueError("mesh_normals, mesh_colours and mesh_capacity need mesh=True")
+        from .recon import _check_rounds
+        self._mesh_refine = _check_rounds(mesh_refine, "mesh_refine")
+        if self._mesh_refine and not mesh:
+            raise ValueError("mesh_refine needs mesh=True")
         if mesh_colours and netC is None:
             raise ValueError("mesh_colours needs netC")
         self.with_mesh, self.with_mesh_normals, self.with_mesh_colours = bool(mesh), bool(mesh_normals), bool(mesh_colours)
@@ -172,6 +179,10 @@ class FrameGraph:
                 self.mesh_faces = torch.empty((f_cap, 3), dtype=torch.int32, device=dev)
                 self.mesh_counts = torch.zeros(2, dtype=torch.int64, device=dev)
                 self._mesh_count32 = torch.zeros(1, dtype=torch.int32, device=dev)
+                if self._mesh_refine:
+                    self._mesh_rscratch = torch.empty(max(1, int(lib.mp_mesh_refine_scratch_bytes(v_cap))), dtype=torch.uint8,
+                                                      device=dev)
+                    self._mesh_world = (ctypes.c_float * 7)(float(R), *self._bmin3, *self._bmax3)
                 if mesh_normals:
                     self.mesh_norm = torch.empty((v_cap, 3), dtype=torch.float32, device=dev)
                     self._mesh_nscratch = torch.empty(3 * v_cap, dtype=torch.float32, device=dev)
@@ -262,6 +273,12 @@ class FrameGraph:
                              list(self._bmin3), list(self._bmax3), workspace=self._mcubes)
         v_cap = self.mesh_verts.shape[0]
         verts, counts, count32 = (ctypes.c_void_p(t.data_ptr()) for t in (self.mesh_verts, self.mesh_counts, self._mesh_count32))
+        if self._mesh_refine:
+            _lib.check(lib.mp_mesh_refine_async_dcal(
+                self._head, self._fh.ptr, self._mcubes.ptr, ctypes.c_void_p(self.volume.data_ptr()), ctypes.c_float(0.5),
+                self._mesh_world, verts, count32, v_cap, self._mesh_refine, cal, self._proj,
+                ctypes.c_float(self.net.normalizer.scale), self.net._mode(), ctypes.c_void_p(self._mesh_rscratch.data_ptr()),
+                st), "mp_mesh_refine_async_dcal")
         if self.with_mesh_normals:
             _lib.check(lib.mp_mesh_normals_async_dcal(
                 self._head, self._fh.ptr, verts, counts, count32, v_cap, cal, self._proj,

@@ -6,6 +6,8 @@
                                  `reconstruction` follows upstream PIFu's signature);
   marching_cubes_async, mesh_normals, mesh_colours: the mesh of a captured frame (FrameGraph(mesh=True)) and its eager
                                  twins -- normals and upstream PIFu's gen_mesh_color vertex colours at the vertices;
+  refine_mesh_async            : its vertices moved along their edges onto the network's own iso-surface
+                                 (FrameGraph(mesh_refine=K), reconstruction(refine=K));
   visulization                 : the demo's display images (RTL/main.py:252-281), the eager twin of
                                  FrameGraph(display=True).
 """
@@ -172,6 +174,67 @@ def marching_cubes_async(vol, verts, faces, counts, count32, iso=0.5, b_min=None
             ctypes.c_void_p(count32.data_ptr()), _lib.stream_ptr(vol.device)), "mp_mcubes_run_async")
 
 
+def _check_rounds(rounds, what):
+    if isinstance(rounds, bool) or not isinstance(rounds, (int, np.integer)) or rounds < 0:
+        raise ValueError("%s must be an integer >= 0; got %r" % (what, rounds))
+    return int(rounds)
+
+
+def _refine_enqueue(net, feat, ws_ptr, vol, iso, b_min, b_max, verts, count32, rounds, calib_tensor, scratch):
+    """mp_mesh_refine_async of `rounds` rounds on the current stream (the arguments checked by the callers)"""
+    v_cap = verts.shape[0]
+    if rounds == 0 or v_cap == 0:
+        return
+    lib = _lib.load()
+    device = vol.device
+    need = int(lib.mp_mesh_refine_scratch_bytes(v_cap))
+    if scratch is None:
+        scratch = torch.empty(need, dtype=torch.uint8, device=device)
+    elif scratch.device != device or not scratch.is_contiguous() or scratch.numel() * scratch.element_size() < need:
+        raise ValueError("scratch must be a contiguous tensor of at least %d bytes on %s" % (need, device))
+    world = (ctypes.c_float * 7)(float(vol.shape[2]), *_lib.f3(b_min), *_lib.f3(b_max))
+    with _lib.device_guard(device):
+        fh = net.feature_handle(feat)
+        _lib.check(lib.mp_mesh_refine_async(
+            net.surface_classifier.handle(), fh.ptr, ws_ptr, ctypes.c_void_p(vol.data_ptr()), ctypes.c_float(iso), world,
+            ctypes.c_void_p(verts.data_ptr()), ctypes.c_void_p(count32.data_ptr()), v_cap, rounds, _lib.calib12(calib_tensor),
+            net._proj(), ctypes.c_float(net.normalizer.scale), net._mode(), ctypes.c_void_p(scratch.data_ptr()),
+            _lib.stream_ptr(device)), "mp_mesh_refine_async")
+
+
+@torch.no_grad()
+def refine_mesh_async(net, feat, vol, verts, count32, rounds, b_min, b_max, calib_tensor, iso=0.5, *, workspace, scratch=None):
+    """Move the vertices of marching_cubes_async's world-space mesh onto the geometry net's own iso-surface, in place and
+    enqueue-only (mp_mesh_refine_async; the algorithm: DESIGN.md §F3.1).  Each vertex stays on its grid edge, which the
+    volume's two end values bracket; `rounds` rounds of regula falsi (Illinois) each evaluate the net once per vertex at
+    its precision (net.precision, like the volume), starting at the marching-cubes vertex, and the candidate with the
+    smallest |sigma - iso| is written back.  Faces and counts are not touched, nor vertices at or beyond min(count32, V_cap).
+    rounds = 0 changes nothing, rounds = 1 rewrites the same bits.
+    feat: the net's [1,C,H,W] feature map (net.filter(image)[-1][0]); vol, iso, b_min, b_max, verts, count32 and workspace:
+    those of the marching_cubes_async call that made the mesh -- the workspace's last run must be that one.
+    scratch: None (allocated per call) or a device tensor of at least mp_mesh_refine_scratch_bytes(V_cap) bytes (a CUDA
+    graph captures the call with a scratch of its own)."""
+    rounds = _check_rounds(rounds, "rounds")
+    if vol.dim() == 5:
+        vol = vol[0, 0]
+    _require(vol, torch.float32, None, "vol")
+    if vol.dim() != 3:
+        raise ValueError("vol must be [D,H,W] or [1,1,D,H,W]; got %s" % (tuple(vol.shape),))
+    if not isinstance(workspace, McubesWorkspace) or workspace.shape != tuple(vol.shape) or not workspace.ptr:
+        raise ValueError("workspace must be an open McubesWorkspace of shape %s" % (tuple(vol.shape),))
+    D, H, W = vol.shape
+    if not D == H == W:
+        raise ValueError("world-space vertices need a cubic volume; got %s" % (tuple(vol.shape),))
+    if verts.dim() != 2:
+        raise ValueError("verts must be [V_cap,3]")
+    _require(verts, torch.float32, (verts.shape[0], 3), "verts")
+    _require(count32, torch.int32, (1,), "count32")
+    for t in (verts, count32, feat):
+        if t.device != vol.device:
+            raise ValueError("the volume, the mesh buffers and the features live on different devices")
+    _refine_enqueue(net, feat, workspace.ptr, vol, iso, b_min, b_max, verts, count32, rounds, calib_tensor, scratch)
+
+
 @torch.no_grad()
 def mesh_normals(net, feats, verts, calib_tensor, precision="auto"):
     """Outward unit normals -grad sigma / |grad sigma| of the geometry net at mesh vertices verts [V,3] (world space, e.g.
@@ -222,7 +285,7 @@ def _unit_or_zero(v):
 
 @torch.no_grad()
 def reconstruction(net, cuda, calib_tensor, resolution, b_min, b_max, use_octree=False, num_samples=10000,
-                   transform=None, feats=None, engine=None, normals=False):
+                   transform=None, feats=None, engine=None, normals=False, refine=0):
     """PIFu-shaped mesh reconstruction (upstream signature, SURVEY.md §8b): evaluate the occupancy field on a
     `resolution`^3 grid over [b_min,b_max] (dense through the fused kernel, or coarse-to-fine when `use_octree`),
     run marching cubes at 0.5, map vertices to world space.  `feats` = net.filter(image) output.
@@ -232,9 +295,12 @@ def reconstruction(net, cuda, calib_tensor, resolution, b_min, b_max, use_octree
     normals: False -> None.  True -> [V,3] outward unit normals -grad sigma / |grad sigma| at the returned vertices (sigma >
     0.5 is inside), evaluated exactly by the fp32 gradient kernel (MonoPortNet.query_gradient); a vertex where the
     gradient vanishes gets a zero vector.  With `transform` they are mapped like the vertices (inverse transpose of its 3x3
-    part, renormalised: a rotation rotates them)."""
+    part, renormalised: a rotation rotates them).
+    refine: 0 -> the marching-cubes vertices.  K > 0 -> each vertex moved along its grid edge onto the net's own iso-surface
+    by K rounds of refine_mesh_async (DESIGN.md §F3.1) before `normals` and `transform`; faces are unchanged."""
     if feats is None:
         raise ValueError("pass feats=net.filter(image)")
+    refine = _check_rounds(refine, "refine")
     R = int(resolution)
     device = torch.device(cuda)
     b_min_t = torch.as_tensor(np.asarray(b_min, dtype=np.float32)).view(3)
@@ -257,12 +323,19 @@ def reconstruction(net, cuda, calib_tensor, resolution, b_min, b_max, use_octree
         vol = sdf[0, 0]
     else:
         vol = net.query_grid(feats[-1][0], calib_tensor, R, b_min_t, b_max_t)
+    if refine and (vol.dtype != torch.float32 or not vol.is_contiguous()):
+        vol = vol.float().contiguous()            # (the one copy marching cubes and the refinement both read)
     verts, faces = marching_cubes(vol, 0.5)
     if verts.shape[0] == 0:
         return -1
     # index space -> world:  (v + 0.5)/R * (b_max-b_min) + b_min  (node-centre convention of the engines)
     scale = ((b_max_t - b_min_t) / R).to(verts.device)
     verts = (verts + 0.5) * scale + b_min_t.to(verts.device)
+    if refine:
+        # on marching_cubes()' per-thread workspace, whose last run read this volume
+        count32 = torch.tensor([verts.shape[0]], dtype=torch.int32, device=verts.device)
+        _refine_enqueue(net, feats[-1][0], _McubesWorkspace.get(vol.shape, vol.device), vol, 0.5, b_min_t, b_max_t, verts,
+                        count32, refine, calib_tensor, None)
     nrm = None
     if normals:
         _, grad = net.query_gradient(feats, verts.t().unsqueeze(0), calib_tensor)
