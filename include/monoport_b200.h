@@ -455,6 +455,25 @@ int mp_mesh_refine_async_dcal(mp_mlp_t* mlp, mp_feat_t* feat, mp_mcubes_t* ws, c
                               const float* world, float* verts_dev, const int32_t* count32_dev, int64_t v_cap, int rounds,
                               const float* calib_dev, int projection, float z_scale, int mode, void* scratch_dev, void* stream);
 
+/* The frame's mesh drawn from V viewer cameras (DESIGN.md §F3.2): the reference GL renderer's normal and colour programs as a
+ * deterministic rasterizer, enqueue-only (graph-capturable).  verts_dev [v_cap][3] / faces_dev [f_cap][3] int32 with
+ * counts_dev = (nV, nF) int64 on the device (mp_mcubes_run_async's buffers); the first min(nF, f_cap) faces are drawn, a
+ * face with an index outside [0, min(nV, v_cap)) is skipped.  mats_dev: views x 32 float32 in device memory, ModelMat then
+ * PerspMat of each view, row-major 4x4 (the numpy matrices the reference uploads with transpose=GL_TRUE).  Per view:
+ * clip = PerspMat (ModelMat [p, 1]); coverage on integer edge functions of the window coordinates snapped to 1/256 px, with
+ * a top-left rule; both windings; GL_LESS on a 24-bit depth in draw order (the lower face id wins a tie).  normals_dev /
+ * colours_dev [v_cap][3] (either may be NULL, not both): out_normal_dev gets (n / |n| + 1) / 2 of the interpolated
+ * (ModelMat [n, 0]).xyz with alpha 1, out_colour_dev the interpolated colour with alpha 1 -- each [views][height][width][4]
+ * float32, row 0 the top of the window (get_color()'s orientation); an uncovered pixel gets clear[4] (host floats).  An image
+ * is written exactly when its attribute is given.  width and height: 1..8192; views: 1..65535.  scratch_dev: at least
+ * mp_render_mesh_scratch_bytes(f_cap, views, width, height) bytes of device memory, private to the call until it completes
+ * (-1 for arguments the call refuses). */
+int64_t mp_render_mesh_scratch_bytes(int64_t f_cap, int views, int width, int height);
+int mp_render_mesh_async(const float* verts_dev, const int32_t* faces_dev, const int64_t* counts_dev, int64_t v_cap,
+                         int64_t f_cap, const float* normals_dev, const float* colours_dev, const float* mats_dev, int views,
+                         int width, int height, const float* clear, float* out_normal_dev, float* out_colour_dev,
+                         void* scratch_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -122,6 +122,9 @@ SIGNATURES = {
                                      c_int, P(c_float), c_int, c_float, c_int, c_void_p, c_void_p]),
     "mp_mesh_refine_async_dcal": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float, P(c_float), c_void_p, c_void_p,
                                           c_int64, c_int, c_void_p, c_int, c_float, c_int, c_void_p, c_void_p]),
+    "mp_render_mesh_scratch_bytes": (c_int64, [c_int64, c_int, c_int, c_int]),
+    "mp_render_mesh_async": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int64, c_void_p, c_void_p, c_void_p, c_int, c_int,
+                                     c_int, P(c_float), c_void_p, c_void_p, c_void_p, c_void_p]),
     "mp_forward_vertices":(c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, P(c_int64),
                                     c_void_p]),
     "mp_forward_vertices_scratch_bytes": (c_int64, [c_int]),

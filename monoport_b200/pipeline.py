@@ -6,6 +6,7 @@ results in order.  All monoport_b200 handles that carry per-call scratch are per
 import ctypes
 import threading
 from collections import deque
+from itertools import repeat
 from concurrent.futures import ThreadPoolExecutor
 
 import torch
@@ -93,6 +94,15 @@ class FrameGraph:
     graph's buffers, valid until its next launch -- or None for a frame without a surface, and raises RuntimeError for a
     frame whose mesh exceeds the capacity (run reconstruction() eagerly for that frame).
 
+    views: the frame's mesh drawn from viewer cameras inside the same step, the reference GL renderer's normal and colour
+      programs (recon.render_mesh, DESIGN.md §F3.2): (model_mat, persp_mat), each [4,4] or [V,4,4], the default cameras of
+      every frame; view_size: (W, H) of the images.  Needs mesh=True and mesh_normals and / or mesh_colours, which give the
+      normal and the colour image.  launch(..., views=(model_mat, persp_mat)) draws one frame from other cameras (the same
+      V), written into a device buffer the graph reads, like calib=.  mesh_rendered() (after result()) returns (normal
+      [V,H,W,4] or None, colour [V,H,W,4] or None) -- views of this graph's buffers, valid until its next launch -- equal to
+      render_mesh(*mesh()[:2], ..., normals=, colours=) of the frame: clear images for a frame without a surface, and
+      RuntimeError for a frame whose mesh exceeds the capacity.
+
     display: the step ends with the demo's display images (RTL/main.py:252-281) of the rendered images, copied into
       page-locked host buffers of this graph (mp_display_async; needs netC and/or render_normals).  displayed() (after
       result()) returns them as recon.visulization(*rendered()) does -- numpy views of those buffers, valid until the next
@@ -100,7 +110,7 @@ class FrameGraph:
 
     def __init__(self, net, engine, calib, direction="front", with_encoder=True, input_shape=None, feature_hook=None,
                  netC=None, render_normals=False, canvas=None, mesh=False, mesh_normals=False, mesh_colours=False,
-                 mesh_capacity=None, display=False, mesh_refine=0):
+                 mesh_capacity=None, display=False, mesh_refine=0, views=None, view_size=None):
         from .modeling.MonoPortNet import FeatureHandle
         from .recon import _DIRS
         if getattr(engine.query_func, "__monoport_fused__", None) is not net:
@@ -128,6 +138,11 @@ class FrameGraph:
         if mesh_colours and netC is None:
             raise ValueError("mesh_colours needs netC")
         self.with_mesh, self.with_mesh_normals, self.with_mesh_colours = bool(mesh), bool(mesh_normals), bool(mesh_colours)
+        self.with_views = views is not None
+        if self.with_views and not (mesh and (mesh_normals or mesh_colours)):
+            raise ValueError("views needs mesh=True and mesh_normals and / or mesh_colours")
+        if (view_size is not None) and not self.with_views:
+            raise ValueError("view_size needs views")
         if display and netC is None and not render_normals:
             raise ValueError("display needs an image to show: netC and/or render_normals")
         self.with_display = bool(display)
@@ -189,6 +204,16 @@ class FrameGraph:
                 if mesh_colours:
                     self._mesh_pred = torch.empty((3, v_cap), dtype=torch.float32, device=dev)
                     self._mesh_rgb = torch.empty((3, v_cap), dtype=torch.float32, device=dev)
+                if self.with_views:
+                    from .recon import MeshRenderer, view_mats
+                    if view_size is None:
+                        raise ValueError("views needs view_size=(W, H)")
+                    self._view_default = view_mats(views[0], views[1], dev)
+                    self._view_dev = self._view_default.clone()
+                    self._view_is_default = True
+                    self._renderer = MeshRenderer(f_cap, self._view_default.shape[0], view_size, mesh_normals, mesh_colours, dev)
+                    # the colours as the [v_cap][3] rows the renderer reads
+                    self._mesh_rgb_rows = torch.empty((v_cap, 3), dtype=torch.float32, device=dev) if mesh_colours else None
             if display:
                 from .recon import DisplayBuffers
                 self._display = DisplayBuffers(self.render_norm is not None, self.render_tex is not None, dev)
@@ -292,6 +317,11 @@ class FrameGraph:
                 self.netC._mode(), st), "mp_query_points_count_dcal")
             torch.mul(self._mesh_pred, 0.5, out=self._mesh_rgb)
             self._mesh_rgb.add_(0.5)
+        if self.with_views:
+            if self.with_mesh_colours:
+                self._mesh_rgb_rows.copy_(self._mesh_rgb.t())
+            self._renderer.enqueue(self.mesh_verts, self.mesh_faces, self.mesh_counts,
+                                   self.mesh_norm if self.with_mesh_normals else None, self._mesh_rgb_rows, self._view_dev, st)
 
     def _calib_rows(self, calib):
         """calib ([1,4,4], [4,4] or [3,4], any float dtype, on the CPU or on the graph's device) -> its rows 0..2 as a
@@ -313,14 +343,23 @@ class FrameGraph:
             c = c[:3, :4].to(torch.float32, copy=True)
         return c[:3, :4]
 
-    def launch(self, x, x_colour=None, calib=None):
+    def launch(self, x, x_colour=None, calib=None, views=None):
         """Enqueue one frame (returns at once).  x_colour: netC's input (its image with the encoder, else its map), required
         exactly when the graph was built with netC.  calib: the frame's camera ([1,4,4], [4,4] or [3,4], CPU or this graph's
         device; rows 0..2 are used, in float32 like calib12), None for the constructor's.  ValueError for another shape, a
-        batch of more than one or another device."""
+        batch of more than one or another device.  views: (model_mat, persp_mat) of the frame's mesh render (graphs built
+        with views=; the constructor's number of views), None for the constructor's."""
         if (x_colour is None) != (self.netC is None):
             raise ValueError("x_colour is required exactly when the FrameGraph renders with netC")
         rows = None if calib is None else self._calib_rows(calib)
+        vrows = None
+        if views is not None:
+            if not self.with_views:
+                raise ValueError("launch(views=...) needs a graph built with views=")
+            from .recon import view_mats
+            vrows = view_mats(views[0], views[1], "cpu")
+            if vrows.shape != self._view_dev.shape:
+                raise ValueError("views: the graph draws %d views; got %d" % (self._view_dev.shape[0], vrows.shape[0]))
         self.stream.wait_stream(torch.cuda.current_stream(self.device))     # x may still be produced on the caller's stream
         with torch.cuda.stream(self.stream):
             if rows is None:
@@ -332,6 +371,14 @@ class FrameGraph:
                 if rows.device.type != "cpu":
                     rows.record_stream(self.stream)      # (read on this stream: its memory is not reused before the copy)
                 self._cal_dev.view(3, 4).copy_(rows, non_blocking=True)
+            if self.with_views:
+                if vrows is None:
+                    if not self._view_is_default:
+                        self._view_dev.copy_(self._view_default, non_blocking=True)
+                        self._view_is_default = True
+                else:
+                    self._view_is_default = False
+                    self._view_dev.copy_(vrows, non_blocking=True)
             self.static_in.copy_(x, non_blocking=True)
             if x_colour is not None:
                 self.static_in_c.copy_(x_colour, non_blocking=True)
@@ -384,15 +431,39 @@ class FrameGraph:
             raise RuntimeError("FrameGraph.mesh() needs the frame's result() first")
         if not self._nonempty:
             return None
+        nv, nf = self._mesh_counts_checked()
+        if nv == 0:
+            return None
+        return (self.mesh_verts[:nv], self.mesh_faces[:nf], self.mesh_norm[:nv] if self.with_mesh_normals else None,
+                self._mesh_rgb.t()[:nv] if self.with_mesh_colours else None)
+
+    def _mesh_counts_checked(self):
         nv, nf = self.mesh_counts.tolist()              # (result() has synchronised the graph's stream)
         v_cap, f_cap = self.mesh_verts.shape[0], self.mesh_faces.shape[0]
         if nv > v_cap or nf > f_cap:
             raise RuntimeError("FrameGraph: the frame's mesh has %d vertices and %d faces, above the capacity of %d and %d "
                                "(mesh_capacity) -- run reconstruction() eagerly for this frame" % (nv, nf, v_cap, f_cap))
-        if nv == 0:
-            return None
-        return (self.mesh_verts[:nv], self.mesh_faces[:nf], self.mesh_norm[:nv] if self.with_mesh_normals else None,
-                self._mesh_rgb.t()[:nv] if self.with_mesh_colours else None)
+        return nv, nf
+
+    def mesh_rendered(self):
+        """After result(): (normal [V,H,W,4] or None, colour [V,H,W,4] or None), the frame's mesh drawn from its views --
+        views of this graph's buffers, valid until its next launch.  A frame without a surface gives images of the clear
+        colour; RuntimeError for a frame whose mesh exceeds the capacity."""
+        if not self.with_views:
+            raise RuntimeError("FrameGraph.mesh_rendered() needs a graph built with views=")
+        if self._nonempty is None:
+            raise RuntimeError("FrameGraph.mesh_rendered() needs the frame's result() first")
+        r = self._renderer
+        if not self._nonempty:
+            clear = torch.tensor(list(r.clear), dtype=torch.float32, device=self.device)
+            with torch.cuda.stream(self.stream):
+                for img in (r.normal, r.colour):
+                    if img is not None:
+                        img.copy_(clear.expand_as(img))
+            self.stream.synchronize()
+        else:
+            self._mesh_counts_checked()
+        return r.normal, r.colour
 
     def displayed(self):
         """After result(): (render_norm [256,256,3] float32, render_tex likewise, mask [256,256,1] bool) -- numpy views of
@@ -428,8 +499,9 @@ class FrameGraphRing:
     counterpart of FramePipeline for the stages of this library).  Lanes built with netC take (x, x_colour) items and yield
     result() + rendered(): (sdf, X, Y, Z, norm, render_norm, render_tex).  Lanes built with mesh=True append mesh()'s
     (verts, faces, normals, colours), four Nones for a frame without a surface.  Lanes built with display=True then append
-    displayed()'s (render_norm, render_tex, mask).  run(items, calibs) takes the cameras of the frames too (zipped with
-    items; see FrameGraph.launch)."""
+    displayed()'s (render_norm, render_tex, mask).  Lanes built with views= then append mesh_rendered()'s (normal, colour).
+    run(items, calibs, views) takes the cameras and the render views of the frames too (each zipped with items, None for
+    the constructor's; see FrameGraph.launch)."""
 
     def __init__(self, make_graph, n_lanes=2):
         self.lanes = [make_graph() for _ in range(int(n_lanes))]
@@ -443,16 +515,19 @@ class FrameGraphRing:
             out = out + (lane.mesh() or (None,) * 4)
         if lane.with_display:
             out = out + lane.displayed()
+        if lane.with_views:
+            out = out + lane.mesh_rendered()
         return out
 
-    def run(self, iterable, calibs=None):
+    def run(self, iterable, calibs=None, views=None):
         inflight = deque()
-        pairs = zip(iterable, calibs) if calibs is not None else ((x, None) for x in iterable)
-        for i, (x, calib) in enumerate(pairs):
+        triples = zip(iterable, repeat(None) if calibs is None else calibs, repeat(None) if views is None else views)
+        for i, (x, calib, view) in enumerate(triples):
             lane = self.lanes[i % len(self.lanes)]
             if len(inflight) >= len(self.lanes):
                 yield self._out(inflight.popleft())
-            inflight.append(lane.launch(*x, calib=calib) if lane.netC is not None else lane.launch(x, calib=calib))
+            kw = dict(calib=calib) if view is None else dict(calib=calib, views=view)
+            inflight.append(lane.launch(*x, **kw) if lane.netC is not None else lane.launch(x, **kw))
         while inflight:
             yield self._out(inflight.popleft())
 

@@ -9,7 +9,9 @@
   refine_mesh_async            : its vertices moved along their edges onto the network's own iso-surface
                                  (FrameGraph(mesh_refine=K), reconstruction(refine=K));
   visulization                 : the demo's display images (RTL/main.py:252-281), the eager twin of
-                                 FrameGraph(display=True).
+                                 FrameGraph(display=True);
+  render_mesh                  : the mesh drawn from viewer cameras by the reference GL renderer's normal and colour
+                                 programs (DESIGN.md §F3.2), the eager twin of FrameGraph(views=...).
 """
 import ctypes
 import threading
@@ -514,3 +516,95 @@ def surface_normals(net, feats, X, Y, Z, calib_tensor, resolution=257, b_min=(-1
     length = (torch.as_tensor(np.asarray(b_max, dtype=np.float32)) - torch.as_tensor(np.asarray(b_min, dtype=np.float32)))
     axis = (length.view(3) / resolution * torch.tensor([1.0, 1.0, -1.0])).to(device)
     return _unit_or_zero(-(grad[0].t() * axis))
+
+
+def view_mats(model_mat, persp_mat, device):
+    """ModelMat and PerspMat ([4,4] or [V,4,4] each, numpy or torch; a [4,4] one serves every view) -> the [V,32] float32
+    device tensor mp_render_mesh_async reads: each view's ModelMat then PerspMat, row-major (the matrices the reference
+    uploads with transpose=GL_TRUE)."""
+    mats = []
+    for m, what in ((model_mat, "model_mat"), (persp_mat, "persp_mat")):
+        t = torch.as_tensor(np.asarray(m.detach().cpu() if torch.is_tensor(m) else m, dtype=np.float32))
+        if t.dim() == 2:
+            t = t[None]
+        if t.dim() != 3 or tuple(t.shape[1:]) != (4, 4) or t.shape[0] < 1:
+            raise ValueError("%s must be [4,4] or [V,4,4]; got %s" % (what, tuple(t.shape)))
+        mats.append(t)
+    M, P = mats
+    if M.shape[0] != P.shape[0] and 1 not in (M.shape[0], P.shape[0]):
+        raise ValueError("model_mat and persp_mat hold %d and %d views" % (M.shape[0], P.shape[0]))
+    V = max(M.shape[0], P.shape[0])
+    M, P = M.expand(V, 4, 4), P.expand(V, 4, 4)
+    return torch.cat([M.reshape(V, 16), P.reshape(V, 16)], dim=1).contiguous().to(device)
+
+
+def _view_size(size):
+    try:
+        W, H = (int(s) for s in size)
+    except (TypeError, ValueError):
+        raise ValueError("size must be (W, H); got %r" % (size,)) from None
+    return W, H
+
+
+class MeshRenderer:
+    """What one mp_render_mesh_async call writes, for meshes of capacity (v_cap, f_cap) drawn from `views` cameras at
+    size (W, H): the normal and / or colour images [V,H,W,4] float32 and the scratch.  enqueue() draws the mesh in the
+    buffers it is given on the current stream; FrameGraph(views=...) captures it."""
+
+    def __init__(self, f_cap, views, size, has_normals, has_colours, device, clear=(0, 0, 0, 0)):
+        W, H = self.size = _view_size(size)
+        self.views = int(views)
+        lib = _lib.load()
+        need = int(lib.mp_render_mesh_scratch_bytes(int(f_cap), self.views, W, H))
+        if need < 0:
+            raise ValueError("mesh render: bad arguments (f_cap=%d, views=%d, size=%dx%d; sides 1..8192)" % (f_cap, views, W, H))
+        self.scratch = torch.empty(need, dtype=torch.uint8, device=device)
+        self.normal = torch.empty((self.views, H, W, 4), dtype=torch.float32, device=device) if has_normals else None
+        self.colour = torch.empty((self.views, H, W, 4), dtype=torch.float32, device=device) if has_colours else None
+        c = [float(x) for x in clear]
+        if len(c) != 4:
+            raise ValueError("clear must hold 4 values; got %r" % (clear,))
+        self.clear = (ctypes.c_float * 4)(*c)
+
+    def enqueue(self, verts, faces, counts, normals, colours, mats, stream):
+        def p(t):
+            return None if t is None else ctypes.c_void_p(t.data_ptr())
+        W, H = self.size
+        _lib.check(_lib.load().mp_render_mesh_async(
+            p(verts), p(faces), p(counts), verts.shape[0], faces.shape[0], p(normals), p(colours), p(mats), self.views, W, H,
+            self.clear, p(self.normal), p(self.colour), p(self.scratch), stream), "mp_render_mesh_async")
+
+
+@torch.no_grad()
+def render_mesh(verts, faces, model_mat, persp_mat, size, normals=None, colours=None, clear=(0, 0, 0, 0)):
+    """The mesh (verts [V,3] float32 CUDA, faces [F,3] int32, e.g. reconstruction()'s) drawn from one or more viewer cameras by
+    the reference GL renderer's two per-vertex programs (DESIGN.md §F3.2): NormalRender's (n / |n| + 1) / 2 of the
+    interpolated (ModelMat [n, 0]).xyz, and ColorRender's interpolated vertex colour, both with alpha 1, GL_LESS depth in
+    face order, no culling.  model_mat / persp_mat: [4,4] or [V,4,4] (numpy or torch; a [4,4] one serves every view), the
+    numpy matrices the reference passes to its renderer.  size: (W, H).  normals / colours: [V,3] per-vertex attributes
+    (either may be None, not both).  clear: the colour of uncovered pixels.
+    Returns (normal_img, colour_img): [V,H,W,4] float32 CUDA tensors, row 0 the top of the image (get_color()'s
+    orientation), None for an attribute not given.  One mp_render_mesh_async call -- what FrameGraph(views=...) captures,
+    so both give the same bits -- with the counts built on the device."""
+    if normals is None and colours is None:
+        raise ValueError("render_mesh needs normals and / or colours")
+    if verts.device.type != "cuda":
+        raise RuntimeError("monoport_b200.render_mesh: CUDA tensors only (no CPU path)")
+    dev = verts.device
+    if verts.dim() != 2 or verts.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError("verts must be [V,3] and faces [F,3]; got %s and %s" % (tuple(verts.shape), tuple(faces.shape)))
+    v = verts.detach().to(torch.float32).contiguous()
+    f = faces.detach().to(device=dev, dtype=torch.int32).contiguous()
+    attrs = []
+    for a, what in ((normals, "normals"), (colours, "colours")):
+        if a is not None:
+            if tuple(a.shape) != tuple(v.shape) or a.device != dev:
+                raise ValueError("%s must be [%d,3] on %s; got %s on %s" % (what, v.shape[0], dev, tuple(a.shape), a.device))
+            a = a.detach().to(torch.float32).contiguous()
+        attrs.append(a)
+    mats = view_mats(model_mat, persp_mat, dev)
+    counts = torch.tensor([v.shape[0], f.shape[0]], dtype=torch.int64, device=dev)
+    with _lib.device_guard(dev):
+        r = MeshRenderer(f.shape[0], mats.shape[0], size, normals is not None, colours is not None, dev, clear)
+        r.enqueue(v, f, counts, attrs[0], attrs[1], mats, _lib.stream_ptr(dev))
+    return r.normal, r.colour
